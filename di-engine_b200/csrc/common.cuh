@@ -65,8 +65,7 @@ __device__ __forceinline__ float warp_max(float v) {
 // elsewhere) thread 0 holds the grid totals in tot[0..K).  `ws` must hold WS_CTRL_WORDS + gridDim.x*K floats,
 // control word `slot` must be zero on entry and is reset to zero on exit (stream-ordered reuse).
 template <int K, int NT>
-__device__ __forceinline__ bool grid_sum(float (&v)[K], double (&tot)[K], float* ws, int slot,
-                                         unsigned long long* trace = nullptr) {
+__device__ __forceinline__ bool grid_sum(float (&v)[K], double (&tot)[K], float* ws, int slot) {
     __shared__ float s_part[K][NT / 32];
     __shared__ double s_tot[K][NT / 32];
     __shared__ bool s_last;
@@ -78,7 +77,6 @@ __device__ __forceinline__ bool grid_sum(float (&v)[K], double (&tot)[K], float*
         if (lane == 0) s_part[k][wid] = r;
     }
     __syncthreads();
-    if (trace && threadIdx.x == 0) trace[0] = gtimer();
     float* part = ws + WS_CTRL_WORDS;
     unsigned int* ctrl = reinterpret_cast<unsigned int*>(ws);
     if (threadIdx.x == 0) {
@@ -96,18 +94,15 @@ __device__ __forceinline__ bool grid_sum(float (&v)[K], double (&tot)[K], float*
         }
         s_dep = dep;  // a real use of the returned values: instructions issue in order, so everything below waits here
         asm volatile("" ::: "memory");
-        if (trace) trace[1] = gtimer();
         // release: the partials above (and, through the barrier before, whatever the CTA's threads stored) happen-before
         // the ticket; acquire: the last CTA's reads below happen-after every earlier ticket (PTX memory model, gpu scope)
         unsigned int ticket;
         asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], 1;" : "=r"(ticket) : "l"(&ctrl[slot]) : "memory");
-        if (trace) trace[2] = gtimer();
         s_last = (ticket == gridDim.x - 1);
     }
     __syncthreads();
     if (!s_last) return false;
     fence_acq_rel_gpu();  // every thread of the last CTA reads other CTAs' results: order those reads after the ticket
-    if (trace && threadIdx.x == 0) trace[3] = gtimer();
     double acc[K];
 #pragma unroll
     for (int k = 0; k < K; ++k) acc[k] = 0.0;
@@ -515,27 +510,8 @@ static inline bool pdl_enabled() {
     return v == 1;
 }
 
-// Optional (B200RL_CARVEOUT=1): ask for the same L1/shared-memory split (maximum shared memory) for every kernel so that
-// consecutive kernels never make the SMs reconfigure.  Off by default: a small L1 bounds the number of cache lines the
-// GAE scan's loaders can keep in flight.
-static inline void pin_carveout(const void* fn) {
-    static const void* seen[64];
-    static int n_seen = 0;
-    for (int i = 0; i < n_seen; ++i)
-        if (seen[i] == fn) return;
-    static int enabled = -1;
-    if (enabled < 0) {
-        const char* e = getenv("B200RL_CARVEOUT");
-        enabled = (e && e[0] == '1') ? 1 : 0;
-    }
-    if (enabled) (void)cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (n_seen < 64) seen[n_seen++] = fn;
-    (void)cudaGetLastError();
-}
-
 template <typename... KArgs, typename... Args>
 static inline int launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-    pin_carveout(reinterpret_cast<const void*>(kern));
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = grid;
     cfg.blockDim = block;

@@ -183,7 +183,7 @@ __global__ void __launch_bounds__(PPO_THREADS, 4) gae_ppo_kernel(FusedArgs f, fl
                 if (full_tile || rit < tail_rows)
                     ppo_row_compute<NC, true, GRADS>(a, L, st, rit, N, adv, full_tile, gtile, row0, up, acc);
             }
-            if (GRADS && full_tile && !(a.dbg & 6)) {
+            if (GRADS && full_tile) {
                 fence_proxy_async_smem();
                 __syncwarp();
                 if (lane == 0) {
@@ -274,7 +274,8 @@ static int launch_fused(const FusedArgs& f, float* out, float* ws, size_t ws_byt
 
 template <bool GRADS>
 static int dispatch_fused(const FusedArgs& f, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
-    // 2 rows per thread once there are four 256-row tiles per SM, where their layout fits; 1 row fits for every N <= 32
+    // 2 rows per thread once there are four 256-row tiles per SM, where their layout fits; 1 row fits for every N <= 32.
+    // The TMA issue rate per SM is bounded per operation, so 256-row tiles double the bytes each bulk copy moves.
     const int rpt = (f.p.S >= 256LL * NUM_SMS * 4 && fused_smem(f, GRADS, 2) <= 227 * 1024) ? 2 : 1;
     switch (f.p.N) {
 #define B200RL_CASE(n)                                                             \
@@ -308,14 +309,6 @@ static void fill_fused(FusedArgs& f, const float* value, float* next_value, cons
     a.kl_type = kl_type;
     f.value = value; f.next_value = next_value; f.reward = reward; f.done = done; f.traj = traj_flag; f.T = T; f.B = B;
     f.gamma = (float)gamma; f.gl = (float)(gamma * lambda_); f.mask_inplace = mask_inplace;
-    {
-        static int dbg = -1;
-        if (dbg < 0) {
-            const char* e = getenv("B200RL_PPO_DBG");
-            dbg = e ? atoi(e) : 0;
-        }
-        a.dbg = dbg;
-    }
     {
         static int tr = -1;
         if (tr < 0) {

@@ -11,11 +11,8 @@
 // T is processed in 128-row slabs from the end of the trajectory, each slab in four 32-row chunks handed from the
 // loaders to the scan warp through named barriers; the carry stays in the scan lanes' registers.
 // Algorithmic traffic: 5 reads + 1 write = 24 B per transition.
-#include <stdlib.h>
-
 #include "../../include/b200rl.h"
 #include "gae_tile.cuh"
-#include "policy_stats.cuh"
 
 namespace b200rl {
 
@@ -34,63 +31,6 @@ __global__ void __launch_bounds__((TC / 4 + 1) * 32) gae_ws_kernel(
     __shared__ __align__(16) float s_f[GAE_NCHUNK][GAE_CH][TC];
     gae_tile_body<TC, VEC>(value, next_value, reward, done, traj, adv, T, C, A, gamma, gl, mask_inplace,
                            (long long)blockIdx.x * TC, s_d, s_f, [](long long, bool) {}, vscale);
-}
-
-// gae + the returns epilogue of PPOPolicy (policy/ppo.py:283-297) in ONE launch: the storer warps, which write the finished
-// advantage chunks off the scan's critical path, also re-read the value row (an L2 hit: the loaders have just streamed it), write
-// unnormalized_return / value / return_ and accumulate the four batch sums; the last CTA turns them into the statistics.
-struct GaeRetHook {
-    const float* value;
-    RetArgs ra;
-    double (*acc)[4];
-    __device__ __forceinline__ void operator()(long long off, const float4& a) const {
-        const float4 v = *reinterpret_cast<const float4*>(value + off);
-        float4 ru, vo, ro;
-        ret_one(ra.vscale, v.x, a.x, ru.x, vo.x, ro.x, *acc);
-        ret_one(ra.vscale, v.y, a.y, ru.y, vo.y, ro.y, *acc);
-        ret_one(ra.vscale, v.z, a.z, ru.z, vo.z, ro.z, *acc);
-        ret_one(ra.vscale, v.w, a.w, ru.w, vo.w, ro.w, *acc);
-        if (ra.ret_unnorm) stg_stream4(reinterpret_cast<float4*>(ra.ret_unnorm + off), ru);
-        if (ra.value_out) stg_stream4(reinterpret_cast<float4*>(ra.value_out + off), vo);
-        if (ra.ret_out) stg_stream4(reinterpret_cast<float4*>(ra.ret_out + off), ro);
-    }
-    __device__ __forceinline__ void operator()(long long off, float a) const {
-        float ru, vo, ro;
-        ret_one(ra.vscale, value[off], a, ru, vo, ro, *acc);
-        if (ra.ret_unnorm) ra.ret_unnorm[off] = ru;
-        if (ra.value_out) ra.value_out[off] = vo;
-        if (ra.ret_out) ra.ret_out[off] = ro;
-    }
-};
-
-template <int TC, bool VEC>
-__global__ void __launch_bounds__((TC / 4 + 1) * 32) gae_ret_ws_kernel(
-    const float* __restrict__ value, float* __restrict__ next_value, const float* __restrict__ reward,
-    const float* __restrict__ done, const float* __restrict__ traj, float* __restrict__ adv, long long T,
-    long long C, float gamma, float gl, int mask_inplace, RetArgs ra, double* ws_d, unsigned int* ws_join) {
-    pdl_prologue();
-    __shared__ __align__(16) float s_d[GAE_NCHUNK][GAE_CH][TC];
-    __shared__ __align__(16) float s_f[GAE_NCHUNK][GAE_CH][TC];
-    double acc[4] = {0.0, 0.0, 0.0, 0.0};
-    gae_tile_body<TC, VEC>(value, next_value, reward, done, traj, adv, T, C, 1, gamma, gl, mask_inplace,
-                           (long long)blockIdx.x * TC, s_d, s_f, [](long long, bool) {}, ra.vscale,
-                           GaeRetHook{value, ra, &acc});
-    if (ra.stats || ra.adv_stats) ret_stats_join<(TC / 4 + 1) * 32>(acc, ra, (double)T * (double)C, ws_d, ws_join);
-}
-
-template <int TC>
-static int launch_gae_ret(const float* value, float* next_value, const float* reward, const float* done, const float* traj,
-                          float* adv, long long T, long long C, float gamma, float gl, int mask_inplace, bool vec,
-                          const RetArgs& ra, double* ws_d, unsigned int* ws_join, cudaStream_t st) {
-    const int grid = div_up(C, TC);
-    constexpr int NT = (TC / 4 + 1) * 32;
-    if (vec)
-        (void)launch_k(gae_ret_ws_kernel<TC, true>, grid, NT, 0, st, value, next_value, reward, done, traj, adv, T, C, gamma, gl,
-                       mask_inplace, ra, ws_d, ws_join);
-    else
-        (void)launch_k(gae_ret_ws_kernel<TC, false>, grid, NT, 0, st, value, next_value, reward, done, traj, adv, T, C, gamma, gl,
-                       mask_inplace, ra, ws_d, ws_join);
-    return (int)cudaGetLastError();
 }
 
 template <int TC>
@@ -114,9 +54,6 @@ namespace b200rl {
 int gae_scan(const float* value, float* next_value, const float* reward, const float* done, const float* traj_flag, float* adv,
              long long T, long long C, long long A, double gamma_d, double lambda_d, int mask_next_value_inplace,
              float vscale, void* stream);
-int gae_scan_returns(const float* value, float* next_value, const float* reward, const float* done, const float* traj_flag,
-                     float* adv, long long T, long long C, double gamma_d, double lambda_d, int mask_next_value_inplace,
-                     const RetArgs& ra, double* ws_d, unsigned int* ws_join, void* stream);
 }
 
 extern "C" int b200rl_gae(const float* value, float* next_value, const float* reward, const float* done,
@@ -139,41 +76,13 @@ int b200rl::gae_scan(const float* value, float* next_value, const float* reward,
     cudaStream_t st = (cudaStream_t)stream;
     bool vec = (A == 1) && (C % 4 == 0) && aligned16(value) && aligned16(next_value) && aligned16(reward) &&
                aligned16(adv) && (!done || aligned16(done)) && (!traj_flag || aligned16(traj_flag));
-    // column-tile width: the widest tile that still gives every SM at least ~2 CTAs;
-    // B200RL_GAE_TC=8|16|32 overrides the choice (tuning experiments)
-    static int forced_tc = -1;
-    if (forced_tc < 0) {
-        const char* e = getenv("B200RL_GAE_TC");
-        forced_tc = e ? atoi(e) : 0;
-    }
-    if (forced_tc == 32 || (forced_tc == 0 && C >= 32 * 2 * NUM_SMS))
+    // column-tile width: the widest tile that still gives every SM at least ~2 CTAs
+    if (C >= 32 * 2 * NUM_SMS)
         return launch_gae<32>(value, next_value, reward, done, traj_flag, adv, T, C, A, gamma, gamma_lambda,
                               mask_next_value_inplace, vec, st, vscale);
-    if (forced_tc == 16 || (forced_tc == 0 && C >= 16 * 2 * NUM_SMS))
+    if (C >= 16 * 2 * NUM_SMS)
         return launch_gae<16>(value, next_value, reward, done, traj_flag, adv, T, C, A, gamma, gamma_lambda,
                               mask_next_value_inplace, vec, st, vscale);
     return launch_gae<8>(value, next_value, reward, done, traj_flag, adv, T, C, A, gamma, gamma_lambda,
                          mask_next_value_inplace, vec, st, vscale);
-}
-
-// (T, C) gae with the returns epilogue in the same launch (b200rl_gae_returns, csrc/policy.cu); A == 1
-int b200rl::gae_scan_returns(const float* value, float* next_value, const float* reward, const float* done,
-                             const float* traj_flag, float* adv, long long T, long long C, double gamma_d, double lambda_d,
-                             int mask_next_value_inplace, const RetArgs& ra, double* ws_d, unsigned int* ws_join, void* stream) {
-    using namespace b200rl;
-    const float gamma = (float)gamma_d, gamma_lambda = (float)(gamma_d * lambda_d);
-    if (T < 1 || C < 1 || !value || !next_value || !reward || !adv) return B200RL_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    const bool vec = (C % 4 == 0) && aligned16(value) && aligned16(next_value) && aligned16(reward) && aligned16(adv) &&
-                     (!done || aligned16(done)) && (!traj_flag || aligned16(traj_flag)) &&
-                     (!ra.ret_unnorm || aligned16(ra.ret_unnorm)) && (!ra.value_out || aligned16(ra.value_out)) &&
-                     (!ra.ret_out || aligned16(ra.ret_out));
-    if (C >= 32 * 2 * NUM_SMS)
-        return launch_gae_ret<32>(value, next_value, reward, done, traj_flag, adv, T, C, gamma, gamma_lambda,
-                                  mask_next_value_inplace, vec, ra, ws_d, ws_join, st);
-    if (C >= 16 * 2 * NUM_SMS)
-        return launch_gae_ret<16>(value, next_value, reward, done, traj_flag, adv, T, C, gamma, gamma_lambda,
-                                  mask_next_value_inplace, vec, ra, ws_d, ws_join, st);
-    return launch_gae_ret<8>(value, next_value, reward, done, traj_flag, adv, T, C, gamma, gamma_lambda,
-                             mask_next_value_inplace, vec, ra, ws_d, ws_join, st);
 }

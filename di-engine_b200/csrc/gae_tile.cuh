@@ -41,13 +41,6 @@ __device__ __forceinline__ void chunk_wait(int k) {
     else named_bar_sync<4, COUNT>();
 }
 
-// storer hook of gae_tile_body: called for every group of elements a storer thread writes to `adv` (element offset, the four /
-// one advantage values) -- gae.cu's returns epilogue hangs on it; the default does nothing
-struct GaeNoStoreHook {
-    __device__ __forceinline__ void operator()(long long, const float4&) const {}
-    __device__ __forceinline__ void operator()(long long, float) const {}
-};
-
 constexpr int GAE_CH = 32;      // rows per chunk (one named barrier per chunk)
 constexpr int GAE_NCHUNK = 4;   // chunks per slab of T
 constexpr int GAE_SLAB = GAE_CH * GAE_NCHUNK;
@@ -56,13 +49,12 @@ constexpr int GAE_SLAB = GAE_CH * GAE_NCHUNK;
 // all T.  Thread roles: threadIdx.x < 32 scan warp, the next TC/4 warps loaders (and, once their loads are consumed,
 // storers of the finished chunks).  `on_chunk_done(global_chunk, any)` is called by a whole storer warp after it has
 // stored the adv rows of a 32-row chunk (newest chunk = 0).
-template <int TC, bool VEC, class OnChunk, class StoreHook = GaeNoStoreHook>
+template <int TC, bool VEC, class OnChunk>
 __device__ __forceinline__ void gae_tile_body(
     const float* __restrict__ value, float* __restrict__ next_value, const float* __restrict__ reward,
     const float* __restrict__ done, const float* __restrict__ traj, float* __restrict__ adv, long long T,
     long long C, long long A, float gamma, float gl, int mask_inplace, long long c0,
-    float (*s_d)[GAE_CH][TC], float (*s_f)[GAE_CH][TC], OnChunk on_chunk_done, float vscale = 0.f,
-    StoreHook on_store = StoreHook()) {
+    float (*s_d)[GAE_CH][TC], float (*s_f)[GAE_CH][TC], OnChunk on_chunk_done, float vscale = 0.f) {
     constexpr int NL = (TC / 4) * 32;  // loader threads
     constexpr int NTHREADS = NL + 32;
     const long long Caux = C / A;
@@ -208,17 +200,13 @@ __device__ __forceinline__ void gae_tile_body(
                         if (r >= 0 && c0 + cq < C) {
                             const float4 a4 = *reinterpret_cast<const float4*>(&s_d[k][rr][cq]);
                             stg_stream4(reinterpret_cast<float4*>(adv + (lo + r) * C + c0 + cq), a4);
-                            on_store((lo + r) * C + c0 + cq, a4);
                         }
                     }
                 } else {
                     for (int i = ll; i < GAE_CH * TC; i += 32) {
                         const int rr = i / TC, cc = i % TC;
                         const int r = rtop - rr;
-                        if (r >= 0 && c0 + cc < C) {
-                            adv[(lo + r) * C + c0 + cc] = s_d[k][rr][cc];
-                            on_store((lo + r) * C + c0 + cc, s_d[k][rr][cc]);
-                        }
+                        if (r >= 0 && c0 + cc < C) adv[(lo + r) * C + c0 + cc] = s_d[k][rr][cc];
                     }
                 }
                 on_chunk_done((T - hi) / GAE_CH + k, rtop >= 0);  // called by the whole storer warp

@@ -18,7 +18,6 @@
 //   adv_stats_kernel      {mean, std(unbiased) + 1e-8} of a batch in one launch; the PPO kernels apply the normalisation on load
 //                         (ppo_math.cuh adv_in), normalize_kernel materialises it for callers that want the tensor.
 #include <math.h>
-#include <stdlib.h>
 
 #include "../../include/b200rl.h"
 #include "policy_stats.cuh"
@@ -170,8 +169,8 @@ __global__ void __launch_bounds__(GS_NT) gae_seq_kernel(const float* __restrict_
 
 // ---------------------------------------------------------------------------------------------------------------
 // (T, B) epilogue behind gae_ws_kernel: returns / value-norm / statistics in one elementwise pass.
-// The two statistics are reduced with the one-round-trip scheme of grid_sum_fx on scaled integers (sum of r and of r^2 as
-// doubles); the CTA that completes the second sum joins them through one more atomic.
+// The four sums (r, r^2, adv, adv^2) are reduced per CTA in fp64 and joined across CTAs with fp64 atomics; the CTA that
+// arrives last writes the statistics (ret_stats_join).
 // ---------------------------------------------------------------------------------------------------------------
 template <bool VEC>
 __global__ void __launch_bounds__(256) returns_kernel(const float* __restrict__ value, const float* __restrict__ adv,
@@ -180,26 +179,15 @@ __global__ void __launch_bounds__(256) returns_kernel(const float* __restrict__ 
     pdl_prologue();
     const float vs = ra.vscale;
     double acc[4] = {0.0, 0.0, 0.0, 0.0};
-    auto one = [&](float v, float a, float& ru, float& vo, float& ro) {
-        if (vs != 0.f) v = fmul(v, vs);
-        const float r = fadd(v, a);
-        ru = r;
-        vo = vs != 0.f ? __fdiv_rn(v, vs) : v;
-        ro = vs != 0.f ? __fdiv_rn(r, vs) : r;
-        acc[0] += (double)r;
-        acc[1] += (double)r * (double)r;
-        acc[2] += (double)a;
-        acc[3] += (double)a * (double)a;
-    };
     if (VEC) {  // n % 4 == 0, 16-byte aligned tensors
         const long long n4 = n >> 2;
         for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
             const float4 v = reinterpret_cast<const float4*>(value)[i], a = reinterpret_cast<const float4*>(adv)[i];
             float4 ru, vo, ro;
-            one(v.x, a.x, ru.x, vo.x, ro.x);
-            one(v.y, a.y, ru.y, vo.y, ro.y);
-            one(v.z, a.z, ru.z, vo.z, ro.z);
-            one(v.w, a.w, ru.w, vo.w, ro.w);
+            ret_one(vs, v.x, a.x, ru.x, vo.x, ro.x, acc);
+            ret_one(vs, v.y, a.y, ru.y, vo.y, ro.y, acc);
+            ret_one(vs, v.z, a.z, ru.z, vo.z, ro.z, acc);
+            ret_one(vs, v.w, a.w, ru.w, vo.w, ro.w, acc);
             if (ra.ret_unnorm) reinterpret_cast<float4*>(ra.ret_unnorm)[i] = ru;
             if (ra.value_out) reinterpret_cast<float4*>(ra.value_out)[i] = vo;
             if (ra.ret_out) reinterpret_cast<float4*>(ra.ret_out)[i] = ro;
@@ -207,39 +195,14 @@ __global__ void __launch_bounds__(256) returns_kernel(const float* __restrict__ 
     } else {
         for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
             float ru, vo, ro;
-            one(value[i], adv[i], ru, vo, ro);
+            ret_one(vs, value[i], adv[i], ru, vo, ro, acc);
             if (ra.ret_unnorm) ra.ret_unnorm[i] = ru;
             if (ra.value_out) ra.value_out[i] = vo;
             if (ra.ret_out) ra.ret_out[i] = ro;
         }
     }
     if (!ra.stats && !ra.adv_stats) return;
-    double tot[4];
-    block_sum_d<4, 256>(acc, tot);
-    if (threadIdx.x == 0) {
-        // fp64 atomics: order-dependent in the last bits of a double only (the results are rounded to fp32 afterwards)
-#pragma unroll
-        for (int k = 0; k < 4; ++k) atomicAdd(ws_d + k, tot[k]);
-        __threadfence();
-        const unsigned int t = atomicAdd(ws_join, 1u);
-        if (t == gridDim.x - 1) {
-            __threadfence();
-            double s[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                s[k] = atomicAdd(ws_d + k, 0.0);
-                ws_d[k] = 0.0;
-            }
-            const double nn = (double)n, m = s[0] / nn;
-            if (ra.stats) {
-                ra.stats[0] = (float)m;
-                ra.stats[1] = (float)fmax(s[1] / nn - m * m, 0.0);
-                ra.stats[2] = (float)nn;
-            }
-            if (ra.adv_stats) write_adv_stats(ra.adv_stats, s[2], s[3], nn);
-            *ws_join = 0u;
-        }
-    }
+    ret_stats_join<256>(acc, ra, (double)n, ws_d, ws_join);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -308,9 +271,6 @@ __global__ void __launch_bounds__(256) impala_mask_kernel(const float* __restric
 using namespace b200rl;
 
 namespace b200rl {
-int gae_scan_returns(const float* value, float* next_value, const float* reward, const float* done, const float* traj_flag,
-                     float* adv, long long T, long long C, double gamma_d, double lambda_d, int mask_next_value_inplace,
-                     const RetArgs& ra, double* ws_d, unsigned int* ws_join, void* stream);
 int gae_scan(const float* value, float* next_value, const float* reward, const float* done, const float* traj_flag, float* adv,
              long long T, long long C, long long A, double gamma_d, double lambda_d, int mask_next_value_inplace,
              float vscale, void* stream);
@@ -366,19 +326,7 @@ extern "C" int b200rl_gae_returns(const float* value, float* next_value, const f
         return (int)cudaGetLastError();
     }
     // (T, B): the streaming scan (value_norm scaling applied on load), then one elementwise epilogue launch (returns_kernel).
-    // B200RL_GAE_RET_FUSED=1: the epilogue rides in the scan kernel's storer stage instead (gae.cu gae_ret_ws_kernel, one
-    // launch) -- built and parity-tested, but no faster: the storer warps then wait on the value re-read and the statistics
-    // join lengthens the kernel's tail by what the second launch cost.
-    static int fused_epi = -1;
-    if (fused_epi < 0) {
-        const char* e = getenv("B200RL_GAE_RET_FUSED");
-        fused_epi = (e && e[0] == '1') ? 1 : 0;
-    }
-    const int split = !fused_epi;
     const bool want_epi = unnormalized_return || value_out || return_out || stats3 || adv_stats2;
-    if (want_epi && A == 1 && !split)
-        return gae_scan_returns(value, next_value, reward, done, traj_flag, adv, T, C, gamma, lambda_, mask_next_value_inplace, ra,
-                                ws_doubles(workspace), ws_joins(workspace), stream);
     int rc = gae_scan(value, next_value, reward, done, traj_flag, adv, T, C, A, gamma, lambda_, mask_next_value_inplace,
                       (float)value_scale, stream);
     if (rc != 0) return rc;

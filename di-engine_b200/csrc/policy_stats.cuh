@@ -1,5 +1,5 @@
 #pragma once
-// Shared by policy.cu and gae.cu: the batch-level pieces PPOPolicy wraps around gae (ding/policy/ppo.py:274-306) -- returns,
+// Used by policy.cu: the batch-level pieces PPOPolicy wraps around gae (ding/policy/ppo.py:274-306) -- returns,
 // value-norm scaling and the two sets of batch statistics -- as an epilogue argument block plus its reductions.
 #include <math.h>
 

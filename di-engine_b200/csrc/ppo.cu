@@ -29,9 +29,11 @@
 
 namespace b200rl {
 
-template <int NC, int WHAT, int RPT>
+template <int NC, int WHAT>
 __global__ void __launch_bounds__(PPO_THREADS) ppo_tile_kernel(PpoArgs a, float* out, float* ws) {
-    constexpr int PPO_R = PPO_CT * RPT;  // rows per tile
+    // rows per tile: one per consumer thread (256-row tiles can help the forward-only variant, not the gradient-writing
+    // ones or the gae -> ppo -> verify sequence)
+    constexpr int PPO_R = PPO_CT;
     pdl_prologue();
     extern __shared__ __align__(128) unsigned char smem[];
     constexpr bool GRADS = (WHAT != PPO_FWD);
@@ -42,7 +44,7 @@ __global__ void __launch_bounds__(PPO_THREADS) ppo_tile_kernel(PpoArgs a, float*
     const bool is_producer = wid == PPO_CW;  // warp 4: TMA issue only
     const bool has_pre = a.logit_pre != nullptr, has_w = a.weight != nullptr;
     const PpoTileLayout L = ppo_layout(N, has_pre, has_w, PPO_R);
-    const int warp_out_bytes = 32 * RPT * N * 4;  // one warp's gradient rows of a tile (32*RPT consecutive rows)
+    const int warp_out_bytes = 32 * N * 4;  // one warp's gradient rows of a tile (32 consecutive rows)
     unsigned char* outbuf = smem + PPO_STAGES * L.stage_bytes;
     uint64_t* full = reinterpret_cast<uint64_t*>(outbuf + (GRADS ? PPO_OUTBUFS * L.logit_bytes : 0));
     uint64_t* empty = full + PPO_STAGES;
@@ -110,6 +112,7 @@ __global__ void __launch_bounds__(PPO_THREADS) ppo_tile_kernel(PpoArgs a, float*
         }
     } else {
     // ---- consumer warps: warp w owns rows [32w, 32w+32) of every tile; no CTA-wide barrier in this loop ------------
+    const int rit = wid * 32 + lane;  // this thread's row in every tile
     for (int i = 0; i < my_n; ++i) {
         const long long t = blockIdx.x + (long long)i * gridDim.x;
         const long long row0 = t * PPO_R;
@@ -119,11 +122,8 @@ __global__ void __launch_bounds__(PPO_THREADS) ppo_tile_kernel(PpoArgs a, float*
         if (full_tile) {
             mbar_wait(&full[sg], (uint32_t)((i / PPO_STAGES) & 1));
         } else {
-            // ragged last tile: every thread fetches its own rows into their own slots of the stage (no sharing)
-#pragma unroll
-            for (int q = 0; q < RPT; ++q) {
-                const int rit = (wid * RPT + q) * 32 + lane;
-                if (rit >= tail_rows) continue;
+            // ragged last tile: every thread fetches its own row into its own slots of the stage (no sharing)
+            if (rit < tail_rows) {
                 float* d0 = reinterpret_cast<float*>(st) + rit * N;
                 float* d1 = reinterpret_cast<float*>(st + L.off_old) + rit * N;
                 float* d2 = reinterpret_cast<float*>(st + L.off_pre) + rit * N;
@@ -141,23 +141,18 @@ __global__ void __launch_bounds__(PPO_THREADS) ppo_tile_kernel(PpoArgs a, float*
             }
         }
         // this warp's slice of the gradient-tile ring (2 buffers per warp inside the CTA's output area)
-        float* gtile = reinterpret_cast<float*>(outbuf + (wid * 2 + (i & 1)) * warp_out_bytes) - wid * 32 * RPT * N;
-#pragma unroll
-        for (int q = 0; q < RPT; ++q) {
-            const int rit = (wid * RPT + q) * 32 + lane;  // row in tile: a warp covers 32*RPT consecutive rows
-            if ((full_tile || rit < tail_rows) && !(a.dbg & 1)) {
-                const float adv = reinterpret_cast<const float*>(st + L.off_adv)[rit];
-                ppo_row_compute<NC, LOSSES, GRADS>(a, L, st, rit, N, adv, full_tile, gtile, row0, up, acc);
-            }
+        float* gtile = reinterpret_cast<float*>(outbuf + (wid * 2 + (i & 1)) * warp_out_bytes) - wid * 32 * N;
+        if (full_tile || rit < tail_rows) {
+            const float adv = reinterpret_cast<const float*>(st + L.off_adv)[rit];
+            ppo_row_compute<NC, LOSSES, GRADS>(a, L, st, rit, N, adv, full_tile, gtile, row0, up, acc);
         }
         if (full_tile) {
-            if (GRADS && !(a.dbg & 6)) {
+            if (GRADS) {
                 // hand this warp's 32 gradient rows to the TMA store engine; keep at most one store reading smem
                 fence_proxy_async_smem();
                 __syncwarp();
                 if (lane == 0) {
-                    tma_store_1d(a.grad_logit + (row0 + wid * 32 * RPT) * N, gtile + wid * 32 * RPT * N,
-                                 warp_out_bytes);
+                    tma_store_1d(a.grad_logit + (row0 + wid * 32) * N, gtile + wid * 32 * N, warp_out_bytes);
                     tma_store_commit();
                     tma_store_wait_read<1>();
                 }
@@ -356,13 +351,13 @@ __global__ void __launch_bounds__(NT) ppo_value_kernel(const float* __restrict__
 }
 
 // launch geometry of the persistent kernel: SM count x resident CTAs per SM for this instantiation / smem size
-template <int NC, int WHAT, int RPT>
+template <int NC, int WHAT>
 static int launch_tile(const PpoArgs& a, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
-    constexpr int PPO_R = PPO_CT * RPT;
+    constexpr int PPO_R = PPO_CT;
     const PpoTileLayout L = ppo_layout(a.N, a.logit_pre != nullptr, a.weight != nullptr, PPO_R);
     const size_t smem = (size_t)PPO_STAGES * L.stage_bytes + (WHAT != PPO_FWD ? (size_t)PPO_OUTBUFS * L.logit_bytes : 0) +
                         2 * PPO_STAGES * sizeof(uint64_t);
-    auto kern = ppo_tile_kernel<NC, WHAT, RPT>;
+    auto kern = ppo_tile_kernel<NC, WHAT>;
     static int sm_count = 0;
     static size_t smem_set = 0;
     cudaError_t e;
@@ -386,14 +381,6 @@ static int launch_tile(const PpoArgs& a, float* out, float* ws, size_t ws_bytes,
         occ_smem = smem;
     }
     if (per_sm < 1) return B200RL_ERR_ARG;
-    {
-        static int cap = -1;
-        if (cap < 0) {
-            const char* e = getenv("B200RL_PPO_CTAS");
-            cap = e ? atoi(e) : 0;
-        }
-        if (cap > 0 && cap < per_sm) per_sm = cap;
-    }
     const long long n_tiles = (a.S + PPO_R - 1) / PPO_R;
     // the verification launch that follows a fused forward normally exits at once: keep its grid to one CTA per SM
     long long grid = (long long)sm_count * ((WHAT == PPO_BWD && a.g_used) ? 1 : per_sm);
@@ -411,35 +398,15 @@ static int launch_tile(const PpoArgs& a, float* out, float* ws, size_t ws_bytes,
     return (int)cudaGetLastError();
 }
 
-// rows per consumer thread (B200RL_PPO_RPT overrides; tools/exp_step.py compares the choices).  The forward-only kernel
-// can gain from 256-row tiles, the gradient-writing variants do not, and the gae -> ppo -> verify sequence prefers 128-row
-// tiles, so 1 is the default.
-static int pick_rpt(long long S) {
-    static int forced = -1;
-    if (forced < 0) {
-        const char* e = getenv("B200RL_PPO_RPT");
-        forced = e ? atoi(e) : 0;
-    }
-    if (forced == 1 || forced == 2 || forced == 4) return forced;
-    (void)S;
-    return 1;
-}
-
 template <int WHAT>
 static int dispatch_tile(const PpoArgs& a, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
-    const int rpt = pick_rpt(a.S);
     switch (a.N) {
-#define B200RL_CASE(n)                                                           \
-    case n:                                                                      \
-        if (rpt == 4) return launch_tile<n, WHAT, 4>(a, out, ws, ws_bytes, st);  \
-        if (rpt == 2) return launch_tile<n, WHAT, 2>(a, out, ws, ws_bytes, st);  \
-        return launch_tile<n, WHAT, 1>(a, out, ws, ws_bytes, st);
+#define B200RL_CASE(n) \
+    case n: return launch_tile<n, WHAT>(a, out, ws, ws_bytes, st);
         B200RL_CASE(2) B200RL_CASE(3) B200RL_CASE(4) B200RL_CASE(5) B200RL_CASE(6) B200RL_CASE(7) B200RL_CASE(8)
         B200RL_CASE(9) B200RL_CASE(10) B200RL_CASE(12) B200RL_CASE(14) B200RL_CASE(16) B200RL_CASE(18)
 #undef B200RL_CASE
-        default:
-            if (rpt >= 2) return launch_tile<0, WHAT, 2>(a, out, ws, ws_bytes, st);
-            return launch_tile<0, WHAT, 1>(a, out, ws, ws_bytes, st);
+        default: return launch_tile<0, WHAT>(a, out, ws, ws_bytes, st);
     }
 }
 
@@ -459,14 +426,6 @@ static int fill_args(PpoArgs& a, const float* logit_new, const float* logit_old,
     a.S = S; a.G = (int)G; a.N = (int)N; a.clip = (float)clip_ratio; a.clip_lo = (float)(1.0 - clip_ratio);
     a.clip_hi = (float)(1.0 + clip_ratio); a.dual_clip = (float)dual_clip;
     a.use_value_clip = use_value_clip; a.kl_type = kl_type;
-    {
-        static int dbg = -1;
-        if (dbg < 0) {
-            const char* e = getenv("B200RL_PPO_DBG");
-            dbg = e ? atoi(e) : 0;
-        }
-        a.dbg = dbg;
-    }
     if (S < 0 || G < 1 || N < 1) return B200RL_ERR_ARG;
     if (!logit_new || !logit_old || !action || !value_new || !value_old || !adv || !return_) return B200RL_ERR_ARG;
     if (kl_type < 1 || kl_type > 3) return B200RL_ERR_ARG;

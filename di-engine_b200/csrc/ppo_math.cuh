@@ -41,7 +41,6 @@ struct PpoArgs {
     // nullable, (S): happo_error's per-sample factor (the other agents' ratio product, ding/rl_utils/happo.py:124-125): the
     // selected surrogate is multiplied by it before the dual clip
     const float* factor;
-    int dbg;        // tuning experiments only (B200RL_PPO_DBG): 1 = consumers skip the row math, 2 = skip gradient stores
 };
 
 // d(selected surrogate)/d(ratio) with torch's tie rules: min/max split the gradient 0.5/0.5 on equality, clamp passes
@@ -92,7 +91,6 @@ __device__ __forceinline__ float value_term(float v, float v_old, float ret, flo
 constexpr int PPO_CW = 4;                       // consumer warps per CTA
 constexpr int PPO_CT = PPO_CW * 32;            // consumer threads per CTA
 constexpr int PPO_THREADS = PPO_CT + 32;      // + one producer warp
-// rows per tile = PPO_CT * RPT (RPT rows per consumer thread): TMA issue rate per SM is bounded per OPERATION, so the bytes per bulk copy decide the load bandwidth -- RPT = 2 doubles them
 constexpr int PPO_STAGES = 3;   // input ring depth
 constexpr int PPO_OUTBUFS = 2;  // gradient tile ring depth (per warp)
 enum { PPO_FWD = 0, PPO_FWD_GRAD = 1, PPO_BWD = 2 };
@@ -308,8 +306,7 @@ template <int NC, bool LOSSES, bool GRADS>
 __device__ __forceinline__ void ppo_row_compute(const PpoArgs& a, const PpoTileLayout& L, const unsigned char* st,
                                                 int tid, int N, float adv, bool full_tile, float* gtile,
                                                 long long row0, const PpoUpstream& up, float (&acc)[6]) {
-    const bool via_smem = full_tile && !(a.dbg & 4);
-    float* gr = GRADS ? (via_smem ? gtile + tid * N : a.grad_logit + (row0 + tid) * N) : nullptr;
+    float* gr = GRADS ? (full_tile ? gtile + tid * N : a.grad_logit + (row0 + tid) * N) : nullptr;
     float* gv = GRADS ? a.grad_value + row0 + tid : nullptr;
     ppo_row_compute_to<NC, LOSSES, GRADS>(a, L, st, tid, N, adv, gr, gv, up, acc, a.factor ? a.factor[row0 + tid] : 1.f);
 }

@@ -26,8 +26,7 @@ namespace b200rl {
 
 constexpr int VW_CW = 8;
 constexpr int VW_CT = VW_CW * 32;        // consumer threads = transitions per chunk
-constexpr int VW_LW = 1;                 // loader warps (2: warp 0 target logits, warp 1 the rest -- slower)
-constexpr int VW_THREADS = VW_CT + VW_LW * 32 + 32;  // consumers + loaders + scanner
+constexpr int VW_THREADS = VW_CT + 32 + 32;  // consumers + loader warp + scanner warp
 constexpr int VW_MAX_STAGES = 4;
 // tile width TC (template parameter): 16 columns x 16 time steps per chunk, or 32 x 8 when 16-column tiles would outnumber
 // the resident CTAs (two per SM): a second wave of 16-column tiles leaves the second half of the kernel under-subscribed,
@@ -53,7 +52,6 @@ struct VtFusedArgs {
     float* grad_logit;        // (T*B, N), nullable = losses only
     float* grad_value;        // (T+1, B)
     int trace;
-    int loader;  // streaming kernel's loader warp: number of leading stages copied with warp_copy_rows (0 = flat loop only, default: all)
 };
 
 // timeline instrumentation (B200RL_FUSED_TRACE=1, tools/trace_vt.py): 64 globaltimer stamps per CTA at workspace word 65536;
@@ -95,7 +93,7 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
     const int off_vs = off_is + VW_CT * 4;                 // [R+1][TC] vs rows (row R = the row above the chunk)
     const int stage_bytes = off_vs + (VW_R + 1) * VW_ROW;  // multiple of 64
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * stage_bytes);
-    uint64_t* full = bars;                           // [S] stage landed (32 * VW_LW loader-lane arrivals)
+    uint64_t* full = bars;                           // [S] stage landed (32 loader-lane arrivals)
     uint64_t* is_ready = bars + VW_MAX_STAGES;       // [S] phase A done (VW_CW arrivals)
     uint64_t* vs_ready = bars + 2 * VW_MAX_STAGES;   // [S] scanner done (1 arrival)
     uint64_t* done = bars + 3 * VW_MAX_STAGES;       // [S] phase B done: stage free (VW_CW arrivals)
@@ -106,7 +104,7 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
 
     if (tid == 0) {
         for (int s = 0; s < VW_MAX_STAGES; ++s) {
-            mbar_init(&full[s], VW_LW * 32);
+            mbar_init(&full[s], 32);
             mbar_init(&is_ready[s], VW_CW);
             mbar_init(&vs_ready[s], 1);
             mbar_init(&done[s], VW_CW);
@@ -144,7 +142,7 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
     const VwItem first{(long long)blockIdx.x, 0};
     float acc[3] = {0.f, 0.f, 0.f};
 
-    if (wid >= VW_CW && wid < VW_CW + VW_LW) {
+    if (wid == VW_CW) {
         // =============================================== loader ===========================================================
         auto rows_of = [&](unsigned char* dst, const void* src, long long t0, long long c0, int esz, int jmin, int W) {
             const int P = VW_TC * esz / 16, Pv = W * esz / 16;
@@ -168,7 +166,7 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
             const int jmin = t0 < 0 ? (int)-t0 : 0;
             const int W = (int)((B - c0) < VW_TC ? (B - c0) : VW_TC);
             unsigned char* st = smem + s * stage_bytes;
-            if (VW_LW == 1 && jmin == 0 && W == VW_TC && j < a.loader) {
+            if (jmin == 0 && W == VW_TC) {
                 // full chunk of a full tile: lane-owns-a-piece-column copies (common.cuh warp_copy_rows); a row segment is
                 // TC * esz / 16 pieces = (TC / 4) * (N | 2 | 1) for logits | actions | weights
                 const uint32_t sb = smem_u32(st);
@@ -178,19 +176,17 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
                 warp_copy_rows<VW_TC / 4, VW_R, 2>(sb + off_act, a.action + e0, B * 8, 2, lane);
                 if (has_w) warp_copy_rows<VW_TC / 4, VW_R, 1>(sb + off_w, a.weight + e0, B * 4, 1, lane);
             } else {
-                if (wid == VW_CW || VW_LW == 1) rows_of(st, a.target, t0, c0, N * 4, jmin, W);
-                if (wid != VW_CW || VW_LW == 1) {
-                    rows_of(st + off_beh, a.behaviour, t0, c0, N * 4, jmin, W);
-                    rows_of(st + off_act, a.action, t0, c0, 8, jmin, W);
-                    if (has_w) rows_of(st + off_w, a.weight, t0, c0, 4, jmin, W);
-                }
+                rows_of(st, a.target, t0, c0, N * 4, jmin, W);
+                rows_of(st + off_beh, a.behaviour, t0, c0, N * 4, jmin, W);
+                rows_of(st + off_act, a.action, t0, c0, 8, jmin, W);
+                if (has_w) rows_of(st + off_w, a.weight, t0, c0, 4, jmin, W);
             }
             cpa_mbar_arrive(&full[s]);
             if (tid == VW_CT && j < 8) VW_TRACE(49 + 2 * j);
             if (++s == S) { s = 0; ph ^= 1; }
             item_next(it);
         }
-    } else if (wid == VW_CW + VW_LW) {
+    } else if (wid == VW_CW + 1) {
         // =============================================== scanner ==========================================================
         // value rows t0 .. t0+R (R+1 rows: the bootstrap row T belongs to the newest chunk) and reward rows t0 .. t0+R-1 of
         // chunk k go to stage k % S; TC/4 16-byte pieces per row and tensor
@@ -663,22 +659,11 @@ __global__ void __launch_bounds__(VR_NT) vtrace_res_kernel(VtFusedArgs a, float*
     if (!a.verify) grid_store_partials<3, VR_NT>(acc, ws);  // summed by finalize_sums_kernel
 }
 
-// widest tile that leaves at least two CTAs per SM (227 KB of shared memory per SM, 1 KB reserved per CTA); 0 = no fit
 static int g_vt_impl = 0;  // b200rl_vtrace_set_impl: 0 = automatic, 1 = streaming column tiles only, 2 = resident tiles first
-static int vr_env() {
-    static int forced = -1;
-    if (forced < 0) {
-        const char* e = getenv("B200RL_VT_RES");  // 0 = never, 4 | 8 = that tile width (and before the streaming kernel)
-        forced = e ? atoi(e) : -2;
-    }
-    return forced;
-}
-static bool vr_forced() { return vr_env() == 4 || vr_env() == 8 || g_vt_impl == 2; }
+// widest tile that leaves at least two CTAs per SM (227 KB of shared memory per SM, 1 KB reserved per CTA); 0 = no fit
 static int vr_pick_tc(const VtFusedArgs& a) {
-    const int forced = vr_env();
-    if (forced == 0 || g_vt_impl == 1 || a.N < 2) return 0;
+    if (g_vt_impl == 1 || a.N < 2) return 0;
     const bool has_w = a.weight != nullptr;
-    if (forced == 4 || forced == 8) return vr_smem_bytes(a.T, a.N, has_w, forced) <= 226 * 1024 ? forced : 0;
     if (a.B % 8 == 0 && vr_smem_bytes(a.T, a.N, has_w, 8) <= 112 * 1024) return 8;
     if (vr_smem_bytes(a.T, a.N, has_w, 4) <= 112 * 1024) return 4;
     return 0;
@@ -783,14 +768,8 @@ static int launch_vtws(const VtFusedArgs& a, float* out, float* ws, size_t ws_by
 
 template <bool GRADS>
 static int dispatch_vtws(const VtFusedArgs& a, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
-    // 32-column tiles when the 16-column tiles would not all be resident at once (two CTAs per SM);
-    // B200RL_VT_TC = 16 | 32 overrides (tuning)
-    static int forced = -1;
-    if (forced < 0) {
-        const char* e = getenv("B200RL_VT_TC");
-        forced = e ? atoi(e) : 0;
-    }
-    const bool wide = forced == 32 || (forced != 16 && (a.B + 15) / 16 > 2 * NUM_SMS && a.B >= 32);
+    // 32-column tiles when the 16-column tiles would not all be resident at once (two CTAs per SM)
+    const bool wide = (a.B + 15) / 16 > 2 * NUM_SMS && a.B >= 32;
     switch (a.N) {
 #define B200RL_CASE(n)                                                         \
     case n:                                                                    \
@@ -822,12 +801,6 @@ static void fill_vt(VtFusedArgs& a, const float* target_output, const float* beh
         tr = (e && e[0] == '1') ? 1 : 0;
     }
     a.trace = tr;
-    static int ld = -1;
-    if (ld < 0) {
-        const char* e = getenv("B200RL_VT_LOADER");  // leading stages copied cheaply (experiments); default: every stage
-        ld = e ? atoi(e) : (1 << 30);
-    }
-    a.loader = ld;
 }
 
 extern "C" int b200rl_vtrace_set_impl(int impl) {
@@ -846,12 +819,7 @@ extern "C" int b200rl_vtrace_fused_supported(const float* target_output, const f
     fill_vt(a, target_output, behaviour_output, action, value, reward, weight, T, B, N, 0.99, 0.95, 1.0, 1.0, 1.0);
     a.grad_logit = const_cast<float*>(grad_target_output);
     a.grad_value = const_cast<float*>(grad_value);
-    static int off = -1;
-    if (off < 0) {
-        const char* e = getenv("B200RL_VTRACE_FUSED");
-        off = (e && e[0] == '0') ? 1 : 0;
-    }
-    return (!off && (vtres_tc(a) || vtws_ok(a))) ? 1 : 0;
+    return (vtres_tc(a) || vtws_ok(a)) ? 1 : 0;
 }
 
 extern "C" int b200rl_vtrace_fwd_grad(const float* target_output, const float* behaviour_output, const long long* action,
@@ -874,8 +842,8 @@ extern "C" int b200rl_vtrace_fwd_grad(const float* target_output, const float* b
     a.g_used = g_used; a.g_hint = g_hint; a.grad_logit = grad_target_output; a.grad_value = grad_value;
     cudaStream_t st = (cudaStream_t)stream;
     // streaming column tiles wherever they fit (faster: they overlap loads with the scan); resident tiles take the shapes
-    // they cannot (N > 14: no three-stage ring) -- B200RL_VT_RES=4|8 forces them (experiments)
-    const int rtc = (vtws_ok(a) && !vr_forced()) ? 0 : vtres_tc(a);
+    // they cannot (N > 14: no three-stage ring), and every shape they fit under b200rl_vtrace_set_impl(2)
+    const int rtc = (vtws_ok(a) && g_vt_impl != 2) ? 0 : vtres_tc(a);
     if (rtc == 8)
         return grads ? dispatch_vtres<true, 8>(a, out3, workspace, workspace_bytes, st)
                      : dispatch_vtres<false, 8>(a, out3, workspace, workspace_bytes, st);

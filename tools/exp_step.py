@@ -1,10 +1,11 @@
-"""Tuning experiments: time the learner step variants under the env knobs (B200RL_PPO_RPT, B200RL_PPO_CTAS...)."""
+"""Time the learner step variants at config D's shape: ppo_fwd_grad, ppo_fwd and gae alone, the one-launch step, and the
+three-launch and one-launch steps with their backward check."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import bench
 from tools.bench_ops import timed
-res = {'rpt': os.environ.get('B200RL_PPO_RPT', 'auto'), 'ctas': os.environ.get('B200RL_PPO_CTAS', '-')}
+res = {}
 sets = [bench.DeviceStep(bench.make_batch(i), 'cuda:0', fused=True) for i in range(6)]
 for s in sets:
     s.gae()
