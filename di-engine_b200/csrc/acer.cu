@@ -120,9 +120,8 @@ extern "C" int b200rl_acer_policy_fwd(const float* q_values, const float* q_retr
     if (!q_values || !q_retraces || !v_pred || !target_logit || !actions || !ratio || !actor_loss || !bias_correction_loss ||
         M < 1 || N < 1)
         return B200RL_ERR_ARG;
-    (void)launch_k(acer_policy_fwd_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, q_values, q_retraces, v_pred,
-                   target_logit, actions, ratio, M, (int)N, (float)c_clip_ratio, actor_loss, bias_correction_loss);
-    return (int)cudaGetLastError();
+    return launch_k(acer_policy_fwd_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, q_values, q_retraces, v_pred,
+                    target_logit, actions, ratio, M, (int)N, (float)c_clip_ratio, actor_loss, bias_correction_loss);
 }
 
 extern "C" int b200rl_acer_policy_bwd(const float* q_values, const float* q_retraces, const float* v_pred,
@@ -131,31 +130,27 @@ extern "C" int b200rl_acer_policy_bwd(const float* q_values, const float* q_retr
                                       double c_clip_ratio, float* grad_target_logit, void* stream) {
     if (!q_values || !q_retraces || !v_pred || !target_logit || !actions || !ratio || !grad_target_logit || M < 1 || N < 1)
         return B200RL_ERR_ARG;
-    (void)launch_k(acer_policy_bwd_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, q_values, q_retraces, v_pred,
-                   target_logit, actions, ratio, g_actor, g_bias, M, (int)N, (float)c_clip_ratio, grad_target_logit);
-    return (int)cudaGetLastError();
+    return launch_k(acer_policy_bwd_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, q_values, q_retraces, v_pred,
+                    target_logit, actions, ratio, g_actor, g_bias, M, (int)N, (float)c_clip_ratio, grad_target_logit);
 }
 
 extern "C" int b200rl_acer_value_fwd(const float* q_values, const float* q_retraces, const long long* actions, long long M,
                                      long long N, float* critic_loss, void* stream) {
     if (!q_values || !q_retraces || !actions || !critic_loss || M < 1 || N < 1) return B200RL_ERR_ARG;
-    (void)launch_k(acer_value_fwd_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, q_values, q_retraces, actions, M, (int)N,
-                   critic_loss);
-    return (int)cudaGetLastError();
+    return launch_k(acer_value_fwd_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, q_values, q_retraces, actions, M, (int)N,
+                    critic_loss);
 }
 
 extern "C" int b200rl_acer_value_bwd(const float* q_values, const float* q_retraces, const long long* actions,
                                      const float* g_loss, long long M, long long N, float* grad_q_values, void* stream) {
     if (!q_values || !q_retraces || !actions || !g_loss || !grad_q_values || M < 1 || N < 1) return B200RL_ERR_ARG;
-    (void)launch_k(acer_value_bwd_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, q_values, q_retraces, actions, g_loss, M,
-                   (int)N, grad_q_values);
-    return (int)cudaGetLastError();
+    return launch_k(acer_value_bwd_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, q_values, q_retraces, actions, g_loss, M,
+                    (int)N, grad_q_values);
 }
 
 extern "C" int b200rl_acer_trust_region(const float* actor_gradient, const float* avg_logit, long long M, long long N,
                                         double trust_region_value, float* out, void* stream) {
     if (!actor_gradient || !avg_logit || !out || M < 1 || N < 1) return B200RL_ERR_ARG;
-    (void)launch_k(acer_trust_region_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, actor_gradient, avg_logit, M, (int)N,
-                   (float)trust_region_value, out);
-    return (int)cudaGetLastError();
+    return launch_k(acer_trust_region_kernel, acer_grid(M), 256, 0, (cudaStream_t)stream, actor_gradient, avg_logit, M, (int)N,
+                    (float)trust_region_value, out);
 }

@@ -34,9 +34,8 @@ extern "C" int b200rl_probe_copy(const float* src, float* dst, long long n_float
     long long grid = (long long)b200rl::NUM_SMS * ctas_per_sm;
     const long long need = (n4 + 255) / 256;
     if (grid > need) grid = need > 0 ? need : 1;
-    (void)b200rl::launch_k(b200rl::probe_copy_kernel, (int)grid, 256, 0, (cudaStream_t)stream, reinterpret_cast<const float4*>(src),
-                                                                          reinterpret_cast<float4*>(dst), n4);
-    return (int)cudaGetLastError();
+    return b200rl::launch_k(b200rl::probe_copy_kernel, (int)grid, 256, 0, (cudaStream_t)stream, reinterpret_cast<const float4*>(src),
+                                                                           reinterpret_cast<float4*>(dst), n4);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -104,9 +103,8 @@ extern "C" int b200rl_p2p_allreduce_mean(const float* local, const unsigned long
     if (!local || !mailbox_ptrs_dev || !seq_dev || !out || n < 1 || n > b200rl::P2P_VALS || world < 1 || world > 64 ||
         rank < 0 || rank >= world)
         return B200RL_ERR_ARG;
-    (void)b200rl::launch_k(b200rl::p2p_allreduce_mean_kernel, 1, 256, 0, (cudaStream_t)stream, local, mailbox_ptrs_dev,
-                           rank, world, n, seq_dev, out);
-    return (int)cudaGetLastError();
+    return b200rl::launch_k(b200rl::p2p_allreduce_mean_kernel, 1, 256, 0, (cudaStream_t)stream, local, mailbox_ptrs_dev,
+                            rank, world, n, seq_dev, out);
 }
 
 extern "C" size_t b200rl_p2p_mailbox_floats(int world) { return (size_t)2 * world * b200rl::P2P_ENTRY; }
@@ -140,7 +138,6 @@ extern "C" int b200rl_p2p_drain_mean(const unsigned long long* mailbox_ptrs_dev,
     if (!mailbox_ptrs_dev || !seq_dev || !out_mean || n < 1 || n > b200rl::P2P_SLOT_VALS || world < 1 || world > 32 ||
         rank < 0 || rank >= world)
         return B200RL_ERR_ARG;
-    (void)b200rl::launch_k(b200rl::p2p_drain_kernel, 1, 256, 0, (cudaStream_t)stream, mailbox_ptrs_dev, rank, world, n,
-                           seq_dev, out_mean);
-    return (int)cudaGetLastError();
+    return b200rl::launch_k(b200rl::p2p_drain_kernel, 1, 256, 0, (cudaStream_t)stream, mailbox_ptrs_dev, rank, world, n,
+                            seq_dev, out_mean);
 }

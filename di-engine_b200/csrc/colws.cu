@@ -380,58 +380,25 @@ static int launch_ws(const FusedArgs& f, float* out, float* ws, size_t ws_bytes,
     const PpoArgs& a = f.p;
     const int stages = cw_pick_stages(f);
     const size_t smem = cw_smem(a.N, a.logit_pre != nullptr, a.weight != nullptr, stages);
-    auto kern = gae_ppo_ws_kernel<NC, GRADS>;
-    static int sm_count = 0;
-    static size_t smem_set = 0;
-    cudaError_t e;
-    if (sm_count == 0) {
-        int dev = 0;
-        if ((e = cudaGetDevice(&dev)) != cudaSuccess) return (int)e;
-        if ((e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return (int)e;
-    }
-    if (smem > smem_set) {
-        if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
-            return (int)e;
-        smem_set = smem;
-    }
-    static size_t occ_smem = (size_t)-1;
-    static int per_sm = 0;
-    if (occ_smem != smem) {
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, CW_THREADS, smem)) != cudaSuccess)
-            return (int)e;
-        occ_smem = smem;
-    }
-    if (per_sm < 1) return B200RL_ERR_ARG;
+    constexpr auto kern = gae_ppo_ws_kernel<NC, GRADS>;
+    int sm_count, per_sm;
+    if (int rc = resident_ctas<kern>(CW_THREADS, smem, sm_count, per_sm)) return rc;
     const long long n_tiles = (f.B + CW_TC - 1) / CW_TC;
     long long grid = (long long)sm_count * per_sm;
     if (grid > n_tiles) grid = n_tiles;
     if (ws_bytes < WS_MIN_BYTES || !ws_partials_fit((long long)(grid * 6), ws_bytes))
         return B200RL_ERR_WORKSPACE;
-    (void)launch_k(kern, (int)grid, CW_THREADS, smem, st, f, ws, stages);
-    FinalizeArgs fa{};
-    const double is = 1.0 / (double)a.S;
-    fa.scale[0] = is; fa.scale[1] = 0.5 * is; fa.scale[2] = is; fa.scale[3] = a.logit_pre ? is : 0.0;
-    fa.scale[4] = is; fa.scale[5] = is;
-    fa.k = 6; fa.n_blocks = (int)grid;
+    if (int rc = launch_k(kern, (int)grid, CW_THREADS, smem, st, f, ws, stages)) return rc;
+    FinalizeArgs fa = ppo_finalize_args(a.S, a.logit_pre != nullptr, (int)grid);
     // data-parallel training: the finalising threads stage the six scalars for the next step's kernel to publish (common.cuh)
     fa.x.mailboxes = f.x_mailboxes; fa.x.state = f.x_seq; fa.x.out_mean = f.x_out_mean; fa.x.rank = f.x_rank;
     fa.x.world = f.x_world;
-    (void)launch_finalize(ws, out, fa, st);
-    return (int)cudaGetLastError();
+    return launch_finalize(ws, out, fa, st);
 }
 
 template <bool GRADS>
 static int dispatch_ws(const FusedArgs& f, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
-    switch (f.p.N) {
-#define B200RL_CASE(n) \
-    case n:            \
-        return launch_ws<n, GRADS>(f, out, ws, ws_bytes, st);
-        B200RL_CASE(2) B200RL_CASE(3) B200RL_CASE(4) B200RL_CASE(5) B200RL_CASE(6) B200RL_CASE(7) B200RL_CASE(8)
-        B200RL_CASE(9) B200RL_CASE(10) B200RL_CASE(12) B200RL_CASE(14) B200RL_CASE(16) B200RL_CASE(18)
-#undef B200RL_CASE
-        default:
-            return launch_ws<0, GRADS>(f, out, ws, ws_bytes, st);
-    }
+    return with_nc(f.p.N, [&](auto nc) { return launch_ws<nc, GRADS>(f, out, ws, ws_bytes, st); });
 }
 
 int launch_colws(const FusedArgs& f, bool grads, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {

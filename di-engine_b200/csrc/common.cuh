@@ -13,6 +13,8 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <type_traits>
+
 #define B200RL_OK 0
 #ifndef B200RL_ERR_ARG
 #define B200RL_ERR_ARG (-1)
@@ -494,7 +496,8 @@ __device__ __forceinline__ void cpa_mbar_arrive(uint64_t* bar) {
 // kernel in the stream begin launching right away (its launch latency and prologue overlap this kernel's execution) and
 // then waits until all PREVIOUS kernels in the stream have completed and flushed their results -- so the usual stream
 // ordering of memory is preserved while the launch gap between dependent kernels disappears.
-// Host side: launch_k() sets cudaLaunchAttributeProgrammaticStreamSerialization (B200RL_PDL=0 disables it).
+// Host side: launch_k() sets cudaLaunchAttributeProgrammaticStreamSerialization (B200RL_PDL=0 disables it) and returns
+// the launch's own error; an operator returns the error of the first launch that fails and queues nothing after it.
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_prologue() {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -510,6 +513,24 @@ static inline bool pdl_enabled() {
     return v == 1;
 }
 
+// B200RL_FUSED_TRACE=1: the column-tile kernels of colws.cu and vtws.cu store per-CTA %globaltimer stamps in the
+// workspace (tools/trace_col.py)
+static inline bool trace_enabled() {
+    static int v = -1;
+    if (v < 0) {
+        const char* e = getenv("B200RL_FUSED_TRACE");
+        v = (e && e[0] == '1') ? 1 : 0;
+    }
+    return v == 1;
+}
+
+// A failed runtime call also records its error as the thread's last error: clear it, so that the library leaves no
+// error pending for an unrelated later call to pick up, and return it.
+static inline int cuda_rc(cudaError_t e) {
+    if (e != cudaSuccess) (void)cudaGetLastError();
+    return (int)e;
+}
+
 template <typename... KArgs, typename... Args>
 static inline int launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
     cudaLaunchConfig_t cfg{};
@@ -522,11 +543,99 @@ static inline int launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pdl_enabled() ? 1 : 0;
-    return (int)cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+    return cuda_rc(cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...));
 }
 
 static inline int launch_finalize(float* ws, float* out, const FinalizeArgs& fa, cudaStream_t st) {
     return launch_k(finalize_sums_kernel, 1, 256, 0, st, (const float*)ws, out, ws, fa);
+}
+
+// finalize of the six PPO loss sums (policy, value, entropy, kl, approx_kl, clipfrac) over S samples; the kl sum counts
+// only with pretrained logits
+static inline FinalizeArgs ppo_finalize_args(long long S, bool has_pre, int grid) {
+    FinalizeArgs fa{};
+    const double is = 1.0 / (double)S;
+    fa.scale[0] = is; fa.scale[1] = 0.5 * is; fa.scale[2] = is; fa.scale[3] = has_pre ? is : 0.0;
+    fa.scale[4] = is; fa.scale[5] = is;
+    fa.k = 6; fa.n_blocks = grid;
+    return fa;
+}
+
+// finalize of the three V-trace loss sums (policy, value, entropy) over T*B transitions
+static inline FinalizeArgs vtrace_finalize_args(long long T, long long B, int grid) {
+    FinalizeArgs fa{};
+    const double im = 1.0 / ((double)T * (double)B);
+    fa.scale[0] = -im; fa.scale[1] = im; fa.scale[2] = im;
+    fa.k = 3; fa.n_blocks = grid;
+    return fa;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Launch geometry of the persistent kernels, cached per (kernel, device).  The dynamic shared-memory opt-in belongs
+// to the kernel in the current device's context, so a process that runs an operator on one device and then on
+// another has to opt the kernel in on each.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int MAX_DEVICES = 64;  // device ordinals the caches can hold; a larger ordinal is B200RL_ERR_ARG
+
+static inline int current_device(int& dev) {
+    if (int rc = cuda_rc(cudaGetDevice(&dev))) return rc;
+    return (dev >= 0 && dev < MAX_DEVICES) ? B200RL_OK : B200RL_ERR_ARG;
+}
+
+// let kernel K use `smem` bytes of dynamic shared memory on the current device (more than 48 KB needs the opt-in)
+template <auto K>
+static inline int smem_opt_in(size_t smem) {
+    static size_t opted[MAX_DEVICES];  // largest size opted in so far
+    if (smem <= 48 * 1024) return B200RL_OK;
+    int dev = 0;
+    if (int rc = current_device(dev)) return rc;
+    if (smem <= opted[dev]) return B200RL_OK;
+    if (int rc = cuda_rc(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))) return rc;
+    opted[dev] = smem;
+    return B200RL_OK;
+}
+
+// SM count of the current device and CTAs of kernel K (threads, smem) resident per SM; opts K into `smem` first.
+// B200RL_ERR_ARG if not even one CTA fits.  The occupancy is cached for the last smem size asked for on each device.
+template <auto K>
+static inline int resident_ctas(int threads, size_t smem, int& sm_count, int& per_sm) {
+    static int sms[MAX_DEVICES];
+    static size_t occ_smem[MAX_DEVICES];
+    static int occ[MAX_DEVICES];  // 0 = not queried yet
+    if (int rc = smem_opt_in<K>(smem)) return rc;
+    int dev = 0;
+    if (int rc = current_device(dev)) return rc;
+    if (sms[dev] == 0)
+        if (int rc = cuda_rc(cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev))) return rc;
+    if (occ[dev] == 0 || occ_smem[dev] != smem) {
+        if (int rc = cuda_rc(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[dev], K, threads, smem))) return rc;
+        occ_smem[dev] = smem;
+    }
+    sm_count = sms[dev];
+    per_sm = occ[dev];
+    return per_sm < 1 ? B200RL_ERR_ARG : B200RL_OK;
+}
+
+// The instantiation table of the row-width-specialised kernels: f(std::integral_constant<int, N>{}) for
+// N in {2..10, 12, 14, 16, 18}, f(std::integral_constant<int, 0>{}) (the generic kernel) for every other N.
+template <class F>
+static inline int with_nc(int n, F&& f) {
+    switch (n) {
+        case 2: return f(std::integral_constant<int, 2>{});
+        case 3: return f(std::integral_constant<int, 3>{});
+        case 4: return f(std::integral_constant<int, 4>{});
+        case 5: return f(std::integral_constant<int, 5>{});
+        case 6: return f(std::integral_constant<int, 6>{});
+        case 7: return f(std::integral_constant<int, 7>{});
+        case 8: return f(std::integral_constant<int, 8>{});
+        case 9: return f(std::integral_constant<int, 9>{});
+        case 10: return f(std::integral_constant<int, 10>{});
+        case 12: return f(std::integral_constant<int, 12>{});
+        case 14: return f(std::integral_constant<int, 14>{});
+        case 16: return f(std::integral_constant<int, 16>{});
+        case 18: return f(std::integral_constant<int, 18>{});
+        default: return f(std::integral_constant<int, 0>{});
+    }
 }
 
 // per-CTA partial sums live in workspace words [WS_CTRL_WORDS, WS_PARTIAL_LIMIT_WORDS): above them sit the packed accumulators of

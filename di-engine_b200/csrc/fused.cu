@@ -228,48 +228,22 @@ static int launch_fused(const FusedArgs& f, float* out, float* ws, size_t ws_byt
     constexpr int PPO_R = PPO_CT * RPT;
     const PpoArgs& a = f.p;
     const size_t smem = fused_smem(f, GRADS, RPT);
-    auto kern = gae_ppo_kernel<NC, GRADS, RPT>;
-    static int sm_count = 0;
-    static size_t smem_set = 0;
-    cudaError_t e;
-    if (sm_count == 0) {
-        int dev = 0;
-        if ((e = cudaGetDevice(&dev)) != cudaSuccess) return (int)e;
-        if ((e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return (int)e;
-    }
-    if (smem > 48 * 1024 && smem > smem_set) {
-        if (smem > 227 * 1024) return B200RL_ERR_ARG;
-        if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
-            return (int)e;
-        smem_set = smem;
-    }
-    static size_t occ_smem = (size_t)-1;
-    static int per_sm = 0;
-    if (occ_smem != smem) {
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, PPO_THREADS, smem)) != cudaSuccess)
-            return (int)e;
-        occ_smem = smem;
-    }
-    if (per_sm < 1) return B200RL_ERR_ARG;
+    constexpr auto kern = gae_ppo_kernel<NC, GRADS, RPT>;
+    if (smem > 227 * 1024) return B200RL_ERR_ARG;
+    int sm_count, per_sm;
+    if (int rc = resident_ctas<kern>(PPO_THREADS, smem, sm_count, per_sm)) return rc;
     const long long n_tiles = (a.S + PPO_R - 1) / PPO_R;
     long long grid = (long long)sm_count * per_sm;  // never more than can be resident (phase P spins on phase G)
     if (grid > n_tiles) grid = n_tiles;
     if (grid < 1) grid = 1;
     if (!ws_partials_fit((long long)(grid * 6), ws_bytes)) return B200RL_ERR_WORKSPACE;
-    (void)launch_k(kern, (int)grid, PPO_THREADS, smem, st, f, out, ws);
-    {
-        FinalizeArgs fa{};
-        const double is = 1.0 / (double)a.S;
-        fa.scale[0] = is; fa.scale[1] = 0.5 * is; fa.scale[2] = is; fa.scale[3] = a.logit_pre ? is : 0.0;
-        fa.scale[4] = is; fa.scale[5] = is;
-        fa.k = 6; fa.n_blocks = (int)grid;
-        fa.clear_ctrl_from = WS_TILE_CTR; fa.clear_ctrl_n = 1;
-        const long long n_groups = (f.B % PPO_R) == 0 ? f.B / PPO_R : 1;
-        fa.clear_tail_off = WS_CHUNK_CTR_OFF;
-        fa.clear_tail_n = (int)(((f.T + GAE_CH - 1) / GAE_CH) * n_groups);
-        (void)launch_finalize(ws, out, fa, st);
-    }
-    return (int)cudaGetLastError();
+    if (int rc = launch_k(kern, (int)grid, PPO_THREADS, smem, st, f, out, ws)) return rc;
+    FinalizeArgs fa = ppo_finalize_args(a.S, a.logit_pre != nullptr, (int)grid);
+    fa.clear_ctrl_from = WS_TILE_CTR; fa.clear_ctrl_n = 1;
+    const long long n_groups = (f.B % PPO_R) == 0 ? f.B / PPO_R : 1;
+    fa.clear_tail_off = WS_CHUNK_CTR_OFF;
+    fa.clear_tail_n = (int)(((f.T + GAE_CH - 1) / GAE_CH) * n_groups);
+    return launch_finalize(ws, out, fa, st);
 }
 
 template <bool GRADS>
@@ -277,18 +251,10 @@ static int dispatch_fused(const FusedArgs& f, float* out, float* ws, size_t ws_b
     // 2 rows per thread once there are four 256-row tiles per SM, where their layout fits; 1 row fits for every N <= 32.
     // The TMA issue rate per SM is bounded per operation, so 256-row tiles double the bytes each bulk copy moves.
     const int rpt = (f.p.S >= 256LL * NUM_SMS * 4 && fused_smem(f, GRADS, 2) <= 227 * 1024) ? 2 : 1;
-    switch (f.p.N) {
-#define B200RL_CASE(n)                                                             \
-    case n:                                                                        \
-        if (rpt == 2) return launch_fused<n, GRADS, 2>(f, out, ws, ws_bytes, st);  \
-        return launch_fused<n, GRADS, 1>(f, out, ws, ws_bytes, st);
-        B200RL_CASE(2) B200RL_CASE(3) B200RL_CASE(4) B200RL_CASE(5) B200RL_CASE(6) B200RL_CASE(7) B200RL_CASE(8)
-        B200RL_CASE(9) B200RL_CASE(10) B200RL_CASE(12) B200RL_CASE(14) B200RL_CASE(16) B200RL_CASE(18)
-#undef B200RL_CASE
-        default:
-            if (rpt == 2) return launch_fused<0, GRADS, 2>(f, out, ws, ws_bytes, st);
-            return launch_fused<0, GRADS, 1>(f, out, ws, ws_bytes, st);
-    }
+    return with_nc(f.p.N, [&](auto nc) {
+        if (rpt == 2) return launch_fused<nc, GRADS, 2>(f, out, ws, ws_bytes, st);
+        return launch_fused<nc, GRADS, 1>(f, out, ws, ws_bytes, st);
+    });
 }
 
 }  // namespace b200rl
@@ -309,14 +275,7 @@ static void fill_fused(FusedArgs& f, const float* value, float* next_value, cons
     a.kl_type = kl_type;
     f.value = value; f.next_value = next_value; f.reward = reward; f.done = done; f.traj = traj_flag; f.T = T; f.B = B;
     f.gamma = (float)gamma; f.gl = (float)(gamma * lambda_); f.mask_inplace = mask_inplace;
-    {
-        static int tr = -1;
-        if (tr < 0) {
-            const char* e = getenv("B200RL_FUSED_TRACE");
-            tr = (e && e[0] == '1') ? 1 : 0;
-        }
-        f.trace = tr;
-    }
+    f.trace = trace_enabled();
 }
 
 extern "C" int b200rl_gae_ppo_supported(const float* value, const float* next_value, const float* reward,

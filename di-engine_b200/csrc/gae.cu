@@ -40,12 +40,10 @@ static int launch_gae(const float* value, float* next_value, const float* reward
     const int grid = div_up(C, TC);
     constexpr int NT = (TC / 4 + 1) * 32;
     if (vec)
-        (void)launch_k(gae_ws_kernel<TC, true>, grid, NT, 0, st, value, next_value, reward, done, traj, adv, T, C, A, gamma, gl,
-                                                      mask_inplace, vscale);
-    else
-        (void)launch_k(gae_ws_kernel<TC, false>, grid, NT, 0, st, value, next_value, reward, done, traj, adv, T, C, A, gamma, gl,
-                                                       mask_inplace, vscale);
-    return (int)cudaGetLastError();
+        return launch_k(gae_ws_kernel<TC, true>, grid, NT, 0, st, value, next_value, reward, done, traj, adv, T, C, A, gamma,
+                        gl, mask_inplace, vscale);
+    return launch_k(gae_ws_kernel<TC, false>, grid, NT, 0, st, value, next_value, reward, done, traj, adv, T, C, A, gamma,
+                    gl, mask_inplace, vscale);
 }
 
 }  // namespace b200rl

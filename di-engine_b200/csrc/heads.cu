@@ -250,8 +250,7 @@ extern "C" int b200rl_a2c_fwd_grad(const float* logit, const long long* action, 
     a.N = (int)N; a.out = out3; a.grad_logit = grad_logit; a.grad_value = grad_value;
     a.h.g_expected = g_expected; a.h.g_actual[0] = g_policy; a.h.g_actual[1] = g_value; a.h.g_actual[2] = g_entropy;
     a.h.g_used = g_used; a.h.g_hint = g_hint; a.h.verify = verify;
-    (void)launch_k(a2c_kernel, head_grid(S), HD_NT, 0, (cudaStream_t)stream, a, workspace);
-    return (int)cudaGetLastError();
+    return launch_k(a2c_kernel, head_grid(S), HD_NT, 0, (cudaStream_t)stream, a, workspace);
 }
 
 extern "C" int b200rl_ppo_continuous_fwd_grad(
@@ -278,8 +277,7 @@ extern "C" int b200rl_ppo_continuous_fwd_grad(
     a.grad_value = grad_value;
     a.h.g_expected = g_expected; a.h.g_actual[0] = g_policy; a.h.g_actual[1] = g_value; a.h.g_actual[2] = g_entropy;
     a.h.g_actual[3] = g_kl; a.h.g_used = g_used; a.h.g_hint = g_hint; a.h.verify = verify;
-    (void)launch_k(ppoc_kernel, head_grid(S), HD_NT, 0, (cudaStream_t)stream, a, workspace);
-    return (int)cudaGetLastError();
+    return launch_k(ppoc_kernel, head_grid(S), HD_NT, 0, (cudaStream_t)stream, a, workspace);
 }
 
 extern "C" int b200rl_ppg_bc_fwd(const float* logit_new, const float* logit_old, const long long* action, long long B,
@@ -287,7 +285,6 @@ extern "C" int b200rl_ppg_bc_fwd(const float* logit_new, const float* logit_old,
                                  void* stream) {
     if (B < 1 || N < 1 || !logit_new || !logit_old || !action || !loss || !workspace || workspace_bytes < WS_MIN_BYTES)
         return B200RL_ERR_ARG;
-    (void)launch_k(ppg_bc_kernel, head_grid(B), HD_NT, 0, (cudaStream_t)stream, logit_new, logit_old, action, B, (int)N, loss,
-                   dlogit_unit, workspace);
-    return (int)cudaGetLastError();
+    return launch_k(ppg_bc_kernel, head_grid(B), HD_NT, 0, (cudaStream_t)stream, logit_new, logit_old, action, B, (int)N, loss,
+                    dlogit_unit, workspace);
 }

@@ -470,14 +470,12 @@ extern "C" int b200rl_upgo_head_fwd(const float* logit, const long long* action,
         int grid = div_up(TB, NT / 32);
         if (grid > MAX_GRID) grid = MAX_GRID;
         if (!ws_partials_fit((long long)(grid), workspace_bytes)) return B200RL_ERR_WORKSPACE;
-        (void)launch_k(upgo_fwd_kernel<NT, 32>, grid, NT, 0, st, a, workspace);
-    } else {
-        int grid = div_up(TB, NT);
-        if (grid > MAX_GRID) grid = MAX_GRID;
-        if (!ws_partials_fit((long long)(grid), workspace_bytes)) return B200RL_ERR_WORKSPACE;
-        (void)launch_k(upgo_fwd_kernel<NT, 1>, grid, NT, 0, st, a, workspace);
+        return launch_k(upgo_fwd_kernel<NT, 32>, grid, NT, 0, st, a, workspace);
     }
-    return (int)cudaGetLastError();
+    int grid = div_up(TB, NT);
+    if (grid > MAX_GRID) grid = MAX_GRID;
+    if (!ws_partials_fit((long long)(grid), workspace_bytes)) return B200RL_ERR_WORKSPACE;
+    return launch_k(upgo_fwd_kernel<NT, 1>, grid, NT, 0, st, a, workspace);
 }
 
 extern "C" int b200rl_upgo_head_bwd(const float* logit, const long long* action, const float* mask,
@@ -491,9 +489,8 @@ extern "C" int b200rl_upgo_head_bwd(const float* logit, const long long* action,
     cudaStream_t st = (cudaStream_t)stream;
     int grid = N > 64 ? div_up(TB * K, NT / 32) : div_up(TB * K, NT);
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
-    if (N > 64) (void)launch_k(upgo_bwd_kernel<NT, 32>, grid, NT, 0, st, a);
-    else (void)launch_k(upgo_bwd_kernel<NT, 1>, grid, NT, 0, st, a);
-    return (int)cudaGetLastError();
+    if (N > 64) return launch_k(upgo_bwd_kernel<NT, 32>, grid, NT, 0, st, a);
+    return launch_k(upgo_bwd_kernel<NT, 1>, grid, NT, 0, st, a);
 }
 
 extern "C" int b200rl_tb_cross_entropy_fwd(const float* logit, const long long* action, const float* mask, long long TB,
@@ -501,9 +498,8 @@ extern "C" int b200rl_tb_cross_entropy_fwd(const float* logit, const long long* 
     if (TB <= 0 || K < 1 || N < 1 || !logit || !action || !ce) return B200RL_ERR_ARG;
     constexpr int NT = 128;
     cudaStream_t st = (cudaStream_t)stream;
-    if (N > 64) (void)launch_k(tbce_fwd_kernel<NT, 32>, div_up(TB, NT / 32), NT, 0, st, logit, action, mask, TB, (int)K, (int)N, ce);
-    else (void)launch_k(tbce_fwd_kernel<NT, 1>, div_up(TB, NT), NT, 0, st, logit, action, mask, TB, (int)K, (int)N, ce);
-    return (int)cudaGetLastError();
+    if (N > 64) return launch_k(tbce_fwd_kernel<NT, 32>, div_up(TB, NT / 32), NT, 0, st, logit, action, mask, TB, (int)K, (int)N, ce);
+    return launch_k(tbce_fwd_kernel<NT, 1>, div_up(TB, NT), NT, 0, st, logit, action, mask, TB, (int)K, (int)N, ce);
 }
 
 extern "C" int b200rl_tb_cross_entropy_bwd(const float* logit, const long long* action, const float* mask,
@@ -512,9 +508,8 @@ extern "C" int b200rl_tb_cross_entropy_bwd(const float* logit, const long long* 
     if (TB <= 0 || K < 1 || N < 1 || !logit || !action || !g_ce || !grad_logit) return B200RL_ERR_ARG;
     constexpr int NT = 128;
     cudaStream_t st = (cudaStream_t)stream;
-    if (N > 64) (void)launch_k(tbce_bwd_kernel<NT, 32>, div_up(TB * K, NT / 32), NT, 0, st, logit, action, mask, g_ce, TB, (int)K, (int)N, grad_logit);
-    else (void)launch_k(tbce_bwd_kernel<NT, 1>, div_up(TB * K, NT), NT, 0, st, logit, action, mask, g_ce, TB, (int)K, (int)N, grad_logit);
-    return (int)cudaGetLastError();
+    if (N > 64) return launch_k(tbce_bwd_kernel<NT, 32>, div_up(TB * K, NT / 32), NT, 0, st, logit, action, mask, g_ce, TB, (int)K, (int)N, grad_logit);
+    return launch_k(tbce_bwd_kernel<NT, 1>, div_up(TB * K, NT), NT, 0, st, logit, action, mask, g_ce, TB, (int)K, (int)N, grad_logit);
 }
 
 // ===============================================================================================================
@@ -779,45 +774,20 @@ static int launch_vt_tile(const VtArgs& a, cudaStream_t st) {
     } else {
         smem = (size_t)PPO_STAGES * ((2 * logit_bytes + VT_R * 8 + 127) & ~127) + 2 * PPO_STAGES * sizeof(uint64_t);
     }
-    void (*kern)(VtArgs) = BWD ? vt_bwd_tile_kernel<NC> : vt_rows_tile_kernel<NC>;
-    static int sm_count = 0;
-    static size_t smem_set = 0, occ_smem = (size_t)-1;
-    static int per_sm = 0;
-    cudaError_t e;
-    if (sm_count == 0) {
-        int dev = 0;
-        if ((e = cudaGetDevice(&dev)) != cudaSuccess) return (int)e;
-        if ((e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return (int)e;
-    }
-    if (smem > 48 * 1024 && smem > smem_set) {
-        if (smem > 227 * 1024) return B200RL_ERR_ARG;
-        if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
-            return (int)e;
-        smem_set = smem;
-    }
-    if (occ_smem != smem) {
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, PPO_THREADS, smem)) != cudaSuccess)
-            return (int)e;
-        if (per_sm > 6) per_sm = 6;
-        occ_smem = smem;
-    }
-    if (per_sm < 1) return B200RL_ERR_ARG;
+    constexpr void (*kern)(VtArgs) = BWD ? vt_bwd_tile_kernel<NC> : vt_rows_tile_kernel<NC>;
+    if (smem > 227 * 1024) return B200RL_ERR_ARG;
+    int sm_count, per_sm;
+    if (int rc = resident_ctas<kern>(PPO_THREADS, smem, sm_count, per_sm)) return rc;
+    if (per_sm > 6) per_sm = 6;
     const long long n_tiles = (a.T * a.B + VT_R - 1) / VT_R;
     long long grid = (long long)sm_count * per_sm;
     if (grid > n_tiles) grid = n_tiles;
-    (void)launch_k(kern, (int)grid, PPO_THREADS, smem, st, a);
-    return (int)cudaGetLastError();
+    return launch_k(kern, (int)grid, PPO_THREADS, smem, st, a);
 }
 
 template <bool BWD>
 static int dispatch_vt_tile(const VtArgs& a, cudaStream_t st) {
-    switch (a.N) {
-#define B200RL_CASE(n) case n: return launch_vt_tile<n, BWD>(a, st);
-        B200RL_CASE(2) B200RL_CASE(3) B200RL_CASE(4) B200RL_CASE(5) B200RL_CASE(6) B200RL_CASE(7) B200RL_CASE(8)
-        B200RL_CASE(9) B200RL_CASE(10) B200RL_CASE(12) B200RL_CASE(14) B200RL_CASE(16) B200RL_CASE(18)
-#undef B200RL_CASE
-        default: return launch_vt_tile<0, BWD>(a, st);
-    }
+    return with_nc(a.N, [&](auto nc) { return launch_vt_tile<nc, BWD>(a, st); });
 }
 
 static bool vt_tile_ok(const VtArgs& a, bool bwd) {
@@ -833,12 +803,10 @@ static bool vt_tile_ok(const VtArgs& a, bool bwd) {
 static int launch_vt_scan(const VtArgs& a, float* workspace, size_t workspace_bytes, cudaStream_t st) {
     if (a.B >= 16 * 2 * NUM_SMS) {
         if (!ws_partials_fit((long long)(3 * div_up(a.B, 16)), workspace_bytes)) return B200RL_ERR_WORKSPACE;
-        (void)launch_k(vtrace_scan_kernel<16, 256, 64>, div_up(a.B, 16), 256, 0, st, a, workspace);
-    } else {
-        if (!ws_partials_fit((long long)(3 * div_up(a.B, 8)), workspace_bytes)) return B200RL_ERR_WORKSPACE;
-        (void)launch_k(vtrace_scan_kernel<8, 64, 64>, div_up(a.B, 8), 64, 0, st, a, workspace);
+        return launch_k(vtrace_scan_kernel<16, 256, 64>, div_up(a.B, 16), 256, 0, st, a, workspace);
     }
-    return (int)cudaGetLastError();
+    if (!ws_partials_fit((long long)(3 * div_up(a.B, 8)), workspace_bytes)) return B200RL_ERR_WORKSPACE;
+    return launch_k(vtrace_scan_kernel<8, 64, 64>, div_up(a.B, 8), 64, 0, st, a, workspace);
 }
 
 static int vt_mode(const VtArgs& a) {
@@ -867,17 +835,15 @@ extern "C" int b200rl_vtrace_fwd(const float* target_output, const float* behavi
     constexpr int NT = 128;
     const long long M = T * B;
     const int mode = vt_mode(a);
-    if (vt_tile_ok(a, false)) {
-        int rc0 = dispatch_vt_tile<false>(a, st);
-        if (rc0) return rc0;
-    } else if (mode == 0) {
-        (void)launch_k(vtrace_rows_kernel<NT, true>, div_up(M, NT), NT, (size_t)2 * NT * a.N * sizeof(float), st, a);
-    } else if (mode == 1) {
-        (void)launch_k(vtrace_rows_kernel<NT, false>, div_up(M, NT), NT, 0, st, a);
-    } else {
-        (void)launch_k(vtrace_rows_warp_kernel<NT>, div_up(M, NT / 32), NT, 0, st, a);
-    }
-    int rc = (int)cudaGetLastError();
+    int rc;
+    if (vt_tile_ok(a, false))
+        rc = dispatch_vt_tile<false>(a, st);
+    else if (mode == 0)
+        rc = launch_k(vtrace_rows_kernel<NT, true>, div_up(M, NT), NT, (size_t)2 * NT * a.N * sizeof(float), st, a);
+    else if (mode == 1)
+        rc = launch_k(vtrace_rows_kernel<NT, false>, div_up(M, NT), NT, 0, st, a);
+    else
+        rc = launch_k(vtrace_rows_warp_kernel<NT>, div_up(M, NT / 32), NT, 0, st, a);
     if (rc) return rc;
     return launch_vt_scan(a, workspace, workspace_bytes, st);
 }
@@ -899,10 +865,9 @@ extern "C" int b200rl_vtrace_bwd(const float* target_output, const long long* ac
     const long long M = T * B;
     const int mode = vt_mode(a);
     if (vt_tile_ok(a, true)) return dispatch_vt_tile<true>(a, st);
-    if (mode == 0) (void)launch_k(vtrace_bwd_kernel<NT, 0>, div_up(M, NT), NT, (size_t)NT * a.N * sizeof(float), st, a);
-    else if (mode == 1) (void)launch_k(vtrace_bwd_kernel<NT, 1>, div_up(M, NT), NT, 0, st, a);
-    else (void)launch_k(vtrace_bwd_kernel<NT, 2>, div_up(M, NT / 32), NT, 0, st, a);
-    return (int)cudaGetLastError();
+    if (mode == 0) return launch_k(vtrace_bwd_kernel<NT, 0>, div_up(M, NT), NT, (size_t)NT * a.N * sizeof(float), st, a);
+    if (mode == 1) return launch_k(vtrace_bwd_kernel<NT, 1>, div_up(M, NT), NT, 0, st, a);
+    return launch_k(vtrace_bwd_kernel<NT, 2>, div_up(M, NT / 32), NT, 0, st, a);
 }
 
 extern "C" int b200rl_vtrace_continuous_fwd(const float* mu_target, const float* sigma_target, const float* mu_behaviour,
@@ -920,9 +885,7 @@ extern "C" int b200rl_vtrace_continuous_fwd(const float* mu_target, const float*
     r.M = T * B; r.D = (int)D; r.lp_t = lp_saved; r.isw = cpg_saved; r.ent = dv_saved;
     long long grid = div_up(r.M, 256);
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
-    (void)launch_k(vtc_rows_kernel, (int)grid, 256, 0, st, r);
-    int rc = (int)cudaGetLastError();
-    if (rc) return rc;
+    if (int rc = launch_k(vtc_rows_kernel, (int)grid, 256, 0, st, r)) return rc;
     VtArgs a{};
     a.value = value; a.reward = reward; a.weight = weight; a.T = T; a.B = B; a.N = (int)D; a.gamma = (float)gamma;
     a.gamma_lambda = (float)(gamma * lambda_);
@@ -946,6 +909,5 @@ extern "C" int b200rl_vtrace_continuous_bwd(const float* mu_target, const float*
     r.grad_value = grad_value;
     long long grid = div_up(r.M + B, 256);
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
-    (void)launch_k(vtc_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, r);
-    return (int)cudaGetLastError();
+    return launch_k(vtc_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, r);
 }

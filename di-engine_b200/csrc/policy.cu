@@ -286,9 +286,8 @@ extern "C" int b200rl_adv_stats(const float* x, long long n, float* stats2, floa
     long long grid = div_up(n, 256 * 8);
     if (grid > NUM_SMS * 4) grid = NUM_SMS * 4;
     if (grid < 1) grid = 1;
-    (void)launch_k(adv_stats_kernel, (int)grid, 256, 0, (cudaStream_t)stream, x, n, stats2, ws_doubles(workspace),
-                   ws_joins(workspace));
-    return (int)cudaGetLastError();
+    return launch_k(adv_stats_kernel, (int)grid, 256, 0, (cudaStream_t)stream, x, n, stats2, ws_doubles(workspace),
+                    ws_joins(workspace));
 }
 
 extern "C" int b200rl_normalize(const float* x, const float* stats2, long long n, float* out, void* stream) {
@@ -296,8 +295,7 @@ extern "C" int b200rl_normalize(const float* x, const float* stats2, long long n
     if (n == 0) return B200RL_OK;
     long long grid = div_up(n, 256 * 4);
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
-    (void)launch_k(normalize_kernel, (int)grid, 256, 0, (cudaStream_t)stream, x, stats2, n, out);
-    return (int)cudaGetLastError();
+    return launch_k(normalize_kernel, (int)grid, 256, 0, (cudaStream_t)stream, x, stats2, n, out);
 }
 
 extern "C" int b200rl_gae_returns(const float* value, float* next_value, const float* reward, const float* done,
@@ -315,35 +313,25 @@ extern "C" int b200rl_gae_returns(const float* value, float* next_value, const f
     cudaStream_t st = (cudaStream_t)stream;
     if (C == 1 && T <= GS_MAX_T) {  // the real PPO learner's call: one sequence, everything in one launch
         const size_t smem = (size_t)2 * T * sizeof(float);
-        static size_t smem_set = 0;
-        if (smem > 48 * 1024 && smem > smem_set) {
-            cudaError_t e = cudaFuncSetAttribute(gae_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return (int)e;
-            smem_set = smem;
-        }
-        (void)launch_k(gae_seq_kernel, 1, GS_NT, smem, st, value, next_value, reward, done, traj_flag, adv, (int)T,
-                       (float)gamma, (float)(gamma * lambda_), mask_next_value_inplace, ra);
-        return (int)cudaGetLastError();
+        if (int rc = smem_opt_in<gae_seq_kernel>(smem)) return rc;
+        return launch_k(gae_seq_kernel, 1, GS_NT, smem, st, value, next_value, reward, done, traj_flag, adv, (int)T,
+                        (float)gamma, (float)(gamma * lambda_), mask_next_value_inplace, ra);
     }
     // (T, B): the streaming scan (value_norm scaling applied on load), then one elementwise epilogue launch (returns_kernel).
     const bool want_epi = unnormalized_return || value_out || return_out || stats3 || adv_stats2;
     int rc = gae_scan(value, next_value, reward, done, traj_flag, adv, T, C, A, gamma, lambda_, mask_next_value_inplace,
                       (float)value_scale, stream);
-    if (rc != 0) return rc;
-    if (want_epi) {
-        const long long n = T * C;
-        const bool vec = (n % 4 == 0) && aligned16(value) && aligned16(adv) && (!unnormalized_return || aligned16(unnormalized_return)) &&
-                         (!value_out || aligned16(value_out)) && (!return_out || aligned16(return_out));
-        long long grid = div_up(n, 256 * (vec ? 8 : 4));
-        if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
-        if (vec)
-            (void)launch_k(returns_kernel<true>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra, ws_doubles(workspace),
-                           ws_joins(workspace));
-        else
-            (void)launch_k(returns_kernel<false>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra, ws_doubles(workspace),
-                           ws_joins(workspace));
-    }
-    return (int)cudaGetLastError();
+    if (rc != 0 || !want_epi) return rc;
+    const long long n = T * C;
+    const bool vec = (n % 4 == 0) && aligned16(value) && aligned16(adv) && (!unnormalized_return || aligned16(unnormalized_return)) &&
+                     (!value_out || aligned16(value_out)) && (!return_out || aligned16(return_out));
+    long long grid = div_up(n, 256 * (vec ? 8 : 4));
+    if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
+    if (vec)
+        return launch_k(returns_kernel<true>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra, ws_doubles(workspace),
+                        ws_joins(workspace));
+    return launch_k(returns_kernel<false>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra, ws_doubles(workspace),
+                    ws_joins(workspace));
 }
 
 /* rewards / rewards_out / weights_out nullable (the backward pass masks a gradient with values = g, the other outputs off) */
@@ -352,7 +340,6 @@ extern "C" int b200rl_impala_mask(const float* values, const float* rewards, con
     if (!values || !done || !values_out || T < 1 || B < 1 || (rewards_out && !rewards)) return B200RL_ERR_ARG;
     long long grid = div_up((T + 1) * B, 256 * 4);
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
-    (void)launch_k(impala_mask_kernel, (int)grid, 256, 0, (cudaStream_t)stream, values, rewards, done, T, B, values_out,
-                   rewards_out, weights_out);
-    return (int)cudaGetLastError();
+    return launch_k(impala_mask_kernel, (int)grid, 256, 0, (cudaStream_t)stream, values, rewards, done, T, B, values_out,
+                    rewards_out, weights_out);
 }

@@ -357,57 +357,24 @@ static int launch_tile(const PpoArgs& a, float* out, float* ws, size_t ws_bytes,
     const PpoTileLayout L = ppo_layout(a.N, a.logit_pre != nullptr, a.weight != nullptr, PPO_R);
     const size_t smem = (size_t)PPO_STAGES * L.stage_bytes + (WHAT != PPO_FWD ? (size_t)PPO_OUTBUFS * L.logit_bytes : 0) +
                         2 * PPO_STAGES * sizeof(uint64_t);
-    auto kern = ppo_tile_kernel<NC, WHAT>;
-    static int sm_count = 0;
-    static size_t smem_set = 0;
-    cudaError_t e;
-    if (sm_count == 0) {
-        int dev = 0;
-        if ((e = cudaGetDevice(&dev)) != cudaSuccess) return (int)e;
-        if ((e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return (int)e;
-    }
-    if (smem > 48 * 1024 && smem > smem_set) {
-        if (smem > 227 * 1024) return B200RL_ERR_ARG;
-        if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
-            return (int)e;
-        smem_set = smem;
-    }
-    static size_t occ_smem = (size_t)-1;
-    static int per_sm = 0;
-    if (occ_smem != smem) {
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, PPO_THREADS, smem)) != cudaSuccess)
-            return (int)e;
-        if (per_sm > 6) per_sm = 6;
-        occ_smem = smem;
-    }
-    if (per_sm < 1) return B200RL_ERR_ARG;
+    constexpr auto kern = ppo_tile_kernel<NC, WHAT>;
+    if (smem > 227 * 1024) return B200RL_ERR_ARG;
+    int sm_count, per_sm;
+    if (int rc = resident_ctas<kern>(PPO_THREADS, smem, sm_count, per_sm)) return rc;
+    if (per_sm > 6) per_sm = 6;
     const long long n_tiles = (a.S + PPO_R - 1) / PPO_R;
     // the verification launch that follows a fused forward normally exits at once: keep its grid to one CTA per SM
     long long grid = (long long)sm_count * ((WHAT == PPO_BWD && a.g_used) ? 1 : per_sm);
     if (grid > n_tiles) grid = n_tiles;
     if (WHAT != PPO_BWD && !ws_partials_fit((long long)(grid * 6), ws_bytes)) return B200RL_ERR_WORKSPACE;
-    (void)launch_k(kern, (int)grid, PPO_THREADS, smem, st, a, out, ws);
-    if (WHAT != PPO_BWD) {
-        FinalizeArgs fa{};
-        const double is = 1.0 / (double)a.S;
-        fa.scale[0] = is; fa.scale[1] = 0.5 * is; fa.scale[2] = is; fa.scale[3] = a.logit_pre ? is : 0.0;
-        fa.scale[4] = is; fa.scale[5] = is;
-        fa.k = 6; fa.n_blocks = (int)grid;
-        (void)launch_finalize(ws, out, fa, st);
-    }
-    return (int)cudaGetLastError();
+    if (int rc = launch_k(kern, (int)grid, PPO_THREADS, smem, st, a, out, ws)) return rc;
+    if (WHAT == PPO_BWD) return B200RL_OK;
+    return launch_finalize(ws, out, ppo_finalize_args(a.S, a.logit_pre != nullptr, (int)grid), st);
 }
 
 template <int WHAT>
 static int dispatch_tile(const PpoArgs& a, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
-    switch (a.N) {
-#define B200RL_CASE(n) \
-    case n: return launch_tile<n, WHAT>(a, out, ws, ws_bytes, st);
-        B200RL_CASE(2) B200RL_CASE(3) B200RL_CASE(4) B200RL_CASE(5) B200RL_CASE(6) B200RL_CASE(7) B200RL_CASE(8)
-        B200RL_CASE(9) B200RL_CASE(10) B200RL_CASE(12) B200RL_CASE(14) B200RL_CASE(16) B200RL_CASE(18)
-#undef B200RL_CASE
-        default: return launch_tile<0, WHAT>(a, out, ws, ws_bytes, st);
-    }
+    return with_nc(a.N, [&](auto nc) { return launch_tile<nc, WHAT>(a, out, ws, ws_bytes, st); });
 }
 
 }  // namespace b200rl
@@ -450,9 +417,8 @@ extern "C" int b200rl_ppo_fwd(const float* logit_new, const float* logit_old, co
     int grid = warp ? div_up(S, NT / 32) : div_up(S, NT);
     if (grid > NUM_SMS * 16) grid = NUM_SMS * 16;  // grid-stride kernel: the workspace need is bounded whatever S is
     if (!ws_partials_fit((long long)((size_t)grid * 6), workspace_bytes)) return B200RL_ERR_WORKSPACE;
-    if (warp) (void)launch_k(ppo_fwd_kernel<NT, 2>, grid, NT, 0, st, a, out, workspace);
-    else (void)launch_k(ppo_fwd_kernel<NT, 1>, grid, NT, 0, st, a, out, workspace);
-    return (int)cudaGetLastError();
+    if (warp) return launch_k(ppo_fwd_kernel<NT, 2>, grid, NT, 0, st, a, out, workspace);
+    return launch_k(ppo_fwd_kernel<NT, 1>, grid, NT, 0, st, a, out, workspace);
 }
 
 extern "C" int b200rl_ppo_fwd_grad(const float* logit_new, const float* logit_old, const float* logit_pretrained,
@@ -510,9 +476,8 @@ extern "C" int b200rl_ppo_bwd(const float* logit_new, const float* logit_old, co
     if (g_used) return B200RL_ERR_ARG;  // the fused forward only exists on the tile path
     long long grid = a.N > 64 ? div_up(S, NT / 32) : div_up(S, NT);
     if (grid > NUM_SMS * 32) grid = NUM_SMS * 32;  // grid-stride kernels
-    if (a.N > 64) (void)launch_k(ppo_bwd_kernel<NT, 2>, (int)grid, NT, 0, st, a);
-    else (void)launch_k(ppo_bwd_kernel<NT, 1>, (int)grid, NT, 0, st, a);
-    return (int)cudaGetLastError();
+    if (a.N > 64) return launch_k(ppo_bwd_kernel<NT, 2>, (int)grid, NT, 0, st, a);
+    return launch_k(ppo_bwd_kernel<NT, 1>, (int)grid, NT, 0, st, a);
 }
 
 extern "C" int b200rl_ppo_value_fwd(const float* value_new, const float* value_old, const float* return_,
@@ -525,7 +490,6 @@ extern "C" int b200rl_ppo_value_fwd(const float* value_new, const float* value_o
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
     if (workspace_bytes < WS_MIN_BYTES || !ws_partials_fit((long long)(grid), workspace_bytes))
         return B200RL_ERR_WORKSPACE;
-    (void)launch_k(ppo_value_kernel<NT>, (int)grid, NT, 0, (cudaStream_t)stream, value_new, value_old, return_, weight, S,
-                   (float)clip_ratio, use_value_clip, loss, dvalue_unit, workspace);
-    return (int)cudaGetLastError();
+    return launch_k(ppo_value_kernel<NT>, (int)grid, NT, 0, (cudaStream_t)stream, value_new, value_old, return_, weight,
+                    S, (float)clip_ratio, use_value_clip, loss, dvalue_unit, workspace);
 }

@@ -191,8 +191,7 @@ extern "C" int b200rl_quantile_td_fwd(const float* q, const float* next_n_q, con
     a.loss = loss; a.td = td; a.dtheta = dtheta; a.grad_unit = grad_q_unit;
     const int grid = (int)(B < (long long)FX_MAX_GRID ? B : (long long)FX_MAX_GRID);
     const size_t smem = (size_t)(2 * n_tau + n_tau_prime) * sizeof(float);
-    (void)launch_k(quantile_td_kernel, grid, QT_NT, smem, (cudaStream_t)stream, a, workspace);
-    return (int)cudaGetLastError();
+    return launch_k(quantile_td_kernel, grid, QT_NT, smem, (cudaStream_t)stream, a, workspace);
 }
 
 extern "C" int b200rl_quantile_td_bwd(const float* dtheta, const float* weight, const long long* action, const float* g_loss,
@@ -206,6 +205,5 @@ extern "C" int b200rl_quantile_td_bwd(const float* dtheta, const float* weight, 
     const long long n = B * N * n_tau;
     long long grid = (n + 255) / 256;
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
-    (void)launch_k(quantile_td_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, a);
-    return (int)cudaGetLastError();
+    return launch_k(quantile_td_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, a);
 }

@@ -77,7 +77,6 @@ extern "C" int b200rl_q_retraces(const float* q_values, const float* v_pred, con
     using namespace b200rl;
     if (T < 0 || B < 1 || N < 1 || !v_pred || !q_retraces) return B200RL_ERR_ARG;
     if (T > 0 && (!q_values || !rewards || !actions || !weights || !ratio)) return B200RL_ERR_ARG;
-    (void)launch_k(retrace_kernel, div_up(B, RT_TC), RT_NT, 0, (cudaStream_t)stream, q_values, v_pred, rewards, actions, weights,
-                   ratio, T, B, N, (float)gamma, q_retraces);
-    return (int)cudaGetLastError();
+    return launch_k(retrace_kernel, div_up(B, RT_TC), RT_NT, 0, (cudaStream_t)stream, q_values, v_pred, rewards, actions, weights,
+                    ratio, T, B, N, (float)gamma, q_retraces);
 }

@@ -708,16 +708,14 @@ extern "C" int b200rl_qntd_fwd(const float* q, const float* next_n_q, const long
     if (workspace_bytes < WS_MIN_BYTES) return B200RL_ERR_WORKSPACE;
     if (S <= 1024 && !priority_out) {  // the usual replay-buffer batch: ONE CTA, no grid reduction at all
         const int nt = S <= 256 ? 256 : (S <= 512 ? 512 : 1024);
-        if (nt == 256) (void)launch_k(qntd_fwd_kernel<256>, 1, 256, 0, (cudaStream_t)stream, a, workspace);
-        else if (nt == 512) (void)launch_k(qntd_fwd_kernel<512>, 1, 512, 0, (cudaStream_t)stream, a, workspace);
-        else (void)launch_k(qntd_fwd_kernel<1024>, 1, 1024, 0, (cudaStream_t)stream, a, workspace);
-        return (int)cudaGetLastError();
+        if (nt == 256) return launch_k(qntd_fwd_kernel<256>, 1, 256, 0, (cudaStream_t)stream, a, workspace);
+        if (nt == 512) return launch_k(qntd_fwd_kernel<512>, 1, 512, 0, (cudaStream_t)stream, a, workspace);
+        return launch_k(qntd_fwd_kernel<1024>, 1, 1024, 0, (cudaStream_t)stream, a, workspace);
     }
     constexpr int NT = 128;
     const int grid = div_up(S, NT);
     if ((size_t)(WS_CTRL_WORDS + grid) > WS_PARTIAL_LIMIT_WORDS) return B200RL_ERR_WORKSPACE;
-    (void)launch_k(qntd_fwd_kernel<NT>, grid, NT, 0, (cudaStream_t)stream, a, workspace);
-    return (int)cudaGetLastError();
+    return launch_k(qntd_fwd_kernel<NT>, grid, NT, 0, (cudaStream_t)stream, a, workspace);
 }
 
 extern "C" int b200rl_qntd_bwd(const float* dcrit_saved, const float* weight, const long long* action,
@@ -727,9 +725,8 @@ extern "C" int b200rl_qntd_bwd(const float* dcrit_saved, const float* weight, co
     long long grid = div_up(S * G * N, 256);
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;  // grid-stride; the verification launch normally returns at once
     const float inv_div = (float)(1.0 / qntd_loss_div(S, G, seq_len));
-    (void)launch_k(qntd_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, dcrit_saved, weight, action, g_loss, g_td, S,
-                   (int)G, (int)N, group_mean, inv_div, skip_if_unit, grad_q);
-    return (int)cudaGetLastError();
+    return launch_k(qntd_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, dcrit_saved, weight, action, g_loss, g_td, S,
+                    (int)G, (int)N, group_mean, inv_div, skip_if_unit, grad_q);
 }
 
 extern "C" int b200rl_dntd_fwd(const float* dist, const float* next_n_dist, const long long* act,
@@ -757,17 +754,15 @@ extern "C" int b200rl_dntd_fwd(const float* dist, const float* next_n_dist, cons
         constexpr int NT = 256;
         const size_t sm = (size_t)(NT / 32) * n_atom * sizeof(float);
         const int grid = div_up(a.R, NT / 32);
-        if (n_atom <= 64) (void)launch_k(dntd_fwd_kernel<NT, 2>, grid, NT, sm, st, a, workspace);
-        else (void)launch_k(dntd_fwd_kernel<NT, 8>, grid, NT, sm, st, a, workspace);
-        return (int)cudaGetLastError();
+        if (n_atom <= 64) return launch_k(dntd_fwd_kernel<NT, 2>, grid, NT, sm, st, a, workspace);
+        return launch_k(dntd_fwd_kernel<NT, 8>, grid, NT, sm, st, a, workspace);
     }
     constexpr int NT = 128;
     const int grid = div_up(a.R, NT / 32);
     if ((size_t)(WS_CTRL_WORDS + grid) > WS_PARTIAL_LIMIT_WORDS) return B200RL_ERR_WORKSPACE;
     const size_t sm = (size_t)(NT / 32) * n_atom * sizeof(float);
-    if (n_atom <= 64) (void)launch_k(dntd_fwd_kernel<NT, 2>, grid, NT, sm, st, a, workspace);
-    else (void)launch_k(dntd_fwd_kernel<NT, 8>, grid, NT, sm, st, a, workspace);
-    return (int)cudaGetLastError();
+    if (n_atom <= 64) return launch_k(dntd_fwd_kernel<NT, 2>, grid, NT, sm, st, a, workspace);
+    return launch_k(dntd_fwd_kernel<NT, 8>, grid, NT, sm, st, a, workspace);
 }
 
 extern "C" int b200rl_dntd_bwd(const float* dist, const long long* act, const float* proj_saved, const float* weight,
@@ -776,19 +771,14 @@ extern "C" int b200rl_dntd_bwd(const float* dist, const long long* act, const fl
     if (R <= 0 || N < 1 || n_atom < 2 || !dist || !act || !proj_saved || !grad_dist) return B200RL_ERR_ARG;
     long long grid = div_up(R * N * n_atom, 256);
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;  // grid-stride; the verification launch normally returns at once
-    (void)launch_k(dntd_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, dist, act, proj_saved, weight, weight_stride, g_loss, g_td,
-                   R, (int)N, n_atom, skip_if_unit, grad_dist);
-    return (int)cudaGetLastError();
+    return launch_k(dntd_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, dist, act, proj_saved, weight, weight_stride, g_loss, g_td,
+                    R, (int)N, n_atom, skip_if_unit, grad_dist);
 }
 
 template <int MODE, int HEAD>
 static int launch_lambda(const LamArgs& a, float* ws, cudaStream_t st) {
-    if (a.B >= 16 * 2 * NUM_SMS) {
-        (void)launch_k(lambda_scan_kernel<16, 256, 64, MODE, HEAD>, div_up(a.B, 16), 256, 0, st, a, ws);
-    } else {
-        (void)launch_k(lambda_scan_kernel<8, 256, 128, MODE, HEAD>, div_up(a.B, 8), 256, 0, st, a, ws);
-    }
-    return (int)cudaGetLastError();
+    if (a.B >= 16 * 2 * NUM_SMS) return launch_k(lambda_scan_kernel<16, 256, 64, MODE, HEAD>, div_up(a.B, 16), 256, 0, st, a, ws);
+    return launch_k(lambda_scan_kernel<8, 256, 128, MODE, HEAD>, div_up(a.B, 8), 256, 0, st, a, ws);
 }
 
 extern "C" int b200rl_lambda_returns(const float* value, const float* reward, const float* gammas, double gamma,
@@ -813,8 +803,7 @@ extern "C" int b200rl_lambda_returns_bwd(const float* g_ret, const float* value,
     a.done = done; a.gamma = (float)gamma; a.lambda = (float)lambda_; a.upgo_mode = upgo_mode; a.T = T; a.B = B;
     a.g_value = grad_value; a.g_reward = grad_reward; a.g_gammas = grad_gammas; a.g_lambdas = grad_lambdas;
     constexpr int NT = 64;
-    (void)launch_k(lambda_returns_bwd_kernel<NT>, div_up(B, NT), NT, 0, (cudaStream_t)stream, a);
-    return (int)cudaGetLastError();
+    return launch_k(lambda_returns_bwd_kernel<NT>, div_up(B, NT), NT, 0, (cudaStream_t)stream, a);
 }
 
 extern "C" int b200rl_td_lambda_fwd(const float* value, const float* reward, const float* weight, double gamma,
@@ -831,6 +820,5 @@ extern "C" int b200rl_td_lambda_fwd(const float* value, const float* reward, con
 extern "C" int b200rl_scale(const float* g, const float* in, float* out, long long n, void* stream) {
     if (n < 0 || !g || (n > 0 && (!in || !out))) return B200RL_ERR_ARG;
     if (n == 0) return B200RL_OK;
-    (void)launch_k(scale_kernel, div_up(n, 256), 256, 0, (cudaStream_t)stream, g, in, out, n);
-    return (int)cudaGetLastError();
+    return launch_k(scale_kernel, div_up(n, 256), 256, 0, (cudaStream_t)stream, g, in, out, n);
 }

@@ -672,37 +672,18 @@ static int vr_pick_tc(const VtFusedArgs& a) {
 template <int NC, bool GRADS, int TC>
 static int launch_vtres(const VtFusedArgs& a, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
     const size_t smem = vr_smem_bytes(a.T, a.N, a.weight != nullptr, TC);
-    auto kern = vtrace_res_kernel<NC, GRADS, TC>;
-    static size_t smem_set = 0;
-    cudaError_t e;
-    if (smem > smem_set) {
-        if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
-            return (int)e;
-        smem_set = smem;
-    }
+    constexpr auto kern = vtrace_res_kernel<NC, GRADS, TC>;
+    if (int rc = smem_opt_in<kern>(smem)) return rc;
     const long long grid = (a.B + TC - 1) / TC;
     if (ws_bytes < WS_MIN_BYTES || !ws_partials_fit((long long)(grid * 3), ws_bytes)) return B200RL_ERR_WORKSPACE;
-    (void)launch_k(kern, (int)grid, VR_NT, smem, st, a, ws);
-    if (!a.verify) {
-        FinalizeArgs fa{};
-        const double im = 1.0 / ((double)a.T * (double)a.B);
-        fa.scale[0] = -im; fa.scale[1] = im; fa.scale[2] = im;
-        fa.k = 3; fa.n_blocks = (int)grid;
-        (void)launch_finalize(ws, out, fa, st);
-    }
-    return (int)cudaGetLastError();
+    if (int rc = launch_k(kern, (int)grid, VR_NT, smem, st, a, ws)) return rc;
+    if (a.verify) return B200RL_OK;
+    return launch_finalize(ws, out, vtrace_finalize_args(a.T, a.B, (int)grid), st);
 }
 
 template <bool GRADS, int TC>
 static int dispatch_vtres(const VtFusedArgs& a, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
-    switch (a.N) {
-#define B200RL_CASE(n) \
-    case n: return launch_vtres<n, GRADS, TC>(a, out, ws, ws_bytes, st);
-        B200RL_CASE(2) B200RL_CASE(3) B200RL_CASE(4) B200RL_CASE(5) B200RL_CASE(6) B200RL_CASE(7) B200RL_CASE(8)
-        B200RL_CASE(9) B200RL_CASE(10) B200RL_CASE(12) B200RL_CASE(14) B200RL_CASE(16) B200RL_CASE(18)
-#undef B200RL_CASE
-        default: return launch_vtres<0, GRADS, TC>(a, out, ws, ws_bytes, st);
-    }
+    return with_nc(a.N, [&](auto nc) { return launch_vtres<nc, GRADS, TC>(a, out, ws, ws_bytes, st); });
 }
 
 
@@ -728,60 +709,27 @@ template <int NC, bool GRADS, int TC>
 static int launch_vtws(const VtFusedArgs& a, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
     const int stages = vw_pick_stages(a.N, a.weight != nullptr, TC);
     const size_t smem = vw_smem(a.N, a.weight != nullptr, stages, TC);
-    auto kern = vtrace_ws_kernel<NC, GRADS, TC>;
-    static int sm_count = 0;
-    static size_t smem_set = 0;
-    cudaError_t e;
-    if (sm_count == 0) {
-        int dev = 0;
-        if ((e = cudaGetDevice(&dev)) != cudaSuccess) return (int)e;
-        if ((e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return (int)e;
-    }
-    if (smem > smem_set) {
-        if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess)
-            return (int)e;
-        smem_set = smem;
-    }
-    static size_t occ_smem = (size_t)-1;
-    static int per_sm = 0;
-    if (occ_smem != smem) {
-        if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, VW_THREADS, smem)) != cudaSuccess)
-            return (int)e;
-        occ_smem = smem;
-    }
-    if (per_sm < 1) return B200RL_ERR_ARG;
+    constexpr auto kern = vtrace_ws_kernel<NC, GRADS, TC>;
+    int sm_count, per_sm;
+    if (int rc = resident_ctas<kern>(VW_THREADS, smem, sm_count, per_sm)) return rc;
     const long long n_tiles = (a.B + TC - 1) / TC;
     long long grid = (long long)sm_count * per_sm;
     if (grid > n_tiles) grid = n_tiles;
     if (ws_bytes < WS_MIN_BYTES || !ws_partials_fit((long long)(grid * 3), ws_bytes))
         return B200RL_ERR_WORKSPACE;
-    (void)launch_k(kern, (int)grid, VW_THREADS, smem, st, a, ws, stages);
-    if (!a.verify) {
-        FinalizeArgs fa{};
-        const double im = 1.0 / ((double)a.T * (double)a.B);
-        fa.scale[0] = -im; fa.scale[1] = im; fa.scale[2] = im;
-        fa.k = 3; fa.n_blocks = (int)grid;
-        (void)launch_finalize(ws, out, fa, st);
-    }
-    return (int)cudaGetLastError();
+    if (int rc = launch_k(kern, (int)grid, VW_THREADS, smem, st, a, ws, stages)) return rc;
+    if (a.verify) return B200RL_OK;
+    return launch_finalize(ws, out, vtrace_finalize_args(a.T, a.B, (int)grid), st);
 }
 
 template <bool GRADS>
 static int dispatch_vtws(const VtFusedArgs& a, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
     // 32-column tiles when the 16-column tiles would not all be resident at once (two CTAs per SM)
     const bool wide = (a.B + 15) / 16 > 2 * NUM_SMS && a.B >= 32;
-    switch (a.N) {
-#define B200RL_CASE(n)                                                         \
-    case n:                                                                    \
-        if (wide) return launch_vtws<n, GRADS, 32>(a, out, ws, ws_bytes, st);  \
-        return launch_vtws<n, GRADS, 16>(a, out, ws, ws_bytes, st);
-        B200RL_CASE(2) B200RL_CASE(3) B200RL_CASE(4) B200RL_CASE(5) B200RL_CASE(6) B200RL_CASE(7) B200RL_CASE(8)
-        B200RL_CASE(9) B200RL_CASE(10) B200RL_CASE(12) B200RL_CASE(14) B200RL_CASE(16) B200RL_CASE(18)
-#undef B200RL_CASE
-        default:
-            if (wide) return launch_vtws<0, GRADS, 32>(a, out, ws, ws_bytes, st);
-            return launch_vtws<0, GRADS, 16>(a, out, ws, ws_bytes, st);
-    }
+    return with_nc(a.N, [&](auto nc) {
+        if (wide) return launch_vtws<nc, GRADS, 32>(a, out, ws, ws_bytes, st);
+        return launch_vtws<nc, GRADS, 16>(a, out, ws, ws_bytes, st);
+    });
 }
 
 }  // namespace b200rl
@@ -795,12 +743,7 @@ static void fill_vt(VtFusedArgs& a, const float* target_output, const float* beh
     a.weight = weight; a.T = T; a.B = B; a.N = (int)N; a.gamma = (float)gamma;
     a.gamma_lambda = (float)(gamma * lambda_);  // `factor = gamma * lambda_` in python double, vtrace.py:23
     a.rho_clip = (float)rho; a.c_clip = (float)c; a.rho_pg_clip = (float)rho_pg;
-    static int tr = -1;
-    if (tr < 0) {
-        const char* e = getenv("B200RL_FUSED_TRACE");
-        tr = (e && e[0] == '1') ? 1 : 0;
-    }
-    a.trace = tr;
+    a.trace = trace_enabled();
 }
 
 extern "C" int b200rl_vtrace_set_impl(int impl) {

@@ -519,6 +519,39 @@ def test_vtrace_one_launch_under_graph_capture():
         assert torch.equal(res[k], eager[k]), k
 
 
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason='needs two GPUs')
+def test_same_operators_on_two_devices_in_one_process():
+    """The shared-memory opt-in of a kernel holds for one device only: run the one-launch gae -> ppo_error step
+    (config D's N), ppo_error at N = 18 and the one-launch V-trace step (config E's N), whose kernels all need more than
+    48 KB of dynamic shared memory, on cuda:0 and then cuda:1.  Every sum has a fixed order, so the results must be
+    bit-identical across the devices."""
+    _, tg, pg = cases.gae_case(41, 128, 4096, p_done=0.03)
+    _, tp, pp = cases.ppo_case(42, 128 * 4096, 6)
+    _, tq, pq = cases.ppo_case(43, 65536, 18)
+    _, tv, pv = cases.vtrace_case(44, 64, 8192, 6)
+
+    def run(dev):
+        dg = {k: (v.clone().to(dev) if isinstance(v, torch.Tensor) else v) for k, v in tg.items()}
+        td = cases.prepare('ppo', tp, dev)
+        adv, loss, _ = b2.gae_ppo_error(
+            b2.gae_data(dg['value'], dg['next_value'], dg['reward'], dg['done'], dg['traj_flag']),
+            b2.ppo_data(td['logit_new'], td['logit_old'], td['action'], td['value_new'], td['value_old'], None,
+                        td['return_'], td['weight'], td['logit_pretrained']), pg['gamma'], pg['lambda_'], **pp)
+        sum(c * l for c, l in zip(cases.LOSS_MIX['ppo'], loss)).backward()
+        tq_dev, loss_q, _ = _ppo_with_mix(tq, pq, cases.LOSS_MIX['ppo'], device=dev)
+        tv_dev, loss_v, _ = _vtrace_once(tv, pv, (1.0, 0.5, -0.01), device=dev)
+        out = {'adv': adv, 'gae_ppo_logit_grad': td['logit_new'].grad, 'gae_ppo_value_grad': td['value_new'].grad,
+               'ppo_logit_grad': tq_dev['logit_new'].grad, 'ppo_value_grad': tq_dev['value_new'].grad,
+               'vtrace_logit_grad': tv_dev['target_output'].grad, 'vtrace_value_grad': tv_dev['value'].grad}
+        for name, ls in (('gae_ppo', loss), ('ppo', loss_q), ('vtrace', loss_v)):
+            out.update({'%s_loss%d' % (name, i): l for i, l in enumerate(ls)})
+        return {k: v.detach().cpu() for k, v in out.items()}
+
+    first, second = run('cuda:0'), run('cuda:1')
+    for k in first:
+        assert torch.equal(first[k], second[k]), k
+
+
 def test_c_abi_from_plain_c():
     """examples/c_abi_gae.c: gcc-compiled caller with cudaMalloc'd buffers and its own stream -- no torch in the process;
     gae must be bit-identical to the host recurrence, including the in-place next_value mask."""
