@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(HD_NT) a2c_kernel(A2cArgs a, float* ws) {
             const float c_act = g[0] * (-adv * w) * inv_s, c_ent = g[2] * w * inv_s;
             float* gz = a.grad_logit + s * a.N;
             for (int j = 0; j < a.N; ++j) {
-                const float lpj = z[j] - lse;
+                const float lpj = fmaxf(z[j] - lse, kF32Min);  // Categorical.entropy's clamp: 0 * finite at a -inf logit
                 const float p = expf(lpj);
                 float gj = -c_act * p - c_ent * p * (lpj + ent);
                 if (j == act) gj += c_act;

@@ -358,7 +358,7 @@ __global__ void __launch_bounds__(NT) vtrace_bwd_kernel(VtArgs a) {
         const float c_act = g_pg * (-a.isw[row]) * inv_m;  // isw now holds adv*w
         const float c_ent = g_ent * w * inv_m;
         for (int j = lane; j < N; j += L) {
-            const float lp = z[j] - lse;
+            const float lp = fmaxf(z[j] - lse, kF32Min);  // Categorical.entropy's clamp: 0 * finite at a -inf logit
             const float p = expf(lp);
             float gj = -c_act * p - c_ent * p * (lp + ent);
             if (j == act) gj += c_act;
@@ -708,7 +708,7 @@ __global__ void __launch_bounds__(PPO_THREADS) vt_bwd_tile_kernel(VtArgs a) {
                 const float m2 = m * kLog2e;
 #pragma unroll
                 for (int j = 0; j < NR; ++j) {
-                    tn[j] = fmaxf(fmaf(tn[j], kLog2e, -m2), kF32Min);
+                    tn[j] = fmaxf(fmaf(tn[j], kLog2e, -m2), kT2Min);
                     en[j] = ex2f_(tn[j]);
                     s += en[j];
                     u2 = fmaf(en[j], tn[j], u2);
@@ -717,7 +717,7 @@ __global__ void __launch_bounds__(PPO_THREADS) vt_bwd_tile_kernel(VtArgs a) {
                 for (int j = 0; j < N; ++j) m = fmaxf(m, z[j]);
                 const float m2 = m * kLog2e;
                 for (int j = 0; j < N; ++j) {
-                    const float x = fmaxf(fmaf(z[j], kLog2e, -m2), kF32Min);
+                    const float x = fmaxf(fmaf(z[j], kLog2e, -m2), kT2Min);
                     const float e = ex2f_(x);
                     s += e;
                     u2 = fmaf(e, x, u2);
@@ -740,7 +740,7 @@ __global__ void __launch_bounds__(PPO_THREADS) vt_bwd_tile_kernel(VtArgs a) {
             } else {
                 const float m2 = m * kLog2e;
                 for (int j = 0; j < N; ++j) {
-                    const float x = fmaxf(fmaf(z[j], kLog2e, -m2), kF32Min);
+                    const float x = fmaxf(fmaf(z[j], kLog2e, -m2), kT2Min);
                     float g = (ex2f_(x) * inv_sum) * fmaf(-k1, x, k0);
                     if (j == act) g += c_act;
                     gr[j] = g;

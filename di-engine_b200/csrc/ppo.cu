@@ -305,7 +305,7 @@ __global__ void __launch_bounds__(NT) ppo_bwd_kernel(PpoArgs a) {
         const float c_ent = g_ent * w * inv_m;  // d entropy_loss / d H(row)
         // grad z_j = c_act*(1[j==a] - p_j) - c_ent * p_j*(logp_j + H)
         for (int j = lane; j < N; j += L) {
-            const float lp = rn[j] - lse_n;
+            const float lp = fmaxf(rn[j] - lse_n, kF32Min);  // Categorical.entropy's clamp: 0 * finite at a -inf logit
             const float p = expf(lp);
             float gj = -c_act * p - c_ent * p * (lp + ent);
             if (j == act) gj += c_act;

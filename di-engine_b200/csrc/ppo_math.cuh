@@ -102,6 +102,11 @@ __device__ __forceinline__ float rcpf_(float x) { float y; asm("rcp.approx.ftz.f
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 constexpr float kF32Min = -3.402823466e38f;
+// Floor of t_j = (z_j - max)*log2(e) in the tile kernels.  2^t_j is already 0 in fp32 far above it, so it changes no
+// probability and no entropy term (Categorical.entropy clamps log p at finfo.min for the same reason: a -inf logit must
+// give 0, not 0 * -inf).  Unlike finfo.min it keeps k1*t_j finite in the gradient factor p_j*(k0 - k1*t_j) for any
+// |k1| < 1e36, so a masked logit (p_j = 0) gets an exact 0 even when |k1| = |g_ent*w*ln2/S| > 1.
+constexpr float kT2Min = -256.f;
 
 // advantage as the loss sees it: raw, or normalised with the batch statistics (two fp32 ops, as torch evaluates the expression)
 __device__ __forceinline__ float adv_in(const PpoArgs& a, float adv) {
@@ -217,7 +222,7 @@ __device__ __forceinline__ void ppo_row_compute_to(const PpoArgs& a, const PpoTi
                 const float m2 = m * kLog2e;
 #pragma unroll
                 for (int j = 0; j < NR; ++j) {
-                    tn[j] = fmaxf(fmaf(tn[j], kLog2e, -m2), kF32Min);  // clamp: Categorical.entropy's finfo.min
+                    tn[j] = fmaxf(fmaf(tn[j], kLog2e, -m2), kT2Min);
                     en[j] = ex2f_(tn[j]);
                     s += en[j];
                     u2 = fmaf(en[j], tn[j], u2);
@@ -226,7 +231,7 @@ __device__ __forceinline__ void ppo_row_compute_to(const PpoArgs& a, const PpoTi
                 for (int j = 0; j < N; ++j) m = fmaxf(m, zn[j]);
                 const float m2 = m * kLog2e;
                 for (int j = 0; j < N; ++j) {
-                    const float t = fmaxf(fmaf(zn[j], kLog2e, -m2), kF32Min);
+                    const float t = fmaxf(fmaf(zn[j], kLog2e, -m2), kT2Min);
                     const float e = ex2f_(t);
                     s += e;
                     u2 = fmaf(e, t, u2);
@@ -290,7 +295,7 @@ __device__ __forceinline__ void ppo_row_compute_to(const PpoArgs& a, const PpoTi
                 } else {
                     const float m2 = m * kLog2e;
                     for (int j = 0; j < N; ++j) {
-                        const float t = fmaxf(fmaf(zn[j], kLog2e, -m2), kF32Min);
+                        const float t = fmaxf(fmaf(zn[j], kLog2e, -m2), kT2Min);
                         float g = (ex2f_(t) * inv_sum) * fmaf(-k1, t, k0);
                         if (j == act) g += c_act;
                         gr[j] = g;

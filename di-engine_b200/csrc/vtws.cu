@@ -387,6 +387,7 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
                         const float* zt = reinterpret_cast<const float*>(st) + tid * N;
                         const int act = (int)reinterpret_cast<const long long*>(st + off_act)[tid];
                         // grad z_j = g_pg (-adv w / M)(1[j==a] - p_j) + g_ent (w / M)(-p_j (log p_j + H))
+                        // (log p_j clamped at finfo.min as Categorical.entropy does: p_j = 0 at a -inf logit times a finite number)
                         const float c_act = g_pg * (-adv * w) * inv_m, c_ent = g_ent * w * inv_m;
                         float* gz = a.grad_logit + g * N;
                         if (NC) {
@@ -394,7 +395,7 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
                             load_row<NR>(zt, z);
 #pragma unroll
                             for (int k = 0; k < NR; ++k) {
-                                const float lpk = z[k] - p_lse;
+                                const float lpk = fmaxf(z[k] - p_lse, kF32Min);
                                 const float p = ex2f_(lpk * kLog2e);
                                 gj[k] = -c_act * p - c_ent * p * (lpk + p_ent);
                                 if (k == act) gj[k] += c_act;
@@ -402,7 +403,7 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
                             store_row<NR>(gz, gj);
                         } else {
                             for (int k = 0; k < N; ++k) {
-                                const float lpk = zt[k] - p_lse;
+                                const float lpk = fmaxf(zt[k] - p_lse, kF32Min);
                                 const float p = ex2f_(lpk * kLog2e);
                                 float gk = -c_act * p - c_ent * p * (lpk + p_ent);
                                 if (k == act) gk += c_act;
@@ -638,7 +639,7 @@ __global__ void __launch_bounds__(VR_NT) vtrace_res_kernel(VtFusedArgs a, float*
                 load_row<NR>(z, zz);
 #pragma unroll
                 for (int k = 0; k < NR; ++k) {
-                    const float lpk = zz[k] - lse;
+                    const float lpk = fmaxf(zz[k] - lse, kF32Min);
                     const float p = ex2f_(lpk * kLog2e);
                     gj[k] = -c_act * p - c_ent * p * (lpk + ent);
                     if (k == act) gj[k] += c_act;
@@ -646,7 +647,7 @@ __global__ void __launch_bounds__(VR_NT) vtrace_res_kernel(VtFusedArgs a, float*
                 store_row<NR>(gz, gj);
             } else {
                 for (int k = 0; k < N; ++k) {
-                    const float lpk = z[k] - lse;
+                    const float lpk = fmaxf(z[k] - lse, kF32Min);
                     const float p = ex2f_(lpk * kLog2e);
                     float gk = -c_act * p - c_ent * p * (lpk + ent);
                     if (k == act) gk += c_act;
