@@ -41,6 +41,27 @@ __device__ __forceinline__ float criterion_eval(int kind, float param, float x, 
     }
 }
 
+// sum_i reward[i] * gamma^i over the nstep rewards of one sample (td.py:261-265 / :277-281): the first 8 are staged in rwv
+// by the caller, the rest are read at rw[i * Bi]; rf returns gamma^nstep as the loop builds it (reward_factor[nstep]).
+// qntd_fwd_kernel keeps its own inline copy of this loop: through the helper its trip-count code compiles differently.
+__device__ __forceinline__ float nstep_reward_sum(const float (&rwv)[8], const float* __restrict__ rw, size_t Bi, int nstep,
+                                                  float g, float& rf) {
+    float ret = 0.f;
+    rf = 1.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        if (i < nstep) {
+            ret = fadd(ret, fmul(rwv[i], rf));
+            rf = fmul(g, rf);
+        }
+    }
+    for (int i = 8; i < nstep; ++i) {
+        ret = fadd(ret, fmul(rw[i * Bi], rf));
+        rf = fmul(g, rf);
+    }
+    return ret;
+}
+
 struct QntdArgs {
     const float* q;            // (S, G, N)
     const float* next_q;       // (S, G, N)
@@ -202,6 +223,215 @@ __global__ void qntd_bwd_kernel(const float* __restrict__ dcrit, const float* __
             float c = g * (weight ? weight[s] : 1.f) * inv_div;
             if (g_td) c += group_mean ? g_td[s] / (float)G : g_td[r];
             out = c * dcrit[r];
+        }
+        grad_q[i] = out;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// DQfD: n-step TD + 1-step TD + supervised large-margin loss (td.py:870-983, with rescale :986-1090), and R2D3's per-step
+// loop over it (ding/policy/r2d3.py:322-388) as the sequence form.  Per sample:
+//   td_n = crit(q_sa, nstep target), td_1 = crit(q_sa, 1-step target), JE = is_expert * (max_j(q_j + m*[j != a]) - q_sa)
+//   loss = mean(w * (ln*td_n + l1*td_1 + ls*JE)),  per-sample = ln*|td_n| + l1*|td_1| + ls*|JE|,  stats = means of the three
+// ---------------------------------------------------------------------------------------------------------------
+struct DqfdArgs {
+    const float* q;           // (S, N)
+    const float* next_q;      // (S, N)
+    const float* next_q1;     // (S, N) new_n_q_one_step
+    const long long* action;  // (S)
+    const long long* next_action;
+    const long long* next_action1;
+    const float* reward;      // (nstep, S), (S) when cum_reward; sequence form (S = Tseq*Bcol): (Tseq, nstep, Bcol)
+    const float* done;        // (S)
+    const float* done1;       // (S) done_one_step
+    const float* weight;      // (S) or null
+    const float* value_gamma; // null, or stride 0 (0-dim) / 1 (S); n-step target only (td.py:955)
+    long long value_gamma_stride;
+    const float* is_expert;   // (S)
+    long long S;
+    long long Bcol;           // == S, or the batch width of the sequence form (sample s = t*Bcol + b)
+    int N;
+    int nstep;
+    float gamma, gamma_pow_n;
+    int cum_reward;
+    int rescale;
+    float eps, four_eps, two_eps;
+    int criterion;            // criterion_eval kind, or -1: no TD terms (the caller applies its own criterion to target_n/1)
+    float crit_param;
+    float lam_n, lam_1, lam_s, margin;
+    double loss_div;          // loss and statistics = sum / loss_div
+    float prio_max_w, prio_mean_w, prio_div;  // sequence form: priority[b] = max_w*max_t e + mean_w*sum_t e / prio_div
+    float* loss;
+    float* td_err;            // (S)
+    float* stats;             // (3): td_n, td_1, JE
+    float4* saved;            // (S): d crit_n, d crit_1, is_expert, argmax | sign codes << 24 -- what the backward launch needs
+    float* target_n;          // nullable (S): the detached targets, for callers that apply their own criterion
+    float* target_1;
+    float* grad_unit;         // nullable (S, N): d loss / d q for a unit upstream gradient
+    float* priority;          // nullable (Bcol): sequence form only
+};
+
+__device__ __forceinline__ int sgn_code(float x) { return x > 0.f ? 2 : (x < 0.f ? 0 : 1); }  // sgn(x) + 1
+
+template <int NT>
+__global__ void __launch_bounds__(NT) dqfd_fwd_kernel(DqfdArgs a, float* ws) {
+    pdl_prologue();
+    __shared__ float s_ca[NT], s_ck[NT];  // unit-gradient coefficient at the action / at the margin argmax
+    __shared__ int s_act[NT], s_k[NT];
+    const long long s0 = (long long)blockIdx.x * NT;
+    const long long s = s0 + threadIdx.x;
+    const float inv_div = (float)(1.0 / a.loss_div);
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    s_ca[threadIdx.x] = s_ck[threadIdx.x] = 0.f;
+    s_act[threadIdx.x] = s_k[threadIdx.x] = -1;
+    if (s < a.S) {
+        const long long tq_ = s / a.Bcol, b = s - tq_ * a.Bcol;
+        // every per-sample operand is requested before any is used
+        const float* __restrict__ rw = a.cum_reward ? a.reward + s : a.reward + tq_ * a.nstep * a.Bcol + b;
+        const size_t Bi = (size_t)a.Bcol;
+        const int nrw = a.cum_reward ? 1 : a.nstep;
+        float rwv[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) rwv[i] = i < nrw ? rw[i * Bi] : 0.f;
+        // cum_reward: reward[0].unsqueeze(0) is sample 0's reward, broadcast to every sample (td.py:954, :958)
+        const float r1c = a.cum_reward ? a.reward[0] : 0.f;
+        const float dn = a.done[s], dn1 = a.done1[s];
+        const float w = a.weight ? a.weight[s] : 1.f;
+        const float vgl = a.value_gamma ? a.value_gamma[s * a.value_gamma_stride] : a.gamma_pow_n;
+        const float ie = a.is_expert[s];
+        const int act = (int)a.action[s], nact = (int)a.next_action[s], nact1 = (int)a.next_action1[s];
+        const float* __restrict__ qr = a.q + s * a.N;
+        const float q_sa = qr[act], nq = a.next_q[s * a.N + nact], nq1 = a.next_q1[s * a.N + nact1];
+        // supervised margin term: max_j(q_j + l_j), l = margin except 0 at the action (td.py:969-972); the gradient of the max
+        // goes to the FIRST maximal index, as torch.max(dim=1) returns it
+        float mx = 0.f;
+        int k = 0;
+        for (int j0 = 0; j0 < a.N; j0 += 4) {
+            float v[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) v[u] = j0 + u < a.N ? qr[j0 + u] : 0.f;
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int j = j0 + u;
+                if (j < a.N) {
+                    const float x = fadd(v[u], j == act ? 0.f : a.margin);
+                    if (j == 0 || x > mx) {
+                        mx = x;
+                        k = j;
+                    }
+                }
+            }
+        }
+        const float je = fmul(ie, fsub(mx, q_sa));
+        // n-step target (td.py:943-949 / :1045-1054)
+        float tq = nq, tq1 = nq1;
+        if (a.rescale) {
+            tq = value_h_inv(tq, a.eps, a.four_eps, a.two_eps);
+            tq1 = value_h_inv(tq1, a.eps, a.four_eps, a.two_eps);
+        }
+        float ret;
+        if (a.cum_reward) {
+            ret = rwv[0];
+        } else {
+            float rf;
+            ret = nstep_reward_sum(rwv, rw, Bi, a.nstep, a.gamma, rf);
+        }
+        float tn = fadd(ret, fmul(fmul(vgl, tq), fsub(1.f, dn)));
+        // 1-step target: reward[0], gamma ** 1, never value_gamma (td.py:953-964 / :1058-1069)
+        float t1 = fadd(a.cum_reward ? r1c : rwv[0], fmul(fmul(a.gamma, tq1), fsub(1.f, dn1)));
+        if (a.rescale) {
+            tn = value_h(tn, a.eps);
+            t1 = value_h(t1, a.eps);
+        }
+        if (a.target_n) a.target_n[s] = tn;
+        if (a.target_1) a.target_1[s] = t1;
+        float dxn = 0.f, dx1 = 0.f, tdn = 0.f, td1 = 0.f;
+        if (a.criterion >= 0) {
+            tdn = criterion_eval(a.criterion, a.crit_param, q_sa, tn, dxn);
+            td1 = criterion_eval(a.criterion, a.crit_param, q_sa, t1, dx1);
+        }
+        const float comb = fadd(fadd(fmul(a.lam_n, tdn), fmul(a.lam_1, td1)), fmul(a.lam_s, je));  // td.py:974-979
+        a.td_err[s] = fadd(fadd(fmul(a.lam_n, fabsf(tdn)), fmul(a.lam_1, fabsf(td1))), fmul(a.lam_s, fabsf(je)));
+        acc[0] = fmul(comb, w);
+        acc[1] = tdn;
+        acc[2] = td1;
+        acc[3] = je;
+        const int code = sgn_code(tdn) | (sgn_code(td1) << 2) | (sgn_code(je) << 4);
+        a.saved[s] = make_float4(dxn, dx1, ie, __int_as_float(k | (code << 24)));
+        if (a.grad_unit) {
+            const float c = w * inv_div;
+            s_ca[threadIdx.x] = c * (a.lam_n * dxn + a.lam_1 * dx1 - a.lam_s * ie);
+            s_ck[threadIdx.x] = c * a.lam_s * ie;
+            s_act[threadIdx.x] = act;
+            s_k[threadIdx.x] = k;
+        }
+    }
+    if (a.grad_unit) {  // the block's NT gradient rows are contiguous: coalesced stores
+        __syncthreads();
+        const long long rows = (a.S - s0) < NT ? (a.S - s0) : NT;
+        float* gq = a.grad_unit + s0 * a.N;
+        for (long long i = threadIdx.x; i < rows * a.N; i += NT) {
+            const int rr = (int)(i / a.N), j = (int)(i - (long long)rr * a.N);
+            gq[i] = (j == s_act[rr] ? s_ca[rr] : 0.f) + (j == s_k[rr] ? s_ck[rr] : 0.f);
+        }
+    }
+    auto fin = [&](int kk, double t) {
+        const float v = (float)(t / a.loss_div);
+        if (kk == 0) a.loss[0] = v;
+        else a.stats[kk - 1] = v;
+    };
+    if (!a.priority && gridDim.x <= FX_MAX_GRID) {
+        grid_sum_fx<4, NT>(acc, ws, fin);
+        return;
+    }
+    double tot[4];
+    const bool last = grid_sum<4, NT>(acc, tot, ws, 0);
+    if (last && threadIdx.x == 0)
+        for (int kk = 0; kk < 4; ++kk) fin(kk, tot[kk]);
+    if (last && a.priority) {
+        // sequence form (r2d3.py:386-388): the per-sample errors are already sums of absolute values, no abs here
+        const long long Tq = a.S / a.Bcol;
+        for (long long b = threadIdx.x; b < a.Bcol; b += NT) {
+            float mx = 0.f, sm = 0.f;
+            for (long long t = 0; t < Tq; ++t) {
+                const float e = __ldcg(a.td_err + t * a.Bcol + b);
+                mx = (t == 0) ? e : fmaxf(mx, e);
+                sm = fadd(sm, e);
+            }
+            a.priority[b] = fadd(fmul(a.prio_max_w, mx), fmul(a.prio_mean_w, __fdiv_rn(sm, a.prio_div)));
+        }
+    }
+}
+
+// grad_q for arbitrary upstream gradients of the loss (g_loss), the per-sample error (g_td, (S)) and the three statistics
+// (g_sn, g_s1, g_sje); each nullable = 0.  skip_if_unit: grad_q already holds the forward's unit-loss gradient -- verify on the
+// device that only g_loss == 1 arrived and leave at once.
+__global__ void dqfd_bwd_kernel(const float4* __restrict__ saved, const float* __restrict__ weight,
+                                const long long* __restrict__ action, const float* __restrict__ g_loss,
+                                const float* __restrict__ g_td, const float* __restrict__ g_sn, const float* __restrict__ g_s1,
+                                const float* __restrict__ g_sje, long long S, int N, float lam_n, float lam_1, float lam_s,
+                                float inv_div, int skip_if_unit, float* __restrict__ grad_q) {
+    pdl_prologue();
+    const float g = g_loss ? *g_loss : 0.f;
+    if (skip_if_unit && !g_td && !g_sn && !g_s1 && !g_sje && g == 1.f) return;
+    const float gn = g_sn ? *g_sn * inv_div : 0.f, g1 = g_s1 ? *g_s1 * inv_div : 0.f, gj = g_sje ? *g_sje * inv_div : 0.f;
+    const long long n = S * N;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long s = i / N;
+        const int j = (int)(i - s * N);
+        const int act = (int)action[s];
+        const float4 r = saved[s];
+        const int bits = __float_as_int(r.w), k = bits & 0xffffff, code = bits >> 24;
+        float out = 0.f;
+        if (j == act || j == k) {
+            const float sn = (float)((code & 3) - 1), s1 = (float)(((code >> 2) & 3) - 1), sj = (float)(((code >> 4) & 3) - 1);
+            const float gt = g_td ? g_td[s] : 0.f;
+            const float cl = g * (weight ? weight[s] : 1.f) * inv_div;
+            // d / d q_sa of the TD terms, and d / d (max - q_sa) of the margin term, per unit of each output
+            const float ctd = cl * (lam_n * r.x + lam_1 * r.y) + gt * (lam_n * sn * r.x + lam_1 * s1 * r.y) + gn * r.x + g1 * r.y;
+            const float cje = (cl * lam_s + gt * lam_s * sj + gj) * r.z;
+            if (j == act) out = ctd - cje;
+            if (j == k) out += cje;
         }
         grad_q[i] = out;
     }
@@ -727,6 +957,70 @@ extern "C" int b200rl_qntd_bwd(const float* dcrit_saved, const float* weight, co
     const float inv_div = (float)(1.0 / qntd_loss_div(S, G, seq_len));
     return launch_k(qntd_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, dcrit_saved, weight, action, g_loss, g_td, S,
                     (int)G, (int)N, group_mean, inv_div, skip_if_unit, grad_q);
+}
+
+extern "C" int b200rl_dqfd_fwd(const float* q, const float* next_n_q, const float* new_n_q_one_step, const long long* action,
+                               const long long* next_n_action, const long long* next_n_action_one_step, const float* reward,
+                               const float* done, const float* done_one_step, const float* weight, const float* value_gamma,
+                               long long value_gamma_stride, const float* is_expert, long long S, long long N, int nstep,
+                               double gamma, int cum_reward, int rescale, double rescale_eps, int criterion,
+                               double criterion_param, double lambda_n_step_td, double lambda_one_step_td,
+                               double lambda_supervised_loss, double margin, long long seq_len, double priority_mix,
+                               float* loss, float* td_error_per_sample, float* loss_statistics, float* saved,
+                               float* target_n_out, float* target_1_out, float* grad_q_unit, float* priority_out,
+                               float* workspace, size_t workspace_bytes, void* stream) {
+    if (S <= 0 || N < 1 || N >= (1 << 24) || nstep < 1 || !q || !next_n_q || !new_n_q_one_step || !action ||
+        !next_n_action || !next_n_action_one_step || !reward || !done || !done_one_step || !is_expert || !loss ||
+        !td_error_per_sample || !loss_statistics || !saved || !workspace)
+        return B200RL_ERR_ARG;
+    if (criterion < -1 || criterion > 3) return B200RL_ERR_ARG;
+    if (seq_len < 0 || (seq_len > 0 && (S % seq_len != 0 || cum_reward)) || (priority_out && seq_len <= 0))
+        return B200RL_ERR_ARG;
+    DqfdArgs a{};
+    a.q = q; a.next_q = next_n_q; a.next_q1 = new_n_q_one_step; a.action = action; a.next_action = next_n_action;
+    a.next_action1 = next_n_action_one_step; a.reward = reward; a.done = done; a.done1 = done_one_step; a.weight = weight;
+    a.value_gamma = value_gamma; a.value_gamma_stride = value_gamma_stride; a.is_expert = is_expert;
+    a.S = S; a.Bcol = seq_len > 0 ? S / seq_len : S; a.N = (int)N; a.nstep = nstep;
+    a.gamma = (float)gamma; a.gamma_pow_n = (float)pow(gamma, (double)nstep);
+    a.cum_reward = cum_reward; a.rescale = rescale; a.eps = (float)rescale_eps;
+    a.four_eps = (float)(4.0 * rescale_eps); a.two_eps = (float)(2.0 * rescale_eps);
+    a.criterion = criterion; a.crit_param = (float)criterion_param;
+    a.lam_n = (float)lambda_n_step_td; a.lam_1 = (float)lambda_one_step_td; a.lam_s = (float)lambda_supervised_loss;
+    a.margin = (float)margin;
+    a.loss_div = qntd_loss_div(S, 1, seq_len);
+    a.prio_max_w = (float)priority_mix; a.prio_mean_w = (float)(1.0 - priority_mix);
+    a.prio_div = (float)((double)seq_len + 1e-8);
+    a.loss = loss; a.td_err = td_error_per_sample; a.stats = loss_statistics; a.saved = reinterpret_cast<float4*>(saved);
+    a.target_n = target_n_out; a.target_1 = target_1_out; a.grad_unit = grad_q_unit; a.priority = priority_out;
+    if (workspace_bytes < WS_MIN_BYTES) return B200RL_ERR_WORKSPACE;
+    if (reinterpret_cast<uintptr_t>(saved) % 16 != 0) return B200RL_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (S <= 1024 && !priority_out) {  // the usual replay-buffer batch: ONE CTA, no grid reduction at all
+        if (S <= 256) return launch_k(dqfd_fwd_kernel<256>, 1, 256, 0, st, a, workspace);
+        if (S <= 512) return launch_k(dqfd_fwd_kernel<512>, 1, 512, 0, st, a, workspace);
+        return launch_k(dqfd_fwd_kernel<1024>, 1, 1024, 0, st, a, workspace);
+    }
+    constexpr int NT = 128;
+    const long long grid = div_up(S, NT);
+    if (!ws_partials_fit(grid * 4, workspace_bytes)) return B200RL_ERR_WORKSPACE;
+    return launch_k(dqfd_fwd_kernel<NT>, (int)grid, NT, 0, st, a, workspace);
+}
+
+extern "C" int b200rl_dqfd_bwd(const float* saved, const float* weight, const long long* action, const float* g_loss,
+                               const float* g_td, const float* g_loss_statistics_n, const float* g_loss_statistics_1,
+                               const float* g_loss_statistics_je, long long S, long long N, double lambda_n_step_td,
+                               double lambda_one_step_td, double lambda_supervised_loss, long long seq_len, int skip_if_unit,
+                               float* grad_q, void* stream) {
+    if (S <= 0 || N < 1 || N >= (1 << 24) || seq_len < 0 || (seq_len > 0 && S % seq_len != 0) || !saved || !action ||
+        !grad_q || reinterpret_cast<uintptr_t>(saved) % 16 != 0)
+        return B200RL_ERR_ARG;
+    long long grid = div_up(S * N, 256);
+    if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;  // grid-stride; the verification launch normally returns at once
+    const float inv_div = (float)(1.0 / qntd_loss_div(S, 1, seq_len));
+    return launch_k(dqfd_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, reinterpret_cast<const float4*>(saved), weight,
+                    action, g_loss, g_td, g_loss_statistics_n, g_loss_statistics_1, g_loss_statistics_je, S, (int)N,
+                    (float)lambda_n_step_td, (float)lambda_one_step_td, (float)lambda_supervised_loss, inv_div, skip_if_unit,
+                    grad_q);
 }
 
 extern "C" int b200rl_dntd_fwd(const float* dist, const float* next_n_dist, const long long* act,

@@ -435,6 +435,73 @@ class QNStepTDFunction(torch.autograd.Function):
         return (grad_q.view(ctx.q_shape), ) + (None, ) * 23
 
 
+class DQfDTDFunction(torch.autograd.Function):
+    """DQfD n-step + 1-step TD + supervised margin loss (csrc/td.cu dqfd_fwd / dqfd_bwd).  Outputs: loss,
+    td_error_per_sample and the three loss statistics (all differentiable w.r.t. q, as in the reference, td.py:974-983), the
+    two detached targets and (sequence form) the priority mix (non differentiable).
+
+    As QNStepTDFunction: ONE forward launch also writes d loss / d q for a unit upstream gradient, which ``backward`` hands
+    to autograd after a verification launch; any other upstream gradient mix is recomputed on the device.  No host sync."""
+
+    @staticmethod
+    def forward(ctx, q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done, done1, weight, value_gamma,
+                vg_stride, is_expert, S, N, nstep, gamma, cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1,
+                lam_s, margin, seq_len, priority_mix, want_targets, want_priority):
+        dev = q.device
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        td = torch.empty(S, dtype=torch.float32, device=dev)
+        stats = torch.empty(3, dtype=torch.float32, device=dev)
+        saved = torch.empty(S, 4, dtype=torch.float32, device=dev)
+        tn = torch.empty(S, dtype=torch.float32, device=dev) if want_targets else None
+        t1 = torch.empty(S, dtype=torch.float32, device=dev) if want_targets else None
+        prio = torch.empty(S // seq_len, dtype=torch.float32, device=dev) if want_priority else None
+        grad_unit = torch.empty(S, N, dtype=torch.float32, device=dev) if ctx.needs_input_grad[0] else None
+        with on_device(dev):
+            ws = workspace(dev)
+            rc = lib().b200rl_dqfd_fwd(
+                ptr(q), ptr(next_n_q), ptr(next_q1), ptr(action), ptr(next_n_action), ptr(next_action1), ptr(reward),
+                ptr(done), ptr(done1), ptr(weight), ptr(value_gamma), vg_stride, ptr(is_expert), S, N, nstep, gamma,
+                cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1, lam_s, margin, seq_len, priority_mix,
+                ptr(loss), ptr(td), ptr(stats), ptr(saved), ptr(tn), ptr(t1), ptr(grad_unit), ptr(prio), ptr(ws),
+                ws.numel() * 4, stream_ptr()
+            )
+        _lib.check(rc, 'b200rl_dqfd_fwd')
+        ctx.save_for_backward(saved, action, weight)
+        ctx.cfg = (S, N, lam_n, lam_1, lam_s, seq_len)
+        ctx.q_shape = q.shape
+        ctx.spec = grad_unit
+        ctx.set_materialize_grads(False)
+        empty = torch.empty(0, dtype=torch.float32, device=dev)
+        tn, t1, prio = (x if x is not None else empty for x in (tn, t1, prio))
+        ctx.mark_non_differentiable(tn, t1, prio)
+        s_n, s_1, s_je = stats.unbind(0)
+        return loss, td, s_n, s_1, s_je, tn, t1, prio
+
+    @staticmethod
+    def backward(ctx, g_loss, g_td, g_sn, g_s1, g_sje, _g_tn, _g_t1, _g_prio):
+        n_in = 30
+        if g_loss is None and g_td is None and g_sn is None and g_s1 is None and g_sje is None:
+            return (None, ) * n_in
+        saved, action, weight = ctx.saved_tensors
+        S, N, lam_n, lam_1, lam_s, seq_len = ctx.cfg
+        keep = [_g(g) for g in (g_loss, g_sn, g_s1, g_sje)]
+        keep_td, ptd = None, None
+        if g_td is not None:
+            keep_td = f32c(g_td)
+            ptd = keep_td.data_ptr()
+        grad_q, skip = ctx.spec, 0
+        ctx.spec = None  # sole owner now: autograd can adopt the buffer as .grad instead of cloning it
+        if grad_q is not None and g_td is None and g_sn is None and g_s1 is None and g_sje is None:
+            skip = 1
+        else:
+            grad_q = torch.empty(S, N, dtype=torch.float32, device=saved.device)
+        with on_device(saved.device):
+            rc = lib().b200rl_dqfd_bwd(ptr(saved), ptr(weight), ptr(action), keep[0][1], ptd, keep[1][1], keep[2][1],
+                                       keep[3][1], S, N, lam_n, lam_1, lam_s, seq_len, skip, ptr(grad_q), stream_ptr())
+        _lib.check(rc, 'b200rl_dqfd_bwd')
+        return (grad_q.view(ctx.q_shape), ) + (None, ) * (n_in - 1)
+
+
 # ----------------------------------------------------------------------------------------------------------------
 # ACER heads (csrc/acer.cu): un-reduced per-transition losses, plain forward / backward launches
 # ----------------------------------------------------------------------------------------------------------------

@@ -3,7 +3,8 @@
   q_nstep_td_error (td.py:649-719), q_nstep_td_error_with_rescale (:810-867), dist_nstep_td_error (:413-523),
   td_lambda_error (:1539-1571), generalized_lambda_returns (:1574-1605),
   and the 1-step / state-value siblings that reuse the q-n-step kernels (SURVEY section 8f rank 2):
-  q_1step_td_error (:26-72), v_1step_td_error (:529-573), v_nstep_td_error (:579-617).
+  q_1step_td_error (:26-72), v_1step_td_error (:529-573), v_nstep_td_error (:579-617);
+  dqfd_nstep_td_error (:870-983) / dqfd_nstep_td_error_with_rescale (:986-1090) on their own kernel (dqfd_fwd / dqfd_bwd).
 """
 from collections import namedtuple
 from typing import Callable, Optional, Union
@@ -459,6 +460,232 @@ def q_nstep_td_error_sequence(
     if host_out:
         loss, prio, per = loss.cpu(), prio.cpu(), per.cpu()
     return loss, prio, per
+
+
+dqfd_nstep_td_data = namedtuple(
+    'dqfd_nstep_td_data', [
+        'q', 'next_n_q', 'action', 'next_n_action', 'reward', 'done', 'done_one_step', 'weight', 'new_n_q_one_step',
+        'next_n_action_one_step', 'is_expert'
+    ]
+)
+dqfd_nstep_td_seq_data = namedtuple('dqfd_nstep_td_seq_data', dqfd_nstep_td_data._fields)
+
+
+def _dqfd_operands(data, S, dev, rows):
+    """Stage the operands of dqfd_nstep_td_data on ``dev``: q keeps its gradient, the rest are detached; ``rows`` is the
+    (T, B) / (B,) shape of the per-sample operands.  is_expert (float, int or bool tensor, or a python scalar) is
+    widened to float, as the reference's ``is_expert * (...)`` promotes it."""
+    q, next_n_q, action, next_n_action, reward, done, done_one_step, weight, next_q1, next_action1, is_expert = data
+    N = q.shape[-1]
+    qd = ops.f32c(ops.to_device(q, dev), 'q')
+    nq = ops.f32c(ops.to_device(next_n_q.detach(), dev), 'next_n_q')
+    nq1 = ops.f32c(ops.to_device(next_q1.detach(), dev), 'new_n_q_one_step')
+    act = ops.i64c(ops.to_device(action, dev), N)
+    nact = ops.i64c(ops.to_device(next_n_action, dev), N, 'next_n_action')
+    nact1 = ops.i64c(ops.to_device(next_action1, dev), N, 'next_n_action_one_step')
+    r = ops.f32c(ops.to_device(reward.detach(), dev), 'reward')
+    d = ops.f32c(ops.to_device(done.detach(), dev), 'done')
+    d1 = ops.f32c(ops.to_device(done_one_step.detach(), dev), 'done_one_step')
+    if not isinstance(is_expert, torch.Tensor):
+        ie = ops.const_scalar(is_expert, dev).expand(S).contiguous()
+    else:
+        ie = ops.f32c(ops.to_device(is_expert.detach(), dev), 'is_expert')
+    if ie.numel() == 1:
+        ie = ie.reshape(1).expand(S).contiguous()
+    w = None
+    if weight is not None:
+        w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
+        if w.numel() == 1:
+            w = w.reshape(1).expand(S).contiguous()
+    shape = tuple(qd.shape[:-1])
+    if (shape != tuple(rows) or nq.shape != qd.shape or nq1.shape != qd.shape or tuple(act.shape) != shape or
+            tuple(nact.shape) != shape or tuple(nact1.shape) != shape or d.numel() != S or d1.numel() != S or
+            ie.numel() != S or (w is not None and w.numel() != S)):
+        raise ValueError("dqfd: q %s / next_n_q %s / new_n_q_one_step %s / actions %s %s %s / done %s %s / is_expert %s / "
+                         "weight %s do not match %s" %
+                         (tuple(q.shape), tuple(next_n_q.shape), tuple(next_q1.shape), tuple(action.shape),
+                          tuple(next_n_action.shape), tuple(next_action1.shape), tuple(done.shape),
+                          tuple(done_one_step.shape), tuple(ie.shape), None if weight is None else tuple(weight.shape),
+                          tuple(rows)))
+    return qd, nq, nq1, act, nact, nact1, r, d, d1, w, ie
+
+
+def _dqfd_gamma(gamma, cum_reward):
+    if isinstance(gamma, list):
+        raise NotImplementedError("dqfd: a list gamma (the NGU per-sample form) is not supported; no policy passes one")
+    if isinstance(gamma, float) or (cum_reward and isinstance(gamma, int)):  # nstep_return takes floats only (td.py:284)
+        return float(gamma)
+    raise TypeError("The type of gamma should be float or list")
+
+
+def _dqfd(data, gamma, lambda_n_step_td, lambda_supervised_loss, lambda_one_step_td, margin_function, nstep, cum_reward,
+          value_gamma, criterion, rescale, trans_fn=None, inv_trans_fn=None):
+    q, next_n_q, action, next_n_action, reward, done, done_one_step, weight, next_q1, next_action1, is_expert = data
+    assert len(action.shape) == 1, action.shape  # td.py:933 / :1031
+    gamma = _dqfd_gamma(gamma, cum_reward)
+    if not cum_reward:
+        assert reward.shape[0] == nstep  # td.py:257
+    if q.dim() != 2:
+        raise ValueError("dqfd: q must be (B, N), got %s" % (tuple(q.shape), ))
+    B, N = q.shape
+    if tuple(reward.shape) != ((B, ) if cum_reward else (nstep, B)):
+        raise ValueError("dqfd: reward %s does not match B=%d, nstep=%d, cum_reward=%s" %
+                         (tuple(reward.shape), B, nstep, cum_reward))
+    host_out = not q.is_cuda
+    dev = ops.compute_device(q, next_n_q, next_q1)
+    qd, nq, nq1, act, nact, nact1, r, d, d1, w, ie = _dqfd_operands(data, B, dev, (B, ))
+    vg, vg_stride = _value_gamma_arg(value_gamma, B, dev)
+    custom_trans = rescale and (trans_fn is not value_transform or inv_trans_fn is not value_inv_transform)
+    code = _criterion_code(criterion)
+    lam_n, lam_1, lam_s = float(lambda_n_step_td), float(lambda_one_step_td), float(lambda_supervised_loss)
+
+    def kernel(nq_, nq1_, resc, crit, param, want_targets):
+        return ops.DQfDTDFunction.apply(qd, nq_, nq1_, act, nact, nact1, r, d, d1, w, vg, vg_stride, ie, B, N, int(nstep),
+                                        gamma, 1 if cum_reward else 0, resc, 1e-2, crit, param, lam_n, lam_1, lam_s,
+                                        float(margin_function), 0, 0.0, want_targets, False)
+
+    if code is not None and not custom_trans:
+        loss, per, s_n, s_1, s_je, _, _, _ = kernel(nq, nq1, 1 if rescale else 0, code[0], code[1], False)
+    else:
+        # user-supplied transforms / criterion are torch callables: the kernel computes the margin term and the detached
+        # targets (of the inverse-transformed next values), the callables run on the device around them
+        if custom_trans:
+            def inv(x, a):  # inv_trans_fn of the selected entries, at the same place of the row (td.py:1039, :1042)
+                sel = a.reshape(B, 1)
+                return torch.zeros_like(x).scatter_(1, sel, inv_trans_fn(x.gather(1, sel).reshape(B)).reshape(B, 1))
+
+            nq, nq1 = inv(nq, nact), inv(nq1, nact1)
+        loss_je, per_je, _, _, s_je, tn, t1, _ = kernel(nq, nq1, 1 if rescale and not custom_trans else 0, -1, 0.0, True)
+        if custom_trans:
+            tn, t1 = trans_fn(tn), trans_fn(t1)  # td.py:1054, :1071
+        q_sa = qd.gather(1, act.reshape(B, 1)).reshape(B)
+        td_n = criterion(q_sa, tn.detach())
+        td_1 = criterion(q_sa, t1.detach())
+        loss = ((lam_n * td_n + lam_1 * td_1) * (w if w is not None else 1.0)).mean() + loss_je
+        per = lam_n * td_n.abs() + lam_1 * td_1.abs() + per_je
+        s_n, s_1 = td_n.mean(), td_1.mean()
+    if host_out:
+        loss, per, s_n, s_1, s_je = loss.cpu(), per.cpu(), s_n.cpu(), s_1.cpu(), s_je.cpu()
+    return loss, per, (s_n, s_1, s_je)
+
+
+def dqfd_nstep_td_error(
+        data: namedtuple,
+        gamma: float,
+        lambda_n_step_td: float,
+        lambda_supervised_loss: float,
+        margin_function: float,
+        lambda_one_step_td: float = 1.,
+        nstep: int = 1,
+        cum_reward: bool = False,
+        value_gamma: Optional[torch.Tensor] = None,
+        criterion: torch.nn.modules = nn.MSELoss(reduction='none'),
+) -> torch.Tensor:
+    """
+    DQfD loss: n-step TD + 1-step TD + supervised large-margin loss, drop-in for ding/rl_utils/td.py:870-983.
+
+    Shapes: q, next_n_q, new_n_q_one_step (B, N); action, next_n_action, next_n_action_one_step (B,) int64; reward
+    (nstep, B) -- (B,) with ``cum_reward``; done, done_one_step (B,) float multipliers; weight (B,) or None; is_expert (B,)
+    float, int or bool (or a python scalar); value_gamma None, scalar, 0-dim or (B,) -- n-step target only.  gamma a float.
+    As in the reference, the 1-step target uses ``reward[0]``: with ``cum_reward`` that is sample 0's reward, for every
+    sample (td.py:954, :958).  Returns ``(loss, td_error_per_sample, (td_n.mean(), td_1.mean(), JE.mean()))``, all
+    differentiable w.r.t. ``q``; the margin term's gradient goes to the first maximal entry of ``q + margin``.
+    One forward and one backward launch.
+    """
+    return _dqfd(data, gamma, lambda_n_step_td, lambda_supervised_loss, lambda_one_step_td, margin_function, nstep,
+                 cum_reward, value_gamma, criterion, False)
+
+
+def dqfd_nstep_td_error_with_rescale(
+    data: namedtuple,
+    gamma: float,
+    lambda_n_step_td: float,
+    lambda_supervised_loss: float,
+    lambda_one_step_td: float,
+    margin_function: float,
+    nstep: int = 1,
+    cum_reward: bool = False,
+    value_gamma: Optional[torch.Tensor] = None,
+    criterion: torch.nn.modules = nn.MSELoss(reduction='none'),
+    trans_fn: Callable = value_transform,
+    inv_trans_fn: Callable = value_inv_transform,
+) -> torch.Tensor:
+    """
+    DQfD loss with value rescaling h / h^-1 on both targets, drop-in for ding/rl_utils/td.py:986-1090.  Note the
+    parameter order, kept from the reference: ``lambda_one_step_td`` comes before ``margin_function`` here, after it in
+    ``dqfd_nstep_td_error``.  With the default transforms everything runs in one kernel.
+    """
+    return _dqfd(data, gamma, lambda_n_step_td, lambda_supervised_loss, lambda_one_step_td, margin_function, nstep,
+                 cum_reward, value_gamma, criterion, True, trans_fn, inv_trans_fn)
+
+
+def dqfd_nstep_td_error_sequence(
+        data: namedtuple,
+        gamma: float,
+        lambda_n_step_td: float,
+        lambda_supervised_loss: float,
+        margin_function: float,
+        lambda_one_step_td: float = 1.,
+        nstep: int = 1,
+        value_gamma: Optional[torch.Tensor] = None,
+        rescale: bool = False,
+        priority_mix: float = 0.9,
+        criterion: torch.nn.modules = nn.MSELoss(reduction='none'),
+):
+    """
+    R2D3's per-time-step loop over the DQfD loss in ONE launch.  Not a reference function: it is what
+    ``R2D3Policy._forward_learn`` computes around the operator (ding/policy/r2d3.py:322-388)::
+
+        for t in range(T):
+            l, e, s = dqfd_nstep_td_error[_with_rescale](dqfd_nstep_td_data(q[t], ..., is_expert[t]), gamma, ...,
+                                                         nstep, False, value_gamma=value_gamma[t])
+            loss.append(l); td_error.append(e); stats.append(s)
+        loss = sum(loss) / (len(loss) + 1e-8)          # and each of the three statistics alike
+        priority = mix * max_t(td_error) + (1 - mix) * sum_t(td_error) / (len(td_error) + 1e-8)   # no abs
+
+    The parameters are named as in ``dqfd_nstep_td_error``.  R2D3 passes the same positional list to both reference
+    functions (r2d3.py:340-370), and ``dqfd_nstep_td_error_with_rescale`` takes ``lambda_one_step_td`` before
+    ``margin_function``: with ``value_rescale`` on, R2D3's margin lands in ``lambda_one_step_td`` and its one-step weight
+    in ``margin_function``.  This function does not swap anything; to reproduce R2D3 with rescale, pass
+    ``margin_function=policy.lambda_one_step_td, lambda_one_step_td=policy.margin_function``.
+
+    Shapes: q, next_n_q, new_n_q_one_step (T, B, N); action, next_n_action, next_n_action_one_step, done, done_one_step,
+    is_expert (T, B); weight (T, B) or None; reward (T, nstep, B) (the policy's permuted layout, r2d3.py:316); value_gamma
+    (T, B) or None.  Returns ``(loss, priority (B,), td_error (T, B), (loss_n, loss_1, loss_sl))``: everything but the
+    priority carries gradient to ``q``.
+    """
+    q, next_n_q, action, next_n_action, reward, done, done_one_step, weight, next_q1, next_action1, is_expert = data
+    if q.dim() != 3 or action.dim() != 2 or reward.dim() != 3:
+        raise ValueError("dqfd_nstep_td_error_sequence: expected q (T, B, N), action (T, B), reward (T, nstep, B); got %s "
+                         "/ %s / %s" % (tuple(q.shape), tuple(action.shape), tuple(reward.shape)))
+    T, B, N = q.shape
+    assert reward.shape[1] == nstep  # td.py:257 for every step
+    gamma = _dqfd_gamma(gamma, False)
+    code = _criterion_code(criterion)
+    if code is None:
+        raise NotImplementedError("dqfd_nstep_td_error_sequence: criterion must be MSELoss / L1Loss / SmoothL1Loss / "
+                                  "HuberLoss with reduction='none'")
+    if tuple(reward.shape) != (T, nstep, B):
+        raise ValueError("dqfd_nstep_td_error_sequence: reward %s does not match T=%d, nstep=%d, B=%d" %
+                         (tuple(reward.shape), T, nstep, B))
+    host_out = not q.is_cuda
+    dev = ops.compute_device(q, next_n_q, next_q1)
+    S = T * B
+    if weight is not None and weight.numel() != S:
+        weight = weight.expand(T, B)
+    qd, nq, nq1, act, nact, nact1, r, d, d1, w, ie = _dqfd_operands(
+        dqfd_nstep_td_data(q, next_n_q, action, next_n_action, reward, done, done_one_step, weight, next_q1, next_action1,
+                           is_expert), S, dev, (T, B))
+    vg, vg_stride = _value_gamma_arg(value_gamma, S, dev)
+    loss, per, s_n, s_1, s_je, _, _, prio = ops.DQfDTDFunction.apply(
+        qd, nq, nq1, act, nact, nact1, r, d, d1, w, vg, vg_stride, ie, S, N, int(nstep), gamma, 0, 1 if rescale else 0,
+        1e-2, code[0], code[1], float(lambda_n_step_td), float(lambda_one_step_td), float(lambda_supervised_loss),
+        float(margin_function), T, float(priority_mix), False, True
+    )
+    per = per.reshape(T, B)
+    if host_out:
+        loss, prio, per, s_n, s_1, s_je = loss.cpu(), prio.cpu(), per.cpu(), s_n.cpu(), s_1.cpu(), s_je.cpu()
+    return loss, prio, per, (s_n, s_1, s_je)
 
 
 def _as_columns(v, next_v, reward, done, weight, value_gamma=None, nstep=None):

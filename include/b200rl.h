@@ -152,6 +152,39 @@ B200RL_API int b200rl_qntd_bwd(const float* dcrit_saved, const float* weight, co
                     const float* g_td, long long S, long long G, long long N, int group_mean, long long seq_len,
                     int skip_if_unit, float* grad_q, void* stream);
 
+/* ---- dqfd_nstep_td_error / dqfd_nstep_td_error_with_rescale: ding/rl_utils/td.py:870-983, :986-1090, and R2D3's per-step
+ *      loop over them (ding/policy/r2d3.py:322-388) as ONE call.
+ * q, next_n_q, new_n_q_one_step: (S, N); action, next_n_action, next_n_action_one_step: (S) int64; reward: (nstep, S), or
+ * (S) when cum_reward; done, done_one_step, is_expert: (S) floats; weight nullable (S); value_gamma as for b200rl_qntd_fwd
+ * (n-step target only: the 1-step target uses gamma and reward[0], td.py:953-964; with cum_reward reward[0] is sample 0's
+ * reward for every sample, as the reference's broadcast gives it).  rescale, rescale_eps, criterion and criterion_param as
+ * for b200rl_qntd_fwd; criterion = -1 computes no TD terms (callers with their own criterion apply it to the targets).
+ * Per sample: td_n / td_1 = criterion(q_sa, target), JE = is_expert * (max_j(q_j + margin*[j != a]) - q_sa) with the
+ * gradient of the max at the first maximal j (td.py:969-972).  Outputs: loss = sum(w*(ln*td_n + l1*td_1 + ls*JE)) / div,
+ * td_error_per_sample = ln*|td_n| + l1*|td_1| + ls*|JE|, loss_statistics[3] = (sum td_n, sum td_1, sum JE) / div, where
+ * div = S, or with seq_len = T > 0 (S = T*B samples in time-major order, reward (T, nstep, B)) div = B*(T + 1e-8)
+ * (r2d3.py:379-383); priority_out (B) nullable, sequence form only: priority_mix * max_t e + (1 - priority_mix) * sum_t e
+ * / (T + 1e-8) on the per-sample errors e, without abs (r2d3.py:353, :386-388).  saved (S, 4) floats, 16-byte aligned: the
+ * record b200rl_dqfd_bwd needs.  target_n_out / target_1_out (S) nullable: the detached targets.  grad_q_unit (S, N)
+ * nullable: d loss / d q for a unit upstream gradient.
+ * b200rl_dqfd_bwd: grad_q for the upstream gradients of the loss, td_error_per_sample (S) and the three statistics (each a
+ * device pointer, nullable = 0).  skip_if_unit != 0: grad_q already holds grad_q_unit; the launch verifies on the device
+ * that only *g_loss == 1 arrived and returns at once, else it recomputes. */
+B200RL_API int b200rl_dqfd_fwd(const float* q, const float* next_n_q, const float* new_n_q_one_step, const long long* action,
+                    const long long* next_n_action, const long long* next_n_action_one_step, const float* reward,
+                    const float* done, const float* done_one_step, const float* weight, const float* value_gamma,
+                    long long value_gamma_stride, const float* is_expert, long long S, long long N, int nstep,
+                    double gamma, int cum_reward, int rescale, double rescale_eps, int criterion, double criterion_param,
+                    double lambda_n_step_td, double lambda_one_step_td, double lambda_supervised_loss, double margin,
+                    long long seq_len, double priority_mix, float* loss, float* td_error_per_sample,
+                    float* loss_statistics, float* saved, float* target_n_out, float* target_1_out, float* grad_q_unit,
+                    float* priority_out, float* workspace, size_t workspace_bytes, void* stream);
+B200RL_API int b200rl_dqfd_bwd(const float* saved, const float* weight, const long long* action, const float* g_loss,
+                    const float* g_td, const float* g_loss_statistics_n, const float* g_loss_statistics_1,
+                    const float* g_loss_statistics_je, long long S, long long N, double lambda_n_step_td,
+                    double lambda_one_step_td, double lambda_supervised_loss, long long seq_len, int skip_if_unit,
+                    float* grad_q, void* stream);
+
 /* ---- dist_nstep_td_error (C51): ding/rl_utils/td.py:413-523; dist_1step_td_error (:294-383) is its nstep = 1 case ---
  * dist, next_n_dist: (B*A, N, n_atom); act, next_n_act: (B*A) int64; reward: (nstep, B); done: (B);
  * weight nullable with stride 0 / 1 over the B*A rows; value_gamma nullable with stride 0 / 1 over B;
