@@ -6,24 +6,42 @@
 // the TMA unit's issue cost is per operation, and a column tile of the (T, B) tensors gives 64-byte box rows, 2 KB per
 // operation (57 operations per tile), so the copies wait on the TMA unit instead.
 //
-// A CTA owns TC = 16 batch columns for ALL T (the recurrence of gae.py:65-69 runs along T only, ppo.py:77-140 is pointwise).
-// Time is walked newest-first in chunks of R = 16 steps (256 transitions).  Warp roles (10 warps, two CTAs per SM):
+// A CTA owns TC batch columns for ALL T (the recurrence of gae.py:65-69 runs along T only, ppo.py:77-140 is pointwise).
+// Time is walked newest-first in chunks of R = 256 / TC steps (256 transitions).  Two geometries, chosen on the host from
+// the SM count and B (cw_pick_tc):
+//   TC = 32, R = 8    one CTA per SM, a ring of up to 8 stages; where 32-column tiles still give nearly every SM a tile
+//                     (config D: B = 4096 -> 128 CTAs on an H100's 132 SMs, 16 chunks each).  Every (T, B) row segment is
+//                     a full 128-byte line.
+//   TC = 16, R = 16   two CTAs per SM, up to 4 stages each; every other shape (at config D: 256 CTAs, 8 chunks each).
+// Warp roles (10 warps):
 //   warp 8     loader: cp.async of the chunk's PPO inputs (logit_new | logit_old | action | value_new | value_old |
-//              return_ [| weight | logit_pre]) into an S-stage ring (S = 4 at N = 6); completion arrives on the stage's
+//              return_ [| weight | logit_pre]) into an S-stage ring (S = 8 / 4 at N = 6); completion arrives on the stage's
 //              mbarrier (cp.async.mbarrier.arrive.noinc); a stage is refilled as soon as the consumers release it.
-//   warp 9     scanner: own two-deep cp.async ring of the five GAE inputs; per chunk delta / f in the reference's operation
-//              order, the in-place next_value mask (gae.py:61), the sequential scan A = delta + f*A (lane = column, separate
-//              round-to-nearest mul and add: bit-identical to the torch loop); publishes the chunk's advantages in an
-//              S-slot shared-memory ring (mbarrier) and writes them to HBM (16-byte coalesced).
+//   warp 9     scanner: own cp.async ring of the five GAE inputs (2 chunks deep; 4 with 32-column tiles, whose chunks
+//              come twice as often); per chunk delta / f in the reference's operation order, the in-place next_value
+//              mask (gae.py:61), the sequential scan A = delta + f*A (lane = column, separate round-to-nearest mul and
+//              add: bit-identical to the torch loop); publishes the chunk's advantages in an S-slot shared-memory ring
+//              (mbarrier) and writes them to HBM (16-byte coalesced).
 //   warps 0-7  consumers: thread = transition; wait for "chunk landed" and "advantages ready", run ppo_row_compute_to (the
-//              row code of ppo.cu) and store the gradient row and the value gradient straight to HBM; arrive on "done".
+//              row code of ppo.cu) and store the gradient row (32-column tiles: through the row's logit_new slot, then
+//              16-byte coalesced per warp) and the value gradient to HBM; arrive on "done".
 // Rings run across tile boundaries (static tile -> CTA assignment: deterministic loss partial sums).
 //
-// Once the ring is primed the chunks stream at the rate HBM delivers them; what separates the kernel from the roofline is
-// the time until the first chunk has landed and the tail (last chunk's math, store drain, partial sums, finalize_sums
-// launch).  Loader variants that were slower: loop-invariant piece offsets in registers with one or two loader warps (the
-// faster refill issues the ring of every CTA in one burst, which delays chunk 0 and costs DRAM efficiency), the same with a
-// throttled prologue, no unrolling of the copy loop, 2 or 3 ring stages.
+// Once the ring is primed the chunks stream at the rate HBM delivers them; what separates the kernel from the roofline
+// is the time until the first chunk has landed and the tail (last chunk's math, store drain, partial sums,
+// finalize_sums launch).  Measured with the stamps of tools/trace_col.py at config D on an H100 SXM (700 W, SM clock
+// 1980 MHz): with 16 x 16 tiles the first chunk of a CTA landed 4.4 us (median) after griddepcontrol.wait -- the
+// prologue requests four stages of all 256 CTAs, about 20 MB, before any has landed -- and the last CTA ended 24.1 us
+// after it; with 32 x 8 tiles the first chunk lands after 2.6 us, a CTA then takes 1.2 - 1.3 us per chunk (3.9 MB over
+// the grid) and 1.0 us from its last chunk landed to its end. That pace was the loader's while it copied with the flat
+// loop (one loader warp per SM): on a 400 W card, whose SM clock drops under this load, the step stayed at 29.0 - 29.2
+// us like the 16 x 16 tiles'; with warp copies and at most two stages in flight it is 27.1 - 27.2 us there.  Slower at
+// config D on the H100: 6 stages instead of 8 (+0.4 us per step), requesting the first 2 or 4 chunks into L2
+// (cp.async.bulk.prefetch) before griddepcontrol.wait (26.1 - 26.8 us and 27.9 us against 26.2; one chunk: no change).
+// Storing the gradient rows straight from registers instead of through the stage: 26.2 - 26.7 us at config D, and 79 us
+// against 52 at N = 18. Loader variants that were slower on B200: loop-invariant piece offsets in registers with one or
+// two loader warps (the faster refill issues the ring of every CTA in one burst, which delays chunk 0 and costs DRAM
+// efficiency), the same with a throttled prologue, no unrolling of the copy loop, 2 or 3 ring stages.
 //
 // Algorithmic traffic: 24 B (GAE) + 104 B (ppo_error forward + gradients, N = 6) = 128 B per transition, each byte once.
 #include "../../include/b200rl.h"
@@ -34,15 +52,28 @@ namespace b200rl {
 constexpr int CW_CW = 8;                  // consumer warps
 constexpr int CW_CT = CW_CW * 32;         // consumer threads = transitions per chunk
 constexpr int CW_THREADS = CW_CT + 64;    // + loader warp + scanner warp
-constexpr int CW_TC = 16;                 // columns per tile
-constexpr int CW_R = CW_CT / CW_TC;       // time steps per chunk (16)
-constexpr int CW_MAX_STAGES = 4;
-constexpr int CW_RAW_ARR = CW_R * CW_TC * 4;  // bytes of one raw GAE array chunk
+// Tile geometry (cw_pick_tc): TC = 16 columns x R = 16 steps per chunk, two CTAs per SM with up to 4 stages each, or
+// TC = 32 columns x R = 8 steps, one CTA per SM with up to 8 stages.  A chunk is 256 transitions either way.
+template <int TC> struct CwGeo {
+    static constexpr int R = CW_CT / TC;                // time steps per chunk
+    static constexpr int MAX_STAGES = TC == 32 ? 8 : 4;  // PPO ring stages
+    static constexpr int CTAS_PER_SM = TC == 32 ? 1 : 2;
+    static constexpr int PR = TC / 4;                   // 16-byte pieces per float row segment
+    static constexpr int RAW_SLOTS = TC == 32 ? 4 : 2;  // scanner's ring of raw GAE chunks
+};
+// 32-column tiles: the loader copies every full stage with warp_copy_rows and keeps at most CW_AHEAD stages in flight
+constexpr int CW_AHEAD = 2;  // 3, 4, 6: slower at config D on the H100 (tools/trace_col.py, bench.py)
+constexpr int CW_RAW_ARR = CW_CT * 4;         // bytes of one raw GAE array chunk
 constexpr int CW_RAW_BYTES = 5 * CW_RAW_ARR;  // value | next_value | reward | done | traj_flag
 
+// B200RL_FUSED_TRACE=1: %globaltimer stamps, 64 per CTA (tools/trace_col.py).  Slots 0-7 frame the CTA: 0 start, 1 the
+// previous launches' results visible (after griddepcontrol.wait), 2 first chunk's advantages published, 3 / 4 / 5 the
+// last chunk landed / advantages ready / computed, 6 end (partial sums stored), 7 the number of chunks (a count).  Chunk
+// j < CW_TRACE_CHUNKS: 8 + 4j landed, 9 + 4j advantages ready, 10 + 4j computed, 11 + 4j its stage issued by the loader.
+constexpr int CW_TRACE_CHUNKS = 14;
 #define CW_TRACE(slot)                                                                                   \
     do {                                                                                                 \
-        if (f.trace) reinterpret_cast<unsigned long long*>(ws + 65536)[blockIdx.x * 32 + (slot)] = gtimer(); \
+        if (f.trace) reinterpret_cast<unsigned long long*>(ws + 65536)[blockIdx.x * 64 + (slot)] = gtimer(); \
     } while (0)
 
 struct CwItem {
@@ -54,8 +85,10 @@ __host__ __device__ inline int cw_stage_bytes(int N, bool has_pre, bool has_w) {
     return (CW_CT * ((has_pre ? 3 : 2) * N * 4 + 8 + 12 + (has_w ? 4 : 0)) + 127) & ~127;
 }
 
-template <int NC, bool GRADS>
-__global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, float* ws, int n_stages) {
+template <int NC, bool GRADS, int TC>
+__global__ void __launch_bounds__(CW_THREADS, CwGeo<TC>::CTAS_PER_SM) gae_ppo_ws_kernel(FusedArgs f, float* ws, int n_stages) {
+    constexpr int CW_R = CwGeo<TC>::R, CW_MAX_STAGES = CwGeo<TC>::MAX_STAGES, PR = CwGeo<TC>::PR;
+    constexpr int RAWS = CwGeo<TC>::RAW_SLOTS;
     // PDL: the next kernel may start launching right away; the wait for the previous kernels' results comes after the
     // barrier set-up below (nothing before it touches global memory except the optional trace stamp)
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -80,16 +113,16 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
         L.tx_bytes = o;
     }
     const int S = n_stages;
-    unsigned char* raw = smem + S * L.stage_bytes;                                            // [2][5][R][TC]
-    auto advr = reinterpret_cast<float (*)[CW_R][CW_TC]>(raw + 2 * CW_RAW_BYTES);            // [S][R][TC]
-    auto fbuf = reinterpret_cast<float (*)[CW_TC]>(reinterpret_cast<unsigned char*>(advr) + CW_MAX_STAGES * CW_RAW_ARR);
+    unsigned char* raw = smem + S * L.stage_bytes;                                            // [RAWS][5][R][TC]
+    auto advr = reinterpret_cast<float (*)[CW_R][TC]>(raw + RAWS * CW_RAW_BYTES);            // [S][R][TC]
+    auto fbuf = reinterpret_cast<float (*)[TC]>(reinterpret_cast<unsigned char*>(advr) + CW_MAX_STAGES * CW_RAW_ARR);
     uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<unsigned char*>(fbuf) + CW_RAW_ARR);
     uint64_t* full = bars;                           // [S] PPO chunk landed (32 loader-lane arrivals)
     uint64_t* done = bars + CW_MAX_STAGES;           // [S] consumers finished the chunk (CW_CW arrivals)
     uint64_t* adv_ready = bars + 2 * CW_MAX_STAGES;  // [S] advantages of the chunk are in advr[s]
 
     const long long T = f.T, B = f.B;
-    const long long n_tiles = (B + CW_TC - 1) / CW_TC;
+    const long long n_tiles = (B + TC - 1) / TC;
     const long long n_chunks = (T + CW_R - 1) / CW_R;
     const bool has_done = f.done != nullptr, has_traj = f.traj != nullptr;
 
@@ -104,6 +137,7 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
     }
     asm volatile("griddepcontrol.wait;" ::: "memory");
     __syncthreads();
+    if (tid == 0) CW_TRACE(1);
     // data-parallel training: consumer warp k of the first CTA consumes the loss scalar k of two steps ago from its mailbox and
     // publishes the previous step's (staged by its finalize launch) to the peers -- while it would otherwise just wait for its
     // first chunk; the NVLink acknowledgements return while this kernel streams (common.cuh)
@@ -126,7 +160,7 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
         // =============================================== loader ===========================================================
         // R segments (one per time step) of `esz` bytes per column: P = TC*esz/16 pieces per segment in shared memory
         auto rows_of = [&](unsigned char* dst, const void* src, long long t0, long long c0, int esz, int jmin, int W) {
-            const int P = CW_TC * esz / 16, Pv = W * esz / 16;
+            const int P = TC * esz / 16, Pv = W * esz / 16;
             const unsigned char* g = reinterpret_cast<const unsigned char*>(src) + (t0 * B + c0) * esz;
             const long long rstride = B * esz;
             const int n = CW_R * P;
@@ -136,29 +170,43 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
                 if (row >= jmin && o < Pv) cpa16(dst + p * 16, g + row * rstride + o * 16);
             }
         };
-        // The FIRST stage of a CTA uses lane-owns-a-piece-column copies (common.cuh warp_copy_rows, ~3 instructions per copy),
-        // every later one the flat loop (~35 instructions per copy).  The kernel streams at the HBM rate in steady state, so a
-        // faster loader buys nothing there -- issued in bursts the copies only deepen the queues in front of everybody's next
-        // chunk -- but the first stage is pure latency: the flat loop's address arithmetic runs before the first byte is
-        // requested.
+        // 16-column tiles: the FIRST stage of a CTA uses lane-owns-a-piece-column copies (common.cuh warp_copy_rows, ~3
+        // instructions per copy), every later one the flat loop (~35 instructions per copy).  Two CTAs per SM stream at the
+        // HBM rate in steady state, so a faster loader buys nothing there -- issued in bursts the copies only deepen the
+        // queues in front of everybody's next chunk -- but the first stage is pure latency: the flat loop's address
+        // arithmetic runs before the first byte is requested.
+        // 32-column tiles (one CTA, so one loader warp per SM): the flat loop takes ~1.3 us to issue a stage at 1980 MHz,
+        // as long as HBM takes to deliver one, and longer at the lower clock of a power-capped card -- the loader, not HBM,
+        // set the pace.  So every full stage uses warp_copy_rows, and the loader keeps at most CW_AHEAD stages in flight:
+        // copying the whole 8-stage ring in one burst made the step 30.1 us against 26.2 (chunk 0 waits behind it).
         CwItem it = first;
         int s = 0, ph = 0;
         for (int j = 0; item_valid(it); ++j) {
             if (j >= S) mbar_wait(&done[s], (uint32_t)(ph ^ 1));
-            if (lane == 0 && j < 6) CW_TRACE(20 + 2 * j);
-            const long long c0 = it.tile * CW_TC;
+            if (TC == 32 && j >= CW_AHEAD) {  // chunk j - CW_AHEAD has landed
+                const int jb = j - CW_AHEAD;
+                mbar_wait(&full[jb % S], (uint32_t)((jb / S) & 1));
+            }
+            const long long c0 = it.tile * TC;
             const long long t0 = T - (it.q + 1) * CW_R;
             const int jmin = t0 < 0 ? (int)-t0 : 0;
-            const int W = (int)((B - c0) < CW_TC ? (B - c0) : CW_TC);
+            const int W = (int)((B - c0) < TC ? (B - c0) : TC);
             unsigned char* st = smem + s * L.stage_bytes;
-            if (jmin == 0 && W == CW_TC && j == 0) {
-                // full chunk of a full tile: a row segment is TC * esz / 16 = esz pieces (4 N | 8 | 4).  Logits and actions
-                // go in 8-piece groups (a lane group covers one full 128-byte line per row: the 4-piece grouping doubles the
-                // number of L2 requests, which makes it slower than the flat loop); the float tensors have 64-byte rows.
+            if (jmin == 0 && W == TC && (TC == 32 || j == 0)) {
+                // full chunk of a full tile, 16 columns: a row segment is TC * esz / 16 = esz pieces (4 N | 8 | 4).  Logits
+                // and actions go in 8-piece groups (a lane group covers one full 128-byte line per row: the 4-piece grouping
+                // doubles the number of L2 requests, which makes it slower than the flat loop); the float tensors have
+                // 64-byte rows.
                 const uint32_t sb = smem_u32(st);
                 const long long e0 = t0 * B + c0;
                 const long long ls = B * N * 4;
-                if (N & 1) {
+                if constexpr (TC == 32) {
+                    // 32-column rows: 8 lanes cover one 128-byte line of every tensor, N lines per logit row segment
+                    warp_copy_rows<8, CW_R, NC>(sb, a.logit_new + e0 * N, ls, N, lane);
+                    warp_copy_rows<8, CW_R, NC>(sb + L.off_old, a.logit_old + e0 * N, ls, N, lane);
+                    if (has_pre) warp_copy_rows<8, CW_R, NC>(sb + L.off_pre, a.logit_pre + e0 * N, ls, N, lane);
+                    warp_copy_rows<8, CW_R, 2>(sb + L.off_act, a.action + e0, B * 8, 2, lane);
+                } else if (N & 1) {
                     warp_copy_rows<4, CW_R, NC>(sb, a.logit_new + e0 * N, ls, N, lane);
                     warp_copy_rows<4, CW_R, NC>(sb + L.off_old, a.logit_old + e0 * N, ls, N, lane);
                     if (has_pre) warp_copy_rows<4, CW_R, NC>(sb + L.off_pre, a.logit_pre + e0 * N, ls, N, lane);
@@ -169,10 +217,10 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
                     if (has_pre) warp_copy_rows<8, CW_R, NC / 2>(sb + L.off_pre, a.logit_pre + e0 * N, ls, N / 2, lane);
                     warp_copy_rows<8, CW_R, 1>(sb + L.off_act, a.action + e0, B * 8, 1, lane);
                 }
-                warp_copy_rows<4, CW_R, 1>(sb + L.off_vn, a.value_new + e0, B * 4, 1, lane);
-                warp_copy_rows<4, CW_R, 1>(sb + L.off_vo, a.value_old + e0, B * 4, 1, lane);
-                warp_copy_rows<4, CW_R, 1>(sb + L.off_ret, a.ret + e0, B * 4, 1, lane);
-                if (has_w) warp_copy_rows<4, CW_R, 1>(sb + L.off_w, a.weight + e0, B * 4, 1, lane);
+                warp_copy_rows<PR, CW_R, 1>(sb + L.off_vn, a.value_new + e0, B * 4, 1, lane);
+                warp_copy_rows<PR, CW_R, 1>(sb + L.off_vo, a.value_old + e0, B * 4, 1, lane);
+                warp_copy_rows<PR, CW_R, 1>(sb + L.off_ret, a.ret + e0, B * 4, 1, lane);
+                if (has_w) warp_copy_rows<PR, CW_R, 1>(sb + L.off_w, a.weight + e0, B * 4, 1, lane);
             } else {
                 rows_of(st, a.logit_new, t0, c0, N * 4, jmin, W);
                 rows_of(st + L.off_old, a.logit_old, t0, c0, N * 4, jmin, W);
@@ -184,21 +232,21 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
                 if (has_w) rows_of(st + L.off_w, a.weight, t0, c0, 4, jmin, W);
             }
             cpa_mbar_arrive(&full[s]);
-            if (lane == 0 && j < 6) CW_TRACE(21 + 2 * j);
+            if (f.trace && lane == 0 && j < CW_TRACE_CHUNKS) CW_TRACE(11 + 4 * j);
             if (++s == S) { s = 0; ph ^= 1; }
             item_next(it);
         }
     } else if (wid == CW_CW + 1) {
         // =============================================== scanner ==========================================================
         auto issue_raw = [&](const CwItem& it, int slot) {
-            const long long c0 = it.tile * CW_TC;
+            const long long c0 = it.tile * TC;
             const long long t0 = T - (it.q + 1) * CW_R;
-            const int W = (int)((B - c0) < CW_TC ? (B - c0) : CW_TC);
+            const int W = (int)((B - c0) < TC ? (B - c0) : TC);
             unsigned char* dst = raw + slot * CW_RAW_BYTES;
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
-                const int p = lane + 32 * k;  // R*4 = 64 pieces per array
-                const int row = p >> 2, o = p & 3;
+                const int p = lane + 32 * k;  // R * TC / 4 = 64 pieces per array
+                const int row = p / PR, o = p % PR;
                 if (t0 + row >= 0 && o * 4 < W) {
                     const long long off = (t0 + row) * B + c0 + o * 4;
                     cpa16(dst + p * 16, f.value + off);
@@ -210,7 +258,7 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
             }
         };
         CwItem it = first, pf = first;
-        for (int k = 0; k < 2; ++k) {
+        for (int k = 0; k < RAWS; ++k) {
             if (item_valid(pf)) {
                 issue_raw(pf, k);
                 item_next(pf);
@@ -220,26 +268,26 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
         float carry = 0.f;
         int s = 0, ph = 0;
         for (int j = 0; item_valid(it); ++j) {
-            const long long c0 = it.tile * CW_TC;
+            const long long c0 = it.tile * TC;
             const long long t0 = T - (it.q + 1) * CW_R;
-            const int slot = j & 1;
+            const int slot = j % RAWS;
             if (it.q == 0) carry = 0.f;
-            cpa_wait<1>();
+            cpa_wait<RAWS - 1>();
             __syncwarp();
             if (j >= S) mbar_wait(&done[s], (uint32_t)(ph ^ 1));  // the consumers are through the chunk that used advr[s]
-            float (*ab)[CW_TC] = advr[s];
+            float (*ab)[TC] = advr[s];
             const float* rv = reinterpret_cast<const float*>(raw + slot * CW_RAW_BYTES);
-            const float* rn = rv + CW_R * CW_TC;
-            const float* rr = rn + CW_R * CW_TC;
-            const float* rd = rr + CW_R * CW_TC;
-            const float* rt = rd + CW_R * CW_TC;
-            const int cq = (lane & 3) * 4;
+            const float* rn = rv + CW_R * TC;
+            const float* rr = rn + CW_R * TC;
+            const float* rd = rr + CW_R * TC;
+            const float* rt = rd + CW_R * TC;
+            const int cq = (lane % PR) * 4;
 #pragma unroll
-            for (int p = 0; p < CW_R / 8; ++p) {
-                const int jj = p * 8 + (lane >> 2);
+            for (int p = 0; p < CW_R * PR / 32; ++p) {
+                const int jj = p * (32 / PR) + lane / PR;
                 const long long t = t0 + jj;
                 if (t >= 0 && c0 + cq < B) {
-                    const int o = jj * CW_TC + cq;
+                    const int o = jj * TC + cq;
                     const float4 v4 = *reinterpret_cast<const float4*>(rv + o);
                     const float4 n4 = *reinterpret_cast<const float4*>(rn + o);
                     const float4 r4 = *reinterpret_cast<const float4*>(rr + o);
@@ -267,14 +315,14 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
                 }
             }
             __syncwarp();
-            // the raw slot has been read by every lane: refill it with the chunk two ahead
+            // the raw slot has been read by every lane: refill it with the chunk RAWS ahead
             if (item_valid(pf)) {
                 issue_raw(pf, slot);
                 item_next(pf);
             }
             cpa_commit();
             // ---- sequential scan, lane = column, newest time step first ---------------------------------------------------
-            if (lane < CW_TC && c0 + lane < B) {
+            if (lane < TC && c0 + lane < B) {
                 if (t0 >= 0) {
                     float d[CW_R], g[CW_R];
 #pragma unroll
@@ -297,13 +345,13 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
             __syncwarp();
             if (lane == 0) {
                 mbar_arrive(&adv_ready[s]);
-                if (j == 0) CW_TRACE(19);
+                if (j == 0) CW_TRACE(2);
             }
-            // advantages -> HBM: R*4 = 64 float4, two per lane
+            // advantages -> HBM: R * TC / 4 = 64 float4, two per lane
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
                 const int p = lane + 32 * k;
-                const int row = p >> 2, o = (p & 3) * 4;
+                const int row = p / PR, o = (p % PR) * 4;
                 if (t0 + row >= 0 && c0 + o < B)
                     stg_stream4(reinterpret_cast<float4*>(a.adv_out + (t0 + row) * B + c0 + o),
                                 *reinterpret_cast<const float4*>(&ab[row][o]));
@@ -324,43 +372,85 @@ __global__ void __launch_bounds__(CW_THREADS, 2) gae_ppo_ws_kernel(FusedArgs f, 
                 a.g_used[0] = up.g_pol; a.g_used[1] = up.g_val; a.g_used[2] = up.g_ent; a.g_used[3] = up.g_kl;
             }
         }
-        const int jj = tid / CW_TC, c = tid % CW_TC;
+        // trace: chunk j's stamp k (0 landed, 1 advantages ready, 2 computed); slots 3-5 are overwritten by every chunk, so
+        // the last chunk's remain
+        auto stamp_chunk = [&](int j, int k) {
+            if (f.trace && tid == 0) {
+                unsigned long long* tr = reinterpret_cast<unsigned long long*>(ws + 65536) + blockIdx.x * 64;
+                const unsigned long long now = gtimer();
+                tr[3 + k] = now;
+                if (j < CW_TRACE_CHUNKS) tr[8 + 4 * j + k] = now;
+                if (k == 2) tr[7] = (unsigned long long)(j + 1);
+            }
+        };
+        const int jj = tid / TC, c = tid % TC;
         CwItem it = first;
         int s = 0, ph = 0;
         for (int j = 0; item_valid(it); ++j) {
-            const long long c0 = it.tile * CW_TC;
+            const long long c0 = it.tile * TC;
             const long long t = T - (it.q + 1) * CW_R + jj;
             unsigned char* st = smem + s * L.stage_bytes;
             mbar_wait(&full[s], (uint32_t)ph);
-            if (tid == 0 && j < 6) CW_TRACE(1 + 3 * j);
+            stamp_chunk(j, 0);
             mbar_wait(&adv_ready[s], (uint32_t)ph);
-            if (tid == 0 && j < 6) CW_TRACE(2 + 3 * j);
+            stamp_chunk(j, 1);
+            // 32-column tiles: a warp is one time step of 32 consecutive transitions, so its gradient rows are one contiguous
+            // 128*N-byte span in HBM.  They go to the rows' own logit_new slots in the stage first and leave as 16-byte
+            // coalesced stores (full lines instead of 8 bytes into each of 24 sectors per store instruction at N = 6).
+            const bool stage_grads = GRADS && TC == 32 && t >= 0 && c0 + TC <= B;  // warp-uniform
             if (t >= 0 && c0 + c < B) {
                 const long long g = t * B + c0 + c;  // global transition index
-                float* grow = GRADS ? a.grad_logit + g * N : nullptr;
+                float* grow = GRADS ? (stage_grads ? reinterpret_cast<float*>(st) + tid * N : a.grad_logit + g * N)
+                                    : nullptr;
                 float* gval = GRADS ? a.grad_value + g : nullptr;
                 ppo_row_compute_to<NC, true, GRADS>(a, L, st, tid, N, advr[s][jj][c], grow, gval, up, acc);
             }
-            __syncwarp();
+            if (stage_grads) {
+                __syncwarp();
+                const float4* src = reinterpret_cast<const float4*>(st) + wid * 8 * N;  // 32 rows of N floats
+                float4* dst = reinterpret_cast<float4*>(a.grad_logit + (t * B + c0) * N);
+                for (int k = lane; k < 8 * N; k += 32) stg_stream4(dst + k, src[k]);
+            }
+            __syncwarp();  // every lane's reads of the stage precede the release
             if (lane == 0) mbar_arrive(&done[s]);
-            if (tid == 0 && j < 6) CW_TRACE(3 + 3 * j);
+            stamp_chunk(j, 2);
             if (++s == S) { s = 0; ph ^= 1; }
             item_next(it);
         }
     }
     grid_store_partials<6, CW_THREADS>(acc, ws);  // summed by finalize_sums_kernel
+    if (tid == 0) CW_TRACE(6);
 }
 
+template <int TC>
 static size_t cw_smem(int N, bool has_pre, bool has_w, int stages) {
-    return (size_t)stages * cw_stage_bytes(N, has_pre, has_w) + 2 * CW_RAW_BYTES + CW_MAX_STAGES * CW_RAW_ARR + CW_RAW_ARR +
-           3 * CW_MAX_STAGES * sizeof(uint64_t) + 32;
+    constexpr int MS = CwGeo<TC>::MAX_STAGES;
+    return (size_t)stages * cw_stage_bytes(N, has_pre, has_w) + CwGeo<TC>::RAW_SLOTS * CW_RAW_BYTES + MS * CW_RAW_ARR +
+           CW_RAW_ARR + 3 * MS * sizeof(uint64_t) + 32;
 }
 
-static int cw_pick_stages(const FusedArgs& f) {
+// deepest PPO ring that keeps CwGeo<TC>::CTAS_PER_SM CTAs resident per SM (0: not even two stages)
+template <int TC>
+static int cw_stages(const FusedArgs& f) {
     const PpoArgs& a = f.p;
-    for (int s = CW_MAX_STAGES; s >= 2; --s)
-        if (cw_smem(a.N, a.logit_pre != nullptr, a.weight != nullptr, s) <= 112 * 1024) return s;  // two CTAs per SM
+    const size_t limit = CwGeo<TC>::CTAS_PER_SM == 2 ? 112 * 1024 : 227 * 1024;
+    for (int s = CwGeo<TC>::MAX_STAGES; s >= 2; --s)
+        if (cw_smem<TC>(a.N, a.logit_pre != nullptr, a.weight != nullptr, s) <= limit) return s;
     return 0;
+}
+
+// Tile width for this shape on a device with `sm_count` SMs.  32-column tiles make every (T, B) row segment a full
+// 128-byte line and give each CTA twice as many chunks (one CTA per SM, a ring of up to 8 stages).  They are taken when
+// they keep at least as many stages in flight per SM, leave at most 1/16 of the SMs without a tile, and give the busiest
+// SM no more columns than 16-column tiles (two CTAs per SM) do: at B = 4096 on 132 SMs, 128 CTAs of 32 columns against
+// 256 CTAs of 16, 32 columns on the busiest SM either way.
+static int cw_pick_tc(const FusedArgs& f, int sm_count) {
+    const int s16 = cw_stages<16>(f), s32 = cw_stages<32>(f);
+    if (s32 < 2 * s16) return 16;
+    const long long n16 = (f.B + 15) / 16, n32 = (f.B + 31) / 32;
+    if (n32 < sm_count - sm_count / 16) return 16;
+    const long long cols16 = 16 * ((n16 + sm_count - 1) / sm_count), cols32 = 32 * ((n32 + sm_count - 1) / sm_count);
+    return cols32 <= cols16 ? 32 : 16;
 }
 
 bool colws_ok(const FusedArgs& f) {
@@ -371,19 +461,21 @@ bool colws_ok(const FusedArgs& f) {
                     (!a.grad_value || aligned16(a.grad_value)) && aligned16(f.value) && aligned16(f.next_value) &&
                     aligned16(f.reward) && aligned16(a.adv) && (!f.done || aligned16(f.done)) &&
                     (!f.traj || aligned16(f.traj));
+    // the 16-column geometry takes every shape; the 32-column one only replaces it where cw_pick_tc says so
     return al && a.N >= 1 && a.N <= 32 && f.T >= 1 && f.B >= 4 && (f.B % 4) == 0 && f.T * f.B == a.S &&
-           cw_pick_stages(f) >= 2;
+           cw_stages<16>(f) >= 2;
 }
 
-template <int NC, bool GRADS>
+template <int NC, bool GRADS, int TC>
 static int launch_ws(const FusedArgs& f, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
     const PpoArgs& a = f.p;
-    const int stages = cw_pick_stages(f);
-    const size_t smem = cw_smem(a.N, a.logit_pre != nullptr, a.weight != nullptr, stages);
-    constexpr auto kern = gae_ppo_ws_kernel<NC, GRADS>;
+    const int stages = cw_stages<TC>(f);
+    const size_t smem = cw_smem<TC>(a.N, a.logit_pre != nullptr, a.weight != nullptr, stages);
+    constexpr auto kern = gae_ppo_ws_kernel<NC, GRADS, TC>;
     int sm_count, per_sm;
     if (int rc = resident_ctas<kern>(CW_THREADS, smem, sm_count, per_sm)) return rc;
-    const long long n_tiles = (f.B + CW_TC - 1) / CW_TC;
+    if (per_sm > CwGeo<TC>::CTAS_PER_SM) per_sm = CwGeo<TC>::CTAS_PER_SM;
+    const long long n_tiles = (f.B + TC - 1) / TC;
     long long grid = (long long)sm_count * per_sm;
     if (grid > n_tiles) grid = n_tiles;
     if (ws_bytes < WS_MIN_BYTES || !ws_partials_fit((long long)(grid * 6), ws_bytes))
@@ -396,9 +488,25 @@ static int launch_ws(const FusedArgs& f, float* out, float* ws, size_t ws_bytes,
     return launch_finalize(ws, out, fa, st);
 }
 
+// SM count of the current device (cached per device)
+static int cw_sm_count(int& n) {
+    static int sms[MAX_DEVICES];
+    int dev = 0;
+    if (int rc = current_device(dev)) return rc;
+    if (sms[dev] == 0)
+        if (int rc = cuda_rc(cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev))) return rc;
+    n = sms[dev];
+    return B200RL_OK;
+}
+
 template <bool GRADS>
 static int dispatch_ws(const FusedArgs& f, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
-    return with_nc(f.p.N, [&](auto nc) { return launch_ws<nc, GRADS>(f, out, ws, ws_bytes, st); });
+    int sm_count = 0;
+    if (int rc = cw_sm_count(sm_count)) return rc;
+    const int tc = cw_pick_tc(f, sm_count);
+    return with_nc(f.p.N, [&](auto nc) {
+        return tc == 32 ? launch_ws<nc, GRADS, 32>(f, out, ws, ws_bytes, st) : launch_ws<nc, GRADS, 16>(f, out, ws, ws_bytes, st);
+    });
 }
 
 int launch_colws(const FusedArgs& f, bool grads, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {

@@ -338,7 +338,9 @@ static int gae_ppo_step(const float* value, float* next_value, const float* rewa
         f.x_mailboxes = mailbox_ptrs_dev; f.x_seq = seq_dev; f.x_out_mean = out_mean; f.x_rank = rank; f.x_world = world;
         return launch_colws(f, grads, out, workspace, workspace_bytes, st);
     }
-    // column tiles need enough columns to fill the machine (16 per CTA); tiny problems are launch-bound either way
+    // column tiles need enough columns to fill the machine (64 CTAs of 16 columns); tiny problems are launch-bound either
+    // way.  colws.cu takes 32-column tiles only where they give nearly every SM one (B >= 3940 on an H100's 132 SMs), far
+    // above this threshold, so it is derived for its 16-column geometry
     const bool want_col = g_impl == 2 || (g_impl == 0 && (B >= 16 * 64 || T * B <= 16384));
     if (col_ok && (want_col || !row_ok)) return launch_colws(f, grads, out, workspace, workspace_bytes, st);
     return grads ? dispatch_fused<true>(f, out, workspace, workspace_bytes, st)
