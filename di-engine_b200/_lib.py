@@ -37,6 +37,8 @@ PROTOTYPES = {
     "b200rl_dqfd_fwd": [P, P, P, P, P, P, P, P, P, P, P, LL, P, LL, LL, I, D, I, I, D, I, D, D, D, D, D, LL, D, P, P, P,
                         P, P, P, P, P, P, c_size_t, P],
     "b200rl_dqfd_bwd": [P, P, P, P, P, P, P, P, LL, LL, D, D, D, LL, I, P, P],
+    "b200rl_soft_td_fwd": [I, P, P, P, P, P, P, P, P, LL, LL, LL, LL, I, D, D, D, I, I, D, P, P, P, P, P, P, P, P, P,
+                           c_size_t, P],
     "b200rl_dntd_fwd":[P, P, P, P, P, P, P, LL, P, LL, P, LL, LL, LL, I, I, D, D, D, P, P, P, P, P, P, c_size_t, P],
     "b200rl_dntd_bwd": [P, P, P, P, LL, P, P, LL, LL, I, I, P, P],
     "b200rl_lambda_returns": [P, P, P, D, P, D, P, I, LL, LL, P, P],

@@ -438,6 +438,181 @@ __global__ void dqfd_bwd_kernel(const float4* __restrict__ saved, const float* _
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// The TD losses of the entropy-regularised value learners, one thread per row.  Only the target differs between modes:
+//   MODE 0 Munchausen (m_q_1step_td_error, td.py:119-158):
+//          r + alpha*clamp(log pi(a), -1, 1) + gamma * sum_j pi'_j * (q'_j - tau*log pi'_j) * (1 - d),
+//          pi = softmax(target_q / tau), pi' = softmax(next_q / tau), each with its row max taken out first;
+//   MODE 1 soft n-step (q_nstep_sql_td_error, :1219-1245): the n-step return of V' = alpha*logsumexp(next_n_q / alpha)
+//          (+inf -> 20, -inf -> -20);
+//   MODE 2 value 1-step (q_v_1step_td_error, :198-219): gamma*(1 - d)*v + r.
+// Gathering q_sa, the criterion, the loss sum and the record qntd_bwd_kernel reads (dcrit, and the unit gradient) are those of
+// qntd_fwd_kernel; every target is detached, so the gradient reaches q through q_sa alone.
+// ---------------------------------------------------------------------------------------------------------------
+struct SoftTdArgs {
+    const float* q;           // (R, N)
+    const float* target_q;    // MODE 0: (R, N), the target network on the current observation
+    const float* next_q;      // MODE 0 / 1: (R, N); MODE 2: the state value v (R)
+    const long long* action;  // (R)
+    const float* reward;      // MODE 1: (nstep, S), (S) when cum_reward; MODE 0 / 2: (S)
+    const float* done;        // (S)
+    const float* weight;      // (R) or null
+    const float* value_gamma; // MODE 1: null, or stride 0 (0-dim) / 1 (S)
+    long long value_gamma_stride;
+    long long R;              // rows
+    int G;                    // rows per sample (S = R / G): reward and done of row r are sample r / G's
+    int N;
+    int nstep;
+    float gamma, gamma_pow_n;
+    float tau, alpha;
+    int cum_reward;
+    int criterion;
+    float crit_param;
+    double loss_div;          // loss = sum(w*td) / loss_div, action_gap = sum(top1 - top2) / loss_div
+    float* loss;
+    float* td_err;            // (R)
+    float* dcrit;             // (R) d criterion / d q_sa: what qntd_bwd_kernel reads (G = 1 there)
+    float* target;            // nullable (R): the detached target, for callers that apply their own criterion
+    float* grad_unit;         // nullable (R, N): d loss / d q for a unit upstream gradient
+    float* action_gap;        // MODE 0
+    float* clipfrac;          // MODE 0 (R): 1 where log pi(a) was clamped
+    float* record_v;          // MODE 1, nullable (R): V' before the return is formed
+};
+
+// torch.logsumexp over a row y(0..n) (ATen logsumexp_out_impl): m = amax(y), NaN propagating, taken as 0 when it is
+// infinite; the result is log(sum_j exp(y_j - m)) + m.  m and the sum are returned too: softmax(y) = exp(y - m) / sum
+// wherever m is finite.
+template <class F>
+__device__ __forceinline__ float row_logsumexp(F y, int n, float& m, float& sum) {
+    m = -INFINITY;
+#pragma unroll 1
+    for (int j = 0; j < n; ++j) {
+        const float x = y(j);
+        if (x > m || x != x) m = x;
+    }
+    if (fabsf(m) == INFINITY) m = 0.f;
+    sum = 0.f;
+#pragma unroll 1
+    for (int j = 0; j < n; ++j) sum = fadd(sum, expf(fsub(y(j), m)));
+    return fadd(logf(sum), m);
+}
+
+template <int NT, int MODE>
+__global__ void __launch_bounds__(NT) soft_td_fwd_kernel(SoftTdArgs a, float* ws) {
+    pdl_prologue();
+    constexpr int K = MODE == 0 ? 2 : 1;  // loss (and the action gap)
+    __shared__ float s_coef[NT];
+    __shared__ int s_act[NT];
+    const long long r0 = (long long)blockIdx.x * NT;
+    const long long r = r0 + threadIdx.x;
+    const float inv_div = (float)(1.0 / a.loss_div);
+    float acc[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) acc[k] = 0.f;
+    s_coef[threadIdx.x] = 0.f;
+    s_act[threadIdx.x] = -1;
+    if (r < a.R) {
+        const long long s = MODE == 2 ? r / a.G : r;  // G == 1 in modes 0 and 1
+        const int N = a.N;
+        const int act = (int)a.action[r];
+        const float q_sa = a.q[r * N + act];
+        const float nd = fsub(1.f, a.done[s]);
+        float target;
+        if (MODE == 0) {
+            const float* __restrict__ tq = a.target_q + r * N;
+            const float* __restrict__ nq = a.next_q + r * N;
+            const float rw = a.reward[s];
+            // row max of target_q (torch.max: NaN propagates) and its top two for the action gap (topk: equal maxima give 0)
+            float v = -INFINITY, t1 = -INFINITY, t2 = -INFINITY, vn = -INFINITY;
+            for (int j = 0; j < N; ++j) {
+                const float x = tq[j], y = nq[j];
+                if (x > v || x != x) v = x;
+                if (y > vn || y != y) vn = y;
+                if (x > t1) {
+                    t2 = t1;
+                    t1 = x;
+                } else if (x > t2) {
+                    t2 = x;
+                }
+            }
+            float m, sm, mn, smn;
+            const float lse = row_logsumexp([&](int j) { return __fdiv_rn(fsub(tq[j], v), a.tau); }, N, m, sm);
+            const float lse_n = row_logsumexp([&](int j) { return __fdiv_rn(fsub(nq[j], vn), a.tau); }, N, mn, smn);
+            const float lp = fsub(fsub(tq[act], v), fmul(a.tau, lse));  // log_pi.gather(1, act), td.py:132-135
+            const float clamped = lp != lp ? lp : fminf(fmaxf(lp, -1.f), 1.f);  // torch.clamp keeps NaN
+            a.clipfrac[r] = (lp > 1.f || lp < -1.f) ? 1.f : 0.f;
+            const float tl = fmul(a.tau, lse_n);
+            float soft = 0.f;  // sum_j pi'_j * (q'_j - tau_log_pi'_j) * (1 - d), td.py:141-145
+            for (int j = 0; j < N; ++j) {
+                const float d = fsub(nq[j], vn);
+                const float pi = __fdiv_rn(expf(fsub(__fdiv_rn(d, a.tau), mn)), smn);
+                soft = fadd(soft, fmul(fmul(pi, fsub(nq[j], fsub(d, tl))), nd));
+            }
+            target = fadd(fadd(rw, fmul(a.alpha, clamped)), fmul(a.gamma, soft));  // td.py:147
+            acc[1] = fsub(t1, t2);
+        } else if (MODE == 1) {
+            const float* __restrict__ nq = a.next_q + r * N;
+            const float* __restrict__ rw = a.reward + r;
+            const size_t Bi = (size_t)a.R;
+            const int nrw = a.cum_reward ? 1 : a.nstep;
+            float rwv[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) rwv[i] = i < nrw ? rw[i * Bi] : 0.f;
+            const float vg = a.value_gamma ? a.value_gamma[r * a.value_gamma_stride] : a.gamma_pow_n;
+            float ret;
+            if (a.cum_reward) {
+                ret = rwv[0];
+            } else {
+                float rf;
+                ret = nstep_reward_sum(rwv, rw, Bi, a.nstep, a.gamma, rf);
+            }
+            float m, sm;
+            float tv = fmul(a.alpha, row_logsumexp([&](int j) { return __fdiv_rn(nq[j], a.alpha); }, N, m, sm));
+            if (tv == INFINITY) tv = 20.f;  // td.py:1230-1231; NaN stays NaN
+            else if (tv == -INFINITY) tv = -20.f;
+            if (a.record_v) a.record_v[r] = tv;
+            target = fadd(ret, fmul(fmul(vg, tv), nd));  // td.py:1239 / :1241 / nstep_return :267, :273
+        } else {
+            target = fadd(fmul(fmul(a.gamma, nd), a.next_q[r]), a.reward[s]);  // td.py:205 / :217
+        }
+        const float w = a.weight ? a.weight[r] : 1.f;  // read after the target: one value fewer live across the row loops
+        float dx;
+        const float td = criterion_eval(a.criterion, a.crit_param, q_sa, target, dx);
+        a.td_err[r] = td;
+        if (a.target) a.target[r] = target;
+        a.dcrit[r] = dx;
+        acc[0] = td * w;
+        if (a.grad_unit) {
+            s_coef[threadIdx.x] = w * dx * inv_div;
+            s_act[threadIdx.x] = act;
+        }
+    }
+    if (a.grad_unit) {  // the block's NT gradient rows are contiguous: coalesced stores
+        __syncthreads();
+        const long long rows = (a.R - r0) < NT ? (a.R - r0) : NT;
+        float* gq = a.grad_unit + r0 * a.N;
+        for (long long i = threadIdx.x; i < rows * a.N; i += NT) {
+            const int rr = (int)(i / a.N), j = (int)(i - (long long)rr * a.N);
+            gq[i] = (j == s_act[rr]) ? s_coef[rr] : 0.f;
+        }
+    }
+    auto fin = [&](int k, double t) {
+        const float v = (float)(t / a.loss_div);
+        if (k == 0) a.loss[0] = v;
+        else a.action_gap[0] = v;
+    };
+    // one atomic round trip (none for a one-CTA grid); the 256 / 512 / 1024-thread builds only ever run as one CTA
+    if (NT > 128 || gridDim.x <= FX_MAX_GRID) {
+        grid_sum_fx<K, NT>(acc, ws, fin);
+        return;
+    }
+    double tot[K];
+    if (grid_sum<K, NT>(acc, tot, ws, 0) && threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) fin(k, tot[k]);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // C51 categorical projection: one warp per (sample, agent) row, lanes stride the atoms, the projected distribution is
 // accumulated with shared-memory atomics (the index_add_ of td.py:510-511) and kept for the backward pass.
 // ---------------------------------------------------------------------------------------------------------------
@@ -1021,6 +1196,52 @@ extern "C" int b200rl_dqfd_bwd(const float* saved, const float* weight, const lo
                     action, g_loss, g_td, g_loss_statistics_n, g_loss_statistics_1, g_loss_statistics_je, S, (int)N,
                     (float)lambda_n_step_td, (float)lambda_one_step_td, (float)lambda_supervised_loss, inv_div, skip_if_unit,
                     grad_q);
+}
+
+template <int MODE>
+static int launch_soft_td(const SoftTdArgs& a, float* ws, size_t ws_bytes, cudaStream_t st) {
+    if (a.R <= 1024) {  // the usual replay-buffer batch: ONE CTA, no grid reduction at all
+        if (a.R <= 256) return launch_k(soft_td_fwd_kernel<256, MODE>, 1, 256, 0, st, a, ws);
+        if (a.R <= 512) return launch_k(soft_td_fwd_kernel<512, MODE>, 1, 512, 0, st, a, ws);
+        return launch_k(soft_td_fwd_kernel<1024, MODE>, 1, 1024, 0, st, a, ws);
+    }
+    constexpr int NT = 128;
+    const long long grid = div_up(a.R, NT);
+    if (!ws_partials_fit(grid * (MODE == 0 ? 2 : 1), ws_bytes)) return B200RL_ERR_WORKSPACE;
+    return launch_k(soft_td_fwd_kernel<NT, MODE>, (int)grid, NT, 0, st, a, ws);
+}
+
+extern "C" int b200rl_soft_td_fwd(int mode, const float* q, const float* target_q, const float* next_q,
+                                  const long long* action, const float* reward, const float* done, const float* weight,
+                                  const float* value_gamma, long long value_gamma_stride, long long S, long long G,
+                                  long long N, int nstep, double gamma, double tau, double alpha, int cum_reward,
+                                  int criterion, double criterion_param, float* loss, float* td_error_per_sample,
+                                  float* dcrit_saved, float* target_out, float* grad_q_unit, float* action_gap,
+                                  float* clipfrac, float* record_target_v, float* workspace, size_t workspace_bytes,
+                                  void* stream) {
+    if (mode < 0 || mode > 2 || S <= 0 || G < 1 || N < 1 || !q || !next_q || !action || !reward || !done || !loss ||
+        !td_error_per_sample || !dcrit_saved || !workspace)
+        return B200RL_ERR_ARG;
+    if (criterion < 0 || criterion > 3) return B200RL_ERR_ARG;
+    if (mode != 2 && G != 1) return B200RL_ERR_ARG;
+    if (mode == 0 && (N < 2 || !target_q || !action_gap || !clipfrac)) return B200RL_ERR_ARG;
+    if (mode == 1 && nstep < 1) return B200RL_ERR_ARG;
+    if (mode != 1 && (cum_reward || value_gamma)) return B200RL_ERR_ARG;
+    if (workspace_bytes < WS_MIN_BYTES) return B200RL_ERR_WORKSPACE;
+    SoftTdArgs a{};
+    a.q = q; a.target_q = target_q; a.next_q = next_q; a.action = action; a.reward = reward; a.done = done;
+    a.weight = weight; a.value_gamma = value_gamma; a.value_gamma_stride = value_gamma_stride;
+    a.R = S * G; a.G = (int)G; a.N = (int)N; a.nstep = mode == 1 ? nstep : 1;
+    a.gamma = (float)gamma; a.gamma_pow_n = (float)pow(gamma, (double)a.nstep);  // python's `gamma ** nstep`, then fp32
+    a.tau = (float)tau; a.alpha = (float)alpha; a.cum_reward = cum_reward;
+    a.criterion = criterion; a.crit_param = (float)criterion_param;
+    a.loss_div = (double)S * (double)G;
+    a.loss = loss; a.td_err = td_error_per_sample; a.dcrit = dcrit_saved; a.target = target_out; a.grad_unit = grad_q_unit;
+    a.action_gap = action_gap; a.clipfrac = clipfrac; a.record_v = record_target_v;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (mode == 0) return launch_soft_td<0>(a, workspace, workspace_bytes, st);
+    if (mode == 1) return launch_soft_td<1>(a, workspace, workspace_bytes, st);
+    return launch_soft_td<2>(a, workspace, workspace_bytes, st);
 }
 
 extern "C" int b200rl_dntd_fwd(const float* dist, const float* next_n_dist, const long long* act,

@@ -502,6 +502,53 @@ class DQfDTDFunction(torch.autograd.Function):
         return (grad_q.view(ctx.q_shape), ) + (None, ) * (n_in - 1)
 
 
+class SoftTDFunction(torch.autograd.Function):
+    """The TD losses of the entropy-regularised value learners (csrc/td.cu soft_td_fwd): mode 0 Munchausen, 1 soft n-step
+    (SQL), 2 value 1-step (discrete SAC).  Outputs: loss and td_error_per_sample (R rows; both differentiable w.r.t. q), the
+    detached target, and the mode's statistics, which carry no gradient as in the reference: action_gap and clipfrac
+    (mode 0), record_target_v (mode 1); the others are empty.
+
+    Every target is detached, so the gradient reaches q through q_sa alone and the backward is QNStepTDFunction's launch
+    (b200rl_qntd_bwd with G = 1 over the R rows).  As there, ONE forward launch also writes d loss / d q for a unit upstream
+    gradient, which the backward verifies on the device and hands to autograd.  No host sync."""
+
+    @staticmethod
+    def forward(ctx, q, target_q, next_q, action, reward, done, weight, value_gamma, vg_stride, mode, S, G, N, nstep, gamma,
+                tau, alpha, cum_reward, criterion, crit_param):
+        dev = q.device
+        R = S * G
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        td = torch.empty(R, dtype=torch.float32, device=dev)
+        dcrit = torch.empty(R, dtype=torch.float32, device=dev)
+        target = torch.empty(R, dtype=torch.float32, device=dev)
+        gap = torch.empty((), dtype=torch.float32, device=dev) if mode == 0 else None
+        clip = torch.empty(R, dtype=torch.float32, device=dev) if mode == 0 else None
+        rec = torch.empty(R, dtype=torch.float32, device=dev) if mode == 1 else None
+        grad_unit = torch.empty(R, N, dtype=torch.float32, device=dev) if ctx.needs_input_grad[0] else None
+        with on_device(dev):
+            ws = workspace(dev)
+            rc = lib().b200rl_soft_td_fwd(
+                mode, ptr(q), ptr(target_q), ptr(next_q), ptr(action), ptr(reward), ptr(done), ptr(weight),
+                ptr(value_gamma), vg_stride, S, G, N, nstep, gamma, tau, alpha, cum_reward, criterion, crit_param,
+                ptr(loss), ptr(td), ptr(dcrit), ptr(target), ptr(grad_unit), ptr(gap), ptr(clip), ptr(rec), ptr(ws),
+                ws.numel() * 4, stream_ptr()
+            )
+        _lib.check(rc, 'b200rl_soft_td_fwd')
+        ctx.save_for_backward(dcrit, action, weight)
+        ctx.cfg = (R, 1, N, 0, 0)  # QNStepTDFunction's (S, G, N, group_mean, seq_len): R rows of one
+        ctx.q_shape = q.shape
+        ctx.spec = grad_unit
+        ctx.set_materialize_grads(False)
+        empty = torch.empty(0, dtype=torch.float32, device=dev)
+        gap, clip, rec = (x if x is not None else empty for x in (gap, clip, rec))
+        ctx.mark_non_differentiable(target, gap, clip, rec)
+        return loss, td, target, gap, clip, rec
+
+    @staticmethod
+    def backward(ctx, g_loss, g_td, _g_target, _g_gap, _g_clip, _g_rec):
+        return QNStepTDFunction.backward(ctx, g_loss, g_td, None, None)[:1] + (None, ) * 19
+
+
 # ----------------------------------------------------------------------------------------------------------------
 # ACER heads (csrc/acer.cu): un-reduced per-transition losses, plain forward / backward launches
 # ----------------------------------------------------------------------------------------------------------------

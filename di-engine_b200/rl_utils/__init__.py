@@ -10,8 +10,9 @@ from .ppo import (normalize_advantage, ppo_data, ppo_error, ppo_error_adv_norm, 
                   ppo_value_data, ppo_value_error, shape_fn_ppo)
 from .td import (bdq_nstep_td_error, dist_1step_td_data, dist_1step_td_error, dist_nstep_td_data, dist_nstep_td_error,
                  dqfd_nstep_td_data, dqfd_nstep_td_error, dqfd_nstep_td_error_sequence, dqfd_nstep_td_error_with_rescale,
-                 dqfd_nstep_td_seq_data, generalized_lambda_returns, q_1step_td_data, q_1step_td_error, q_nstep_td_data, q_nstep_td_error,
-                 q_nstep_td_error_sequence, q_nstep_td_error_with_rescale, q_nstep_td_seq_data, shape_fn_dntd,
+                 dqfd_nstep_td_seq_data, generalized_lambda_returns, m_q_1step_td_data, m_q_1step_td_error, q_1step_td_data,
+                 q_1step_td_error, q_nstep_sql_td_error, q_nstep_td_data, q_nstep_td_error, q_nstep_td_error_sequence,
+                 q_nstep_td_error_with_rescale, q_nstep_td_seq_data, q_v_1step_td_data, q_v_1step_td_error, shape_fn_dntd,
                  shape_fn_qntd, shape_fn_qntd_rescale, shape_fn_td_lambda, td_lambda_data, td_lambda_error,
                  v_1step_td_data, v_1step_td_error, v_nstep_td_data, v_nstep_td_error)
 from .ppg import ppg_data, ppg_joint_error, ppg_joint_loss
@@ -32,7 +33,8 @@ HOT_PATH_FUNCTIONS = [
     'vtrace_error_continuous_action', 'qrdqn_nstep_td_error', 'iqn_nstep_td_error', 'fqf_nstep_td_error',
     'compute_q_retraces', 'happo_error', 'happo_policy_error', 'happo_value_error', 'happo_error_continuous', 'happo_policy_error_continuous',
     'acer_policy_error', 'acer_value_error', 'acer_trust_region_update', 'ppg_joint_error',
-    'dqfd_nstep_td_error', 'dqfd_nstep_td_error_with_rescale'
+    'dqfd_nstep_td_error', 'dqfd_nstep_td_error_with_rescale',
+    'm_q_1step_td_error', 'q_nstep_sql_td_error', 'q_v_1step_td_error'
 ]
 HOT_PATH_TYPES = [
     'gae_data', 'ppo_data', 'ppo_loss', 'ppo_info', 'q_nstep_td_data', 'dist_nstep_td_data', 'td_lambda_data',
@@ -40,5 +42,5 @@ HOT_PATH_TYPES = [
     'ppo_policy_data', 'ppo_policy_loss', 'ppo_value_data', 'dist_1step_td_data', 'a2c_data', 'a2c_loss',
     'qrdqn_nstep_td_data', 'iqn_nstep_td_data', 'fqf_nstep_td_data',
     'happo_data', 'happo_policy_data', 'happo_value_data', 'happo_loss', 'happo_policy_loss', 'happo_info', 'ppg_data', 'ppg_joint_loss',
-    'dqfd_nstep_td_data'
+    'dqfd_nstep_td_data', 'm_q_1step_td_data', 'q_v_1step_td_data'
 ]

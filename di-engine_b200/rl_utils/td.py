@@ -4,7 +4,9 @@
   td_lambda_error (:1539-1571), generalized_lambda_returns (:1574-1605),
   and the 1-step / state-value siblings that reuse the q-n-step kernels (SURVEY section 8f rank 2):
   q_1step_td_error (:26-72), v_1step_td_error (:529-573), v_nstep_td_error (:579-617);
-  dqfd_nstep_td_error (:870-983) / dqfd_nstep_td_error_with_rescale (:986-1090) on their own kernel (dqfd_fwd / dqfd_bwd).
+  dqfd_nstep_td_error (:870-983) / dqfd_nstep_td_error_with_rescale (:986-1090) on their own kernel (dqfd_fwd / dqfd_bwd);
+  m_q_1step_td_error (:75-158), q_nstep_sql_td_error (:1175-1245) and q_v_1step_td_error (:161-219) on one forward kernel
+  (soft_td_fwd) and the q-n-step backward.
 """
 from collections import namedtuple
 from typing import Callable, Optional, Union
@@ -686,6 +688,208 @@ def dqfd_nstep_td_error_sequence(
     if host_out:
         loss, prio, per, s_n, s_1, s_je = loss.cpu(), prio.cpu(), per.cpu(), s_n.cpu(), s_1.cpu(), s_je.cpu()
     return loss, prio, per, (s_n, s_1, s_je)
+
+
+m_q_1step_td_data = namedtuple('m_q_1step_td_data', ['q', 'target_q', 'next_q', 'act', 'reward', 'done', 'weight'])
+q_v_1step_td_data = namedtuple('q_v_1step_td_data', ['q', 'v', 'act', 'reward', 'done', 'weight'])
+
+
+def _soft_done(done, dev):
+    """``done`` as the float multiplier of ``(1 - done)``; a bool tensor raises as the reference's ``1 - done`` does"""
+    if done.dtype == torch.bool:
+        raise RuntimeError("Subtraction, the `-` operator, with a bool tensor is not supported. If you are trying to invert a "
+                           "mask, use the `~` or `logical_not()` operator instead.")
+    return ops.f32c(ops.to_device(done.detach(), dev), 'done')
+
+
+def _soft_weight(weight, td_shape, dev):
+    """``(td_error_per_sample * weight).mean()``: a weight that broadcasts to the error's shape, expanded to one per row"""
+    if weight is None:
+        return None
+    w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
+    if torch.broadcast_shapes(tuple(w.shape), tuple(td_shape)) != tuple(td_shape):
+        raise ValueError("weight %s does not broadcast to the td error shape %s" % (tuple(weight.shape), tuple(td_shape)))
+    return w.expand(td_shape).reshape(-1).contiguous()
+
+
+def _soft_td(mode, q, target_q, next_q, act, reward, done, weight, S, G, gamma, criterion, nstep=1, tau=0.0, alpha=0.0,
+             cum_reward=False, value_gamma=None):
+    """The three losses on the soft_td kernel: q (S*G, N) on the compute device, carrying its gradient; the other operands
+    staged there and detached.  -> (loss, td (S*G,), action_gap, clipfrac (S*G,), record_target_v (S*G,)), the last three
+    empty where the mode has none."""
+    R, N = q.shape
+    vg, vg_stride = _value_gamma_arg(value_gamma, S, q.device)
+    code = _criterion_code(criterion)
+
+    def kernel(q_, crit, param):
+        return ops.SoftTDFunction.apply(q_, target_q, next_q, act, reward, done, weight, vg, vg_stride, mode, S, G, N,
+                                        int(nstep), float(gamma), float(tau), float(alpha), 1 if cum_reward else 0, crit,
+                                        param)
+
+    if code is not None:
+        loss, per, _, gap, clip, rec = kernel(q, code[0], code[1])
+        return loss, per, gap, clip, rec
+    # a criterion the kernel does not know runs as torch ops on the kernel's detached target
+    _, _, target, gap, clip, rec = kernel(q.detach(), 0, 0.0)
+    per = criterion(q.gather(1, act.reshape(R, 1)).reshape(R), target)
+    loss = (per * (weight if weight is not None else 1.0)).mean()
+    return loss, per, gap, clip, rec
+
+
+def m_q_1step_td_error(
+        data: namedtuple,
+        gamma: float,
+        tau: float,
+        alpha: float,
+        criterion: torch.nn.modules = nn.MSELoss(reduction='none')  # noqa
+) -> torch.Tensor:
+    """
+    Munchausen 1-step TD error (M-DQN), drop-in for ding/rl_utils/td.py:75-158.  The target is
+    ``reward + alpha*clamp(log_pi[act], -1, 1) + gamma * sum_j pi'_j * (next_q_j - tau*log pi'_j) * (1 - done)``, with
+    ``log_pi`` the log-softmax policy of ``target_q / tau`` and ``pi'`` the softmax policy of ``next_q / tau``.
+
+    Shapes: q, target_q (the target network on the current observation), next_q (B, N) with N >= 2; act (B,) int64;
+    reward, done (B,); weight (B,) or None.  ``tau`` and ``alpha`` are divided by as fp32 values.  Returns ``(loss,
+    td_error_per_sample (B,), action_gap, clipfrac (B, 1))``: the first two differentiable w.r.t. ``q``; ``action_gap`` is
+    the mean of top-1 minus top-2 of ``target_q`` and ``clipfrac`` the per-sample float flag of a clamped ``log_pi[act]``,
+    neither with gradient.  One forward and one backward launch.
+    """
+    q, target_q, next_q, act, reward, done, weight = data
+    assert len(act.shape) == 1, act.shape        # td.py:121
+    assert len(reward.shape) == 1, reward.shape  # td.py:122
+    if q.dim() != 2:
+        raise ValueError("m_q_1step_td_error: q must be (B, N), got %s" % (tuple(q.shape), ))
+    B, N = q.shape
+    if N < 2:
+        raise RuntimeError("selected index k out of range")  # target_q.topk(2), td.py:152
+    host_out = not q.is_cuda
+    dev = ops.compute_device(q, target_q, next_q)
+    qd = ops.f32c(ops.to_device(q, dev), 'q')
+    tq = ops.f32c(ops.to_device(target_q.detach(), dev), 'target_q')
+    nq = ops.f32c(ops.to_device(next_q.detach(), dev), 'next_q')
+    a = ops.i64c(ops.to_device(act, dev), N, 'act')
+    r = ops.f32c(ops.to_device(reward.detach(), dev), 'reward')
+    d = _soft_done(done, dev)
+    if tq.shape != qd.shape or nq.shape != qd.shape or a.numel() != B or r.numel() != B or d.numel() != B:
+        raise ValueError("m_q_1step_td_error: q %s / target_q %s / next_q %s / act %s / reward %s / done %s do not match" %
+                         (tuple(q.shape), tuple(target_q.shape), tuple(next_q.shape), tuple(act.shape),
+                          tuple(reward.shape), tuple(done.shape)))
+    w = _soft_weight(weight, (B, ), dev)
+    loss, per, gap, clip, _ = _soft_td(0, qd, tq, nq, a, r, d, w, B, 1, gamma, criterion, tau=tau, alpha=alpha)
+    clip = clip.reshape(B, 1)
+    if host_out:
+        loss, per, gap, clip = loss.cpu(), per.cpu(), gap.cpu(), clip.cpu()
+    return loss, per, gap, clip
+
+
+def q_nstep_sql_td_error(
+        data: namedtuple,
+        gamma: float,
+        alpha: float,
+        nstep: int = 1,
+        cum_reward: bool = False,
+        value_gamma: Optional[torch.Tensor] = None,
+        criterion: torch.nn.modules = nn.MSELoss(reduction='none'),
+) -> torch.Tensor:
+    """
+    Soft Q-learning n-step TD error (SQL), drop-in for ding/rl_utils/td.py:1175-1245: the n-step return (td.py:230-286) of
+    the soft state value ``alpha * logsumexp(next_n_q / alpha)``, with +inf replaced by 20 and -inf by -20.
+
+    Shapes: q, next_n_q (B, N); action (B,) int64 (next_n_action is not used, as in the reference); reward (nstep, B), or
+    (B,) with ``cum_reward``; done (B,); weight (B,) or None; value_gamma None, scalar, 0-dim or (B,); gamma a float (an int
+    too with ``cum_reward``).  With ``cum_reward`` a (K, B) reward broadcasts the error to (K, B), as the reference's own test
+    does (tests/test_td.py:449-454).  ``alpha`` is divided by as an fp32 value.  Returns ``(loss, td_error_per_sample,
+    record_target_v (B,))``; ``record_target_v`` is the soft value before the return is formed, without gradient.
+    """
+    q, next_n_q, action, next_n_action, reward, done, weight = data
+    assert len(action.shape) == 1, action.shape  # td.py:1220
+    if isinstance(gamma, list):
+        raise NotImplementedError("q_nstep_sql_td_error: a list gamma (the NGU per-sample form) is not supported; no policy "
+                                  "passes one")
+    if not (isinstance(gamma, float) or (cum_reward and isinstance(gamma, int))):
+        raise TypeError("The type of gamma should be float or list")  # nstep_return, td.py:284
+    if not cum_reward:
+        assert reward.shape[0] == nstep  # td.py:257
+    if q.dim() != 2:
+        raise ValueError("q_nstep_sql_td_error: q must be (B, N), got %s" % (tuple(q.shape), ))
+    B, N = q.shape
+    host_out = not q.is_cuda
+    dev = ops.compute_device(q, next_n_q)
+    qd = ops.f32c(ops.to_device(q, dev), 'q')
+    nq = ops.f32c(ops.to_device(next_n_q.detach(), dev), 'next_n_q')
+    a = ops.i64c(ops.to_device(action, dev), N)
+    r = ops.f32c(ops.to_device(reward.detach(), dev), 'reward')
+    d = _soft_done(done, dev)
+    if nq.shape != qd.shape or a.numel() != B or d.numel() != B:
+        raise ValueError("q_nstep_sql_td_error: q %s / next_n_q %s / action %s / done %s do not match" %
+                         (tuple(q.shape), tuple(next_n_q.shape), tuple(action.shape), tuple(done.shape)))
+    td_shape = (B, )
+    vg = value_gamma
+    if cum_reward and r.dim() == 2 and r.shape[1] == B:
+        # reward + v * target_v * (1 - done) broadcasts to (K, B) (td.py:1239-1241): K independent row sets of the same q
+        K = r.shape[0]
+        td_shape = (K, B)
+
+        def rep(x):
+            return x.unsqueeze(0).expand((K, ) + tuple(x.shape)).reshape((K * B, ) + tuple(x.shape[1:]))
+
+        qd, nq, a, d = rep(qd), rep(nq), rep(a), rep(d)
+        r = r.reshape(K * B)
+        if isinstance(vg, torch.Tensor) and vg.numel() == B:
+            vg = rep(ops.to_device(vg.detach(), dev).reshape(B))
+    elif tuple(r.shape) != ((B, ) if cum_reward else (nstep, B)):
+        raise ValueError("q_nstep_sql_td_error: reward %s does not match B=%d, nstep=%d, cum_reward=%s" %
+                         (tuple(reward.shape), B, nstep, cum_reward))
+    w = _soft_weight(weight, td_shape, dev)
+    S = qd.shape[0]
+    loss, per, _, _, rec = _soft_td(1, qd, None, nq, a, r, d, w, S, 1, gamma, criterion, nstep=nstep, alpha=alpha,
+                                    cum_reward=cum_reward, value_gamma=vg)
+    per, rec = per.reshape(td_shape), rec[:B]
+    if host_out:
+        loss, per, rec = loss.cpu(), per.cpu(), rec.cpu()
+    return loss, per, rec
+
+
+def q_v_1step_td_error(
+        data: namedtuple, gamma: float, criterion: torch.nn.modules = nn.MSELoss(reduction='none')
+) -> torch.Tensor:
+    """
+    1-step TD error between q and a state value (the discrete SAC critic), drop-in for ding/rl_utils/td.py:161-219:
+    ``target = gamma * (1 - done) * v + reward``.
+
+    Shapes: q (B, N), act (B,) int64, v (B,); or the multi-agent form q (B, A, N), act (B, A), v (B, A), whose reward and
+    done are broadcast over the A agents.  reward, done (B,); weight None or broadcastable to the error's shape.  Returns
+    ``(loss, td_error_per_sample)``, the error shaped like ``act``; both differentiable w.r.t. ``q``.
+    """
+    q, v, act, reward, done, weight = data
+    assert len(reward.shape) == 1, reward.shape  # td.py:200 / :207
+    if act.dim() == 1:
+        B, A = act.shape[0], 1
+    elif act.dim() == 2:
+        B, A = act.shape
+    else:
+        raise ValueError("q_v_1step_td_error: act must be (B,) or (B, A), got %s" % (tuple(act.shape), ))
+    td_shape = tuple(act.shape)
+    N = q.shape[-1]
+    if tuple(q.shape) != td_shape + (N, ) or tuple(v.shape) != td_shape:
+        raise ValueError("q_v_1step_td_error: q %s / v %s do not match act %s" %
+                         (tuple(q.shape), tuple(v.shape), tuple(act.shape)))
+    host_out = not q.is_cuda
+    dev = ops.compute_device(q, v)
+    qd = ops.f32c(ops.to_device(q, dev), 'q').reshape(B * A, N)
+    vv = ops.f32c(ops.to_device(v.detach(), dev), 'v')
+    a = ops.i64c(ops.to_device(act, dev), N, 'act')
+    r = ops.f32c(ops.to_device(reward.detach(), dev), 'reward')
+    d = _soft_done(done, dev)
+    if r.numel() != B or d.numel() != B:
+        raise ValueError("q_v_1step_td_error: reward %s / done %s do not match B=%d" %
+                         (tuple(reward.shape), tuple(done.shape), B))
+    w = _soft_weight(weight, td_shape, dev)
+    loss, per, _, _, _ = _soft_td(2, qd, None, vv, a, r, d, w, B, A, gamma, criterion)
+    per = per.reshape(td_shape)
+    if host_out:
+        loss, per = loss.cpu(), per.cpu()
+    return loss, per
 
 
 def _as_columns(v, next_v, reward, done, weight, value_gamma=None, nstep=None):

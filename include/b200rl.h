@@ -185,6 +185,32 @@ B200RL_API int b200rl_dqfd_bwd(const float* saved, const float* weight, const lo
                     double lambda_one_step_td, double lambda_supervised_loss, long long seq_len, int skip_if_unit,
                     float* grad_q, void* stream);
 
+/* ---- the TD losses of the entropy-regularised value learners, one forward entry point (csrc/td.cu soft_td_fwd_kernel):
+ *      mode 0  m_q_1step_td_error (Munchausen DQN): ding/rl_utils/td.py:75-158
+ *      mode 1  q_nstep_sql_td_error (soft Q-learning): td.py:1175-1245, nstep_return :230-286
+ *      mode 2  q_v_1step_td_error (discrete SAC critic): td.py:161-219
+ * S samples with G rows each (G = 1; the agent dim of mode 2's multi-agent branch, td.py:206-217), R = S*G rows.
+ * q: (R, N); action: (R) int64; done: (S) floats; weight nullable (R); reward: (S), mode 1 (nstep, S) or (S) when cum_reward.
+ * Mode 0: target_q (R, N) is the target network on the current observation, next_q (R, N) on the next one; target = reward
+ *   + alpha*clamp(log_pi[a], -1, 1) + gamma * sum_j pi'_j * (next_q_j - tau*log pi'_j) * (1 - done), with log_pi / pi' the
+ *   softmax policies of target_q / tau and next_q / tau (row max taken out first); action_gap (1) = mean over R of top-1 minus
+ *   top-2 of target_q; clipfrac (R) = 1 where log_pi[a] lies outside [-1, 1].  N >= 2.
+ * Mode 1: next_q = next_n_q (R, N); V' = alpha*logsumexp(next_n_q / alpha) with +inf -> 20, -inf -> -20, written to
+ *   record_target_v (R, nullable) before the return is formed; the return is nstep_return's (value_gamma as for
+ *   b200rl_qntd_fwd) or, with cum_reward, reward + (value_gamma or gamma**nstep) * V' * (1 - done).
+ * Mode 2: next_q = v (R); target = gamma * (1 - done) * v + reward.
+ * tau and alpha are divided by as fp32 values (true division).  criterion / criterion_param as for b200rl_qntd_fwd.
+ * ONE launch writes loss (1) = sum(w*td) / R, td_error_per_sample (R), dcrit_saved (R), the detached target (target_out,
+ * nullable) and -- grad_q_unit (R, N), nullable -- d loss / d q for a unit upstream gradient.  Every target is detached, so
+ * the backward is b200rl_qntd_bwd(dcrit_saved, weight, action, g_loss, g_td, R, 1, N, 0, 0, skip_if_unit, grad_q). */
+B200RL_API int b200rl_soft_td_fwd(int mode, const float* q, const float* target_q, const float* next_q, const long long* action,
+                       const float* reward, const float* done, const float* weight, const float* value_gamma,
+                       long long value_gamma_stride, long long S, long long G, long long N, int nstep, double gamma,
+                       double tau, double alpha, int cum_reward, int criterion, double criterion_param, float* loss,
+                       float* td_error_per_sample, float* dcrit_saved, float* target_out, float* grad_q_unit,
+                       float* action_gap, float* clipfrac, float* record_target_v, float* workspace,
+                       size_t workspace_bytes, void* stream);
+
 /* ---- dist_nstep_td_error (C51): ding/rl_utils/td.py:413-523; dist_1step_td_error (:294-383) is its nstep = 1 case ---
  * dist, next_n_dist: (B*A, N, n_atom); act, next_n_act: (B*A) int64; reward: (nstep, B); done: (B);
  * weight nullable with stride 0 / 1 over the B*A rows; value_gamma nullable with stride 0 / 1 over B;
