@@ -63,6 +63,7 @@ PROTOTYPES = {
     "b200rl_a2c_fwd_grad": [P, P, P, P, P, P, LL, LL, P, I, P, P, P, P, P, P, P, P, P, c_size_t, P],
     "b200rl_ppo_continuous_fwd_grad": [P, P, P, P, P, P, P, P, P, P, P, P, P, LL, LL, D, I, D, I, P, I, P, P, P, P, P, P, P, P, P,
                                        P, P, c_size_t, P],
+    "b200rl_a2c_continuous_fwd_grad": [P, P, P, P, P, P, P, LL, LL, P, I, P, P, P, P, P, P, P, P, P, P, c_size_t, P],
     "b200rl_gae_ppo_set_impl": [I],
     "b200rl_vtrace_set_impl": [I],
     "b200rl_acer_policy_fwd": [P, P, P, P, P, P, LL, LL, D, P, P, P],

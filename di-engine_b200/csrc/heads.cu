@@ -1,5 +1,6 @@
 // Sibling loss heads of the hot path (SURVEY section 8f rank 3), each forward + gradients in ONE launch:
 //   a2c_error              ding/rl_utils/a2c.py:10-44      policy -mean(logp*adv*w), value mean(w*(ret-v)^2), entropy mean(H*w)
+//   a2c_error_continuous   ding/rl_utils/a2c.py:50-88      the same three losses on an Independent(Normal(mu, sigma)) policy
 //   ppo_error_continuous   ding/rl_utils/ppo.py:278-374    the PPO loss of ppo.cu on an Independent(Normal(mu, sigma)) policy
 // Scheme of the other heads: thread = row, grid-stride, the forward launch also writes the gradients for the upstream
 // gradients it expects (the loss weights of the training loop, remembered on the device); the backward launch is the same
@@ -194,6 +195,62 @@ __global__ void __launch_bounds__(HD_NT) ppoc_kernel(PpocArgs a, float* ws) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// a2c_error_continuous: a2c_kernel's three losses on an Independent(Normal(mu, sigma)) policy
+// ---------------------------------------------------------------------------------------------------------------
+struct A2ccArgs {
+    const float* mu;      // (S, D)
+    const float* sigma;   // (S, D)
+    const float* action;  // (S, D)
+    const float* value;   // (S)
+    const float* adv;     // (S)
+    const float* ret;     // (S)
+    const float* weight;  // nullable (S)
+    long long S;
+    int D;
+    float* out;        // 3 losses
+    float* grad_mu;    // nullable: losses only
+    float* grad_sigma;
+    float* grad_value;
+    HeadGrads h;
+};
+
+__global__ void __launch_bounds__(HD_NT) a2cc_kernel(A2ccArgs a, float* ws) {
+    pdl_prologue();
+    float g[3];
+    if (head_upstream<3>(a.h, g)) return;
+    const bool grads = a.grad_mu != nullptr;
+    const float inv_s = 1.f / (float)a.S;
+    float acc[3] = {0.f, 0.f, 0.f};
+    for (long long s = (long long)blockIdx.x * HD_NT + threadIdx.x; s < a.S; s += (long long)gridDim.x * HD_NT) {
+        const long long o = s * a.D;
+        const float* mu = a.mu + o;
+        const float* sg = a.sigma + o;
+        const float* ac = a.action + o;
+        const float w = a.weight ? a.weight[s] : 1.f;
+        const float adv = a.adv[s], v = a.value[s], ret = a.ret[s];
+        const float lp = normal_logp(mu, sg, ac, a.D);
+        float ent = 0.f;
+        for (int d = 0; d < a.D; ++d) ent += kHalfPlusHalfLog2Pi + logf(sg[d]);
+        const float dv = ret - v;
+        acc[0] -= lp * adv * w;
+        acc[1] += dv * dv * w;
+        acc[2] += ent * w;
+        if (grads) {
+            const float c_lp = g[0] * (-adv * w) * inv_s, c_ent = g[2] * w * inv_s;
+            for (int d = 0; d < a.D; ++d) {
+                const float sd = sg[d], df = ac[d] - mu[d], inv = 1.f / sd;
+                a.grad_mu[o + d] = c_lp * df * inv * inv;
+                a.grad_sigma[o + d] = c_lp * (df * df * inv * inv * inv - inv) + c_ent * inv;
+            }
+            a.grad_value[s] = g[1] * (-2.f * w * dv) * inv_s;
+        }
+    }
+    if (a.h.verify) return;
+    const double is = 1.0 / (double)a.S;
+    grid_sum_fx<3, HD_NT>(acc, ws, [&](int k, double t) { a.out[k] = (float)(t * is); });
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // ppg_joint_error's behavioural-cloning term (ding/rl_utils/ppg.py:62-67): F.kl_div(logp_new, logp_old, 'batchmean') with the
 // LOG-probability of the old policy passed as the (non-log) target, exactly as the reference does:
 //   loss = (1/B) sum_b [ xlogy(t_b, t_b) - t_b * x_b ],   x_b = log pi_new(a_b), t_b = log pi_old(a_b) <= 0
@@ -278,6 +335,26 @@ extern "C" int b200rl_ppo_continuous_fwd_grad(
     a.h.g_expected = g_expected; a.h.g_actual[0] = g_policy; a.h.g_actual[1] = g_value; a.h.g_actual[2] = g_entropy;
     a.h.g_actual[3] = g_kl; a.h.g_used = g_used; a.h.g_hint = g_hint; a.h.verify = verify;
     return launch_k(ppoc_kernel, head_grid(S), HD_NT, 0, (cudaStream_t)stream, a, workspace);
+}
+
+extern "C" int b200rl_a2c_continuous_fwd_grad(const float* mu, const float* sigma, const float* action, const float* value,
+                                              const float* adv, const float* return_, const float* weight, long long S,
+                                              long long D, const float* g_expected, int verify, const float* g_policy,
+                                              const float* g_value, const float* g_entropy, float* g_used, float* g_hint,
+                                              float* out3, float* grad_mu, float* grad_sigma, float* grad_value,
+                                              float* workspace, size_t workspace_bytes, void* stream) {
+    if (S < 1 || D < 1 || !mu || !sigma || !action || !value || !adv || !return_ || !workspace ||
+        workspace_bytes < WS_MIN_BYTES)
+        return B200RL_ERR_ARG;
+    if (verify ? (!g_used || !grad_mu || !grad_sigma || !grad_value)
+               : (!out3 || (grad_mu && (!g_expected || !g_used || !grad_sigma || !grad_value))))
+        return B200RL_ERR_ARG;
+    A2ccArgs a{};
+    a.mu = mu; a.sigma = sigma; a.action = action; a.value = value; a.adv = adv; a.ret = return_; a.weight = weight;
+    a.S = S; a.D = (int)D; a.out = out3; a.grad_mu = grad_mu; a.grad_sigma = grad_sigma; a.grad_value = grad_value;
+    a.h.g_expected = g_expected; a.h.g_actual[0] = g_policy; a.h.g_actual[1] = g_value; a.h.g_actual[2] = g_entropy;
+    a.h.g_used = g_used; a.h.g_hint = g_hint; a.h.verify = verify;
+    return launch_k(a2cc_kernel, head_grid(S), HD_NT, 0, (cudaStream_t)stream, a, workspace);
 }
 
 extern "C" int b200rl_ppg_bc_fwd(const float* logit_new, const float* logit_old, const long long* action, long long B,

@@ -934,12 +934,72 @@ class A2CFunction(torch.autograd.Function):
         return gl, gv, None, None, None, None, None, None
 
 
+class A2CContinuousFunction(torch.autograd.Function):
+    """a2c_error_continuous (ding/rl_utils/a2c.py:50-88): three differentiable 0-dim losses; gradients reach mu, sigma and
+    value.  One launch forward (losses + gradients for the expected upstream gradients), one verification launch backward
+    (csrc/heads.cu)."""
+
+    @staticmethod
+    def forward(ctx, mu, sigma, value, action, adv, return_, weight, S, D):
+        dev = mu.device
+        out = torch.empty(4, dtype=torch.float32, device=dev)
+        want = any(ctx.needs_input_grad[:3])
+        gm = torch.empty_like(mu) if want else None
+        gs = torch.empty_like(sigma) if want else None
+        gv = torch.empty_like(value) if want else None
+        g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
+        ctx.hint = head_hint(dev, 'a2cc', [1.0, 0.5, -0.01, 0.0])
+        with on_device(dev):
+            ws = workspace(dev)
+            rc = lib().b200rl_a2c_continuous_fwd_grad(
+                ptr(mu), ptr(sigma), ptr(action), ptr(value), ptr(adv), ptr(return_), ptr(weight), S, D,
+                ptr(ctx.hint) if want else None, 0, None, None, None, ptr(g_used), None, ptr(out), ptr(gm), ptr(gs), ptr(gv),
+                ptr(ws), ws.numel() * 4, stream_ptr())
+        _lib.check(rc, 'b200rl_a2c_continuous_fwd_grad')
+        ctx.save_for_backward(mu, sigma, value, action, adv, return_, weight)
+        ctx.cfg = (S, D)
+        ctx.spec = (gm, gs, gv, g_used)
+        ctx.set_materialize_grads(False)
+        return out[0], out[1], out[2]
+
+    @staticmethod
+    def backward(ctx, g_p, g_v, g_e):
+        mu, sigma, value, action, adv, return_, weight = ctx.saved_tensors
+        S, D = ctx.cfg
+        kp, pp = _g(g_p)
+        kv, pv = _g(g_v)
+        ke, pe = _g(g_e)
+        spec, ctx.spec = ctx.spec, None
+        if spec is not None and spec[0] is not None:
+            gm, gs, gv, g_used = spec
+        else:  # a repeated backward: the first call's buffers may now belong to .grad -> recompute into fresh ones
+            gm, gs, gv = torch.empty_like(mu), torch.empty_like(sigma), torch.empty_like(value)
+            g_used = torch.full((4, ), float('nan'), dtype=torch.float32, device=mu.device)
+        with on_device(mu.device):
+            ws = workspace(mu.device)
+            rc = lib().b200rl_a2c_continuous_fwd_grad(
+                ptr(mu), ptr(sigma), ptr(action), ptr(value), ptr(adv), ptr(return_), ptr(weight), S, D, None, 1, pp, pv,
+                pe, ptr(g_used), ptr(ctx.hint), None, ptr(gm), ptr(gs), ptr(gv), ptr(ws), ws.numel() * 4, stream_ptr())
+        _lib.check(rc, 'b200rl_a2c_continuous_fwd_grad(verify)')
+        return gm, gs, gv, None, None, None, None, None, None
+
+
+# initial expected upstream gradients of each continuous-PPO call site: PPO's default loss weights; the policy-only half
+# (ppo_policy_error_continuous) has no value term
+_PPOC_HINT_INIT = {
+    'ppoc': [1.0, 0.5, -0.01, 0.0],
+    'happoc': [1.0, 0.5, -0.01, 0.0],
+    'ppoc_policy': [1.0, 0.0, -0.01, 0.0],
+}
+
+
 class PPOContinuousFunction(torch.autograd.Function):
-    """ppo_error_continuous (ding/rl_utils/ppo.py:278-374): gradients reach mu_new, sigma_new and value_new (csrc/heads.cu)."""
+    """ppo_error_continuous (ding/rl_utils/ppo.py:278-374): gradients reach mu_new, sigma_new and value_new (csrc/heads.cu).
+    ``hint_kind`` names the call site's expected-upstream-gradient record (a key of ``_PPOC_HINT_INIT``)."""
 
     @staticmethod
     def forward(ctx, mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight, S,
-                D, clip_ratio, use_value_clip, dual_clip, kl_type, factor=None):
+                D, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, factor=None):
         dev = mu.device
         ctx.factor = factor  # happo_error_continuous's per-sample factor (S,) or None; kept alive for the backward launch
         out = torch.empty(8, dtype=torch.float32, device=dev)
@@ -948,7 +1008,7 @@ class PPOContinuousFunction(torch.autograd.Function):
         gs = torch.empty_like(sigma) if want else None
         gv = torch.empty_like(value_new) if want else None
         g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
-        ctx.hint = head_hint(dev, 'ppoc' if factor is None else 'happoc', [1.0, 0.5, -0.01, 0.0])
+        ctx.hint = head_hint(dev, hint_kind, _PPOC_HINT_INIT[hint_kind])
         ctx.args = (ptr(factor), S, D, clip_ratio, use_value_clip, dual_clip, kl_type)
         with on_device(dev):
             ws = workspace(dev)
@@ -984,7 +1044,7 @@ class PPOContinuousFunction(torch.autograd.Function):
                 keep[3][1], ptr(g_used), ptr(ctx.hint), None, ptr(gm), ptr(gs), ptr(gv), ptr(ws), ws.numel() * 4,
                 stream_ptr())
         _lib.check(rc, 'b200rl_ppo_continuous_fwd_grad(verify)')
-        return (gm, gs, gv) + (None, ) * 16
+        return (gm, gs, gv) + (None, ) * 17
 
 
 class ImpalaMaskFunction(torch.autograd.Function):

@@ -1,12 +1,13 @@
 """Mirror of the hot-path part of ``ding.rl_utils`` (ding/rl_utils/__init__.py:1-27): identical names, signatures and
 namedtuples, computed by the sm_90a kernels behind the C ABI of ``include/b200rl.h``."""
-from .a2c import a2c_data, a2c_error, a2c_loss
+from .a2c import a2c_data, a2c_error, a2c_error_continuous, a2c_loss
 from .acer import acer_policy_error, acer_trust_region_update, acer_value_error
 from .fused import gae_ppo_error
 from .happo import (happo_data, happo_error, happo_error_continuous, happo_policy_error_continuous, happo_info, happo_loss, happo_policy_data, happo_policy_error, happo_policy_loss,
                     happo_value_data, happo_value_error)
 from .gae import gae, gae_data, gae_returns, gae_returns_out, shape_fn_gae
-from .ppo import (normalize_advantage, ppo_data, ppo_error, ppo_error_adv_norm, ppo_error_continuous, ppo_info, ppo_loss, ppo_policy_data, ppo_policy_error, ppo_policy_loss,
+from .ppo import (normalize_advantage, ppo_data, ppo_data_continuous, ppo_error, ppo_error_adv_norm, ppo_error_continuous, ppo_info, ppo_loss,
+                  ppo_policy_data, ppo_policy_data_continuous, ppo_policy_error, ppo_policy_error_continuous, ppo_policy_loss,
                   ppo_value_data, ppo_value_error, shape_fn_ppo)
 from .td import (bdq_nstep_td_error, dist_1step_td_data, dist_1step_td_error, dist_nstep_td_data, dist_nstep_td_error,
                  dqfd_nstep_td_data, dqfd_nstep_td_error, dqfd_nstep_td_error_sequence, dqfd_nstep_td_error_with_rescale,
@@ -34,7 +35,8 @@ HOT_PATH_FUNCTIONS = [
     'compute_q_retraces', 'happo_error', 'happo_policy_error', 'happo_value_error', 'happo_error_continuous', 'happo_policy_error_continuous',
     'acer_policy_error', 'acer_value_error', 'acer_trust_region_update', 'ppg_joint_error',
     'dqfd_nstep_td_error', 'dqfd_nstep_td_error_with_rescale',
-    'm_q_1step_td_error', 'q_nstep_sql_td_error', 'q_v_1step_td_error'
+    'm_q_1step_td_error', 'q_nstep_sql_td_error', 'q_v_1step_td_error',
+    'a2c_error_continuous', 'ppo_policy_error_continuous'
 ]
 HOT_PATH_TYPES = [
     'gae_data', 'ppo_data', 'ppo_loss', 'ppo_info', 'q_nstep_td_data', 'dist_nstep_td_data', 'td_lambda_data',
@@ -42,5 +44,5 @@ HOT_PATH_TYPES = [
     'ppo_policy_data', 'ppo_policy_loss', 'ppo_value_data', 'dist_1step_td_data', 'a2c_data', 'a2c_loss',
     'qrdqn_nstep_td_data', 'iqn_nstep_td_data', 'fqf_nstep_td_data',
     'happo_data', 'happo_policy_data', 'happo_value_data', 'happo_loss', 'happo_policy_loss', 'happo_info', 'ppg_data', 'ppg_joint_loss',
-    'dqfd_nstep_td_data', 'm_q_1step_td_data', 'q_v_1step_td_data'
+    'dqfd_nstep_td_data', 'm_q_1step_td_data', 'q_v_1step_td_data', 'ppo_data_continuous', 'ppo_policy_data_continuous'
 ]

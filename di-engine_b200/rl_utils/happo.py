@@ -80,7 +80,7 @@ def happo_error_continuous(
     mu_sigma_new, mu_sigma_old, action, value_new, value_old, adv, return_, weight, factor = data
     loss, info = _ppo_error_continuous(
         ppo_data(mu_sigma_new, mu_sigma_old, action, value_new, value_old, adv, return_, weight, None), clip_ratio,
-        use_value_clip, dual_clip, 'k1', factor=factor
+        use_value_clip, dual_clip, 'k1', 'happoc', factor=factor
     )
     return happo_loss(loss.policy_loss, loss.value_loss, loss.entropy_loss), happo_info(info.approx_kl, info.clipfrac)
 
@@ -96,6 +96,7 @@ def happo_policy_error_continuous(data: namedtuple,
     mu_sigma_new, mu_sigma_old, action, adv, weight = data
     zero = torch.zeros_like(adv)
     loss, info = _ppo_error_continuous(
-        ppo_data(mu_sigma_new, mu_sigma_old, action, zero, zero, adv, zero, weight, None), clip_ratio, False, dual_clip, 'k1'
+        ppo_data(mu_sigma_new, mu_sigma_old, action, zero, zero, adv, zero, weight, None), clip_ratio, False, dual_clip, 'k1',
+        'ppoc'
     )
     return happo_policy_loss(loss.policy_loss, loss.entropy_loss), happo_info(info.approx_kl, info.clipfrac)

@@ -1,6 +1,7 @@
 """``ppo_error`` with the signature and namedtuples of ding/rl_utils/ppo.py:8-27,77-83 -- csrc/ppo.cu; and its two halves as
 the reference exposes them separately (PPG, off-policy PPO, the hybrid-action PPO): ``ppo_policy_error`` (ppo.py:143-230) and
-``ppo_value_error`` (ppo.py:233-275)."""
+``ppo_value_error`` (ppo.py:233-275).  The continuous-action forms ``ppo_error_continuous`` (ppo.py:278-374) and
+``ppo_policy_error_continuous`` (ppo.py:377-450) run on csrc/heads.cu."""
 from collections import namedtuple
 from typing import Optional, Tuple
 
@@ -12,9 +13,18 @@ ppo_data = namedtuple(
     'ppo_data',
     ['logit_new', 'logit_old', 'action', 'value_new', 'value_old', 'adv', 'return_', 'weight', 'logit_pretrained']
 )
+ppo_data_continuous = namedtuple(
+    'ppo_data_continuous', [
+        'mu_sigma_new', 'mu_sigma_old', 'action', 'value_new', 'value_old', 'adv', 'return_', 'weight',
+        'logit_pretrained'
+    ]
+)
 ppo_loss = namedtuple('ppo_loss', ['policy_loss', 'value_loss', 'entropy_loss', 'kl_div'])
 ppo_info = namedtuple('ppo_info', ['approx_kl', 'clipfrac'])
 ppo_policy_data = namedtuple('ppo_policy_data', ['logit_new', 'logit_old', 'action', 'adv', 'weight', 'logit_pretrained'])
+ppo_policy_data_continuous = namedtuple(
+    'ppo_policy_data_continuous', ['mu_sigma_new', 'mu_sigma_old', 'action', 'adv', 'weight', 'logit_pretrained']
+)
 ppo_policy_loss = namedtuple('ppo_policy_loss', ['policy_loss', 'entropy_loss', 'kl_div'])
 ppo_value_data = namedtuple('ppo_value_data', ['value_new', 'value_old', 'return_', 'weight'])
 
@@ -162,10 +172,11 @@ def ppo_error_continuous(
     Returns ``(ppo_loss, ppo_info)``; gradients reach ``mu``, ``sigma`` of the new policy and ``value_new``.  Forward and
     gradients in one launch (csrc/heads.cu), device-verified backward.
     """
-    return _ppo_error_continuous(data, clip_ratio, use_value_clip, dual_clip, kl_type)
+    return _ppo_error_continuous(data, clip_ratio, use_value_clip, dual_clip, kl_type, 'ppoc')
 
 
-def _ppo_error_continuous(data, clip_ratio, use_value_clip, dual_clip, kl_type, factor=None):
+def _ppo_error_continuous(data, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, factor=None):
+    """``hint_kind``: the call site's expected-upstream-gradient record (ops._PPOC_HINT_INIT)"""
     assert dual_clip is None or dual_clip > 1.0, "dual_clip value must be greater than 1.0, but get value: {}".format(
         dual_clip
     )
@@ -199,7 +210,7 @@ def _ppo_error_continuous(data, clip_ratio, use_value_clip, dual_clip, kl_type, 
     fac = stage(factor.detach(), 'factor', S).reshape(-1) if factor is not None else None
     p, v, e, k, out = ops.PPOContinuousFunction.apply(
         *args, S, D, float(clip_ratio), 1 if use_value_clip else 0, float(dual_clip) if dual_clip is not None else 0.0,
-        _KL_TYPES.get(kl_type, 1), fac)
+        _KL_TYPES.get(kl_type, 1), hint_kind, fac)
     if LAZY_INFO:
         info = ppo_info(out[4], out[5])
     else:
@@ -231,6 +242,30 @@ def ppo_policy_error(
     )
     entropy = loss.entropy_loss if entropy_bonus else torch.tensor(0.0)  # ppo.py:203
     return ppo_policy_loss(loss.policy_loss, entropy, loss.kl_div), info
+
+
+def ppo_policy_error_continuous(
+        data: namedtuple,
+        clip_ratio: float = 0.2,
+        dual_clip: Optional[float] = None,
+        kl_type: str = 'k1'
+) -> Tuple[namedtuple, namedtuple]:
+    """
+    Policy half of the continuous-action PPO loss, drop-in for ding/rl_utils/ppo.py:377-450: six fields ``(mu_sigma_new,
+    mu_sigma_old, action, adv, weight, logit_pretrained)`` (``ppo_policy_data_continuous``, or ``ppo_policy_data`` as
+    PPOPGPolicy and PPOOffPolicy pass it), the policies dicts ``{'mu': (B, D), 'sigma': (B, D)}``, action (B, D) float.
+    Returns ``(ppo_policy_loss(policy_loss, entropy_loss, kl_div), ppo_info)``; ``kl_div`` is the python int ``0`` without a
+    pretrained policy, as in the reference.  Runs on the ``ppo_error_continuous`` kernel with a zero value head; its
+    expected-upstream-gradient record is kept apart from ``ppo_error_continuous``'s.
+    """
+    mu_sigma_new, mu_sigma_old, action, adv, weight, logit_pretrained = data
+    zero = torch.zeros_like(adv)
+    loss, info = _ppo_error_continuous(
+        ppo_data(mu_sigma_new, mu_sigma_old, action, zero, zero, adv, zero, weight, logit_pretrained), clip_ratio, False,
+        dual_clip, kl_type, 'ppoc_policy'
+    )
+    kl_div = loss.kl_div if logit_pretrained is not None else 0  # ppo.py:448
+    return ppo_policy_loss(loss.policy_loss, loss.entropy_loss, kl_div), info
 
 
 def ppo_value_error(

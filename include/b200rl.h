@@ -402,6 +402,14 @@ B200RL_API int b200rl_ppo_continuous_fwd_grad(
     int use_value_clip, double dual_clip, int kl_type, const float* g_expected, int verify, const float* g_policy,
     const float* g_value, const float* g_entropy, const float* g_kl, float* g_used, float* g_hint, float* out6, float* grad_mu,
     float* grad_sigma, float* grad_value, float* workspace, size_t workspace_bytes, void* stream);
+/* a2c_error_continuous (ding/rl_utils/a2c.py:50-88): Independent(Normal(mu, sigma)) policy, mu / sigma / action (S, D) float,
+ * value / adv / return_ / weight(nullable) (S); out3 and the backward contract as b200rl_a2c_fwd_grad, gradients reach mu,
+ * sigma and value. */
+B200RL_API int b200rl_a2c_continuous_fwd_grad(const float* mu, const float* sigma, const float* action, const float* value,
+                        const float* adv, const float* return_, const float* weight, long long S, long long D,
+                        const float* g_expected, int verify, const float* g_policy, const float* g_value,
+                        const float* g_entropy, float* g_used, float* g_hint, float* out3, float* grad_mu, float* grad_sigma,
+                        float* grad_value, float* workspace, size_t workspace_bytes, void* stream);
 
 /* ppg_joint_error's behavioural-cloning term (ding/rl_utils/ppg.py:62-67): F.kl_div(logp_new, logp_old, 'batchmean') -- the
  * reference passes the old LOG-probability as the non-log target, so the value is NaN whenever an old log-probability is
