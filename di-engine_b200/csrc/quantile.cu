@@ -47,7 +47,7 @@ __global__ void __launch_bounds__(QT_NT) quantile_td_kernel(QtdArgs a, float* ws
     float* th = sm;            // [ni]
     float* tp = th + a.ni;     // [nj]
     float* ta = tp + a.nj;     // [ni]
-    __shared__ float s_red[QT_NT / 32];
+    __shared__ double s_red[QT_NT / 32];
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     float acc[1] = {0.f};
     const float inv_b = 1.f / (float)a.B;
@@ -68,10 +68,12 @@ __global__ void __launch_bounds__(QT_NT) quantile_td_kernel(QtdArgs a, float* ws
         for (int j = tid; j < a.nj; j += QT_NT)
             tp[j] = fadd(R, fmul(fmul(gb, a.nq[b * a.nq_sb + j * a.nq_sj + na * a.nq_sa]), nd));
         __syncthreads();
-        float lsum = 0.f;
+        // the n' terms of theta_i are summed in fp64: an fp32 chain grows an error like sqrt(n') (n' up to 2048), and the
+        // gradient sum cancels (d huber / d u changes sign across the target quantiles); the terms themselves stay fp32
+        double lsum = 0.0;
         for (int i = tid; i < a.ni; i += QT_NT) {
             const float t = th[i], tq = ta[i];
-            float li = 0.f, gi = 0.f;
+            double li = 0.0, gi = 0.0;
             for (int j = 0; j < a.nj; ++j) {
                 const float u = tp[j] - t;
                 const float au = fabsf(u);
@@ -80,21 +82,22 @@ __global__ void __launch_bounds__(QT_NT) quantile_td_kernel(QtdArgs a, float* ws
                 const float dh = quad ? u : (u > 0.f ? a.kappa : -a.kappa);  // d huber / d u
                 const bool ind = a.strict ? (u < 0.f) : (u <= 0.f);
                 const float w = fabsf(tq - (ind ? 1.f : 0.f));
-                li = fmaf(w, hub, li);
-                gi = fmaf(w, dh, gi);
+                li = fma((double)w, (double)hub, li);
+                gi = fma((double)w, (double)dh, gi);
             }
             lsum += li;
-            const float dti = -gi * a.norm / a.divisor;  // d u / d theta_i = -1
+            const float dti = (float)(-gi * (double)a.norm / (double)a.divisor);  // d u / d theta_i = -1
             a.dtheta[b * a.ni + i] = dti;
             th[i] = dti;  // own slot: the gradient pass below reads it back
         }
-        lsum = warp_sum(lsum);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) lsum += __shfl_xor_sync(0xffffffffu, lsum, o);
         if (lane == 0) s_red[wid] = lsum;
         __syncthreads();
-        float tot = 0.f;
+        double tot = 0.0;
 #pragma unroll
         for (int w = 0; w < QT_NT / 32; ++w) tot += s_red[w];
-        const float lb = tot * a.norm / a.divisor;
+        const float lb = (float)(tot * (double)a.norm / (double)a.divisor);
         const float wb = a.weight ? a.weight[b] : 1.f;
         if (tid == 0) {
             a.td[b] = lb;

@@ -9,7 +9,6 @@
 
 #include "../../include/b200rl.h"
 #include "common.cuh"
-#include "ppo_math.cuh"  // lg2f_ / rcpf_ / kLn2
 
 namespace b200rl {
 
@@ -657,8 +656,8 @@ __global__ void __launch_bounds__(NT) dntd_fwd_kernel(DntdArgs a, float* ws) {
     const int na = a.n_atom;
     float* pj = s_proj + wid * na;
     float acc[1] = {0.f};
-    // a row's work is one serial chain in one warp (~700 instructions): 32-bit index arithmetic, MUFU log / reciprocal where
-    // the reference's bits do not depend on them (the bin positions keep the IEEE division of td.py:500)
+    // a row's work is one serial chain in one warp (~700 instructions): 32-bit index arithmetic; the bin positions keep the
+    // IEEE division of td.py:500
     if (r < a.R) {
         const long long b = r / a.A;
         const int sel = (int)a.act[r], nsel = (int)a.next_act[r];
@@ -744,7 +743,9 @@ __global__ void __launch_bounds__(NT) dntd_fwd_kernel(DntdArgs a, float* ws) {
             if (j < na) {
                 m_[u] = pj[j];
                 bad |= !(d_[u] > 0.f);
-                td = fmaf(lg2f_(d_[u]) * kLn2, m_[u], td);
+                // IEEE logf: the MUFU lg2 flushes a subnormal probability to -inf (NaN against zero mass) and is off by
+                // ~2^-22 near 1, i.e. by percents on the TD error of a near-converged row
+                td = fmaf(logf(d_[u]), m_[u], td);
                 prow[j] = m_[u];
             }
         }
@@ -759,7 +760,7 @@ __global__ void __launch_bounds__(NT) dntd_fwd_kernel(DntdArgs a, float* ws) {
             float* __restrict__ gr = a.grad_unit + r * a.N * na;
             float g_[NJ];
 #pragma unroll
-            for (int u = 0; u < NJ; ++u) g_[u] = c * m_[u] * rcpf_(d_[u]);
+            for (int u = 0; u < NJ; ++u) g_[u] = __fdiv_rn(c * m_[u], d_[u]);  // IEEE division, as dntd_bwd_kernel
             const int Ni = a.N;
             for (int n = 0; n < Ni; ++n) {
 #pragma unroll
