@@ -130,12 +130,73 @@ def const_scalar(value, device):
     return t
 
 
-def _g(grad):
-    """Upstream gradient of a 0-dim loss as a device pointer (None -> the kernel treats it as 0)."""
-    if grad is None:
-        return None, None
-    g = grad if grad.dtype == torch.float32 else grad.float()
-    return g, g.data_ptr()
+def _grads(*grads):
+    """Upstream gradients as contiguous fp32 tensors, to be kept alive across the launch, and their device pointers
+    (None -> the kernel treats that gradient as 0)."""
+    keep = [None if g is None else g.float().contiguous() for g in grads]
+    return keep, [ptr(g) for g in keep]
+
+
+# The forward launch of the wrappers below also writes the gradients for the upstream gradients it expects: the loss
+# weights of the training loop, remembered on the device per call-site kind (a policy-only caller must not disturb its
+# full loss's record) and started from these defaults.  The backward launch verifies them on the device and recomputes on
+# a mismatch -- exact for any upstream gradient, no host sync.
+_HINT_INIT = {
+    'ppo': [1.0, 0.5, -0.01, 0.0],
+    'happo': [1.0, 0.5, -0.01, 0.0],
+    'a2c': [1.0, 0.5, -0.01, 0.0],
+    'a2cc': [1.0, 0.5, -0.01, 0.0],
+    'ppoc': [1.0, 0.5, -0.01, 0.0],
+    'happoc': [1.0, 0.5, -0.01, 0.0],
+    'policy': [1.0, 0.0, -0.01, 0.0],
+    'happo_policy': [1.0, 0.0, -0.01, 0.0],
+    'ppoc_policy': [1.0, 0.0, -0.01, 0.0],
+    'vtrace': [1.0, 0.5, -0.01],
+}
+_HINT = {}
+
+
+def head_hint(device, kind, init):
+    """device-resident expectation of the upstream gradients of a loss head (one record per head kind and device)"""
+    key = (device.index, kind)
+    h = _HINT.get(key)
+    if h is None:
+        h = torch.tensor(init, dtype=torch.float32, device=device)
+        _HINT[key] = h
+    return h
+
+
+def ppo_hint(device, kind='ppo'):
+    """The record of call-site ``kind`` (a key of ``_HINT_INIT``): (d total/d policy_loss, d/d value_loss, d/d entropy_loss
+    [, d/d kl_div])."""
+    return head_hint(device, kind, _HINT_INIT[kind])
+
+
+def vtrace_hint(device):
+    return ppo_hint(device, 'vtrace')
+
+
+def _forward_grads(ctx):
+    """The gradient buffers the forward launch wrote (``ctx.spec``), handed out once.  The first backward takes them, and
+    dropping ctx's reference lets autograd adopt them as .grad without a copy; any later backward gets None and must
+    recompute into fresh buffers, since by then .grad may own the first ones."""
+    spec, ctx.spec = ctx.spec, None
+    return spec
+
+
+def _nan_g_used(n, device):
+    """an expected-gradient slot that matches no upstream gradient: the verify launch recomputes"""
+    return torch.full((n, ), float('nan'), dtype=torch.float32, device=device)
+
+
+def _unit_grad(ctx, other_grads, fresh):
+    """For the backward launches that take ``skip_if_unit`` (TD family, UPGO): (the forward-written gradient for a unit
+    upstream gradient, 1) when it is still there and no gradient arrived through an output other than the loss; else
+    (fresh(), 0), and the launch recomputes."""
+    grad = _forward_grads(ctx)
+    if grad is not None and all(g is None for g in other_grads):
+        return grad, 1
+    return fresh(), 0
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -208,23 +269,9 @@ def normalize_(x, stats):
 # ----------------------------------------------------------------------------------------------------------------
 # ppo
 # ----------------------------------------------------------------------------------------------------------------
-# The forward pass also writes the gradients for the upstream gradients it expects (the loss weights of the training
-# loop, remembered on the device from the previous backward pass); backward() verifies them on the device and only
-# recomputes on a mismatch -- exact for any upstream gradient, no host sync.  False: separate backward kernel always.
+# True: the forward pass also writes the gradients for the expected upstream gradients (``ppo_hint``), verified by the
+# backward pass.  False: separate backward kernel always.
 PPO_FUSED_BACKWARD = True
-_PPO_HINT = {}
-
-
-def ppo_hint(device, kind='ppo'):
-    """Device-resident expectation of (d total/d policy_loss, d/d value_loss, d/d entropy_loss, d/d kl_div), one per call
-    site kind: a policy-only caller (``ppo_policy_error``: no value term) must not disturb ``ppo_error``'s expectation."""
-    key = (device.index, kind)
-    h = _PPO_HINT.get(key)
-    if h is None:
-        init = [1.0, 0.5, -0.01, 0.0] if kind in ('ppo', 'happo') else [1.0, 0.0, -0.01, 0.0]
-        h = torch.tensor(init, dtype=torch.float32, device=device)
-        _PPO_HINT[key] = h
-    return h
 
 
 class PPOFunction(torch.autograd.Function):
@@ -243,7 +290,7 @@ class PPOFunction(torch.autograd.Function):
         tensors = (ptr(logit_new), ptr(logit_old), ptr(logit_pre), ptr(action), ptr(value_new), ptr(value_old),
                    ptr(adv), ptr(return_), ptr(weight))
         cfg = (S, G, N, clip_ratio, use_value_clip, dual_clip, kl_type, ptr(adv_stats), ptr(factor))
-        ctx.fused = False
+        ctx.spec = None
         want_grad = PPO_FUSED_BACKWARD and (ctx.needs_input_grad[0] or ctx.needs_input_grad[1])
         with on_device(dev):
             ws = workspace(dev)
@@ -256,14 +303,12 @@ class PPOFunction(torch.autograd.Function):
                                                ptr(grad_logit), ptr(grad_value), ptr(ws), ws.numel() * 4,
                                                stream_ptr())
                     _lib.check(rc, 'b200rl_ppo_fwd_grad')
-                    ctx.fused = True
                     ctx.spec = (grad_logit, grad_value, g_used)
-            if not ctx.fused:
+            if ctx.spec is None:
                 rc = L.b200rl_ppo_fwd(*tensors, *cfg, ptr(out), ptr(ws), ws.numel() * 4, stream_ptr())
                 _lib.check(rc, 'b200rl_ppo_fwd')
         ctx.save_for_backward(logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre)
         ctx.cfg = cfg
-        ctx.bwd_calls = 0
         ctx.mark_non_differentiable(out)
         p, v, e, k = out[0], out[1], out[2], out[3]
         return p, v, e, k, out
@@ -272,17 +317,12 @@ class PPOFunction(torch.autograd.Function):
     def backward(ctx, g_p, g_v, g_e, g_k, _g_out):
         logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre = ctx.saved_tensors
         dev = logit_new.device
-        kp, pp = _g(g_p)
-        kv, pv = _g(g_v)
-        ke, pe = _g(g_e)
-        kk, pk = _g(g_k)
-        first = ctx.bwd_calls == 0
-        ctx.bwd_calls += 1
-        if ctx.fused and first:
-            grad_logit, grad_value, g_used = ctx.spec  # valid if the expectation held; the kernel checks on the device
-            ctx.spec = None  # sole owner now: autograd can adopt the buffers as .grad instead of cloning them
-            p_used, p_hint = ptr(g_used), ptr(ppo_hint(dev, getattr(ctx, 'hint_kind', 'ppo')))
-        else:  # no fused forward, or a repeated backward (the first call's buffers may now belong to .grad)
+        keep, (pp, pv, pe, pk) = _grads(g_p, g_v, g_e, g_k)
+        spec = _forward_grads(ctx)
+        if spec is not None:  # valid if the expectation held; the kernel checks on the device
+            grad_logit, grad_value, g_used = spec
+            p_used, p_hint = ptr(g_used), ptr(ppo_hint(dev, ctx.hint_kind))
+        else:  # no fused forward, or a repeated backward: null g_used / hint -> the kernel recomputes
             grad_logit = torch.empty_like(logit_new)
             grad_value = torch.empty_like(value_new)
             p_used, p_hint = None, None
@@ -304,6 +344,7 @@ class GAEPPOFunction(torch.autograd.Function):
     def forward(ctx, logit_new, value_new, value, next_value, reward, done, traj_flag, logit_old, action, value_old,
                 return_, weight, logit_pre, T, B, N, gamma, lambda_, clip_ratio, use_value_clip, dual_clip, kl_type):
         dev = logit_new.device
+        ctx.hint_kind = 'ppo'
         out = torch.empty(8, dtype=torch.float32, device=dev)
         adv = torch.empty_like(value)
         want_grad = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
@@ -316,15 +357,13 @@ class GAEPPOFunction(torch.autograd.Function):
                 ptr(value), ptr(next_value), ptr(reward), ptr(done), ptr(traj_flag), T, B, gamma, lambda_, 1,
                 ptr(logit_new), ptr(logit_old), ptr(logit_pre), ptr(action), ptr(value_new), ptr(value_old),
                 ptr(return_), ptr(weight), N, clip_ratio, use_value_clip, dual_clip, kl_type,
-                ptr(ppo_hint(dev)) if want_grad else None, ptr(g_used), ptr(adv), ptr(out), ptr(grad_logit),
-                ptr(grad_value), ptr(ws), ws.numel() * 4, stream_ptr()
+                ptr(ppo_hint(dev, ctx.hint_kind)) if want_grad else None, ptr(g_used), ptr(adv), ptr(out),
+                ptr(grad_logit), ptr(grad_value), ptr(ws), ws.numel() * 4, stream_ptr()
             )
         _lib.check(rc, 'b200rl_gae_ppo_fwd_grad')
         ctx.save_for_backward(logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre)
         ctx.cfg = (T * B, 1, N, clip_ratio, use_value_clip, dual_clip, kl_type, None, None)  # no adv_stats, no factor
-        ctx.fused = want_grad
-        ctx.spec = (grad_logit, grad_value, g_used)
-        ctx.bwd_calls = 0
+        ctx.spec = (grad_logit, grad_value, g_used) if want_grad else None
         ctx.mark_non_differentiable(out, adv)
         return adv, out[0], out[1], out[2], out[3], out
 
@@ -417,17 +456,8 @@ class QNStepTDFunction(torch.autograd.Function):
             return (None, ) * 24
         dcrit, action, weight = ctx.saved_tensors
         S, G, N, group_mean, seq_len = ctx.cfg
-        keep, pg = _g(g_loss)
-        keep_td, ptd = None, None
-        if g_td is not None:
-            keep_td = f32c(g_td)
-            ptd = keep_td.data_ptr()
-        grad_q, skip = ctx.spec, 0
-        ctx.spec = None  # sole owner now: autograd can adopt the buffer as .grad instead of cloning it
-        if grad_q is not None and g_td is None:
-            skip = 1
-        else:
-            grad_q = torch.empty(S * G, N, dtype=torch.float32, device=dcrit.device)
+        keep, (pg, ptd) = _grads(g_loss, g_td)
+        grad_q, skip = _unit_grad(ctx, (g_td, ), lambda: torch.empty(S * G, N, dtype=torch.float32, device=dcrit.device))
         with on_device(dcrit.device):
             rc = lib().b200rl_qntd_bwd(ptr(dcrit), ptr(weight), ptr(action), pg, ptd, S, G, N, group_mean, seq_len, skip,
                                        ptr(grad_q), stream_ptr())
@@ -484,20 +514,12 @@ class DQfDTDFunction(torch.autograd.Function):
             return (None, ) * n_in
         saved, action, weight = ctx.saved_tensors
         S, N, lam_n, lam_1, lam_s, seq_len = ctx.cfg
-        keep = [_g(g) for g in (g_loss, g_sn, g_s1, g_sje)]
-        keep_td, ptd = None, None
-        if g_td is not None:
-            keep_td = f32c(g_td)
-            ptd = keep_td.data_ptr()
-        grad_q, skip = ctx.spec, 0
-        ctx.spec = None  # sole owner now: autograd can adopt the buffer as .grad instead of cloning it
-        if grad_q is not None and g_td is None and g_sn is None and g_s1 is None and g_sje is None:
-            skip = 1
-        else:
-            grad_q = torch.empty(S, N, dtype=torch.float32, device=saved.device)
+        keep, (pg, ptd, psn, ps1, psje) = _grads(g_loss, g_td, g_sn, g_s1, g_sje)
+        grad_q, skip = _unit_grad(ctx, (g_td, g_sn, g_s1, g_sje),
+                                  lambda: torch.empty(S, N, dtype=torch.float32, device=saved.device))
         with on_device(saved.device):
-            rc = lib().b200rl_dqfd_bwd(ptr(saved), ptr(weight), ptr(action), keep[0][1], ptd, keep[1][1], keep[2][1],
-                                       keep[3][1], S, N, lam_n, lam_1, lam_s, seq_len, skip, ptr(grad_q), stream_ptr())
+            rc = lib().b200rl_dqfd_bwd(ptr(saved), ptr(weight), ptr(action), pg, ptd, psn, ps1, psje, S, N, lam_n, lam_1,
+                                       lam_s, seq_len, skip, ptr(grad_q), stream_ptr())
         _lib.check(rc, 'b200rl_dqfd_bwd')
         return (grad_q.view(ctx.q_shape), ) + (None, ) * (n_in - 1)
 
@@ -658,14 +680,11 @@ class QuantileTDFunction(torch.autograd.Function):
             return (None, ) * 21
         dtheta, action, weight = ctx.saved_tensors
         B, N, n_tau, q_strides = ctx.cfg
-        keep, pg = _g(g_loss)
-        keep_td = f32c(g_td) if g_td is not None else None
-        grad_q, skip = ctx.spec, 1
-        ctx.spec = None
-        if grad_q is None or g_td is not None:  # repeated backward / a gradient through the per-sample losses
-            grad_q, skip = torch.empty(ctx.q_shape, dtype=torch.float32, device=dtheta.device), 0
+        keep, (pg, ptd) = _grads(g_loss, g_td)
+        grad_q, skip = _unit_grad(ctx, (g_td, ),
+                                  lambda: torch.empty(ctx.q_shape, dtype=torch.float32, device=dtheta.device))
         with on_device(dtheta.device):
-            rc = lib().b200rl_quantile_td_bwd(ptr(dtheta), ptr(weight), ptr(action), pg, ptr(keep_td), B, N, n_tau,
+            rc = lib().b200rl_quantile_td_bwd(ptr(dtheta), ptr(weight), ptr(action), pg, ptd, B, N, n_tau,
                                               *q_strides, skip, ptr(grad_q), stream_ptr())
         _lib.check(rc, 'b200rl_quantile_td_bwd')
         return (grad_q, ) + (None, ) * 20
@@ -707,15 +726,11 @@ class DistNStepTDFunction(torch.autograd.Function):
             return (None, ) * 20
         dist, act, proj, weight = ctx.saved_tensors
         R, N, n_atom, w_stride = ctx.cfg
-        keep, pg = _g(g_loss)
-        keep_td = f32c(g_td) if g_td is not None else None
-        grad, skip = ctx.spec, 1
-        ctx.spec = None
-        if grad is None or g_td is not None:  # a repeated backward (the first buffer may belong to .grad) / per-sample path
-            grad, skip = torch.empty_like(dist), 0
+        keep, (pg, ptd) = _grads(g_loss, g_td)
+        grad, skip = _unit_grad(ctx, (g_td, ), lambda: torch.empty_like(dist))
         with on_device(dist.device):
             rc = lib().b200rl_dntd_bwd(
-                ptr(dist), ptr(act), ptr(proj), ptr(weight), w_stride, pg, ptr(keep_td), R, N, n_atom, skip, ptr(grad),
+                ptr(dist), ptr(act), ptr(proj), ptr(weight), w_stride, pg, ptd, R, N, n_atom, skip, ptr(grad),
                 stream_ptr()
             )
         _lib.check(rc, 'b200rl_dntd_bwd')
@@ -807,7 +822,7 @@ class _ScaleSaved(torch.autograd.Function):
     def backward(ctx, g):
         saved, = ctx.saved_tensors
         out = torch.empty_like(saved)
-        keep, pg = _g(g)
+        keep, (pg, ) = _grads(g)
         with on_device(saved.device):
             rc = lib().b200rl_scale(pg, ptr(saved), ptr(out), saved.numel(), stream_ptr())
         _lib.check(rc, 'b200rl_scale')
@@ -861,30 +876,14 @@ class UPGOFunction(torch.autograd.Function):
     def backward(ctx, g):
         logit, action, mask, adv = ctx.saved_tensors
         TB, K, N = ctx.cfg
-        grad, skip = ctx.spec, 1
-        ctx.spec = None  # sole owner now: autograd can adopt the buffer as .grad
-        if grad is None:  # a repeated backward: the first buffer may belong to .grad
-            grad, skip = torch.empty_like(logit), 0
-        keep, pg = _g(g)
+        grad, skip = _unit_grad(ctx, (), lambda: torch.empty_like(logit))
+        keep, (pg, ) = _grads(g)
         with on_device(logit.device):
             rc = lib().b200rl_upgo_head_bwd(
                 ptr(logit), ptr(action), ptr(mask), ptr(adv), pg, TB, K, N, skip, ptr(grad), stream_ptr()
             )
         _lib.check(rc, 'b200rl_upgo_head_bwd')
         return (grad, ) + (None, ) * 8
-
-
-_HEAD_HINT = {}
-
-
-def head_hint(device, kind, init):
-    """device-resident expectation of the upstream gradients of a loss head (one record per head kind and device)"""
-    key = (device.index, kind)
-    h = _HEAD_HINT.get(key)
-    if h is None:
-        h = torch.tensor(init, dtype=torch.float32, device=device)
-        _HEAD_HINT[key] = h
-    return h
 
 
 class A2CFunction(torch.autograd.Function):
@@ -899,7 +898,7 @@ class A2CFunction(torch.autograd.Function):
         gl = torch.empty_like(logit) if want else None
         gv = torch.empty_like(value) if want else None
         g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
-        ctx.hint = head_hint(dev, 'a2c', [1.0, 0.5, -0.01, 0.0])
+        ctx.hint = ppo_hint(dev, 'a2c')
         with on_device(dev):
             ws = workspace(dev)
             rc = lib().b200rl_a2c_fwd_grad(ptr(logit), ptr(action), ptr(value), ptr(adv), ptr(return_), ptr(weight), S, N,
@@ -908,7 +907,7 @@ class A2CFunction(torch.autograd.Function):
         _lib.check(rc, 'b200rl_a2c_fwd_grad')
         ctx.save_for_backward(logit, value, action, adv, return_, weight)
         ctx.cfg = (S, N)
-        ctx.spec = (gl, gv, g_used)
+        ctx.spec = (gl, gv, g_used) if want else None
         ctx.set_materialize_grads(False)
         return out[0], out[1], out[2]
 
@@ -916,15 +915,9 @@ class A2CFunction(torch.autograd.Function):
     def backward(ctx, g_p, g_v, g_e):
         logit, value, action, adv, return_, weight = ctx.saved_tensors
         S, N = ctx.cfg
-        kp, pp = _g(g_p)
-        kv, pv = _g(g_v)
-        ke, pe = _g(g_e)
-        spec, ctx.spec = ctx.spec, None
-        if spec is not None and spec[0] is not None:
-            gl, gv, g_used = spec
-        else:  # a repeated backward: the first call's buffers may now belong to .grad -> recompute into fresh ones
-            gl, gv = torch.empty_like(logit), torch.empty_like(value)
-            g_used = torch.full((4, ), float('nan'), dtype=torch.float32, device=logit.device)
+        keep, (pp, pv, pe) = _grads(g_p, g_v, g_e)
+        gl, gv, g_used = _forward_grads(ctx) or (torch.empty_like(logit), torch.empty_like(value),
+                                                 _nan_g_used(4, logit.device))
         with on_device(logit.device):
             ws = workspace(logit.device)
             rc = lib().b200rl_a2c_fwd_grad(ptr(logit), ptr(action), ptr(value), ptr(adv), ptr(return_), ptr(weight), S, N,
@@ -948,7 +941,7 @@ class A2CContinuousFunction(torch.autograd.Function):
         gs = torch.empty_like(sigma) if want else None
         gv = torch.empty_like(value) if want else None
         g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
-        ctx.hint = head_hint(dev, 'a2cc', [1.0, 0.5, -0.01, 0.0])
+        ctx.hint = ppo_hint(dev, 'a2cc')
         with on_device(dev):
             ws = workspace(dev)
             rc = lib().b200rl_a2c_continuous_fwd_grad(
@@ -958,7 +951,7 @@ class A2CContinuousFunction(torch.autograd.Function):
         _lib.check(rc, 'b200rl_a2c_continuous_fwd_grad')
         ctx.save_for_backward(mu, sigma, value, action, adv, return_, weight)
         ctx.cfg = (S, D)
-        ctx.spec = (gm, gs, gv, g_used)
+        ctx.spec = (gm, gs, gv, g_used) if want else None
         ctx.set_materialize_grads(False)
         return out[0], out[1], out[2]
 
@@ -966,15 +959,9 @@ class A2CContinuousFunction(torch.autograd.Function):
     def backward(ctx, g_p, g_v, g_e):
         mu, sigma, value, action, adv, return_, weight = ctx.saved_tensors
         S, D = ctx.cfg
-        kp, pp = _g(g_p)
-        kv, pv = _g(g_v)
-        ke, pe = _g(g_e)
-        spec, ctx.spec = ctx.spec, None
-        if spec is not None and spec[0] is not None:
-            gm, gs, gv, g_used = spec
-        else:  # a repeated backward: the first call's buffers may now belong to .grad -> recompute into fresh ones
-            gm, gs, gv = torch.empty_like(mu), torch.empty_like(sigma), torch.empty_like(value)
-            g_used = torch.full((4, ), float('nan'), dtype=torch.float32, device=mu.device)
+        keep, (pp, pv, pe) = _grads(g_p, g_v, g_e)
+        gm, gs, gv, g_used = _forward_grads(ctx) or (torch.empty_like(mu), torch.empty_like(sigma), torch.empty_like(value),
+                                                     _nan_g_used(4, mu.device))
         with on_device(mu.device):
             ws = workspace(mu.device)
             rc = lib().b200rl_a2c_continuous_fwd_grad(
@@ -984,18 +971,9 @@ class A2CContinuousFunction(torch.autograd.Function):
         return gm, gs, gv, None, None, None, None, None, None
 
 
-# initial expected upstream gradients of each continuous-PPO call site: PPO's default loss weights; the policy-only half
-# (ppo_policy_error_continuous) has no value term
-_PPOC_HINT_INIT = {
-    'ppoc': [1.0, 0.5, -0.01, 0.0],
-    'happoc': [1.0, 0.5, -0.01, 0.0],
-    'ppoc_policy': [1.0, 0.0, -0.01, 0.0],
-}
-
-
 class PPOContinuousFunction(torch.autograd.Function):
     """ppo_error_continuous (ding/rl_utils/ppo.py:278-374): gradients reach mu_new, sigma_new and value_new (csrc/heads.cu).
-    ``hint_kind`` names the call site's expected-upstream-gradient record (a key of ``_PPOC_HINT_INIT``)."""
+    ``hint_kind`` names the call site's expected-upstream-gradient record (a key of ``_HINT_INIT``)."""
 
     @staticmethod
     def forward(ctx, mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight, S,
@@ -1008,7 +986,7 @@ class PPOContinuousFunction(torch.autograd.Function):
         gs = torch.empty_like(sigma) if want else None
         gv = torch.empty_like(value_new) if want else None
         g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
-        ctx.hint = head_hint(dev, hint_kind, _PPOC_HINT_INIT[hint_kind])
+        ctx.hint = ppo_hint(dev, hint_kind)
         ctx.args = (ptr(factor), S, D, clip_ratio, use_value_clip, dual_clip, kl_type)
         with on_device(dev):
             ws = workspace(dev)
@@ -1020,7 +998,7 @@ class PPOContinuousFunction(torch.autograd.Function):
         _lib.check(rc, 'b200rl_ppo_continuous_fwd_grad')
         ctx.save_for_backward(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_,
                               weight)
-        ctx.spec = (gm, gs, gv, g_used)
+        ctx.spec = (gm, gs, gv, g_used) if want else None
         ctx.set_materialize_grads(False)
         ctx.mark_non_differentiable(out)
         return out[0], out[1], out[2], out[3], out
@@ -1029,20 +1007,15 @@ class PPOContinuousFunction(torch.autograd.Function):
     def backward(ctx, g_p, g_v, g_e, g_k, _g_out):
         (mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_,
          weight) = ctx.saved_tensors
-        keep = [_g(x) for x in (g_p, g_v, g_e, g_k)]
-        spec, ctx.spec = ctx.spec, None
-        if spec is not None and spec[0] is not None:
-            gm, gs, gv, g_used = spec
-        else:
-            gm, gs, gv = torch.empty_like(mu), torch.empty_like(sigma), torch.empty_like(value_new)
-            g_used = torch.full((4, ), float('nan'), dtype=torch.float32, device=mu.device)
+        keep, (pp, pv, pe, pk) = _grads(g_p, g_v, g_e, g_k)
+        gm, gs, gv, g_used = _forward_grads(ctx) or (torch.empty_like(mu), torch.empty_like(sigma),
+                                                     torch.empty_like(value_new), _nan_g_used(4, mu.device))
         with on_device(mu.device):
             ws = workspace(mu.device)
             rc = lib().b200rl_ppo_continuous_fwd_grad(
                 ptr(mu), ptr(sigma), ptr(mu_old), ptr(sigma_old), ptr(mu_pre), ptr(sigma_pre), ptr(action), ptr(value_new),
-                ptr(value_old), ptr(adv), ptr(return_), ptr(weight), *ctx.args, None, 1, keep[0][1], keep[1][1], keep[2][1],
-                keep[3][1], ptr(g_used), ptr(ctx.hint), None, ptr(gm), ptr(gs), ptr(gv), ptr(ws), ws.numel() * 4,
-                stream_ptr())
+                ptr(value_old), ptr(adv), ptr(return_), ptr(weight), *ctx.args, None, 1, pp, pv, pe, pk, ptr(g_used),
+                ptr(ctx.hint), None, ptr(gm), ptr(gs), ptr(gv), ptr(ws), ws.numel() * 4, stream_ptr())
         _lib.check(rc, 'b200rl_ppo_continuous_fwd_grad(verify)')
         return (gm, gs, gv) + (None, ) * 17
 
@@ -1080,20 +1053,10 @@ class ImpalaMaskFunction(torch.autograd.Function):
 # ----------------------------------------------------------------------------------------------------------------
 # V-trace
 # ----------------------------------------------------------------------------------------------------------------
-# The one-launch kernel (csrc/vtws.cu) writes the gradients in the forward pass for the upstream gradients it expects (the
-# loss weights of the training loop, remembered on the device from the previous backward pass; IMPALA's defaults to start
-# with); backward() verifies them on the device and only recomputes on a mismatch.  False: rows / scan / backward kernels.
+# True: the one-launch kernel (csrc/vtws.cu) also writes the gradients for the expected upstream gradients
+# (``vtrace_hint``, IMPALA's loss weights to start with), verified by the backward pass.  False: rows / scan / backward
+# kernels.
 VTRACE_FUSED = True
-_VT_HINT = {}
-
-
-def vtrace_hint(device):
-    """Device-resident expectation of (d total/d policy_loss, d/d value_loss, d/d entropy_loss)."""
-    h = _VT_HINT.get(device.index)
-    if h is None:
-        h = torch.tensor([1.0, 0.5, -0.01], dtype=torch.float32, device=device)
-        _VT_HINT[device.index] = h
-    return h
 
 
 class VTraceFunction(torch.autograd.Function):
@@ -1109,8 +1072,7 @@ class VTraceFunction(torch.autograd.Function):
         tensors = (ptr(target_output), ptr(behaviour_output), ptr(action), ptr(value), ptr(reward), ptr(weight))
         want_grad = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         ctx.cfg = (T, B, N)
-        ctx.fused = False
-        ctx.bwd_calls = 0
+        ctx.scal = None  # the scalars of the verify launch: set on the one-launch path only
         with on_device(dev):
             ws = workspace(dev)
             if VTRACE_FUSED:
@@ -1124,8 +1086,7 @@ class VTraceFunction(torch.autograd.Function):
                         ptr(grad_logit), ptr(grad_value), ptr(ws), ws.numel() * 4, stream_ptr()
                     )
                     _lib.check(rc, 'b200rl_vtrace_fwd_grad')
-                    ctx.fused = True
-                    ctx.spec = (grad_logit, grad_value, g_used)
+                    ctx.spec = (grad_logit, grad_value, g_used) if want_grad else None
                     ctx.scal = (gamma, lambda_, rho_clip, c_clip, rho_pg_clip)
                     ctx.save_for_backward(target_output, behaviour_output, action, value, reward, weight)
                     return out[0], out[1], out[2]
@@ -1143,21 +1104,12 @@ class VTraceFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_p, g_v, g_e):
         T, B, N = ctx.cfg
-        kp, pp = _g(g_p)
-        kv, pv = _g(g_v)
-        ke, pe = _g(g_e)
-        if ctx.fused:
+        keep, (pp, pv, pe) = _grads(g_p, g_v, g_e)
+        if ctx.scal is not None:
             target_output, behaviour_output, action, value, reward, weight = ctx.saved_tensors
             dev = target_output.device
-            first = ctx.bwd_calls == 0
-            ctx.bwd_calls += 1
-            if first:
-                grad_logit, grad_value, g_used = ctx.spec  # valid if the expectation held; the kernel checks on the device
-                ctx.spec = None  # sole owner now: autograd can adopt the buffers as .grad instead of cloning them
-            else:  # a repeated backward: the first call's buffers may now belong to .grad -> recompute into fresh ones
-                grad_logit = torch.empty_like(target_output)
-                grad_value = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
-                g_used = torch.full((3, ), float('nan'), dtype=torch.float32, device=dev)
+            grad_logit, grad_value, g_used = _forward_grads(ctx) or (
+                torch.empty_like(target_output), torch.empty(T + 1, B, dtype=torch.float32, device=dev), _nan_g_used(3, dev))
             with on_device(dev):
                 ws = workspace(dev)
                 rc = lib().b200rl_vtrace_fwd_grad(
@@ -1208,12 +1160,11 @@ class VTraceContinuousFunction(torch.autograd.Function):
     def backward(ctx, g_p, g_v, g_e):
         mu, sigma, action, weight, cpg, dv = ctx.saved_tensors
         T, B, D = ctx.cfg
-        keep = [_g(x) for x in (g_p, g_v, g_e)]
+        keep, (pp, pv, pe) = _grads(g_p, g_v, g_e)
         gm, gs = torch.empty_like(mu), torch.empty_like(sigma)
         gv = torch.empty(T + 1, B, dtype=torch.float32, device=mu.device)
         with on_device(mu.device):
-            rc = lib().b200rl_vtrace_continuous_bwd(ptr(mu), ptr(sigma), ptr(action), ptr(weight), ptr(cpg), ptr(dv),
-                                                    keep[0][1], keep[1][1], keep[2][1], T, B, D, ptr(gm), ptr(gs), ptr(gv),
-                                                    stream_ptr())
+            rc = lib().b200rl_vtrace_continuous_bwd(ptr(mu), ptr(sigma), ptr(action), ptr(weight), ptr(cpg), ptr(dv), pp, pv,
+                                                    pe, T, B, D, ptr(gm), ptr(gs), ptr(gv), stream_ptr())
         _lib.check(rc, 'b200rl_vtrace_continuous_bwd')
         return (gm, gs, gv) + (None, ) * 11

@@ -176,7 +176,7 @@ def ppo_error_continuous(
 
 
 def _ppo_error_continuous(data, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, factor=None):
-    """``hint_kind``: the call site's expected-upstream-gradient record (ops._PPOC_HINT_INIT)"""
+    """``hint_kind``: the call site's expected-upstream-gradient record (a key of ops._HINT_INIT)"""
     assert dual_clip is None or dual_clip > 1.0, "dual_clip value must be greater than 1.0, but get value: {}".format(
         dual_clip
     )
