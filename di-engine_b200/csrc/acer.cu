@@ -15,6 +15,10 @@ namespace b200rl {
 
 constexpr float ACER_EPS = 1e-8f;
 
+// torch.clamp keeps NaN; fminf / fmaxf would return the other operand
+__device__ __forceinline__ float clamp_max_nan(float x, float hi) { return x != x ? x : fminf(x, hi); }
+__device__ __forceinline__ float clamp_min_nan(float x, float lo) { return x != x ? x : fmaxf(x, lo); }
+
 __global__ void __launch_bounds__(256) acer_policy_fwd_kernel(const float* __restrict__ q, const float* __restrict__ qret,
                                                               const float* __restrict__ v, const float* __restrict__ logit,
                                                               const long long* __restrict__ act,
@@ -27,10 +31,10 @@ __global__ void __launch_bounds__(256) acer_policy_fwd_kernel(const float* __res
         const float* lg = logit + i * N;
         const float* rt = ratio + i * N;
         const float* qq = q + i * N;
-        actor[i] = fmul(fmul(fminf(rt[a], c), fsub(qret[i], vv)), lg[a]);
+        actor[i] = fmul(fmul(clamp_max_nan(rt[a], c), fsub(qret[i], vv)), lg[a]);
         float s = 0.f;
         for (int j = 0; j < N; ++j) {
-            const float w = fmaxf(fsub(1.0f, __fdiv_rn(c, fadd(rt[j], ACER_EPS))), 0.f);
+            const float w = clamp_min_nan(fsub(1.0f, __fdiv_rn(c, fadd(rt[j], ACER_EPS))), 0.f);
             s = fadd(s, fmul(fmul(fmul(w, expf(lg[j])), fsub(qq[j], vv)), lg[j]));
         }
         bias[i] = s;
@@ -53,11 +57,12 @@ __global__ void __launch_bounds__(256) acer_policy_bwd_kernel(const float* __res
         const float* rt = ratio + i * N;
         const float* qq = q + i * N;
         float* go = grad_logit + i * N;
-        const float ca = ga * (fminf(rt[a], c) * (qret[i] - vv));
+        // a loss with no upstream gradient is not in the graph: it contributes nothing, not 0 * (a non-finite term)
+        const float ca = g_actor ? ga * (clamp_max_nan(rt[a], c) * (qret[i] - vv)) : 0.f;
         for (int j = 0; j < N; ++j) {
-            const float w = fmaxf(1.0f - c / (rt[j] + ACER_EPS), 0.f);
-            float g = gb * (w * expf(lg[j]) * (qq[j] - vv));
-            if (j == a) g += ca;
+            const float w = clamp_min_nan(1.0f - c / (rt[j] + ACER_EPS), 0.f);
+            float g = g_bias ? gb * (w * expf(lg[j]) * (qq[j] - vv)) : 0.f;
+            if (j == a && g_actor) g += ca;
             go[j] = g;
         }
     }
@@ -98,7 +103,7 @@ __global__ void __launch_bounds__(256) acer_trust_region_kernel(const float* __r
             gk = fadd(gk, fmul(g[j], k));
             kk = fadd(kk, fmul(k, k));
         }
-        const float scale = fmaxf(__fdiv_rn(fsub(gk, delta), kk), 0.f);
+        const float scale = clamp_min_nan(__fdiv_rn(fsub(gk, delta), kk), 0.f);
         for (int j = 0; j < N; ++j) out[i * N + j] = fsub(g[j], fmul(scale, expf(al[j])));
     }
 }

@@ -46,6 +46,19 @@ struct UpgoArgs {
     int skip_if_unit;   // backward: grad_logit already holds the unit gradient -> return when *g_loss == 1
 };
 
+// log softmax in torch's order, (z - max) - log(sum exp(z - max)): z - (max + log sum) loses |max| * 2^-24 on logits
+// shifted far from 0 (a row shifted by 50 carried 4e-6 of error into every log-probability and probability)
+template <int L, class Ld>
+__device__ __forceinline__ void row_max_logsum(Ld ld, int n, int lane, float& m, float& ls) {
+    m = -INFINITY;
+    for (int j = lane; j < n; j += L) m = fmaxf(m, ld(j));
+    if (L == 32) m = warp_max(m);
+    float s = 0.f;
+    for (int j = lane; j < n; j += L) s += expf(ld(j) - m);
+    if (L == 32) s = warp_sum(s);
+    ls = logf(s);
+}
+
 template <int NT, int L>
 __global__ void __launch_bounds__(NT) upgo_fwd_kernel(UpgoArgs a, float* ws) {
     pdl_prologue();
@@ -62,9 +75,10 @@ __global__ void __launch_bounds__(NT) upgo_fwd_kernel(UpgoArgs a, float* ws) {
         for (int k = 0; k < a.K; ++k) {
             const long long row = s * a.K + k;
             const float* z = a.logit + row * a.N;
-            const float lse = row_lse<L>([&](int j) { return z[j]; }, a.N, lane);
+            float m, ls;
+            row_max_logsum<L>([&](int j) { return z[j]; }, a.N, lane, m, ls);
             const int act = (int)a.action[row];
-            float lp = z[act] - lse;
+            float lp = (z[act] - m) - ls;
             const float mk = a.mask ? a.mask[row] : 1.f;
             lp *= mk;
             metric += lp;
@@ -72,7 +86,7 @@ __global__ void __launch_bounds__(NT) upgo_fwd_kernel(UpgoArgs a, float* ws) {
                 const float c = -adv * mk / (float)a.TB;  // d loss / d logp(row)
                 float* gz = a.grad_unit + row * a.N;
                 for (int j = lane; j < a.N; j += L) {
-                    float gj = -c * expf(z[j] - lse);
+                    float gj = -c * expf((z[j] - m) - ls);
                     if (j == act) gj += c;
                     gz[j] = gj;
                 }
@@ -101,12 +115,13 @@ __global__ void __launch_bounds__(NT) upgo_bwd_kernel(UpgoArgs a) {
         const long long s = row / a.K;
         const float* z = a.logit + row * a.N;
         float* gz = a.grad_logit + row * a.N;
-        const float lse = row_lse<L>([&](int j) { return z[j]; }, a.N, lane);
+        float m, ls;
+        row_max_logsum<L>([&](int j) { return z[j]; }, a.N, lane, m, ls);
         float c = -g * a.adv_saved[s] / (float)a.TB;  // d loss / d logp(row)
         if (a.mask) c *= a.mask[row];
         const int act = (int)a.action[row];
         for (int j = lane; j < a.N; j += L) {
-            float gj = -c * expf(z[j] - lse);
+            float gj = -c * expf((z[j] - m) - ls);
             if (j == act) gj += c;
             gz[j] = gj;
         }
@@ -128,8 +143,9 @@ __global__ void __launch_bounds__(NT) tbce_fwd_kernel(const float* __restrict__ 
     for (int k = 0; k < K; ++k) {
         const long long row = s * K + k;
         const float* z = logit + row * N;
-        const float lse = row_lse<L>([&](int j) { return z[j]; }, N, lane);
-        float lp = z[action[row]] - lse;
+        float m, ls;
+        row_max_logsum<L>([&](int j) { return z[j]; }, N, lane, m, ls);
+        float lp = (z[action[row]] - m) - ls;
         if (mask) lp *= mask[row];
         metric += lp;
     }
@@ -147,12 +163,13 @@ __global__ void __launch_bounds__(NT) tbce_bwd_kernel(const float* __restrict__ 
     if (row >= TB * K) return;
     const float* z = logit + row * N;
     float* gz = grad_logit + row * N;
-    const float lse = row_lse<L>([&](int j) { return z[j]; }, N, lane);
+    float m, ls;
+    row_max_logsum<L>([&](int j) { return z[j]; }, N, lane, m, ls);
     float c = g_ce[row / K];
     if (mask) c *= mask[row];
     const int act = (int)action[row];
     for (int j = lane; j < N; j += L) {
-        float gj = -c * expf(z[j] - lse);
+        float gj = -c * expf((z[j] - m) - ls);
         if (j == act) gj += c;
         gz[j] = gj;
     }
@@ -270,12 +287,13 @@ __global__ void __launch_bounds__(NT) vtrace_scan_kernel(VtArgs a, float* ws) {
             if (c < B) {
                 const long long off = (lo + r) * B + c;
                 const float is = ldg_stream(a.isw + off);
+                const bool nan = is != is;  // torch.clamp keeps NaN, fminf would return the clip
                 const float v = a.value[off], vn = a.value[off + B];
                 const float rw = ldg_stream(a.reward + off);
-                s_d[r][cc] = fmul(fminf(is, a.rho_clip), fsub(fadd(rw, fmul(a.gamma, vn)), v));
-                s_f[r][cc] = fmul(a.gamma_lambda, fminf(is, a.c_clip));
+                s_d[r][cc] = fmul(nan ? is : fminf(is, a.rho_clip), fsub(fadd(rw, fmul(a.gamma, vn)), v));
+                s_f[r][cc] = fmul(a.gamma_lambda, nan ? is : fminf(is, a.c_clip));
                 s_v[r][cc] = v;
-                s_g[r][cc] = fminf(is, a.rho_pg_clip);
+                s_g[r][cc] = nan ? is : fminf(is, a.rho_pg_clip);
                 s_r[r][cc] = rw;
                 s_w[r][cc] = a.weight ? ldg_stream(a.weight + off) : 1.f;
                 s_l[r][cc] = ldg_stream(a.lp_t + off);

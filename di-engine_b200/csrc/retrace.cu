@@ -47,7 +47,8 @@ __global__ void __launch_bounds__(RT_NT) retrace_kernel(const float* __restrict_
                 s_r[j][c] = reward[e];
                 s_gw[j][c] = fmul(gamma, weight[e]);
                 s_v[j][c] = v[e];
-                s_c[j][c] = fminf(ratio[e * N + a], 1.0f);
+                const float ra = ratio[e * N + a];
+                s_c[j][c] = ra != ra ? ra : fminf(ra, 1.0f);  // clamp(max=1) keeps NaN
                 s_qa[j][c] = q[e * N + a];
             }
         }
