@@ -1,11 +1,18 @@
 // n-step TD heads of ding/rl_utils/td.py:
-//   q_nstep_td_error (:649-719) / q_nstep_td_error_with_rescale (:810-867)  -> qntd_fwd / qntd_bwd
+//   q_nstep_td_error (:649-719) / q_nstep_td_error_with_rescale (:810-867), bdq_nstep_td_error and
+//   R2D2's sequence loss (ding/policy/r2d2.py)                               -> qntd_fwd / qntd_bwd
+//   dqfd_nstep_td_error (:870-983, with rescale :986-1090) and R2D3's sequence loop -> dqfd_fwd / dqfd_bwd
+//   m_q_1step_td_error, q_nstep_sql_td_error, q_v_1step_td_error             -> soft_td_fwd / qntd_bwd
 //   dist_nstep_td_error (C51 projection, :413-523)                           -> dntd_fwd / dntd_bwd
 //   generalized_lambda_returns / multistep_forward_view (:1574-1651), td_lambda_error (:1539-1571) and the
 //   UPGO return (upgo.py:46-68)                                              -> lambda_returns (+ fused TD(lambda) head)
 // Each reference call is ~20-35 tiny torch launches plus an autograd backward; here it is one forward and one
 // backward launch.  These batches are small (B ~ 32..512): latency, not bandwidth, is what the kernels minimise.
+// qntd, dqfd and soft_td run one thread per row and share the n-step return, the loss reduction, the one-hot gradient
+// store and the host launch plan below; only their targets differ.
 #include <math.h>
+
+#include <type_traits>
 
 #include "../../include/b200rl.h"
 #include "common.cuh"
@@ -40,9 +47,16 @@ __device__ __forceinline__ float criterion_eval(int kind, float param, float x, 
     }
 }
 
-// sum_i reward[i] * gamma^i over the nstep rewards of one sample (td.py:261-265 / :277-281): the first 8 are staged in rwv
-// by the caller, the rest are read at rw[i * Bi]; rf returns gamma^nstep as the loop builds it (reward_factor[nstep]).
-// qntd_fwd_kernel keeps its own inline copy of this loop: through the helper its trip-count code compiles differently.
+// The first min(n, 8) rewards of one sample, rw[i * Bi], into registers.  Callers issue this together with their other
+// per-sample loads, before any of them is used: a load inside the n-step loop is one L2 round trip per step.
+__device__ __forceinline__ void nstep_reward_load(float (&rwv)[8], const float* __restrict__ rw, size_t Bi, int n) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) rwv[i] = i < n ? rw[i * Bi] : 0.f;
+}
+
+// sum_i reward[i] * gamma^i over the nstep rewards of one sample (td.py:261-265 / :277-281, matmul(reward_factor, reward)
+// :453-456): the first 8 come from nstep_reward_load, the rest are read at rw[i * Bi]; rf returns gamma^nstep as the loop
+// builds it (reward_factor[nstep]).
 __device__ __forceinline__ float nstep_reward_sum(const float (&rwv)[8], const float* __restrict__ rw, size_t Bi, int nstep,
                                                   float g, float& rf) {
     float ret = 0.f;
@@ -61,7 +75,51 @@ __device__ __forceinline__ float nstep_reward_sum(const float (&rwv)[8], const f
     return ret;
 }
 
-struct QntdArgs {
+// Loss reduction of the one-thread-per-row TD kernels and C51: fin(k, total) receives the grid total of acc[k].  The
+// one-round-trip grid_sum_fx when no last CTA is needed and the grid has at most FX_MAX_GRID CTAs; otherwise the ticket
+// grid_sum, and the return value says whether this is the last CTA, which then sees every row's stores.  The host
+// launches the NT > 128 builds only on such grids and never with need_last, so they compile only grid_sum_fx.
+template <int K, int NT, class Fin>
+__device__ __forceinline__ bool td_loss_sum(float (&acc)[K], float* ws, bool need_last, Fin fin) {
+    if (NT > 128 || (!need_last && gridDim.x <= FX_MAX_GRID)) {
+        grid_sum_fx<K, NT>(acc, ws, fin);
+        return false;
+    }
+    double tot[K];
+    const bool last = grid_sum<K, NT>(acc, tot, ws, 0);
+    if (last && threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) fin(k, tot[k]);
+    }
+    return last;
+}
+
+// The CTA's gradient rows [r0, r0 + NT) of g (R rows of N): row r0 + t, staged by thread t, is coef0[t] at idx0[t] (plus
+// coef1[t] at idx1[t] when given) and zero elsewhere.  The rows are contiguous, so the CTA stores them together, coalesced.
+template <int NT>
+__device__ __forceinline__ void store_onehot_rows(float* __restrict__ g, long long r0, long long R, int N, const float* coef0,
+                                                  const int* idx0, const float* coef1 = nullptr, const int* idx1 = nullptr) {
+    __syncthreads();
+    const long long rows = (R - r0) < NT ? (R - r0) : NT;
+    float* gq = g + r0 * N;
+    for (long long i = threadIdx.x; i < rows * N; i += NT) {
+        const int rr = (int)(i / N), j = (int)(i - (long long)rr * N);
+        float v = (j == idx0[rr]) ? coef0[rr] : 0.f;
+        if (coef1) v += (j == idx1[rr]) ? coef1[rr] : 0.f;
+        gq[i] = v;
+    }
+}
+
+// The scalars that qntd, dqfd and soft_td derive alike on the host (td_scalars below).
+struct TdScalars {
+    float gamma, gamma_pow_n;
+    float eps, four_eps, two_eps;  // value rescaling (qntd, dqfd)
+    double loss_div;               // loss = sum(w*td) / loss_div
+    // sequence form (qntd, dqfd): priority[b] = max_w*max_t e + mean_w*sum_t e / prio_div over the per-step errors e
+    float prio_max_w, prio_mean_w, prio_div;
+};
+
+struct QntdArgs : TdScalars {
     const float* q;            // (S, G, N)
     const float* next_q;       // (S, G, N)
     const long long* action;   // (S, G)
@@ -77,16 +135,11 @@ struct QntdArgs {
     int G;                     // rows per sample: 1, the agent dim of the multi-agent form or the BDQ branches
     int N;
     int nstep;
-    float gamma;
-    float gamma_pow_n;
     int cum_reward;
     int rescale;
-    float eps, four_eps, two_eps;
     int criterion;
     float crit_param;
     int group_mean;    // td_error_per_sample (S) = mean over the G rows (bdq_nstep_td_error, td.py:788) instead of (S, G)
-    double loss_div;   // loss = sum(w*td) / loss_div
-    float prio_max_w, prio_mean_w, prio_div;  // sequence form: priority[b] = max_w*max_t|td| + mean_w*sum_t|td|/prio_div
     float* loss;
     float* td_err;
     float* dcrit;      // (S, G) d criterion / d q_sa (unweighted): what the backward launch needs
@@ -110,18 +163,16 @@ __global__ void __launch_bounds__(NT) qntd_fwd_kernel(QntdArgs a, float* ws) {
     s_act[threadIdx.x] = -1;
     if (s < a.S) {
         const long long tq_ = s / a.Bcol, b = s - tq_ * a.Bcol;  // sequence step / batch column (tq_ = 0 when Bcol == S)
-        // every per-sample operand is requested before any is used: a load inside the n-step loop is one L2 round trip per step
+        // every per-sample operand is requested before any is used, the action indices first: q[action] waits on them
+        const int act0 = (int)a.action[s * a.G], nact0 = (int)a.next_action[s * a.G];
         const float* __restrict__ rw = a.cum_reward ? a.reward + s : a.reward + tq_ * a.nstep * a.Bcol + b;
         const size_t Bi = (size_t)a.Bcol;
-        const int nrw = a.cum_reward ? 1 : a.nstep;
         float rwv[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) rwv[i] = i < nrw ? rw[i * Bi] : 0.f;
+        nstep_reward_load(rwv, rw, Bi, a.cum_reward ? 1 : a.nstep);
         const float dn = a.done[s];
         const float w = a.weight ? a.weight[s] : 1.f;
         const float vgl = a.value_gamma ? a.value_gamma[s * a.value_gamma_stride] : a.gamma_pow_n;
         const float g = a.gamma_ps ? a.gamma_ps[b] : a.gamma;
-        const int act0 = (int)a.action[s * a.G], nact0 = (int)a.next_action[s * a.G];
         const float q0 = a.q[s * a.G * a.N + act0], nq0 = a.next_q[s * a.G * a.N + nact0];
         const float nd = fsub(1.f, dn);
         float ret = 0.f, vg;
@@ -129,18 +180,8 @@ __global__ void __launch_bounds__(NT) qntd_fwd_kernel(QntdArgs a, float* ws) {
             ret = rwv[0];
             vg = vgl;
         } else {
-            float rf = 1.f;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {  // td.py:261-264 / :277-281
-                if (i < a.nstep) {
-                    ret = fadd(ret, fmul(rwv[i], rf));
-                    rf = fmul(g, rf);
-                }
-            }
-            for (int i = 8; i < a.nstep; ++i) {
-                ret = fadd(ret, fmul(rw[i * Bi], rf));
-                rf = fmul(g, rf);
-            }
+            float rf;
+            ret = nstep_reward_sum(rwv, rw, Bi, a.nstep, g, rf);
             vg = a.gamma_ps ? rf : vgl;  // reward_factor[nstep] for the NGU list-gamma form
         }
         float td_sum = 0.f;
@@ -172,22 +213,8 @@ __global__ void __launch_bounds__(NT) qntd_fwd_kernel(QntdArgs a, float* ws) {
         }
         if (a.group_mean) a.td_err[s] = td_sum / (float)a.G;
     }
-    if (a.grad_unit && a.G == 1) {  // the block's NT gradient rows are contiguous: coalesced stores
-        __syncthreads();
-        const long long rows = (a.S - s0) < NT ? (a.S - s0) : NT;
-        float* gq = a.grad_unit + s0 * a.N;
-        for (long long i = threadIdx.x; i < rows * a.N; i += NT) {
-            const int rr = (int)(i / a.N), j = (int)(i - (long long)rr * a.N);
-            gq[i] = (j == s_act[rr]) ? s_coef[rr] : 0.f;
-        }
-    }
-    if (!a.priority && gridDim.x <= FX_MAX_GRID) {  // one atomic round trip (none for a one-CTA grid)
-        grid_sum_fx<1, NT>(acc, ws, [&](int, double t) { a.loss[0] = (float)(t / a.loss_div); });
-        return;
-    }
-    double tot[1];
-    const bool last = grid_sum<1, NT>(acc, tot, ws, 0);
-    if (last && threadIdx.x == 0) a.loss[0] = (float)(tot[0] / a.loss_div);
+    if (a.grad_unit && a.G == 1) store_onehot_rows<NT>(a.grad_unit, s0, a.S, a.N, s_coef, s_act);
+    const bool last = td_loss_sum<1, NT>(acc, ws, a.priority, [&](int, double t) { a.loss[0] = (float)(t / a.loss_div); });
     if (last && a.priority) {
         // sequence form (ding/policy/r2d2.py:367-369): the last CTA sees every per-step error (published before the tickets)
         const long long Tq = a.S / a.Bcol;
@@ -233,7 +260,7 @@ __global__ void qntd_bwd_kernel(const float* __restrict__ dcrit, const float* __
 //   td_n = crit(q_sa, nstep target), td_1 = crit(q_sa, 1-step target), JE = is_expert * (max_j(q_j + m*[j != a]) - q_sa)
 //   loss = mean(w * (ln*td_n + l1*td_1 + ls*JE)),  per-sample = ln*|td_n| + l1*|td_1| + ls*|JE|,  stats = means of the three
 // ---------------------------------------------------------------------------------------------------------------
-struct DqfdArgs {
+struct DqfdArgs : TdScalars {
     const float* q;           // (S, N)
     const float* next_q;      // (S, N)
     const float* next_q1;     // (S, N) new_n_q_one_step
@@ -251,18 +278,14 @@ struct DqfdArgs {
     long long Bcol;           // == S, or the batch width of the sequence form (sample s = t*Bcol + b)
     int N;
     int nstep;
-    float gamma, gamma_pow_n;
     int cum_reward;
     int rescale;
-    float eps, four_eps, two_eps;
     int criterion;            // criterion_eval kind, or -1: no TD terms (the caller applies its own criterion to target_n/1)
     float crit_param;
     float lam_n, lam_1, lam_s, margin;
-    double loss_div;          // loss and statistics = sum / loss_div
-    float prio_max_w, prio_mean_w, prio_div;  // sequence form: priority[b] = max_w*max_t e + mean_w*sum_t e / prio_div
     float* loss;
     float* td_err;            // (S)
-    float* stats;             // (3): td_n, td_1, JE
+    float* stats;             // (3): td_n, td_1, JE, each sum / loss_div
     float4* saved;            // (S): d crit_n, d crit_1, is_expert, argmax | sign codes << 24 -- what the backward launch needs
     float* target_n;          // nullable (S): the detached targets, for callers that apply their own criterion
     float* target_1;
@@ -285,20 +308,18 @@ __global__ void __launch_bounds__(NT) dqfd_fwd_kernel(DqfdArgs a, float* ws) {
     s_act[threadIdx.x] = s_k[threadIdx.x] = -1;
     if (s < a.S) {
         const long long tq_ = s / a.Bcol, b = s - tq_ * a.Bcol;
-        // every per-sample operand is requested before any is used
+        // every per-sample operand is requested before any is used, the action indices first: q[action] waits on them
+        const int act = (int)a.action[s], nact = (int)a.next_action[s], nact1 = (int)a.next_action1[s];
         const float* __restrict__ rw = a.cum_reward ? a.reward + s : a.reward + tq_ * a.nstep * a.Bcol + b;
         const size_t Bi = (size_t)a.Bcol;
-        const int nrw = a.cum_reward ? 1 : a.nstep;
         float rwv[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) rwv[i] = i < nrw ? rw[i * Bi] : 0.f;
+        nstep_reward_load(rwv, rw, Bi, a.cum_reward ? 1 : a.nstep);
         // cum_reward: reward[0].unsqueeze(0) is sample 0's reward, broadcast to every sample (td.py:954, :958)
         const float r1c = a.cum_reward ? a.reward[0] : 0.f;
         const float dn = a.done[s], dn1 = a.done1[s];
         const float w = a.weight ? a.weight[s] : 1.f;
         const float vgl = a.value_gamma ? a.value_gamma[s * a.value_gamma_stride] : a.gamma_pow_n;
         const float ie = a.is_expert[s];
-        const int act = (int)a.action[s], nact = (int)a.next_action[s], nact1 = (int)a.next_action1[s];
         const float* __restrict__ qr = a.q + s * a.N;
         const float q_sa = qr[act], nq = a.next_q[s * a.N + nact], nq1 = a.next_q1[s * a.N + nact1];
         // supervised margin term: max_j(q_j + l_j), l = margin except 0 at the action (td.py:969-972); the gradient of the max
@@ -365,28 +386,12 @@ __global__ void __launch_bounds__(NT) dqfd_fwd_kernel(DqfdArgs a, float* ws) {
             s_k[threadIdx.x] = k;
         }
     }
-    if (a.grad_unit) {  // the block's NT gradient rows are contiguous: coalesced stores
-        __syncthreads();
-        const long long rows = (a.S - s0) < NT ? (a.S - s0) : NT;
-        float* gq = a.grad_unit + s0 * a.N;
-        for (long long i = threadIdx.x; i < rows * a.N; i += NT) {
-            const int rr = (int)(i / a.N), j = (int)(i - (long long)rr * a.N);
-            gq[i] = (j == s_act[rr] ? s_ca[rr] : 0.f) + (j == s_k[rr] ? s_ck[rr] : 0.f);
-        }
-    }
-    auto fin = [&](int kk, double t) {
+    if (a.grad_unit) store_onehot_rows<NT>(a.grad_unit, s0, a.S, a.N, s_ca, s_act, s_ck, s_k);
+    const bool last = td_loss_sum<4, NT>(acc, ws, a.priority, [&](int kk, double t) {
         const float v = (float)(t / a.loss_div);
         if (kk == 0) a.loss[0] = v;
         else a.stats[kk - 1] = v;
-    };
-    if (!a.priority && gridDim.x <= FX_MAX_GRID) {
-        grid_sum_fx<4, NT>(acc, ws, fin);
-        return;
-    }
-    double tot[4];
-    const bool last = grid_sum<4, NT>(acc, tot, ws, 0);
-    if (last && threadIdx.x == 0)
-        for (int kk = 0; kk < 4; ++kk) fin(kk, tot[kk]);
+    });
     if (last && a.priority) {
         // sequence form (r2d3.py:386-388): the per-sample errors are already sums of absolute values, no abs here
         const long long Tq = a.S / a.Bcol;
@@ -447,7 +452,7 @@ __global__ void dqfd_bwd_kernel(const float4* __restrict__ saved, const float* _
 // Gathering q_sa, the criterion, the loss sum and the record qntd_bwd_kernel reads (dcrit, and the unit gradient) are those of
 // qntd_fwd_kernel; every target is detached, so the gradient reaches q through q_sa alone.
 // ---------------------------------------------------------------------------------------------------------------
-struct SoftTdArgs {
+struct SoftTdArgs : TdScalars {
     const float* q;           // (R, N)
     const float* target_q;    // MODE 0: (R, N), the target network on the current observation
     const float* next_q;      // MODE 0 / 1: (R, N); MODE 2: the state value v (R)
@@ -461,18 +466,16 @@ struct SoftTdArgs {
     int G;                    // rows per sample (S = R / G): reward and done of row r are sample r / G's
     int N;
     int nstep;
-    float gamma, gamma_pow_n;
     float tau, alpha;
     int cum_reward;
     int criterion;
     float crit_param;
-    double loss_div;          // loss = sum(w*td) / loss_div, action_gap = sum(top1 - top2) / loss_div
     float* loss;
     float* td_err;            // (R)
     float* dcrit;             // (R) d criterion / d q_sa: what qntd_bwd_kernel reads (G = 1 there)
     float* target;            // nullable (R): the detached target, for callers that apply their own criterion
     float* grad_unit;         // nullable (R, N): d loss / d q for a unit upstream gradient
-    float* action_gap;        // MODE 0
+    float* action_gap;        // MODE 0: sum(top1 - top2) / loss_div
     float* clipfrac;          // MODE 0 (R): 1 where log pi(a) was clamped
     float* record_v;          // MODE 1, nullable (R): V' before the return is formed
 };
@@ -552,10 +555,8 @@ __global__ void __launch_bounds__(NT) soft_td_fwd_kernel(SoftTdArgs a, float* ws
             const float* __restrict__ nq = a.next_q + r * N;
             const float* __restrict__ rw = a.reward + r;
             const size_t Bi = (size_t)a.R;
-            const int nrw = a.cum_reward ? 1 : a.nstep;
             float rwv[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) rwv[i] = i < nrw ? rw[i * Bi] : 0.f;
+            nstep_reward_load(rwv, rw, Bi, a.cum_reward ? 1 : a.nstep);
             const float vg = a.value_gamma ? a.value_gamma[r * a.value_gamma_stride] : a.gamma_pow_n;
             float ret;
             if (a.cum_reward) {
@@ -585,30 +586,12 @@ __global__ void __launch_bounds__(NT) soft_td_fwd_kernel(SoftTdArgs a, float* ws
             s_act[threadIdx.x] = act;
         }
     }
-    if (a.grad_unit) {  // the block's NT gradient rows are contiguous: coalesced stores
-        __syncthreads();
-        const long long rows = (a.R - r0) < NT ? (a.R - r0) : NT;
-        float* gq = a.grad_unit + r0 * a.N;
-        for (long long i = threadIdx.x; i < rows * a.N; i += NT) {
-            const int rr = (int)(i / a.N), j = (int)(i - (long long)rr * a.N);
-            gq[i] = (j == s_act[rr]) ? s_coef[rr] : 0.f;
-        }
-    }
-    auto fin = [&](int k, double t) {
+    if (a.grad_unit) store_onehot_rows<NT>(a.grad_unit, r0, a.R, a.N, s_coef, s_act);
+    td_loss_sum<K, NT>(acc, ws, false, [&](int k, double t) {
         const float v = (float)(t / a.loss_div);
         if (k == 0) a.loss[0] = v;
         else a.action_gap[0] = v;
-    };
-    // one atomic round trip (none for a one-CTA grid); the 256 / 512 / 1024-thread builds only ever run as one CTA
-    if (NT > 128 || gridDim.x <= FX_MAX_GRID) {
-        grid_sum_fx<K, NT>(acc, ws, fin);
-        return;
-    }
-    double tot[K];
-    if (grid_sum<K, NT>(acc, tot, ws, 0) && threadIdx.x == 0) {
-#pragma unroll
-        for (int k = 0; k < K; ++k) fin(k, tot[k]);
-    }
+    });
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -673,28 +656,16 @@ __global__ void __launch_bounds__(NT) dntd_fwd_kernel(DntdArgs a, float* ws) {
             z_[u] = ok ? a.support[j] : 0.f;
             if (ok) pj[j] = 0.f;
         }
-        // every per-sample scalar is requested before any is used (a load inside the n-step loop costs one L2 round trip per
-        // step, serialised)
+        // every per-sample scalar is requested before any is used
         const float* __restrict__ rw = a.reward + b;
         const size_t Bi = (size_t)a.B;
         float rwv[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) rwv[i] = i < a.nstep ? rw[i * Bi] : 0.f;
+        nstep_reward_load(rwv, rw, Bi, a.nstep);
         const float dn = a.done[b];
         const float vg = a.value_gamma ? a.value_gamma[b * a.value_gamma_stride] : a.gamma_pow_n;
         const float w = a.weight ? a.weight[r * a.weight_stride] : 1.f;
-        float rf = 1.f, ret = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {  // matmul(reward_factor, reward), td.py:453-456
-            if (i < a.nstep) {
-                ret = fadd(ret, fmul(rf, rwv[i]));
-                rf = fmul(a.gamma, rf);
-            }
-        }
-        for (int i = 8; i < a.nstep; ++i) {
-            ret = fadd(ret, fmul(rf, rw[i * Bi]));
-            rf = fmul(a.gamma, rf);
-        }
+        float rf;
+        const float ret = nstep_reward_sum(rwv, rw, Bi, a.nstep, a.gamma, rf);
         const float scale = fmul(fsub(1.f, dn), vg);  // (1-done) * gamma**n, td.py:492-498
         __syncwarp();
 #pragma unroll
@@ -771,12 +742,7 @@ __global__ void __launch_bounds__(NT) dntd_fwd_kernel(DntdArgs a, float* ws) {
             }
         }
     }
-    if (gridDim.x <= FX_MAX_GRID) {
-        grid_sum_fx<1, NT>(acc, ws, [&](int, double t) { a.loss[0] = (float)(t / (double)a.R); });
-        return;
-    }
-    double tot[1];
-    if (grid_sum<1, NT>(acc, tot, ws, 0) && threadIdx.x == 0) a.loss[0] = (float)(tot[0] / (double)a.R);
+    td_loss_sum<1, NT>(acc, ws, false, [&](int, double t) { a.loss[0] = (float)(t / (double)a.R); });
 }
 
 __global__ void dntd_bwd_kernel(const float* __restrict__ dist, const long long* __restrict__ act,
@@ -1081,6 +1047,37 @@ static double qntd_loss_div(long long S, long long G, long long seq_len) {
     return (double)(S / seq_len) * (double)G * (double)(float)((double)seq_len + 1e-8);
 }
 
+// python's `gamma ** nstep`: libm pow in double, then fp32
+static float gamma_pow(double gamma, int nstep) { return (float)pow(gamma, (double)nstep); }
+
+static TdScalars td_scalars(double gamma, int nstep, double rescale_eps, long long S, long long G, long long seq_len,
+                            double priority_mix) {
+    TdScalars c{};
+    c.gamma = (float)gamma;
+    c.gamma_pow_n = gamma_pow(gamma, nstep);
+    c.eps = (float)rescale_eps; c.four_eps = (float)(4.0 * rescale_eps); c.two_eps = (float)(2.0 * rescale_eps);
+    c.loss_div = qntd_loss_div(S, G, seq_len);
+    c.prio_max_w = (float)priority_mix; c.prio_mean_w = (float)(1.0 - priority_mix);
+    c.prio_div = (float)((double)seq_len + 1e-8);
+    return c;
+}
+
+// Launch plan of qntd, dqfd and soft_td; kern(std::integral_constant<int, NT>()) names the NT-thread build.  Up to 1024 rows
+// without a sequence priority -- the usual replay-buffer batch -- run as ONE CTA of 256 / 512 / 1024 threads, which reduces
+// the loss without any grid round trip; anything else runs as 128-thread CTAs, whose K partial sums each must fit the
+// workspace.
+template <int K, class Args, class Kern>
+static int launch_td_rows(Kern kern, const Args& a, long long rows, bool priority, float* ws, size_t ws_bytes,
+                          cudaStream_t st) {
+    const bool one_cta = rows <= 1024 && !priority;
+    const long long grid = (rows + 127) / 128;
+    if (!ws_partials_fit(one_cta ? 0 : grid * K, ws_bytes)) return B200RL_ERR_WORKSPACE;
+    if (!one_cta) return launch_k(kern(std::integral_constant<int, 128>()), (int)grid, 128, 0, st, a, ws);
+    if (rows <= 256) return launch_k(kern(std::integral_constant<int, 256>()), 1, 256, 0, st, a, ws);
+    if (rows <= 512) return launch_k(kern(std::integral_constant<int, 512>()), 1, 512, 0, st, a, ws);
+    return launch_k(kern(std::integral_constant<int, 1024>()), 1, 1024, 0, st, a, ws);
+}
+
 extern "C" int b200rl_qntd_fwd(const float* q, const float* next_n_q, const long long* action,
                                const long long* next_n_action, const float* reward, const float* done,
                                const float* weight, const float* value_gamma, long long value_gamma_stride,
@@ -1097,31 +1094,16 @@ extern "C" int b200rl_qntd_fwd(const float* q, const float* next_n_q, const long
     if (seq_len < 0 || (seq_len > 0 && (S % seq_len != 0 || cum_reward)) || (priority_out && seq_len <= 0) ||
         (priority_out && (G != 1 || group_mean)))
         return B200RL_ERR_ARG;
-    QntdArgs a{};
+    QntdArgs a{td_scalars(gamma, nstep, rescale_eps, S, G, seq_len, priority_mix)};
     a.q = q; a.next_q = next_n_q; a.action = action; a.next_action = next_n_action; a.reward = reward; a.done = done;
     a.weight = weight; a.value_gamma = value_gamma; a.value_gamma_stride = value_gamma_stride;
     a.gamma_ps = gamma_per_sample; a.S = S; a.Bcol = seq_len > 0 ? S / seq_len : S; a.G = (int)G; a.N = (int)N;
-    a.nstep = nstep; a.gamma = (float)gamma;
-    a.gamma_pow_n = (float)pow(gamma, (double)nstep);  // python's `gamma ** nstep` (libm pow in double), then fp32
-    a.cum_reward = cum_reward; a.rescale = rescale; a.eps = (float)rescale_eps;
-    a.four_eps = (float)(4.0 * rescale_eps); a.two_eps = (float)(2.0 * rescale_eps);
+    a.nstep = nstep; a.cum_reward = cum_reward; a.rescale = rescale;
     a.criterion = criterion; a.crit_param = (float)criterion_param; a.group_mean = group_mean;
-    a.loss_div = qntd_loss_div(S, G, seq_len);
-    a.prio_max_w = (float)priority_mix; a.prio_mean_w = (float)(1.0 - priority_mix);
-    a.prio_div = (float)((double)seq_len + 1e-8);
     a.loss = loss; a.td_err = td_error_per_sample; a.dcrit = dcrit_saved; a.target = target_out;
     a.grad_unit = grad_q_unit; a.priority = priority_out;
-    if (workspace_bytes < WS_MIN_BYTES) return B200RL_ERR_WORKSPACE;
-    if (S <= 1024 && !priority_out) {  // the usual replay-buffer batch: ONE CTA, no grid reduction at all
-        const int nt = S <= 256 ? 256 : (S <= 512 ? 512 : 1024);
-        if (nt == 256) return launch_k(qntd_fwd_kernel<256>, 1, 256, 0, (cudaStream_t)stream, a, workspace);
-        if (nt == 512) return launch_k(qntd_fwd_kernel<512>, 1, 512, 0, (cudaStream_t)stream, a, workspace);
-        return launch_k(qntd_fwd_kernel<1024>, 1, 1024, 0, (cudaStream_t)stream, a, workspace);
-    }
-    constexpr int NT = 128;
-    const int grid = div_up(S, NT);
-    if ((size_t)(WS_CTRL_WORDS + grid) > WS_PARTIAL_LIMIT_WORDS) return B200RL_ERR_WORKSPACE;
-    return launch_k(qntd_fwd_kernel<NT>, grid, NT, 0, (cudaStream_t)stream, a, workspace);
+    return launch_td_rows<1>([](auto nt) { return qntd_fwd_kernel<decltype(nt)::value>; }, a, S, priority_out, workspace,
+                             workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int b200rl_qntd_bwd(const float* dcrit_saved, const float* weight, const long long* action,
@@ -1152,34 +1134,20 @@ extern "C" int b200rl_dqfd_fwd(const float* q, const float* next_n_q, const floa
     if (criterion < -1 || criterion > 3) return B200RL_ERR_ARG;
     if (seq_len < 0 || (seq_len > 0 && (S % seq_len != 0 || cum_reward)) || (priority_out && seq_len <= 0))
         return B200RL_ERR_ARG;
-    DqfdArgs a{};
+    // a workspace under WS_MIN_BYTES is reported before a misaligned `saved`
+    if (workspace_bytes >= WS_MIN_BYTES && reinterpret_cast<uintptr_t>(saved) % 16 != 0) return B200RL_ERR_ARG;
+    DqfdArgs a{td_scalars(gamma, nstep, rescale_eps, S, 1, seq_len, priority_mix)};
     a.q = q; a.next_q = next_n_q; a.next_q1 = new_n_q_one_step; a.action = action; a.next_action = next_n_action;
     a.next_action1 = next_n_action_one_step; a.reward = reward; a.done = done; a.done1 = done_one_step; a.weight = weight;
     a.value_gamma = value_gamma; a.value_gamma_stride = value_gamma_stride; a.is_expert = is_expert;
     a.S = S; a.Bcol = seq_len > 0 ? S / seq_len : S; a.N = (int)N; a.nstep = nstep;
-    a.gamma = (float)gamma; a.gamma_pow_n = (float)pow(gamma, (double)nstep);
-    a.cum_reward = cum_reward; a.rescale = rescale; a.eps = (float)rescale_eps;
-    a.four_eps = (float)(4.0 * rescale_eps); a.two_eps = (float)(2.0 * rescale_eps);
-    a.criterion = criterion; a.crit_param = (float)criterion_param;
+    a.cum_reward = cum_reward; a.rescale = rescale; a.criterion = criterion; a.crit_param = (float)criterion_param;
     a.lam_n = (float)lambda_n_step_td; a.lam_1 = (float)lambda_one_step_td; a.lam_s = (float)lambda_supervised_loss;
     a.margin = (float)margin;
-    a.loss_div = qntd_loss_div(S, 1, seq_len);
-    a.prio_max_w = (float)priority_mix; a.prio_mean_w = (float)(1.0 - priority_mix);
-    a.prio_div = (float)((double)seq_len + 1e-8);
     a.loss = loss; a.td_err = td_error_per_sample; a.stats = loss_statistics; a.saved = reinterpret_cast<float4*>(saved);
     a.target_n = target_n_out; a.target_1 = target_1_out; a.grad_unit = grad_q_unit; a.priority = priority_out;
-    if (workspace_bytes < WS_MIN_BYTES) return B200RL_ERR_WORKSPACE;
-    if (reinterpret_cast<uintptr_t>(saved) % 16 != 0) return B200RL_ERR_ARG;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (S <= 1024 && !priority_out) {  // the usual replay-buffer batch: ONE CTA, no grid reduction at all
-        if (S <= 256) return launch_k(dqfd_fwd_kernel<256>, 1, 256, 0, st, a, workspace);
-        if (S <= 512) return launch_k(dqfd_fwd_kernel<512>, 1, 512, 0, st, a, workspace);
-        return launch_k(dqfd_fwd_kernel<1024>, 1, 1024, 0, st, a, workspace);
-    }
-    constexpr int NT = 128;
-    const long long grid = div_up(S, NT);
-    if (!ws_partials_fit(grid * 4, workspace_bytes)) return B200RL_ERR_WORKSPACE;
-    return launch_k(dqfd_fwd_kernel<NT>, (int)grid, NT, 0, st, a, workspace);
+    return launch_td_rows<4>([](auto nt) { return dqfd_fwd_kernel<decltype(nt)::value>; }, a, S, priority_out, workspace,
+                             workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int b200rl_dqfd_bwd(const float* saved, const float* weight, const long long* action, const float* g_loss,
@@ -1199,19 +1167,6 @@ extern "C" int b200rl_dqfd_bwd(const float* saved, const float* weight, const lo
                     grad_q);
 }
 
-template <int MODE>
-static int launch_soft_td(const SoftTdArgs& a, float* ws, size_t ws_bytes, cudaStream_t st) {
-    if (a.R <= 1024) {  // the usual replay-buffer batch: ONE CTA, no grid reduction at all
-        if (a.R <= 256) return launch_k(soft_td_fwd_kernel<256, MODE>, 1, 256, 0, st, a, ws);
-        if (a.R <= 512) return launch_k(soft_td_fwd_kernel<512, MODE>, 1, 512, 0, st, a, ws);
-        return launch_k(soft_td_fwd_kernel<1024, MODE>, 1, 1024, 0, st, a, ws);
-    }
-    constexpr int NT = 128;
-    const long long grid = div_up(a.R, NT);
-    if (!ws_partials_fit(grid * (MODE == 0 ? 2 : 1), ws_bytes)) return B200RL_ERR_WORKSPACE;
-    return launch_k(soft_td_fwd_kernel<NT, MODE>, (int)grid, NT, 0, st, a, ws);
-}
-
 extern "C" int b200rl_soft_td_fwd(int mode, const float* q, const float* target_q, const float* next_q,
                                   const long long* action, const float* reward, const float* done, const float* weight,
                                   const float* value_gamma, long long value_gamma_stride, long long S, long long G,
@@ -1228,21 +1183,24 @@ extern "C" int b200rl_soft_td_fwd(int mode, const float* q, const float* target_
     if (mode == 0 && (N < 2 || !target_q || !action_gap || !clipfrac)) return B200RL_ERR_ARG;
     if (mode == 1 && nstep < 1) return B200RL_ERR_ARG;
     if (mode != 1 && (cum_reward || value_gamma)) return B200RL_ERR_ARG;
-    if (workspace_bytes < WS_MIN_BYTES) return B200RL_ERR_WORKSPACE;
-    SoftTdArgs a{};
+    if (mode != 1) nstep = 1;
+    SoftTdArgs a{td_scalars(gamma, nstep, 0.0, S, G, 0, 0.0)};
     a.q = q; a.target_q = target_q; a.next_q = next_q; a.action = action; a.reward = reward; a.done = done;
     a.weight = weight; a.value_gamma = value_gamma; a.value_gamma_stride = value_gamma_stride;
-    a.R = S * G; a.G = (int)G; a.N = (int)N; a.nstep = mode == 1 ? nstep : 1;
-    a.gamma = (float)gamma; a.gamma_pow_n = (float)pow(gamma, (double)a.nstep);  // python's `gamma ** nstep`, then fp32
+    a.R = S * G; a.G = (int)G; a.N = (int)N; a.nstep = nstep;
     a.tau = (float)tau; a.alpha = (float)alpha; a.cum_reward = cum_reward;
     a.criterion = criterion; a.crit_param = (float)criterion_param;
-    a.loss_div = (double)S * (double)G;
     a.loss = loss; a.td_err = td_error_per_sample; a.dcrit = dcrit_saved; a.target = target_out; a.grad_unit = grad_q_unit;
     a.action_gap = action_gap; a.clipfrac = clipfrac; a.record_v = record_target_v;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (mode == 0) return launch_soft_td<0>(a, workspace, workspace_bytes, st);
-    if (mode == 1) return launch_soft_td<1>(a, workspace, workspace_bytes, st);
-    return launch_soft_td<2>(a, workspace, workspace_bytes, st);
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (mode == 0)
+        return launch_td_rows<2>([](auto nt) { return soft_td_fwd_kernel<decltype(nt)::value, 0>; }, a, a.R, false, workspace,
+                                 workspace_bytes, st);
+    if (mode == 1)
+        return launch_td_rows<1>([](auto nt) { return soft_td_fwd_kernel<decltype(nt)::value, 1>; }, a, a.R, false, workspace,
+                                 workspace_bytes, st);
+    return launch_td_rows<1>([](auto nt) { return soft_td_fwd_kernel<decltype(nt)::value, 2>; }, a, a.R, false, workspace,
+                             workspace_bytes, st);
 }
 
 extern "C" int b200rl_dntd_fwd(const float* dist, const float* next_n_dist, const long long* act,
@@ -1259,7 +1217,7 @@ extern "C" int b200rl_dntd_fwd(const float* dist, const float* next_n_dist, cons
     a.dist = dist; a.next_dist = next_n_dist; a.act = act; a.next_act = next_n_act; a.reward = reward; a.done = done;
     a.weight = weight; a.weight_stride = weight_stride; a.value_gamma = value_gamma;
     a.value_gamma_stride = value_gamma_stride; a.support = support; a.R = B * A; a.A = A; a.B = B; a.N = (int)N;
-    a.n_atom = n_atom; a.nstep = nstep; a.gamma = (float)gamma; a.gamma_pow_n = (float)pow(gamma, (double)nstep);
+    a.n_atom = n_atom; a.nstep = nstep; a.gamma = (float)gamma; a.gamma_pow_n = gamma_pow(gamma, nstep);
     a.v_min = (float)v_min; a.v_max = (float)v_max; a.delta_z = (float)((v_max - v_min) / (double)(n_atom - 1));
     a.loss = loss; a.td_err = td_error_per_sample; a.proj = proj_saved; a.bad_flag = bad_flag;
     a.grad_unit = grad_dist_unit;
