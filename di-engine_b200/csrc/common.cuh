@@ -148,15 +148,23 @@ __device__ __forceinline__ bool grid_sum(float (&v)[K], double (&tot)[K], float*
 // Grid reduction with ONE atomic round trip per CTA for the SMALL, latency-bound kernels (q-n-step, C51, ...): no ticket, no
 // fence, no second read -- and nothing that relies on when another CTA's plain stores become visible.
 // Every sum k owns two packed 64-bit accumulators in the workspace.  A CTA turns its partial sum (double) into 128-bit fixed
-// point c = hi + lo*2^-40 and adds   word0 += lo<<9 | 1,   word1 += hi<<18 | poison<<9 | 1   with two returning atomics in
+// point c = hi + lo*2^-40 and adds   word0 += lo<<9 | 1,   word1 += hi<<18 | spill<<9 | 1   with two returning atomics in
 // flight together.  The low 9 bits count the CTAs that have added (grid <= 511): the CTA whose add to word0 returns
 // count == grid-1 knows that word0 is complete and equal to (returned + own); it takes word1 the same way (or, if another
 // CTA's add to word1 is still in flight, polls it until its count is complete), calls fin(k, total) and resets both words for
 // the next launch.  Integer addition is associative: the result is bit-identical from run to run whatever the order of
-// arrival.  Resolution 2^-40 absolute, |CTA partial| < 2^36 (larger / non-finite partials are counted in the poison field and
-// the total is NaN).  A one-CTA grid skips the atomics.  (In the big streaming kernels the same scheme LOSES to a dependent
-// finalize launch -- the atomics return only after the SM's store traffic has drained.)
-#define WS_FX_OFF_WORDS 257024  // 16 packed u64 accumulators (zero between launches), above every kernel's partial sums
+// arrival.  Resolution 2^-40 absolute for |CTA partial| < 2^36.  A CTA whose partial is larger or not finite ("spilled")
+// counts itself in word1's spill field and first adds, to two more words of sum k,
+//   word2 += m2<<9 | 1,   word3 += m3<<36 | nan<<27 | -inf<<18 | +inf<<9 | 1
+// where c = m3*2^81 + m2*2^36 + rest exactly, every part with c's sign (|m2| < 2^45 and |m3| < 2^18 signed fields,
+// |rest| < 2^36 goes to words 0 / 1 as usual);
+// a non-finite partial, or a finite one of 2^99 or more, adds rest = 0 and counts as NaN / -inf / +inf.  The last CTA
+// polls words 2 and 3 until their counts equal the spill count, so the total is the exact fixed-point sum for every finite
+// partial below 2^99 (6.3e29), +-inf / NaN as the rows give it, and bit-identical from run to run.  A launch without a
+// spilled CTA never touches words 2 / 3.  A one-CTA grid skips the atomics.  (In the big streaming kernels the same scheme
+// LOSES to a dependent finalize launch -- the atomics return only after the SM's store traffic has drained.)
+#define WS_FX_OFF_WORDS 257024   // 16 packed u64 accumulators (zero between launches), above every kernel's partial sums
+#define WS_FX_SPILL_WORDS 257088 // 16 more (words 2 / 3 of each sum), past the doubles and joins policy.cu keeps at +32..+49
 constexpr int FX_MAX_K = 8;
 constexpr unsigned int FX_MAX_GRID = 511;
 
@@ -164,6 +172,47 @@ __device__ __forceinline__ unsigned long long ld_relaxed_gpu_u64(const unsigned 
     unsigned long long v;
     asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
     return v;
+}
+
+// A spilled CTA partial c (|c| >= 2^36 or not finite): adds its words 2 / 3 (a2 points at them) and returns the rest for
+// words 0 / 1.  Every step is exact: c / 2^81 and c / 2^36 are power-of-two scalings, and the quotients are truncated
+// toward zero, so each m*2^k has c's sign and at most c's magnitude, and c - m*2^k is a multiple of c's last bit smaller
+// than c (flooring instead would turn a negative c into 2^81 - |c| and round its low bits away).
+static __device__ __noinline__ double fx_spill(double c, unsigned long long* a2) {
+    long long m2 = 0;
+    unsigned long long w3 = 1ull;
+    double rest = 0.0;
+    if (c != c) {
+        w3 += 1ull << 27;
+    } else if (!(fabs(c) < 633825300114114700748351602688.0)) {  // 2^99, and +-inf
+        w3 += c > 0.0 ? (1ull << 9) : (1ull << 18);
+    } else {
+        const double m3 = trunc(c * (1.0 / 2417851639229258349412352.0));  // 2^81
+        const double r3 = c - m3 * 2417851639229258349412352.0;
+        const double f2 = trunc(r3 * (1.0 / 68719476736.0));               // 2^36
+        rest = r3 - f2 * 68719476736.0;
+        m2 = (long long)f2;
+        w3 += (unsigned long long)(long long)m3 << 36;
+    }
+    atomicAdd(a2, ((unsigned long long)m2 << 9) + 1ull);
+    atomicAdd(a2 + 1, w3);
+    return rest;
+}
+
+// The last CTA of a launch with `spilled` spilled CTAs: waits for their words 2 / 3, resets them and adds them to the total
+// of words 0 / 1.
+static __device__ __noinline__ double fx_spill_total(double tot, unsigned long long* a2, unsigned int spilled) {
+    unsigned long long t2, t3;
+    do t2 = ld_relaxed_gpu_u64(a2); while ((unsigned int)(t2 & 511ull) != spilled);
+    do t3 = ld_relaxed_gpu_u64(a2 + 1); while ((unsigned int)(t3 & 511ull) != spilled);
+    a2[0] = 0ull;
+    a2[1] = 0ull;
+    const unsigned int pinf = (unsigned int)(t3 >> 9) & 511u, ninf = (unsigned int)(t3 >> 18) & 511u,
+                       nan = (unsigned int)(t3 >> 27) & 511u;
+    if (nan || (pinf && ninf)) return (double)__int_as_float(0x7fc00000);
+    if (pinf) return (double)INFINITY;
+    if (ninf) return -(double)INFINITY;
+    return tot + (double)((long long)t2 >> 9) * 68719476736.0 + (double)((long long)t3 >> 36) * 2417851639229258349412352.0;
 }
 
 template <int K, int NT, class Fin>
@@ -186,12 +235,18 @@ __device__ __forceinline__ void grid_sum_fx(float (&v)[K], float* ws, Fin fin) {
         return;
     }
     const bool bad = !(fabs(c) < 68719476736.0);  // 2^36; also catches NaN
+    unsigned long long* a2 = reinterpret_cast<unsigned long long*>(ws + WS_FX_SPILL_WORDS) + 2 * k;
     long long hi = 0;
     unsigned long long lo = 0;
     if (!bad) {
         const double fl = floor(c);
         hi = (long long)fl;
         lo = (unsigned long long)((c - fl) * 1099511627776.0);  // (c - floor c) is exact; 2^40
+    } else {
+        const double r = fx_spill(c, a2);  // |r| < 2^36
+        const double fl = floor(r);
+        hi = (long long)fl;
+        lo = (unsigned long long)((r - fl) * 1099511627776.0);
     }
     const unsigned long long w0 = (lo << 9) + 1ull;
     const unsigned long long w1 = ((unsigned long long)hi << 18) + (bad ? (1ull << 9) : 0ull) + 1ull;
@@ -202,11 +257,11 @@ __device__ __forceinline__ void grid_sum_fx(float (&v)[K], float* ws, Fin fin) {
     const unsigned long long t0 = old0 + w0;
     unsigned long long t1 = old1 + w1;
     while ((unsigned int)(t1 & 511ull) != gridDim.x) t1 = ld_relaxed_gpu_u64(a0 + 1);
-    const unsigned int poison = (unsigned int)(t1 >> 9) & 511u;
+    const unsigned int spilled = (unsigned int)(t1 >> 9) & 511u;
     const double tot = (double)((long long)t1 >> 18) + (double)(t0 >> 9) * (1.0 / 1099511627776.0);
     a0[0] = 0ull;  // every CTA of this launch has added; the next launch adds only after this one has completed
     a0[1] = 0ull;
-    fin(k, poison ? (double)__int_as_float(0x7fc00000) : tot);
+    fin(k, spilled ? fx_spill_total(tot, a2, spilled) : tot);
 }
 
 // Two-launch variant of the grid reduction for the big streaming kernels: every CTA just stores its K partial sums (no

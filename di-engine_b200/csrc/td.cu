@@ -323,7 +323,7 @@ __global__ void __launch_bounds__(NT) dqfd_fwd_kernel(DqfdArgs a, float* ws) {
         const float* __restrict__ qr = a.q + s * a.N;
         const float q_sa = qr[act], nq = a.next_q[s * a.N + nact], nq1 = a.next_q1[s * a.N + nact1];
         // supervised margin term: max_j(q_j + l_j), l = margin except 0 at the action (td.py:969-972); the gradient of the max
-        // goes to the FIRST maximal index, as torch.max(dim=1) returns it
+        // goes to the FIRST maximal index, as torch.max(dim=1) returns it (a NaN is maximal: the first NaN)
         float mx = 0.f;
         int k = 0;
         for (int j0 = 0; j0 < a.N; j0 += 4) {
@@ -335,7 +335,7 @@ __global__ void __launch_bounds__(NT) dqfd_fwd_kernel(DqfdArgs a, float* ws) {
                 const int j = j0 + u;
                 if (j < a.N) {
                     const float x = fadd(v[u], j == act ? 0.f : a.margin);
-                    if (j == 0 || x > mx) {
+                    if (j == 0 || x > mx || (x != x && mx == mx)) {
                         mx = x;
                         k = j;
                     }
@@ -523,13 +523,14 @@ __global__ void __launch_bounds__(NT) soft_td_fwd_kernel(SoftTdArgs a, float* ws
             const float* __restrict__ tq = a.target_q + r * N;
             const float* __restrict__ nq = a.next_q + r * N;
             const float rw = a.reward[s];
-            // row max of target_q (torch.max: NaN propagates) and its top two for the action gap (topk: equal maxima give 0)
+            // row max of target_q (torch.max: NaN propagates) and its top two for the action gap (topk: equal maxima give 0,
+            // NaN ranks above every number)
             float v = -INFINITY, t1 = -INFINITY, t2 = -INFINITY, vn = -INFINITY;
             for (int j = 0; j < N; ++j) {
                 const float x = tq[j], y = nq[j];
                 if (x > v || x != x) v = x;
                 if (y > vn || y != y) vn = y;
-                if (x > t1) {
+                if (x > t1 || x != x) {
                     t2 = t1;
                     t1 = x;
                 } else if (x > t2) {
