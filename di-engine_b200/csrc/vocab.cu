@@ -1,0 +1,529 @@
+// Vocabulary-scale token losses of the language-model policy-gradient family, on fp32 or bf16 logits:
+//   grpo_policy_error                 ding/rl_utils/grpo.py             clipped ratio loss + beta * k3 KL to the reference policy
+//   rloo_policy_error                 ding/rl_utils/rloo.py             clipped ratio loss, leave-one-out advantage from reward (K, B')
+//   naive / efficient / less_efficient_method   ding/rl_utils/log_prob_utils.py   per-token log p(a) and its backward
+//
+// vocab_rows_kernel<T, MODE>: persistent CTAs of VOCAB_NT threads, each owning one token row of V logits at a time
+// (row += gridDim.x).  Per row, in ONE streaming pass over every logit tensor of the call (16-byte vector loads, all
+// streams' loads of an iteration in flight together), an online max / sum of exp in fp32 per tensor gives
+// logsumexp = max + log(sum exp(z - max)) with torch's rule for an infinite max (treated as 0); the gathered z[a] gives
+// lp = z[a] - logsumexp.  The row epilogue (thread 0) runs the token head (token_head below, in the reference's operation
+// order) and forms c = d loss / d lp_new for a unit upstream gradient; the CTA then writes
+// d loss / d logit_new[row] = c * (onehot(a) - softmax(logit_new[row])) in T.  MODE = LOGP writes lp and logsumexp only;
+// MODE = BWD applies a per-row coefficient g * coef[row] to (onehot - softmax) -- the backward of the log-prob methods, and
+// of the GRPO / RLOO launch when the upstream gradient is not the unit one the forward launch assumed.
+//
+// Traffic floor per token row: every logit read once plus the gradient written once, (3 + 1) * V * sizeof(T) for GRPO and
+// (2 + 1) * V * sizeof(T) for RLOO; per-row side data (action, weight, lse, coefficient) is O(1) per row.
+//
+// The softmax of the gradient needs logit_new a second time.  The forward launch keeps the row in dynamic shared memory
+// as it streams it, up to VOCAB_SMEM_CAP bytes (all of V = 32k in fp32 or V = 64k in bf16).  A longer row (bf16
+// V = 152 064 is 304 KB) keeps its first VOCAB_SMEM_CAP bytes there and reads the rest back from L2 right after the
+// same CTA streamed it: such a row runs one CTA per SM, so the bytes to re-read across the GPU are at most 132 * 84 KB
+// = 11 MB, a fifth of the H100's 50 MB L2, and the other streams are loaded evict-first so they do not push it out.
+// Chosen over splitting the row across a thread-block cluster because it keeps one code path for every V: a cluster
+// split needs a second, DSMEM-level max / sum combine and a cluster size chosen per V, for the 28 % of the row that
+// the L2 serves here.  The L2 holds the re-read only while 132 * (V * sizeof(T) - 220 KB) stays well below its 50 MB:
+// up to about V = 190k in bf16 and V = 95k in fp32.  Past that (e.g. fp32 V = 152 064: 388 KB re-read per row, 51 MB
+// across the GPU) part of the second read of logit_new goes to HBM and the call moves up to 5 * V * sizeof(T) bytes per
+// row (GRPO) instead of the floor.
+//
+// The loss head on a custom log_prob_fn's (B, S) output is a second, small kernel (token_head_kernel below): it reads no
+// logits, so it shares the head arithmetic (token_head) but none of the row machinery.
+//
+// Loss sums (loss, approx_kl, clipfrac): per-CTA partials (grid_store_partials) added in a fixed order by
+// finalize_sums_kernel -- deterministic, no atomics, no host sync.
+#include <cuda_bf16.h>
+#include <math.h>
+
+#include "../../include/b200rl.h"
+#include "common.cuh"
+
+namespace b200rl {
+
+constexpr int VOCAB_NT = 512;
+constexpr int VOCAB_HEAD_NT = 256;
+constexpr int VOCAB_SMEM_CAP = 220 * 1024;  // dynamic shared memory for the cached part of logit_new (227 KB opt-in max)
+constexpr int VM_GRPO = 0, VM_RLOO = 1, VM_LOGP = 2, VM_BWD = 3;
+constexpr float kL2E = 1.4426950408889634f;
+
+// 16-byte vectors of T, widened to fp32
+template <class T>
+struct VecT;
+template <>
+struct VecT<float> {
+    static constexpr int W = 4;
+    static __device__ __forceinline__ void unpack(uint4 u, float (&x)[4]) {
+        x[0] = __uint_as_float(u.x); x[1] = __uint_as_float(u.y); x[2] = __uint_as_float(u.z); x[3] = __uint_as_float(u.w);
+    }
+    static __device__ __forceinline__ uint4 pack(const float (&x)[4]) {
+        return make_uint4(__float_as_uint(x[0]), __float_as_uint(x[1]), __float_as_uint(x[2]), __float_as_uint(x[3]));
+    }
+    static __device__ __forceinline__ float to_f(float v) { return v; }
+    static __device__ __forceinline__ float from_f(float v) { return v; }
+};
+template <>
+struct VecT<__nv_bfloat16> {
+    static constexpr int W = 8;
+    static __device__ __forceinline__ void unpack(uint4 u, float (&x)[8]) {
+        const unsigned int w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            x[2 * i] = __uint_as_float(w[i] << 16);
+            x[2 * i + 1] = __uint_as_float(w[i] & 0xffff0000u);
+        }
+    }
+    static __device__ __forceinline__ uint4 pack(const float (&x)[8]) {
+        unsigned int w[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            __nv_bfloat162 h = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
+            w[i] = *reinterpret_cast<unsigned int*>(&h);
+        }
+        return make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    static __device__ __forceinline__ float to_f(__nv_bfloat16 v) { return __bfloat162float(v); }
+    static __device__ __forceinline__ __nv_bfloat16 from_f(float v) { return __float2bfloat16_rn(v); }
+};
+
+// torch's logsumexp takes an infinite maximum as 0
+__device__ __forceinline__ float lse_ref(float m) { return fabsf(m) == INFINITY ? 0.f : m; }
+
+// online (max, sum exp(z - lse_ref(max))) over n values
+template <int N>
+__device__ __forceinline__ void ms_add(float& m, float& s, const float (&x)[N]) {
+    float mc = x[0];
+#pragma unroll
+    for (int i = 1; i < N; ++i) mc = fmaxf(mc, x[i]);
+    if (mc > m) {
+        if (s != 0.f) s *= exp2f((lse_ref(m) - lse_ref(mc)) * kL2E);
+        m = mc;
+    }
+    const float r = lse_ref(m);
+    float e[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i) e[i] = exp2f((x[i] - r) * kL2E);
+    // pairwise within the vector, then one add to the running sum: a thread's sequential chain over a 152k-entry row is
+    // N times shorter, and so is its fp32 rounding
+#pragma unroll
+    for (int w = 1; w < N; w *= 2)
+#pragma unroll
+        for (int i = 0; i + w < N; i += 2 * w) e[i] += e[i + w];
+    s += e[0];
+}
+
+__device__ __forceinline__ void ms_merge(float& m, float& s, float m2, float s2) {
+    if (m2 > m) {
+        const float tm = m, ts = s;
+        m = m2; s = s2; m2 = tm; s2 = ts;
+    }
+    if (s2 != 0.f) s += s2 * exp2f((lse_ref(m2) - lse_ref(m)) * kL2E);
+}
+
+// The per-token head of grpo.py / rloo.py.  In: lp_new, lp_old, lp_ref (GRPO only), the row's advantage, the clamp
+// bounds fp32(1 - clip) / fp32(1 + clip), beta, and gt = d loss / d per_token_loss (the unit-upstream factor
+// (1 / B) / sum_s(w) * w).  Out: the per-token loss, the clip indicator and d loss / d lp_new.  Gradients follow torch:
+// min() splits a tie evenly between its two operands, clamp() passes the gradient at its edges.
+struct TokenHead {
+    float loss, clipped, dlp;
+};
+
+template <bool KL>
+__device__ __forceinline__ TokenHead token_head(float lp_new, float lp_old, float lp_ref, float adv, float lo, float hi,
+                                                float beta, float gt) {
+    TokenHead h;
+    const float ratio = expf(lp_new - lp_old);
+    const float rc = ratio < lo ? lo : (ratio > hi ? hi : ratio);  // NaN stays NaN, as torch.clamp
+    const float u = ratio * adv, c = rc * adv;
+    float mn = u < c ? u : c;
+    if (u != u) mn = u;  // torch.min propagates NaN from either side
+    h.loss = -mn;
+    const float gm = -gt;
+    const float gu = u < c ? gm : (u == c ? 0.5f * gm : 0.f);
+    const float gc = c < u ? gm : (u == c ? 0.5f * gm : 0.f);
+    const float inside = (ratio >= lo && ratio <= hi) ? 1.f : 0.f;
+    h.dlp = (gu * adv + gc * adv * inside) * ratio;
+    if (KL) {
+        const float dr = lp_ref - lp_new;
+        const float e = expf(dr);
+        h.loss = h.loss + beta * (e - dr - 1.f);
+        const float gk = gt * beta;
+        h.dlp -= gk * e - gk;
+    }
+    h.clipped = (ratio > hi || ratio < lo) ? 1.f : 0.f;
+    return h;
+}
+
+// leave-one-out advantage of row b from reward (K, Bp): (k, j) = (b / Bp, b % Bp), baseline = (sum_k r[k, j] - r) / (K - 1)
+__device__ __forceinline__ float rloo_adv(const float* __restrict__ reward, int K, long long Bp, long long b) {
+    const long long k = b / Bp, j = b - k * Bp;
+    float sum = 0.f;
+    for (int q = 0; q < K; ++q) sum += reward[(long long)q * Bp + j];
+    const float r = reward[k * Bp + j];
+    return r - (sum - r) / (float)(K - 1);
+}
+
+struct VocabArgs {
+    const void* x[3];          // logit_new, logit_old, logit_ref (streams in that order; BWD / LOGP: x[0] only)
+    const long long* action;   // (rows)
+    const float* adv;          // GRPO: (B)
+    const float* reward;       // RLOO: (K, B / K)
+    const float* weight;       // (B, S) nullable = ones
+    const float* coef_in;      // BWD: per-row coefficient
+    const float* g;            // BWD: upstream scalar (nullable = 1)
+    float* lp;                 // LOGP: (rows)
+    float* lse;                // forward: logsumexp of logit_new per row; BWD: read
+    float* coef;               // GRPO / RLOO: d loss / d lp_new per row for a unit upstream gradient
+    void* grad;                // d / d logit_new (nullable in the forward = no gradient)
+    float* ws;
+    long long rows, S, V, Bp;
+    int K, skip_if_unit, capv;  // capv: 16-byte vectors of logit_new kept in shared memory
+    float lo, hi, beta, inv_b;
+};
+
+template <int NR, bool CACHE, class T>
+__device__ __forceinline__ void stream_vecs(const uint4* const (&p)[NR], int i, float (&m)[NR], float (&s)[NR],
+                                            uint4* cache, int capv) {
+    constexpr int W = VecT<T>::W;
+    uint4 u[NR];
+#pragma unroll
+    for (int r = 0; r < NR; ++r) u[r] = r == 0 ? __ldg(p[0] + i) : __ldcs(p[r] + i);
+    if (CACHE && i < capv) cache[i] = u[0];
+#pragma unroll
+    for (int r = 0; r < NR; ++r) {
+        float x[W];
+        VecT<T>::unpack(u[r], x);
+        ms_add<W>(m[r], s[r], x);
+    }
+}
+
+template <class T, int MODE>
+__global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
+    pdl_prologue();
+    using V_ = VecT<T>;
+    constexpr int W = V_::W;
+    constexpr int NR = MODE == VM_GRPO ? 3 : (MODE == VM_RLOO ? 2 : 1);
+    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO;
+    extern __shared__ uint4 s_row[];
+    __shared__ float s_m[NR][VOCAB_NT / 32], s_s[NR][VOCAB_NT / 32], s_w[VOCAB_NT / 32];
+    __shared__ float s_c, s_lse;
+    __shared__ long long s_a;
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const long long V = a.V;
+    const bool want_grad = a.grad != nullptr;
+    float gscale = 1.f;
+    if (MODE == VM_BWD) {
+        if (a.g) gscale = *a.g;
+        if (a.skip_if_unit && gscale == 1.f) return;  // the forward launch already wrote exactly this gradient
+    }
+    float part[3] = {0.f, 0.f, 0.f};  // thread 0: loss, approx_kl, clipfrac partial sums of this CTA's rows
+    float w_tot = (float)a.S;  // thread 0: sum_s w[b, s] of the current row's sequence (S without weights)
+    for (long long row = blockIdx.x; row < a.rows; row += gridDim.x) {
+        const size_t off = (size_t)row * (size_t)V;
+        // elements before the row's first 16-byte boundary (the base pointers are 16-byte aligned)
+        const long long mis = (long long)((off * sizeof(T)) & 15u) / (long long)sizeof(T);
+        const long long h = mis ? min((long long)(16 / sizeof(T)) - mis, V) : 0;
+        const int nvec = (int)((V - h) / W);
+        const long long tail0 = h + (long long)nvec * W;
+        const T* rp[NR];
+        const uint4* vp[NR];
+#pragma unroll
+        for (int r = 0; r < NR; ++r) {
+            rp[r] = reinterpret_cast<const T*>(a.x[r]) + off;
+            vp[r] = reinterpret_cast<const uint4*>(rp[r] + h);
+        }
+        float c = 0.f, lse = 0.f;
+        long long act = 0;
+        if (MODE == VM_BWD) {
+            c = gscale * a.coef_in[row];
+            lse = a.lse[row];
+            act = a.action[row];
+        } else {
+            float m[NR], s[NR];
+#pragma unroll
+            for (int r = 0; r < NR; ++r) m[r] = -INFINITY, s[r] = 0.f;
+            const bool cache = LOSS && want_grad;
+            int i = tid;
+            for (; i + VOCAB_NT < nvec; i += 2 * VOCAB_NT) {
+                if (cache) {
+                    stream_vecs<NR, true, T>(vp, i, m, s, s_row, a.capv);
+                    stream_vecs<NR, true, T>(vp, i + VOCAB_NT, m, s, s_row, a.capv);
+                } else {
+                    stream_vecs<NR, false, T>(vp, i, m, s, s_row, 0);
+                    stream_vecs<NR, false, T>(vp, i + VOCAB_NT, m, s, s_row, 0);
+                }
+            }
+            if (i < nvec) {
+                if (cache) stream_vecs<NR, true, T>(vp, i, m, s, s_row, a.capv);
+                else stream_vecs<NR, false, T>(vp, i, m, s, s_row, 0);
+            }
+            // the unaligned head and tail, < 16 bytes each
+            for (long long j = tid; j < h + (V - tail0); j += VOCAB_NT) {
+                const long long e = j < h ? j : tail0 + (j - h);
+#pragma unroll
+                for (int r = 0; r < NR; ++r) {
+                    const float x[1] = {V_::to_f(rp[r][e])};
+                    ms_add<1>(m[r], s[r], x);
+                }
+            }
+            float wsum = 0.f;
+            // a CTA's rows step by gridDim.x (< S at language-model sizes): it sums a sequence's weights once per visit to
+            // that sequence, not once per token
+            const bool new_seq = LOSS && a.weight && (row < gridDim.x || row / a.S != (row - gridDim.x) / a.S);
+            if (new_seq) {
+                const float* wr = a.weight + (row / a.S) * a.S;
+                for (long long j = tid; j < a.S; j += VOCAB_NT) wsum += wr[j];
+            }
+#pragma unroll
+            for (int r = 0; r < NR; ++r) {
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) {
+                    const float m2 = __shfl_down_sync(0xffffffffu, m[r], o), s2 = __shfl_down_sync(0xffffffffu, s[r], o);
+                    ms_merge(m[r], s[r], m2, s2);
+                }
+                if (lane == 0) s_m[r][wid] = m[r], s_s[r][wid] = s[r];
+            }
+            if (new_seq) {
+                wsum = warp_sum(wsum);
+                if (lane == 0) s_w[wid] = wsum;
+            }
+            __syncthreads();
+            if (tid == 0) {
+                float lp[NR];
+                act = a.action[row];
+                const bool ok = act >= 0 && act < V;
+#pragma unroll
+                for (int r = 0; r < NR; ++r) {
+                    float mm = s_m[r][0], ss = s_s[r][0];
+                    for (int w = 1; w < VOCAB_NT / 32; ++w) ms_merge(mm, ss, s_m[r][w], s_s[r][w]);
+                    const float l = logf(ss) + lse_ref(mm);
+                    if (r == 0) lse = l;
+                    lp[r] = ok ? V_::to_f(rp[r][act]) - l : __int_as_float(0x7fc00000);
+                }
+                a.lse[row] = lse;
+                if (MODE == VM_LOGP) a.lp[row] = lp[0];
+                if (LOSS) {
+                    const long long b = row / a.S;
+                    if (new_seq) {
+                        w_tot = 0.f;
+                        for (int w = 0; w < VOCAB_NT / 32; ++w) w_tot += s_w[w];
+                    }
+                    const float W_ = w_tot;
+                    const float w = a.weight ? a.weight[row] : 1.f;
+                    const float adv = MODE == VM_GRPO ? a.adv[b] : rloo_adv(a.reward, a.K, a.Bp, b);
+                    const float gt = a.inv_b / W_ * w;
+                    const TokenHead th = token_head<MODE == VM_GRPO>(lp[0], lp[1], NR > 2 ? lp[NR - 1] : 0.f, adv, a.lo,
+                                                                     a.hi, a.beta, gt);
+                    c = th.dlp;
+                    a.coef[row] = c;
+                    part[0] += th.loss * w / W_;
+                    part[1] += lp[1] - lp[0];
+                    part[2] += th.clipped;
+                }
+                s_c = c;
+                s_lse = lse;
+                s_a = act;
+            }
+            __syncthreads();
+            if (!LOSS || !want_grad) continue;
+            c = s_c;
+            lse = s_lse;
+            act = s_a;
+        }
+        // d / d logit_new[row] = c * (onehot(a) - softmax)
+        T* gr = reinterpret_cast<T*>(a.grad) + off;
+        uint4* gv = reinterpret_cast<uint4*>(gr + h);
+        for (int i = tid; i < nvec; i += VOCAB_NT) {
+            const uint4 u = (LOSS && i < a.capv) ? s_row[i] : (MODE == VM_BWD ? __ldcs(vp[0] + i) : __ldg(vp[0] + i));
+            float x[W];
+            V_::unpack(u, x);
+            const long long e0 = h + (long long)i * W;
+#pragma unroll
+            for (int k = 0; k < W; ++k) x[k] = c * ((e0 + k == act ? 1.f : 0.f) - exp2f((x[k] - lse) * kL2E));
+            __stcs(gv + i, V_::pack(x));
+        }
+        for (long long j = tid; j < h + (V - tail0); j += VOCAB_NT) {
+            const long long e = j < h ? j : tail0 + (j - h);
+            const float x = V_::to_f(rp[0][e]);
+            gr[e] = V_::from_f(c * ((e == act ? 1.f : 0.f) - exp2f((x - lse) * kL2E)));
+        }
+        if (LOSS) __syncthreads();  // s_row and s_c are rewritten by the next row
+    }
+    if (LOSS) {
+        float v[3] = {0.f, 0.f, 0.f};
+        if (tid == 0) v[0] = part[0], v[1] = part[1], v[2] = part[2];
+        grid_store_partials<3, VOCAB_NT>(v, a.ws);
+    }
+}
+
+// The token head alone, on per-token log-probabilities a caller computed itself (a custom log_prob_fn): one CTA per
+// sequence b at a time, thread = token.  Writes d loss / d lp_new for a unit upstream gradient and the loss partials.
+template <bool KL>
+__global__ void __launch_bounds__(VOCAB_HEAD_NT) token_head_kernel(const float* __restrict__ lp_new,
+                                                                   const float* __restrict__ lp_old,
+                                                                   const float* __restrict__ lp_ref, VocabArgs a) {
+    pdl_prologue();
+    __shared__ float s_w[VOCAB_HEAD_NT / 32];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const long long B = a.rows / a.S;
+    float part[3] = {0.f, 0.f, 0.f};
+    for (long long b = blockIdx.x; b < B; b += gridDim.x) {
+        const long long o = b * a.S;
+        float W_ = (float)a.S;
+        if (a.weight) {
+            float ws = 0.f;
+            for (long long j = tid; j < a.S; j += VOCAB_HEAD_NT) ws += a.weight[o + j];
+            ws = warp_sum(ws);
+            if (lane == 0) s_w[wid] = ws;
+            __syncthreads();
+            W_ = 0.f;
+            for (int w = 0; w < VOCAB_HEAD_NT / 32; ++w) W_ += s_w[w];
+            __syncthreads();
+        }
+        const float adv = KL ? a.adv[b] : rloo_adv(a.reward, a.K, a.Bp, b);
+        for (long long j = tid; j < a.S; j += VOCAB_HEAD_NT) {
+            const float w = a.weight ? a.weight[o + j] : 1.f;
+            const float ln = lp_new[o + j], lo_ = lp_old[o + j];
+            const TokenHead th = token_head<KL>(ln, lo_, KL ? lp_ref[o + j] : 0.f, adv, a.lo, a.hi, a.beta, a.inv_b / W_ * w);
+            a.coef[o + j] = th.dlp;
+            part[0] += th.loss * w / W_;
+            part[1] += lo_ - ln;
+            part[2] += th.clipped;
+        }
+    }
+    grid_store_partials<3, VOCAB_HEAD_NT>(part, a.ws);
+}
+
+}  // namespace b200rl
+
+using namespace b200rl;
+
+namespace {
+
+bool aligned_logits(const void* p) { return p && aligned16(p); }
+
+template <class T, int MODE>
+int launch_rows(VocabArgs& a, float* out3, size_t ws_bytes, long long B, cudaStream_t st) {
+    constexpr auto kern = vocab_rows_kernel<T, MODE>;
+    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO;
+    const long long nvec_max = (a.V * (long long)sizeof(T) + 15) / 16;
+    a.capv = (LOSS && a.grad) ? (int)min(nvec_max, (long long)(VOCAB_SMEM_CAP / 16)) : 0;
+    const size_t smem = (size_t)a.capv * 16;
+    int sms = 0, per_sm = 0;
+    if (int rc = resident_ctas<kern>(VOCAB_NT, smem, sms, per_sm)) return rc;
+    long long grid = (long long)sms * per_sm;
+    if (grid > a.rows) grid = a.rows;
+    if (LOSS && !ws_partials_fit(grid * 3, ws_bytes)) return B200RL_ERR_WORKSPACE;
+    if (int rc = launch_k(kern, (int)grid, VOCAB_NT, smem, st, a)) return rc;
+    if (!LOSS) return B200RL_OK;
+    FinalizeArgs fa{};
+    fa.scale[0] = 1.0 / (double)B;
+    fa.scale[1] = fa.scale[2] = 1.0 / (double)a.rows;
+    fa.k = 3;
+    fa.n_blocks = (int)grid;
+    return launch_finalize(a.ws, out3, fa, st);
+}
+
+template <int MODE>
+int launch_dtype(int dtype, VocabArgs& a, float* out3, size_t ws_bytes, long long B, cudaStream_t st) {
+    if (dtype == B200RL_DTYPE_F32) return launch_rows<float, MODE>(a, out3, ws_bytes, B, st);
+    if (dtype == B200RL_DTYPE_BF16) return launch_rows<__nv_bfloat16, MODE>(a, out3, ws_bytes, B, st);
+    return B200RL_ERR_ARG;
+}
+
+bool sizes_ok(long long B, long long S, long long V) {
+    return B > 0 && S > 0 && V > 0 && V < (1ll << 31) && B * S < (1ll << 40);
+}
+
+}  // namespace
+
+extern "C" int b200rl_grpo_fwd_grad(int dtype, const void* logit_new, const void* logit_old, const void* logit_ref,
+                                    const long long* action, const float* adv, const float* weight, long long B,
+                                    long long S, long long V, double clip_ratio, double beta, float* out3, float* lse_new,
+                                    float* dlogp_unit, void* grad_logit_new, float* workspace, size_t workspace_bytes,
+                                    void* stream) {
+    if (!sizes_ok(B, S, V) || !aligned_logits(logit_new) || !aligned_logits(logit_old) || !aligned_logits(logit_ref) ||
+        !action || !adv || !out3 || !lse_new || !dlogp_unit || !workspace ||
+        (grad_logit_new && !aligned16(grad_logit_new)))
+        return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logit_new; a.x[1] = logit_old; a.x[2] = logit_ref;
+    a.action = action; a.adv = adv; a.weight = weight;
+    a.lse = lse_new; a.coef = dlogp_unit; a.grad = grad_logit_new; a.ws = workspace;
+    a.rows = B * S; a.S = S; a.V = V;
+    a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio); a.beta = (float)beta;
+    a.inv_b = (float)(1.0 / (double)B);
+    return launch_dtype<VM_GRPO>(dtype, a, out3, workspace_bytes, B, (cudaStream_t)stream);
+}
+
+extern "C" int b200rl_rloo_fwd_grad(int dtype, const void* logit_new, const void* logit_old, const long long* action,
+                                    const float* reward, long long K, const float* weight, long long B, long long S,
+                                    long long V, double clip_ratio, float* out3, float* lse_new, float* dlogp_unit,
+                                    void* grad_logit_new, float* workspace, size_t workspace_bytes, void* stream) {
+    if (!sizes_ok(B, S, V) || K < 1 || K > (1 << 20) || B % K || !aligned_logits(logit_new) ||
+        !aligned_logits(logit_old) || !action || !reward || !out3 || !lse_new || !dlogp_unit || !workspace ||
+        (grad_logit_new && !aligned16(grad_logit_new)))
+        return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logit_new; a.x[1] = logit_old;
+    a.action = action; a.reward = reward; a.K = (int)K; a.Bp = B / K; a.weight = weight;
+    a.lse = lse_new; a.coef = dlogp_unit; a.grad = grad_logit_new; a.ws = workspace;
+    a.rows = B * S; a.S = S; a.V = V;
+    a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio);
+    a.inv_b = (float)(1.0 / (double)B);
+    return launch_dtype<VM_RLOO>(dtype, a, out3, workspace_bytes, B, (cudaStream_t)stream);
+}
+
+extern "C" int b200rl_token_logp_fwd(int dtype, const void* logits, const long long* index, long long rows, long long V,
+                                     float* logp, float* lse, void* stream) {
+    if (!sizes_ok(rows, 1, V) || !aligned_logits(logits) || !index || !logp || !lse) return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logits; a.action = index; a.lp = logp; a.lse = lse;
+    a.rows = rows; a.S = 1; a.V = V;
+    return launch_dtype<VM_LOGP>(dtype, a, nullptr, 0, rows, (cudaStream_t)stream);
+}
+
+extern "C" int b200rl_token_logp_bwd(int dtype, const void* logits, const long long* index, const float* lse,
+                                     const float* dlogp, const float* g_scale, int skip_if_unit, long long rows,
+                                     long long V, void* grad_logits, void* stream) {
+    if (!sizes_ok(rows, 1, V) || !aligned_logits(logits) || !index || !lse || !dlogp || !grad_logits ||
+        !aligned16(grad_logits) || (skip_if_unit && !g_scale))
+        return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logits; a.action = index; a.lse = const_cast<float*>(lse); a.coef_in = dlogp; a.g = g_scale;
+    a.skip_if_unit = skip_if_unit; a.grad = grad_logits;
+    a.rows = rows; a.S = 1; a.V = V;
+    return launch_dtype<VM_BWD>(dtype, a, nullptr, 0, rows, (cudaStream_t)stream);
+}
+
+extern "C" int b200rl_token_head_fwd(const float* logp_new, const float* logp_old, const float* logp_ref,
+                                     const float* adv, const float* reward, long long K, const float* weight, long long B,
+                                     long long S, double clip_ratio, double beta, float* out3, float* dlogp_unit,
+                                     float* workspace, size_t workspace_bytes, void* stream) {
+    const bool grpo = logp_ref != nullptr;
+    if (!sizes_ok(B, S, 1) || !logp_new || !logp_old || !out3 || !dlogp_unit || !workspace ||
+        (grpo ? !adv : (!reward || K < 1 || K > (1 << 20) || B % K)))
+        return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.adv = adv; a.reward = reward; a.K = (int)K; a.Bp = grpo ? 0 : B / K; a.weight = weight;
+    a.coef = dlogp_unit; a.ws = workspace;
+    a.rows = B * S; a.S = S; a.V = 1;
+    a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio); a.beta = (float)beta;
+    a.inv_b = (float)(1.0 / (double)B);
+    auto kern = grpo ? token_head_kernel<true> : token_head_kernel<false>;
+    int sms = 0, per_sm = 0;
+    if (int rc = grpo ? resident_ctas<token_head_kernel<true>>(VOCAB_HEAD_NT, 0, sms, per_sm)
+                      : resident_ctas<token_head_kernel<false>>(VOCAB_HEAD_NT, 0, sms, per_sm))
+        return rc;
+    long long grid = (long long)sms * per_sm;
+    if (grid > B) grid = B;
+    if (!ws_partials_fit(grid * 3, workspace_bytes)) return B200RL_ERR_WORKSPACE;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = launch_k(kern, (int)grid, VOCAB_HEAD_NT, 0, st, logp_new, logp_old, logp_ref, a)) return rc;
+    FinalizeArgs fa{};
+    fa.scale[0] = 1.0 / (double)B;
+    fa.scale[1] = fa.scale[2] = 1.0 / (double)a.rows;
+    fa.k = 3;
+    fa.n_blocks = (int)grid;
+    return launch_finalize(workspace, out3, fa, st);
+}

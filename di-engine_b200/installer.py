@@ -20,9 +20,10 @@ def _originals():
     """name -> set of objects that count as 'the reference implementation' of that name."""
     found = {}
     base = sys.modules.get('ding.rl_utils')
-    for name in _ours.HOT_PATH_FUNCTIONS:
+    for name in _ours.HOT_PATH_FUNCTIONS + _ours.LM_HOT_PATH_FUNCTIONS:
         objs = set()
-        cands = [base] + [sys.modules.get('ding.rl_utils.' + m) for m in ('gae', 'ppo', 'td', 'vtrace', 'upgo', 'a2c', 'retrace', 'happo', 'acer', 'ppg')]
+        cands = [base] + [sys.modules.get('ding.rl_utils.' + m) for m in ('gae', 'ppo', 'td', 'vtrace', 'upgo', 'a2c', 'retrace', 'happo', 'acer', 'ppg',
+                                                                          'grpo', 'rloo', 'log_prob_utils')]
         for mod in cands:
             fn = getattr(mod, name, None) if mod is not None else None
             if fn is not None and fn is not getattr(_ours, name):

@@ -1168,3 +1168,152 @@ class VTraceContinuousFunction(torch.autograd.Function):
                                                     pe, T, B, D, ptr(gm), ptr(gs), ptr(gv), stream_ptr())
         _lib.check(rc, 'b200rl_vtrace_continuous_bwd')
         return (gm, gs, gv) + (None, ) * 11
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# language-model policy losses on vocabulary-scale logits (csrc/vocab.cu)
+# ----------------------------------------------------------------------------------------------------------------
+_LOGIT_DTYPES = {torch.float32: 0, torch.bfloat16: 1}  # B200RL_DTYPE_F32, B200RL_DTYPE_BF16
+
+
+def logit_dtype(*logits):
+    """dtype code of csrc/vocab.cu for the logits of one call: fp32 or bf16, every logit tensor in the same dtype.  These
+    kernels read bf16 as it arrives and compute in fp32; every other operator keeps to ``f32c``."""
+    dt = logits[0].dtype
+    if dt not in _LOGIT_DTYPES:
+        raise TypeError("di_engine_b200: logits must be float32 or bfloat16 (got %s)" % dt)
+    for t in logits[1:]:
+        if t.dtype != dt:
+            raise TypeError("di_engine_b200: all logits of one call must share a dtype (got %s and %s)" % (dt, t.dtype))
+    return _LOGIT_DTYPES[dt]
+
+
+def logits_c(t):
+    """contiguous and 16-byte aligned, as the kernel's vector loads need (a view at an odd offset is copied)"""
+    t = t.contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
+class GRPOFunction(torch.autograd.Function):
+    """grpo_policy_error (ding/rl_utils/grpo.py) on logits (B, S, V): outputs loss (differentiable w.r.t. logit_new),
+    approx_kl and clipfrac.  ONE forward launch (+ the loss-sum finalize) also writes d loss / d logit_new for a unit
+    upstream gradient; ``backward`` hands that buffer to autograd after a launch that returns at once on the device when
+    the upstream gradient really is 1, and recomputes otherwise from the saved per-row logsumexp and coefficient."""
+
+    @staticmethod
+    def forward(ctx, logit_new, logit_old, logit_ref, action, adv, weight, dt, clip_ratio, beta):
+        B, S, V = logit_new.shape
+        out, lse, dlp, grad = _vocab_outputs(ctx, logit_new)
+        with on_device(logit_new.device):
+            ws = workspace(logit_new.device)
+            rc = lib().b200rl_grpo_fwd_grad(dt, ptr(logit_new), ptr(logit_old), ptr(logit_ref), ptr(action), ptr(adv),
+                                            ptr(weight), B, S, V, clip_ratio, beta, ptr(out), ptr(lse), ptr(dlp),
+                                            ptr(grad), ptr(ws), ws.numel() * 4, stream_ptr())
+        _lib.check(rc, 'b200rl_grpo_fwd_grad')
+        return _vocab_saved(ctx, logit_new, action, lse, dlp, grad, dt, out)
+
+    @staticmethod
+    def backward(ctx, g_loss, _g_kl, _g_cf):
+        return (_vocab_backward(ctx, g_loss), ) + (None, ) * 8
+
+
+class RLOOFunction(torch.autograd.Function):
+    """rloo_policy_error (ding/rl_utils/rloo.py) on logits (B, S, V); the leave-one-out advantage is formed in the kernel
+    from reward (K, B / K).  Outputs and backward as ``GRPOFunction``."""
+
+    @staticmethod
+    def forward(ctx, logit_new, logit_old, action, reward, weight, dt, clip_ratio):
+        B, S, V = logit_new.shape
+        out, lse, dlp, grad = _vocab_outputs(ctx, logit_new)
+        with on_device(logit_new.device):
+            ws = workspace(logit_new.device)
+            rc = lib().b200rl_rloo_fwd_grad(dt, ptr(logit_new), ptr(logit_old), ptr(action), ptr(reward), reward.shape[0],
+                                            ptr(weight), B, S, V, clip_ratio, ptr(out), ptr(lse), ptr(dlp), ptr(grad),
+                                            ptr(ws), ws.numel() * 4, stream_ptr())
+        _lib.check(rc, 'b200rl_rloo_fwd_grad')
+        return _vocab_saved(ctx, logit_new, action, lse, dlp, grad, dt, out)
+
+    @staticmethod
+    def backward(ctx, g_loss, _g_kl, _g_cf):
+        return (_vocab_backward(ctx, g_loss), ) + (None, ) * 6
+
+
+def _vocab_outputs(ctx, logit_new):
+    dev = logit_new.device
+    rows = logit_new.shape[0] * logit_new.shape[1]
+    out = torch.empty(3, dtype=torch.float32, device=dev)
+    lse = torch.empty(rows, dtype=torch.float32, device=dev)
+    dlp = torch.empty(rows, dtype=torch.float32, device=dev)
+    grad = torch.empty_like(logit_new) if ctx.needs_input_grad[0] else None
+    return out, lse, dlp, grad
+
+
+def _vocab_saved(ctx, logit_new, action, lse, dlp, grad, dt, out):
+    ctx.save_for_backward(logit_new, action, lse, dlp)
+    ctx.dt = dt
+    ctx.spec = grad
+    ctx.set_materialize_grads(False)
+    loss, approx_kl, clipfrac = out[0], out[1], out[2]
+    ctx.mark_non_differentiable(approx_kl, clipfrac)
+    return loss, approx_kl, clipfrac
+
+
+def _vocab_backward(ctx, g_loss):
+    if g_loss is None:
+        return None
+    logit_new, action, lse, dlp = ctx.saved_tensors
+    keep, (pg, ) = _grads(g_loss)
+    grad, skip = _unit_grad(ctx, (), lambda: torch.empty_like(logit_new))
+    with on_device(logit_new.device):
+        rc = lib().b200rl_token_logp_bwd(ctx.dt, ptr(logit_new), ptr(action), ptr(lse), ptr(dlp), pg, skip, lse.numel(),
+                                         logit_new.shape[-1], ptr(grad), stream_ptr())
+    _lib.check(rc, 'b200rl_token_logp_bwd')
+    return grad
+
+
+class TokenLogProbFunction(torch.autograd.Function):
+    """log p(index) under softmax(logits) per token (ding/rl_utils/log_prob_utils.py): logits (rows, V) fp32 or bf16,
+    index (rows) -> fp32 (rows).  Backward: d / d logits = g * (onehot - softmax), one launch."""
+
+    @staticmethod
+    def forward(ctx, logits, index, dt):
+        rows, V = logits.shape
+        lp = torch.empty(rows, dtype=torch.float32, device=logits.device)
+        lse = torch.empty(rows, dtype=torch.float32, device=logits.device)
+        with on_device(logits.device):
+            rc = lib().b200rl_token_logp_fwd(dt, ptr(logits), ptr(index), rows, V, ptr(lp), ptr(lse), stream_ptr())
+        _lib.check(rc, 'b200rl_token_logp_fwd')
+        ctx.save_for_backward(logits, index, lse)
+        ctx.dt = dt
+        return lp
+
+    @staticmethod
+    def backward(ctx, g):
+        logits, index, lse = ctx.saved_tensors
+        g = g.float().contiguous()
+        grad = torch.empty_like(logits)
+        with on_device(logits.device):
+            rc = lib().b200rl_token_logp_bwd(ctx.dt, ptr(logits), ptr(index), ptr(lse), ptr(g), None, 0, lse.numel(),
+                                             logits.shape[-1], ptr(grad), stream_ptr())
+        _lib.check(rc, 'b200rl_token_logp_bwd')
+        return grad, None, None
+
+
+def token_head_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
+    """The GRPO (``lp_ref`` given) or RLOO head on per-token log-probabilities (B, S) fp32 from a caller's own
+    log_prob_fn: returns (loss, approx_kl, clipfrac); the gradient reaches ``lp_new`` (b200rl_scale of the saved
+    unit-upstream gradient), and through it whatever computed it."""
+    dev = lp_new.device
+    B, S = lp_new.shape
+    out = torch.empty(3, dtype=torch.float32, device=dev)
+    dlp = torch.empty(B, S, dtype=torch.float32, device=dev)
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_token_head_fwd(ptr(lp_new), ptr(lp_old), ptr(lp_ref), ptr(adv), ptr(reward),
+                                         0 if reward is None else reward.shape[0], ptr(weight), B, S, clip_ratio, beta,
+                                         ptr(out), ptr(dlp), ptr(ws), ws.numel() * 4, stream_ptr())
+    _lib.check(rc, 'b200rl_token_head_fwd')
+    loss = out[0]
+    if lp_new.requires_grad and torch.is_grad_enabled():
+        loss = _ScaleSaved.apply(lp_new, loss, dlp)
+    return loss, out[1], out[2]

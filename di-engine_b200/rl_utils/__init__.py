@@ -5,6 +5,8 @@ from .acer import acer_policy_error, acer_trust_region_update, acer_value_error
 from .fused import gae_ppo_error
 from .happo import (happo_data, happo_error, happo_error_continuous, happo_policy_error_continuous, happo_info, happo_loss, happo_policy_data, happo_policy_error, happo_policy_loss,
                     happo_value_data, happo_value_error)
+from .grpo import grpo_info, grpo_policy_data, grpo_policy_error
+from .log_prob_utils import efficient_method, less_efficient_method, naive_method
 from .gae import gae, gae_data, gae_returns, gae_returns_out, shape_fn_gae
 from .ppo import (normalize_advantage, ppo_data, ppo_data_continuous, ppo_error, ppo_error_adv_norm, ppo_error_continuous, ppo_info, ppo_loss,
                   ppo_policy_data, ppo_policy_data_continuous, ppo_policy_error, ppo_policy_error_continuous, ppo_policy_loss,
@@ -20,6 +22,7 @@ from .ppg import ppg_data, ppg_joint_error, ppg_joint_loss
 from .quantile import (fqf_nstep_td_data, fqf_nstep_td_error, iqn_nstep_td_data, iqn_nstep_td_error, qrdqn_nstep_td_data,
                        qrdqn_nstep_td_error)
 from .retrace import compute_q_retraces
+from .rloo import rloo_info, rloo_policy_data, rloo_policy_error
 from .upgo import tb_cross_entropy, upgo_loss, upgo_returns
 from .value_rescale import value_inv_transform, value_transform
 from .vtrace import (impala_reshape_data, shape_fn_vtrace_discrete_action, vtrace_data, vtrace_error_continuous_action,
@@ -46,3 +49,9 @@ HOT_PATH_TYPES = [
     'happo_data', 'happo_policy_data', 'happo_value_data', 'happo_loss', 'happo_policy_loss', 'happo_info', 'ppg_data', 'ppg_joint_loss',
     'dqfd_nstep_td_data', 'm_q_1step_td_data', 'q_v_1step_td_data', 'ppo_data_continuous', 'ppo_policy_data_continuous'
 ]
+# the language-model losses (ding/rl_utils/{grpo,rloo,log_prob_utils}.py), listed apart from the classic hot path above:
+# the test suite's reference loader covers only the files those lists come from.  install() rebinds both lists
+LM_HOT_PATH_FUNCTIONS = [
+    'grpo_policy_error', 'rloo_policy_error', 'naive_method', 'efficient_method', 'less_efficient_method'
+]
+LM_HOT_PATH_TYPES = ['grpo_policy_data', 'grpo_info', 'rloo_policy_data', 'rloo_info']

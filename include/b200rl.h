@@ -473,6 +473,46 @@ B200RL_API int b200rl_p2p_drain_mean(const unsigned long long* mailbox_ptrs_dev,
  * (or B200RL_ERR_ARG for any other value).  Test hook, process-wide: runs each kernel on every shape. */
 B200RL_API int b200rl_gae_ppo_set_impl(int impl);
 
+/* ---- language-model policy losses on vocabulary-scale logits (csrc/vocab.cu) -------------------------------------
+ * grpo_policy_error (ding/rl_utils/grpo.py), rloo_policy_error (ding/rl_utils/rloo.py) and the per-token log-probability
+ * methods of ding/rl_utils/log_prob_utils.py.  Logits are (rows, V) row-major in the dtype given by `dtype`
+ * (B200RL_DTYPE_F32 or B200RL_DTYPE_BF16; every logit pointer of a call in that dtype, 16-byte aligned); all arithmetic is
+ * fp32.  Rows are the B*S tokens, row = b*S + s.  action / index: (rows) int64.  weight nullable (B, S) = ones.
+ *
+ * b200rl_grpo_fwd_grad: logit_new, logit_old, logit_ref (B, S, V), adv (B).  out3 = {loss, approx_kl, clipfrac}:
+ *   loss = mean_b(sum_s(w * l) / sum_s(w)), l = -min(r*adv, clamp(r, 1-clip, 1+clip)*adv) + beta*(exp(d) - d - 1),
+ *   r = exp(lp_new - lp_old), d = lp_ref - lp_new; approx_kl = mean(lp_old - lp_new); clipfrac = mean(r > 1+clip or
+ *   r < 1-clip).  Saved for the backward: lse_new (rows) = logsumexp(logit_new[row]) and dlogp_unit (rows) =
+ *   d loss / d lp_new for a unit upstream gradient.  grad_logit_new (nullable = no gradient; dtype of the logits) =
+ *   dlogp_unit[row] * (onehot(a) - softmax(logit_new[row])).
+ * b200rl_rloo_fwd_grad: as GRPO without logit_ref and beta; the advantage of row b is computed from reward (K, B / K):
+ *   (k, j) = (b / (B/K), b % (B/K)), adv = r[k, j] - (sum_k' r[k', j] - r[k, j]) / (K - 1).
+ * b200rl_token_logp_fwd: logp (rows) = z[a] - logsumexp(z), lse (rows) saved for the backward.
+ * b200rl_token_logp_bwd: grad_logits[row] = g * dlogp[row] * (onehot(a) - softmax(z)), g = *g_scale (nullable = 1).
+ *   skip_if_unit != 0: grad_logits already holds the gradient for g = 1 (written by a forward above); the launch returns
+ *   at once on the device when *g_scale == 1, else it recomputes -- the backward of GRPO / RLOO, with no host sync.
+ * b200rl_token_head_fwd: the GRPO (logp_ref != null, adv) or RLOO (logp_ref null, reward / K) head alone on per-token
+ *   log-probabilities (B, S) fp32 that the caller computed; out3 and dlogp_unit as above (backward = b200rl_scale). */
+#define B200RL_DTYPE_F32 0
+#define B200RL_DTYPE_BF16 1
+B200RL_API int b200rl_grpo_fwd_grad(int dtype, const void* logit_new, const void* logit_old, const void* logit_ref,
+                         const long long* action, const float* adv, const float* weight, long long B, long long S,
+                         long long V, double clip_ratio, double beta, float* out3, float* lse_new, float* dlogp_unit,
+                         void* grad_logit_new, float* workspace, size_t workspace_bytes, void* stream);
+B200RL_API int b200rl_rloo_fwd_grad(int dtype, const void* logit_new, const void* logit_old, const long long* action,
+                         const float* reward, long long K, const float* weight, long long B, long long S, long long V,
+                         double clip_ratio, float* out3, float* lse_new, float* dlogp_unit, void* grad_logit_new,
+                         float* workspace, size_t workspace_bytes, void* stream);
+B200RL_API int b200rl_token_logp_fwd(int dtype, const void* logits, const long long* index, long long rows, long long V,
+                          float* logp, float* lse, void* stream);
+B200RL_API int b200rl_token_logp_bwd(int dtype, const void* logits, const long long* index, const float* lse,
+                          const float* dlogp, const float* g_scale, int skip_if_unit, long long rows, long long V,
+                          void* grad_logits, void* stream);
+B200RL_API int b200rl_token_head_fwd(const float* logp_new, const float* logp_old, const float* logp_ref, const float* adv,
+                          const float* reward, long long K, const float* weight, long long B, long long S,
+                          double clip_ratio, double beta, float* out3, float* dlogp_unit, float* workspace,
+                          size_t workspace_bytes, void* stream);
+
 /* ---- data-parallel exchange step: one-shot all-reduce (mean) of n <= 8 floats over NVLink peer memory -----------
  * Replaces the small-message NCCL all-reduce of the packed loss scalars (mean of rank means,
  * ding/utils/pytorch_ddp_dist_helper.py:38-47).  mailbox_ptrs_dev: device array of `world` pointers, entry r = the
