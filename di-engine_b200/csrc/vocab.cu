@@ -33,11 +33,25 @@
 //
 // Loss sums (loss, approx_kl, clipfrac): per-CTA partials (grid_store_partials) added in a fixed order by
 // finalize_sums_kernel -- deterministic, no atomics, no host sync.
+//
+// PPO on token rows (ppo_policy_error / the policy part of ppo_error, ding/rl_utils/ppo.py:143-230, at (B, S, V)): MODE =
+// VM_PPO + PPO_ENT (entropy bonus) + PPO_KL (logit_pretrained given), so the common RLHF call (no entropy, 2 or 3 streams)
+// carries neither the entropy accumulator nor the third stream.  Next to logit_new's online max / sum of exp the pass keeps
+// t = sum e^(z - r) * max(z - r, -FLT_MAX) (r the running max, rescaled with it like s), so H = log s - t / s reuses the
+// exponentials already taken.  The row epilogue runs surrogate / kl_term (ppo_math.cuh) and, for the upstream gradients
+// the call site expects (g_pol, g_ent, g_kl: its device-resident record), writes
+// d / d logit_new = c_act * (onehot(a) - p) - c_ent * p * (log p + H), c_act = g_pol * (-w / M) * dsel * r + g_kl * dk / M,
+// c_ent = g_ent * w / M (M rows).  Saved per row: lse, H (entropy only) and the unit coefficients (-w / M) * dsel * r and
+// dk / M, from which VM_PPO_BWD recomputes the gradient for the actual upstream gradients (one read of logit_new, one
+// write) -- unless they are the ones the forward used, in which case it returns at once on the device.  Loss sums:
+// policy, entropy, kl, approx_kl, clipfrac, all over M.  Traffic: (3 + 1) * V * sizeof(T) per row with logit_pretrained,
+// (2 + 1) without -- the same streams and the same L2 re-read of logit_new as GRPO / RLOO.
 #include <cuda_bf16.h>
 #include <math.h>
 
 #include "../../include/b200rl.h"
 #include "common.cuh"
+#include "ppo_math.cuh"
 
 namespace b200rl {
 
@@ -45,6 +59,7 @@ constexpr int VOCAB_NT = 512;
 constexpr int VOCAB_HEAD_NT = 256;
 constexpr int VOCAB_SMEM_CAP = 220 * 1024;  // dynamic shared memory for the cached part of logit_new (227 KB opt-in max)
 constexpr int VM_GRPO = 0, VM_RLOO = 1, VM_LOGP = 2, VM_BWD = 3;
+constexpr int VM_PPO = 4, VM_PPO_BWD = 8, PPO_ENT = 1, PPO_KL = 2;  // VM_PPO + flags: 4..7; VM_PPO_BWD + PPO_ENT: 8, 9
 constexpr float kL2E = 1.4426950408889634f;
 
 // 16-byte vectors of T, widened to fp32
@@ -120,6 +135,48 @@ __device__ __forceinline__ void ms_merge(float& m, float& s, float m2, float s2)
     if (s2 != 0.f) s += s2 * exp2f((lse_ref(m2) - lse_ref(m)) * kL2E);
 }
 
+// ms_add with the entropy accumulator t = sum e^(z - r) * max(z - r, -FLT_MAX), r = lse_ref(max): a new max r' rescales
+// it as t <- alpha * (t + s * (r - r')), alpha = e^(r - r'), and -inf logits add 0 (Categorical.entropy's clamp)
+template <int N>
+__device__ __forceinline__ void mst_add(float& m, float& s, float& t, const float (&x)[N]) {
+    float mc = x[0];
+#pragma unroll
+    for (int i = 1; i < N; ++i) mc = fmaxf(mc, x[i]);
+    if (mc > m) {
+        if (s != 0.f) {
+            const float d = lse_ref(m) - lse_ref(mc), al = exp2f(d * kL2E);
+            t = al * fmaf(s, d, t);
+            s *= al;
+        }
+        m = mc;
+    }
+    const float r = lse_ref(m);
+    float e[N], u[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+        e[i] = exp2f((x[i] - r) * kL2E);
+        u[i] = e[i] * fmaxf(x[i] - r, kF32Min);
+    }
+#pragma unroll
+    for (int w = 1; w < N; w *= 2)
+#pragma unroll
+        for (int i = 0; i + w < N; i += 2 * w) e[i] += e[i + w], u[i] += u[i + w];
+    s += e[0];
+    t += u[0];
+}
+
+__device__ __forceinline__ void mst_merge(float& m, float& s, float& t, float m2, float s2, float t2) {
+    if (m2 > m) {
+        const float tm = m, ts = s, tt = t;
+        m = m2; s = s2; t = t2; m2 = tm; s2 = ts; t2 = tt;
+    }
+    if (s2 != 0.f) {
+        const float d = lse_ref(m2) - lse_ref(m), al = exp2f(d * kL2E);
+        s += s2 * al;
+        t += al * fmaf(s2, d, t2);
+    }
+}
+
 // The per-token head of grpo.py / rloo.py.  In: lp_new, lp_old, lp_ref (GRPO only), the row's advantage, the clamp
 // bounds fp32(1 - clip) / fp32(1 + clip), beta, and gt = d loss / d per_token_loss (the unit-upstream factor
 // (1 / B) / sum_s(w) * w).  Out: the per-token loss, the clip indicator and d loss / d lp_new.  Gradients follow torch:
@@ -179,11 +236,19 @@ struct VocabArgs {
     long long rows, S, V, Bp;
     int K, skip_if_unit, capv;  // capv: 16-byte vectors of logit_new kept in shared memory
     float lo, hi, beta, inv_b;
+    // PPO (VM_PPO*, VM_PPO_BWD*); adv is then per row and coef / coef_in the policy term's unit coefficient
+    float* ent;                // forward: entropy of logit_new per row (PPO_ENT); VM_PPO_BWD: read (null = no entropy)
+    float* coef_kl;            // forward: d kl_div / d lp_new per row (PPO_KL); VM_PPO_BWD: read (null = no KL)
+    const float *g_pol, *g_ent, *g_kl;  // forward: the expected upstream gradients; VM_PPO_BWD: the actual ones (null = 0)
+    float* g_used;             // forward: the upstream gradients its gradient was written for; VM_PPO_BWD: read (nullable)
+    float* g_hint;             // VM_PPO_BWD: refreshed with the actual upstream gradients (nullable)
+    float dual_clip, inv_m;    // dual_clip <= 0: off; inv_m = 1 / rows
+    int kl_type;
 };
 
-template <int NR, bool CACHE, class T>
+template <int NR, bool CACHE, class T, bool ENT = false>
 __device__ __forceinline__ void stream_vecs(const uint4* const (&p)[NR], int i, float (&m)[NR], float (&s)[NR],
-                                            uint4* cache, int capv) {
+                                            uint4* cache, int capv, float* t = nullptr) {
     constexpr int W = VecT<T>::W;
     uint4 u[NR];
 #pragma unroll
@@ -193,8 +258,34 @@ __device__ __forceinline__ void stream_vecs(const uint4* const (&p)[NR], int i, 
     for (int r = 0; r < NR; ++r) {
         float x[W];
         VecT<T>::unpack(u[r], x);
-        ms_add<W>(m[r], s[r], x);
+        if (ENT && r == 0) mst_add<W>(m[0], s[0], *t, x);
+        else ms_add<W>(m[r], s[r], x);
     }
+}
+
+// PPO upstream gradients {policy, entropy, kl} (null = 0).  They are read where they are used, once per row, rather than
+// held in registers across the row loop.
+template <bool ENT>
+__device__ __forceinline__ void ppo_g(const VocabArgs& a, float& gp, float& ge, float& gk) {
+    gp = a.g_pol ? *a.g_pol : 0.f;
+    ge = (ENT && a.g_ent) ? *a.g_ent : 0.f;
+    gk = a.g_kl ? *a.g_kl : 0.f;
+}
+
+// the backward's view of the PPO upstream gradients: refresh the call site's record and report whether the forward
+// already wrote the gradient for exactly these values
+template <bool ENT>
+__device__ __forceinline__ bool ppo_upstream(const VocabArgs& a) {
+    float gp, ge, gk;
+    ppo_g<ENT>(a, gp, ge, gk);
+    if (a.g_hint && blockIdx.x == 0 && threadIdx.x == 0) {
+        a.g_hint[0] = gp;
+        if (ENT) a.g_hint[2] = ge;
+        a.g_hint[3] = gk;
+    }
+    return a.g_used && __float_as_uint(a.g_used[0]) == __float_as_uint(gp) &&
+           (!ENT || __float_as_uint(a.g_used[2]) == __float_as_uint(ge)) &&
+           (!a.coef_kl || __float_as_uint(a.g_used[3]) == __float_as_uint(gk));
 }
 
 template <class T, int MODE>
@@ -202,12 +293,17 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
     pdl_prologue();
     using V_ = VecT<T>;
     constexpr int W = V_::W;
-    constexpr int NR = MODE == VM_GRPO ? 3 : (MODE == VM_RLOO ? 2 : 1);
-    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO;
+    constexpr bool PPO = MODE >= VM_PPO && MODE < VM_PPO_BWD, PBWD = MODE >= VM_PPO_BWD;
+    constexpr bool ENT = (PPO || PBWD) && (MODE & PPO_ENT), KL = PPO && (MODE & PPO_KL);
+    constexpr bool BWD = MODE == VM_BWD || PBWD;
+    constexpr int NR = MODE == VM_GRPO ? 3 : (MODE == VM_RLOO ? 2 : (PPO ? (KL ? 3 : 2) : 1));
+    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO;
+    constexpr int NP = PPO ? 5 : 3;
     extern __shared__ uint4 s_row[];
     __shared__ float s_m[NR][VOCAB_NT / 32], s_s[NR][VOCAB_NT / 32], s_w[VOCAB_NT / 32];
     __shared__ float s_c, s_lse;
     __shared__ long long s_a;
+    __shared__ float s_t[ENT ? VOCAB_NT / 32 : 1], s_ce, s_h;  // PPO entropy: t partials, c_ent, H
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const long long V = a.V;
     const bool want_grad = a.grad != nullptr;
@@ -216,7 +312,13 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
         if (a.g) gscale = *a.g;
         if (a.skip_if_unit && gscale == 1.f) return;  // the forward launch already wrote exactly this gradient
     }
-    float part[3] = {0.f, 0.f, 0.f};  // thread 0: loss, approx_kl, clipfrac partial sums of this CTA's rows
+    if (PBWD && ppo_upstream<ENT>(a)) return;
+    if (PPO && want_grad && blockIdx.x == 0 && tid == 0) {  // record the upstream gradients the forward writes for
+        float gp, ge, gk;
+        ppo_g<ENT>(a, gp, ge, gk);
+        a.g_used[0] = gp; a.g_used[1] = 0.f; a.g_used[2] = ge; a.g_used[3] = KL ? gk : 0.f;
+    }
+    float part[NP] = {0.f, 0.f, 0.f};  // thread 0: the loss partial sums of this CTA's rows (loss, approx_kl, clipfrac; PPO: 5)
     float w_tot = (float)a.S;  // thread 0: sum_s w[b, s] of the current row's sequence (S without weights)
     for (long long row = blockIdx.x; row < a.rows; row += gridDim.x) {
         const size_t off = (size_t)row * (size_t)V;
@@ -232,30 +334,40 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
             rp[r] = reinterpret_cast<const T*>(a.x[r]) + off;
             vp[r] = reinterpret_cast<const uint4*>(rp[r] + h);
         }
-        float c = 0.f, lse = 0.f;
+        float c = 0.f, lse = 0.f, ce = 0.f, H = 0.f;  // ce, H: PPO entropy term
         long long act = 0;
         if (MODE == VM_BWD) {
             c = gscale * a.coef_in[row];
             lse = a.lse[row];
             act = a.action[row];
+        } else if (PBWD) {
+            float gp, ge, gk;
+            ppo_g<ENT>(a, gp, ge, gk);
+            c = gp * a.coef_in[row] + (a.coef_kl ? gk * a.coef_kl[row] : 0.f);
+            if (ENT) {
+                ce = ge * (a.weight ? a.weight[row] : 1.f) * a.inv_m;
+                H = a.ent[row];
+            }
+            lse = a.lse[row];
+            act = a.action[row];
         } else {
-            float m[NR], s[NR];
+            float m[NR], s[NR], t = 0.f;  // t: PPO entropy accumulator of logit_new
 #pragma unroll
             for (int r = 0; r < NR; ++r) m[r] = -INFINITY, s[r] = 0.f;
             const bool cache = LOSS && want_grad;
             int i = tid;
             for (; i + VOCAB_NT < nvec; i += 2 * VOCAB_NT) {
                 if (cache) {
-                    stream_vecs<NR, true, T>(vp, i, m, s, s_row, a.capv);
-                    stream_vecs<NR, true, T>(vp, i + VOCAB_NT, m, s, s_row, a.capv);
+                    stream_vecs<NR, true, T, ENT>(vp, i, m, s, s_row, a.capv, &t);
+                    stream_vecs<NR, true, T, ENT>(vp, i + VOCAB_NT, m, s, s_row, a.capv, &t);
                 } else {
-                    stream_vecs<NR, false, T>(vp, i, m, s, s_row, 0);
-                    stream_vecs<NR, false, T>(vp, i + VOCAB_NT, m, s, s_row, 0);
+                    stream_vecs<NR, false, T, ENT>(vp, i, m, s, s_row, 0, &t);
+                    stream_vecs<NR, false, T, ENT>(vp, i + VOCAB_NT, m, s, s_row, 0, &t);
                 }
             }
             if (i < nvec) {
-                if (cache) stream_vecs<NR, true, T>(vp, i, m, s, s_row, a.capv);
-                else stream_vecs<NR, false, T>(vp, i, m, s, s_row, 0);
+                if (cache) stream_vecs<NR, true, T, ENT>(vp, i, m, s, s_row, a.capv, &t);
+                else stream_vecs<NR, false, T, ENT>(vp, i, m, s, s_row, 0, &t);
             }
             // the unaligned head and tail, < 16 bytes each
             for (long long j = tid; j < h + (V - tail0); j += VOCAB_NT) {
@@ -263,13 +375,15 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
 #pragma unroll
                 for (int r = 0; r < NR; ++r) {
                     const float x[1] = {V_::to_f(rp[r][e])};
-                    ms_add<1>(m[r], s[r], x);
+                    if (ENT && r == 0) mst_add<1>(m[0], s[0], t, x);
+                    else ms_add<1>(m[r], s[r], x);
                 }
             }
             float wsum = 0.f;
             // a CTA's rows step by gridDim.x (< S at language-model sizes): it sums a sequence's weights once per visit to
             // that sequence, not once per token
-            const bool new_seq = LOSS && a.weight && (row < gridDim.x || row / a.S != (row - gridDim.x) / a.S);
+            const bool new_seq = (MODE == VM_GRPO || MODE == VM_RLOO) && a.weight &&
+                                 (row < gridDim.x || row / a.S != (row - gridDim.x) / a.S);
             if (new_seq) {
                 const float* wr = a.weight + (row / a.S) * a.S;
                 for (long long j = tid; j < a.S; j += VOCAB_NT) wsum += wr[j];
@@ -279,10 +393,12 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) {
                     const float m2 = __shfl_down_sync(0xffffffffu, m[r], o), s2 = __shfl_down_sync(0xffffffffu, s[r], o);
-                    ms_merge(m[r], s[r], m2, s2);
+                    if (ENT && r == 0) mst_merge(m[0], s[0], t, m2, s2, __shfl_down_sync(0xffffffffu, t, o));
+                    else ms_merge(m[r], s[r], m2, s2);
                 }
                 if (lane == 0) s_m[r][wid] = m[r], s_s[r][wid] = s[r];
             }
+            if (ENT && lane == 0) s_t[wid] = t;
             if (new_seq) {
                 wsum = warp_sum(wsum);
                 if (lane == 0) s_w[wid] = wsum;
@@ -295,14 +411,45 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
 #pragma unroll
                 for (int r = 0; r < NR; ++r) {
                     float mm = s_m[r][0], ss = s_s[r][0];
-                    for (int w = 1; w < VOCAB_NT / 32; ++w) ms_merge(mm, ss, s_m[r][w], s_s[r][w]);
+                    if (ENT && r == 0) {
+                        float tt = s_t[0];
+                        for (int w = 1; w < VOCAB_NT / 32; ++w) mst_merge(mm, ss, tt, s_m[0][w], s_s[0][w], s_t[w]);
+                        H = logf(ss) - tt / ss;
+                    } else {
+                        for (int w = 1; w < VOCAB_NT / 32; ++w) ms_merge(mm, ss, s_m[r][w], s_s[r][w]);
+                    }
                     const float l = logf(ss) + lse_ref(mm);
                     if (r == 0) lse = l;
                     lp[r] = ok ? V_::to_f(rp[r][act]) - l : __int_as_float(0x7fc00000);
                 }
                 a.lse[row] = lse;
                 if (MODE == VM_LOGP) a.lp[row] = lp[0];
-                if (LOSS) {
+                if constexpr (PPO) {
+                    const float w = a.weight ? a.weight[row] : 1.f;
+                    const float ratio = expf(lp[0] - lp[1]);
+                    float dsel, dk = 0.f, klv = 0.f;
+                    const float sel = surrogate(ratio, a.adv[row], a.lo, a.hi, a.dual_clip, dsel);
+                    const float cp = -w * a.inv_m * dsel * ratio;  // d policy_loss / d lp_new
+                    a.coef[row] = cp;
+                    if (KL) {
+                        klv = kl_term(lp[0] - lp[NR - 1], a.kl_type, dk);
+                        a.coef_kl[row] = dk * a.inv_m;  // d kl_div / d lp_new
+                    }
+                    if (ENT) a.ent[row] = H;
+                    if (want_grad) {
+                        float gp, ge, gk;
+                        ppo_g<ENT>(a, gp, ge, gk);
+                        c = gp * cp + (KL ? gk * dk * a.inv_m : 0.f);
+                        ce = ge * w * a.inv_m;
+                    }
+                    part[0] -= sel * w;
+                    part[1] += H * w;
+                    part[2] += klv;
+                    part[3] += lp[1] - lp[0];
+                    part[4] += (ratio > a.hi || ratio < a.lo) ? 1.f : 0.f;
+                    s_ce = ce;
+                    s_h = H;
+                } else if (LOSS) {
                     const long long b = row / a.S;
                     if (new_seq) {
                         w_tot = 0.f;
@@ -329,30 +476,46 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
             c = s_c;
             lse = s_lse;
             act = s_a;
+            if (ENT) ce = s_ce, H = s_h;
         }
-        // d / d logit_new[row] = c * (onehot(a) - softmax)
+        // d / d logit_new[row] = c * (onehot(a) - softmax) [PPO entropy: - ce * p * (max(log p, -FLT_MAX) + H)]
         T* gr = reinterpret_cast<T*>(a.grad) + off;
         uint4* gv = reinterpret_cast<uint4*>(gr + h);
         for (int i = tid; i < nvec; i += VOCAB_NT) {
-            const uint4 u = (LOSS && i < a.capv) ? s_row[i] : (MODE == VM_BWD ? __ldcs(vp[0] + i) : __ldg(vp[0] + i));
+            const uint4 u = (LOSS && i < a.capv) ? s_row[i] : (BWD ? __ldcs(vp[0] + i) : __ldg(vp[0] + i));
             float x[W];
             V_::unpack(u, x);
             const long long e0 = h + (long long)i * W;
 #pragma unroll
-            for (int k = 0; k < W; ++k) x[k] = c * ((e0 + k == act ? 1.f : 0.f) - exp2f((x[k] - lse) * kL2E));
+            for (int k = 0; k < W; ++k) {
+                if (ENT) {
+                    const float z = x[k] - lse, p = exp2f(z * kL2E);
+                    x[k] = c * ((e0 + k == act ? 1.f : 0.f) - p) - ce * p * (fmaxf(z, kF32Min) + H);
+                } else {
+                    x[k] = c * ((e0 + k == act ? 1.f : 0.f) - exp2f((x[k] - lse) * kL2E));
+                }
+            }
             __stcs(gv + i, V_::pack(x));
         }
         for (long long j = tid; j < h + (V - tail0); j += VOCAB_NT) {
             const long long e = j < h ? j : tail0 + (j - h);
             const float x = V_::to_f(rp[0][e]);
-            gr[e] = V_::from_f(c * ((e == act ? 1.f : 0.f) - exp2f((x - lse) * kL2E)));
+            if (ENT) {
+                const float z = x - lse, p = exp2f(z * kL2E);
+                gr[e] = V_::from_f(c * ((e == act ? 1.f : 0.f) - p) - ce * p * (fmaxf(z, kF32Min) + H));
+            } else {
+                gr[e] = V_::from_f(c * ((e == act ? 1.f : 0.f) - exp2f((x - lse) * kL2E)));
+            }
         }
         if (LOSS) __syncthreads();  // s_row and s_c are rewritten by the next row
     }
     if (LOSS) {
-        float v[3] = {0.f, 0.f, 0.f};
+        float v[NP] = {0.f, 0.f, 0.f};
         if (tid == 0) v[0] = part[0], v[1] = part[1], v[2] = part[2];
-        grid_store_partials<3, VOCAB_NT>(v, a.ws);
+        if constexpr (PPO) {
+            if (tid == 0) v[3] = part[3], v[4] = part[4];
+        }
+        grid_store_partials<NP, VOCAB_NT>(v, a.ws);
     }
 }
 
@@ -405,7 +568,9 @@ bool aligned_logits(const void* p) { return p && aligned16(p); }
 template <class T, int MODE>
 int launch_rows(VocabArgs& a, float* out3, size_t ws_bytes, long long B, cudaStream_t st) {
     constexpr auto kern = vocab_rows_kernel<T, MODE>;
-    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO;
+    constexpr bool PPO = MODE >= VM_PPO && MODE < VM_PPO_BWD;
+    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO;
+    constexpr int NP = PPO ? 5 : 3;
     const long long nvec_max = (a.V * (long long)sizeof(T) + 15) / 16;
     a.capv = (LOSS && a.grad) ? (int)min(nvec_max, (long long)(VOCAB_SMEM_CAP / 16)) : 0;
     const size_t smem = (size_t)a.capv * 16;
@@ -413,13 +578,17 @@ int launch_rows(VocabArgs& a, float* out3, size_t ws_bytes, long long B, cudaStr
     if (int rc = resident_ctas<kern>(VOCAB_NT, smem, sms, per_sm)) return rc;
     long long grid = (long long)sms * per_sm;
     if (grid > a.rows) grid = a.rows;
-    if (LOSS && !ws_partials_fit(grid * 3, ws_bytes)) return B200RL_ERR_WORKSPACE;
+    if (LOSS && !ws_partials_fit(grid * NP, ws_bytes)) return B200RL_ERR_WORKSPACE;
     if (int rc = launch_k(kern, (int)grid, VOCAB_NT, smem, st, a)) return rc;
     if (!LOSS) return B200RL_OK;
     FinalizeArgs fa{};
-    fa.scale[0] = 1.0 / (double)B;
-    fa.scale[1] = fa.scale[2] = 1.0 / (double)a.rows;
-    fa.k = 3;
+    if (PPO) {  // policy, entropy, kl, approx_kl, clipfrac: means over the rows
+        for (int k = 0; k < 5; ++k) fa.scale[k] = 1.0 / (double)a.rows;
+    } else {
+        fa.scale[0] = 1.0 / (double)B;
+        fa.scale[1] = fa.scale[2] = 1.0 / (double)a.rows;
+    }
+    fa.k = NP;
     fa.n_blocks = (int)grid;
     return launch_finalize(a.ws, out3, fa, st);
 }
@@ -472,6 +641,60 @@ extern "C" int b200rl_rloo_fwd_grad(int dtype, const void* logit_new, const void
     a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio);
     a.inv_b = (float)(1.0 / (double)B);
     return launch_dtype<VM_RLOO>(dtype, a, out3, workspace_bytes, B, (cudaStream_t)stream);
+}
+
+extern "C" int b200rl_ppo_lm_fwd_grad(int dtype, const void* logit_new, const void* logit_old,
+                                      const void* logit_pretrained, const long long* action, const float* adv,
+                                      const float* weight, long long rows, long long V, double clip_ratio,
+                                      double dual_clip, int kl_type, int entropy, const float* g_expected, float* g_used,
+                                      float* out5, float* lse_new, float* entropy_row, float* dlogp_policy,
+                                      float* dlogp_kl, void* grad_logit_new, float* workspace, size_t workspace_bytes,
+                                      void* stream) {
+    const bool kl = logit_pretrained != nullptr;
+    if (!sizes_ok(rows, 1, V) || !aligned_logits(logit_new) || !aligned_logits(logit_old) ||
+        (kl && (!aligned16(logit_pretrained) || !dlogp_kl || kl_type < 1 || kl_type > 3)) || !action || !adv ||
+        !out5 || !lse_new || !dlogp_policy || (entropy && !entropy_row) || !workspace ||
+        (grad_logit_new && (!aligned16(grad_logit_new) || !g_expected || !g_used)))
+        return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logit_new; a.x[1] = logit_old; a.x[2] = logit_pretrained;
+    a.action = action; a.adv = adv; a.weight = weight;
+    a.lse = lse_new; a.coef = dlogp_policy; a.coef_kl = dlogp_kl; a.ent = entropy_row; a.grad = grad_logit_new;
+    a.ws = workspace;
+    if (g_expected) a.g_pol = g_expected, a.g_ent = g_expected + 2, a.g_kl = g_expected + 3;
+    a.g_used = g_used;
+    a.rows = rows; a.S = 1; a.V = V;
+    a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio); a.dual_clip = (float)dual_clip;
+    a.kl_type = kl_type; a.inv_m = (float)(1.0 / (double)rows);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int mode = VM_PPO + (entropy ? PPO_ENT : 0) + (kl ? PPO_KL : 0);
+    switch (mode) {
+        case VM_PPO: return launch_dtype<VM_PPO>(dtype, a, out5, workspace_bytes, rows, st);
+        case VM_PPO + PPO_ENT: return launch_dtype<VM_PPO + PPO_ENT>(dtype, a, out5, workspace_bytes, rows, st);
+        case VM_PPO + PPO_KL: return launch_dtype<VM_PPO + PPO_KL>(dtype, a, out5, workspace_bytes, rows, st);
+        default: return launch_dtype<VM_PPO + PPO_ENT + PPO_KL>(dtype, a, out5, workspace_bytes, rows, st);
+    }
+}
+
+extern "C" int b200rl_ppo_lm_bwd(int dtype, const void* logit_new, const long long* action, const float* weight,
+                                 long long rows, long long V, const float* lse_new, const float* entropy_row,
+                                 const float* dlogp_policy, const float* dlogp_kl, const float* g_policy,
+                                 const float* g_entropy, const float* g_kl, const float* g_used, float* g_hint,
+                                 void* grad_logit_new, void* stream) {
+    if (!sizes_ok(rows, 1, V) || !aligned_logits(logit_new) || !action || !lse_new || !dlogp_policy ||
+        !grad_logit_new || !aligned16(grad_logit_new))
+        return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logit_new; a.action = action; a.weight = weight;
+    a.lse = const_cast<float*>(lse_new); a.ent = const_cast<float*>(entropy_row); a.coef_in = dlogp_policy;
+    a.coef_kl = const_cast<float*>(dlogp_kl);
+    a.g_pol = g_policy; a.g_ent = g_entropy; a.g_kl = g_kl; a.g_used = const_cast<float*>(g_used); a.g_hint = g_hint;
+    a.grad = grad_logit_new;
+    a.rows = rows; a.S = 1; a.V = V;
+    a.inv_m = (float)(1.0 / (double)rows);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (entropy_row) return launch_dtype<VM_PPO_BWD + PPO_ENT>(dtype, a, nullptr, 0, rows, st);
+    return launch_dtype<VM_PPO_BWD>(dtype, a, nullptr, 0, rows, st);
 }
 
 extern "C" int b200rl_token_logp_fwd(int dtype, const void* logits, const long long* index, long long rows, long long V,

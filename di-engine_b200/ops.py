@@ -1238,6 +1238,63 @@ class RLOOFunction(torch.autograd.Function):
         return (_vocab_backward(ctx, g_loss), ) + (None, ) * 6
 
 
+class PPOLMFunction(torch.autograd.Function):
+    """ppo_policy_error (ding/rl_utils/ppo.py:143-230) on token rows: logits (..., V) fp32 or bf16, action / adv / weight
+    over the same rows.  Outputs: policy_loss, entropy_loss, kl_div (differentiable; the gradient reaches logit_new only)
+    and the raw result vector {policy, entropy, kl, approx_kl, clipfrac} (non differentiable).  The forward launch also
+    writes d / d logit_new for the upstream gradients the call site's record ``hint_kind`` expects (its policy, entropy and
+    kl slots); ``backward`` hands that buffer to autograd after a launch that returns at once on the device when the
+    expectation held, and otherwise recomputes from the saved per-row values -- PPOFunction's scheme, at vocabulary scale."""
+
+    @staticmethod
+    def forward(ctx, logit_new, logit_old, logit_pre, action, adv, weight, dt, clip_ratio, dual_clip, kl_type, entropy,
+                hint_kind):
+        dev = logit_new.device
+        V = logit_new.shape[-1]
+        rows = logit_new.numel() // V
+        out = torch.empty(5, dtype=torch.float32, device=dev)
+        lse = torch.empty(rows, dtype=torch.float32, device=dev)
+        ent = torch.empty(rows, dtype=torch.float32, device=dev) if entropy else None
+        dpol = torch.empty(rows, dtype=torch.float32, device=dev)
+        dkl = torch.empty(rows, dtype=torch.float32, device=dev) if logit_pre is not None else None
+        want = ctx.needs_input_grad[0]
+        grad = torch.empty_like(logit_new) if want else None
+        g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
+        ctx.hint_kind = hint_kind
+        with on_device(dev):
+            ws = workspace(dev)
+            rc = lib().b200rl_ppo_lm_fwd_grad(
+                dt, ptr(logit_new), ptr(logit_old), ptr(logit_pre), ptr(action), ptr(adv), ptr(weight), rows, V,
+                clip_ratio, dual_clip, kl_type, 1 if entropy else 0, ptr(ppo_hint(dev, hint_kind)) if want else None,
+                ptr(g_used), ptr(out), ptr(lse), ptr(ent), ptr(dpol), ptr(dkl), ptr(grad), ptr(ws), ws.numel() * 4,
+                stream_ptr())
+        _lib.check(rc, 'b200rl_ppo_lm_fwd_grad')
+        ctx.save_for_backward(logit_new, action, weight, lse, ent, dpol, dkl)
+        ctx.dt = dt
+        ctx.spec = (grad, g_used) if want else None
+        ctx.mark_non_differentiable(out)
+        return out[0], out[1], out[2], out
+
+    @staticmethod
+    def backward(ctx, g_p, g_e, g_k, _g_out):
+        logit_new, action, weight, lse, ent, dpol, dkl = ctx.saved_tensors
+        dev = logit_new.device
+        keep, (pp, pe, pk) = _grads(g_p, g_e, g_k)
+        spec = _forward_grads(ctx)
+        if spec is not None:  # valid if the expectation held; the kernel checks on the device
+            grad, g_used = spec
+            p_used, p_hint = ptr(g_used), ptr(ppo_hint(dev, ctx.hint_kind))
+        else:  # a repeated backward: null g_used / hint -> the kernel recomputes
+            grad, p_used, p_hint = torch.empty_like(logit_new), None, None
+        V = logit_new.shape[-1]
+        with on_device(dev):
+            rc = lib().b200rl_ppo_lm_bwd(ctx.dt, ptr(logit_new), ptr(action), ptr(weight), lse.numel(), V, ptr(lse),
+                                         ptr(ent), ptr(dpol), ptr(dkl), pp, pe, pk, p_used, p_hint, ptr(grad),
+                                         stream_ptr())
+        _lib.check(rc, 'b200rl_ppo_lm_bwd')
+        return (grad, ) + (None, ) * 11
+
+
 def _vocab_outputs(ctx, logit_new):
     dev = logit_new.device
     rows = logit_new.shape[0] * logit_new.shape[1]

@@ -37,6 +37,8 @@ def gae_ppo_error(
     logit_new, logit_old, action, value_new, value_old, _adv, return_, weight, logit_pretrained = ppo_in
     if logit_pretrained is not None and kl_type not in _KL_TYPES:
         raise ValueError(f"Unknown kl_type: {kl_type}")
+    if logit_new.dtype == torch.bfloat16:  # not even through the two-operator fallback
+        raise TypeError(_ppo._BF16_SHAPES)
 
     def fallback():
         adv = gae(gae_data(value, next_value, reward, done, traj_flag), gamma, lambda_)

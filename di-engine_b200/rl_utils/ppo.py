@@ -1,7 +1,9 @@
 """``ppo_error`` with the signature and namedtuples of ding/rl_utils/ppo.py:8-27,77-83 -- csrc/ppo.cu; and its two halves as
 the reference exposes them separately (PPG, off-policy PPO, the hybrid-action PPO): ``ppo_policy_error`` (ppo.py:143-230) and
 ``ppo_value_error`` (ppo.py:233-275).  The continuous-action forms ``ppo_error_continuous`` (ppo.py:278-374) and
-``ppo_policy_error_continuous`` (ppo.py:377-450) run on csrc/heads.cu."""
+``ppo_policy_error_continuous`` (ppo.py:377-450) run on csrc/heads.cu.  Language-model calls of ``ppo_policy_error`` /
+``ppo_error`` -- one logit row per advantage, bf16 logits or fp32 with V >= ``LM_MIN_VOCAB`` -- run on the vocabulary-scale
+row kernel of csrc/vocab.cu."""
 from collections import namedtuple
 from typing import Optional, Tuple
 
@@ -33,6 +35,14 @@ _KL_TYPES = {'k1': 1, 'k2': 2, 'k3': 3}
 # When True ``ppo_info`` carries 0-dim device tensors instead of python floats, so a training step never blocks on
 # the host (the reference's two ``.item()`` calls, ppo.py:218-220, are the only host syncs of its PPO loss).
 LAZY_INFO = False
+
+# fp32 logits with at least this many classes per row (and one row per advantage) run on the vocabulary-scale row kernel
+# (csrc/vocab.cu: 16-byte loads, one pass over each logit tensor) instead of csrc/ppo.cu's warp-per-row kernel, which was
+# written for action spaces of ~100; bf16 logits always do, no other PPO kernel reads them
+LM_MIN_VOCAB = 1024
+_BF16_SHAPES = ("di_engine_b200: bfloat16 logits are taken by ppo_policy_error and ppo_error with one logit row per "
+                "advantage -- logits (..., V) against action / adv / weight (...), e.g. (B, S, V) against (B, S) -- and "
+                "no advantage normalisation; every other PPO call needs float32 logits")
 
 
 def shape_fn_ppo(args, kwargs):
@@ -68,7 +78,15 @@ def ppo_error(
     Returns ``(ppo_loss, ppo_info)``: four differentiable 0-dim tensors (gradients reach ``logit_new`` and
     ``value_new``) and two python floats.
 
+    Language-model shapes (one logit row per advantage, bf16 logits or fp32 with V >= ``LM_MIN_VOCAB``) run as the
+    reference composes them: ``ppo_policy_error`` on csrc/vocab.cu plus ``ppo_value_error``.
     """
+    if _lm_path(data[0], data[5]):
+        logit_new, logit_old, action, value_new, value_old, adv, return_, weight, logit_pretrained = data
+        policy, info = _ppo_lm(ppo_policy_data(logit_new, logit_old, action, adv, weight, logit_pretrained), clip_ratio,
+                               dual_clip, True, kl_type, 'ppo')
+        value_loss = ppo_value_error(ppo_value_data(value_new, value_old, return_, weight), clip_ratio, use_value_clip)
+        return ppo_loss(policy.policy_loss, value_loss, policy.entropy_loss, policy.kl_div), info
     return _ppo_error(data, clip_ratio, use_value_clip, dual_clip, kl_type, 'ppo')
 
 
@@ -97,6 +115,8 @@ def _ppo_error(data, clip_ratio, use_value_clip, dual_clip, kl_type, _hint_kind,
     logit_new, logit_old, action, value_new, value_old, adv, return_, weight, logit_pretrained = data
     if logit_pretrained is not None and kl_type not in _KL_TYPES:
         raise ValueError(f"Unknown kl_type: {kl_type}")
+    if logit_new.dtype == torch.bfloat16:
+        raise TypeError(_BF16_SHAPES)
     dev = ops.compute_device(logit_new, value_new, logit_old)
     host_out = not logit_new.is_cuda
     N = logit_new.shape[-1]
@@ -232,8 +252,12 @@ def ppo_policy_error(
     Policy half of the PPO loss, drop-in for ding/rl_utils/ppo.py:143-230: ``(ppo_policy_loss(policy_loss, entropy_loss,
     kl_div), ppo_info)``.  Runs on the ``ppo_error`` kernel with a zero value head (value_new = value_old = return_ = 0
     contributes nothing and receives no gradient); its expected-upstream-gradient record is kept apart from
-    ``ppo_error``'s, so alternating the two never forces a recomputation.
+    ``ppo_error``'s, so alternating the two never forces a recomputation.  Language-model shapes -- logits (..., V) with
+    one row per advantage, e.g. (B, S, V) against (B, S) adv / action / weight, in bf16 or in fp32 with
+    V >= ``LM_MIN_VOCAB`` -- run on the vocabulary-scale row kernel of csrc/vocab.cu.
     """
+    if _lm_path(data[0], data[3]):
+        return _ppo_lm(data, clip_ratio, dual_clip, entropy_bonus, kl_type, 'policy')
     logit_new, logit_old, action, adv, weight, logit_pretrained = data
     zero = torch.zeros_like(adv)
     loss, info = _ppo_error(
@@ -242,6 +266,58 @@ def ppo_policy_error(
     )
     entropy = loss.entropy_loss if entropy_bonus else torch.tensor(0.0)  # ppo.py:203
     return ppo_policy_loss(loss.policy_loss, entropy, loss.kl_div), info
+
+
+def _lm_path(logit_new, adv):
+    """whether a ppo_policy_error / ppo_error call runs on csrc/vocab.cu: one logit row per advantage, and bf16 logits or
+    fp32 with V >= LM_MIN_VOCAB"""
+    if logit_new.dtype not in (torch.float32, torch.bfloat16) or logit_new.dim() < 1 or logit_new.shape[-1] == 0:
+        return False
+    V = logit_new.shape[-1]
+    return adv.numel() == logit_new.numel() // V and (logit_new.dtype == torch.bfloat16 or V >= LM_MIN_VOCAB)
+
+
+def _ppo_lm(data, clip_ratio, dual_clip, entropy_bonus, kl_type, hint_kind):
+    """ppo_policy_error on token rows (csrc/vocab.cu, ops.PPOLMFunction): the reference's plain means over all rows;
+    ``hint_kind`` is the call site's expected-upstream-gradient record, of which the policy, entropy and kl slots are read"""
+    assert dual_clip is None or dual_clip > 1.0, "dual_clip value must be greater than 1.0, but get value: {}".format(
+        dual_clip
+    )
+    logit_new, logit_old, action, adv, weight, logit_pretrained = data
+    if logit_pretrained is not None and kl_type not in _KL_TYPES:
+        raise ValueError(f"Unknown kl_type: {kl_type}")
+    logits = [logit_new, logit_old] + ([logit_pretrained] if logit_pretrained is not None else [])
+    dt = ops.logit_dtype(*logits)
+    V = logit_new.shape[-1]
+    rows = logit_new.numel() // V
+    for name, t_ in (('logit_old', logit_old), ('logit_pretrained', logit_pretrained), ('action', action)):
+        if t_ is not None and t_.numel() != (rows if name == 'action' else rows * V):
+            raise ValueError("ppo_policy_error: %s %s does not match logit_new %s" %
+                             (name, tuple(t_.shape), tuple(logit_new.shape)))
+    dev = ops.compute_device(*logits)
+    host_out = not logit_new.is_cuda
+    # logit_old / logit_pretrained get no gradient; weight and adv are read as fp32 whatever their dtype
+    xs = [ops.logits_c(ops.to_device(x, dev)) for x in logits]
+    xs[1:] = [x.detach() for x in xs[1:]]
+    ad = ops.to_device(adv.detach(), dev).float().contiguous()
+    w = None
+    if weight is not None:
+        w = ops.to_device(weight.detach(), dev).float()
+        w = (w if w.numel() == rows else w.expand_as(ad)).contiguous()
+    act = ops.i64c(ops.to_device(action, dev), V)
+    p, e, k, out = ops.PPOLMFunction.apply(
+        xs[0], xs[1], xs[2] if len(xs) > 2 else None, act, ad, w, dt, float(clip_ratio),
+        float(dual_clip) if dual_clip is not None else 0.0, _KL_TYPES.get(kl_type, 1), bool(entropy_bonus), hint_kind
+    )
+    if LAZY_INFO:
+        info = ppo_info(out[3], out[4])
+    else:
+        approx_kl, clipfrac = out[3:5].tolist()
+        info = ppo_info(approx_kl, clipfrac)
+    if host_out:
+        p, e, k = p.cpu(), e.cpu(), k.cpu()
+    entropy = e if entropy_bonus else torch.tensor(0.0)  # ppo.py:203
+    return ppo_policy_loss(p, entropy, k), info
 
 
 def ppo_policy_error_continuous(

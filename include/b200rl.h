@@ -492,7 +492,23 @@ B200RL_API int b200rl_gae_ppo_set_impl(int impl);
  *   skip_if_unit != 0: grad_logits already holds the gradient for g = 1 (written by a forward above); the launch returns
  *   at once on the device when *g_scale == 1, else it recomputes -- the backward of GRPO / RLOO, with no host sync.
  * b200rl_token_head_fwd: the GRPO (logp_ref != null, adv) or RLOO (logp_ref null, reward / K) head alone on per-token
- *   log-probabilities (B, S) fp32 that the caller computed; out3 and dlogp_unit as above (backward = b200rl_scale). */
+ *   log-probabilities (B, S) fp32 that the caller computed; out3 and dlogp_unit as above (backward = b200rl_scale).
+ * b200rl_ppo_lm_fwd_grad: ppo_policy_error (ding/rl_utils/ppo.py:143-230) on token rows: logit_new, logit_old,
+ *   logit_pretrained (nullable = no KL) (rows, V); adv, weight (rows).  M = rows.  out5 = {policy_loss, entropy_loss,
+ *   kl_div, approx_kl, clipfrac}: policy_loss = mean(-sel * w), sel = min(r*adv, clamp(r, 1-clip, 1+clip)*adv) (with
+ *   dual_clip > 0 and adv < 0: max(sel, dual_clip*adv)), r = exp(lp_new - lp_old); entropy_loss = mean(H * w) with H the
+ *   entropy of softmax(logit_new[row]) (entropy = 0: not computed, 0); kl_div = mean(k(lp_new - lp_pre)), k1 = x,
+ *   k2 = x^2 / 2, k3 = exp(-x) - 1 + x (0 without logit_pretrained); approx_kl = mean(lp_old - lp_new); clipfrac =
+ *   mean(r > 1+clip or r < 1-clip).  Saved for the backward: lse_new (rows), entropy_row (rows, only with entropy) = H,
+ *   dlogp_policy (rows) = (-w / M) * dsel/dr * r and dlogp_kl (rows, only with logit_pretrained) = dk/dx / M.
+ *   grad_logit_new (nullable = no gradient; dtype of the logits) = c_act * (onehot(a) - p) - c_ent * p * (log p + H),
+ *   p = softmax(logit_new[row]), log p clamped at -FLT_MAX, c_act = g_pol * dlogp_policy + g_kl * dlogp_kl,
+ *   c_ent = g_ent * w / M, for the expected upstream gradients g_expected[0] (policy), [2] (entropy), [3] (kl) -- a device
+ *   record laid out as the PPO records {policy, value, entropy, kl}; g_used (4 floats) receives the values used.
+ * b200rl_ppo_lm_bwd: the same gradient for the actual upstream gradients g_policy, g_entropy, g_kl (device scalars,
+ *   nullable = 0) from the saved rows (entropy_row / dlogp_kl null = no entropy / KL term): one read of logit_new, one
+ *   write.  g_used (nullable): the launch returns at once on the device when the upstream gradients equal it (the forward
+ *   already wrote exactly this gradient); g_hint (nullable) is refreshed with them ([0], [2] with entropy, [3]). */
 #define B200RL_DTYPE_F32 0
 #define B200RL_DTYPE_BF16 1
 B200RL_API int b200rl_grpo_fwd_grad(int dtype, const void* logit_new, const void* logit_old, const void* logit_ref,
@@ -512,6 +528,16 @@ B200RL_API int b200rl_token_head_fwd(const float* logp_new, const float* logp_ol
                           const float* reward, long long K, const float* weight, long long B, long long S,
                           double clip_ratio, double beta, float* out3, float* dlogp_unit, float* workspace,
                           size_t workspace_bytes, void* stream);
+B200RL_API int b200rl_ppo_lm_fwd_grad(int dtype, const void* logit_new, const void* logit_old,
+                           const void* logit_pretrained, const long long* action, const float* adv, const float* weight,
+                           long long rows, long long V, double clip_ratio, double dual_clip, int kl_type, int entropy,
+                           const float* g_expected, float* g_used, float* out5, float* lse_new, float* entropy_row,
+                           float* dlogp_policy, float* dlogp_kl, void* grad_logit_new, float* workspace,
+                           size_t workspace_bytes, void* stream);
+B200RL_API int b200rl_ppo_lm_bwd(int dtype, const void* logit_new, const long long* action, const float* weight,
+                      long long rows, long long V, const float* lse_new, const float* entropy_row,
+                      const float* dlogp_policy, const float* dlogp_kl, const float* g_policy, const float* g_entropy,
+                      const float* g_kl, const float* g_used, float* g_hint, void* grad_logit_new, void* stream);
 
 /* ---- data-parallel exchange step: one-shot all-reduce (mean) of n <= 8 floats over NVLink peer memory -----------
  * Replaces the small-message NCCL all-reduce of the packed loss scalars (mean of rank means,
