@@ -83,6 +83,8 @@ PROTOTYPES = {
     "b200rl_quantile_td_fwd": [P, P, P, P, P, P, P, P, P, LL, LL, LL, LL, LL, LL, D, LL, LL, LL, LL, LL, LL, LL, LL, I, D, P, P,
                                P, P, P, c_size_t, P],
     "b200rl_quantile_td_bwd": [P, P, P, P, P, LL, LL, LL, LL, LL, LL, I, P, P],
+    "b200rl_fqf_fraction_fwd": [P, P, P, P, LL, LL, LL, LL, LL, LL, LL, LL, LL, LL, LL, LL, P, P, P, P, c_size_t, P],
+    "b200rl_fqf_fraction_bwd": [P, P, LL, LL, I, P, P],
     "b200rl_p2p_allreduce_mean": [P, P, I, I, I, P, P, P],
     "b200rl_p2p_mailbox_floats": [I],
     "b200rl_probe_copy": [P, P, LL, I, P],

@@ -699,6 +699,42 @@ static inline bool ws_partials_fit(long long n_words, size_t ws_bytes) {
     return ws_bytes >= (size_t)WS_MIN_BYTES && (long long)WS_CTRL_WORDS + n_words <= (long long)WS_PARTIAL_LIMIT_WORDS;
 }
 
+// Loss reduction of the per-sample heads (the one-thread-per-row TD kernels and C51 of td.cu, FQF's fraction loss of
+// quantile.cu): fin(k, total) receives the grid total of acc[k].  The one-round-trip grid_sum_fx when no last CTA is needed
+// and the grid has at most FX_MAX_GRID CTAs; otherwise the ticket grid_sum, and the return value says whether this is the
+// last CTA, which then sees every row's stores.  The host launches the NT > 128 builds only on such grids and never with
+// need_last, so they compile only grid_sum_fx.
+template <int K, int NT, class Fin>
+__device__ __forceinline__ bool td_loss_sum(float (&acc)[K], float* ws, bool need_last, Fin fin) {
+    if (NT > 128 || (!need_last && gridDim.x <= FX_MAX_GRID)) {
+        grid_sum_fx<K, NT>(acc, ws, fin);
+        return false;
+    }
+    double tot[K];
+    const bool last = grid_sum<K, NT>(acc, tot, ws, 0);
+    if (last && threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) fin(k, tot[k]);
+    }
+    return last;
+}
+
+// Launch plan of the per-sample heads (qntd, dqfd, soft_td, fqf_fraction); kern(std::integral_constant<int, NT>()) names
+// the NT-thread build, and CTA x owns rows [x * NT, x * NT + NT).  Up to 1024 rows without a sequence priority -- the usual
+// replay-buffer batch -- run as ONE CTA of 256 / 512 / 1024 threads, which reduces the loss without any grid round trip;
+// anything else runs as 128-thread CTAs, whose K partial sums each must fit the workspace.
+template <int K, class Args, class Kern>
+static int launch_td_rows(Kern kern, const Args& a, long long rows, bool priority, float* ws, size_t ws_bytes,
+                          cudaStream_t st) {
+    const bool one_cta = rows <= 1024 && !priority;
+    const long long grid = (rows + 127) / 128;
+    if (!ws_partials_fit(one_cta ? 0 : grid * K, ws_bytes)) return B200RL_ERR_WORKSPACE;
+    if (!one_cta) return launch_k(kern(std::integral_constant<int, 128>()), (int)grid, 128, 0, st, a, ws);
+    if (rows <= 256) return launch_k(kern(std::integral_constant<int, 256>()), 1, 256, 0, st, a, ws);
+    if (rows <= 512) return launch_k(kern(std::integral_constant<int, 512>()), 1, 512, 0, st, a, ws);
+    return launch_k(kern(std::integral_constant<int, 1024>()), 1, 1024, 0, st, a, ws);
+}
+
 static inline int div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 

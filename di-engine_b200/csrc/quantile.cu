@@ -1,6 +1,7 @@
 // Quantile-regression n-step TD heads: qrdqn_nstep_td_error (ding/rl_utils/td.py:1098-1166), iqn_nstep_td_error (:1253-1346),
 // fqf_nstep_td_error (:1359-1436).  One kernel for the three: they differ in the memory layout of the quantile tensors
-// (strides), in the Huber threshold / indicator / divisor and in which axis is summed and which averaged.
+// (strides), in the Huber threshold / indicator / divisor and in which axis is summed and which averaged.  FQF's other loss,
+// the fraction loss (fqf_calculate_fraction_loss, :1466-1513), has its own kernel at the end of the file.
 //
 //   theta_i   = q[b, i, action_b]                         i < n_i   (current quantiles, differentiable)
 //   theta'_j  = R_b + g_b * next_n_q[b, j, next_action_b] * (1 - done_b)      j < n_j   (n-step target, td.py:1150-1159)
@@ -157,6 +158,91 @@ __global__ void __launch_bounds__(256) quantile_td_bwd_kernel(QtdBwdArgs a) {
     }
 }
 
+// FQF's fraction loss, fqf_calculate_fraction_loss (ding/rl_utils/td.py:1466-1513).  With s_i = q_tau_i[b, i, a_b] (i < N-1)
+// and h_k = q_value[b, k, a_b] (k < N), both taken without gradient:
+//   g_i  = where(s_i > (i == 0 ? h_0 : s_{i-1}), s_i - h_i, -(s_i - h_i))
+//        + where(s_i < (i == N-2 ? h_{N-1} : s_{i+1}), s_i - h_{i+1}, -(s_i - h_{i+1}))      (strict; NaN picks the negation)
+//   loss = mean_b sum_i g_i * quantiles[b, i+1]
+// so d loss / d quantiles[b, i+1] = (u / B) * g_i and the end columns 0 and N get zero.  CTA x owns samples [x*NT, x*NT + NT)
+// (launch_td_rows); its threads stride over their (sample, column of quantiles) pairs, so the saved g (B, N-1) and the unit
+// gradient (B, N+1) are stored coalesced whatever N is, and the gathered columns are read through element strides.
+struct FqfFracArgs {
+    const float* qt;  // q_tau_i, strided (b, i, a)
+    const float* qv;  // q_value, strided (b, k, a)
+    const float* qn;  // quantiles, strided (b, k)
+    const long long* act;
+    long long B, A_t, A_v;  // an action outside [0, A) reads NaN
+    int N;
+    long long qt_sb, qt_si, qt_sa, qv_sb, qv_si, qv_sa, qn_sb, qn_si;
+    float* loss;
+    float* g;          // (B, N-1)
+    float* grad_unit;  // nullable (B, N+1): d loss / d quantiles for a unit upstream gradient
+};
+
+template <int NT>
+__global__ void __launch_bounds__(NT) fqf_fraction_kernel(FqfFracArgs a, float* ws) {
+    pdl_prologue();
+    const float* __restrict__ qt = a.qt;
+    const float* __restrict__ qv = a.qv;
+    const float* __restrict__ qn = a.qn;
+    float* __restrict__ g = a.g;
+    float* __restrict__ gu = a.grad_unit;
+    const long long r0 = (long long)blockIdx.x * NT;
+    const int rows = (int)((a.B - r0) < NT ? (a.B - r0) : NT);
+    const int N = a.N, W = N + 1;
+    // torch's mean backward on CUDA multiplies by the fp32 reciprocal of B, then MulBackward by g
+    const float inv_b = 1.f / (float)a.B;
+    const float qnan = __int_as_float(0x7fffffff);
+    float acc[1] = {0.f};
+#pragma unroll 4
+    for (int e = threadIdx.x; e < rows * W; e += NT) {
+        const int r = e / W, c = e - r * W;
+        const long long b = r0 + r;
+        float gr = 0.f;
+        if (c > 0 && c < N) {
+            const int i = c - 1;
+            const long long ac = a.act[b];
+            const bool in_t = ac >= 0 && ac < a.A_t, in_v = ac >= 0 && ac < a.A_v;
+            const float* st = qt + b * a.qt_sb + ac * a.qt_sa;
+            const float* hv = qv + b * a.qv_sb + ac * a.qv_sa;
+            const float s = in_t ? st[i * a.qt_si] : qnan;
+            const float h0 = in_v ? hv[i * a.qv_si] : qnan;
+            const float h1 = in_v ? hv[(i + 1) * a.qv_si] : qnan;
+            const float lo = i == 0 ? h0 : (in_t ? st[(i - 1) * a.qt_si] : qnan);
+            const float hi = i == N - 2 ? h1 : (in_t ? st[(i + 1) * a.qt_si] : qnan);
+            const float v1 = fsub(s, h0), v2 = fsub(s, h1);
+            const float gi = fadd(s > lo ? v1 : -v1, s < hi ? v2 : -v2);
+            g[b * (N - 1) + i] = gi;
+            acc[0] += fmul(gi, qn[b * a.qn_sb + c * a.qn_si]);
+            gr = fmul(inv_b, gi);
+        }
+        if (gu) gu[b * W + c] = gr;
+    }
+    float* loss = a.loss;
+    const double nb = (double)a.B;
+    td_loss_sum<1, NT>(acc, ws, false, [=](int, double tot) { *loss = (float)(tot / nb); });
+}
+
+struct FqfFracBwdArgs {
+    const float* g;       // (B, N-1), saved by the forward launch
+    const float* g_loss;  // device scalar
+    long long B;
+    int N, skip_if_unit;
+    float* grad;  // (B, N+1)
+};
+
+__global__ void __launch_bounds__(256) fqf_fraction_bwd_kernel(FqfFracBwdArgs a) {
+    pdl_prologue();
+    const float u = *a.g_loss;
+    if (a.skip_if_unit && u == 1.f) return;  // the forward launch already wrote exactly this gradient
+    const float c = fmul(u, 1.f / (float)a.B);  // (u / B) as torch's mean backward forms it on CUDA, then times g
+    const long long W = a.N + 1, n = a.B * W;
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (long long)gridDim.x * blockDim.x) {
+        const long long b = e / W, k = e - b * W;
+        a.grad[e] = (k > 0 && k < a.N) ? fmul(c, a.g[b * (a.N - 1) + k - 1]) : 0.f;
+    }
+}
+
 }  // namespace b200rl
 
 using namespace b200rl;
@@ -209,4 +295,33 @@ extern "C" int b200rl_quantile_td_bwd(const float* dtheta, const float* weight, 
     long long grid = (n + 255) / 256;
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
     return launch_k(quantile_td_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, a);
+}
+
+extern "C" int b200rl_fqf_fraction_fwd(const float* q_tau_i, const float* q_value, const float* quantiles,
+                                       const long long* actions, long long B, long long N, long long A_tau,
+                                       long long A_value, long long qt_sb, long long qt_si, long long qt_sa, long long qv_sb,
+                                       long long qv_si, long long qv_sa, long long qn_sb, long long qn_si, float* loss,
+                                       float* g_saved, float* grad_quantiles_unit, float* workspace, size_t workspace_bytes,
+                                       void* stream) {
+    if (!q_tau_i || !q_value || !quantiles || !actions || !loss || !g_saved || !workspace) return B200RL_ERR_ARG;
+    // N <= 2^20: a CTA's (sample, column) pairs, at most 1024 * (N + 1), are counted in int
+    if (B < 1 || N < 1 || N > (1 << 20) || A_tau < 1 || A_value < 1) return B200RL_ERR_ARG;
+    FqfFracArgs a{};
+    a.qt = q_tau_i; a.qv = q_value; a.qn = quantiles; a.act = actions; a.B = B; a.A_t = A_tau; a.A_v = A_value;
+    a.N = (int)N; a.qt_sb = qt_sb; a.qt_si = qt_si; a.qt_sa = qt_sa; a.qv_sb = qv_sb; a.qv_si = qv_si; a.qv_sa = qv_sa;
+    a.qn_sb = qn_sb; a.qn_si = qn_si; a.loss = loss; a.g = g_saved; a.grad_unit = grad_quantiles_unit;
+    return launch_td_rows<1>([](auto nt) { return fqf_fraction_kernel<decltype(nt)::value>; }, a, B, false, workspace,
+                             workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int b200rl_fqf_fraction_bwd(const float* g_saved, const float* g_loss, long long B, long long N,
+                                       int skip_if_unit, float* grad_quantiles, void* stream) {
+    if (!g_saved || !g_loss || !grad_quantiles || B < 1 || N < 1) return B200RL_ERR_ARG;
+    FqfFracBwdArgs a{};
+    a.g = g_saved; a.g_loss = g_loss; a.B = B; a.N = (int)N; a.skip_if_unit = skip_if_unit ? 1 : 0;
+    a.grad = grad_quantiles;
+    const long long n = B * (N + 1);
+    long long grid = (n + 255) / 256;
+    if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
+    return launch_k(fqf_fraction_bwd_kernel, (int)grid, 256, 0, (cudaStream_t)stream, a);
 }

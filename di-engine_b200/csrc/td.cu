@@ -8,8 +8,8 @@
 //   UPGO return (upgo.py:46-68)                                              -> lambda_returns (+ fused TD(lambda) head)
 // Each reference call is ~20-35 tiny torch launches plus an autograd backward; here it is one forward and one
 // backward launch.  These batches are small (B ~ 32..512): latency, not bandwidth, is what the kernels minimise.
-// qntd, dqfd and soft_td run one thread per row and share the n-step return, the loss reduction, the one-hot gradient
-// store and the host launch plan below; only their targets differ.
+// qntd, dqfd and soft_td run one thread per row and share the n-step return and the one-hot gradient store below, and the
+// loss reduction and host launch plan of common.cuh (td_loss_sum, launch_td_rows); only their targets differ.
 #include <math.h>
 
 #include <type_traits>
@@ -73,25 +73,6 @@ __device__ __forceinline__ float nstep_reward_sum(const float (&rwv)[8], const f
         rf = fmul(g, rf);
     }
     return ret;
-}
-
-// Loss reduction of the one-thread-per-row TD kernels and C51: fin(k, total) receives the grid total of acc[k].  The
-// one-round-trip grid_sum_fx when no last CTA is needed and the grid has at most FX_MAX_GRID CTAs; otherwise the ticket
-// grid_sum, and the return value says whether this is the last CTA, which then sees every row's stores.  The host
-// launches the NT > 128 builds only on such grids and never with need_last, so they compile only grid_sum_fx.
-template <int K, int NT, class Fin>
-__device__ __forceinline__ bool td_loss_sum(float (&acc)[K], float* ws, bool need_last, Fin fin) {
-    if (NT > 128 || (!need_last && gridDim.x <= FX_MAX_GRID)) {
-        grid_sum_fx<K, NT>(acc, ws, fin);
-        return false;
-    }
-    double tot[K];
-    const bool last = grid_sum<K, NT>(acc, tot, ws, 0);
-    if (last && threadIdx.x == 0) {
-#pragma unroll
-        for (int k = 0; k < K; ++k) fin(k, tot[k]);
-    }
-    return last;
 }
 
 // The CTA's gradient rows [r0, r0 + NT) of g (R rows of N): row r0 + t, staged by thread t, is coef0[t] at idx0[t] (plus
@@ -1061,22 +1042,6 @@ static TdScalars td_scalars(double gamma, int nstep, double rescale_eps, long lo
     c.prio_max_w = (float)priority_mix; c.prio_mean_w = (float)(1.0 - priority_mix);
     c.prio_div = (float)((double)seq_len + 1e-8);
     return c;
-}
-
-// Launch plan of qntd, dqfd and soft_td; kern(std::integral_constant<int, NT>()) names the NT-thread build.  Up to 1024 rows
-// without a sequence priority -- the usual replay-buffer batch -- run as ONE CTA of 256 / 512 / 1024 threads, which reduces
-// the loss without any grid round trip; anything else runs as 128-thread CTAs, whose K partial sums each must fit the
-// workspace.
-template <int K, class Args, class Kern>
-static int launch_td_rows(Kern kern, const Args& a, long long rows, bool priority, float* ws, size_t ws_bytes,
-                          cudaStream_t st) {
-    const bool one_cta = rows <= 1024 && !priority;
-    const long long grid = (rows + 127) / 128;
-    if (!ws_partials_fit(one_cta ? 0 : grid * K, ws_bytes)) return B200RL_ERR_WORKSPACE;
-    if (!one_cta) return launch_k(kern(std::integral_constant<int, 128>()), (int)grid, 128, 0, st, a, ws);
-    if (rows <= 256) return launch_k(kern(std::integral_constant<int, 256>()), 1, 256, 0, st, a, ws);
-    if (rows <= 512) return launch_k(kern(std::integral_constant<int, 512>()), 1, 512, 0, st, a, ws);
-    return launch_k(kern(std::integral_constant<int, 1024>()), 1, 1024, 0, st, a, ws);
 }
 
 extern "C" int b200rl_qntd_fwd(const float* q, const float* next_n_q, const long long* action,

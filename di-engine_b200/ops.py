@@ -690,6 +690,46 @@ class QuantileTDFunction(torch.autograd.Function):
         return (grad_q, ) + (None, ) * 20
 
 
+class FQFFractionFunction(torch.autograd.Function):
+    """FQF's fraction loss (td.py:1466-1513), differentiable w.r.t. ``quantiles`` only (q_tau_i and q_value enter detached,
+    as the reference gathers them under no_grad); the forward launch also writes d loss / d quantiles for a unit upstream
+    gradient (verified on the device by the backward launch, as QuantileTDFunction).  ``*_strides``: element strides of
+    (sample, quantile[, action])."""
+
+    @staticmethod
+    def forward(ctx, q_tau_i, q_value, quantiles, action, B, N, qt_strides, qv_strides, qn_strides):
+        dev = quantiles.device
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        g = torch.empty(B, N - 1, dtype=torch.float32, device=dev)
+        grad_unit = torch.empty(B, N + 1, dtype=torch.float32, device=dev) if ctx.needs_input_grad[2] else None
+        with on_device(dev):
+            ws = workspace(dev)
+            rc = lib().b200rl_fqf_fraction_fwd(
+                ptr(q_tau_i), ptr(q_value), ptr(quantiles), ptr(action), B, N, q_tau_i.shape[2], q_value.shape[2],
+                *qt_strides, *qv_strides, *qn_strides, ptr(loss), ptr(g), ptr(grad_unit), ptr(ws), ws.numel() * 4,
+                stream_ptr()
+            )
+        _lib.check(rc, 'b200rl_fqf_fraction_fwd')
+        ctx.save_for_backward(g)
+        ctx.cfg = (B, N)
+        ctx.spec = grad_unit
+        ctx.set_materialize_grads(False)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g_loss):
+        if g_loss is None:
+            return (None, ) * 9
+        g, = ctx.saved_tensors
+        B, N = ctx.cfg
+        keep, (pg, ) = _grads(g_loss)
+        grad, skip = _unit_grad(ctx, (), lambda: torch.empty(B, N + 1, dtype=torch.float32, device=g.device))
+        with on_device(g.device):
+            rc = lib().b200rl_fqf_fraction_bwd(ptr(g), pg, B, N, skip, ptr(grad), stream_ptr())
+        _lib.check(rc, 'b200rl_fqf_fraction_bwd')
+        return (None, None, grad) + (None, ) * 6
+
+
 # ----------------------------------------------------------------------------------------------------------------
 # distributional n-step TD (C51)
 # ----------------------------------------------------------------------------------------------------------------

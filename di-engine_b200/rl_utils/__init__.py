@@ -19,8 +19,8 @@ from .td import (bdq_nstep_td_error, dist_1step_td_data, dist_1step_td_error, di
                  shape_fn_qntd, shape_fn_qntd_rescale, shape_fn_td_lambda, td_lambda_data, td_lambda_error,
                  v_1step_td_data, v_1step_td_error, v_nstep_td_data, v_nstep_td_error)
 from .ppg import ppg_data, ppg_joint_error, ppg_joint_loss
-from .quantile import (fqf_nstep_td_data, fqf_nstep_td_error, iqn_nstep_td_data, iqn_nstep_td_error, qrdqn_nstep_td_data,
-                       qrdqn_nstep_td_error)
+from .quantile import (fqf_calculate_fraction_loss, fqf_nstep_td_data, fqf_nstep_td_error, iqn_nstep_td_data,
+                       iqn_nstep_td_error, qrdqn_nstep_td_data, qrdqn_nstep_td_error)
 from .retrace import compute_q_retraces
 from .rloo import rloo_info, rloo_policy_data, rloo_policy_error
 from .upgo import tb_cross_entropy, upgo_loss, upgo_returns
@@ -35,7 +35,7 @@ HOT_PATH_FUNCTIONS = [
     'q_1step_td_error', 'v_1step_td_error', 'v_nstep_td_error', 'ppo_policy_error', 'ppo_value_error',
     'dist_1step_td_error', 'bdq_nstep_td_error', 'upgo_returns', 'tb_cross_entropy', 'ppo_error_continuous', 'a2c_error',
     'vtrace_error_continuous_action', 'qrdqn_nstep_td_error', 'iqn_nstep_td_error', 'fqf_nstep_td_error',
-    'compute_q_retraces', 'happo_error', 'happo_policy_error', 'happo_value_error', 'happo_error_continuous', 'happo_policy_error_continuous',
+    'fqf_calculate_fraction_loss', 'compute_q_retraces', 'happo_error', 'happo_policy_error', 'happo_value_error', 'happo_error_continuous', 'happo_policy_error_continuous',
     'acer_policy_error', 'acer_value_error', 'acer_trust_region_update', 'ppg_joint_error',
     'dqfd_nstep_td_error', 'dqfd_nstep_td_error_with_rescale',
     'm_q_1step_td_error', 'q_nstep_sql_td_error', 'q_v_1step_td_error',

@@ -1,6 +1,7 @@
 """Quantile-regression n-step TD heads with the signatures of ding/rl_utils/td.py: ``qrdqn_nstep_td_error`` (:1098),
 ``iqn_nstep_td_error`` (:1253), ``fqf_nstep_td_error`` (:1359) -- one kernel (csrc/quantile.cu), the three tensor layouts are
-handed over as strides, so no ``gather`` / ``permute`` / ``repeat`` copy is made."""
+handed over as strides, so no ``gather`` / ``permute`` / ``repeat`` copy is made.  FQF's fraction loss,
+``fqf_calculate_fraction_loss`` (:1466), runs on its own kernel in the same file and reads its inputs through strides too."""
 from collections import namedtuple
 from typing import Optional
 
@@ -123,3 +124,38 @@ def fqf_nstep_td_error(
     B, tau = q.shape[0], q.shape[1]
     t = quantiles_hats.expand(B, tau)
     return _run(q, next_n_q, action, next_n_action, reward, done, t, weight, gamma, nstep, value_gamma, 2, kappa, (0, 1, 2))
+
+
+def _f32(t, name):
+    # fp32 as it is, views included: the kernel reads through strides
+    return t if t.dtype == torch.float32 else ops.f32c(t, name)
+
+
+def _gather_check(q_s, actions):
+    # evaluate_quantile_at_action (td.py:1452-1463): its assertion, and the shapes its gather accepts
+    assert q_s.shape[0] == actions.shape[0]
+    if q_s.dim() != 3 or actions.dim() != 1:
+        raise RuntimeError("fqf_calculate_fraction_loss: gather needs a (B, n, A) tensor and (B,) actions, got %s and %s" %
+                           (tuple(q_s.shape), tuple(actions.shape)))
+
+
+def fqf_calculate_fraction_loss(q_tau_i, q_value, quantiles, actions):
+    """
+    Drop-in for ding/rl_utils/td.py:1466-1513.  q_tau_i (B, N-1, A), q_value (B, N, A) (must require grad; neither gets a
+    gradient), quantiles (B, N+1), actions (B,).  Returns the fraction loss, a 0-dim tensor attached to ``quantiles`` only
+    (no grad_fn when quantiles does not require grad).
+    """
+    assert q_value.requires_grad
+    batch_size, num_quantiles = q_value.shape[0], q_value.shape[1]
+    _gather_check(q_tau_i, actions)
+    assert (q_tau_i.shape[0], q_tau_i.shape[1]) == (batch_size, num_quantiles - 1)  # td.py:1487
+    _gather_check(q_value, actions)
+    assert quantiles[:, 1:-1].shape == (batch_size, num_quantiles - 1)  # td.py:1507
+    dev = ops.compute_device(q_tau_i, q_value, quantiles, actions)
+    host_out = not quantiles.is_cuda
+    qt = _f32(ops.to_device(q_tau_i.detach(), dev), 'q_tau_i')
+    qv = _f32(ops.to_device(q_value.detach(), dev), 'q_value')
+    qn = _f32(ops.to_device(quantiles, dev), 'quantiles')
+    act = ops.i64c(ops.to_device(actions, dev), min(qt.shape[2], qv.shape[2]), 'actions')
+    loss = ops.FQFFractionFunction.apply(qt, qv, qn, act, batch_size, num_quantiles, qt.stride(), qv.stride(), qn.stride())
+    return loss.cpu() if host_out else loss

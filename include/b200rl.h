@@ -379,6 +379,22 @@ B200RL_API int b200rl_quantile_td_bwd(const float* dtheta, const float* weight, 
                            const float* g_loss, const float* g_td, long long B, long long N, long long n_tau,
                            long long q_sb, long long q_si, long long q_sa, int skip_if_unit, float* grad_q, void* stream);
 
+/* ---- FQF's fraction loss: fqf_calculate_fraction_loss (ding/rl_utils/td.py:1466-1513) -- csrc/quantile.cu.
+ * s_i = q_tau_i[b*qt_sb + i*qt_si + a_b*qt_sa] (i < N-1, A_tau actions), h_k = q_value[b*qv_sb + k*qv_si + a_b*qv_sa]
+ * (k < N, A_value actions), quantiles[b*qn_sb + k*qn_si] (k <= N); actions (B) int64, an action out of range reads NaN.
+ * g_i = (s_i > (i == 0 ? h_0 : s_{i-1}) ? 1 : -1) * (s_i - h_i) + (s_i < (i == N-2 ? h_{N-1} : s_{i+1}) ? 1 : -1) *
+ * (s_i - h_{i+1}); writes loss = mean_b sum_i g_i * quantiles[b, i+1] (scalar), g_saved (B, N-1) and -- non-null --
+ * grad_quantiles_unit (B, N+1), contiguous: fp32(1/B) * g_i in column i+1, zero in columns 0 and N.
+ * b200rl_fqf_fraction_bwd: grad_quantiles (B, N+1) = (*g_loss * fp32(1/B)) * g_i likewise; skip_if_unit = 1: grad_quantiles
+ * already holds the unit gradient, the launch returns at once when *g_loss == 1. */
+B200RL_API int b200rl_fqf_fraction_fwd(const float* q_tau_i, const float* q_value, const float* quantiles,
+                            const long long* actions, long long B, long long N, long long A_tau, long long A_value,
+                            long long qt_sb, long long qt_si, long long qt_sa, long long qv_sb, long long qv_si,
+                            long long qv_sa, long long qn_sb, long long qn_si, float* loss, float* g_saved,
+                            float* grad_quantiles_unit, float* workspace, size_t workspace_bytes, void* stream);
+B200RL_API int b200rl_fqf_fraction_bwd(const float* g_saved, const float* g_loss, long long B, long long N,
+                            int skip_if_unit, float* grad_quantiles, void* stream);
+
 /* ---- sibling heads (SURVEY section 8f rank 3), forward + gradients in ONE launch each (csrc/heads.cu) ---------------------
  * Same backward contract as b200rl_vtrace_fwd_grad: verify = 0 writes the losses and (grad_* non-null) the gradients for the
  * expected upstream gradients g_expected[k], recording them in g_used; verify = 1 with the actual upstream gradients (device
