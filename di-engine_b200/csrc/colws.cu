@@ -362,16 +362,9 @@ __global__ void __launch_bounds__(CW_THREADS, CwGeo<TC>::CTAS_PER_SM) gae_ppo_ws
         cpa_wait<0>();
     } else {
         // =============================================== consumers ========================================================
-        PpoUpstream up{0.f, 0.f, 0.f, 0.f, 1.f / (float)a.S};
-        if (GRADS) {
-            up.g_pol = a.g_policy ? *a.g_policy : 0.f;
-            up.g_val = a.g_value ? *a.g_value : 0.f;
-            up.g_ent = a.g_entropy ? *a.g_entropy : 0.f;
-            up.g_kl = (a.g_kl && has_pre) ? *a.g_kl : 0.f;
-            if (a.g_used && blockIdx.x == 0 && tid == 0) {
-                a.g_used[0] = up.g_pol; a.g_used[1] = up.g_val; a.g_used[2] = up.g_ent; a.g_used[3] = up.g_kl;
-            }
-        }
+        float g[4] = {0.f, 0.f, 0.f, 0.f};
+        if (GRADS) upstream<4>(a.rec, false, ppo_owned(a), g);  // a forward launch: records `used`, never skips
+        const PpoUpstream up{g[0], g[1], g[2], g[3], 1.f / (float)a.S};
         // trace: chunk j's stamp k (0 landed, 1 advantages ready, 2 computed); slots 3-5 are overwritten by every chunk, so
         // the last chunk's remain
         auto stamp_chunk = [&](int j, int k) {

@@ -626,6 +626,70 @@ static inline FinalizeArgs vtrace_finalize_args(long long T, long long B, int gr
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Forward-written gradients (include/b200rl.h states the contract).  The forward launch of a loss also writes its gradients
+// for the upstream gradients the call site expects and records the values it used; the backward ("verify") launch of the
+// same loss returns at once when the actual upstream gradients are bit-identical to that record, and recomputes otherwise.
+// Slot k of every record: 0 policy, 1 value, 2 entropy, 3 kl; `owned` is the mask of the slots a kernel computes.
+// ---------------------------------------------------------------------------------------------------------------
+struct UpstreamRecord {
+    const float* g[4];  // the upstream gradients the launch applies, device scalars (nullable = 0): forward the expected,
+                        // verify the actual ones
+    float* used;        // forward: receives every slot (nullable); verify: compared (null = recompute)
+    float* hint;        // verify: its owned slots are refreshed with the actual values (nullable)
+    int verify;         // which of the two launches this is
+};
+
+// the record of a forward launch: `expected` holds one device float per slot (nullable = 0)
+static inline UpstreamRecord forward_record(const float* expected, float* used) {
+    UpstreamRecord r{};
+    for (int k = 0; k < 4; ++k) r.g[k] = expected ? expected + k : nullptr;
+    r.used = used;
+    return r;
+}
+
+// the record of a verify launch: the actual upstream gradient of every slot
+static inline UpstreamRecord verify_record(const float* g0, const float* g1, const float* g2, const float* g3,
+                                           const float* used, float* hint) {
+    return UpstreamRecord{{g0, g1, g2, g3}, const_cast<float*>(used), hint, 1};
+}
+
+// the upstream gradient of slot k, 0 for a slot the kernel does not own
+__device__ __forceinline__ float upstream_value(const UpstreamRecord& r, unsigned owned, int k) {
+    return ((owned >> k) & 1u) && r.g[k] ? *r.g[k] : 0.f;
+}
+
+// g[k] = upstream_value of every slot.  Block 0, thread 0 records every slot in `used` (forward; an unowned one as 0) or
+// refreshes the owned slots in `hint` (verify).  -> true when the verify launch may return: `used` is given and every owned
+// slot of it is bit-identical to the actual value -- the same decision in every thread of the grid.  `verify` is r.verify,
+// or a constant where the kernel's mode is a template parameter (the compiler then drops the other mode's code).  Every
+// load comes before the one store, so the loads are issued together: a verify launch that returns at once sits between
+// two steps of the training loop.
+template <int K>
+__device__ __forceinline__ bool upstream(const UpstreamRecord& r, bool verify, unsigned owned, float (&g)[K]) {
+    const bool cmp = verify && r.used != nullptr;
+    bool same = cmp;
+#pragma unroll
+    for (int k = 0; k < K; ++k) g[k] = upstream_value(r, owned, k);
+#pragma unroll
+    for (int k = 0; k < K; ++k)
+        if (cmp && ((owned >> k) & 1u)) same &= __float_as_uint(g[k]) == __float_as_uint(r.used[k]);
+    float* rec = verify ? r.hint : r.used;
+    if (rec && blockIdx.x == 0 && threadIdx.x == 0)
+#pragma unroll
+        for (int k = 0; k < K; ++k)
+            if (!verify || ((owned >> k) & 1u)) rec[k] = g[k];
+    return same;
+}
+
+// The argument rule of every entry point with a record.  verify: the launch may have to recompute, so it needs every
+// gradient buffer it writes (`bufs`); a null `used` means recompute.  forward: it needs `out`, and when it writes gradients
+// (`grads`) every gradient buffer, the expected upstream gradients and the record to write.
+static inline bool upstream_args_ok(int verify, const float* out, bool grads, bool bufs, const float* expected,
+                                    const float* used) {
+    return verify ? bufs : (out && (!grads || (bufs && expected && used)));
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // Launch geometry of the persistent kernels, cached per (kernel, device).  The dynamic shared-memory opt-in belongs
 // to the kernel in the current device's context, so a process that runs an operator on one device and then on
 // another has to opt the kernel in on each.

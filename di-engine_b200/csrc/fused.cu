@@ -53,16 +53,9 @@ __global__ void __launch_bounds__(PPO_THREADS, 4) gae_ppo_kernel(FusedArgs f, fl
     unsigned int* ctrl = reinterpret_cast<unsigned int*>(ws);
     unsigned int* chunk_ctr = ctrl + WS_CHUNK_CTR_OFF;
 
-    PpoUpstream up{0.f, 0.f, 0.f, 0.f, 1.f / (float)a.S};
-    if (GRADS) {
-        up.g_pol = a.g_policy ? *a.g_policy : 0.f;
-        up.g_val = a.g_value ? *a.g_value : 0.f;
-        up.g_ent = a.g_entropy ? *a.g_entropy : 0.f;
-        up.g_kl = (a.g_kl && has_pre) ? *a.g_kl : 0.f;
-        if (a.g_used && blockIdx.x == 0 && tid == 0) {
-            a.g_used[0] = up.g_pol; a.g_used[1] = up.g_val; a.g_used[2] = up.g_ent; a.g_used[3] = up.g_kl;
-        }
-    }
+    float g[4] = {0.f, 0.f, 0.f, 0.f};
+    if (GRADS) upstream<4>(a.rec, false, ppo_owned(a), g);  // a forward launch: records `used`, never skips
+    const PpoUpstream up{g[0], g[1], g[2], g[3], 1.f / (float)a.S};
 
     // ---- phase G: GAE column tiles (shared memory aliased onto the not-yet-used PPO stage ring) -----------------------
     const long long n_col_tiles = (f.B + FUSED_TC - 1) / FUSED_TC;
@@ -315,19 +308,18 @@ static int gae_ppo_step(const float* value, float* next_value, const float* rewa
                         float* g_used, float* adv, float* out, float* grad_logit_new, float* grad_value_new,
                         const unsigned long long* mailbox_ptrs_dev, int rank, int world, unsigned int* seq_dev,
                         float* out_mean, float* workspace, size_t workspace_bytes, void* stream) {
+    const bool grads = g_expected != nullptr;
     if (!value || !next_value || !reward || !logit_new || !logit_old || !action || !value_new || !value_old ||
-        !return_ || !adv || !out || !workspace || T < 1 || B < 1 || N < 1 || kl_type < 1 || kl_type > 3)
+        !return_ || !adv || !workspace || T < 1 || B < 1 || N < 1 || kl_type < 1 || kl_type > 3 ||
+        !upstream_args_ok(0, out, grads, grad_logit_new && grad_value_new, g_expected, g_used))
         return B200RL_ERR_ARG;
     FusedArgs f{};
     fill_fused(f, value, next_value, reward, done, traj_flag, T, B, gamma, lambda_, mask_next_value_inplace,
                logit_new, logit_old, logit_pretrained, action, value_new, value_old, return_, weight, N, clip_ratio,
                use_value_clip, dual_clip, kl_type, adv);
-    const bool grads = g_expected != nullptr;
     if (grads) {
-        if (!g_used || !grad_logit_new || !grad_value_new) return B200RL_ERR_ARG;
-        f.p.g_policy = g_expected; f.p.g_value = g_expected + 1; f.p.g_entropy = g_expected + 2;
-        f.p.g_kl = g_expected + 3; f.p.g_used = g_used; f.p.grad_logit = grad_logit_new;
-        f.p.grad_value = grad_value_new;
+        f.p.rec = forward_record(g_expected, g_used);
+        f.p.grad_logit = grad_logit_new; f.p.grad_value = grad_value_new;
     }
     cudaStream_t st = (cudaStream_t)stream;
     const bool row_ok = fused_ok(f), col_ok = colws_ok(f);

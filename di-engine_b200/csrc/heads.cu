@@ -17,37 +17,6 @@ constexpr int HD_NT = 256;
 constexpr float kLogSqrt2Pi = 0.9189385332046727f;       // math.log(math.sqrt(2 * math.pi))
 constexpr float kHalfPlusHalfLog2Pi = 1.4189385332046727f;  // 0.5 + 0.5 * math.log(2 * math.pi)
 
-struct HeadGrads {
-    const float* g_expected;  // forward: K expected upstream gradients (device)
-    const float* g_actual[4];  // verify: actual upstream gradients (device scalars, nullable = 0)
-    float* g_used;            // forward: recorded; verify: compared
-    float* g_hint;            // verify: refreshed (nullable)
-    int verify;
-};
-
-// -> true when the verify launch may return (the gradients in memory were produced for exactly these upstream values)
-template <int K>
-__device__ __forceinline__ bool head_upstream(const HeadGrads& h, float (&g)[K], unsigned ignore = 0u) {
-    if (h.verify) {
-        bool same = true;
-#pragma unroll
-        for (int k = 0; k < K; ++k) {
-            g[k] = h.g_actual[k] ? *h.g_actual[k] : 0.f;
-            if (!((ignore >> k) & 1u)) same &= __float_as_uint(g[k]) == __float_as_uint(h.g_used[k]);
-        }
-        if (h.g_hint && blockIdx.x == 0 && threadIdx.x == 0)
-#pragma unroll
-            for (int k = 0; k < K; ++k) h.g_hint[k] = g[k];
-        return same;
-    }
-#pragma unroll
-    for (int k = 0; k < K; ++k) g[k] = h.g_expected ? h.g_expected[k] : 0.f;
-    if (h.g_used && blockIdx.x == 0 && threadIdx.x == 0)
-#pragma unroll
-        for (int k = 0; k < K; ++k) h.g_used[k] = g[k];
-    return false;
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // a2c_error (discrete)
 // ---------------------------------------------------------------------------------------------------------------
@@ -63,13 +32,13 @@ struct A2cArgs {
     float* out;         // 3 losses
     float* grad_logit;  // nullable: losses only
     float* grad_value;
-    HeadGrads h;
+    UpstreamRecord rec;  // slots policy, value, entropy
 };
 
 __global__ void __launch_bounds__(HD_NT) a2c_kernel(A2cArgs a, float* ws) {
     pdl_prologue();
     float g[3];
-    if (head_upstream<3>(a.h, g)) return;
+    if (upstream<3>(a.rec, a.rec.verify, 7u, g)) return;
     const bool grads = a.grad_logit != nullptr;
     const float inv_s = 1.f / (float)a.S;
     float acc[3] = {0.f, 0.f, 0.f};
@@ -98,7 +67,7 @@ __global__ void __launch_bounds__(HD_NT) a2c_kernel(A2cArgs a, float* ws) {
             a.grad_value[s] = g[1] * (-2.f * w * dv) * inv_s;
         }
     }
-    if (a.h.verify) return;  // the losses were written by the forward launch
+    if (a.rec.verify) return;  // the losses were written by the forward launch
     const double is = 1.0 / (double)a.S;
     grid_sum_fx<3, HD_NT>(acc, ws, [&](int k, double t) { a.out[k] = (float)(t * is); });
 }
@@ -130,7 +99,7 @@ struct PpocArgs {
     float* grad_mu;     // nullable: losses only
     float* grad_sigma;
     float* grad_value;
-    HeadGrads h;
+    UpstreamRecord rec;  // slots policy, value, entropy, and kl with the pretrained policy
 };
 
 // log N(a; mu, sigma) summed over the D action dims, torch.distributions.Normal.log_prob's expression
@@ -147,8 +116,7 @@ __global__ void __launch_bounds__(HD_NT) ppoc_kernel(PpocArgs a, float* ws) {
     pdl_prologue();
     float g[4];
     const bool grads = a.grad_mu != nullptr, has_pre = a.mu_pre != nullptr;
-    if (head_upstream<4>(a.h, g, has_pre ? 0u : 8u)) return;  // no pretrained policy: the kl term has no gradient to compare
-    if (!has_pre) g[3] = 0.f;
+    if (upstream<4>(a.rec, a.rec.verify, has_pre ? 15u : 7u, g)) return;
     const float inv_s = 1.f / (float)a.S;
     const float ent_scale = a.factor ? 1.f / (float)a.D : 1.f;  // happo: mean over S * D elements
     float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -184,7 +152,7 @@ __global__ void __launch_bounds__(HD_NT) ppoc_kernel(PpocArgs a, float* ws) {
             a.grad_value[s] = g[1] * 0.5f * w * inv_s * dterm;
         }
     }
-    if (a.h.verify) return;
+    if (a.rec.verify) return;
     const double is = 1.0 / (double)a.S;
     const double per_dim = a.factor ? 1.0 / (double)a.D : 1.0;
     grid_sum_fx<6, HD_NT>(acc, ws, [&](int k, double t) {
@@ -211,13 +179,13 @@ struct A2ccArgs {
     float* grad_mu;    // nullable: losses only
     float* grad_sigma;
     float* grad_value;
-    HeadGrads h;
+    UpstreamRecord rec;  // slots policy, value, entropy
 };
 
 __global__ void __launch_bounds__(HD_NT) a2cc_kernel(A2ccArgs a, float* ws) {
     pdl_prologue();
     float g[3];
-    if (head_upstream<3>(a.h, g)) return;
+    if (upstream<3>(a.rec, a.rec.verify, 7u, g)) return;
     const bool grads = a.grad_mu != nullptr;
     const float inv_s = 1.f / (float)a.S;
     float acc[3] = {0.f, 0.f, 0.f};
@@ -245,7 +213,7 @@ __global__ void __launch_bounds__(HD_NT) a2cc_kernel(A2ccArgs a, float* ws) {
             a.grad_value[s] = g[1] * (-2.f * w * dv) * inv_s;
         }
     }
-    if (a.h.verify) return;
+    if (a.rec.verify) return;
     const double is = 1.0 / (double)a.S;
     grid_sum_fx<3, HD_NT>(acc, ws, [&](int k, double t) { a.out[k] = (float)(t * is); });
 }
@@ -300,13 +268,12 @@ extern "C" int b200rl_a2c_fwd_grad(const float* logit, const long long* action, 
                                    float* grad_value, float* workspace, size_t workspace_bytes, void* stream) {
     if (S < 1 || N < 1 || !logit || !action || !value || !adv || !return_ || !workspace || workspace_bytes < WS_MIN_BYTES)
         return B200RL_ERR_ARG;
-    if (verify ? (!g_used || !grad_logit || !grad_value) : (!out3 || (grad_logit && (!g_expected || !g_used || !grad_value))))
-        return B200RL_ERR_ARG;
+    if (!upstream_args_ok(verify, out3, grad_logit, grad_logit && grad_value, g_expected, g_used)) return B200RL_ERR_ARG;
     A2cArgs a{};
     a.logit = logit; a.action = action; a.value = value; a.adv = adv; a.ret = return_; a.weight = weight; a.S = S;
     a.N = (int)N; a.out = out3; a.grad_logit = grad_logit; a.grad_value = grad_value;
-    a.h.g_expected = g_expected; a.h.g_actual[0] = g_policy; a.h.g_actual[1] = g_value; a.h.g_actual[2] = g_entropy;
-    a.h.g_used = g_used; a.h.g_hint = g_hint; a.h.verify = verify;
+    a.rec = verify ? verify_record(g_policy, g_value, g_entropy, nullptr, g_used, g_hint)
+                   : forward_record(g_expected, g_used);
     return launch_k(a2c_kernel, head_grid(S), HD_NT, 0, (cudaStream_t)stream, a, workspace);
 }
 
@@ -322,8 +289,7 @@ extern "C" int b200rl_ppo_continuous_fwd_grad(
         !return_ || !workspace || workspace_bytes < WS_MIN_BYTES || kl_type < 1 || kl_type > 3 ||
         (!mu_pretrained) != (!sigma_pretrained))
         return B200RL_ERR_ARG;
-    if (verify ? (!g_used || !grad_mu || !grad_sigma || !grad_value)
-               : (!out6 || (grad_mu && (!g_expected || !g_used || !grad_sigma || !grad_value))))
+    if (!upstream_args_ok(verify, out6, grad_mu, grad_mu && grad_sigma && grad_value, g_expected, g_used))
         return B200RL_ERR_ARG;
     PpocArgs a{};
     a.mu_new = mu_new; a.sigma_new = sigma_new; a.mu_old = mu_old; a.sigma_old = sigma_old; a.mu_pre = mu_pretrained;
@@ -332,8 +298,8 @@ extern "C" int b200rl_ppo_continuous_fwd_grad(
     a.clip_lo = (float)(1.0 - clip_ratio); a.clip_hi = (float)(1.0 + clip_ratio); a.dual_clip = (float)dual_clip;
     a.use_value_clip = use_value_clip; a.kl_type = kl_type; a.out = out6; a.grad_mu = grad_mu; a.grad_sigma = grad_sigma;
     a.grad_value = grad_value;
-    a.h.g_expected = g_expected; a.h.g_actual[0] = g_policy; a.h.g_actual[1] = g_value; a.h.g_actual[2] = g_entropy;
-    a.h.g_actual[3] = g_kl; a.h.g_used = g_used; a.h.g_hint = g_hint; a.h.verify = verify;
+    a.rec = verify ? verify_record(g_policy, g_value, g_entropy, g_kl, g_used, g_hint)
+                   : forward_record(g_expected, g_used);
     return launch_k(ppoc_kernel, head_grid(S), HD_NT, 0, (cudaStream_t)stream, a, workspace);
 }
 
@@ -346,14 +312,13 @@ extern "C" int b200rl_a2c_continuous_fwd_grad(const float* mu, const float* sigm
     if (S < 1 || D < 1 || !mu || !sigma || !action || !value || !adv || !return_ || !workspace ||
         workspace_bytes < WS_MIN_BYTES)
         return B200RL_ERR_ARG;
-    if (verify ? (!g_used || !grad_mu || !grad_sigma || !grad_value)
-               : (!out3 || (grad_mu && (!g_expected || !g_used || !grad_sigma || !grad_value))))
+    if (!upstream_args_ok(verify, out3, grad_mu, grad_mu && grad_sigma && grad_value, g_expected, g_used))
         return B200RL_ERR_ARG;
     A2ccArgs a{};
     a.mu = mu; a.sigma = sigma; a.action = action; a.value = value; a.adv = adv; a.ret = return_; a.weight = weight;
     a.S = S; a.D = (int)D; a.out = out3; a.grad_mu = grad_mu; a.grad_sigma = grad_sigma; a.grad_value = grad_value;
-    a.h.g_expected = g_expected; a.h.g_actual[0] = g_policy; a.h.g_actual[1] = g_value; a.h.g_actual[2] = g_entropy;
-    a.h.g_used = g_used; a.h.g_hint = g_hint; a.h.verify = verify;
+    a.rec = verify ? verify_record(g_policy, g_value, g_entropy, nullptr, g_used, g_hint)
+                   : forward_record(g_expected, g_used);
     return launch_k(a2cc_kernel, head_grid(S), HD_NT, 0, (cudaStream_t)stream, a, workspace);
 }
 

@@ -49,28 +49,10 @@ __global__ void __launch_bounds__(PPO_THREADS) ppo_tile_kernel(PpoArgs a, float*
     uint64_t* full = reinterpret_cast<uint64_t*>(outbuf + (GRADS ? PPO_OUTBUFS * L.logit_bytes : 0));
     uint64_t* empty = full + PPO_STAGES;
 
-    float g_pol = 0.f, g_val = 0.f, g_ent = 0.f, g_kl = 0.f;
-    if (GRADS) {
-        g_pol = a.g_policy ? *a.g_policy : 0.f;
-        g_val = a.g_value ? *a.g_value : 0.f;
-        g_ent = a.g_entropy ? *a.g_entropy : 0.f;
-        g_kl = (a.g_kl && has_pre) ? *a.g_kl : 0.f;
-        if (WHAT == PPO_BWD) {
-            if (a.g_hint && blockIdx.x == 0 && tid == 0) {
-                a.g_hint[0] = g_pol; a.g_hint[1] = g_val; a.g_hint[2] = g_ent; a.g_hint[3] = a.g_kl ? *a.g_kl : 0.f;
-            }
-            if (a.g_used) {  // gradients were already produced by the forward pass for exactly these upstream values?
-                const bool same = __float_as_uint(a.g_used[0]) == __float_as_uint(g_pol) &&
-                                  __float_as_uint(a.g_used[1]) == __float_as_uint(g_val) &&
-                                  __float_as_uint(a.g_used[2]) == __float_as_uint(g_ent) &&
-                                  (!has_pre || __float_as_uint(a.g_used[3]) == __float_as_uint(g_kl));
-                if (same) return;
-            }
-        } else if (a.g_used && blockIdx.x == 0 && tid == 0) {
-            a.g_used[0] = g_pol; a.g_used[1] = g_val; a.g_used[2] = g_ent; a.g_used[3] = g_kl;
-        }
-    }
-    const PpoUpstream up{g_pol, g_val, g_ent, g_kl, 1.f / (float)a.S};
+    float g[4] = {0.f, 0.f, 0.f, 0.f};
+    // BWD: returns when the forward pass wrote exactly these gradients
+    if (GRADS && upstream<4>(a.rec, WHAT == PPO_BWD, ppo_owned(a), g)) return;
+    const PpoUpstream up{g[0], g[1], g[2], g[3], 1.f / (float)a.S};
 
     const long long n_full = a.S / PPO_R;
     const int tail_rows = (int)(a.S - n_full * PPO_R);
@@ -239,22 +221,11 @@ __global__ void __launch_bounds__(NT) ppo_bwd_kernel(PpoArgs a) {
     constexpr int L = (MODE == 2) ? 32 : 1;
     const int lane = (MODE == 2) ? (threadIdx.x & 31) : 0;
     const int N = a.N, G = a.G;
-    const float g_pol = a.g_policy ? *a.g_policy : 0.f;
-    const float g_val = a.g_value ? *a.g_value : 0.f;
-    const float g_ent = a.g_entropy ? *a.g_entropy : 0.f;
-    const float g_kl = (a.g_kl && a.logit_pre) ? *a.g_kl : 0.f;
-    // verification launch behind a fused forward (no shared memory, small grid: it normally returns right here):
-    // refresh the expectation for the next forward and leave if the gradients in grad_* were produced for these values
-    if (a.g_hint && blockIdx.x == 0 && threadIdx.x == 0) {
-        a.g_hint[0] = g_pol; a.g_hint[1] = g_val; a.g_hint[2] = g_ent; a.g_hint[3] = a.g_kl ? *a.g_kl : 0.f;
-    }
-    if (a.g_used) {
-        const bool same = __float_as_uint(a.g_used[0]) == __float_as_uint(g_pol) &&
-                          __float_as_uint(a.g_used[1]) == __float_as_uint(g_val) &&
-                          __float_as_uint(a.g_used[2]) == __float_as_uint(g_ent) &&
-                          (!a.logit_pre || __float_as_uint(a.g_used[3]) == __float_as_uint(g_kl));
-        if (same) return;
-    }
+    // reads the upstream gradients and refreshes the hint; the host never passes a `used` record here (the fused forward
+    // exists on the tile path only), so this launch always computes
+    float g[4];
+    upstream<4>(a.rec, true, ppo_owned(a), g);
+    const float g_pol = g[0], g_val = g[1], g_ent = g[2], g_kl = g[3];
     const float inv_s = 1.f / (float)a.S;
     const float inv_m = 1.f / ((float)a.S * (float)G);
     const long long per_cta = (MODE == 1) ? NT : NT / 32;
@@ -364,7 +335,7 @@ static int launch_tile(const PpoArgs& a, float* out, float* ws, size_t ws_bytes,
     if (per_sm > 6) per_sm = 6;
     const long long n_tiles = (a.S + PPO_R - 1) / PPO_R;
     // the verification launch that follows a fused forward normally exits at once: keep its grid to one CTA per SM
-    long long grid = (long long)sm_count * ((WHAT == PPO_BWD && a.g_used) ? 1 : per_sm);
+    long long grid = (long long)sm_count * ((WHAT == PPO_BWD && a.rec.used) ? 1 : per_sm);
     if (grid > n_tiles) grid = n_tiles;
     if (WHAT != PPO_BWD && !ws_partials_fit((long long)(grid * 6), ws_bytes)) return B200RL_ERR_WORKSPACE;
     if (int rc = launch_k(kern, (int)grid, PPO_THREADS, smem, st, a, out, ws)) return rc;
@@ -433,10 +404,9 @@ extern "C" int b200rl_ppo_fwd_grad(const float* logit_new, const float* logit_ol
     int rc = fill_args(a, logit_new, logit_old, logit_pretrained, action, value_new, value_old, adv, return_, weight,
                        S, G, N, clip_ratio, use_value_clip, dual_clip, kl_type, adv_stats, factor);
     if (rc != B200RL_OK) return rc;
-    if (!out || !workspace || !g_expected || !g_used || !grad_logit_new || !grad_value_new || S == 0)
+    if (!workspace || S == 0 || !upstream_args_ok(0, out, true, grad_logit_new && grad_value_new, g_expected, g_used))
         return B200RL_ERR_ARG;
-    a.g_policy = g_expected; a.g_value = g_expected + 1; a.g_entropy = g_expected + 2; a.g_kl = g_expected + 3;
-    a.g_used = g_used; a.grad_logit = grad_logit_new; a.grad_value = grad_value_new;
+    a.rec = forward_record(g_expected, g_used); a.grad_logit = grad_logit_new; a.grad_value = grad_value_new;
     if (!tile_path_ok(a)) return B200RL_ERR_ARG;  // callers probe with b200rl_ppo_fused_supported first
     return dispatch_tile<PPO_FWD_GRAD>(a, out, workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -465,10 +435,9 @@ extern "C" int b200rl_ppo_bwd(const float* logit_new, const float* logit_old, co
     int rc = fill_args(a, logit_new, logit_old, logit_pretrained, action, value_new, value_old, adv, return_, weight,
                        S, G, N, clip_ratio, use_value_clip, dual_clip, kl_type, adv_stats, factor);
     if (rc != B200RL_OK) return rc;
-    a.g_policy = g_policy; a.g_value = g_value; a.g_entropy = g_entropy; a.g_kl = g_kl;
-    a.g_used = const_cast<float*>(g_used); a.g_hint = g_hint;
+    if (!upstream_args_ok(1, nullptr, true, grad_logit_new && grad_value_new, nullptr, g_used)) return B200RL_ERR_ARG;
+    a.rec = verify_record(g_policy, g_value, g_entropy, g_kl, g_used, g_hint);
     a.grad_logit = grad_logit_new; a.grad_value = grad_value_new;
-    if (!grad_logit_new || !grad_value_new) return B200RL_ERR_ARG;
     if (S == 0) return B200RL_OK;
     cudaStream_t st = (cudaStream_t)stream;
     constexpr int NT = 128;

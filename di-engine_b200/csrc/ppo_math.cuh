@@ -24,17 +24,9 @@ struct PpoArgs {
     float dual_clip;  // <= 0: disabled
     int use_value_clip;
     int kl_type;  // 1,2,3
-    // upstream gradients (device scalars, nullable = 0): actual ones for BWD, expected ones for FWD_GRAD
-    const float* g_policy;
-    const float* g_value;
-    const float* g_entropy;
-    const float* g_kl;
     float* grad_logit;
     float* grad_value;
-    // FWD_GRAD: the 4 upstream values the gradients were scaled with are recorded here;
-    // BWD: when non-null and equal to the actual upstream values the launch is a no-op (gradients already written)
-    float* g_used;
-    float* g_hint;  // BWD: refreshed with the actual upstream values for the next forward pass (nullable)
+    UpstreamRecord rec;  // FWD_GRAD and BWD (ppo_owned slots)
     // nullable: {mean, std + 1e-8} of the advantage batch (device floats, b200rl_adv_stats): when given every kernel uses
     // (adv - mean) / (std + 1e-8) -- PPOPolicy's per-batch advantage normalisation (ding/policy/ppo.py:304-306) applied on load
     const float* adv_stats;
@@ -190,6 +182,9 @@ __host__ __device__ inline PpoTileLayout ppo_layout(int N, bool has_pre, bool ha
 struct PpoUpstream {
     float g_pol, g_val, g_ent, g_kl, inv_s;
 };
+
+// slots of the upstream-gradient record a PPO kernel owns: policy, value, entropy, and kl with logit_pretrained
+__device__ __forceinline__ unsigned ppo_owned(const PpoArgs& a) { return a.logit_pre ? 15u : 7u; }
 
 // One row (thread = row `tid` of the tile staged at `st`): softmax statistics, clipped surrogate, value term, optional
 // KL, loss partial sums (LOSSES) and the gradient row (GRADS; into the shared-memory tile `gtile` for full tiles, straight

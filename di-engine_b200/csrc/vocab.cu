@@ -239,9 +239,7 @@ struct VocabArgs {
     // PPO (VM_PPO*, VM_PPO_BWD*); adv is then per row and coef / coef_in the policy term's unit coefficient
     float* ent;                // forward: entropy of logit_new per row (PPO_ENT); VM_PPO_BWD: read (null = no entropy)
     float* coef_kl;            // forward: d kl_div / d lp_new per row (PPO_KL); VM_PPO_BWD: read (null = no KL)
-    const float *g_pol, *g_ent, *g_kl;  // forward: the expected upstream gradients; VM_PPO_BWD: the actual ones (null = 0)
-    float* g_used;             // forward: the upstream gradients its gradient was written for; VM_PPO_BWD: read (nullable)
-    float* g_hint;             // VM_PPO_BWD: refreshed with the actual upstream gradients (nullable)
+    UpstreamRecord rec;        // PPO forward and VM_PPO_BWD (slots policy, entropy, kl)
     float dual_clip, inv_m;    // dual_clip <= 0: off; inv_m = 1 / rows
     int kl_type;
 };
@@ -261,31 +259,6 @@ __device__ __forceinline__ void stream_vecs(const uint4* const (&p)[NR], int i, 
         if (ENT && r == 0) mst_add<W>(m[0], s[0], *t, x);
         else ms_add<W>(m[r], s[r], x);
     }
-}
-
-// PPO upstream gradients {policy, entropy, kl} (null = 0).  They are read where they are used, once per row, rather than
-// held in registers across the row loop.
-template <bool ENT>
-__device__ __forceinline__ void ppo_g(const VocabArgs& a, float& gp, float& ge, float& gk) {
-    gp = a.g_pol ? *a.g_pol : 0.f;
-    ge = (ENT && a.g_ent) ? *a.g_ent : 0.f;
-    gk = a.g_kl ? *a.g_kl : 0.f;
-}
-
-// the backward's view of the PPO upstream gradients: refresh the call site's record and report whether the forward
-// already wrote the gradient for exactly these values
-template <bool ENT>
-__device__ __forceinline__ bool ppo_upstream(const VocabArgs& a) {
-    float gp, ge, gk;
-    ppo_g<ENT>(a, gp, ge, gk);
-    if (a.g_hint && blockIdx.x == 0 && threadIdx.x == 0) {
-        a.g_hint[0] = gp;
-        if (ENT) a.g_hint[2] = ge;
-        a.g_hint[3] = gk;
-    }
-    return a.g_used && __float_as_uint(a.g_used[0]) == __float_as_uint(gp) &&
-           (!ENT || __float_as_uint(a.g_used[2]) == __float_as_uint(ge)) &&
-           (!a.coef_kl || __float_as_uint(a.g_used[3]) == __float_as_uint(gk));
 }
 
 template <class T, int MODE>
@@ -312,11 +285,13 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
         if (a.g) gscale = *a.g;
         if (a.skip_if_unit && gscale == 1.f) return;  // the forward launch already wrote exactly this gradient
     }
-    if (PBWD && ppo_upstream<ENT>(a)) return;
-    if (PPO && want_grad && blockIdx.x == 0 && tid == 0) {  // record the upstream gradients the forward writes for
-        float gp, ge, gk;
-        ppo_g<ENT>(a, gp, ge, gk);
-        a.g_used[0] = gp; a.g_used[1] = 0.f; a.g_used[2] = ge; a.g_used[3] = KL ? gk : 0.f;
+    // PPO upstream-gradient slots: policy, entropy with the bonus, kl with logit_pretrained.  The record is written (forward)
+    // or verified (VM_PPO_BWD) here; the values are read again where they are used, once per row, rather than held in
+    // registers across the row loop.
+    const unsigned owned = 1u | (ENT ? 4u : 0u) | ((KL || (PBWD && a.coef_kl)) ? 8u : 0u);
+    if (PBWD || (PPO && want_grad)) {
+        float g[4];
+        if (upstream<4>(a.rec, PBWD, owned, g)) return;  // VM_PPO_BWD: the forward wrote exactly this gradient
     }
     float part[NP] = {0.f, 0.f, 0.f};  // thread 0: the loss partial sums of this CTA's rows (loss, approx_kl, clipfrac; PPO: 5)
     float w_tot = (float)a.S;  // thread 0: sum_s w[b, s] of the current row's sequence (S without weights)
@@ -341,11 +316,10 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
             lse = a.lse[row];
             act = a.action[row];
         } else if (PBWD) {
-            float gp, ge, gk;
-            ppo_g<ENT>(a, gp, ge, gk);
+            const float gp = upstream_value(a.rec, owned, 0), gk = upstream_value(a.rec, owned, 3);
             c = gp * a.coef_in[row] + (a.coef_kl ? gk * a.coef_kl[row] : 0.f);
             if (ENT) {
-                ce = ge * (a.weight ? a.weight[row] : 1.f) * a.inv_m;
+                ce = upstream_value(a.rec, owned, 2) * (a.weight ? a.weight[row] : 1.f) * a.inv_m;
                 H = a.ent[row];
             }
             lse = a.lse[row];
@@ -437,10 +411,9 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
                     }
                     if (ENT) a.ent[row] = H;
                     if (want_grad) {
-                        float gp, ge, gk;
-                        ppo_g<ENT>(a, gp, ge, gk);
-                        c = gp * cp + (KL ? gk * dk * a.inv_m : 0.f);
-                        ce = ge * w * a.inv_m;
+                        c = upstream_value(a.rec, owned, 0) * cp +
+                            (KL ? upstream_value(a.rec, owned, 3) * dk * a.inv_m : 0.f);
+                        ce = upstream_value(a.rec, owned, 2) * w * a.inv_m;
                     }
                     part[0] -= sel * w;
                     part[1] += H * w;
@@ -653,16 +626,16 @@ extern "C" int b200rl_ppo_lm_fwd_grad(int dtype, const void* logit_new, const vo
     const bool kl = logit_pretrained != nullptr;
     if (!sizes_ok(rows, 1, V) || !aligned_logits(logit_new) || !aligned_logits(logit_old) ||
         (kl && (!aligned16(logit_pretrained) || !dlogp_kl || kl_type < 1 || kl_type > 3)) || !action || !adv ||
-        !out5 || !lse_new || !dlogp_policy || (entropy && !entropy_row) || !workspace ||
-        (grad_logit_new && (!aligned16(grad_logit_new) || !g_expected || !g_used)))
+        !lse_new || !dlogp_policy || (entropy && !entropy_row) || !workspace ||
+        (grad_logit_new && !aligned16(grad_logit_new)) ||
+        !upstream_args_ok(0, out5, grad_logit_new, grad_logit_new, g_expected, g_used))
         return B200RL_ERR_ARG;
     VocabArgs a{};
     a.x[0] = logit_new; a.x[1] = logit_old; a.x[2] = logit_pretrained;
     a.action = action; a.adv = adv; a.weight = weight;
     a.lse = lse_new; a.coef = dlogp_policy; a.coef_kl = dlogp_kl; a.ent = entropy_row; a.grad = grad_logit_new;
     a.ws = workspace;
-    if (g_expected) a.g_pol = g_expected, a.g_ent = g_expected + 2, a.g_kl = g_expected + 3;
-    a.g_used = g_used;
+    a.rec = forward_record(g_expected, g_used);
     a.rows = rows; a.S = 1; a.V = V;
     a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio); a.dual_clip = (float)dual_clip;
     a.kl_type = kl_type; a.inv_m = (float)(1.0 / (double)rows);
@@ -682,13 +655,13 @@ extern "C" int b200rl_ppo_lm_bwd(int dtype, const void* logit_new, const long lo
                                  const float* g_entropy, const float* g_kl, const float* g_used, float* g_hint,
                                  void* grad_logit_new, void* stream) {
     if (!sizes_ok(rows, 1, V) || !aligned_logits(logit_new) || !action || !lse_new || !dlogp_policy ||
-        !grad_logit_new || !aligned16(grad_logit_new))
+        !upstream_args_ok(1, nullptr, true, grad_logit_new, nullptr, g_used) || !aligned16(grad_logit_new))
         return B200RL_ERR_ARG;
     VocabArgs a{};
     a.x[0] = logit_new; a.action = action; a.weight = weight;
     a.lse = const_cast<float*>(lse_new); a.ent = const_cast<float*>(entropy_row); a.coef_in = dlogp_policy;
     a.coef_kl = const_cast<float*>(dlogp_kl);
-    a.g_pol = g_policy; a.g_ent = g_entropy; a.g_kl = g_kl; a.g_used = const_cast<float*>(g_used); a.g_hint = g_hint;
+    a.rec = verify_record(g_policy, nullptr, g_entropy, g_kl, g_used, g_hint);
     a.grad = grad_logit_new;
     a.rows = rows; a.S = 1; a.V = V;
     a.inv_m = (float)(1.0 / (double)rows);

@@ -17,8 +17,9 @@
 //
 // Backward contract (as ppo.cu's FWD_GRAD): the gradients are produced in the forward launch for the upstream gradients the
 // training loop is expected to send (g_expected, remembered on the device).  backward() launches the same kernel in verify
-// mode: every CTA compares the actual upstream gradients with the recorded ones and exits at once when they agree;
-// otherwise the whole step is recomputed with the actual values.  Exact for any upstream gradient, no host sync.
+// mode: every CTA compares the actual upstream gradients with the recorded ones (upstream(), common.cuh) and exits at once
+// when they agree; otherwise the whole step is recomputed with the actual values.  Exact for any upstream gradient, no host
+// sync.
 #include "../../include/b200rl.h"
 #include "ppo_math.cuh"
 
@@ -42,13 +43,7 @@ struct VtFusedArgs {
     long long T, B;
     int N;
     float gamma, gamma_lambda, rho_clip, c_clip, rho_pg_clip;
-    const float* g_expected;  // 3 device scalars: d total / d (policy, value, entropy) loss the forward launch assumes
-    const float* g_pg;        // verify mode: the actual upstream gradients (nullable = 0)
-    const float* g_val;
-    const float* g_ent;
-    int verify;
-    float* g_used;            // forward: the 3 values the gradients were scaled with; verify: compared, never written
-    float* g_hint;            // verify: refreshed with the actual values for the next forward launch (nullable)
+    UpstreamRecord rec;       // slots policy, value, entropy
     float* grad_logit;        // (T*B, N), nullable = losses only
     float* grad_value;        // (T+1, B)
     int trace;
@@ -112,24 +107,9 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
         mbar_fence_init();
     }
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    // upstream gradients: expected ones in the forward launch, actual ones in verify mode (exit when they were expected)
-    float g_pg = 0.f, g_val = 0.f, g_ent = 0.f;
-    if (GRADS) {
-        if (a.verify) {
-            g_pg = a.g_pg ? *a.g_pg : 0.f;
-            g_val = a.g_val ? *a.g_val : 0.f;
-            g_ent = a.g_ent ? *a.g_ent : 0.f;
-            if (a.g_hint && blockIdx.x == 0 && tid == 0) {
-                a.g_hint[0] = g_pg; a.g_hint[1] = g_val; a.g_hint[2] = g_ent;
-            }
-            if (g_pg == a.g_used[0] && g_val == a.g_used[1] && g_ent == a.g_used[2]) return;  // uniform over the grid
-        } else {
-            g_pg = a.g_expected[0]; g_val = a.g_expected[1]; g_ent = a.g_expected[2];
-            if (blockIdx.x == 0 && tid == 0) {
-                a.g_used[0] = g_pg; a.g_used[1] = g_val; a.g_used[2] = g_ent;
-            }
-        }
-    }
+    float g[3] = {0.f, 0.f, 0.f};
+    if (GRADS && upstream<3>(a.rec, a.rec.verify, 7u, g)) return;  // uniform over the grid
+    const float g_pg = g[0], g_val = g[1], g_ent = g[2];
     __syncthreads();
 
     auto item_valid = [&](const VwItem& it) { return it.tile < n_tiles; };
@@ -422,7 +402,7 @@ __global__ void __launch_bounds__(VW_THREADS, 2) vtrace_ws_kernel(VtFusedArgs a,
             p_lse = n_lse; p_lp = n_lp; p_ent = n_ent; p_is = n_is;
         }
     }
-    if (!a.verify) grid_store_partials<3, VW_THREADS>(acc, ws);  // summed by finalize_sums_kernel
+    if (!a.rec.verify) grid_store_partials<3, VW_THREADS>(acc, ws);  // summed by finalize_sums_kernel
 }
 
 static size_t vw_smem(int N, bool has_w, int stages, int tc) {
@@ -474,23 +454,9 @@ __global__ void __launch_bounds__(VR_NT) vtrace_res_kernel(VtFusedArgs a, float*
     float* sis = sr + E;               // [T][TC]
     float* svs = sis + E;              // [T+1][TC]
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    float g_pg = 0.f, g_val = 0.f, g_ent = 0.f;
-    if (GRADS) {
-        if (a.verify) {
-            g_pg = a.g_pg ? *a.g_pg : 0.f;
-            g_val = a.g_val ? *a.g_val : 0.f;
-            g_ent = a.g_ent ? *a.g_ent : 0.f;
-            if (a.g_hint && blockIdx.x == 0 && tid == 0) {
-                a.g_hint[0] = g_pg; a.g_hint[1] = g_val; a.g_hint[2] = g_ent;
-            }
-            if (g_pg == a.g_used[0] && g_val == a.g_used[1] && g_ent == a.g_used[2]) return;  // uniform over the grid
-        } else {
-            g_pg = a.g_expected[0]; g_val = a.g_expected[1]; g_ent = a.g_expected[2];
-            if (blockIdx.x == 0 && tid == 0) {
-                a.g_used[0] = g_pg; a.g_used[1] = g_val; a.g_used[2] = g_ent;
-            }
-        }
-    }
+    float g[3] = {0.f, 0.f, 0.f};
+    if (GRADS && upstream<3>(a.rec, a.rec.verify, 7u, g)) return;  // uniform over the grid
+    const float g_pg = g[0], g_val = g[1], g_ent = g[2];
     // ---- the whole tile, one burst: per time step one contiguous segment of W * esz bytes per tensor ------------------------
     // A thread owns one 16-byte column of the row segment and walks down the rows: two pointer increments per copy, no
     // division in the loop (the p -> (row, piece) arithmetic of a flat loop was 31 % of the kernel's instructions).
@@ -657,7 +623,7 @@ __global__ void __launch_bounds__(VR_NT) vtrace_res_kernel(VtFusedArgs a, float*
             a.grad_value[g] = g_val * (2.f * w * dv * inv_m);
         }
     }
-    if (!a.verify) grid_store_partials<3, VR_NT>(acc, ws);  // summed by finalize_sums_kernel
+    if (!a.rec.verify) grid_store_partials<3, VR_NT>(acc, ws);  // summed by finalize_sums_kernel
 }
 
 static int g_vt_impl = 0;  // b200rl_vtrace_set_impl: 0 = automatic, 1 = streaming column tiles only, 2 = resident tiles first
@@ -678,7 +644,7 @@ static int launch_vtres(const VtFusedArgs& a, float* out, float* ws, size_t ws_b
     const long long grid = (a.B + TC - 1) / TC;
     if (ws_bytes < WS_MIN_BYTES || !ws_partials_fit((long long)(grid * 3), ws_bytes)) return B200RL_ERR_WORKSPACE;
     if (int rc = launch_k(kern, (int)grid, VR_NT, smem, st, a, ws)) return rc;
-    if (a.verify) return B200RL_OK;
+    if (a.rec.verify) return B200RL_OK;
     return launch_finalize(ws, out, vtrace_finalize_args(a.T, a.B, (int)grid), st);
 }
 
@@ -719,7 +685,7 @@ static int launch_vtws(const VtFusedArgs& a, float* out, float* ws, size_t ws_by
     if (ws_bytes < WS_MIN_BYTES || !ws_partials_fit((long long)(grid * 3), ws_bytes))
         return B200RL_ERR_WORKSPACE;
     if (int rc = launch_k(kern, (int)grid, VW_THREADS, smem, st, a, ws, stages)) return rc;
-    if (a.verify) return B200RL_OK;
+    if (a.rec.verify) return B200RL_OK;
     return launch_finalize(ws, out, vtrace_finalize_args(a.T, a.B, (int)grid), st);
 }
 
@@ -776,14 +742,13 @@ extern "C" int b200rl_vtrace_fwd_grad(const float* target_output, const float* b
     if (!target_output || !behaviour_output || !action || !value || !reward || !workspace || T < 1 || B < 1 || N < 1)
         return B200RL_ERR_ARG;
     const bool grads = grad_target_output != nullptr;
-    if (grads && (!grad_value || !g_used || (!verify && !g_expected))) return B200RL_ERR_ARG;
-    if (verify && !grads) return B200RL_ERR_ARG;
-    if (!verify && !out3) return B200RL_ERR_ARG;
+    if (!upstream_args_ok(verify, out3, grads, grads && grad_value, g_expected, g_used)) return B200RL_ERR_ARG;
     VtFusedArgs a{};
     fill_vt(a, target_output, behaviour_output, action, value, reward, weight, T, B, N, gamma, lambda_, rho_clip_ratio,
             c_clip_ratio, rho_pg_clip_ratio);
-    a.g_expected = g_expected; a.verify = verify ? 1 : 0; a.g_pg = g_policy; a.g_val = g_value; a.g_ent = g_entropy;
-    a.g_used = g_used; a.g_hint = g_hint; a.grad_logit = grad_target_output; a.grad_value = grad_value;
+    a.rec = verify ? verify_record(g_policy, g_value, g_entropy, nullptr, g_used, g_hint)
+                   : forward_record(g_expected, g_used);
+    a.grad_logit = grad_target_output; a.grad_value = grad_value;
     cudaStream_t st = (cudaStream_t)stream;
     // streaming column tiles wherever they fit (faster: they overlap loads with the scan); resident tiles take the shapes
     // they cannot (N > 14: no three-stage ring), and every shape they fit under b200rl_vtrace_set_impl(2)

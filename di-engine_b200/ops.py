@@ -184,11 +184,6 @@ def _forward_grads(ctx):
     return spec
 
 
-def _nan_g_used(n, device):
-    """an expected-gradient slot that matches no upstream gradient: the verify launch recomputes"""
-    return torch.full((n, ), float('nan'), dtype=torch.float32, device=device)
-
-
 def _unit_grad(ctx, other_grads, fresh):
     """For the backward launches that take ``skip_if_unit`` (TD family, UPGO): (the forward-written gradient for a unit
     upstream gradient, 1) when it is still there and no gradient arrived through an output other than the loss; else
@@ -956,8 +951,7 @@ class A2CFunction(torch.autograd.Function):
         logit, value, action, adv, return_, weight = ctx.saved_tensors
         S, N = ctx.cfg
         keep, (pp, pv, pe) = _grads(g_p, g_v, g_e)
-        gl, gv, g_used = _forward_grads(ctx) or (torch.empty_like(logit), torch.empty_like(value),
-                                                 _nan_g_used(4, logit.device))
+        gl, gv, g_used = _forward_grads(ctx) or (torch.empty_like(logit), torch.empty_like(value), None)
         with on_device(logit.device):
             ws = workspace(logit.device)
             rc = lib().b200rl_a2c_fwd_grad(ptr(logit), ptr(action), ptr(value), ptr(adv), ptr(return_), ptr(weight), S, N,
@@ -1001,7 +995,7 @@ class A2CContinuousFunction(torch.autograd.Function):
         S, D = ctx.cfg
         keep, (pp, pv, pe) = _grads(g_p, g_v, g_e)
         gm, gs, gv, g_used = _forward_grads(ctx) or (torch.empty_like(mu), torch.empty_like(sigma), torch.empty_like(value),
-                                                     _nan_g_used(4, mu.device))
+                                                     None)
         with on_device(mu.device):
             ws = workspace(mu.device)
             rc = lib().b200rl_a2c_continuous_fwd_grad(
@@ -1049,7 +1043,7 @@ class PPOContinuousFunction(torch.autograd.Function):
          weight) = ctx.saved_tensors
         keep, (pp, pv, pe, pk) = _grads(g_p, g_v, g_e, g_k)
         gm, gs, gv, g_used = _forward_grads(ctx) or (torch.empty_like(mu), torch.empty_like(sigma),
-                                                     torch.empty_like(value_new), _nan_g_used(4, mu.device))
+                                                     torch.empty_like(value_new), None)
         with on_device(mu.device):
             ws = workspace(mu.device)
             rc = lib().b200rl_ppo_continuous_fwd_grad(
@@ -1149,7 +1143,7 @@ class VTraceFunction(torch.autograd.Function):
             target_output, behaviour_output, action, value, reward, weight = ctx.saved_tensors
             dev = target_output.device
             grad_logit, grad_value, g_used = _forward_grads(ctx) or (
-                torch.empty_like(target_output), torch.empty(T + 1, B, dtype=torch.float32, device=dev), _nan_g_used(3, dev))
+                torch.empty_like(target_output), torch.empty(T + 1, B, dtype=torch.float32, device=dev), None)
             with on_device(dev):
                 ws = workspace(dev)
                 rc = lib().b200rl_vtrace_fwd_grad(

@@ -21,6 +21,15 @@
  *     the two calls (the autograd context in the PyTorch binding).
  *   - upstream gradients of the scalar losses are passed as device pointers to single floats (nullable = 0), so a
  *     backward launch never needs a host read.
+ *   - forward-written gradients: the forward launch of several losses also writes their gradients for the upstream
+ *     gradients the caller EXPECTS -- g_expected, device floats indexed by slot (0 policy, 1 value, 2 entropy, 3 kl), the
+ *     loss weights of the training loop -- and records the values it used in g_used.  The backward ("verify") launch
+ *     takes the actual upstream gradients: it does nothing when every slot the loss owns is bit-identical to g_used (the
+ *     gradients in memory are the right ones), and otherwise recomputes them with the actual values, so the pair is exact
+ *     for any upstream gradient.  A null g_used makes the verify launch recompute.  g_hint (nullable) receives the actual
+ *     values of the owned slots, for the caller's next forward launch to expect.  Slots a loss does not own read as 0: the
+ *     forward launch records them as 0, the verify launch neither compares nor refreshes them.  Each entry point below
+ *     names the slots it owns.
  */
 #ifndef B200RL_H_
 #define B200RL_H_
@@ -98,19 +107,17 @@ B200RL_API int b200rl_ppo_fwd(const float* logit_new, const float* logit_old, co
                    const float* factor, float* out, float* workspace, size_t workspace_bytes, void* stream);
 /* gradients of  g_policy*policy_loss + g_value*value_loss + g_entropy*entropy_loss + g_kl*kl_div  w.r.t.
  * logit_new (S*G, N) and value_new (S); autograd tie rules of torch.min/max/clamp reproduced (ppo.py:208-216,:269-272).
- * g_used / g_hint (both nullable) belong to the fused forward below: when g_used is given and equals the four actual
- * upstream values bit for bit, the gradients already sitting in grad_* are valid and the launch does nothing; g_hint
- * (4 floats) is refreshed with the actual upstream values so the next forward pass can expect them. */
+ * With g_used / g_hint (both nullable) it is the verify launch of b200rl_ppo_fwd_grad (forward-written gradients; owned
+ * slots: policy, value, entropy, and kl with logit_pretrained); a non-null g_used needs b200rl_ppo_fused_supported. */
 B200RL_API int b200rl_ppo_bwd(const float* logit_new, const float* logit_old, const float* logit_pretrained,
                    const long long* action, const float* value_new, const float* value_old, const float* adv,
                    const float* return_, const float* weight, long long S, long long G, long long N,
                    double clip_ratio, int use_value_clip, double dual_clip, int kl_type, const float* adv_stats,
                    const float* factor, const float* g_policy, const float* g_value, const float* g_entropy, const float* g_kl,
                    const float* g_used, float* g_hint, float* grad_logit_new, float* grad_value_new, void* stream);
-/* Fused forward: the losses of b200rl_ppo_fwd AND the gradients of b200rl_ppo_bwd for the EXPECTED upstream gradients
- * g_expected[0..3] (policy, value, entropy, kl; device floats -- the loss weights of the training loop), in one pass
- * over the batch.  g_used[0..3] records what was applied; pass it to b200rl_ppo_bwd, which verifies the expectation on
- * the device and only recomputes when it was wrong, so the pair is exact for any upstream gradient.
+/* Fused forward: the losses of b200rl_ppo_fwd AND the gradients of b200rl_ppo_bwd for the expected upstream gradients
+ * g_expected[0..3], in one pass over the batch -- the forward launch of the forward-written gradients (owned slots as
+ * b200rl_ppo_bwd, which is its verify launch; g_used has room for 4 floats).
  * Only available where b200rl_ppo_fused_supported(...) returns 1 (G == 1, N <= 32, 16-byte aligned tensors). */
 B200RL_API int b200rl_ppo_fwd_grad(const float* logit_new, const float* logit_old, const float* logit_pretrained,
                         const long long* action, const float* value_new, const float* value_old, const float* adv,
@@ -302,12 +309,10 @@ B200RL_API int b200rl_vtrace_continuous_bwd(const float* mu_target, const float*
 /* ---- vtrace_error_discrete_action in one launch: ding/rl_utils/vtrace.py:72-136 (returns :9-29, advantages :32-45,
  * importance weights isw.py:55-58), forward AND gradients (csrc/vtws.cu) -------------------------------------------------
  * Same semantics as b200rl_vtrace_fwd followed by b200rl_vtrace_bwd, but the batch crosses HBM once (96 B per transition at
- * N = 6): column tiles, warp-specialised loader / scanner / consumer warps.  The gradients are produced in the forward
- * launch (verify = 0) for the upstream gradients g_expected[3] = d total / d (policy, value, entropy) loss and the values
- * used are recorded in g_used[3].  backward() calls the function again with verify = 1 and the actual upstream gradients
- * (device scalars, null = 0): the launch is a no-op when they equal g_used, otherwise everything is recomputed with the
- * actual values (exact for any upstream gradient, no host sync); g_hint (nullable) is refreshed with the actual values.
- * grad_target_output == null (verify = 0 only): losses only.  out3 is written by the verify = 0 launch only.
+ * N = 6): column tiles, warp-specialised loader / scanner / consumer warps.  Forward-written gradients: verify = 0 is the
+ * forward launch (g_expected, g_used), verify = 1 the verify launch (g_policy, g_value, g_entropy, g_used, g_hint); owned
+ * slots: policy, value, entropy.  grad_target_output == null (verify = 0 only): losses only.  out3 is written by the
+ * verify = 0 launch only.
  * Two kernels behind the entry point: the streaming column tiles (any T; N <= 14 with weights: the stage ring has to fit two
  * CTAs per SM) and, for the rows they cannot take, resident tiles (the T x 8 | 4-column tile of a CTA fits shared memory twice
  * per SM: IMPALA unroll lengths, any N that fits).  Requires b200rl_vtrace_fused_supported(...) == 1 (one of the two fits,
@@ -396,10 +401,8 @@ B200RL_API int b200rl_fqf_fraction_bwd(const float* g_saved, const float* g_loss
                             int skip_if_unit, float* grad_quantiles, void* stream);
 
 /* ---- sibling heads (SURVEY section 8f rank 3), forward + gradients in ONE launch each (csrc/heads.cu) ---------------------
- * Same backward contract as b200rl_vtrace_fwd_grad: verify = 0 writes the losses and (grad_* non-null) the gradients for the
- * expected upstream gradients g_expected[k], recording them in g_used; verify = 1 with the actual upstream gradients (device
- * scalars, null = 0) returns at once when they equal g_used and recomputes the gradients otherwise; g_hint (nullable) is
- * refreshed with the actual values.
+ * Forward-written gradients with verify = 0 / 1 as b200rl_vtrace_fwd_grad (grad_* null, verify = 0 only: losses only).
+ * Owned slots: policy, value, entropy; ppo_error_continuous also kl with the pretrained pair.
  * a2c_error (ding/rl_utils/a2c.py:10-44): logit (S, N), action (S) int64, value / adv / return_ / weight(nullable) (S);
  * out3 = policy_loss -mean(logp*adv*w), value_loss mean(w*(return_-value)^2), entropy_loss mean(H*w).
  * ppo_error_continuous (ding/rl_utils/ppo.py:278-374): Independent(Normal(mu, sigma)) policies, mu / sigma / action (S, D)
@@ -519,12 +522,12 @@ B200RL_API int b200rl_gae_ppo_set_impl(int impl);
  *   dlogp_policy (rows) = (-w / M) * dsel/dr * r and dlogp_kl (rows, only with logit_pretrained) = dk/dx / M.
  *   grad_logit_new (nullable = no gradient; dtype of the logits) = c_act * (onehot(a) - p) - c_ent * p * (log p + H),
  *   p = softmax(logit_new[row]), log p clamped at -FLT_MAX, c_act = g_pol * dlogp_policy + g_kl * dlogp_kl,
- *   c_ent = g_ent * w / M, for the expected upstream gradients g_expected[0] (policy), [2] (entropy), [3] (kl) -- a device
- *   record laid out as the PPO records {policy, value, entropy, kl}; g_used (4 floats) receives the values used.
+ *   c_ent = g_ent * w / M, for the expected upstream gradients g_expected (forward-written gradients; owned slots: policy,
+ *   entropy with `entropy`, kl with logit_pretrained; g_expected and g_used hold 4 floats).
  * b200rl_ppo_lm_bwd: the same gradient for the actual upstream gradients g_policy, g_entropy, g_kl (device scalars,
  *   nullable = 0) from the saved rows (entropy_row / dlogp_kl null = no entropy / KL term): one read of logit_new, one
- *   write.  g_used (nullable): the launch returns at once on the device when the upstream gradients equal it (the forward
- *   already wrote exactly this gradient); g_hint (nullable) is refreshed with them ([0], [2] with entropy, [3]). */
+ *   write.  The verify launch of b200rl_ppo_lm_fwd_grad (g_used, g_hint nullable; owned slots: policy, entropy with
+ *   entropy_row, kl with dlogp_kl). */
 #define B200RL_DTYPE_F32 0
 #define B200RL_DTYPE_BF16 1
 B200RL_API int b200rl_grpo_fwd_grad(int dtype, const void* logit_new, const void* logit_old, const void* logit_ref,

@@ -83,6 +83,34 @@ def test_gae_ppo_supported_shapes():
     assert supported(128, 4098, 6) == 0  # B % 4 != 0
 
 
+def test_upstream_record_arguments_are_checked_before_any_launch():
+    """the argument rule of the forward-written gradients (host arithmetic, no CUDA call): a verify launch needs its
+    gradient buffers, a forward launch that writes gradients needs the expected values and the record"""
+    lib = _lib.load()
+    a = 1 << 20
+    ws = 1 << 20
+
+    def a2c(verify, g_expected, g_used, grad_logit):
+        return lib.b200rl_a2c_fwd_grad(a, a, a, a, a, None, 4, 5, g_expected, verify, a, a, a, g_used, None, a,
+                                       grad_logit, a, a, ws, None)
+
+    def vtrace(verify, g_expected, g_used, grad_target):
+        return lib.b200rl_vtrace_fwd_grad(a, a, a, a, a, None, 3, 4, 5, 0.99, 0.95, 1.0, 1.0, 1.0, g_expected, verify, a,
+                                          a, a, g_used, None, a, grad_target, a, a, ws, None)
+
+    for call in (a2c, vtrace):
+        assert call(1, None, a, None) == B200RL_ERR_ARG
+        assert call(0, a, None, a) == B200RL_ERR_ARG
+        assert call(0, None, a, a) == B200RL_ERR_ARG
+    assert lib.b200rl_ppo_lm_bwd(0, a, a, None, 4, 64, a, None, a, None, a, None, None, None, None, None,
+                                 None) == B200RL_ERR_ARG
+    assert lib.b200rl_ppo_lm_fwd_grad(0, a, a, None, a, a, None, 4, 64, 0.2, 0.0, 1, 0, a, None, a, a, None, a, None, a,
+                                      a, ws, None) == B200RL_ERR_ARG
+
+
+B200RL_ERR_ARG = -1
+
+
 def test_namedtuple_fields_match_reference():
     r = b2.rl_utils
     assert r.gae_data._fields == ('value', 'next_value', 'reward', 'done', 'traj_flag')  # gae.py:5
