@@ -104,20 +104,25 @@ struct VecT<__nv_bfloat16> {
 // torch's logsumexp takes an infinite maximum as 0
 __device__ __forceinline__ float lse_ref(float m) { return fabsf(m) == INFINITY ? 0.f : m; }
 
+// e^d: exp2f(d * log2 e), or expf(d) where the entropy accumulator takes it (EXPF, see mst_add), so that every logit
+// stream of a kernel forms its logsumexp with the same arithmetic (bit-identical streams give a ratio of exactly 1)
+template <bool EXPF>
+__device__ __forceinline__ float exp_of(float d) { return EXPF ? expf(d) : exp2f(d * kL2E); }
+
 // online (max, sum exp(z - lse_ref(max))) over n values
-template <int N>
+template <int N, bool EXPF = false>
 __device__ __forceinline__ void ms_add(float& m, float& s, const float (&x)[N]) {
     float mc = x[0];
 #pragma unroll
     for (int i = 1; i < N; ++i) mc = fmaxf(mc, x[i]);
     if (mc > m) {
-        if (s != 0.f) s *= exp2f((lse_ref(m) - lse_ref(mc)) * kL2E);
+        if (s != 0.f) s *= exp_of<EXPF>(lse_ref(m) - lse_ref(mc));
         m = mc;
     }
     const float r = lse_ref(m);
     float e[N];
 #pragma unroll
-    for (int i = 0; i < N; ++i) e[i] = exp2f((x[i] - r) * kL2E);
+    for (int i = 0; i < N; ++i) e[i] = exp_of<EXPF>(x[i] - r);
     // pairwise within the vector, then one add to the running sum: a thread's sequential chain over a 152k-entry row is
     // N times shorter, and so is its fp32 rounding
 #pragma unroll
@@ -127,16 +132,20 @@ __device__ __forceinline__ void ms_add(float& m, float& s, const float (&x)[N]) 
     s += e[0];
 }
 
+template <bool EXPF = false>
 __device__ __forceinline__ void ms_merge(float& m, float& s, float m2, float s2) {
     if (m2 > m) {
         const float tm = m, ts = s;
         m = m2; s = s2; m2 = tm; s2 = ts;
     }
-    if (s2 != 0.f) s += s2 * exp2f((lse_ref(m2) - lse_ref(m)) * kL2E);
+    if (s2 != 0.f) s += s2 * exp_of<EXPF>(lse_ref(m2) - lse_ref(m));
 }
 
 // ms_add with the entropy accumulator t = sum e^(z - r) * max(z - r, -FLT_MAX), r = lse_ref(max): a new max r' rescales
-// it as t <- alpha * (t + s * (r - r')), alpha = e^(r - r'), and -inf logits add 0 (Categorical.entropy's clamp)
+// it as t <- alpha * (t + s * (r - r')), alpha = e^(r - r'), and -inf logits add 0 (Categorical.entropy's clamp).  The
+// exponentials here are expf, not exp2f((z - r) * log2 e): fp32 log2 e is off by 1.3e-8 relative, so every term with
+// z - r ~ -50 carries the same ~7e-7 relative error, which does not average out and is all of H on a peaked row; the
+// other logit streams of these kernels (ms_add / ms_merge with EXPF) take the same exponentials
 template <int N>
 __device__ __forceinline__ void mst_add(float& m, float& s, float& t, const float (&x)[N]) {
     float mc = x[0];
@@ -144,7 +153,7 @@ __device__ __forceinline__ void mst_add(float& m, float& s, float& t, const floa
     for (int i = 1; i < N; ++i) mc = fmaxf(mc, x[i]);
     if (mc > m) {
         if (s != 0.f) {
-            const float d = lse_ref(m) - lse_ref(mc), al = exp2f(d * kL2E);
+            const float d = lse_ref(m) - lse_ref(mc), al = exp_of<true>(d);
             t = al * fmaf(s, d, t);
             s *= al;
         }
@@ -154,7 +163,7 @@ __device__ __forceinline__ void mst_add(float& m, float& s, float& t, const floa
     float e[N], u[N];
 #pragma unroll
     for (int i = 0; i < N; ++i) {
-        e[i] = exp2f((x[i] - r) * kL2E);
+        e[i] = exp_of<true>(x[i] - r);
         u[i] = e[i] * fmaxf(x[i] - r, kF32Min);
     }
 #pragma unroll
@@ -171,7 +180,7 @@ __device__ __forceinline__ void mst_merge(float& m, float& s, float& t, float m2
         m = m2; s = s2; t = t2; m2 = tm; s2 = ts; t2 = tt;
     }
     if (s2 != 0.f) {
-        const float d = lse_ref(m2) - lse_ref(m), al = exp2f(d * kL2E);
+        const float d = lse_ref(m2) - lse_ref(m), al = exp_of<true>(d);
         s += s2 * al;
         t += al * fmaf(s2, d, t2);
     }
@@ -198,8 +207,10 @@ __device__ __forceinline__ TokenHead token_head(float lp_new, float lp_old, floa
     const float gm = -gt;
     const float gu = u < c ? gm : (u == c ? 0.5f * gm : 0.f);
     const float gc = c < u ? gm : (u == c ? 0.5f * gm : 0.f);
-    const float inside = (ratio >= lo && ratio <= hi) ? 1.f : 0.f;
-    h.dlp = (gu * adv + gc * adv * inside) * ratio;
+    // clamp() passes its gradient by selection, as torch's where(): a NaN gt (a sequence whose weights sum to 0) reaches
+    // only the rows whose selected branch carries it, so the NaN pattern is the reference's
+    const bool inside = ratio >= lo && ratio <= hi;
+    h.dlp = (gu * adv + (inside ? gc * adv : 0.f)) * ratio;
     if (KL) {
         const float dr = lp_ref - lp_new;
         const float e = expf(dr);
@@ -211,13 +222,15 @@ __device__ __forceinline__ TokenHead token_head(float lp_new, float lp_old, floa
     return h;
 }
 
-// leave-one-out advantage of row b from reward (K, Bp): (k, j) = (b / Bp, b % Bp), baseline = (sum_k r[k, j] - r) / (K - 1)
+// leave-one-out advantage of row b from reward (K, Bp): (k, j) = (b / Bp, b % Bp), baseline = (sum_k r[k, j] - r) / (K - 1),
+// in fp64 and rounded once: rewards with a large common offset and a small spread cancel here, and an fp32 sum of K of
+// them loses the spread (K equal rewards give exactly 0 only so)
 __device__ __forceinline__ float rloo_adv(const float* __restrict__ reward, int K, long long Bp, long long b) {
     const long long k = b / Bp, j = b - k * Bp;
-    float sum = 0.f;
-    for (int q = 0; q < K; ++q) sum += reward[(long long)q * Bp + j];
-    const float r = reward[k * Bp + j];
-    return r - (sum - r) / (float)(K - 1);
+    double sum = 0.0;
+    for (int q = 0; q < K; ++q) sum += (double)reward[(long long)q * Bp + j];
+    const double r = reward[k * Bp + j];
+    return (float)(r - (sum - r) / (double)(K - 1));
 }
 
 struct VocabArgs {
@@ -257,7 +270,7 @@ __device__ __forceinline__ void stream_vecs(const uint4* const (&p)[NR], int i, 
         float x[W];
         VecT<T>::unpack(u[r], x);
         if (ENT && r == 0) mst_add<W>(m[0], s[0], *t, x);
-        else ms_add<W>(m[r], s[r], x);
+        else ms_add<W, ENT>(m[r], s[r], x);
     }
 }
 
@@ -350,7 +363,7 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
                 for (int r = 0; r < NR; ++r) {
                     const float x[1] = {V_::to_f(rp[r][e])};
                     if (ENT && r == 0) mst_add<1>(m[0], s[0], t, x);
-                    else ms_add<1>(m[r], s[r], x);
+                    else ms_add<1, ENT>(m[r], s[r], x);
                 }
             }
             float wsum = 0.f;
@@ -368,7 +381,7 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
                 for (int o = 16; o > 0; o >>= 1) {
                     const float m2 = __shfl_down_sync(0xffffffffu, m[r], o), s2 = __shfl_down_sync(0xffffffffu, s[r], o);
                     if (ENT && r == 0) mst_merge(m[0], s[0], t, m2, s2, __shfl_down_sync(0xffffffffu, t, o));
-                    else ms_merge(m[r], s[r], m2, s2);
+                    else ms_merge<ENT>(m[r], s[r], m2, s2);
                 }
                 if (lane == 0) s_m[r][wid] = m[r], s_s[r][wid] = s[r];
             }
@@ -390,7 +403,7 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
                         for (int w = 1; w < VOCAB_NT / 32; ++w) mst_merge(mm, ss, tt, s_m[0][w], s_s[0][w], s_t[w]);
                         H = logf(ss) - tt / ss;
                     } else {
-                        for (int w = 1; w < VOCAB_NT / 32; ++w) ms_merge(mm, ss, s_m[r][w], s_s[r][w]);
+                        for (int w = 1; w < VOCAB_NT / 32; ++w) ms_merge<ENT>(mm, ss, s_m[r][w], s_s[r][w]);
                     }
                     const float l = logf(ss) + lse_ref(mm);
                     if (r == 0) lse = l;
@@ -402,7 +415,9 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
                     const float w = a.weight ? a.weight[row] : 1.f;
                     const float ratio = expf(lp[0] - lp[1]);
                     float dsel, dk = 0.f, klv = 0.f;
-                    const float sel = surrogate(ratio, a.adv[row], a.lo, a.hi, a.dual_clip, dsel);
+                    const float adv = a.adv[row];
+                    float sel = surrogate(ratio, adv, a.lo, a.hi, a.dual_clip, dsel);
+                    if (ratio * adv != ratio * adv) sel = __int_as_float(0x7fc00000);  // torch.min / max propagate NaN
                     const float cp = -w * a.inv_m * dsel * ratio;  // d policy_loss / d lp_new
                     a.coef[row] = cp;
                     if (KL) {

@@ -56,13 +56,14 @@ def checksum(d):
     return np.array([float(d[k].double().abs().sum()) for k in sorted(d) if isinstance(d[k], torch.Tensor)])
 
 
-def logp64(logits, index):
-    x = logits.double()
+def logp64(logits, index, dtype=torch.float64):
+    """log softmax(logits)[index] in ``dtype`` (float32: the reference's efficient_method on fp32 logits)"""
+    x = logits.to(dtype)
     return x.gather(-1, index.unsqueeze(-1)).squeeze(-1) - torch.logsumexp(x, -1)
 
 
-def rloo_adv64(reward):
-    r = reward.double().reshape(reward.shape[0], -1)
+def rloo_adv64(reward, dtype=torch.float64):
+    r = reward.to(dtype).reshape(reward.shape[0], -1)
     return (r - (r.sum(0) - r) / (r.shape[0] - 1)).flatten()
 
 
@@ -81,14 +82,15 @@ def head64(lp_new, lp_old, lp_ref, adv, weight, clip=CLIP, beta=BETA):
     return loss, (lp_old - lp_new).mean().detach(), ((ratio > hi) | (ratio < lo)).to(tok.dtype).mean()
 
 
-def run64(d, clip=CLIP, beta=BETA):
+def run64(d, clip=CLIP, beta=BETA, dtype=torch.float64):
     """float64 results of the case dict `d` (any device): loss, approx_kl, clipfrac, lp_new (B, S) and dlp (B, S) =
-    d loss / d lp_new; d loss / d logit_new[row] = dlp[row] * (onehot - softmax) (``grad_rows64``)"""
+    d loss / d lp_new; d loss / d logit_new[row] = dlp[row] * (onehot - softmax) (``grad_rows64``).  ``dtype`` float32
+    restates the reference's own fp32 arithmetic on the same inputs (bf16 logits widened to fp32); 'scale' stays float64"""
     B = d['logit_new'].shape[0]
-    lp = {k: torch.stack([logp64(d[k][b], d['action'][b]) for b in range(B)])
+    lp = {k: torch.stack([logp64(d[k][b], d['action'][b], dtype) for b in range(B)])
           for k in ('logit_new', 'logit_old', 'logit_ref') if k in d}
     lp_new = lp['logit_new'].clone().requires_grad_(True)
-    adv = d['adv'] if 'adv' in d else rloo_adv64(d['reward'])
+    adv = d['adv'] if 'adv' in d else rloo_adv64(d['reward'], dtype)
     loss, kl, cf = head64(lp_new, lp['logit_old'], lp.get('logit_ref'), adv.to(lp_new.device), d['weight'], clip,
                           beta if 'logit_ref' in d else 0.0)
     loss.backward()
@@ -98,16 +100,19 @@ def run64(d, clip=CLIP, beta=BETA):
     w = torch.ones_like(lp_new) if d['weight'] is None else d['weight'].double().to(lp_new.device)
     gt = w / w.sum(1, keepdim=True) / B
     a = adv.double().to(lp_new.device).reshape(-1, 1).abs()
-    scale = gt * a * torch.exp(lp['logit_new'] - lp['logit_old'])
+    lpd = {k: v.double() for k, v in lp.items()}
+    scale = gt * a * torch.exp(lpd['logit_new'] - lpd['logit_old'])
     if 'logit_ref' in d:
-        scale = scale + gt * beta * (torch.exp(lp['logit_ref'] - lp['logit_new']) + 1)
+        scale = scale + gt * beta * (torch.exp(lpd['logit_ref'] - lpd['logit_new']) + 1)
     return {'loss': loss.item(), 'approx_kl': kl.item(), 'clipfrac': cf.item(), 'lp_new': lp['logit_new'],
             'dlp': lp_new.grad, 'scale': scale.detach()}
 
 
-def grad_rows64(logits, action, dlp):
-    """dlp[..., None] * (onehot(action) - softmax(logits)) in float64"""
-    x = logits.double()
-    g = -torch.softmax(x, -1) * dlp.unsqueeze(-1)
-    g.scatter_add_(-1, action.unsqueeze(-1), dlp.unsqueeze(-1).double())
+def grad_rows64(logits, action, dlp, dtype=torch.float64):
+    """dlp[..., None] * (onehot(action) - softmax(logits)) in float64; in float32 as the reference's autograd of
+    gather - logsumexp forms it, with softmax = exp(logits - logsumexp)"""
+    x = logits.to(dtype)
+    p = torch.softmax(x, -1) if dtype == torch.float64 else torch.exp(x - torch.logsumexp(x, -1, keepdim=True))
+    g = -p * dlp.unsqueeze(-1)
+    g.scatter_add_(-1, action.unsqueeze(-1), dlp.unsqueeze(-1).to(dtype))
     return g

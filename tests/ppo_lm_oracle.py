@@ -75,17 +75,26 @@ def checksum(d):
     return np.array(out)
 
 
-def run64(d, clip=CLIP, dual_clip=None, kl_type='k1', entropy_bonus=True, mix=MIX):
+def _normalized(x):
+    """log softmax(x): float64 as log_softmax; float32 as Categorical(logits=x).logits forms it, x - logsumexp(x)"""
+    if x.dtype == torch.float64:
+        return torch.log_softmax(x, -1)
+    return x - x.logsumexp(-1, keepdim=True)
+
+
+def run64(d, clip=CLIP, dual_clip=None, kl_type='k1', entropy_bonus=True, mix=MIX, dtype=torch.float64):
     """float64 results of the case dict `d` (any device): policy, entropy, kl, approx_kl, clipfrac and grad = d (mix[0] *
-    policy + mix[1] * entropy + mix[2] * kl) / d logit_new.  The clamp / clipfrac bounds are fp32(1 -+ clip), as torch
-    forms them for fp32 ratios; Categorical.entropy's clamp of log p at finfo.min makes a -inf logit contribute 0."""
-    x = d['logit_new'].double().requires_grad_(True)
+    policy + mix[1] * entropy + mix[2] * kl) / d logit_new, and per row lse, lp_new and H (entropy_bonus).  The clamp /
+    clipfrac bounds are fp32(1 -+ clip), as torch forms them for fp32 ratios; Categorical.entropy's clamp of log p at
+    finfo.min makes a -inf logit contribute 0.  ``dtype`` float32 restates the reference's own fp32 arithmetic on the same
+    inputs (bf16 logits widened to fp32), the clamp at finfo(float32).min included."""
+    x = d['logit_new'].detach().to(dtype, copy=True).requires_grad_(True)
     a = d['action'].unsqueeze(-1)
-    lsm = torch.log_softmax(x, -1)
+    lsm = _normalized(x)
     lp_new = lsm.gather(-1, a).squeeze(-1)
-    lp_old = torch.log_softmax(d['logit_old'].double(), -1).gather(-1, a).squeeze(-1)
-    adv = d['adv'].double().reshape(lp_new.shape)
-    w = torch.ones_like(adv) if d['weight'] is None else d['weight'].double().expand_as(adv)
+    lp_old = _normalized(d['logit_old'].to(dtype)).gather(-1, a).squeeze(-1)
+    adv = d['adv'].to(dtype).reshape(lp_new.shape)
+    w = torch.ones_like(adv) if d['weight'] is None else d['weight'].to(dtype).expand_as(adv)
     ratio = torch.exp(lp_new - lp_old)
     lo, hi = float(np.float32(1 - clip)), float(np.float32(1 + clip))
     sel = torch.min(ratio * adv, ratio.clamp(lo, hi) * adv)
@@ -93,19 +102,23 @@ def run64(d, clip=CLIP, dual_clip=None, kl_type='k1', entropy_bonus=True, mix=MI
         sel = torch.where(adv < 0, torch.max(sel, dual_clip * adv), sel)
     policy = (-sel * w).mean()
     total = mix[0] * policy
-    ent = torch.zeros((), dtype=torch.float64)
+    ent = torch.zeros((), dtype=dtype)
+    H = None
     if entropy_bonus:
-        H = -(torch.exp(lsm) * lsm.clamp(min=torch.finfo(torch.float64).min)).sum(-1)
+        p = torch.exp(lsm) if dtype == torch.float64 else torch.softmax(lsm, -1)
+        H = -(p * lsm.clamp(min=torch.finfo(dtype).min)).sum(-1)
         ent = (H * w).mean()
         total = total + mix[1] * ent
-    kl = torch.zeros((), dtype=torch.float64)
+    kl = torch.zeros((), dtype=dtype)
     if d['logit_pretrained'] is not None:
-        lr = lp_new - torch.log_softmax(d['logit_pretrained'].double(), -1).gather(-1, a).squeeze(-1)
+        lr = lp_new - _normalized(d['logit_pretrained'].to(dtype)).gather(-1, a).squeeze(-1)
         kl = {'k1': lr, 'k2': lr ** 2 / 2, 'k3': torch.exp(-lr) - 1 + lr}[kl_type].mean()
         total = total + mix[2] * kl
     total.backward()
     with torch.no_grad():
         approx_kl = (lp_old - lp_new).mean()
-        clipfrac = ((ratio > hi) | (ratio < lo)).double().mean()
+        clipfrac = ((ratio > hi) | (ratio < lo)).to(dtype).mean()
+        lse = torch.logsumexp(x, -1)
     return {'policy': policy.item(), 'entropy': ent.item(), 'kl': kl.item(), 'approx_kl': approx_kl.item(),
-            'clipfrac': clipfrac.item(), 'grad': x.grad}
+            'clipfrac': clipfrac.item(), 'grad': x.grad, 'lse': lse, 'lp_new': lp_new.detach(),
+            'H': None if H is None else H.detach()}
