@@ -71,6 +71,8 @@ PROTOTYPES = {
     "b200rl_token_head_fwd": [P, P, P, P, P, LL, P, LL, LL, D, D, P, P, P, c_size_t, P],
     "b200rl_ppo_lm_fwd_grad": [I, P, P, P, P, P, P, LL, LL, D, D, I, I, P, P, P, P, P, P, P, P, P, c_size_t, P],
     "b200rl_ppo_lm_bwd": [I, P, P, P, LL, LL, P, P, P, P, P, P, P, P, P, P, P],
+    "b200rl_a2c_lm_fwd_grad": [I, P, P, P, P, P, P, LL, LL, P, P, P, P, P, P, P, P, P, P, c_size_t, P],
+    "b200rl_a2c_lm_bwd": [I, P, P, P, LL, LL, P, P, P, P, P, P, P, P, P, P, P, P],
     "b200rl_gae_ppo_set_impl": [I],
     "b200rl_vtrace_set_impl": [I],
     "b200rl_acer_policy_fwd": [P, P, P, P, P, P, LL, LL, D, P, P, P],

@@ -46,6 +46,18 @@
 // write) -- unless they are the ones the forward used, in which case it returns at once on the device.  Loss sums:
 // policy, entropy, kl, approx_kl, clipfrac, all over M.  Traffic: (3 + 1) * V * sizeof(T) per row with logit_pretrained,
 // (2 + 1) without -- the same streams and the same L2 re-read of logit_new as GRPO / RLOO.
+//
+// A2C on token rows (a2c_error, ding/rl_utils/a2c.py:10-44, at (B, S, V) with a per-token value head): MODE = VM_A2C
+// streams logit_new alone (NR = 1) with the entropy accumulator always on, and keeps the row in shared memory for the
+// gradient's softmax as the other loss modes do.  The row epilogue follows the reference's order: lp = z[a] - lse,
+// H, dv = return_ - value, partials -lp * adv * w, dv^2 * w, H * w (w = 1 without weight), all three means over M rows.
+// For the expected upstream gradients (g_pol, g_val, g_ent: the call site's record) it writes
+// d / d logit_new = c * (onehot(a) - p) - c_ent * p * (log p + H), c = g_pol * (-adv * w / M), c_ent = g_ent * w / M,
+// and d / d value = g_val * (-2 * w * dv / M) in fp32.  Saved per row: lse, H, the unit coefficients -adv * w / M and
+// -2 * w * dv / M.  The backward is VM_PPO_BWD + PPO_ENT + PPO_VAL, the PPO backward pass with the value slot: it returns
+// at once when all three upstream gradients are the forward's, rewrites only d / d value (O(1) per row) when just g_val
+// differs, and otherwise recomputes both.  Traffic: (1 + 1) * V * sizeof(T) per row, plus O(1) per row -- logit_new read
+// once, its gradient written once, with the same L2 re-read of logit_new past VOCAB_SMEM_CAP.
 #include <cuda_bf16.h>
 #include <math.h>
 
@@ -60,6 +72,8 @@ constexpr int VOCAB_HEAD_NT = 256;
 constexpr int VOCAB_SMEM_CAP = 220 * 1024;  // dynamic shared memory for the cached part of logit_new (227 KB opt-in max)
 constexpr int VM_GRPO = 0, VM_RLOO = 1, VM_LOGP = 2, VM_BWD = 3;
 constexpr int VM_PPO = 4, VM_PPO_BWD = 8, PPO_ENT = 1, PPO_KL = 2;  // VM_PPO + flags: 4..7; VM_PPO_BWD + PPO_ENT: 8, 9
+// A2C: forward 12; backward VM_PPO_BWD + PPO_ENT + PPO_VAL = 11 (the PPO backward with the value slot)
+constexpr int PPO_VAL = 2, VM_A2C = 12;
 constexpr float kL2E = 1.4426950408889634f;
 
 // 16-byte vectors of T, widened to fp32
@@ -255,6 +269,11 @@ struct VocabArgs {
     UpstreamRecord rec;        // PPO forward and VM_PPO_BWD (slots policy, entropy, kl)
     float dual_clip, inv_m;    // dual_clip <= 0: off; inv_m = 1 / rows
     int kl_type;
+    // A2C (VM_A2C, VM_PPO_BWD + PPO_ENT + PPO_VAL); adv is per row, rec also owns the value slot
+    const float* value;        // forward: (rows)
+    const float* ret;          // forward: return_ (rows)
+    float* dval;               // forward: d value_loss / d value per row; backward: read
+    float* grad_value;         // d / d value (rows), fp32
 };
 
 template <int NR, bool CACHE, class T, bool ENT = false>
@@ -279,11 +298,12 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
     pdl_prologue();
     using V_ = VecT<T>;
     constexpr int W = V_::W;
-    constexpr bool PPO = MODE >= VM_PPO && MODE < VM_PPO_BWD, PBWD = MODE >= VM_PPO_BWD;
-    constexpr bool ENT = (PPO || PBWD) && (MODE & PPO_ENT), KL = PPO && (MODE & PPO_KL);
+    constexpr bool PPO = MODE >= VM_PPO && MODE < VM_PPO_BWD, PBWD = MODE >= VM_PPO_BWD && MODE < VM_A2C;
+    constexpr bool A2C = MODE == VM_A2C, VAL = A2C || (PBWD && (MODE & PPO_VAL));  // VAL: the A2C value slot
+    constexpr bool ENT = ((PPO || PBWD) && (MODE & PPO_ENT)) || A2C, KL = PPO && (MODE & PPO_KL);
     constexpr bool BWD = MODE == VM_BWD || PBWD;
     constexpr int NR = MODE == VM_GRPO ? 3 : (MODE == VM_RLOO ? 2 : (PPO ? (KL ? 3 : 2) : 1));
-    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO;
+    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO || A2C;
     constexpr int NP = PPO ? 5 : 3;
     extern __shared__ uint4 s_row[];
     __shared__ float s_m[NR][VOCAB_NT / 32], s_s[NR][VOCAB_NT / 32], s_w[VOCAB_NT / 32];
@@ -301,10 +321,19 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
     // PPO upstream-gradient slots: policy, entropy with the bonus, kl with logit_pretrained.  The record is written (forward)
     // or verified (VM_PPO_BWD) here; the values are read again where they are used, once per row, rather than held in
     // registers across the row loop.
-    const unsigned owned = 1u | (ENT ? 4u : 0u) | ((KL || (PBWD && a.coef_kl)) ? 8u : 0u);
-    if (PBWD || (PPO && want_grad)) {
+    const unsigned owned = 1u | (VAL ? 2u : 0u) | (ENT ? 4u : 0u) | ((KL || (PBWD && a.coef_kl)) ? 8u : 0u);
+    if (PBWD || ((PPO || A2C) && want_grad)) {
         float g[4];
         if (upstream<4>(a.rec, PBWD, owned, g)) return;  // VM_PPO_BWD: the forward wrote exactly this gradient
+        if (PBWD && VAL) {
+            // A2C: d / d value = g_val * dval, O(1) per row and always rewritten; d / d logit_new only when the policy
+            // or entropy upstream gradient differs from the forward's (the gradient the forward wrote stays exact)
+            for (long long r = (long long)blockIdx.x * VOCAB_NT + tid; r < a.rows; r += (long long)gridDim.x * VOCAB_NT)
+                a.grad_value[r] = g[1] * a.dval[r];
+            const float* u = a.rec.used;
+            if (u && __float_as_uint(g[0]) == __float_as_uint(u[0]) && __float_as_uint(g[2]) == __float_as_uint(u[2]))
+                return;
+        }
     }
     float part[NP] = {0.f, 0.f, 0.f};  // thread 0: the loss partial sums of this CTA's rows (loss, approx_kl, clipfrac; PPO: 5)
     float w_tot = (float)a.S;  // thread 0: sum_s w[b, s] of the current row's sequence (S without weights)
@@ -437,6 +466,25 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
                     part[4] += (ratio > a.hi || ratio < a.lo) ? 1.f : 0.f;
                     s_ce = ce;
                     s_h = H;
+                } else if constexpr (A2C) {  // a2c.py:39-44, in its operation order
+                    const float w = a.weight ? a.weight[row] : 1.f;
+                    const float adv = a.adv[row];
+                    const float dv = a.ret[row] - a.value[row];
+                    const float cp = -adv * w * a.inv_m;            // d policy_loss / d lp
+                    const float dvu = -2.f * w * dv * a.inv_m;      // d value_loss / d value
+                    a.coef[row] = cp;
+                    a.dval[row] = dvu;
+                    a.ent[row] = H;
+                    if (want_grad) {
+                        c = upstream_value(a.rec, owned, 0) * cp;
+                        ce = upstream_value(a.rec, owned, 2) * w * a.inv_m;
+                        a.grad_value[row] = upstream_value(a.rec, owned, 1) * dvu;
+                    }
+                    part[0] -= lp[0] * adv * w;
+                    part[1] += dv * dv * w;
+                    part[2] += H * w;
+                    s_ce = ce;
+                    s_h = H;
                 } else if (LOSS) {
                     const long long b = row / a.S;
                     if (new_seq) {
@@ -557,7 +605,7 @@ template <class T, int MODE>
 int launch_rows(VocabArgs& a, float* out3, size_t ws_bytes, long long B, cudaStream_t st) {
     constexpr auto kern = vocab_rows_kernel<T, MODE>;
     constexpr bool PPO = MODE >= VM_PPO && MODE < VM_PPO_BWD;
-    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO;
+    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO || MODE == VM_A2C;
     constexpr int NP = PPO ? 5 : 3;
     const long long nvec_max = (a.V * (long long)sizeof(T) + 15) / 16;
     a.capv = (LOSS && a.grad) ? (int)min(nvec_max, (long long)(VOCAB_SMEM_CAP / 16)) : 0;
@@ -570,8 +618,8 @@ int launch_rows(VocabArgs& a, float* out3, size_t ws_bytes, long long B, cudaStr
     if (int rc = launch_k(kern, (int)grid, VOCAB_NT, smem, st, a)) return rc;
     if (!LOSS) return B200RL_OK;
     FinalizeArgs fa{};
-    if (PPO) {  // policy, entropy, kl, approx_kl, clipfrac: means over the rows
-        for (int k = 0; k < 5; ++k) fa.scale[k] = 1.0 / (double)a.rows;
+    if (PPO || MODE == VM_A2C) {  // PPO: policy, entropy, kl, approx_kl, clipfrac; A2C: policy, value, entropy; row means
+        for (int k = 0; k < NP; ++k) fa.scale[k] = 1.0 / (double)a.rows;
     } else {
         fa.scale[0] = 1.0 / (double)B;
         fa.scale[1] = fa.scale[2] = 1.0 / (double)a.rows;
@@ -683,6 +731,47 @@ extern "C" int b200rl_ppo_lm_bwd(int dtype, const void* logit_new, const long lo
     cudaStream_t st = (cudaStream_t)stream;
     if (entropy_row) return launch_dtype<VM_PPO_BWD + PPO_ENT>(dtype, a, nullptr, 0, rows, st);
     return launch_dtype<VM_PPO_BWD>(dtype, a, nullptr, 0, rows, st);
+}
+
+extern "C" int b200rl_a2c_lm_fwd_grad(int dtype, const void* logit, const long long* action, const float* value,
+                                      const float* adv, const float* return_, const float* weight, long long rows,
+                                      long long V, const float* g_expected, float* g_used, float* out3, float* lse,
+                                      float* entropy_row, float* dlogp_policy, float* dvalue, void* grad_logit,
+                                      float* grad_value, float* workspace, size_t workspace_bytes, void* stream) {
+    if (!sizes_ok(rows, 1, V) || !aligned_logits(logit) || !action || !value || !adv || !return_ || !lse ||
+        !entropy_row || !dlogp_policy || !dvalue || !workspace || (grad_logit && !aligned16(grad_logit)) ||
+        (grad_value && !grad_logit) ||
+        !upstream_args_ok(0, out3, grad_logit != nullptr, grad_logit && grad_value, g_expected, g_used))
+        return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logit;
+    a.action = action; a.adv = adv; a.weight = weight; a.value = value; a.ret = return_;
+    a.lse = lse; a.ent = entropy_row; a.coef = dlogp_policy; a.dval = dvalue;
+    a.grad = grad_logit; a.grad_value = grad_value; a.ws = workspace;
+    a.rec = forward_record(g_expected, g_used);
+    a.rows = rows; a.S = 1; a.V = V;
+    a.inv_m = (float)(1.0 / (double)rows);
+    return launch_dtype<VM_A2C>(dtype, a, out3, workspace_bytes, rows, (cudaStream_t)stream);
+}
+
+extern "C" int b200rl_a2c_lm_bwd(int dtype, const void* logit, const long long* action, const float* weight,
+                                 long long rows, long long V, const float* lse, const float* entropy_row,
+                                 const float* dlogp_policy, const float* dvalue, const float* g_policy,
+                                 const float* g_value, const float* g_entropy, const float* g_used, float* g_hint,
+                                 void* grad_logit, float* grad_value, void* stream) {
+    if (!sizes_ok(rows, 1, V) || !aligned_logits(logit) || !action || !lse || !entropy_row || !dlogp_policy ||
+        !dvalue || !upstream_args_ok(1, nullptr, true, grad_logit && grad_value, nullptr, g_used) ||
+        !aligned16(grad_logit))
+        return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logit; a.action = action; a.weight = weight;
+    a.lse = const_cast<float*>(lse); a.ent = const_cast<float*>(entropy_row); a.coef_in = dlogp_policy;
+    a.dval = const_cast<float*>(dvalue);
+    a.rec = verify_record(g_policy, g_value, g_entropy, nullptr, g_used, g_hint);
+    a.grad = grad_logit; a.grad_value = grad_value;
+    a.rows = rows; a.S = 1; a.V = V;
+    a.inv_m = (float)(1.0 / (double)rows);
+    return launch_dtype<VM_PPO_BWD + PPO_ENT + PPO_VAL>(dtype, a, nullptr, 0, rows, (cudaStream_t)stream);
 }
 
 extern "C" int b200rl_token_logp_fwd(int dtype, const void* logits, const long long* index, long long rows, long long V,

@@ -1329,6 +1329,57 @@ class PPOLMFunction(torch.autograd.Function):
         return (grad, ) + (None, ) * 11
 
 
+class A2CLMFunction(torch.autograd.Function):
+    """a2c_error (ding/rl_utils/a2c.py:10-44) on token rows: logit (..., V) fp32 or bf16; value, action, adv, return_,
+    weight over the same rows, value fp32.  Outputs policy_loss, value_loss, entropy_loss (differentiable; the gradient
+    reaches logit and value).  The forward launch also writes d / d logit and d / d value for the upstream gradients the
+    ``'a2c'`` record expects; ``backward`` hands them to autograd after a launch that returns at once on the device when
+    the expectation held, rewrites only d / d value when just the value weight changed, and otherwise recomputes from the
+    saved per-row values -- A2CFunction's scheme, at vocabulary scale."""
+
+    @staticmethod
+    def forward(ctx, logit, value, action, adv, return_, weight, dt):
+        dev = logit.device
+        V = logit.shape[-1]
+        rows = logit.numel() // V
+        out = torch.empty(3, dtype=torch.float32, device=dev)
+        lse, ent, dpol, dval = torch.empty(4, rows, dtype=torch.float32, device=dev).unbind(0)
+        want = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        gl = torch.empty_like(logit) if want else None
+        gv = torch.empty_like(value) if want else None
+        g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
+        with on_device(dev):
+            ws = workspace(dev)
+            rc = lib().b200rl_a2c_lm_fwd_grad(
+                dt, ptr(logit), ptr(action), ptr(value), ptr(adv), ptr(return_), ptr(weight), rows, V,
+                ptr(ppo_hint(dev, 'a2c')) if want else None, ptr(g_used), ptr(out), ptr(lse), ptr(ent), ptr(dpol),
+                ptr(dval), ptr(gl), ptr(gv), ptr(ws), ws.numel() * 4, stream_ptr())
+        _lib.check(rc, 'b200rl_a2c_lm_fwd_grad')
+        ctx.save_for_backward(logit, value, action, weight, lse, ent, dpol, dval)
+        ctx.dt = dt
+        ctx.spec = (gl, gv, g_used) if want else None
+        ctx.set_materialize_grads(False)
+        return out[0], out[1], out[2]
+
+    @staticmethod
+    def backward(ctx, g_p, g_v, g_e):
+        logit, value, action, weight, lse, ent, dpol, dval = ctx.saved_tensors
+        dev = logit.device
+        keep, (pp, pv, pe) = _grads(g_p, g_v, g_e)
+        spec = _forward_grads(ctx)
+        if spec is not None:  # valid if the expectation held; the kernel checks on the device
+            gl, gv, g_used = spec
+            p_used, p_hint = ptr(g_used), ptr(ppo_hint(dev, 'a2c'))
+        else:  # a repeated backward: null g_used / hint -> the kernel recomputes
+            gl, gv, p_used, p_hint = torch.empty_like(logit), torch.empty_like(value), None, None
+        with on_device(dev):
+            rc = lib().b200rl_a2c_lm_bwd(ctx.dt, ptr(logit), ptr(action), ptr(weight), lse.numel(), logit.shape[-1],
+                                         ptr(lse), ptr(ent), ptr(dpol), ptr(dval), pp, pv, pe, p_used, p_hint, ptr(gl),
+                                         ptr(gv), stream_ptr())
+        _lib.check(rc, 'b200rl_a2c_lm_bwd')
+        return gl, gv, None, None, None, None, None
+
+
 def _vocab_outputs(ctx, logit_new):
     dev = logit_new.device
     rows = logit_new.shape[0] * logit_new.shape[1]

@@ -1,10 +1,12 @@
 """``a2c_error`` and ``a2c_error_continuous`` with the signatures and namedtuples of ding/rl_utils/a2c.py:6-88 -- csrc/heads.cu
-(SURVEY section 8f rank 3)."""
+(SURVEY section 8f rank 3); language-model calls of ``a2c_error`` (bf16 logits, or fp32 with V >= ``ppo.LM_MIN_VOCAB``) run
+on the vocabulary-scale row kernel of csrc/vocab.cu."""
 from collections import namedtuple
 
 import torch
 
 from .. import ops
+from . import ppo as _ppo
 
 a2c_data = namedtuple('a2c_data', ['logit', 'action', 'value', 'adv', 'return_', 'weight'])
 a2c_loss = namedtuple('a2c_loss', ['policy_loss', 'value_loss', 'entropy_loss'])
@@ -16,8 +18,13 @@ def a2c_error(data: namedtuple) -> namedtuple:
     ``value_loss = mean(w * (return_ - value)^2)``, ``entropy_loss = mean(H * w)``.  logit (B, N); action (B,) int64; value,
     adv, return_, weight (B,) (weight may be None).  Three differentiable 0-dim tensors; gradients reach ``logit`` and
     ``value``.  Forward and gradients in one launch, device-verified backward.
+
+    Language-model shapes -- logits (..., V), e.g. (B, S, V) against (B, S) action / value / adv / return_ / weight, in
+    bf16 or in fp32 with V >= ``ppo.LM_MIN_VOCAB`` -- run on the vocabulary-scale row kernel of csrc/vocab.cu.
     """
     logit, action, value, adv, return_, weight = data
+    if _ppo._lm_path(logit, adv):
+        return _a2c_lm(logit, action, value, adv, return_, weight)
     dev = ops.compute_device(logit, value)
     host_out = not logit.is_cuda
     N = logit.shape[-1]
@@ -32,6 +39,32 @@ def a2c_error(data: namedtuple) -> namedtuple:
     rt = ops.f32c(ops.to_device(return_.detach(), dev), 'return_')
     w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight') if weight is not None else None
     p, vl, e = ops.A2CFunction.apply(z, v, a, ad, rt, w, S, N)
+    if host_out:
+        p, vl, e = p.cpu(), vl.cpu(), e.cpu()
+    return a2c_loss(p, vl, e)
+
+
+def _a2c_lm(logit, action, value, adv, return_, weight):
+    """a2c_error on token rows (csrc/vocab.cu, ops.A2CLMFunction): the reference's plain means over all rows, under the
+    call site's existing ``'a2c'`` expected-upstream-gradient record"""
+    dt = ops.logit_dtype(logit)
+    V = logit.shape[-1]
+    rows = logit.numel() // V
+    for name, t_ in (('action', action), ('value', value), ('adv', adv), ('return_', return_), ('weight', weight)):
+        if t_ is not None and t_.numel() != rows:
+            raise ValueError("a2c_error: %s %s does not match logit %s" % (name, tuple(t_.shape), tuple(logit.shape)))
+    if value.dtype not in (torch.float32, torch.bfloat16):
+        raise TypeError("di_engine_b200: a2c_error on language-model logits takes a float32 or bfloat16 value (got %s)" %
+                        value.dtype)
+    dev = ops.compute_device(logit, value)
+    host_out = not logit.is_cuda
+    z = ops.logits_c(ops.to_device(logit, dev))
+    # a bf16 value is read as fp32; autograd's cast hands its gradient back in bf16
+    v = ops.to_device(value, dev).float().contiguous()
+    a = ops.i64c(ops.to_device(action, dev), V)
+    ad, rt = (ops.to_device(t_.detach(), dev).float().contiguous() for t_ in (adv, return_))
+    w = ops.to_device(weight.detach(), dev).float().contiguous() if weight is not None else None
+    p, vl, e = ops.A2CLMFunction.apply(z, v, a, ad, rt, w, dt)
     if host_out:
         p, vl, e = p.cpu(), vl.cpu(), e.cpu()
     return a2c_loss(p, vl, e)

@@ -527,7 +527,20 @@ B200RL_API int b200rl_gae_ppo_set_impl(int impl);
  * b200rl_ppo_lm_bwd: the same gradient for the actual upstream gradients g_policy, g_entropy, g_kl (device scalars,
  *   nullable = 0) from the saved rows (entropy_row / dlogp_kl null = no entropy / KL term): one read of logit_new, one
  *   write.  The verify launch of b200rl_ppo_lm_fwd_grad (g_used, g_hint nullable; owned slots: policy, entropy with
- *   entropy_row, kl with dlogp_kl). */
+ *   entropy_row, kl with dlogp_kl).
+ * b200rl_a2c_lm_fwd_grad: a2c_error (ding/rl_utils/a2c.py:10-44) on token rows: logit (rows, V); action, value, adv,
+ *   return_, weight (rows) fp32.  M = rows.  out3 = {policy_loss, value_loss, entropy_loss}: policy_loss =
+ *   mean(-lp * adv * w), lp = z[a] - logsumexp(z); value_loss = mean((return_ - value)^2 * w); entropy_loss = mean(H * w)
+ *   with H the entropy of softmax(logit[row]).  Saved for the backward (all (rows) fp32): lse, entropy_row = H,
+ *   dlogp_policy = -adv * w / M and dvalue = -2 * w * (return_ - value) / M.  grad_logit (nullable = no gradient; dtype
+ *   of the logits) = c * (onehot(a) - p) - c_ent * p * (log p + H), p = softmax(logit[row]), log p clamped at -FLT_MAX,
+ *   c = g_pol * dlogp_policy, c_ent = g_ent * w / M; grad_value (rows) fp32 = g_val * dvalue, given with grad_logit; both
+ *   for the expected upstream gradients g_expected (forward-written gradients; owned slots: policy, value, entropy;
+ *   g_expected and g_used hold 4 floats).
+ * b200rl_a2c_lm_bwd: the same gradients for the actual upstream gradients g_policy, g_value, g_entropy (device scalars,
+ *   nullable = 0) from the saved rows.  The verify launch of b200rl_a2c_lm_fwd_grad (g_used, g_hint nullable; owned slots:
+ *   policy, value, entropy): it returns at once when all three match g_used; grad_value is rewritten whenever they do not,
+ *   and grad_logit (one read of logit, one write) only when the policy or entropy slot differs. */
 #define B200RL_DTYPE_F32 0
 #define B200RL_DTYPE_BF16 1
 B200RL_API int b200rl_grpo_fwd_grad(int dtype, const void* logit_new, const void* logit_old, const void* logit_ref,
@@ -557,6 +570,15 @@ B200RL_API int b200rl_ppo_lm_bwd(int dtype, const void* logit_new, const long lo
                       long long rows, long long V, const float* lse_new, const float* entropy_row,
                       const float* dlogp_policy, const float* dlogp_kl, const float* g_policy, const float* g_entropy,
                       const float* g_kl, const float* g_used, float* g_hint, void* grad_logit_new, void* stream);
+B200RL_API int b200rl_a2c_lm_fwd_grad(int dtype, const void* logit, const long long* action, const float* value,
+                           const float* adv, const float* return_, const float* weight, long long rows, long long V,
+                           const float* g_expected, float* g_used, float* out3, float* lse, float* entropy_row,
+                           float* dlogp_policy, float* dvalue, void* grad_logit, float* grad_value, float* workspace,
+                           size_t workspace_bytes, void* stream);
+B200RL_API int b200rl_a2c_lm_bwd(int dtype, const void* logit, const long long* action, const float* weight,
+                      long long rows, long long V, const float* lse, const float* entropy_row, const float* dlogp_policy,
+                      const float* dvalue, const float* g_policy, const float* g_value, const float* g_entropy,
+                      const float* g_used, float* g_hint, void* grad_logit, float* grad_value, void* stream);
 
 /* ---- data-parallel exchange step: one-shot all-reduce (mean) of n <= 8 floats over NVLink peer memory -----------
  * Replaces the small-message NCCL all-reduce of the packed loss scalars (mean of rank means,
