@@ -25,6 +25,9 @@ PROTOTYPES = {
     "b200rl_gae_returns": [P, P, P, P, P, LL, LL, LL, D, D, I, D, P, P, P, P, P, P, P, c_size_t, P],
     "b200rl_adv_stats": [P, LL, P, P, c_size_t, P],
     "b200rl_normalize": [P, P, LL, P, P],
+    "b200rl_gae_returns_norm": [P, P, P, P, P, LL, LL, D, D, I, D, P, P, P, P, P, P, P, P, P, c_size_t, P],
+    "b200rl_value_map_fwd": [I, P, LL, P, P],
+    "b200rl_value_map_bwd": [I, P, P, LL, P, P],
     "b200rl_impala_mask": [P, P, P, LL, LL, P, P, P, P],
     "b200rl_ppo_fwd": [P, P, P, P, P, P, P, P, P, LL, LL, LL, D, I, D, I, P, P, P, P, c_size_t, P],
     "b200rl_ppo_bwd": [P, P, P, P, P, P, P, P, P, LL, LL, LL, D, I, D, I, P, P, P, P, P, P, P, P, P, P, P],

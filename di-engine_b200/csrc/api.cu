@@ -2,7 +2,7 @@
 #include "../../include/b200rl.h"
 #include "common.cuh"
 
-extern "C" int b200rl_version(void) { return 108; }
+extern "C" int b200rl_version(void) { return 109; }
 extern "C" int b200rl_built_for_sm(void) { return 90; }
 extern "C" size_t b200rl_workspace_bytes(void) { return (size_t)WS_MIN_BYTES; }
 

@@ -17,6 +17,9 @@
 //   returns_kernel        the same epilogue for (T, B) batches behind gae_ws_kernel: one elementwise pass + statistics.
 //   adv_stats_kernel      {mean, std(unbiased) + 1e-8} of a batch in one launch; the PPO kernels apply the normalisation on load
 //                         (ppo_math.cuh adv_in), normalize_kernel materialises it for callers that want the tensor.
+// gae_seq_kernel and returns_kernel are templated on the value normalisation (policy_stats.cuh): VN_PPO is the above, the
+// other four are PPOFPolicy's value_norm modes (ding/policy/ppof.py:160-210, b200rl_gae_returns_norm).  value_map_kernel is
+// symlog / inv_symlog and the decode pass of PPOF's (T, B) path; value_map_bwd_kernel the autograd of the first two.
 #include <math.h>
 
 #include "../../include/b200rl.h"
@@ -30,6 +33,8 @@ namespace b200rl {
 constexpr int GS_NT = 1024;
 constexpr int GS_MAX_T = 24576;  // 2 arrays x 4 B x T of dynamic shared memory (192 KB)
 
+// VN: the value normalisation around gae (policy_stats.cuh), decoded in phase 1 and encoded in phase 4
+template <int VN>
 __global__ void __launch_bounds__(GS_NT) gae_seq_kernel(const float* __restrict__ value, float* __restrict__ next_value,
                                                        const float* __restrict__ reward, const float* __restrict__ done,
                                                        const float* __restrict__ traj, float* __restrict__ adv, int T,
@@ -42,20 +47,25 @@ __global__ void __launch_bounds__(GS_NT) gae_seq_kernel(const float* __restrict_
     __shared__ int s_cnt[GS_NT / 32];
     const int tid = threadIdx.x;
     const float vs = ra.vscale;
-    // ---- phase 1: delta_t, f_t in the reference's operation order (gae.py:61-63), value_norm scaling first (ppo.py:276-278)
+    float mu = 0.f, sigma = 1.f;
+    if constexpr (VN == VN_POPART) {
+        mu = *ra.mu;
+        sigma = *ra.sigma;
+    }
+    // ---- phase 1: delta_t, f_t in the reference's operation order (gae.py:61-63), value_norm decoding first (ppo.py:276-278,
+    // ppof.py:171-189)
     for (int t = tid; t < T; t += GS_NT) {
-        float v = value[t], nv = next_value[t];
-        if (vs != 0.f) {
-            v = fmul(v, vs);
-            nv = fmul(nv, vs);
-        }
+        const float v = vn_decode<VN>(value[t], vs);
+        float nv = vn_decode<VN>(next_value[t], vs);
+        float r = reward[t];
+        if constexpr (VN == VN_POPART) r = __fdiv_rn(fsub(r, mu), sigma);
         const float d = done ? done[t] : 0.f;
         const float tf = traj ? traj[t] : d;
         if (done) {
             nv = fmul(nv, fsub(1.f, d));
-            if (mask_inplace && d != 0.f) next_value[t] = nv;
+            if (VN == VN_PPO && mask_inplace && d != 0.f) next_value[t] = nv;
         }
-        s_d[t] = fsub(fadd(reward[t], fmul(gamma, nv)), v);
+        s_d[t] = fsub(fadd(r, fmul(gamma, nv)), v);
         s_f[t] = fmul(gl, fsub(1.f, tf));
     }
     __syncthreads();
@@ -134,6 +144,22 @@ __global__ void __launch_bounds__(GS_NT) gae_seq_kernel(const float* __restrict_
         }
     }
     __syncthreads();
+    if constexpr (VN != VN_PPO) {
+        // The loop carries 0 * adv[t + 1] across a segment end t, so a non-finite adv[t + 1] there makes adv[0 .. t] NaN; the
+        // lanes above restarted from 0.  Take the last such end and poison everything up to it, as the loop does.  (The PPO
+        // build keeps the lane result there, the deviation DESIGN.md documents for gae.)
+        __shared__ int s_cut;
+        if (tid == 0) s_cut = -1;
+        __syncthreads();
+        int cut = -1;
+        for (int t = tid; t < T - 1; t += GS_NT)
+            if (s_f[t] == 0.f && !isfinite(s_d[t + 1])) cut = t;
+        if (cut >= 0) atomicMax(&s_cut, cut);
+        __syncthreads();
+        const int c = s_cut;
+        for (int t = tid; t <= c; t += GS_NT) s_d[t] = __int_as_float(0x7fc00000);
+        __syncthreads();
+    }
     // ---- phase 4: write-out (+ returns, value-norm, statistics)
     double acc[4] = {0.0, 0.0, 0.0, 0.0};
     for (int t = tid; t < T; t += GS_NT) {
@@ -142,14 +168,11 @@ __global__ void __launch_bounds__(GS_NT) gae_seq_kernel(const float* __restrict_
         acc[2] += (double)a;
         acc[3] += (double)a * (double)a;
         if (ra.ret_unnorm || ra.value_out || ra.ret_out || ra.stats) {
-            float v = value[t];
-            if (vs != 0.f) v = fmul(v, vs);
-            const float r = fadd(v, a);  // unnormalized_returns = value + adv (ppo.py:284)
-            if (ra.ret_unnorm) ra.ret_unnorm[t] = r;
-            if (ra.value_out) ra.value_out[t] = vs != 0.f ? __fdiv_rn(v, vs) : v;
-            if (ra.ret_out) ra.ret_out[t] = vs != 0.f ? __fdiv_rn(r, vs) : r;
-            acc[0] += (double)r;
-            acc[1] += (double)r * (double)r;
+            float ru, vo, ro;
+            ret_encode<VN>(vs, vn_decode<VN>(value[t], vs), a, ru, vo, ro, acc);
+            if (ra.ret_unnorm) ra.ret_unnorm[t] = ru;
+            if (ra.value_out) ra.value_out[t] = vo;
+            if (ra.ret_out) ra.ret_out[t] = ro;
         }
     }
     if (ra.stats || ra.adv_stats) {
@@ -159,7 +182,7 @@ __global__ void __launch_bounds__(GS_NT) gae_seq_kernel(const float* __restrict_
             const double n = (double)T, m = tot[0] / n;
             if (ra.stats) {
                 ra.stats[0] = (float)m;
-                ra.stats[1] = (float)fmax(tot[1] / n - m * m, 0.0);  // np.var: population variance
+                ra.stats[1] = (float)pop_var<VN>(tot[1] / n - m * m);
                 ra.stats[2] = (float)n;
             }
             if (ra.adv_stats) write_adv_stats(ra.adv_stats, tot[2], tot[3], n);
@@ -168,11 +191,12 @@ __global__ void __launch_bounds__(GS_NT) gae_seq_kernel(const float* __restrict_
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// (T, B) epilogue behind gae_ws_kernel: returns / value-norm / statistics in one elementwise pass.
+// (T, B) epilogue behind gae_ws_kernel: returns / value-norm / statistics in one elementwise pass.  The scaling modes read the
+// raw value; the others read the value the decode pass (value_map_kernel) wrote.
 // The four sums (r, r^2, adv, adv^2) are reduced per CTA in fp64 and joined across CTAs with fp64 atomics; the CTA that
 // arrives last writes the statistics (ret_stats_join).
 // ---------------------------------------------------------------------------------------------------------------
-template <bool VEC>
+template <int VN, bool VEC>
 __global__ void __launch_bounds__(256) returns_kernel(const float* __restrict__ value, const float* __restrict__ adv,
                                                       long long n, RetArgs ra, double* __restrict__ ws_d,
                                                       unsigned int* __restrict__ ws_join) {
@@ -184,10 +208,10 @@ __global__ void __launch_bounds__(256) returns_kernel(const float* __restrict__ 
         for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
             const float4 v = reinterpret_cast<const float4*>(value)[i], a = reinterpret_cast<const float4*>(adv)[i];
             float4 ru, vo, ro;
-            ret_one(vs, v.x, a.x, ru.x, vo.x, ro.x, acc);
-            ret_one(vs, v.y, a.y, ru.y, vo.y, ro.y, acc);
-            ret_one(vs, v.z, a.z, ru.z, vo.z, ro.z, acc);
-            ret_one(vs, v.w, a.w, ru.w, vo.w, ro.w, acc);
+            ret_one<VN>(vs, v.x, a.x, ru.x, vo.x, ro.x, acc);
+            ret_one<VN>(vs, v.y, a.y, ru.y, vo.y, ro.y, acc);
+            ret_one<VN>(vs, v.z, a.z, ru.z, vo.z, ro.z, acc);
+            ret_one<VN>(vs, v.w, a.w, ru.w, vo.w, ro.w, acc);
             if (ra.ret_unnorm) reinterpret_cast<float4*>(ra.ret_unnorm)[i] = ru;
             if (ra.value_out) reinterpret_cast<float4*>(ra.value_out)[i] = vo;
             if (ra.ret_out) reinterpret_cast<float4*>(ra.ret_out)[i] = ro;
@@ -195,14 +219,14 @@ __global__ void __launch_bounds__(256) returns_kernel(const float* __restrict__ 
     } else {
         for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
             float ru, vo, ro;
-            ret_one(vs, value[i], adv[i], ru, vo, ro, acc);
+            ret_one<VN>(vs, value[i], adv[i], ru, vo, ro, acc);
             if (ra.ret_unnorm) ra.ret_unnorm[i] = ru;
             if (ra.value_out) ra.value_out[i] = vo;
             if (ra.ret_out) ra.ret_out[i] = ro;
         }
     }
     if (!ra.stats && !ra.adv_stats) return;
-    ret_stats_join<256>(acc, ra, (double)n, ws_d, ws_join);
+    ret_stats_join<256, VN>(acc, ra, (double)n, ws_d, ws_join);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -266,6 +290,52 @@ __global__ void __launch_bounds__(256) impala_mask_kernel(const float* __restric
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Element-wise value maps: symlog / inv_symlog forward and backward (value_rescale.py:37-66), and the decode pass of a
+// PPOF advantage recompute that does not fit gae_seq_kernel -- h^-1 or inv_symlog of value and next_value (two arrays in one
+// launch), or PopArt's (reward - mu) / sigma (ppof.py:177).
+// ---------------------------------------------------------------------------------------------------------------
+enum ValueMap : int { VM_SYMLOG = 0, VM_INV_SYMLOG = 1, VM_H_INV = 2, VM_POPART_REWARD = 3 };
+
+template <int M>
+__device__ __forceinline__ float value_map(float x, float mu, float sigma) {
+    if constexpr (M == VM_SYMLOG) return vn_symlog(x);
+    else if constexpr (M == VM_INV_SYMLOG) return vn_inv_symlog(x);
+    else if constexpr (M == VM_H_INV) return vn_h_inv(x);
+    else return __fdiv_rn(fsub(x, mu), sigma);
+}
+
+// y0 = map(x0) and, when x1 is given, y1 = map(x1); mu / sigma: device floats, read only by VM_POPART_REWARD
+template <int M>
+__global__ void __launch_bounds__(256) value_map_kernel(const float* __restrict__ x0, float* __restrict__ y0,
+                                                        const float* __restrict__ x1, float* __restrict__ y1, long long n,
+                                                        const float* __restrict__ mu, const float* __restrict__ sigma) {
+    pdl_prologue();
+    float m = 0.f, sg = 1.f;
+    if constexpr (M == VM_POPART_REWARD) {
+        m = *mu;
+        sg = *sigma;
+    }
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        y0[i] = value_map<M>(x0[i], m, sg);
+        if (x1) y1[i] = value_map<M>(x1[i], m, sg);
+    }
+}
+
+// torch autograd of the reference expressions, op by op (sign contributes a zero gradient, accumulated last):
+//   symlog      sign(x) * log(|x| + 1):  dx = 0 + ((g * sign(x)) / (|x| + 1)) * sign(x)
+//   inv_symlog  sign(x) * (exp(|x|) - 1): dx = 0 + ((g * sign(x)) * exp(|x|)) * sign(x)
+template <int M>
+__global__ void __launch_bounds__(256) value_map_bwd_kernel(const float* __restrict__ x, const float* __restrict__ g,
+                                                            float* __restrict__ dx, long long n) {
+    pdl_prologue();
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        const float xi = x[i], s = vn_sign(xi), gs = fmul(g[i], s);
+        const float d = M == VM_SYMLOG ? __fdiv_rn(gs, fadd(fabsf(xi), 1.f)) : fmul(gs, expf(fabsf(xi)));
+        dx[i] = fadd(0.f, fmul(d, s));
+    }
+}
+
 }  // namespace b200rl
 
 using namespace b200rl;
@@ -313,8 +383,8 @@ extern "C" int b200rl_gae_returns(const float* value, float* next_value, const f
     cudaStream_t st = (cudaStream_t)stream;
     if (C == 1 && T <= GS_MAX_T) {  // the real PPO learner's call: one sequence, everything in one launch
         const size_t smem = (size_t)2 * T * sizeof(float);
-        if (int rc = smem_opt_in<gae_seq_kernel>(smem)) return rc;
-        return launch_k(gae_seq_kernel, 1, GS_NT, smem, st, value, next_value, reward, done, traj_flag, adv, (int)T,
+        if (int rc = smem_opt_in<gae_seq_kernel<VN_PPO>>(smem)) return rc;
+        return launch_k(gae_seq_kernel<VN_PPO>, 1, GS_NT, smem, st, value, next_value, reward, done, traj_flag, adv, (int)T,
                         (float)gamma, (float)(gamma * lambda_), mask_next_value_inplace, ra);
     }
     // (T, B): the streaming scan (value_norm scaling applied on load), then one elementwise epilogue launch (returns_kernel).
@@ -328,10 +398,137 @@ extern "C" int b200rl_gae_returns(const float* value, float* next_value, const f
     long long grid = div_up(n, 256 * (vec ? 8 : 4));
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
     if (vec)
-        return launch_k(returns_kernel<true>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra, ws_doubles(workspace),
+        return launch_k(returns_kernel<VN_PPO, true>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra,
+                        ws_doubles(workspace), ws_joins(workspace));
+    return launch_k(returns_kernel<VN_PPO, false>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra,
+                    ws_doubles(workspace), ws_joins(workspace));
+}
+
+// ---- PPOFPolicy's advantage recompute (ding/policy/ppof.py:160-210) -----------------------------------------------------------
+static long long map_grid(long long n) {
+    long long grid = div_up(n, 256 * 4);
+    if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
+    return grid < 1 ? 1 : grid;
+}
+
+template <int VN>
+static int launch_gae_seq(const float* value, const float* next_value, const float* reward, const float* done,
+                          const float* traj_flag, float* adv, long long T, double gamma, double lambda_, const RetArgs& ra,
+                          cudaStream_t st) {
+    const size_t smem = (size_t)2 * T * sizeof(float);
+    if (int rc = smem_opt_in<gae_seq_kernel<VN>>(smem)) return rc;
+    return launch_k(gae_seq_kernel<VN>, 1, GS_NT, smem, st, value, const_cast<float*>(next_value), reward, done, traj_flag,
+                    adv, (int)T, (float)gamma, (float)(gamma * lambda_), 0, ra);
+}
+
+template <int VN>
+static int launch_returns(const float* value, const float* adv, long long n, const RetArgs& ra, float* workspace,
+                          cudaStream_t st) {
+    const bool vec = (n % 4 == 0) && aligned16(value) && aligned16(adv) && (!ra.value_out || aligned16(ra.value_out)) &&
+                     (!ra.ret_out || aligned16(ra.ret_out));
+    long long grid = div_up(n, 256 * (vec ? 8 : 4));
+    if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
+    if (vec)
+        return launch_k(returns_kernel<VN, true>, (int)grid, 256, 0, st, value, adv, n, ra, ws_doubles(workspace),
                         ws_joins(workspace));
-    return launch_k(returns_kernel<false>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra, ws_doubles(workspace),
+    return launch_k(returns_kernel<VN, false>, (int)grid, 256, 0, st, value, adv, n, ra, ws_doubles(workspace),
                     ws_joins(workspace));
+}
+
+// (T, C) or a sequence longer than GS_MAX_T: decode pass (not for baseline: gae_scan scales on load), gae_scan, the mode's
+// returns_kernel
+template <int VN>
+static int launch_gae_returns_tc(const float* value, const float* next_value, const float* reward, const float* done,
+                                 const float* traj_flag, float* adv, long long T, long long C, double gamma, double lambda_,
+                                 const RetArgs& ra, float* scratch, float* workspace, cudaStream_t st) {
+    const long long n = T * C;
+    const float* v = value;
+    const float* nv = next_value;
+    const float* r = reward;
+    int rc = 0;
+    if constexpr (VN == VN_RESCALE || VN == VN_SYMLOG) {
+        constexpr int M = VN == VN_RESCALE ? VM_H_INV : VM_INV_SYMLOG;
+        rc = launch_k(value_map_kernel<M>, (int)map_grid(n), 256, 0, st, value, scratch, next_value, scratch + n, n,
+                      (const float*)nullptr, (const float*)nullptr);
+        v = scratch;
+        nv = scratch + n;
+    } else if constexpr (VN == VN_POPART) {
+        rc = launch_k(value_map_kernel<VM_POPART_REWARD>, (int)map_grid(n), 256, 0, st, reward, scratch,
+                      (const float*)nullptr, (float*)nullptr, n, ra.mu, ra.sigma);
+        r = scratch;
+    }
+    if (rc) return rc;
+    // mask_next_value_inplace = 0: next_value is only read
+    rc = gae_scan(v, const_cast<float*>(nv), r, done, traj_flag, adv, T, C, 1, gamma, lambda_, 0,
+                  VN == VN_BASELINE ? ra.vscale : 0.f, st);
+    if (rc || !(ra.value_out || ra.ret_out || ra.stats || ra.adv_stats)) return rc;
+    return launch_returns<VN>(v, adv, n, ra, workspace, st);
+}
+
+template <int VN>
+static int gae_returns_norm(const float* value, const float* next_value, const float* reward, const float* done,
+                            const float* traj_flag, float* adv, long long T, long long C, double gamma, double lambda_,
+                            const RetArgs& ra, float* scratch, float* workspace, cudaStream_t st) {
+    if (C == 1 && T <= GS_MAX_T)  // every PPOF call: one sequence of n_sample steps, one launch
+        return launch_gae_seq<VN>(value, next_value, reward, done, traj_flag, adv, T, gamma, lambda_, ra, st);
+    return launch_gae_returns_tc<VN>(value, next_value, reward, done, traj_flag, adv, T, C, gamma, lambda_, ra, scratch,
+                                     workspace, st);
+}
+
+extern "C" int b200rl_gae_returns_norm(const float* value, const float* next_value, const float* reward, const float* done,
+                                       const float* traj_flag, long long T, long long C, double gamma, double lambda_,
+                                       int value_norm, double std, const float* popart_mu, const float* popart_sigma,
+                                       float* adv, float* value_out, float* return_out, float* stats3, float* adv_stats2,
+                                       float* scratch, float* workspace, size_t workspace_bytes, void* stream) {
+    if (T < 1 || C < 1 || !value || !next_value || !reward || !adv || !workspace || workspace_bytes < WS_MIN_BYTES)
+        return B200RL_ERR_ARG;
+    if (value_norm < VN_BASELINE || value_norm > VN_POPART) return B200RL_ERR_ARG;
+    if (value_norm == VN_BASELINE && !(std > 0.0)) return B200RL_ERR_ARG;
+    if (value_norm == VN_POPART && (!popart_mu || !popart_sigma)) return B200RL_ERR_ARG;
+    const bool one_launch = C == 1 && T <= GS_MAX_T;
+    if (!one_launch && value_norm != VN_BASELINE && !scratch) return B200RL_ERR_ARG;
+    RetArgs ra{};
+    ra.vscale = value_norm == VN_BASELINE ? (float)std : 0.f;
+    ra.value_out = value_out; ra.ret_out = return_out; ra.stats = stats3; ra.adv_stats = adv_stats2;
+    ra.mu = popart_mu; ra.sigma = popart_sigma;
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (value_norm) {
+        case VN_BASELINE:
+            return gae_returns_norm<VN_BASELINE>(value, next_value, reward, done, traj_flag, adv, T, C, gamma, lambda_, ra,
+                                                 scratch, workspace, st);
+        case VN_RESCALE:
+            return gae_returns_norm<VN_RESCALE>(value, next_value, reward, done, traj_flag, adv, T, C, gamma, lambda_, ra,
+                                                scratch, workspace, st);
+        case VN_SYMLOG:
+            return gae_returns_norm<VN_SYMLOG>(value, next_value, reward, done, traj_flag, adv, T, C, gamma, lambda_, ra,
+                                               scratch, workspace, st);
+        default:
+            return gae_returns_norm<VN_POPART>(value, next_value, reward, done, traj_flag, adv, T, C, gamma, lambda_, ra,
+                                               scratch, workspace, st);
+    }
+}
+
+extern "C" int b200rl_value_map_fwd(int mode, const float* x, long long n, float* y, void* stream) {
+    if (n < 0 || (mode != VM_SYMLOG && mode != VM_INV_SYMLOG)) return B200RL_ERR_ARG;
+    if (n == 0) return B200RL_OK;
+    if (!x || !y) return B200RL_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int grid = (int)map_grid(n);
+    if (mode == VM_SYMLOG)
+        return launch_k(value_map_kernel<VM_SYMLOG>, grid, 256, 0, st, x, y, (const float*)nullptr, (float*)nullptr, n,
+                        (const float*)nullptr, (const float*)nullptr);
+    return launch_k(value_map_kernel<VM_INV_SYMLOG>, grid, 256, 0, st, x, y, (const float*)nullptr, (float*)nullptr, n,
+                    (const float*)nullptr, (const float*)nullptr);
+}
+
+extern "C" int b200rl_value_map_bwd(int mode, const float* x, const float* g, long long n, float* dx, void* stream) {
+    if (n < 0 || (mode != VM_SYMLOG && mode != VM_INV_SYMLOG)) return B200RL_ERR_ARG;
+    if (n == 0) return B200RL_OK;
+    if (!x || !g || !dx) return B200RL_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int grid = (int)map_grid(n);
+    if (mode == VM_SYMLOG) return launch_k(value_map_bwd_kernel<VM_SYMLOG>, grid, 256, 0, st, x, g, dx, n);
+    return launch_k(value_map_bwd_kernel<VM_INV_SYMLOG>, grid, 256, 0, st, x, g, dx, n);
 }
 
 /* rewards / rewards_out / weights_out nullable (the backward pass masks a gradient with values = g, the other outputs off) */

@@ -43,7 +43,71 @@ struct RetArgs {
     float* ret_out;     // nullable: unnormalized / s
     float* stats;       // nullable: {mean, population variance, count} of the unnormalized returns (RunningMeanStd.update input)
     float* adv_stats;   // nullable: {mean, std(unbiased) + 1e-8} of adv (ppo.py:304-306 when the whole batch is one minibatch)
+    const float* mu;     // VN_POPART: the PopArt head's mu / sigma, one device float each
+    const float* sigma;
 };
+
+// ---------------------------------------------------------------------------------------------------------------
+// Value normalisation around gae.  VN_PPO is PPOPolicy's (value scaled by ra.vscale when it is not 0, statistics of the
+// unnormalised return).  The other four are PPOFPolicy's value_norm modes (ding/policy/ppof.py:171-208), in the order of
+// the C ABI's value_norm argument:
+//   VN_BASELINE  value * std on load, / std on store; statistics of the STORED return (ppof.py:206-208 divides in place)
+//   VN_RESCALE   h^-1 on load, h on store (value_rescale.py:4-34, eps = 1e-2)
+//   VN_SYMLOG    inv_symlog on load, symlog on store (value_rescale.py:37-66)
+//   VN_POPART    reward -> (reward - mu) / sigma on load, value as it is (ppof.py:171-179)
+// Every expression is the reference's torch expression, one rounded fp32 operation per torch op, in its order.
+// ---------------------------------------------------------------------------------------------------------------
+enum ValueNorm : int { VN_BASELINE = 0, VN_RESCALE = 1, VN_SYMLOG = 2, VN_POPART = 3, VN_PPO = 4 };
+
+// torch.sign: (0 < x) - (x < 0), so sign(NaN) = sign(-0) = 0
+__device__ __forceinline__ float vn_sign(float x) { return (float)((0.f < x) - (x < 0.f)); }
+
+// value_transform: sign(x) * (sqrt(|x| + 1) - 1) + eps * x
+__device__ __forceinline__ float vn_h(float x) {
+    return fadd(fmul(vn_sign(x), fsub(__fsqrt_rn(fadd(fabsf(x), 1.f)), 1.f)), fmul(0.01f, x));
+}
+// value_inv_transform: sign(x) * (((sqrt(1 + 4 eps ((|x| + 1) + eps)) - 1) / (2 eps)) ** 2 - 1); 4 eps and 2 eps are python
+// doubles rounded to fp32 scalars, and the division by a python scalar is a true division
+__device__ __forceinline__ float vn_h_inv(float x) {
+    const float u = __fdiv_rn(fsub(__fsqrt_rn(fadd(1.f, fmul(0.04f, fadd(fadd(fabsf(x), 1.f), 0.01f)))), 1.f), 0.02f);
+    return fmul(vn_sign(x), fsub(fmul(u, u), 1.f));
+}
+// symlog: sign(x) * log(|x| + 1)  (logf of |x| + 1, as torch.log computes it, not log1pf)
+__device__ __forceinline__ float vn_symlog(float x) { return fmul(vn_sign(x), logf(fadd(fabsf(x), 1.f))); }
+// inv_symlog: sign(x) * (exp(|x|) - 1)
+__device__ __forceinline__ float vn_inv_symlog(float x) { return fmul(vn_sign(x), fsub(expf(fabsf(x)), 1.f)); }
+
+// the critic's output as gae sees it, for a kernel that reads the raw value (VN_POPART decodes the reward instead)
+template <int VN>
+__device__ __forceinline__ float vn_decode(float v, float vs) {
+    if constexpr (VN == VN_PPO || VN == VN_BASELINE) return vs != 0.f ? fmul(v, vs) : v;
+    else if constexpr (VN == VN_RESCALE) return vn_h_inv(v);
+    else if constexpr (VN == VN_SYMLOG) return vn_inv_symlog(v);
+    else return v;
+}
+
+// the stored form of a decoded value or return
+template <int VN>
+__device__ __forceinline__ float vn_encode(float v, float vs) {
+    if constexpr (VN == VN_PPO || VN == VN_BASELINE) return vs != 0.f ? __fdiv_rn(v, vs) : v;
+    else if constexpr (VN == VN_RESCALE) return vn_h(v);
+    else if constexpr (VN == VN_SYMLOG) return vn_symlog(v);
+    else return v;
+}
+
+// the element-wise part of the epilogue for a DECODED value v and its advantage a: unnormalized return
+// (unnormalized_returns = value + adv, ppo.py:284 / ppof.py:195), stored value / return, and the sums of the return the
+// statistics describe (PPOPolicy: the unnormalised one; PPOF: the stored one)
+template <int VN>
+__device__ __forceinline__ void ret_encode(float vs, float v, float a, float& ru, float& vo, float& ro, double (&acc)[4]) {
+    const float r = fadd(v, a);
+    ru = r;
+    vo = vn_encode<VN>(v, vs);
+    ro = vn_encode<VN>(r, vs);
+    const float s = VN == VN_PPO ? r : ro;
+    acc[0] += (double)s;
+    acc[1] += (double)s * (double)s;
+}
 
 // {mean, torch.std (unbiased) + 1e-8} from the fp64 sums of x and x^2
 __device__ __forceinline__ void write_adv_stats(float* out, double s1, double s2, double nn) {
@@ -55,22 +119,26 @@ __device__ __forceinline__ void write_adv_stats(float* out, double s1, double s2
 }
 
 
-// the element-wise part of the epilogue for one (value, adv) pair: unnormalized return, stored value / return, the four sums
+// the element-wise part of the (T, B) epilogue for one (value, adv) pair: the value as returns_kernel reads it (raw for the
+// scaling modes, already decoded by the decode pass for the others), then ret_encode, then the advantage sums
+template <int VN>
 __device__ __forceinline__ void ret_one(float vs, float v, float a, float& ru, float& vo, float& ro, double (&acc)[4]) {
-    if (vs != 0.f) v = fmul(v, vs);
-    const float r = fadd(v, a);  // unnormalized_returns = value + adv (ppo.py:284)
-    ru = r;
-    vo = vs != 0.f ? __fdiv_rn(v, vs) : v;
-    ro = vs != 0.f ? __fdiv_rn(r, vs) : r;
-    acc[0] += (double)r;
-    acc[1] += (double)r * (double)r;
+    if constexpr (VN == VN_PPO || VN == VN_BASELINE) v = vn_decode<VN>(v, vs);
+    ret_encode<VN>(vs, v, a, ru, vo, ro, acc);
     acc[2] += (double)a;
     acc[3] += (double)a * (double)a;
 }
 
+// np.var (population variance) from the fp64 sums: the PPO build clamps a NaN to 0, as it always has; PPOF's modes keep it,
+// as np.var of returns holding a NaN or an inf gives NaN
+template <int VN>
+__device__ __forceinline__ double pop_var(double v) {
+    return (VN != VN_PPO && v != v) ? v : fmax(v, 0.0);
+}
+
 // CTA partial sums -> workspace doubles (fp64 atomics: order-dependent in the last bits of a double only; the results are rounded
 // to fp32), the CTA that arrives last writes the statistics and re-zeroes the workspace words
-template <int NT>
+template <int NT, int VN>
 __device__ __forceinline__ void ret_stats_join(double (&acc)[4], const RetArgs& ra, double nn, double* ws_d,
                                                unsigned int* ws_join) {
     double tot[4];
@@ -90,7 +158,7 @@ __device__ __forceinline__ void ret_stats_join(double (&acc)[4], const RetArgs& 
     const double m = s[0] / nn;
     if (ra.stats) {
         ra.stats[0] = (float)m;
-        ra.stats[1] = (float)fmax(s[1] / nn - m * m, 0.0);  // np.var: population variance
+        ra.stats[1] = (float)pop_var<VN>(s[1] / nn - m * m);
         ra.stats[2] = (float)nn;
     }
     if (ra.adv_stats) write_adv_stats(ra.adv_stats, s[2], s[3], nn);

@@ -261,6 +261,64 @@ def normalize_(x, stats):
     return out
 
 
+# the value_norm modes of PPOFPolicy (ding/policy/ppof.py:167), in the order of b200rl_gae_returns_norm's argument
+VALUE_NORMS = ('baseline', 'value_rescale', 'symlog', 'popart')
+GAE_SEQ_MAX_T = 24576  # longest sequence csrc/policy.cu's one-launch kernel takes (GS_MAX_T)
+
+
+def gae_returns_norm_(value, next_value, reward, done, traj_flag, gamma, lambda_, value_norm, std, mu, sigma, want_stats):
+    """PPOFPolicy's advantage recompute (ding/policy/ppof.py:160-210) -- csrc/policy.cu.  value / next_value / reward /
+    done / traj_flag (T, C) contiguous fp32 on one CUDA device; mu / sigma one device float each ('popart').
+    -> (adv, value_out, return_out, stats3 or None, adv_stats2)."""
+    T = value.shape[0]
+    C = value.numel() // T
+    dev = value.device
+    adv = torch.empty_like(value)
+    vout = torch.empty_like(value)
+    rout = torch.empty_like(value)
+    stats = torch.empty(3, dtype=torch.float32, device=dev) if want_stats else None
+    astats = torch.empty(2, dtype=torch.float32, device=dev)
+    scratch = None
+    if not (C == 1 and T <= GAE_SEQ_MAX_T) and value_norm != 'baseline':  # the decode pass of the multi-launch path
+        scratch = torch.empty((1 if value_norm == 'popart' else 2) * value.numel(), dtype=torch.float32, device=dev)
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_gae_returns_norm(
+            ptr(value), ptr(next_value), ptr(reward), ptr(done), ptr(traj_flag), T, C, float(gamma), float(lambda_),
+            VALUE_NORMS.index(value_norm), float(std), ptr(mu), ptr(sigma), ptr(adv), ptr(vout), ptr(rout), ptr(stats),
+            ptr(astats), ptr(scratch), ptr(ws), ws.numel() * 4, stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_gae_returns_norm')
+    return adv, vout, rout, stats, astats
+
+
+class ValueMapFunction(torch.autograd.Function):
+    """symlog (mode 0) / inv_symlog (mode 1) of ding/rl_utils/value_rescale.py:37-66 on a contiguous fp32 CUDA tensor; the
+    backward is torch's autograd of the reference expression (include/b200rl.h)."""
+
+    @staticmethod
+    def forward(ctx, x, mode):
+        y = torch.empty_like(x)
+        if x.numel():
+            with on_device(x.device):
+                rc = lib().b200rl_value_map_fwd(mode, ptr(x), x.numel(), ptr(y), stream_ptr())
+            _lib.check(rc, 'b200rl_value_map_fwd')
+        ctx.mode = mode
+        ctx.save_for_backward(x)
+        return y
+
+    @staticmethod
+    def backward(ctx, g):
+        x, = ctx.saved_tensors
+        g = f32c(g, 'grad')
+        dx = torch.empty_like(x)
+        if x.numel():
+            with on_device(x.device):
+                rc = lib().b200rl_value_map_bwd(ctx.mode, ptr(x), ptr(g), x.numel(), ptr(dx), stream_ptr())
+            _lib.check(rc, 'b200rl_value_map_bwd')
+        return dx, None
+
+
 # ----------------------------------------------------------------------------------------------------------------
 # ppo
 # ----------------------------------------------------------------------------------------------------------------

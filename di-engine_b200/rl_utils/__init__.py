@@ -7,7 +7,7 @@ from .happo import (happo_data, happo_error, happo_error_continuous, happo_polic
                     happo_value_data, happo_value_error)
 from .grpo import grpo_info, grpo_policy_data, grpo_policy_error
 from .log_prob_utils import efficient_method, less_efficient_method, naive_method
-from .gae import gae, gae_data, gae_returns, gae_returns_out, shape_fn_gae
+from .gae import gae, gae_data, gae_returns, gae_returns_out, ppof_gae_returns, ppof_gae_returns_out, shape_fn_gae
 from .ppo import (normalize_advantage, ppo_data, ppo_data_continuous, ppo_error, ppo_error_adv_norm, ppo_error_continuous, ppo_info, ppo_loss,
                   ppo_policy_data, ppo_policy_data_continuous, ppo_policy_error, ppo_policy_error_continuous, ppo_policy_loss,
                   ppo_value_data, ppo_value_error, shape_fn_ppo)
@@ -24,7 +24,7 @@ from .quantile import (fqf_calculate_fraction_loss, fqf_nstep_td_data, fqf_nstep
 from .retrace import compute_q_retraces
 from .rloo import rloo_info, rloo_policy_data, rloo_policy_error
 from .upgo import tb_cross_entropy, upgo_loss, upgo_returns
-from .value_rescale import value_inv_transform, value_transform
+from .value_rescale import inv_symlog, symlog, value_inv_transform, value_transform
 from .vtrace import (impala_reshape_data, shape_fn_vtrace_discrete_action, vtrace_data, vtrace_error_continuous_action,
                      vtrace_error_discrete_action, vtrace_loss)
 
@@ -39,7 +39,9 @@ HOT_PATH_FUNCTIONS = [
     'acer_policy_error', 'acer_value_error', 'acer_trust_region_update', 'ppg_joint_error',
     'dqfd_nstep_td_error', 'dqfd_nstep_td_error_with_rescale',
     'm_q_1step_td_error', 'q_nstep_sql_td_error', 'q_v_1step_td_error',
-    'a2c_error_continuous', 'ppo_policy_error_continuous'
+    'a2c_error_continuous', 'ppo_policy_error_continuous',
+    # PPOFPolicy's value normalisation (ding/policy/ppof.py:13)
+    'symlog', 'inv_symlog'
 ]
 HOT_PATH_TYPES = [
     'gae_data', 'ppo_data', 'ppo_loss', 'ppo_info', 'q_nstep_td_data', 'dist_nstep_td_data', 'td_lambda_data',

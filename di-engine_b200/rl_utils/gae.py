@@ -95,3 +95,77 @@ def gae_returns(data: namedtuple, gamma: float = 0.99, lambda_: float = 0.97, va
         vout, rout = v, unnorm
     out = gae_returns_out(adv, vout, rout, unnorm, stats, astats)
     return gae_returns_out(*[t.cpu() for t in out]) if host_out else out
+
+
+ppof_gae_returns_out = namedtuple('ppof_gae_returns_out', ['adv', 'value', 'return_', 'return_stats', 'adv_stats'])
+
+
+def ppof_gae_returns(data: namedtuple, gamma: float = 0.99, lambda_: float = 0.97, value_norm: str = 'baseline', std=None,
+                     popart_mu=None, popart_sigma=None) -> namedtuple:
+    """
+    ``PPOFPolicy.forward``'s advantage recompute (ding/policy/ppof.py:160-210) in one call -- not a reference function, exactly
+    those reference lines (csrc/policy.cu)::
+
+        # decode the critic's output ('pred') -- ppof.py:171-189
+        popart:        reward = (reward - mu) / sigma            value, next_value as they are
+        value_rescale: value = value_inv_transform(value)        next_value likewise
+        symlog:        value = inv_symlog(value)                 next_value likewise
+        baseline:      value = value * std                       next_value likewise   (std = RunningMeanStd.std)
+        adv = gae(gae_data(value, next_value, reward, done, traj_flag), gamma, lambda_)
+        unnormalized_returns = value + adv
+        # encode -- ppof.py:197-210
+        value_rescale: value, return_ = value_transform(value), value_transform(unnormalized_returns)
+        symlog:        value, return_ = symlog(value), symlog(unnormalized_returns)
+        baseline:      value, return_ = value / std, unnormalized_returns / std
+                       running_mean_std.update(return_.cpu().numpy())   # here: three device floats {mean, np.var, count}
+        popart:        value, return_ = value, unnormalized_returns
+
+    ``data`` as for ``gae``: value shaped like reward ((n,) -- PPOF's one sequence of n_sample steps, scanned in one launch --
+    or (T, B)), or with a trailing dim of 1 against that reward (PopArt's (n, 1) prediction, gae.py:56-59).  ``std``: the
+    running std, required for 'baseline'.  ``popart_mu`` / ``popart_sigma``: the PopArt head's ``mu`` / ``sigma`` buffers
+    (one float each, read on the device), required for 'popart'.  The inputs are NOT modified (the reference masks
+    ``next_value`` in place inside ``gae``).  Returns ``ppof_gae_returns_out(adv, value, return_, return_stats, adv_stats)``
+    with adv / value / return_ shaped like value; ``return_stats`` = (mean, population variance, count) of ``return_`` in
+    'baseline' (what ``RunningMeanStd.update`` computes from it), None otherwise; ``adv_stats`` = (adv.mean(), adv.std() + 1e-8)
+    of the whole batch from the same pass.  PopArt's ``update_parameters`` and ``RunningMeanStd.update`` stay with the caller.
+    """
+    value, next_value, reward, done, traj_flag = data
+    if value_norm not in ops.VALUE_NORMS:
+        raise ValueError("ppof_gae_returns: value_norm must be one of %s, got %r" % (ops.VALUE_NORMS, value_norm))
+    if value_norm == 'baseline':
+        if std is None:
+            raise ValueError("ppof_gae_returns: value_norm='baseline' needs std (RunningMeanStd.std)")
+        std = float(std)
+        if not std > 0.0:
+            raise ValueError("ppof_gae_returns: std must be > 0, got %r" % std)
+    else:
+        std = 0.0
+    if value_norm == 'popart' and (popart_mu is None or popart_sigma is None):
+        raise ValueError("ppof_gae_returns: value_norm='popart' needs popart_mu and popart_sigma")
+    lead = value.shape[:-1] if (value.dim() == reward.dim() + 1 and value.shape[-1] == 1) else value.shape
+    if tuple(lead) != tuple(reward.shape) or next_value.shape != value.shape or reward.dim() not in (1, 2):
+        raise ValueError("ppof_gae_returns: value %s / next_value %s / reward %s must share a (T,) or (T, B) shape" %
+                         (tuple(value.shape), tuple(next_value.shape), tuple(reward.shape)))
+    dev = ops.compute_device(value, next_value, reward)
+    host_out = not value.is_cuda
+    v = ops.f32c(ops.to_device(value.detach(), dev), 'value').reshape(reward.shape)
+    nv = ops.f32c(ops.to_device(next_value.detach(), dev), 'next_value').reshape(reward.shape)
+    r = ops.f32c(ops.to_device(reward.detach(), dev), 'reward')
+    d = ops.f32c(ops.to_device(done.detach(), dev), 'done') if done is not None else None
+    tf = ops.f32c(ops.to_device(traj_flag.detach(), dev), 'traj_flag') if traj_flag is not None else None
+    if d is not None and d.shape != r.shape:
+        d = d.expand_as(r).contiguous()
+    if tf is not None and tf.shape != r.shape:
+        tf = tf.expand_as(r).contiguous()
+    mu = sigma = None
+    if value_norm == 'popart':
+        mu = ops.f32c(ops.to_device(popart_mu.detach(), dev), 'popart_mu').reshape(-1)
+        sigma = ops.f32c(ops.to_device(popart_sigma.detach(), dev), 'popart_sigma').reshape(-1)
+        if mu.numel() != 1 or sigma.numel() != 1:
+            raise ValueError("ppof_gae_returns: popart_mu / popart_sigma must hold one float each (a single-output PopArt head)")
+    adv, vout, rout, stats, astats = ops.gae_returns_norm_(v, nv, r, d, tf, gamma, lambda_, value_norm, std, mu, sigma,
+                                                           value_norm == 'baseline')
+    out = ppof_gae_returns_out(adv.reshape(value.shape), vout.reshape(value.shape), rout.reshape(value.shape), stats, astats)
+    if host_out:
+        out = ppof_gae_returns_out(*[None if t is None else t.cpu() for t in out])
+    return out

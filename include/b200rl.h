@@ -84,6 +84,37 @@ B200RL_API int b200rl_adv_stats(const float* x, long long n, float* stats2, floa
                      void* stream);
 B200RL_API int b200rl_normalize(const float* x, const float* stats2, long long n, float* out, void* stream);
 
+/* ---- PPOFPolicy's advantage recompute (ding/policy/ppof.py:160-210) in one call --------------------------------------
+ * value, next_value, reward, adv, value_out, return_out: (T, C); done / traj_flag (T, C) nullable as for b200rl_gae.  The
+ * inputs are only read.  value_norm selects how the critic's output is decoded before gae and the value / return encoded
+ * after it (unnormalized_returns = value + adv, ppof.py:195):
+ *   0 'baseline'       value * std, next_value * std on load; value_out = (value * std) / std, return_out = (value * std + adv)
+ *                      / std; stats3 = {mean, population variance, count} of return_out -- the array RunningMeanStd.update
+ *                      receives (ppof.py:206-208 divides in place).  std > 0.
+ *   1 'value_rescale'  value_inv_transform on load (eps = 1e-2); value_out = h(h^-1(value)), return_out = h(h^-1(value) + adv)
+ *   2 'symlog'         inv_symlog on load; value_out = symlog(inv_symlog(value)), return_out = symlog(inv_symlog(value) + adv)
+ *   3 'popart'         reward -> (reward - mu) / sigma on load, popart_mu / popart_sigma one device float each (read on the
+ *                      device); value_out = value, return_out = value + adv
+ * adv_stats2 = {mean, std(unbiased) + 1e-8} of adv as for b200rl_gae_returns.  Every output but adv is nullable.
+ * C == 1 and T <= 24576 (every PPOF call): one launch.  Otherwise one element-wise decode launch ('value_rescale' / 'symlog':
+ * value and next_value into scratch[0, 2 T C); 'popart': reward into scratch[0, T C); 'baseline' needs none: the scan scales
+ * on load), the streaming scan of b200rl_gae, and one element-wise epilogue launch; scratch may be null on the one-launch path
+ * and for 'baseline'.  B200RL_ERR_ARG before any launch for an unknown value_norm, std <= 0 in 'baseline', a missing mu /
+ * sigma in 'popart' or a missing scratch. */
+B200RL_API int b200rl_gae_returns_norm(const float* value, const float* next_value, const float* reward, const float* done,
+                            const float* traj_flag, long long T, long long C, double gamma, double lambda_,
+                            int value_norm, double std, const float* popart_mu, const float* popart_sigma, float* adv,
+                            float* value_out, float* return_out, float* stats3, float* adv_stats2, float* scratch,
+                            float* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- symlog / inv_symlog: ding/rl_utils/value_rescale.py:37-66, element-wise over n floats -------------------------------
+ * mode 0: y = sign(x) * log(|x| + 1);  mode 1: y = sign(x) * (exp(|x|) - 1)  (sign(NaN) = sign(-0) = 0, as torch.sign).
+ * The backward is torch's autograd of those expressions for the upstream gradient g:
+ *   mode 0: dx = ((g * sign(x)) / (|x| + 1)) * sign(x);  mode 1: dx = ((g * sign(x)) * exp(|x|)) * sign(x)
+ * plus sign's zero gradient, so dx = +0 where x = 0.  n == 0 launches nothing. */
+B200RL_API int b200rl_value_map_fwd(int mode, const float* x, long long n, float* y, void* stream);
+B200RL_API int b200rl_value_map_bwd(int mode, const float* x, const float* g, long long n, float* dx, void* stream);
+
 /* IMPALAPolicy._reshape_data masking (ding/policy/impala.py:316-322) in one elementwise launch: values (T+1, B), rewards /
  * done (T, B) -> values_out[t] = values[t] * (1 - done[t-1]) (t >= 1), weights_out[t] = 1 - done[t-1] (1 at t = 0),
  * rewards_out = rewards * weights_out.  rewards_out / weights_out nullable: the backward pass masks d/d values with the same
