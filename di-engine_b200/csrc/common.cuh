@@ -164,7 +164,7 @@ __device__ __forceinline__ bool grid_sum(float (&v)[K], double (&tot)[K], float*
 // spilled CTA never touches words 2 / 3.  A one-CTA grid skips the atomics.  (In the big streaming kernels the same scheme
 // LOSES to a dependent finalize launch -- the atomics return only after the SM's store traffic has drained.)
 #define WS_FX_OFF_WORDS 257024   // 16 packed u64 accumulators (zero between launches), above every kernel's partial sums
-#define WS_FX_SPILL_WORDS 257088 // 16 more (words 2 / 3 of each sum), past the doubles and joins policy.cu keeps at +32..+49
+#define WS_FX_SPILL_WORDS 257088 // 16 more (words 2 / 3 of each sum), past the statistics ticket policy.cu keeps at +48
 constexpr int FX_MAX_K = 8;
 constexpr unsigned int FX_MAX_GRID = 511;
 

@@ -160,16 +160,16 @@ __global__ void __launch_bounds__(GS_NT) gae_seq_kernel(const float* __restrict_
         for (int t = tid; t <= c; t += GS_NT) s_d[t] = __int_as_float(0x7fc00000);
         __syncthreads();
     }
-    // ---- phase 4: write-out (+ returns, value-norm, statistics)
-    double acc[4] = {0.0, 0.0, 0.0, 0.0};
+    // ---- phase 4: write-out (+ returns, value-norm, statistics around element 0's pivots)
+    double acc[4] = {0.0, 0.0, 0.0, 0.0}, pv[2];
+    ret_pivots<VN>(vs, vn_decode<VN>(ld_after_wait(value), vs), s_d[0], pv);
     for (int t = tid; t < T; t += GS_NT) {
         const float a = s_d[t];
         adv[t] = a;
-        acc[2] += (double)a;
-        acc[3] += (double)a * (double)a;
+        moments_add(acc[2], acc[3], a, pv[1]);
         if (ra.ret_unnorm || ra.value_out || ra.ret_out || ra.stats) {
             float ru, vo, ro;
-            ret_encode<VN>(vs, vn_decode<VN>(value[t], vs), a, ru, vo, ro, acc);
+            moments_add(acc[0], acc[1], ret_encode<VN>(vs, vn_decode<VN>(value[t], vs), a, ru, vo, ro), pv[0]);
             if (ra.ret_unnorm) ra.ret_unnorm[t] = ru;
             if (ra.value_out) ra.value_out[t] = vo;
             if (ra.ret_out) ra.ret_out[t] = ro;
@@ -177,93 +177,92 @@ __global__ void __launch_bounds__(GS_NT) gae_seq_kernel(const float* __restrict_
     }
     if (ra.stats || ra.adv_stats) {
         double tot[4];
-        block_sum_d<4, GS_NT>(acc, tot);
-        if (tid == 0) {
-            const double n = (double)T, m = tot[0] / n;
-            if (ra.stats) {
-                ra.stats[0] = (float)m;
-                ra.stats[1] = (float)pop_var<VN>(tot[1] / n - m * m);
-                ra.stats[2] = (float)n;
-            }
-            if (ra.adv_stats) write_adv_stats(ra.adv_stats, tot[2], tot[3], n);
-        }
+        if (stats_grid_join<4, GS_NT>(acc, tot, nullptr, nullptr)) write_ret_stats<VN>(ra, tot, pv, (double)T);
     }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // (T, B) epilogue behind gae_ws_kernel: returns / value-norm / statistics in one elementwise pass.  The scaling modes read the
 // raw value; the others read the value the decode pass (value_map_kernel) wrote.
-// The four sums (r, r^2, adv, adv^2) are reduced per CTA in fp64 and joined across CTAs with fp64 atomics; the CTA that
-// arrives last writes the statistics (ret_stats_join).
+// The four shifted sums of r and adv (ret_one) are reduced per CTA in fp64 and joined across CTAs in a fixed order; the CTA
+// that arrives last writes the statistics (stats_grid_join, write_ret_stats).
 // ---------------------------------------------------------------------------------------------------------------
 template <int VN, bool VEC>
 __global__ void __launch_bounds__(256) returns_kernel(const float* __restrict__ value, const float* __restrict__ adv,
-                                                      long long n, RetArgs ra, double* __restrict__ ws_d,
+                                                      long long n, RetArgs ra, double* __restrict__ ws_part,
                                                       unsigned int* __restrict__ ws_join) {
     pdl_prologue();
     const float vs = ra.vscale;
-    double acc[4] = {0.0, 0.0, 0.0, 0.0};
+    double acc[4] = {0.0, 0.0, 0.0, 0.0}, pv[2];
+    // the first element of each thread is loaded together with the pivots, so that their latency is paid once
+    const long long stride = (long long)gridDim.x * 256;
+    long long i = (long long)blockIdx.x * 256 + threadIdx.x;
     if (VEC) {  // n % 4 == 0, 16-byte aligned tensors
         const long long n4 = n >> 2;
-        for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
-            const float4 v = reinterpret_cast<const float4*>(value)[i], a = reinterpret_cast<const float4*>(adv)[i];
+        const float4* v4 = reinterpret_cast<const float4*>(value);
+        const float4* a4 = reinterpret_cast<const float4*>(adv);
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f), a = v;
+        if (i < n4) {
+            v = v4[i];
+            a = a4[i];
+        }
+        ret_pivots<VN>(vs, ret_value<VN>(ld_after_wait(value), vs), ld_after_wait(adv), pv);
+        for (; i < n4; i += stride) {
             float4 ru, vo, ro;
-            ret_one<VN>(vs, v.x, a.x, ru.x, vo.x, ro.x, acc);
-            ret_one<VN>(vs, v.y, a.y, ru.y, vo.y, ro.y, acc);
-            ret_one<VN>(vs, v.z, a.z, ru.z, vo.z, ro.z, acc);
-            ret_one<VN>(vs, v.w, a.w, ru.w, vo.w, ro.w, acc);
+            ret_one<VN>(vs, v.x, a.x, ru.x, vo.x, ro.x, acc, pv);
+            ret_one<VN>(vs, v.y, a.y, ru.y, vo.y, ro.y, acc, pv);
+            ret_one<VN>(vs, v.z, a.z, ru.z, vo.z, ro.z, acc, pv);
+            ret_one<VN>(vs, v.w, a.w, ru.w, vo.w, ro.w, acc, pv);
             if (ra.ret_unnorm) reinterpret_cast<float4*>(ra.ret_unnorm)[i] = ru;
             if (ra.value_out) reinterpret_cast<float4*>(ra.value_out)[i] = vo;
             if (ra.ret_out) reinterpret_cast<float4*>(ra.ret_out)[i] = ro;
+            if (i + stride < n4) {
+                v = v4[i + stride];
+                a = a4[i + stride];
+            }
         }
     } else {
-        for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+        float v = 0.f, a = 0.f;
+        if (i < n) {
+            v = value[i];
+            a = adv[i];
+        }
+        ret_pivots<VN>(vs, ret_value<VN>(ld_after_wait(value), vs), ld_after_wait(adv), pv);
+        for (; i < n; i += stride) {
             float ru, vo, ro;
-            ret_one<VN>(vs, value[i], adv[i], ru, vo, ro, acc);
+            ret_one<VN>(vs, v, a, ru, vo, ro, acc, pv);
             if (ra.ret_unnorm) ra.ret_unnorm[i] = ru;
             if (ra.value_out) ra.value_out[i] = vo;
             if (ra.ret_out) ra.ret_out[i] = ro;
+            if (i + stride < n) {
+                v = value[i + stride];
+                a = adv[i + stride];
+            }
         }
     }
     if (!ra.stats && !ra.adv_stats) return;
-    ret_stats_join<256, VN>(acc, ra, (double)n, ws_d, ws_join);
+    double tot[4];
+    if (stats_grid_join<4, 256>(acc, tot, ws_part, ws_join)) write_ret_stats<VN>(ra, tot, pv, (double)n);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // advantage statistics {mean, std (unbiased, torch.std) + 1e-8} and the normalisation itself
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) adv_stats_kernel(const float* __restrict__ x, long long n, float* __restrict__ out,
-                                                        double* __restrict__ ws_d, unsigned int* __restrict__ ws_join) {
+                                                        double* __restrict__ ws_part, unsigned int* __restrict__ ws_join) {
     pdl_prologue();
+    const double p = stats_pivot(ld_after_wait(x));
     double acc[2] = {0.0, 0.0};
-    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
-        const double v = (double)x[i];
-        acc[0] += v;
-        acc[1] += v * v;
-    }
+    for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256)
+        moments_add(acc[0], acc[1], x[i], p);
     double tot[2];
-    block_sum_d<2, 256>(acc, tot);
-    if (threadIdx.x != 0) return;
-    double s1 = tot[0], s2 = tot[1];
-    if (gridDim.x > 1) {
-        atomicAdd(ws_d, s1);
-        atomicAdd(ws_d + 1, s2);
-        __threadfence();
-        if (atomicAdd(ws_join, 1u) != gridDim.x - 1) return;
-        __threadfence();
-        s1 = atomicAdd(ws_d, 0.0);
-        s2 = atomicAdd(ws_d + 1, 0.0);
-        ws_d[0] = 0.0;
-        ws_d[1] = 0.0;
-        *ws_join = 0u;
-    }
-    write_adv_stats(out, s1, s2, (double)n);
+    if (stats_grid_join<2, 256>(acc, tot, ws_part, ws_join)) write_adv_stats(out, tot[0], tot[1], p, (double)n);
 }
 
 __global__ void __launch_bounds__(256) normalize_kernel(const float* __restrict__ x, const float* __restrict__ stats,
                                                         long long n, float* __restrict__ out) {
     pdl_prologue();
-    const float m = stats[0], d = stats[1];
+    const float m = ld_after_wait(stats), d = ld_after_wait(stats + 1);  // adv_stats_kernel wrote them just before
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256)
         out[i] = __fdiv_rn(fsub(x[i], m), d);
 }
@@ -346,9 +345,12 @@ int gae_scan(const float* value, float* next_value, const float* reward, const f
              float vscale, void* stream);
 }
 
-// workspace words used by the two-sum joins above: 4 doubles + 2 counters right after the packed accumulators of grid_sum_fx
-static double* ws_doubles(float* ws) { return reinterpret_cast<double*>(ws + WS_FX_OFF_WORDS + 32); }
+// workspace of the statistics joins above: the per-CTA rows of fp64 sums (at most NUM_SMS * 8 CTAs x 4 doubles) in the partial
+// region, and the ticket right after the packed accumulators of grid_sum_fx
+static double* ws_stats_part(float* ws) { return reinterpret_cast<double*>(ws + WS_CTRL_WORDS); }
 static unsigned int* ws_joins(float* ws) { return reinterpret_cast<unsigned int*>(ws + WS_FX_OFF_WORDS + 48); }
+static_assert(WS_CTRL_WORDS % 2 == 0 && WS_CTRL_WORDS + NUM_SMS * 8 * 4 * 2 <= WS_PARTIAL_LIMIT_WORDS,
+              "the statistics rows fit the workspace's partial region");
 
 extern "C" int b200rl_adv_stats(const float* x, long long n, float* stats2, float* workspace, size_t workspace_bytes,
                                 void* stream) {
@@ -356,7 +358,7 @@ extern "C" int b200rl_adv_stats(const float* x, long long n, float* stats2, floa
     long long grid = div_up(n, 256 * 8);
     if (grid > NUM_SMS * 4) grid = NUM_SMS * 4;
     if (grid < 1) grid = 1;
-    return launch_k(adv_stats_kernel, (int)grid, 256, 0, (cudaStream_t)stream, x, n, stats2, ws_doubles(workspace),
+    return launch_k(adv_stats_kernel, (int)grid, 256, 0, (cudaStream_t)stream, x, n, stats2, ws_stats_part(workspace),
                     ws_joins(workspace));
 }
 
@@ -399,9 +401,9 @@ extern "C" int b200rl_gae_returns(const float* value, float* next_value, const f
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
     if (vec)
         return launch_k(returns_kernel<VN_PPO, true>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra,
-                        ws_doubles(workspace), ws_joins(workspace));
+                        ws_stats_part(workspace), ws_joins(workspace));
     return launch_k(returns_kernel<VN_PPO, false>, (int)grid, 256, 0, st, value, (const float*)adv, n, ra,
-                    ws_doubles(workspace), ws_joins(workspace));
+                    ws_stats_part(workspace), ws_joins(workspace));
 }
 
 // ---- PPOFPolicy's advantage recompute (ding/policy/ppof.py:160-210) -----------------------------------------------------------
@@ -429,9 +431,9 @@ static int launch_returns(const float* value, const float* adv, long long n, con
     long long grid = div_up(n, 256 * (vec ? 8 : 4));
     if (grid > NUM_SMS * 8) grid = NUM_SMS * 8;
     if (vec)
-        return launch_k(returns_kernel<VN, true>, (int)grid, 256, 0, st, value, adv, n, ra, ws_doubles(workspace),
+        return launch_k(returns_kernel<VN, true>, (int)grid, 256, 0, st, value, adv, n, ra, ws_stats_part(workspace),
                         ws_joins(workspace));
-    return launch_k(returns_kernel<VN, false>, (int)grid, 256, 0, st, value, adv, n, ra, ws_doubles(workspace),
+    return launch_k(returns_kernel<VN, false>, (int)grid, 256, 0, st, value, adv, n, ra, ws_stats_part(workspace),
                     ws_joins(workspace));
 }
 

@@ -96,73 +96,121 @@ __device__ __forceinline__ float vn_encode(float v, float vs) {
 }
 
 // the element-wise part of the epilogue for a DECODED value v and its advantage a: unnormalized return
-// (unnormalized_returns = value + adv, ppo.py:284 / ppof.py:195), stored value / return, and the sums of the return the
-// statistics describe (PPOPolicy: the unnormalised one; PPOF: the stored one)
+// (unnormalized_returns = value + adv, ppo.py:284 / ppof.py:195) and stored value / return; returns the value the return
+// statistics describe (PPOPolicy: the unnormalised return; PPOF: the stored one)
 template <int VN>
-__device__ __forceinline__ void ret_encode(float vs, float v, float a, float& ru, float& vo, float& ro, double (&acc)[4]) {
+__device__ __forceinline__ float ret_encode(float vs, float v, float a, float& ru, float& vo, float& ro) {
     const float r = fadd(v, a);
     ru = r;
     vo = vn_encode<VN>(v, vs);
     ro = vn_encode<VN>(r, vs);
-    const float s = VN == VN_PPO ? r : ro;
-    acc[0] += (double)s;
-    acc[1] += (double)s * (double)s;
+    return VN == VN_PPO ? r : ro;
 }
 
-// {mean, torch.std (unbiased) + 1e-8} from the fp64 sums of x and x^2
-__device__ __forceinline__ void write_adv_stats(float* out, double s1, double s2, double nn) {
-    const double m = s1 / nn;
-    const double var = (s2 - s1 * m) / (nn - 1.0);  // n == 1 -> nan, as torch.std
+// ---------------------------------------------------------------------------------------------------------------
+// Batch statistics.  Every kernel accumulates, per statistic, the fp64 sums of (x - p) and (x - p)^2 around a pivot p: one
+// element of the batch (element 0, 0 when it is not finite), the same in every thread.  The plain sums of x and x^2 lose
+// (mean / sd)^2 of the double's precision to cancellation in S2/n - m^2 -- all of fp32's with a mean 1e4 sd away.  With a
+// pivot from the batch, (p - mean)^2 <= n * var, so the loss is bounded by the batch size, whatever the offset.
+// Per-CTA sums are joined across the grid in a fixed order (stats_grid_join): bit-identical from run to run.
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ double stats_pivot(float x0) { return isfinite(x0) ? (double)x0 : 0.0; }
+
+// A global load that stays behind pdl_prologue's griddepcontrol.wait.  The compiler may hoist a loop-invariant load through
+// a const __restrict__ pointer above it (it takes the data as read-only for the kernel's lifetime): with plain value[0] /
+// adv[0] loads, the sm_90a build of returns_kernel issued both as LDG.E.CONSTANT ahead of PREEXIT / ACQBULK, so the pivot was
+// read before gae_scan -- which writes adv[0] last -- had finished, and the statistics changed from run to run.  __ldcg is
+// not such a load; the compiler keeps it behind the wait.
+__device__ __forceinline__ float ld_after_wait(const float* p) { return __ldcg(p); }
+
+__device__ __forceinline__ void moments_add(double& s1, double& s2, float x, double p) {
+    const double d = (double)x - p;
+    s1 += d;
+    s2 = fma(d, d, s2);
+}
+
+// the decoded value of a value returns_kernel reads: raw for the scaling modes, already decoded by the decode pass for the
+// others
+template <int VN>
+__device__ __forceinline__ float ret_value(float v, float vs) {
+    if constexpr (VN == VN_PPO || VN == VN_BASELINE) return vn_decode<VN>(v, vs);
+    else return v;
+}
+
+// (T, B) epilogue element: ret_encode of the decoded value, then the shifted sums of the return (acc[0..1], pivot pv[0]) and
+// of adv (acc[2..3], pv[1])
+template <int VN>
+__device__ __forceinline__ void ret_one(float vs, float v, float a, float& ru, float& vo, float& ro, double (&acc)[4],
+                                        const double (&pv)[2]) {
+    moments_add(acc[0], acc[1], ret_encode<VN>(vs, ret_value<VN>(v, vs), a, ru, vo, ro), pv[0]);
+    moments_add(acc[2], acc[3], a, pv[1]);
+}
+
+// the pivots of the shifted sums: element 0's statistics source and advantage, from its DECODED value v0 (the value
+// ret_encode receives for element 0: the pivot must be a member of the batch)
+template <int VN>
+__device__ __forceinline__ void ret_pivots(float vs, float v0, float a0, double (&pv)[2]) {
+    float ru, vo, ro;
+    pv[0] = stats_pivot(ret_encode<VN>(vs, v0, a0, ru, vo, ro));
+    pv[1] = stats_pivot(a0);
+}
+
+// Grid-wide totals of K per-thread fp64 sums.  Thread 0 of every CTA stores the CTA's sums to the workspace's partial rows
+// (part[blockIdx.x * K + k]) and takes a ticket; the CTA that draws the last one adds the rows in a fixed order (thread i:
+// rows i, i + NT, ...; then block_sum_d) and resets the ticket.  Returns true in thread 0 of that CTA, which then holds the
+// totals in tot.  A one-CTA grid touches neither the rows nor the ticket.
+template <int K, int NT>
+__device__ __forceinline__ bool stats_grid_join(double (&acc)[K], double (&tot)[K], double* part, unsigned int* ticket) {
+    __shared__ bool s_last;
+    block_sum_d<K, NT>(acc, tot);
+    if (gridDim.x == 1) return threadIdx.x == 0;
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) part[(size_t)blockIdx.x * K + k] = tot[k];
+        __threadfence();
+        s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!s_last) return false;
+    __threadfence();
+    double v[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) v[k] = 0.0;
+    for (unsigned int b = threadIdx.x; b < gridDim.x; b += NT)
+#pragma unroll
+        for (int k = 0; k < K; ++k) v[k] += __ldcg(part + (size_t)b * K + k);
+    block_sum_d<K, NT>(v, tot);
+    if (threadIdx.x == 0) *ticket = 0u;
+    return threadIdx.x == 0;
+}
+
+// {mean, torch.std (unbiased) + 1e-8} from the shifted sums s1 = sum(x - p), s2 = sum((x - p)^2)
+__device__ __forceinline__ void write_adv_stats(float* out, double s1, double s2, double p, double nn) {
+    const double d = s1 / nn;
+    const double var = (s2 - s1 * d) / (nn - 1.0);  // n == 1 -> nan, as torch.std
     const double sd = var != var ? var : sqrt(fmax(var, 0.0));
-    out[0] = (float)m;
+    out[0] = (float)(p + d);
     out[1] = fadd((float)sd, 1e-8f);
 }
 
-
-// the element-wise part of the (T, B) epilogue for one (value, adv) pair: the value as returns_kernel reads it (raw for the
-// scaling modes, already decoded by the decode pass for the others), then ret_encode, then the advantage sums
-template <int VN>
-__device__ __forceinline__ void ret_one(float vs, float v, float a, float& ru, float& vo, float& ro, double (&acc)[4]) {
-    if constexpr (VN == VN_PPO || VN == VN_BASELINE) v = vn_decode<VN>(v, vs);
-    ret_encode<VN>(vs, v, a, ru, vo, ro, acc);
-    acc[2] += (double)a;
-    acc[3] += (double)a * (double)a;
-}
-
-// np.var (population variance) from the fp64 sums: the PPO build clamps a NaN to 0, as it always has; PPOF's modes keep it,
-// as np.var of returns holding a NaN or an inf gives NaN
+// np.var (population variance) from the shifted sums: the PPO build clamps a NaN to 0, as it always has; PPOF's modes keep
+// it, as np.var of returns holding a NaN or an inf gives NaN
 template <int VN>
 __device__ __forceinline__ double pop_var(double v) {
     return (VN != VN_PPO && v != v) ? v : fmax(v, 0.0);
 }
 
-// CTA partial sums -> workspace doubles (fp64 atomics: order-dependent in the last bits of a double only; the results are rounded
-// to fp32), the CTA that arrives last writes the statistics and re-zeroes the workspace words
-template <int NT, int VN>
-__device__ __forceinline__ void ret_stats_join(double (&acc)[4], const RetArgs& ra, double nn, double* ws_d,
-                                               unsigned int* ws_join) {
-    double tot[4];
-    block_sum_d<4, NT>(acc, tot);
-    if (threadIdx.x != 0) return;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) atomicAdd(ws_d + k, tot[k]);
-    __threadfence();
-    if (atomicAdd(ws_join, 1u) != gridDim.x - 1) return;
-    __threadfence();
-    double s[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        s[k] = atomicAdd(ws_d + k, 0.0);
-        ws_d[k] = 0.0;
-    }
-    const double m = s[0] / nn;
+// the statistics of gae_seq_kernel / returns_kernel from the grid totals of ret_one's four sums
+template <int VN>
+__device__ __forceinline__ void write_ret_stats(const RetArgs& ra, const double (&tot)[4], const double (&pv)[2],
+                                                double nn) {
     if (ra.stats) {
-        ra.stats[0] = (float)m;
-        ra.stats[1] = (float)pop_var<VN>(s[1] / nn - m * m);
+        const double d = tot[0] / nn;
+        ra.stats[0] = (float)(pv[0] + d);
+        ra.stats[1] = (float)pop_var<VN>(tot[1] / nn - d * d);
         ra.stats[2] = (float)nn;
     }
-    if (ra.adv_stats) write_adv_stats(ra.adv_stats, s[2], s[3], nn);
-    *ws_join = 0u;
+    if (ra.adv_stats) write_adv_stats(ra.adv_stats, tot[2], tot[3], pv[1], nn);
 }
 
 }  // namespace b200rl
