@@ -2,6 +2,83 @@
 #include "../../include/b200rl.h"
 #include "common.cuh"
 
+#include <mutex>
+
+// ---------------------------------------------------------------------------------------------------------------
+// The record of the step chain on each (device, stream) (common.cuh): the capture it belongs to, the node of its last
+// launch, and the bytes its launches may write since the last column kernel.
+// ---------------------------------------------------------------------------------------------------------------
+namespace b200rl {
+namespace {
+constexpr int CHAIN_STREAMS = 8;  // streams per device with a record; the oldest record gives way
+constexpr int CHAIN_SPANS = 16;   // write spans per record (a column kernel + finalize + check report 11 at most)
+struct StepChain {
+    cudaStream_t st;
+    unsigned long long id;
+    void* last;  // null: no record
+    int n;
+    ByteSpan w[CHAIN_SPANS];
+};
+StepChain g_chain[MAX_DEVICES][CHAIN_STREAMS];
+int g_chain_next[MAX_DEVICES];
+std::mutex g_chain_mu;
+
+StepChain* chain_of(int dev, cudaStream_t st) {
+    for (StepChain& c : g_chain[dev])
+        if (c.last && c.st == st) return &c;
+    return nullptr;
+}
+bool overlaps(const ByteSpan& a, const ByteSpan& b) { return a.lo < b.hi && b.lo < a.hi; }
+}  // namespace
+
+ChainPoint capture_now(cudaStream_t st) {
+    ChainPoint at{};
+    if (current_device(at.dev) != B200RL_OK) return at;
+    cudaStreamCaptureStatus s;
+    const cudaGraphNode_t* deps = nullptr;
+    size_t nd = 0;
+    // a stream that cannot be queried is treated as not captured: the launch itself reports what is wrong with it
+    if (cuda_rc(cudaStreamGetCaptureInfo(st, &s, &at.id, nullptr, &deps, &nd)) != B200RL_OK) return at;
+    at.capturing = s == cudaStreamCaptureStatusActive;
+    at.dep = (at.capturing && nd == 1) ? (void*)deps[0] : nullptr;
+    return at;
+}
+
+bool chain_may_defer(cudaStream_t st, const ChainPoint& at, const ByteSpan* reads, int n_reads) {
+    if (!at.capturing || !at.dep || !pdl_enabled()) return false;
+    std::lock_guard<std::mutex> lock(g_chain_mu);
+    const StepChain* c = chain_of(at.dev, st);
+    if (!c || c->id != at.id || c->last != at.dep) return false;
+    for (int i = 0; i < n_reads; ++i)
+        for (int k = 0; k < c->n; ++k)
+            if (overlaps(reads[i], c->w[k])) return false;
+    return true;
+}
+
+void chain_report(cudaStream_t st, const ChainPoint& at, bool starts, const ByteSpan* writes, int n_writes) {
+    std::lock_guard<std::mutex> lock(g_chain_mu);
+    StepChain* c = chain_of(at.dev, st);
+    ChainPoint now{};
+    if (at.capturing) now = capture_now(st);
+    // the chain goes on only where this launch followed it directly (a check) or starts it, in the same capture
+    const bool follows = c && c->id == at.id && at.dep && c->last == at.dep;
+    if (!now.capturing || !now.dep || now.id != at.id || (!starts && !follows) ||
+        (starts ? 0 : c->n) + n_writes > CHAIN_SPANS) {
+        if (c) c->last = nullptr;
+        return;
+    }
+    if (!c) {
+        c = &g_chain[at.dev][g_chain_next[at.dev]];
+        g_chain_next[at.dev] = (g_chain_next[at.dev] + 1) % CHAIN_STREAMS;
+    }
+    if (starts) c->n = 0;
+    c->st = st;
+    c->id = at.id;
+    c->last = now.dep;
+    for (int i = 0; i < n_writes; ++i) c->w[c->n++] = writes[i];
+}
+}  // namespace b200rl
+
 extern "C" int b200rl_version(void) { return 109; }
 extern "C" int b200rl_built_for_sm(void) { return 90; }
 extern "C" size_t b200rl_workspace_bytes(void) { return (size_t)WS_MIN_BYTES; }

@@ -43,6 +43,14 @@
 // two loader warps (the faster refill issues the ring of every CTA in one burst, which delays chunk 0 and costs DRAM
 // efficiency), the same with a throttled prologue, no unrolling of the copy loop, 2 or 3 ring stages.
 //
+// Between two steps HBM idled: a CTA of the next step started 0.4 - 0.5 us (median over SMs) after the previous step's
+// CTA on the same SM had ended (the 8-stage ring leaves no room for both), then waited for finalize_sums and the check
+// launch and had its first chunk 5.8 - 6.5 us after that end.  A captured step that reads nothing those launches write
+// therefore defers its griddepcontrol.wait (FusedArgs::defer_wait, decided on the host, common.cuh): its first chunk lands
+// 2.4 - 5.4 us before the previous check has completed, and config D went from 25.8 to 24.2 us per step (H100 SXM, 700 W,
+// 1980 MHz).  Slower: a 4-stage ring with __launch_bounds__(..., 2) (80 registers) in that mode, which lets the next
+// step's CTA share the SM with the previous one on most SMs but streams slower: 27.7 us.
+//
 // Algorithmic traffic: 24 B (GAE) + 104 B (ppo_error forward + gradients, N = 6) = 128 B per transition, each byte once.
 #include "../../include/b200rl.h"
 #include "fused_args.cuh"
@@ -68,9 +76,11 @@ constexpr int CW_RAW_BYTES = 5 * CW_RAW_ARR;  // value | next_value | reward | d
 
 // B200RL_FUSED_TRACE=1: %globaltimer stamps, 64 per CTA (tools/trace_col.py).  Slots 0-7 frame the CTA: 0 start, 1 the
 // previous launches' results visible (after griddepcontrol.wait), 2 first chunk's advantages published, 3 / 4 / 5 the
-// last chunk landed / advantages ready / computed, 6 end (partial sums stored), 7 the number of chunks (a count).  Chunk
-// j < CW_TRACE_CHUNKS: 8 + 4j landed, 9 + 4j advantages ready, 10 + 4j computed, 11 + 4j its stage issued by the loader.
-constexpr int CW_TRACE_CHUNKS = 14;
+// last chunk landed / advantages ready / computed, 6 end (partial sums stored), 7 the number of chunks (low 32 bits) and
+// the SM the CTA ran on (high 32 bits).  Chunk j < CW_TRACE_CHUNKS: 8 + 4j landed, 9 + 4j advantages ready, 10 + 4j
+// computed, 11 + 4j its stage issued by the loader.  Slot 60: chunk 0 landed as the loader sees it (32-column tiles; in
+// a deferred launch that can be before the consumers' wait).
+constexpr int CW_TRACE_CHUNKS = 13;
 #define CW_TRACE(slot)                                                                                   \
     do {                                                                                                 \
         if (f.trace) reinterpret_cast<unsigned long long*>(ws + 65536)[blockIdx.x * 64 + (slot)] = gtimer(); \
@@ -89,9 +99,6 @@ template <int NC, bool GRADS, int TC>
 __global__ void __launch_bounds__(CW_THREADS, CwGeo<TC>::CTAS_PER_SM) gae_ppo_ws_kernel(FusedArgs f, float* ws, int n_stages) {
     constexpr int CW_R = CwGeo<TC>::R, CW_MAX_STAGES = CwGeo<TC>::MAX_STAGES, PR = CwGeo<TC>::PR;
     constexpr int RAWS = CwGeo<TC>::RAW_SLOTS;
-    // PDL: the next kernel may start launching right away; the wait for the previous kernels' results comes after the
-    // barrier set-up below (nothing before it touches global memory except the optional trace stamp)
-    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     extern __shared__ __align__(128) unsigned char smem[];
     const PpoArgs& a = f.p;
     const int N = NC ? NC : a.N;
@@ -135,9 +142,17 @@ __global__ void __launch_bounds__(CW_THREADS, CwGeo<TC>::CTAS_PER_SM) gae_ppo_ws
         }
         mbar_fence_init();
     }
-    asm volatile("griddepcontrol.wait;" ::: "memory");
+    // PDL.  The wait for the previous launches' results comes after the barrier set-up (nothing before it touches global
+    // memory except the optional trace stamp), and the next launch may start only after it: so when a later column kernel
+    // starts, everything enqueued before this one has completed.  Deferred (f.defer_wait, common.cuh): only the warps that
+    // write wait -- the loader streams the chunks in while the previous step's finalize and check launches finish.
+    auto dep_wait = [] {
+        asm volatile("griddepcontrol.wait;" ::: "memory");
+        asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    };
+    if (!f.defer_wait) dep_wait();
     __syncthreads();
-    if (tid == 0) CW_TRACE(1);
+    if (tid == 0 && !f.defer_wait) CW_TRACE(1);
     // data-parallel training: consumer warp k of the first CTA consumes the loss scalar k of two steps ago from its mailbox and
     // publishes the previous step's (staged by its finalize launch) to the peers -- while it would otherwise just wait for its
     // first chunk; the NVLink acknowledgements return while this kernel streams (common.cuh)
@@ -186,6 +201,7 @@ __global__ void __launch_bounds__(CW_THREADS, CwGeo<TC>::CTAS_PER_SM) gae_ppo_ws
             if (TC == 32 && j >= CW_AHEAD) {  // chunk j - CW_AHEAD has landed
                 const int jb = j - CW_AHEAD;
                 mbar_wait(&full[jb % S], (uint32_t)((jb / S) & 1));
+                if (jb == 0 && lane == 0) CW_TRACE(60);
             }
             const long long c0 = it.tile * TC;
             const long long t0 = T - (it.q + 1) * CW_R;
@@ -264,6 +280,10 @@ __global__ void __launch_bounds__(CW_THREADS, CwGeo<TC>::CTAS_PER_SM) gae_ppo_ws
                 item_next(pf);
             }
             cpa_commit();
+        }
+        if (f.defer_wait) {  // before the first store (the in-place next_value mask, the advantages)
+            dep_wait();
+            if (lane == 0) CW_TRACE(1);
         }
         float carry = 0.f;
         int s = 0, ph = 0;
@@ -362,6 +382,7 @@ __global__ void __launch_bounds__(CW_THREADS, CwGeo<TC>::CTAS_PER_SM) gae_ppo_ws
         cpa_wait<0>();
     } else {
         // =============================================== consumers ========================================================
+        if (f.defer_wait) dep_wait();  // before the upstream-gradient record and every gradient store
         float g[4] = {0.f, 0.f, 0.f, 0.f};
         if (GRADS) upstream<4>(a.rec, false, ppo_owned(a), g);  // a forward launch: records `used`, never skips
         const PpoUpstream up{g[0], g[1], g[2], g[3], 1.f / (float)a.S};
@@ -373,7 +394,7 @@ __global__ void __launch_bounds__(CW_THREADS, CwGeo<TC>::CTAS_PER_SM) gae_ppo_ws
                 const unsigned long long now = gtimer();
                 tr[3 + k] = now;
                 if (j < CW_TRACE_CHUNKS) tr[8 + 4 * j + k] = now;
-                if (k == 2) tr[7] = (unsigned long long)(j + 1);
+                if (k == 2) tr[7] = (unsigned long long)smid() << 32 | (unsigned long long)(j + 1);
             }
         };
         const int jj = tid / TC, c = tid % TC;
@@ -459,9 +480,44 @@ bool colws_ok(const FusedArgs& f) {
            cw_stages<16>(f) >= 2;
 }
 
-template <int NC, bool GRADS, int TC>
-static int launch_ws(const FusedArgs& f, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
+// the bytes a deferred launch reads before its dependency wait: the loader's and the scanner's inputs
+static int cw_early_reads(const FusedArgs& f, ByteSpan* r) {
     const PpoArgs& a = f.p;
+    const long long S = a.S, L = S * a.N * 4, F = S * 4;
+    const ByteSpan s[] = {byte_span(a.logit_new, L), byte_span(a.logit_old, L), byte_span(a.logit_pre, L),
+                          byte_span(a.action, S * 8),   byte_span(a.value_new, F), byte_span(a.value_old, F),
+                          byte_span(a.ret, F),          byte_span(a.weight, F),    byte_span(f.value, F),
+                          byte_span(f.next_value, F),   byte_span(f.reward, F),    byte_span(f.done, F),
+                          byte_span(f.traj, F)};
+    for (const ByteSpan& x : s) *r++ = x;
+    return (int)(sizeof(s) / sizeof(s[0]));
+}
+
+// the bytes the column kernel and its finalize launch may write
+static int cw_writes(const FusedArgs& f, float* out, float* ws, size_t ws_bytes, ByteSpan* w) {
+    const PpoArgs& a = f.p;
+    const long long S = a.S, F = S * 4;
+    const ByteSpan s[] = {byte_span(a.adv_out, F),
+                          byte_span(a.grad_logit, S * a.N * 4),
+                          byte_span(a.grad_value, F),
+                          byte_span(f.mask_inplace ? f.next_value : nullptr, F),
+                          byte_span(a.rec.used, 4 * sizeof(float)),
+                          byte_span(ws, (long long)ws_bytes),
+                          byte_span(out, 8 * sizeof(float)),
+                          byte_span(f.x_seq, 24 * sizeof(unsigned int)),
+                          byte_span(f.x_out_mean, 16 * sizeof(float))};
+    for (const ByteSpan& x : s) *w++ = x;
+    return (int)(sizeof(s) / sizeof(s[0]));
+}
+
+template <int NC, bool GRADS, int TC>
+static int launch_ws(const FusedArgs& f_in, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
+    FusedArgs f = f_in;
+    const PpoArgs& a = f.p;
+    // captured straight behind the previous step's launches and reading nothing they write: defer the wait (common.cuh)
+    const ChainPoint at = capture_now(st);
+    ByteSpan span[16];
+    f.defer_wait = !f.x_mailboxes && chain_may_defer(st, at, span, cw_early_reads(f, span));
     const int stages = cw_stages<TC>(f);
     const size_t smem = cw_smem<TC>(a.N, a.logit_pre != nullptr, a.weight != nullptr, stages);
     constexpr auto kern = gae_ppo_ws_kernel<NC, GRADS, TC>;
@@ -478,7 +534,9 @@ static int launch_ws(const FusedArgs& f, float* out, float* ws, size_t ws_bytes,
     // data-parallel training: the finalising threads stage the six scalars for the next step's kernel to publish (common.cuh)
     fa.x.mailboxes = f.x_mailboxes; fa.x.state = f.x_seq; fa.x.out_mean = f.x_out_mean; fa.x.rank = f.x_rank;
     fa.x.world = f.x_world;
-    return launch_finalize(ws, out, fa, st);
+    if (int rc = launch_finalize(ws, out, fa, st)) return rc;
+    chain_report(st, at, true, span, cw_writes(f, out, ws, ws_bytes, span));
+    return B200RL_OK;
 }
 
 // SM count of the current device (cached per device)

@@ -52,6 +52,12 @@ __device__ __forceinline__ unsigned long long gtimer() {
     return t;
 }
 
+__device__ __forceinline__ unsigned int smid() {
+    unsigned int r;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(r));
+    return r;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -756,6 +762,37 @@ static inline int with_nc(int n, F&& f) {
         default: return f(std::integral_constant<int, 0>{});
     }
 }
+
+// ---------------------------------------------------------------------------------------------------------------
+// Overlap of consecutive captured learner steps (colws.cu).  The column kernel of step q+1 may start streaming its inputs
+// before step q's column kernel, finalize and check launches have completed -- its loads then run while HBM would otherwise
+// sit idle between the steps -- when that cannot change a result: it is captured into a CUDA graph straight behind the
+// last launch this library captured on the stream (no foreign node in between), PDL is on, and none of the bytes it reads
+// before its griddepcontrol.wait is written by a launch of that chain since the previous column kernel.  Earlier work has
+// completed by then: the column kernel lets its dependents launch only after its own wait.  The record of the chain is
+// kept per (device, stream) in api.cu; a launch that does not report to it breaks the chain (its node is not the chain's).
+// ---------------------------------------------------------------------------------------------------------------
+struct ByteSpan {
+    uintptr_t lo, hi;  // [lo, hi); empty when lo == hi
+};
+static inline ByteSpan byte_span(const void* p, long long bytes) {
+    const uintptr_t lo = reinterpret_cast<uintptr_t>(p);
+    return (p && bytes > 0) ? ByteSpan{lo, lo + (uintptr_t)bytes} : ByteSpan{0, 0};
+}
+
+// Capture state of a stream just before a launch of the chain (capture_now), kept to report the launch afterwards.
+struct ChainPoint {
+    int dev;
+    bool capturing;
+    unsigned long long id;  // capture sequence
+    void* dep;              // the capture's only current dependency (null: none or several)
+};
+ChainPoint capture_now(cudaStream_t st);
+// column kernel: may it defer its dependency wait?  `reads` are the bytes it reads before the wait
+bool chain_may_defer(cudaStream_t st, const ChainPoint& at, const ByteSpan* reads, int n_reads);
+// after a launch of the chain made at `at`: a column kernel (with its finalize) starts a new chain, a check extends the one
+// it follows; `writes` are the bytes the launches may write
+void chain_report(cudaStream_t st, const ChainPoint& at, bool starts, const ByteSpan* writes, int n_writes);
 
 // per-CTA partial sums live in workspace words [WS_CTRL_WORDS, WS_PARTIAL_LIMIT_WORDS): above them sit the packed accumulators of
 // grid_sum_fx and the scheduling counters of fused.cu, which must stay zero between launches

@@ -15,6 +15,7 @@ struct FusedArgs {
     long long T, B;
     float gamma, gl;
     int mask_inplace;
+    int defer_wait;  // colws.cu: only the writing warps wait for the previous launches (captured steps, common.cuh)
     int trace;  // colws.cu: per-CTA %globaltimer stamps in the workspace (B200RL_FUSED_TRACE=1; tools/trace_col.py)
     // optional data-parallel exchange of the six loss scalars, fused into the step's finalize launch (colws.cu; common.cuh)
     const unsigned long long* x_mailboxes;

@@ -441,7 +441,15 @@ extern "C" int b200rl_ppo_bwd(const float* logit_new, const float* logit_old, co
     if (S == 0) return B200RL_OK;
     cudaStream_t st = (cudaStream_t)stream;
     constexpr int NT = 128;
-    if (tile_path_ok(a)) return dispatch_tile<PPO_BWD>(a, nullptr, nullptr, 0, st);
+    if (tile_path_ok(a)) {
+        // the check of a learner step: it extends the step chain it follows (common.cuh) by what it may write
+        const ChainPoint at = capture_now(st);
+        if (int rc = dispatch_tile<PPO_BWD>(a, nullptr, nullptr, 0, st)) return rc;
+        const ByteSpan w[] = {byte_span(grad_logit_new, S * G * N * 4), byte_span(grad_value_new, S * 4),
+                              byte_span(g_hint, 4 * sizeof(float))};
+        chain_report(st, at, false, w, 3);
+        return B200RL_OK;
+    }
     if (g_used) return B200RL_ERR_ARG;  // the fused forward only exists on the tile path
     long long grid = a.N > 64 ? div_up(S, NT / 32) : div_up(S, NT);
     if (grid > NUM_SMS * 32) grid = NUM_SMS * 32;  // grid-stride kernels

@@ -6,7 +6,10 @@ bench.py does, then reads the stamps of the last replay and prints, as median / 
   chunk   time per chunk in the middle: (last landed - first landed) / (chunks - 1)
   tail    last chunk landed -> CTA end (partial sums stored)
 and the step boundary: one set's kernel end (latest CTA) -> the next set's kernel start and its griddepcontrol.wait
-(finalize_sums and the check launch sit between them).  --json prints one JSON line instead of the table.
+(finalize_sums and the check launch sit between them).  Per SM (median over the SMs that run a CTA of both steps), the
+next step's CTA start, wait returned and first chunk landed relative to the end of the previous step's CTA on that SM,
+and the share of SMs on which the next step's CTA started before the previous one ended.  --json prints one JSON line
+instead of the table.
 """
 import json
 import os
@@ -55,7 +58,7 @@ tr = trs[0].astype(np.float64)
 grid = tr.shape[0]
 t0 = tr[:, 0].min()
 us = lambda a: (a - t0) / 1e3  # noqa: E731
-nch = trs[0][:, 7].astype(np.int64)
+nch = (trs[0][:, 7] & 0xffffffff).astype(np.int64)
 first_landed = us(tr[:, 8])
 last_landed = us(tr[:, 3])
 end = us(tr[:, 6])
@@ -73,7 +76,7 @@ res = {
 }
 # per chunk j (as stamped): landed, advantages ready, computed, issued by the loader
 per = {}
-for j in range(14):
+for j in range(13):
     c = tr[:, 8 + 4 * j]
     if (c > 0).sum() == 0:
         break
@@ -87,6 +90,22 @@ res['boundary_end_to_next_wait_done'] = [round(float((b[:, 1].min() - a[:, 6].ma
                                          for a, b in zip(trs[:-1], trs[1:])]
 res['step_wait_done_to_wait_done'] = [round(float((b[:, 1].min() - a[:, 1].min()) / 1e3), 3)
                                       for a, b in zip(trs[:-1], trs[1:])]
+
+
+def per_sm(a, b):
+    """step a -> step b on each SM that ran a CTA of both: b's start / wait returned / first landed minus a's CTA end (us)"""
+    end = {int(r[7]) >> 32: r[6] for r in a}
+    rows = [(r[0] - end[s], r[1] - end[s], r[8] - end[s]) for r in b if (s := int(r[7]) >> 32) in end]
+    d = np.asarray(rows, dtype=np.float64) / 1e3
+    return {'sms': len(rows), 'start': round(float(np.median(d[:, 0])), 3), 'wait_done': round(float(np.median(d[:, 1])), 3),
+            'first_landed': round(float(np.median(d[:, 2])), 3),
+            'started_before_end': round(float((d[:, 0] < 0).mean()), 3)}
+
+
+res['per_sm_next_vs_prev_end'] = [per_sm(a, b) for a, b in zip(trs[:-1], trs[1:])]
+# the next step's first chunk as its loader saw it land, against its own griddepcontrol.wait returning (negative: it
+# landed before the previous step's finalize and check launches had completed)
+res['next_first_landed_minus_wait_done'] = [round(float(np.median((b[:, 60] - b[:, 1]) / 1e3)), 3) for b in trs[1:]]
 if '--json' in sys.argv:
     print(json.dumps(res))
 else:
