@@ -6,6 +6,7 @@ Nothing here computes on the CPU.  Host (CPU) tensors are accepted by the public
 to the current CUDA device and returning results on the host -- the "host buffers" end-to-end path.
 """
 import os
+import threading
 
 import torch
 
@@ -25,7 +26,8 @@ def require_cuda():
             "di_engine_b200 needs a CUDA device (sm_90a). There is no CPU implementation of the operators; "
             "the CPU oracle under oracle/ is test infrastructure only."
         )
-    lib()
+    if not torch.compiler.is_compiling():  # a traced call loads the library when its custom ops run
+        lib()
 
 
 def stream_ptr():
@@ -58,6 +60,38 @@ def on_device(device):
     return torch.cuda.device(device)
 
 
+def lasting(make, device):
+    """``make()``, for a buffer kept for the life of the process (the workspace, the upstream-gradient records, cached
+    constants).  CUDA graphs must not own such a buffer: torch.compile's ``mode="reduce-overhead"`` sends every allocation
+    of its warm-up run to the graphs' private memory pool, whose blocks it hands out again to later graphs.  So the buffer is
+    made on a helper thread, whose allocations go to the ordinary pool, and synchronised before it is used.  Inside a stream
+    capture nothing may be allocated or synchronised, so a first use there is an error."""
+    if device.type != 'cuda':
+        return make()
+    if torch.cuda.is_current_stream_capturing():
+        raise _lib.B200RLError(
+            "di_engine_b200: a workspace or upstream-gradient record is first needed inside a CUDA graph capture. Run the "
+            "step once on the capturing stream before capturing it (torch.compile's mode='reduce-overhead' does so in its "
+            "warm-up call; with torch.cuda.graph, run one eager step on the capture stream first)."
+        )
+    made = []
+
+    def run():
+        try:
+            with torch.cuda.device(device):
+                made.append(make())
+                torch.cuda.current_stream().synchronize()
+        except BaseException as e:  # re-raised on the calling thread
+            made.append(e)
+
+    t = threading.Thread(target=run)
+    t.start()
+    t.join()
+    if isinstance(made[0], BaseException):
+        raise made[0]
+    return made[0]
+
+
 def workspace(device):
     """One zero-initialised scratch buffer per (device, stream): launches sharing it are stream-ordered."""
     idx = device.index
@@ -67,7 +101,7 @@ def workspace(device):
     ws = _WS.get(key)
     if ws is None:
         nbytes = lib().b200rl_workspace_bytes()
-        ws = torch.zeros(nbytes // 4, dtype=torch.float32, device=device)
+        ws = lasting(lambda: torch.zeros(nbytes // 4, dtype=torch.float32, device=device), device)
         _WS[key] = ws
     return ws
 
@@ -125,7 +159,7 @@ def const_scalar(value, device):
     key = (float(value), device.index)
     t = _CONST.get(key)
     if t is None:
-        t = torch.full((1, ), float(value), dtype=torch.float32, device=device)
+        t = lasting(lambda: torch.full((1, ), float(value), dtype=torch.float32, device=device), device)
         _CONST[key] = t
     return t
 
@@ -161,7 +195,7 @@ def head_hint(device, kind, init):
     key = (device.index, kind)
     h = _HINT.get(key)
     if h is None:
-        h = torch.tensor(init, dtype=torch.float32, device=device)
+        h = lasting(lambda: torch.tensor(init, dtype=torch.float32, device=device), device)
         _HINT[key] = h
     return h
 
@@ -327,6 +361,59 @@ class ValueMapFunction(torch.autograd.Function):
 PPO_FUSED_BACKWARD = True
 
 
+def ppo_fwd_(logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre, S, G, N, clip_ratio,
+             use_value_clip, dual_clip, kl_type, hint_kind, adv_stats, factor, want_grad):
+    """The forward launch of ppo_error (PPOFunction and the ``b200rl::ppo_loss`` custom op).  -> (the 8-float result vector,
+    the forward-written (grad_logit, grad_value, g_used) or None when this launch wrote no gradients)."""
+    dev = logit_new.device
+    out = torch.empty(8, dtype=torch.float32, device=dev)
+    L = lib()
+    tensors = (ptr(logit_new), ptr(logit_old), ptr(logit_pre), ptr(action), ptr(value_new), ptr(value_old),
+               ptr(adv), ptr(return_), ptr(weight))
+    cfg = (S, G, N, clip_ratio, use_value_clip, dual_clip, kl_type, ptr(adv_stats), ptr(factor))
+    spec = None
+    with on_device(dev):
+        ws = workspace(dev)
+        if PPO_FUSED_BACKWARD and want_grad:
+            grad_logit = torch.empty_like(logit_new)
+            grad_value = torch.empty_like(value_new)
+            if L.b200rl_ppo_fused_supported(*tensors, ptr(grad_logit), G, N):
+                g_used = torch.empty(4, dtype=torch.float32, device=dev)
+                rc = L.b200rl_ppo_fwd_grad(*tensors, *cfg, ptr(ppo_hint(dev, hint_kind)), ptr(g_used), ptr(out),
+                                           ptr(grad_logit), ptr(grad_value), ptr(ws), ws.numel() * 4,
+                                           stream_ptr())
+                _lib.check(rc, 'b200rl_ppo_fwd_grad')
+                spec = (grad_logit, grad_value, g_used)
+        if spec is None:
+            rc = L.b200rl_ppo_fwd(*tensors, *cfg, ptr(out), ptr(ws), ws.numel() * 4, stream_ptr())
+            _lib.check(rc, 'b200rl_ppo_fwd')
+    return out, spec
+
+
+def ppo_bwd_(saved, cfg, upstream, spec, hint_kind):
+    """The backward launch of ppo_error: ``saved`` the nine tensors of ppo_fwd_'s launch, ``cfg`` its (S, G, N, clip_ratio,
+    use_value_clip, dual_clip, kl_type, adv_stats ptr, factor ptr), ``upstream`` the four device pointers of the upstream
+    gradients (None = 0).  With ``spec`` (the forward-written gradients) it verifies them on the device and recomputes them
+    in place on a mismatch; without, it computes into fresh buffers.  -> (grad_logit, grad_value)."""
+    logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre = saved
+    dev = logit_new.device
+    if spec is not None:  # valid if the expectation held; the kernel checks on the device
+        grad_logit, grad_value, g_used = spec
+        p_used, p_hint = ptr(g_used), ptr(ppo_hint(dev, hint_kind))
+    else:  # no fused forward, or a repeated backward: null g_used / hint -> the kernel recomputes
+        grad_logit = torch.empty_like(logit_new)
+        grad_value = torch.empty_like(value_new)
+        p_used, p_hint = None, None
+    with on_device(dev):
+        rc = lib().b200rl_ppo_bwd(
+            ptr(logit_new), ptr(logit_old), ptr(logit_pre), ptr(action), ptr(value_new), ptr(value_old), ptr(adv),
+            ptr(return_), ptr(weight), *cfg, *upstream, p_used, p_hint, ptr(grad_logit), ptr(grad_value),
+            stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_ppo_bwd')
+    return grad_logit, grad_value
+
+
 class PPOFunction(torch.autograd.Function):
     """Outputs: policy_loss, value_loss, entropy_loss, kl_div (differentiable 0-dim) and the raw 8-float result vector
     (non differentiable; [4]=approx_kl, [5]=clipfrac)."""
@@ -334,58 +421,22 @@ class PPOFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre, S, G, N,
                 clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, adv_stats=None, factor=None):
-        dev = logit_new.device
         ctx.hint_kind = hint_kind
         ctx.adv_stats = adv_stats  # {mean, std + 1e-8} device floats or None; kept alive for the backward launch
         ctx.factor = factor        # happo_error's per-sample factor (S,) or None; likewise
-        out = torch.empty(8, dtype=torch.float32, device=dev)
-        L = lib()
-        tensors = (ptr(logit_new), ptr(logit_old), ptr(logit_pre), ptr(action), ptr(value_new), ptr(value_old),
-                   ptr(adv), ptr(return_), ptr(weight))
-        cfg = (S, G, N, clip_ratio, use_value_clip, dual_clip, kl_type, ptr(adv_stats), ptr(factor))
-        ctx.spec = None
-        want_grad = PPO_FUSED_BACKWARD and (ctx.needs_input_grad[0] or ctx.needs_input_grad[1])
-        with on_device(dev):
-            ws = workspace(dev)
-            if want_grad:
-                grad_logit = torch.empty_like(logit_new)
-                grad_value = torch.empty_like(value_new)
-                if L.b200rl_ppo_fused_supported(*tensors, ptr(grad_logit), G, N):
-                    g_used = torch.empty(4, dtype=torch.float32, device=dev)
-                    rc = L.b200rl_ppo_fwd_grad(*tensors, *cfg, ptr(ppo_hint(dev, hint_kind)), ptr(g_used), ptr(out),
-                                               ptr(grad_logit), ptr(grad_value), ptr(ws), ws.numel() * 4,
-                                               stream_ptr())
-                    _lib.check(rc, 'b200rl_ppo_fwd_grad')
-                    ctx.spec = (grad_logit, grad_value, g_used)
-            if ctx.spec is None:
-                rc = L.b200rl_ppo_fwd(*tensors, *cfg, ptr(out), ptr(ws), ws.numel() * 4, stream_ptr())
-                _lib.check(rc, 'b200rl_ppo_fwd')
+        out, ctx.spec = ppo_fwd_(logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre, S,
+                                 G, N, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, adv_stats, factor,
+                                 ctx.needs_input_grad[0] or ctx.needs_input_grad[1])
         ctx.save_for_backward(logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre)
-        ctx.cfg = cfg
+        ctx.cfg = (S, G, N, clip_ratio, use_value_clip, dual_clip, kl_type, ptr(adv_stats), ptr(factor))
         ctx.mark_non_differentiable(out)
         p, v, e, k = out[0], out[1], out[2], out[3]
         return p, v, e, k, out
 
     @staticmethod
     def backward(ctx, g_p, g_v, g_e, g_k, _g_out):
-        logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre = ctx.saved_tensors
-        dev = logit_new.device
-        keep, (pp, pv, pe, pk) = _grads(g_p, g_v, g_e, g_k)
-        spec = _forward_grads(ctx)
-        if spec is not None:  # valid if the expectation held; the kernel checks on the device
-            grad_logit, grad_value, g_used = spec
-            p_used, p_hint = ptr(g_used), ptr(ppo_hint(dev, ctx.hint_kind))
-        else:  # no fused forward, or a repeated backward: null g_used / hint -> the kernel recomputes
-            grad_logit = torch.empty_like(logit_new)
-            grad_value = torch.empty_like(value_new)
-            p_used, p_hint = None, None
-        with on_device(dev):
-            rc = lib().b200rl_ppo_bwd(
-                ptr(logit_new), ptr(logit_old), ptr(logit_pre), ptr(action), ptr(value_new), ptr(value_old), ptr(adv),
-                ptr(return_), ptr(weight), *ctx.cfg, pp, pv, pe, pk, p_used, p_hint, ptr(grad_logit), ptr(grad_value),
-                stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_ppo_bwd')
+        keep, upstream = _grads(g_p, g_v, g_e, g_k)
+        grad_logit, grad_value = ppo_bwd_(ctx.saved_tensors, ctx.cfg, upstream, _forward_grads(ctx), ctx.hint_kind)
         return (grad_logit, grad_value) + (None, ) * 17
 
 
@@ -477,22 +528,10 @@ class QNStepTDFunction(torch.autograd.Function):
                 N, nstep, gamma, cum_reward, rescale, eps, criterion, crit_param, group_mean, seq_len, priority_mix,
                 want_priority):
         dev = q.device
-        R = S * G
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        td = torch.empty(S if group_mean else R, dtype=torch.float32, device=dev)
-        dcrit = torch.empty(R, dtype=torch.float32, device=dev)
-        target = torch.empty(R, dtype=torch.float32, device=dev)
-        prio = torch.empty(S // seq_len, dtype=torch.float32, device=dev) if want_priority else None
-        grad_unit = torch.empty(R, N, dtype=torch.float32, device=dev) if ctx.needs_input_grad[0] else None
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_qntd_fwd(
-                ptr(q), ptr(next_n_q), ptr(action), ptr(next_n_action), ptr(reward), ptr(done), ptr(weight),
-                ptr(value_gamma), vg_stride, ptr(gamma_ps), S, G, N, nstep, gamma, cum_reward, rescale, eps, criterion,
-                crit_param, group_mean, seq_len, priority_mix, ptr(loss), ptr(td), ptr(dcrit), ptr(target),
-                ptr(grad_unit), ptr(prio), ptr(ws), ws.numel() * 4, stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_qntd_fwd')
+        loss, td, dcrit, target, prio, grad_unit = qntd_fwd_(
+            q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, vg_stride, gamma_ps, S, G, N, nstep,
+            gamma, cum_reward, rescale, eps, criterion, crit_param, group_mean, seq_len, priority_mix, want_priority,
+            ctx.needs_input_grad[0])
         ctx.save_for_backward(dcrit, action, weight)
         ctx.cfg = (S, G, N, group_mean, seq_len)
         ctx.q_shape = q.shape
@@ -511,11 +550,43 @@ class QNStepTDFunction(torch.autograd.Function):
         S, G, N, group_mean, seq_len = ctx.cfg
         keep, (pg, ptd) = _grads(g_loss, g_td)
         grad_q, skip = _unit_grad(ctx, (g_td, ), lambda: torch.empty(S * G, N, dtype=torch.float32, device=dcrit.device))
-        with on_device(dcrit.device):
-            rc = lib().b200rl_qntd_bwd(ptr(dcrit), ptr(weight), ptr(action), pg, ptd, S, G, N, group_mean, seq_len, skip,
-                                       ptr(grad_q), stream_ptr())
-        _lib.check(rc, 'b200rl_qntd_bwd')
+        qntd_bwd_(dcrit, weight, action, pg, ptd, S, G, N, group_mean, seq_len, skip, grad_q)
         return (grad_q.view(ctx.q_shape), ) + (None, ) * 23
+
+
+def qntd_fwd_(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, vg_stride, gamma_ps, S, G, N, nstep,
+              gamma, cum_reward, rescale, eps, criterion, crit_param, group_mean, seq_len, priority_mix, want_priority,
+              want_grad):
+    """The forward launch of the q-n-step TD family (QNStepTDFunction and the ``b200rl::qntd_fwd`` custom op).
+    -> (loss, td, dcrit, target, prio or None, grad_unit or None)."""
+    dev = q.device
+    R = S * G
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    td = torch.empty(S if group_mean else R, dtype=torch.float32, device=dev)
+    dcrit = torch.empty(R, dtype=torch.float32, device=dev)
+    target = torch.empty(R, dtype=torch.float32, device=dev)
+    prio = torch.empty(S // seq_len, dtype=torch.float32, device=dev) if want_priority else None
+    grad_unit = torch.empty(R, N, dtype=torch.float32, device=dev) if want_grad else None
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_qntd_fwd(
+            ptr(q), ptr(next_n_q), ptr(action), ptr(next_n_action), ptr(reward), ptr(done), ptr(weight),
+            ptr(value_gamma), vg_stride, ptr(gamma_ps), S, G, N, nstep, gamma, cum_reward, rescale, eps, criterion,
+            crit_param, group_mean, seq_len, priority_mix, ptr(loss), ptr(td), ptr(dcrit), ptr(target),
+            ptr(grad_unit), ptr(prio), ptr(ws), ws.numel() * 4, stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_qntd_fwd')
+    return loss, td, dcrit, target, prio, grad_unit
+
+
+def qntd_bwd_(dcrit, weight, action, pg, ptd, S, G, N, group_mean, seq_len, skip, grad_q):
+    """The backward launch of the q-n-step TD family into ``grad_q``: ``pg`` / ``ptd`` the device pointers of the upstream
+    gradients (None = 0); ``skip`` 1 when ``grad_q`` holds the forward-written unit gradient (verified on the device)."""
+    with on_device(dcrit.device):
+        rc = lib().b200rl_qntd_bwd(ptr(dcrit), ptr(weight), ptr(action), pg, ptd, S, G, N, group_mean, seq_len, skip,
+                                   ptr(grad_q), stream_ptr())
+    _lib.check(rc, 'b200rl_qntd_bwd')
+    return grad_q
 
 
 class DQfDTDFunction(torch.autograd.Function):
@@ -793,22 +864,11 @@ class DistNStepTDFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, dist, next_n_dist, act, next_n_act, reward, done, weight, w_stride, value_gamma, vg_stride,
                 support, B, A, N, n_atom, nstep, gamma, v_min, v_max, bad_flag):
-        dev = dist.device
-        R = B * A
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        td = torch.empty(R, dtype=torch.float32, device=dev)
-        proj = torch.empty(R, n_atom, dtype=torch.float32, device=dev)
-        grad_unit = torch.empty_like(dist) if ctx.needs_input_grad[0] else None
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_dntd_fwd(
-                ptr(dist), ptr(next_n_dist), ptr(act), ptr(next_n_act), ptr(reward), ptr(done), ptr(weight), w_stride,
-                ptr(value_gamma), vg_stride, ptr(support), B, A, N, n_atom, nstep, gamma, v_min, v_max, ptr(loss),
-                ptr(td), ptr(proj), ptr(bad_flag), ptr(grad_unit), ptr(ws), ws.numel() * 4, stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_dntd_fwd')
+        loss, td, proj, grad_unit = dntd_fwd_(dist, next_n_dist, act, next_n_act, reward, done, weight, w_stride,
+                                              value_gamma, vg_stride, support, B, A, N, n_atom, nstep, gamma, v_min,
+                                              v_max, bad_flag, ctx.needs_input_grad[0])
         ctx.save_for_backward(dist, act, proj, weight)
-        ctx.cfg = (R, N, n_atom, w_stride)
+        ctx.cfg = (B * A, N, n_atom, w_stride)
         ctx.spec = grad_unit
         ctx.set_materialize_grads(False)
         return loss, td
@@ -821,13 +881,40 @@ class DistNStepTDFunction(torch.autograd.Function):
         R, N, n_atom, w_stride = ctx.cfg
         keep, (pg, ptd) = _grads(g_loss, g_td)
         grad, skip = _unit_grad(ctx, (g_td, ), lambda: torch.empty_like(dist))
-        with on_device(dist.device):
-            rc = lib().b200rl_dntd_bwd(
-                ptr(dist), ptr(act), ptr(proj), ptr(weight), w_stride, pg, ptd, R, N, n_atom, skip, ptr(grad),
-                stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_dntd_bwd')
+        dntd_bwd_(dist, act, proj, weight, w_stride, pg, ptd, R, N, n_atom, skip, grad)
         return (grad, ) + (None, ) * 19
+
+
+def dntd_fwd_(dist, next_n_dist, act, next_n_act, reward, done, weight, w_stride, value_gamma, vg_stride, support, B, A, N,
+              n_atom, nstep, gamma, v_min, v_max, bad_flag, want_grad):
+    """The forward launch of dist_nstep_td_error (DistNStepTDFunction and the ``b200rl::dntd_fwd`` custom op).
+    -> (loss, td, proj, grad_unit or None)."""
+    dev = dist.device
+    R = B * A
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    td = torch.empty(R, dtype=torch.float32, device=dev)
+    proj = torch.empty(R, n_atom, dtype=torch.float32, device=dev)
+    grad_unit = torch.empty_like(dist) if want_grad else None
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_dntd_fwd(
+            ptr(dist), ptr(next_n_dist), ptr(act), ptr(next_n_act), ptr(reward), ptr(done), ptr(weight), w_stride,
+            ptr(value_gamma), vg_stride, ptr(support), B, A, N, n_atom, nstep, gamma, v_min, v_max, ptr(loss),
+            ptr(td), ptr(proj), ptr(bad_flag), ptr(grad_unit), ptr(ws), ws.numel() * 4, stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_dntd_fwd')
+    return loss, td, proj, grad_unit
+
+
+def dntd_bwd_(dist, act, proj, weight, w_stride, pg, ptd, R, N, n_atom, skip, grad):
+    """The backward launch of dist_nstep_td_error into ``grad`` (arguments as qntd_bwd_)."""
+    with on_device(dist.device):
+        rc = lib().b200rl_dntd_bwd(
+            ptr(dist), ptr(act), ptr(proj), ptr(weight), w_stride, pg, ptd, R, N, n_atom, skip, ptr(grad),
+            stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_dntd_bwd')
+    return grad
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -914,15 +1001,21 @@ class _ScaleSaved(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         saved, = ctx.saved_tensors
-        out = torch.empty_like(saved)
         keep, (pg, ) = _grads(g)
-        with on_device(saved.device):
-            rc = lib().b200rl_scale(pg, ptr(saved), ptr(out), saved.numel(), stream_ptr())
-        _lib.check(rc, 'b200rl_scale')
-        return out, None, None
+        return scale_(pg, saved), None, None
 
 
-def td_lambda_(value, reward, weight, gamma, lambda_):
+def scale_(pg, saved):
+    """``*pg * saved`` into a fresh tensor: the backward launch of the heads whose forward saved the unit gradient."""
+    out = torch.empty_like(saved)
+    with on_device(saved.device):
+        rc = lib().b200rl_scale(pg, ptr(saved), ptr(out), saved.numel(), stream_ptr())
+    _lib.check(rc, 'b200rl_scale')
+    return out
+
+
+def td_lambda_fwd_(value, reward, weight, gamma, lambda_):
+    """The one launch of td_lambda_error -> (loss, d loss / d value for a unit upstream gradient)."""
     T, B = reward.shape
     dev = value.device
     loss = torch.empty((), dtype=torch.float32, device=dev)
@@ -934,6 +1027,11 @@ def td_lambda_(value, reward, weight, gamma, lambda_):
             ws.numel() * 4, stream_ptr()
         )
     _lib.check(rc, 'b200rl_td_lambda_fwd')
+    return loss, dvalue
+
+
+def td_lambda_(value, reward, weight, gamma, lambda_):
+    loss, dvalue = td_lambda_fwd_(value, reward, weight, gamma, lambda_)
     if value.requires_grad and torch.is_grad_enabled():
         return _ScaleSaved.apply(value, loss, dvalue)
     return loss
@@ -949,17 +1047,7 @@ class UPGOFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, logit, action, mask, rho, ret, value, TB, K, N):
-        dev = logit.device
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        adv = torch.empty(TB, dtype=torch.float32, device=dev)
-        grad_unit = torch.empty_like(logit) if ctx.needs_input_grad[0] else None
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_upgo_head_fwd(
-                ptr(logit), ptr(action), ptr(mask), ptr(rho), ptr(ret), ptr(value), TB, K, N, ptr(loss), ptr(adv),
-                ptr(grad_unit), ptr(ws), ws.numel() * 4, stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_upgo_head_fwd')
+        loss, adv, grad_unit = upgo_fwd_(logit, action, mask, rho, ret, value, TB, K, N, ctx.needs_input_grad[0])
         ctx.save_for_backward(logit, action, mask, adv)
         ctx.cfg = (TB, K, N)
         ctx.spec = grad_unit
@@ -971,12 +1059,34 @@ class UPGOFunction(torch.autograd.Function):
         TB, K, N = ctx.cfg
         grad, skip = _unit_grad(ctx, (), lambda: torch.empty_like(logit))
         keep, (pg, ) = _grads(g)
-        with on_device(logit.device):
-            rc = lib().b200rl_upgo_head_bwd(
-                ptr(logit), ptr(action), ptr(mask), ptr(adv), pg, TB, K, N, skip, ptr(grad), stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_upgo_head_bwd')
-        return (grad, ) + (None, ) * 8
+        return (upgo_bwd_(logit, action, mask, adv, pg, TB, K, N, skip, grad), ) + (None, ) * 8
+
+
+def upgo_fwd_(logit, action, mask, rho, ret, value, TB, K, N, want_grad):
+    """The forward launch of the upgo_loss head (UPGOFunction and the ``b200rl::upgo_fwd`` custom op).
+    -> (loss, adv, grad_unit or None)."""
+    dev = logit.device
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    adv = torch.empty(TB, dtype=torch.float32, device=dev)
+    grad_unit = torch.empty_like(logit) if want_grad else None
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_upgo_head_fwd(
+            ptr(logit), ptr(action), ptr(mask), ptr(rho), ptr(ret), ptr(value), TB, K, N, ptr(loss), ptr(adv),
+            ptr(grad_unit), ptr(ws), ws.numel() * 4, stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_upgo_head_fwd')
+    return loss, adv, grad_unit
+
+
+def upgo_bwd_(logit, action, mask, adv, pg, TB, K, N, skip, grad):
+    """The backward launch of the upgo_loss head into ``grad`` (``pg`` / ``skip`` as qntd_bwd_)."""
+    with on_device(logit.device):
+        rc = lib().b200rl_upgo_head_bwd(
+            ptr(logit), ptr(action), ptr(mask), ptr(adv), pg, TB, K, N, skip, ptr(grad), stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_upgo_head_bwd')
+    return grad
 
 
 class A2CFunction(torch.autograd.Function):
@@ -1156,72 +1266,98 @@ class VTraceFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, target_output, value, behaviour_output, action, reward, weight, gamma, lambda_, rho_clip, c_clip,
                 rho_pg_clip):
-        T, B = reward.shape
-        N = target_output.shape[-1]
-        dev = target_output.device
-        out = torch.empty(4, dtype=torch.float32, device=dev)
-        L = lib()
-        tensors = (ptr(target_output), ptr(behaviour_output), ptr(action), ptr(value), ptr(reward), ptr(weight))
-        want_grad = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
-        ctx.cfg = (T, B, N)
-        ctx.scal = None  # the scalars of the verify launch: set on the one-launch path only
-        with on_device(dev):
-            ws = workspace(dev)
-            if VTRACE_FUSED:
-                grad_logit = torch.empty_like(target_output) if want_grad else None
-                grad_value = torch.empty(T + 1, B, dtype=torch.float32, device=dev) if want_grad else None
-                if L.b200rl_vtrace_fused_supported(*tensors, T, B, N, ptr(grad_logit), ptr(grad_value)):
-                    g_used = torch.empty(3, dtype=torch.float32, device=dev) if want_grad else None
-                    rc = L.b200rl_vtrace_fwd_grad(
-                        *tensors, T, B, N, gamma, lambda_, rho_clip, c_clip, rho_pg_clip,
-                        ptr(vtrace_hint(dev)) if want_grad else None, 0, None, None, None, ptr(g_used), None, ptr(out),
-                        ptr(grad_logit), ptr(grad_value), ptr(ws), ws.numel() * 4, stream_ptr()
-                    )
-                    _lib.check(rc, 'b200rl_vtrace_fwd_grad')
-                    ctx.spec = (grad_logit, grad_value, g_used) if want_grad else None
-                    ctx.scal = (gamma, lambda_, rho_clip, c_clip, rho_pg_clip)
-                    ctx.save_for_backward(target_output, behaviour_output, action, value, reward, weight)
-                    return out[0], out[1], out[2]
-            lp = torch.empty(T, B, dtype=torch.float32, device=dev)
-            cpg = torch.empty(T, B, dtype=torch.float32, device=dev)
-            dv = torch.empty(T, B, dtype=torch.float32, device=dev)
-            rc = L.b200rl_vtrace_fwd(
-                *tensors, T, B, N, gamma, lambda_, rho_clip, c_clip, rho_pg_clip, ptr(out), ptr(lp), ptr(cpg), ptr(dv),
-                ptr(ws), ws.numel() * 4, stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_vtrace_fwd')
-        ctx.save_for_backward(target_output, action, weight, cpg, dv)
+        scal = (gamma, lambda_, rho_clip, c_clip, rho_pg_clip)
+        out, fused, spec, cpg, dv = vtrace_fwd_(target_output, value, behaviour_output, action, reward, weight, scal,
+                                                ctx.needs_input_grad[0] or ctx.needs_input_grad[1])
+        ctx.scal = scal if fused else None  # the scalars of the verify launch: set on the one-launch path only
+        if fused:
+            ctx.spec = spec
+            ctx.save_for_backward(target_output, behaviour_output, action, value, reward, weight)
+        else:
+            ctx.save_for_backward(target_output, action, weight, cpg, dv)
         return out[0], out[1], out[2]
 
     @staticmethod
     def backward(ctx, g_p, g_v, g_e):
-        T, B, N = ctx.cfg
-        keep, (pp, pv, pe) = _grads(g_p, g_v, g_e)
+        keep, upstream = _grads(g_p, g_v, g_e)
         if ctx.scal is not None:
-            target_output, behaviour_output, action, value, reward, weight = ctx.saved_tensors
-            dev = target_output.device
-            grad_logit, grad_value, g_used = _forward_grads(ctx) or (
-                torch.empty_like(target_output), torch.empty(T + 1, B, dtype=torch.float32, device=dev), None)
-            with on_device(dev):
-                ws = workspace(dev)
-                rc = lib().b200rl_vtrace_fwd_grad(
-                    ptr(target_output), ptr(behaviour_output), ptr(action), ptr(value), ptr(reward), ptr(weight), T, B,
-                    N, *ctx.scal, None, 1, pp, pv, pe, ptr(g_used), ptr(vtrace_hint(dev)), None, ptr(grad_logit),
-                    ptr(grad_value), ptr(ws), ws.numel() * 4, stream_ptr()
+            grads = vtrace_verify_(ctx.saved_tensors, ctx.scal, upstream, _forward_grads(ctx))
+        else:
+            target_output, action, weight, cpg, dv = ctx.saved_tensors
+            grads = vtrace_bwd_(target_output, action, weight, cpg, dv, upstream)
+        return grads + (None, ) * 9
+
+
+def vtrace_fwd_(target_output, value, behaviour_output, action, reward, weight, scal, want_grad):
+    """The forward launch of vtrace_error_discrete_action (VTraceFunction and the ``b200rl::vtrace_loss`` custom op); ``scal``
+    = (gamma, lambda_, rho_clip, c_clip, rho_pg_clip).  -> (out, fused, spec, cpg, dv): ``fused`` when the one-launch kernel
+    ran, with ``spec`` its forward-written (grad_logit, grad_value, g_used) when ``want_grad``; otherwise the rows / scan
+    kernels ran and ``cpg`` / ``dv`` are the (T, B) records of their backward."""
+    T, B = reward.shape
+    N = target_output.shape[-1]
+    dev = target_output.device
+    out = torch.empty(4, dtype=torch.float32, device=dev)
+    L = lib()
+    tensors = (ptr(target_output), ptr(behaviour_output), ptr(action), ptr(value), ptr(reward), ptr(weight))
+    with on_device(dev):
+        ws = workspace(dev)
+        if VTRACE_FUSED:
+            grad_logit = torch.empty_like(target_output) if want_grad else None
+            grad_value = torch.empty(T + 1, B, dtype=torch.float32, device=dev) if want_grad else None
+            if L.b200rl_vtrace_fused_supported(*tensors, T, B, N, ptr(grad_logit), ptr(grad_value)):
+                g_used = torch.empty(3, dtype=torch.float32, device=dev) if want_grad else None
+                rc = L.b200rl_vtrace_fwd_grad(
+                    *tensors, T, B, N, *scal, ptr(vtrace_hint(dev)) if want_grad else None, 0, None, None, None,
+                    ptr(g_used), None, ptr(out), ptr(grad_logit), ptr(grad_value), ptr(ws), ws.numel() * 4, stream_ptr()
                 )
-            _lib.check(rc, 'b200rl_vtrace_fwd_grad(verify)')
-            return (grad_logit, grad_value) + (None, ) * 9
-        target_output, action, weight, cpg, dv = ctx.saved_tensors
-        dev = target_output.device
-        grad_logit = torch.empty_like(target_output)
-        grad_value = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
-        with on_device(dev):
-            rc = lib().b200rl_vtrace_bwd(
-                ptr(target_output), ptr(action), ptr(weight), ptr(cpg), ptr(dv), pp, pv, pe, T, B, N, ptr(grad_logit),
-                ptr(grad_value), stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_vtrace_bwd')
-        return (grad_logit, grad_value) + (None, ) * 9
+                _lib.check(rc, 'b200rl_vtrace_fwd_grad')
+                return out, True, (grad_logit, grad_value, g_used) if want_grad else None, None, None
+        lp = torch.empty(T, B, dtype=torch.float32, device=dev)
+        cpg = torch.empty(T, B, dtype=torch.float32, device=dev)
+        dv = torch.empty(T, B, dtype=torch.float32, device=dev)
+        rc = L.b200rl_vtrace_fwd(
+            *tensors, T, B, N, *scal, ptr(out), ptr(lp), ptr(cpg), ptr(dv), ptr(ws), ws.numel() * 4, stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_vtrace_fwd')
+    return out, False, None, cpg, dv
+
+
+def vtrace_verify_(saved, scal, upstream, spec):
+    """The backward launch after a one-launch forward: ``saved`` = (target_output, behaviour_output, action, value, reward,
+    weight), ``upstream`` the three device pointers of the upstream gradients (None = 0).  With ``spec`` it verifies the
+    forward-written gradients on the device (recomputing in place on a mismatch), else it recomputes into fresh buffers.
+    -> (grad_logit, grad_value)."""
+    target_output, behaviour_output, action, value, reward, weight = saved
+    T, B = reward.shape
+    N = target_output.shape[-1]
+    dev = target_output.device
+    grad_logit, grad_value, g_used = spec or (
+        torch.empty_like(target_output), torch.empty(T + 1, B, dtype=torch.float32, device=dev), None)
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_vtrace_fwd_grad(
+            ptr(target_output), ptr(behaviour_output), ptr(action), ptr(value), ptr(reward), ptr(weight), T, B,
+            N, *scal, None, 1, *upstream, ptr(g_used), ptr(vtrace_hint(dev)), None, ptr(grad_logit),
+            ptr(grad_value), ptr(ws), ws.numel() * 4, stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_vtrace_fwd_grad(verify)')
+    return grad_logit, grad_value
+
+
+def vtrace_bwd_(target_output, action, weight, cpg, dv, upstream):
+    """The backward launch after the rows / scan forward -> (grad_logit, grad_value)."""
+    T, B = cpg.shape
+    N = target_output.shape[-1]
+    dev = target_output.device
+    grad_logit = torch.empty_like(target_output)
+    grad_value = torch.empty(T + 1, B, dtype=torch.float32, device=dev)
+    with on_device(dev):
+        rc = lib().b200rl_vtrace_bwd(
+            ptr(target_output), ptr(action), ptr(weight), ptr(cpg), ptr(dv), *upstream, T, B, N, ptr(grad_logit),
+            ptr(grad_value), stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_vtrace_bwd')
+    return grad_logit, grad_value
 
 
 class VTraceContinuousFunction(torch.autograd.Function):

@@ -3,7 +3,7 @@ from collections import namedtuple
 
 import torch
 
-from .. import ops
+from .. import ops, torch_ops
 
 gae_data = namedtuple('gae_data', ['value', 'next_value', 'reward', 'done', 'traj_flag'])
 gae_returns_out = namedtuple('gae_returns_out', ['adv', 'value', 'return_', 'unnormalized_return', 'return_stats', 'adv_stats'])
@@ -49,8 +49,13 @@ def gae(data: namedtuple, gamma: float = 0.99, lambda_: float = 0.97) -> torch.F
         d = d.expand_as(r).contiguous()
     if tf is not None and tf.shape != r.shape:
         tf = tf.expand_as(r).contiguous()
-    adv = ops.gae_(v, nv, r, d, tf, gamma, lambda_, agents)
-    if d is not None and nv.data_ptr() != nv_src.data_ptr():
+    if torch.compiler.is_compiling():
+        adv = torch_ops.gae_op(v, nv, r, d, tf, float(gamma), float(lambda_), agents)
+        staged = nv is not nv_src
+    else:
+        adv = ops.gae_(v, nv, r, d, tf, gamma, lambda_, agents)
+        staged = nv.data_ptr() != nv_src.data_ptr()
+    if d is not None and staged:
         # the kernel masked a staged / re-laid-out copy: propagate the reference's in-place side effect
         with torch.no_grad():
             next_value.copy_(nv.to(next_value.device))

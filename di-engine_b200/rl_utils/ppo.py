@@ -9,7 +9,7 @@ from typing import Optional, Tuple
 
 import torch
 
-from .. import ops
+from .. import ops, torch_ops
 
 ppo_data = namedtuple(
     'ppo_data',
@@ -164,15 +164,20 @@ def _ppo_error(data, clip_ratio, use_value_clip, dual_clip, kl_type, _hint_kind,
         fac = stage(factor.detach(), 'factor').reshape(-1)
         if fac.numel() != S:
             raise ValueError("happo_error: factor %s does not match adv %s" % (tuple(factor.shape), tuple(adv.shape)))
-    p, v, e, k, out = ops.PPOFunction.apply(
-        ln, vn, lo, act, vo, ad, rt, w, lp, S, G, N, float(clip_ratio), 1 if use_value_clip else 0,
-        float(dual_clip) if dual_clip is not None else 0.0, _KL_TYPES.get(kl_type, 1), _hint_kind, stats, fac
-    )
-    if LAZY_INFO:
-        info = ppo_info(out[4], out[5])
+    args = (ln, vn, lo, act, vo, ad, rt, w, lp, S, G, N, float(clip_ratio), 1 if use_value_clip else 0,
+            float(dual_clip) if dual_clip is not None else 0.0, _KL_TYPES.get(kl_type, 1), _hint_kind, stats, fac)
+    if torch.compiler.is_compiling():
+        out = torch_ops.ppo(*args)
+        p, v, e, k = out[0], out[1], out[2], out[3]
+        # the reference's two .item() calls (ppo.py:218-220): what a traced graph can take
+        info = ppo_info(out[4].detach(), out[5].detach()) if LAZY_INFO else ppo_info(out[4].item(), out[5].item())
     else:
-        approx_kl, clipfrac = out[4:6].tolist()  # one D2H read for both monitors (reference: two .item() syncs)
-        info = ppo_info(approx_kl, clipfrac)
+        p, v, e, k, out = ops.PPOFunction.apply(*args)
+        if LAZY_INFO:
+            info = ppo_info(out[4], out[5])
+        else:
+            approx_kl, clipfrac = out[4:6].tolist()  # one D2H read for both monitors (reference: two .item() syncs)
+            info = ppo_info(approx_kl, clipfrac)
     if host_out:
         p, v, e, k = p.cpu(), v.cpu(), e.cpu(), k.cpu()
     return ppo_loss(p, v, e, k), info

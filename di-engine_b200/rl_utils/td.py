@@ -14,7 +14,7 @@ from typing import Callable, Optional, Union
 import torch
 import torch.nn as nn
 
-from .. import ops
+from .. import ops, torch_ops
 from .value_rescale import value_inv_transform, value_transform
 
 q_nstep_td_data = namedtuple(
@@ -98,6 +98,14 @@ def _value_gamma_arg(value_gamma, B, dev):
     return vg.reshape(B), 1
 
 
+def _value_gamma_op_arg(value_gamma, B, dev):
+    """``_value_gamma_arg`` for the custom ops (rl_utils' traced path): a python scalar stays a float, which the op reads
+    from the cached device constant when it runs, so that tracing allocates nothing"""
+    if value_gamma is not None and not isinstance(value_gamma, torch.Tensor):
+        return float(value_gamma), 0
+    return _value_gamma_arg(value_gamma, B, dev)
+
+
 def _gamma_arg(gamma, B, dev, cum_reward):
     """python float -> (gamma, None); the NGU list of B 0-dim tensors (td.py:275-282) -> (0.0, (B,) device tensor)."""
     if isinstance(gamma, float):
@@ -137,12 +145,15 @@ def _qntd_rows(q, next_n_q, action, next_n_action, reward, done, weight, value_g
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.numel() != S:
             w = w.expand(S).contiguous()
-    vg, vg_stride = _value_gamma_arg(value_gamma, S, dev)
+    vg, vg_stride = (_value_gamma_op_arg if torch.compiler.is_compiling() else _value_gamma_arg)(value_gamma, S, dev)
     custom_trans = rescale and (trans_fn is not value_transform or inv_trans_fn is not value_inv_transform)
     code = _criterion_code(criterion)
     gm = 1 if group_mean else 0
 
     def kernel(q_, nq_, act_, nact_, n_, resc, crit, param):
+        if torch.compiler.is_compiling():
+            return torch_ops.qntd(q_, nq_, act_, nact_, r, d, w, vg, vg_stride, gamma_ps, S, G, n_, int(nstep),
+                                  float(gamma_f), 1 if cum_reward else 0, resc, 1e-2, crit, param, gm) + (None, )
         return ops.QNStepTDFunction.apply(q_, nq_, act_, nact_, r, d, w, vg, vg_stride, gamma_ps, S, G, n_, int(nstep),
                                           float(gamma_f), 1 if cum_reward else 0, resc, 1e-2, crit, param, gm, 0, 0.0,
                                           False)
@@ -971,7 +982,7 @@ def _support(v_min, v_max, n_atom, dev):
     s = _SUPPORT_CACHE.get(key)
     if s is None:
         # built on the host then moved, exactly like td.py:457 -- CPU and CUDA linspace differ in the last bit
-        s = torch.linspace(v_min, v_max, n_atom).to(dev)
+        s = ops.lasting(lambda: torch.linspace(v_min, v_max, n_atom).to(dev), dev)
         _SUPPORT_CACHE[key] = s
     return s
 
@@ -1019,7 +1030,7 @@ def _dntd(data, gamma, v_min, v_max, n_atom, nstep, value_gamma, check_positive)
     if weight is None:
         w, w_stride = None, 0
     elif not isinstance(weight, torch.Tensor):
-        w, w_stride = ops.const_scalar(weight, dev), 0
+        w, w_stride = (float(weight) if torch.compiler.is_compiling() else ops.const_scalar(weight, dev)), 0
     else:
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.numel() == 1:
@@ -1028,6 +1039,11 @@ def _dntd(data, gamma, v_min, v_max, n_atom, nstep, value_gamma, check_positive)
             w, w_stride = w.reshape(R), 1
         else:
             raise ValueError("weight must have 1 or %d elements, got %s" % (R, tuple(weight.shape)))
+    if torch.compiler.is_compiling():
+        vg, vg_stride = _value_gamma_op_arg(value_gamma, B, dev)
+        loss, per = torch_ops.dist_nstep_td(dd, nd, a, na, r, d, w, w_stride, vg, vg_stride, B, A, N, int(n_atom),
+                                            int(nstep), float(gamma), float(v_min), float(v_max), check_positive)
+        return (loss.cpu(), per.cpu()) if host_out else (loss, per)
     vg, vg_stride = _value_gamma_arg(value_gamma, B, dev)
     bad = torch.zeros(1, dtype=torch.int32, device=dev) if check_positive else None
     loss, per = ops.DistNStepTDFunction.apply(
@@ -1145,5 +1161,8 @@ def td_lambda_error(data: namedtuple, gamma: float = 0.9, lambda_: float = 0.8) 
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.shape != r.shape:
             w = w.expand_as(r).contiguous()
-    loss = ops.td_lambda_(v, r, w, gamma, lambda_)
+    if torch.compiler.is_compiling():
+        loss = torch_ops.td_lambda(v, r, w, float(gamma), float(lambda_))
+    else:
+        loss = ops.td_lambda_(v, r, w, gamma, lambda_)
     return loss.cpu() if host_out else loss

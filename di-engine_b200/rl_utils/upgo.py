@@ -2,7 +2,7 @@
 csrc/pg.cu."""
 import torch
 
-from .. import ops
+from .. import ops, torch_ops
 
 
 def tb_cross_entropy(logit: torch.Tensor, label: torch.Tensor, mask=None) -> torch.Tensor:
@@ -86,6 +86,9 @@ def upgo_loss(
     rho = ops.f32c(ops.to_device(rhos.detach(), dev), 'rhos')
     r = ops.f32c(ops.to_device(rewards.detach(), dev), 'rewards')
     v = ops.f32c(ops.to_device(bootstrap_values.detach(), dev), 'bootstrap_values')
-    ret = ops.lambda_returns_(v, r, None, 1.0, None, 1.0, None, True)
-    loss = ops.UPGOFunction.apply(logit, act, m, rho, ret, v, T * B, K, N)
+    if torch.compiler.is_compiling():
+        loss = torch_ops.upgo(logit, act, m, rho, r, v, T * B, K, N)
+    else:
+        ret = ops.lambda_returns_(v, r, None, 1.0, None, 1.0, None, True)
+        loss = ops.UPGOFunction.apply(logit, act, m, rho, ret, v, T * B, K, N)
     return loss.cpu() if host_out else loss

@@ -3,7 +3,7 @@ from collections import namedtuple
 
 import torch
 
-from .. import ops
+from .. import ops, torch_ops
 
 vtrace_data = namedtuple('vtrace_data', ['target_output', 'behaviour_output', 'action', 'value', 'reward', 'weight'])
 vtrace_loss = namedtuple('vtrace_loss', ['policy_loss', 'value_loss', 'entropy_loss'])
@@ -50,10 +50,9 @@ def vtrace_error_discrete_action(
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.shape != r.shape:
             w = w.expand_as(r).contiguous()
-    p, vl, e = ops.VTraceFunction.apply(
-        tgt, v, beh, act, r, w, float(gamma), float(lambda_), float(rho_clip_ratio), float(c_clip_ratio),
-        float(rho_pg_clip_ratio)
-    )
+    args = (tgt, v, beh, act, r, w, float(gamma), float(lambda_), float(rho_clip_ratio), float(c_clip_ratio),
+            float(rho_pg_clip_ratio))
+    p, vl, e = torch_ops.vtrace(*args) if torch.compiler.is_compiling() else ops.VTraceFunction.apply(*args)
     if host_out:
         p, vl, e = p.cpu(), vl.cpu(), e.cpu()
     return vtrace_loss(p, vl, e)
