@@ -477,11 +477,11 @@ class GAEPPOFunction(torch.autograd.Function):
         return (grads[0], grads[1]) + (None, ) * 20
 
 
-def ppo_value_(value_new, value_old, return_, weight, clip_ratio, use_value_clip):
-    """ppo_value_error (ppo.py:233-275): loss and, if needed, its gradient for a unit upstream gradient in one launch."""
+def ppo_value_fwd_(value_new, value_old, return_, weight, clip_ratio, use_value_clip, want_grad):
+    """The one launch of ppo_value_error (ppo.py:233-275) -> (loss, d loss / d value_new for a unit upstream gradient, or
+    None without ``want_grad``)"""
     dev = value_new.device
     loss = torch.empty((), dtype=torch.float32, device=dev)
-    want_grad = value_new.requires_grad and torch.is_grad_enabled()
     dvalue = torch.empty_like(value_new) if want_grad else None
     with on_device(dev):
         ws = workspace(dev)
@@ -490,6 +490,13 @@ def ppo_value_(value_new, value_old, return_, weight, clip_ratio, use_value_clip
             1 if use_value_clip else 0, ptr(loss), ptr(dvalue), ptr(ws), ws.numel() * 4, stream_ptr()
         )
     _lib.check(rc, 'b200rl_ppo_value_fwd')
+    return loss, dvalue
+
+
+def ppo_value_(value_new, value_old, return_, weight, clip_ratio, use_value_clip):
+    """ppo_value_error (ppo.py:233-275): loss and, if needed, its gradient for a unit upstream gradient in one launch."""
+    want_grad = value_new.requires_grad and torch.is_grad_enabled()
+    loss, dvalue = ppo_value_fwd_(value_new, value_old, return_, weight, clip_ratio, use_value_clip, want_grad)
     if want_grad:
         return _ScaleSaved.apply(value_new, loss, dvalue)
     return loss
@@ -1422,6 +1429,43 @@ def logits_c(t):
     return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
+def _vocab_rows(dev, rows):
+    """the per-call outputs of a GRPO / RLOO launch: the three loss sums, logsumexp and the unit coefficient per row"""
+    return (torch.empty(3, dtype=torch.float32, device=dev), torch.empty(rows, dtype=torch.float32, device=dev),
+            torch.empty(rows, dtype=torch.float32, device=dev))
+
+
+def grpo_fwd_(logit_new, logit_old, logit_ref, action, adv, weight, dt, clip_ratio, beta, grad):
+    """The forward launch of grpo_policy_error (GRPOFunction and the ``b200rl::lm_policy_fwd`` custom op): logits
+    (B, S, V) contiguous and 16-byte aligned.  -> (loss / approx_kl / clipfrac, logsumexp of logit_new per row, d loss /
+    d lp_new per row for a unit upstream gradient); also writes d loss / d logit_new for that gradient into ``grad``
+    unless it is None."""
+    B, S, V = logit_new.shape
+    dev = logit_new.device
+    out, lse, dlp = _vocab_rows(dev, B * S)
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_grpo_fwd_grad(dt, ptr(logit_new), ptr(logit_old), ptr(logit_ref), ptr(action), ptr(adv),
+                                        ptr(weight), B, S, V, clip_ratio, beta, ptr(out), ptr(lse), ptr(dlp),
+                                        ptr(grad), ptr(ws), ws.numel() * 4, stream_ptr())
+    _lib.check(rc, 'b200rl_grpo_fwd_grad')
+    return out, lse, dlp
+
+
+def rloo_fwd_(logit_new, logit_old, action, reward, weight, dt, clip_ratio, grad):
+    """The forward launch of rloo_policy_error, reward (K, B / K); as ``grpo_fwd_``"""
+    B, S, V = logit_new.shape
+    dev = logit_new.device
+    out, lse, dlp = _vocab_rows(dev, B * S)
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_rloo_fwd_grad(dt, ptr(logit_new), ptr(logit_old), ptr(action), ptr(reward), reward.shape[0],
+                                        ptr(weight), B, S, V, clip_ratio, ptr(out), ptr(lse), ptr(dlp), ptr(grad),
+                                        ptr(ws), ws.numel() * 4, stream_ptr())
+    _lib.check(rc, 'b200rl_rloo_fwd_grad')
+    return out, lse, dlp
+
+
 class GRPOFunction(torch.autograd.Function):
     """grpo_policy_error (ding/rl_utils/grpo.py) on logits (B, S, V): outputs loss (differentiable w.r.t. logit_new),
     approx_kl and clipfrac.  ONE forward launch (+ the loss-sum finalize) also writes d loss / d logit_new for a unit
@@ -1430,14 +1474,8 @@ class GRPOFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, logit_new, logit_old, logit_ref, action, adv, weight, dt, clip_ratio, beta):
-        B, S, V = logit_new.shape
-        out, lse, dlp, grad = _vocab_outputs(ctx, logit_new)
-        with on_device(logit_new.device):
-            ws = workspace(logit_new.device)
-            rc = lib().b200rl_grpo_fwd_grad(dt, ptr(logit_new), ptr(logit_old), ptr(logit_ref), ptr(action), ptr(adv),
-                                            ptr(weight), B, S, V, clip_ratio, beta, ptr(out), ptr(lse), ptr(dlp),
-                                            ptr(grad), ptr(ws), ws.numel() * 4, stream_ptr())
-        _lib.check(rc, 'b200rl_grpo_fwd_grad')
+        grad = torch.empty_like(logit_new) if ctx.needs_input_grad[0] else None
+        out, lse, dlp = grpo_fwd_(logit_new, logit_old, logit_ref, action, adv, weight, dt, clip_ratio, beta, grad)
         return _vocab_saved(ctx, logit_new, action, lse, dlp, grad, dt, out)
 
     @staticmethod
@@ -1451,19 +1489,49 @@ class RLOOFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, logit_new, logit_old, action, reward, weight, dt, clip_ratio):
-        B, S, V = logit_new.shape
-        out, lse, dlp, grad = _vocab_outputs(ctx, logit_new)
-        with on_device(logit_new.device):
-            ws = workspace(logit_new.device)
-            rc = lib().b200rl_rloo_fwd_grad(dt, ptr(logit_new), ptr(logit_old), ptr(action), ptr(reward), reward.shape[0],
-                                            ptr(weight), B, S, V, clip_ratio, ptr(out), ptr(lse), ptr(dlp), ptr(grad),
-                                            ptr(ws), ws.numel() * 4, stream_ptr())
-        _lib.check(rc, 'b200rl_rloo_fwd_grad')
+        grad = torch.empty_like(logit_new) if ctx.needs_input_grad[0] else None
+        out, lse, dlp = rloo_fwd_(logit_new, logit_old, action, reward, weight, dt, clip_ratio, grad)
         return _vocab_saved(ctx, logit_new, action, lse, dlp, grad, dt, out)
 
     @staticmethod
     def backward(ctx, g_loss, _g_kl, _g_cf):
         return (_vocab_backward(ctx, g_loss), ) + (None, ) * 6
+
+
+def ppo_lm_fwd_(logit_new, logit_old, logit_pre, action, adv, weight, dt, clip_ratio, dual_clip, kl_type, entropy, hint,
+                grad, g_used):
+    """The forward launch of ppo_policy_error on token rows (PPOLMFunction and the ``b200rl::ppo_lm_fwd`` custom op).
+    -> (the five loss sums, and per row: logsumexp, entropy (None without ``entropy``), the policy term's unit coefficient,
+    the kl term's (None without logit_pre)).  With ``grad`` it also writes d / d logit_new for the upstream gradients of
+    the record ``hint`` and records them in ``g_used``."""
+    dev = logit_new.device
+    V = logit_new.shape[-1]
+    rows = logit_new.numel() // V
+    out = torch.empty(5, dtype=torch.float32, device=dev)
+    lse = torch.empty(rows, dtype=torch.float32, device=dev)
+    ent = torch.empty(rows, dtype=torch.float32, device=dev) if entropy else None
+    dpol = torch.empty(rows, dtype=torch.float32, device=dev)
+    dkl = torch.empty(rows, dtype=torch.float32, device=dev) if logit_pre is not None else None
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_ppo_lm_fwd_grad(
+            dt, ptr(logit_new), ptr(logit_old), ptr(logit_pre), ptr(action), ptr(adv), ptr(weight), rows, V,
+            clip_ratio, dual_clip, kl_type, 1 if entropy else 0, ptr(hint), ptr(g_used), ptr(out), ptr(lse), ptr(ent),
+            ptr(dpol), ptr(dkl), ptr(grad), ptr(ws), ws.numel() * 4, stream_ptr())
+    _lib.check(rc, 'b200rl_ppo_lm_fwd_grad')
+    return out, lse, ent, dpol, dkl
+
+
+def ppo_lm_bwd_(dt, logit_new, action, weight, lse, ent, dpol, dkl, upstream, g_used, hint, grad):
+    """The backward launch of ppo_policy_error on token rows: ``upstream`` the device pointers of the policy, entropy and
+    kl upstream gradients (None = 0).  With ``g_used`` (the forward-written gradient's record) it returns at once on the
+    device when they match it and rewrites ``grad`` otherwise; without, it computes ``grad``.  -> grad."""
+    with on_device(logit_new.device):
+        rc = lib().b200rl_ppo_lm_bwd(dt, ptr(logit_new), ptr(action), ptr(weight), lse.numel(), logit_new.shape[-1],
+                                     ptr(lse), ptr(ent), ptr(dpol), ptr(dkl), *upstream, ptr(g_used), ptr(hint),
+                                     ptr(grad), stream_ptr())
+    _lib.check(rc, 'b200rl_ppo_lm_bwd')
+    return grad
 
 
 class PPOLMFunction(torch.autograd.Function):
@@ -1478,25 +1546,13 @@ class PPOLMFunction(torch.autograd.Function):
     def forward(ctx, logit_new, logit_old, logit_pre, action, adv, weight, dt, clip_ratio, dual_clip, kl_type, entropy,
                 hint_kind):
         dev = logit_new.device
-        V = logit_new.shape[-1]
-        rows = logit_new.numel() // V
-        out = torch.empty(5, dtype=torch.float32, device=dev)
-        lse = torch.empty(rows, dtype=torch.float32, device=dev)
-        ent = torch.empty(rows, dtype=torch.float32, device=dev) if entropy else None
-        dpol = torch.empty(rows, dtype=torch.float32, device=dev)
-        dkl = torch.empty(rows, dtype=torch.float32, device=dev) if logit_pre is not None else None
         want = ctx.needs_input_grad[0]
         grad = torch.empty_like(logit_new) if want else None
         g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
         ctx.hint_kind = hint_kind
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_ppo_lm_fwd_grad(
-                dt, ptr(logit_new), ptr(logit_old), ptr(logit_pre), ptr(action), ptr(adv), ptr(weight), rows, V,
-                clip_ratio, dual_clip, kl_type, 1 if entropy else 0, ptr(ppo_hint(dev, hint_kind)) if want else None,
-                ptr(g_used), ptr(out), ptr(lse), ptr(ent), ptr(dpol), ptr(dkl), ptr(grad), ptr(ws), ws.numel() * 4,
-                stream_ptr())
-        _lib.check(rc, 'b200rl_ppo_lm_fwd_grad')
+        out, lse, ent, dpol, dkl = ppo_lm_fwd_(logit_new, logit_old, logit_pre, action, adv, weight, dt, clip_ratio,
+                                               dual_clip, kl_type, entropy, ppo_hint(dev, hint_kind) if want else None,
+                                               grad, g_used)
         ctx.save_for_backward(logit_new, action, weight, lse, ent, dpol, dkl)
         ctx.dt = dt
         ctx.spec = (grad, g_used) if want else None
@@ -1506,21 +1562,47 @@ class PPOLMFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_p, g_e, g_k, _g_out):
         logit_new, action, weight, lse, ent, dpol, dkl = ctx.saved_tensors
-        dev = logit_new.device
-        keep, (pp, pe, pk) = _grads(g_p, g_e, g_k)
+        keep, upstream = _grads(g_p, g_e, g_k)
         spec = _forward_grads(ctx)
         if spec is not None:  # valid if the expectation held; the kernel checks on the device
             grad, g_used = spec
-            p_used, p_hint = ptr(g_used), ptr(ppo_hint(dev, ctx.hint_kind))
+            hint = ppo_hint(logit_new.device, ctx.hint_kind)
         else:  # a repeated backward: null g_used / hint -> the kernel recomputes
-            grad, p_used, p_hint = torch.empty_like(logit_new), None, None
-        V = logit_new.shape[-1]
-        with on_device(dev):
-            rc = lib().b200rl_ppo_lm_bwd(ctx.dt, ptr(logit_new), ptr(action), ptr(weight), lse.numel(), V, ptr(lse),
-                                         ptr(ent), ptr(dpol), ptr(dkl), pp, pe, pk, p_used, p_hint, ptr(grad),
-                                         stream_ptr())
-        _lib.check(rc, 'b200rl_ppo_lm_bwd')
+            grad, g_used, hint = torch.empty_like(logit_new), None, None
+        grad = ppo_lm_bwd_(ctx.dt, logit_new, action, weight, lse, ent, dpol, dkl, upstream, g_used, hint, grad)
         return (grad, ) + (None, ) * 11
+
+
+def a2c_lm_fwd_(logit, value, action, adv, return_, weight, dt, hint, gl, gv, g_used):
+    """The forward launch of a2c_error on token rows (A2CLMFunction and the ``b200rl::a2c_lm_fwd`` custom op).  -> (the
+    three loss sums, (4, rows): per row logsumexp, entropy, the policy term's unit coefficient, d value_loss / d value).  With
+    ``gl`` / ``gv`` it also writes d / d logit and d / d value for the upstream gradients of the record ``hint`` and records
+    them in ``g_used``."""
+    dev = logit.device
+    V = logit.shape[-1]
+    rows = logit.numel() // V
+    out = torch.empty(3, dtype=torch.float32, device=dev)
+    per_row = torch.empty(4, rows, dtype=torch.float32, device=dev)
+    lse, ent, dpol, dval = per_row.unbind(0)
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_a2c_lm_fwd_grad(
+            dt, ptr(logit), ptr(action), ptr(value), ptr(adv), ptr(return_), ptr(weight), rows, V, ptr(hint),
+            ptr(g_used), ptr(out), ptr(lse), ptr(ent), ptr(dpol), ptr(dval), ptr(gl), ptr(gv), ptr(ws), ws.numel() * 4,
+            stream_ptr())
+    _lib.check(rc, 'b200rl_a2c_lm_fwd_grad')
+    return out, per_row
+
+
+def a2c_lm_bwd_(dt, logit, action, weight, lse, ent, dpol, dval, upstream, g_used, hint, gl, gv):
+    """The backward launch of a2c_error on token rows: ``upstream`` the device pointers of the policy, value and entropy
+    upstream gradients (None = 0); with ``g_used`` it verifies as ``ppo_lm_bwd_``.  -> (gl, gv)."""
+    with on_device(logit.device):
+        rc = lib().b200rl_a2c_lm_bwd(dt, ptr(logit), ptr(action), ptr(weight), lse.numel(), logit.shape[-1], ptr(lse),
+                                     ptr(ent), ptr(dpol), ptr(dval), *upstream, ptr(g_used), ptr(hint), ptr(gl),
+                                     ptr(gv), stream_ptr())
+    _lib.check(rc, 'b200rl_a2c_lm_bwd')
+    return gl, gv
 
 
 class A2CLMFunction(torch.autograd.Function):
@@ -1534,22 +1616,13 @@ class A2CLMFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logit, value, action, adv, return_, weight, dt):
         dev = logit.device
-        V = logit.shape[-1]
-        rows = logit.numel() // V
-        out = torch.empty(3, dtype=torch.float32, device=dev)
-        lse, ent, dpol, dval = torch.empty(4, rows, dtype=torch.float32, device=dev).unbind(0)
         want = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
         gl = torch.empty_like(logit) if want else None
         gv = torch.empty_like(value) if want else None
         g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_a2c_lm_fwd_grad(
-                dt, ptr(logit), ptr(action), ptr(value), ptr(adv), ptr(return_), ptr(weight), rows, V,
-                ptr(ppo_hint(dev, 'a2c')) if want else None, ptr(g_used), ptr(out), ptr(lse), ptr(ent), ptr(dpol),
-                ptr(dval), ptr(gl), ptr(gv), ptr(ws), ws.numel() * 4, stream_ptr())
-        _lib.check(rc, 'b200rl_a2c_lm_fwd_grad')
-        ctx.save_for_backward(logit, value, action, weight, lse, ent, dpol, dval)
+        out, per_row = a2c_lm_fwd_(logit, value, action, adv, return_, weight, dt, ppo_hint(dev, 'a2c') if want else None,
+                                   gl, gv, g_used)
+        ctx.save_for_backward(logit, value, action, weight, *per_row.unbind(0))
         ctx.dt = dt
         ctx.spec = (gl, gv, g_used) if want else None
         ctx.set_materialize_grads(False)
@@ -1558,30 +1631,15 @@ class A2CLMFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_p, g_v, g_e):
         logit, value, action, weight, lse, ent, dpol, dval = ctx.saved_tensors
-        dev = logit.device
-        keep, (pp, pv, pe) = _grads(g_p, g_v, g_e)
+        keep, upstream = _grads(g_p, g_v, g_e)
         spec = _forward_grads(ctx)
         if spec is not None:  # valid if the expectation held; the kernel checks on the device
             gl, gv, g_used = spec
-            p_used, p_hint = ptr(g_used), ptr(ppo_hint(dev, 'a2c'))
+            hint = ppo_hint(logit.device, 'a2c')
         else:  # a repeated backward: null g_used / hint -> the kernel recomputes
-            gl, gv, p_used, p_hint = torch.empty_like(logit), torch.empty_like(value), None, None
-        with on_device(dev):
-            rc = lib().b200rl_a2c_lm_bwd(ctx.dt, ptr(logit), ptr(action), ptr(weight), lse.numel(), logit.shape[-1],
-                                         ptr(lse), ptr(ent), ptr(dpol), ptr(dval), pp, pv, pe, p_used, p_hint, ptr(gl),
-                                         ptr(gv), stream_ptr())
-        _lib.check(rc, 'b200rl_a2c_lm_bwd')
+            gl, gv, g_used, hint = torch.empty_like(logit), torch.empty_like(value), None, None
+        gl, gv = a2c_lm_bwd_(ctx.dt, logit, action, weight, lse, ent, dpol, dval, upstream, g_used, hint, gl, gv)
         return gl, gv, None, None, None, None, None
-
-
-def _vocab_outputs(ctx, logit_new):
-    dev = logit_new.device
-    rows = logit_new.shape[0] * logit_new.shape[1]
-    out = torch.empty(3, dtype=torch.float32, device=dev)
-    lse = torch.empty(rows, dtype=torch.float32, device=dev)
-    dlp = torch.empty(rows, dtype=torch.float32, device=dev)
-    grad = torch.empty_like(logit_new) if ctx.needs_input_grad[0] else None
-    return out, lse, dlp, grad
 
 
 def _vocab_saved(ctx, logit_new, action, lse, dlp, grad, dt, out):
@@ -1600,9 +1658,29 @@ def _vocab_backward(ctx, g_loss):
     logit_new, action, lse, dlp = ctx.saved_tensors
     keep, (pg, ) = _grads(g_loss)
     grad, skip = _unit_grad(ctx, (), lambda: torch.empty_like(logit_new))
-    with on_device(logit_new.device):
-        rc = lib().b200rl_token_logp_bwd(ctx.dt, ptr(logit_new), ptr(action), ptr(lse), ptr(dlp), pg, skip, lse.numel(),
-                                         logit_new.shape[-1], ptr(grad), stream_ptr())
+    return token_logp_bwd_(ctx.dt, logit_new, action, lse, dlp, pg, skip, grad)
+
+
+def token_logp_fwd_(dt, logits, index):
+    """The forward launch of the log-prob methods: logits (rows, V) -> (log p(index), logsumexp) per row, fp32"""
+    rows = logits.shape[0]
+    lp = torch.empty(rows, dtype=torch.float32, device=logits.device)
+    lse = torch.empty(rows, dtype=torch.float32, device=logits.device)
+    with on_device(logits.device):
+        rc = lib().b200rl_token_logp_fwd(dt, ptr(logits), ptr(index), rows, logits.shape[-1], ptr(lp), ptr(lse),
+                                         stream_ptr())
+    _lib.check(rc, 'b200rl_token_logp_fwd')
+    return lp, lse
+
+
+def token_logp_bwd_(dt, logits, index, lse, coef, pg, skip, grad):
+    """The backward launch of the vocabulary rows: ``grad`` = (*pg, or 1 for a null pg) * coef[row] * (onehot(index) -
+    softmax(logits[row])), the gradient of the log-prob methods (coef = their upstream gradient) and of GRPO / RLOO (coef
+    = the unit coefficient).  With ``skip`` the launch returns at once on the device when *pg is 1: ``grad`` then holds
+    the forward-written gradient.  -> grad."""
+    with on_device(logits.device):
+        rc = lib().b200rl_token_logp_bwd(dt, ptr(logits), ptr(index), ptr(lse), ptr(coef), pg, skip, lse.numel(),
+                                         logits.shape[-1], ptr(grad), stream_ptr())
     _lib.check(rc, 'b200rl_token_logp_bwd')
     return grad
 
@@ -1613,12 +1691,7 @@ class TokenLogProbFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, logits, index, dt):
-        rows, V = logits.shape
-        lp = torch.empty(rows, dtype=torch.float32, device=logits.device)
-        lse = torch.empty(rows, dtype=torch.float32, device=logits.device)
-        with on_device(logits.device):
-            rc = lib().b200rl_token_logp_fwd(dt, ptr(logits), ptr(index), rows, V, ptr(lp), ptr(lse), stream_ptr())
-        _lib.check(rc, 'b200rl_token_logp_fwd')
+        lp, lse = token_logp_fwd_(dt, logits, index)
         ctx.save_for_backward(logits, index, lse)
         ctx.dt = dt
         return lp
@@ -1627,18 +1700,12 @@ class TokenLogProbFunction(torch.autograd.Function):
     def backward(ctx, g):
         logits, index, lse = ctx.saved_tensors
         g = g.float().contiguous()
-        grad = torch.empty_like(logits)
-        with on_device(logits.device):
-            rc = lib().b200rl_token_logp_bwd(ctx.dt, ptr(logits), ptr(index), ptr(lse), ptr(g), None, 0, lse.numel(),
-                                             logits.shape[-1], ptr(grad), stream_ptr())
-        _lib.check(rc, 'b200rl_token_logp_bwd')
-        return grad, None, None
+        return token_logp_bwd_(ctx.dt, logits, index, lse, g, None, 0, torch.empty_like(logits)), None, None
 
 
-def token_head_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
-    """The GRPO (``lp_ref`` given) or RLOO head on per-token log-probabilities (B, S) fp32 from a caller's own
-    log_prob_fn: returns (loss, approx_kl, clipfrac); the gradient reaches ``lp_new`` (b200rl_scale of the saved
-    unit-upstream gradient), and through it whatever computed it."""
+def token_head_fwd_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
+    """The one launch of the GRPO (``lp_ref`` given) or RLOO head on per-token log-probabilities (B, S) fp32: -> (loss /
+    approx_kl / clipfrac, d loss / d lp_new (B, S) for a unit upstream gradient)"""
     dev = lp_new.device
     B, S = lp_new.shape
     out = torch.empty(3, dtype=torch.float32, device=dev)
@@ -1649,6 +1716,14 @@ def token_head_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
                                          0 if reward is None else reward.shape[0], ptr(weight), B, S, clip_ratio, beta,
                                          ptr(out), ptr(dlp), ptr(ws), ws.numel() * 4, stream_ptr())
     _lib.check(rc, 'b200rl_token_head_fwd')
+    return out, dlp
+
+
+def token_head_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
+    """The GRPO (``lp_ref`` given) or RLOO head on per-token log-probabilities (B, S) fp32 from a caller's own
+    log_prob_fn: returns (loss, approx_kl, clipfrac); the gradient reaches ``lp_new`` (b200rl_scale of the saved
+    unit-upstream gradient), and through it whatever computed it."""
+    out, dlp = token_head_fwd_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta)
     loss = out[0]
     if lp_new.requires_grad and torch.is_grad_enabled():
         loss = _ScaleSaved.apply(lp_new, loss, dlp)

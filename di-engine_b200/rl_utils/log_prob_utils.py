@@ -8,7 +8,7 @@ from typing import Callable
 import torch
 from torch import Tensor
 
-from .. import ops
+from .. import ops, torch_ops
 
 LogProbFunction = Callable[[Tensor, Tensor], Tensor]
 
@@ -29,9 +29,13 @@ def _token_logp(logits: Tensor, index: Tensor) -> Tensor:
     dev = ops.compute_device(logits, index)
     host_out = not logits.is_cuda
     V = logits.shape[-1]
-    x = ops.logits_c(ops.to_device(logits, dev)).view(-1, V)
+    x = ops.to_device(logits, dev)
     a = ops.i64c(ops.to_device(index, dev), V, 'index').view(-1)
-    lp = ops.TokenLogProbFunction.apply(x, a, dt).view(index.shape)
+    if torch.compiler.is_compiling():  # the custom op makes the kernel's 16-byte-aligned copy itself
+        lp = torch_ops.token_logp(x.contiguous().view(-1, V), a)
+    else:
+        lp = ops.TokenLogProbFunction.apply(ops.logits_c(x).view(-1, V), a, dt)
+    lp = lp.view(index.shape)
     return lp.cpu() if host_out else lp
 
 

@@ -301,8 +301,10 @@ def _ppo_lm(data, clip_ratio, dual_clip, entropy_bonus, kl_type, hint_kind):
                              (name, tuple(t_.shape), tuple(logit_new.shape)))
     dev = ops.compute_device(*logits)
     host_out = not logit_new.is_cuda
-    # logit_old / logit_pretrained get no gradient; weight and adv are read as fp32 whatever their dtype
-    xs = [ops.logits_c(ops.to_device(x, dev)) for x in logits]
+    compiling = torch.compiler.is_compiling()
+    # logit_old / logit_pretrained get no gradient; weight and adv are read as fp32 whatever their dtype.  A traced tensor
+    # has no address: the custom op makes the kernel's 16-byte-aligned copy itself
+    xs = [ops.to_device(x, dev).contiguous() if compiling else ops.logits_c(ops.to_device(x, dev)) for x in logits]
     xs[1:] = [x.detach() for x in xs[1:]]
     ad = ops.to_device(adv.detach(), dev).float().contiguous()
     w = None
@@ -310,15 +312,20 @@ def _ppo_lm(data, clip_ratio, dual_clip, entropy_bonus, kl_type, hint_kind):
         w = ops.to_device(weight.detach(), dev).float()
         w = (w if w.numel() == rows else w.expand_as(ad)).contiguous()
     act = ops.i64c(ops.to_device(action, dev), V)
-    p, e, k, out = ops.PPOLMFunction.apply(
-        xs[0], xs[1], xs[2] if len(xs) > 2 else None, act, ad, w, dt, float(clip_ratio),
-        float(dual_clip) if dual_clip is not None else 0.0, _KL_TYPES.get(kl_type, 1), bool(entropy_bonus), hint_kind
-    )
-    if LAZY_INFO:
-        info = ppo_info(out[3], out[4])
+    args = (xs[0], xs[1], xs[2] if len(xs) > 2 else None, act, ad, w)
+    cfg = (float(clip_ratio), float(dual_clip) if dual_clip is not None else 0.0, _KL_TYPES.get(kl_type, 1),
+           bool(entropy_bonus))
+    if compiling:
+        p, e, k, out = torch_ops.ppo_lm(*args, *cfg)
+        # the reference's two .item() calls (ppo.py:218-220): what a traced graph can take
+        info = ppo_info(out[3].detach(), out[4].detach()) if LAZY_INFO else ppo_info(out[3].item(), out[4].item())
     else:
-        approx_kl, clipfrac = out[3:5].tolist()
-        info = ppo_info(approx_kl, clipfrac)
+        p, e, k, out = ops.PPOLMFunction.apply(*args, dt, *cfg, hint_kind)
+        if LAZY_INFO:
+            info = ppo_info(out[3], out[4])
+        else:
+            approx_kl, clipfrac = out[3:5].tolist()
+            info = ppo_info(approx_kl, clipfrac)
     if host_out:
         p, e, k = p.cpu(), e.cpu(), k.cpu()
     entropy = e if entropy_bonus else torch.tensor(0.0)  # ppo.py:203
@@ -372,5 +379,6 @@ def ppo_value_error(
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.numel() != vn.numel():
             w = w.expand_as(vn).contiguous()
-    loss = ops.ppo_value_(vn, vo, rt, w, clip_ratio, use_value_clip)
+    value = torch_ops.ppo_value if torch.compiler.is_compiling() else ops.ppo_value_
+    loss = value(vn, vo, rt, w, clip_ratio, use_value_clip)
     return loss.cpu() if host_out else loss

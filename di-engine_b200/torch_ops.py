@@ -1,7 +1,9 @@
 """The hot-path launches of ``ops`` as ``torch.library`` custom ops (namespace ``b200rl``), so that ``torch.compile`` can
 trace the eight operators of the reference's plugin boundary (gae, ppo_error, q_nstep_td_error,
-q_nstep_td_error_with_rescale, dist_nstep_td_error, td_lambda_error, upgo_loss, vtrace_error_discrete_action) without a
-graph break, and ``mode="reduce-overhead"`` can replay a compiled learner step as a CUDA graph.
+q_nstep_td_error_with_rescale, dist_nstep_td_error, td_lambda_error, upgo_loss, vtrace_error_discrete_action) and the
+language-model losses on (B, S, V) logits (grpo_policy_error, rloo_policy_error, the log-prob methods, ppo_policy_error /
+ppo_error / a2c_error on token rows, ppo_value_error) without a graph break, and ``mode="reduce-overhead"`` can replay a
+compiled learner step as a CUDA graph.
 
 Each op's implementation is the launch function ``ops`` runs in eager mode; ``rl_utils`` calls the wrappers at the bottom
 of this module only while ``torch.compiler.is_compiling()``.  The schemas hold tensors and scalars only: the workspace, the
@@ -10,6 +12,8 @@ upstream-gradient records and cached constants are looked up inside the implemen
 The forward-written gradients work as in eager mode, with one difference that functional ops impose: a backward op may
 not return its input, so after a forward launch that wrote the gradients the backward op copies them once and runs the
 verify launch on the copy (recomputing on the device when the upstream gradients differ from the record, no host sync).
+At vocabulary scale that copy would cost as much as the loss: the language-model ops write no gradient in the forward op
+and recompute it in the backward op from the saved per-row values, at the price of one more read of logit_new.
 """
 from typing import Optional
 
@@ -436,6 +440,250 @@ vtrace_loss.register_autograd(_vtrace_backward, setup_context=_vtrace_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# ppo_value_error: the forward launch writes d loss / d value_new for a unit upstream gradient; backward scales it
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::ppo_value_fwd', mutates_args=())
+def ppo_value_fwd(value_new: Tensor, value_old: Tensor, return_: Tensor, weight: Optional[Tensor], clip_ratio: float,
+                  use_value_clip: bool, want_grad: bool) -> tuple[Tensor, Tensor]:
+    """-> (loss, d loss / d value_new; empty without ``want_grad``)"""
+    loss, dvalue = ops.ppo_value_fwd_(value_new, value_old, return_, weight, clip_ratio, use_value_clip, want_grad)
+    return loss, dvalue if dvalue is not None else _empty(loss)
+
+
+@ppo_value_fwd.register_fake
+def _(value_new, value_old, return_, weight, clip_ratio, use_value_clip, want_grad):
+    loss = value_new.new_empty(())
+    return loss, torch.empty_like(value_new) if want_grad else _empty(loss)
+
+
+def _ppo_value_setup(ctx, inputs, output):
+    ctx.save_for_backward(output[1])
+    ctx.mark_non_differentiable(output[1])
+
+
+def _ppo_value_backward(ctx, g_loss, _g_dvalue):
+    dvalue, = ctx.saved_tensors
+    return (scale(g_loss, dvalue), ) + (None, ) * 6
+
+
+ppo_value_fwd.register_autograd(_ppo_value_backward, setup_context=_ppo_value_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The language-model losses on (B, S, V) logits (csrc/vocab.cu).  Their gradients are recomputed in the backward op from
+# the per-row values the forward op saves: the forward op writes no gradient, so nothing of (B, S, V) size is copied.
+# A backward op that rewrote the forward's gradient buffer in place would have to declare that buffer mutated; after
+# functionalization the buffer is an input of the backward graph that nothing copies back into, and inductor does not
+# reinplace such an input -- it copies it first, which is the (B, S, V) copy this design avoids.  The cost instead is one
+# more read of logit_new, in the backward op.  Each op makes the kernel's 16-byte-aligned copy of an odd-offset view
+# itself (ops.logits_c): a traced tensor has no address to decide it by.
+# ---------------------------------------------------------------------------------------------------------------------
+def _rows(x):
+    """the token rows of logits (..., V), symbolic under dynamic shapes"""
+    return x.numel() // x.shape[-1]
+
+
+def _f32(x, n):
+    return x.new_empty(n, dtype=torch.float32)
+
+
+@torch.library.custom_op('b200rl::token_logp', mutates_args=())
+def token_logp_op(logits: Tensor, index: Tensor) -> tuple[Tensor, Tensor]:
+    """the log-prob methods: logits (rows, V) fp32 or bf16, index (rows) -> (log p(index), logsumexp), fp32 per row"""
+    x = ops.logits_c(logits)
+    return ops.token_logp_fwd_(ops.logit_dtype(x), x, index)
+
+
+@token_logp_op.register_fake
+def _(logits, index):
+    return _f32(logits, logits.shape[0]), _f32(logits, logits.shape[0])
+
+
+@torch.library.custom_op('b200rl::vocab_bwd', mutates_args=())
+def vocab_bwd(logits: Tensor, index: Tensor, lse: Tensor, coef: Tensor, g: Optional[Tensor]) -> Tensor:
+    """d / d logits = (g[0], or 1 without ``g``) * coef[row] * (onehot(index) - softmax(logits[row])), in the logits'
+    dtype: the backward of ``token_logp`` (coef its upstream gradient) and of ``lm_policy_fwd`` (coef the unit
+    coefficient, g the loss's upstream gradient)"""
+    x = ops.logits_c(logits)
+    keep, pg = _one(g)
+    return ops.token_logp_bwd_(ops.logit_dtype(x), x, index, lse, coef, pg, 0, torch.empty_like(logits))
+
+
+@vocab_bwd.register_fake
+def _(logits, *args):
+    return torch.empty_like(logits)
+
+
+def _token_logp_setup(ctx, inputs, output):
+    ctx.save_for_backward(inputs[0], inputs[1], output[1])
+    ctx.mark_non_differentiable(output[1])
+
+
+def _token_logp_backward(ctx, g_lp, _g_lse):
+    logits, index, lse = ctx.saved_tensors
+    return vocab_bwd(logits, index, lse, g_lp.float().contiguous(), None), None
+
+
+token_logp_op.register_autograd(_token_logp_backward, setup_context=_token_logp_setup)
+
+
+@torch.library.custom_op('b200rl::lm_policy_fwd', mutates_args=())
+def lm_policy_fwd(logit_new: Tensor, logit_old: Tensor, logit_ref: Optional[Tensor], action: Tensor, side: Tensor,
+                  weight: Optional[Tensor], mode: str, clip_ratio: float, beta: float) -> tuple[Tensor, Tensor, Tensor]:
+    """grpo_policy_error (``mode`` 'grpo': side = adv (B)) or rloo_policy_error ('rloo': side = reward (K, B / K)) on
+    logits (B, S, V) -> (loss / approx_kl / clipfrac, logsumexp of logit_new per row, d loss / d lp_new per row for a unit
+    upstream gradient)"""
+    xs = [ops.logits_c(x) if x is not None else None for x in (logit_new, logit_old, logit_ref)]
+    dt = ops.logit_dtype(xs[0])
+    if mode == 'grpo':
+        return ops.grpo_fwd_(xs[0], xs[1], xs[2], action, side, weight, dt, clip_ratio, beta, None)
+    return ops.rloo_fwd_(xs[0], xs[1], action, side, weight, dt, clip_ratio, None)
+
+
+@lm_policy_fwd.register_fake
+def _(logit_new, logit_old, logit_ref, action, side, weight, mode, clip_ratio, beta):
+    rows = logit_new.shape[0] * logit_new.shape[1]
+    return _f32(logit_new, 3), _f32(logit_new, rows), _f32(logit_new, rows)
+
+
+def _lm_policy_setup(ctx, inputs, output):
+    ctx.save_for_backward(inputs[0], inputs[3], output[1], output[2])
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(output[1], output[2])
+
+
+def _lm_policy_backward(ctx, g_out, _g_lse, _g_dlp):
+    if g_out is None:
+        return (None, ) * 9
+    logit_new, action, lse, dlp = ctx.saved_tensors
+    return (vocab_bwd(logit_new, action, lse, dlp, g_out), ) + (None, ) * 8
+
+
+lm_policy_fwd.register_autograd(_lm_policy_backward, setup_context=_lm_policy_setup)
+
+
+@torch.library.custom_op('b200rl::token_head_fwd', mutates_args=())
+def token_head_fwd(lp_new: Tensor, lp_old: Tensor, lp_ref: Optional[Tensor], adv: Optional[Tensor],
+                   reward: Optional[Tensor], weight: Optional[Tensor], clip_ratio: float,
+                   beta: float) -> tuple[Tensor, Tensor]:
+    """the GRPO (``lp_ref`` given) or RLOO head on a custom log_prob_fn's (B, S) fp32 output -> (loss / approx_kl /
+    clipfrac, d loss / d lp_new for a unit upstream gradient)"""
+    return ops.token_head_fwd_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta)
+
+
+@token_head_fwd.register_fake
+def _(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
+    return _f32(lp_new, 3), torch.empty_like(lp_new)
+
+
+def _token_head_setup(ctx, inputs, output):
+    ctx.save_for_backward(output[1])
+    ctx.mark_non_differentiable(output[1])
+
+
+def _token_head_backward(ctx, g_out, _g_dlp):
+    dlp, = ctx.saved_tensors
+    return (scale(g_out[:1], dlp), ) + (None, ) * 7
+
+
+token_head_fwd.register_autograd(_token_head_backward, setup_context=_token_head_setup)
+
+
+@torch.library.custom_op('b200rl::ppo_lm_fwd', mutates_args=())
+def ppo_lm_fwd(logit_new: Tensor, logit_old: Tensor, logit_pre: Optional[Tensor], action: Tensor, adv: Tensor,
+               weight: Optional[Tensor], clip_ratio: float, dual_clip: float, kl_type: int,
+               entropy: bool) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """ppo_policy_error on token rows -> (policy / entropy / kl / approx_kl / clipfrac, and per row: logsumexp, entropy
+    (empty without ``entropy``), the policy term's unit coefficient, the kl term's (empty without logit_pre))"""
+    xs = [ops.logits_c(x) if x is not None else None for x in (logit_new, logit_old, logit_pre)]
+    out, lse, ent, dpol, dkl = ops.ppo_lm_fwd_(xs[0], xs[1], xs[2], action, adv, weight, ops.logit_dtype(xs[0]),
+                                               clip_ratio, dual_clip, kl_type, entropy, None, None, None)
+    return out, lse, ent if ent is not None else _empty(out), dpol, dkl if dkl is not None else _empty(out)
+
+
+@ppo_lm_fwd.register_fake
+def _(logit_new, logit_old, logit_pre, action, adv, weight, clip_ratio, dual_clip, kl_type, entropy):
+    rows = _rows(logit_new)
+    return (_f32(logit_new, 5), _f32(logit_new, rows), _f32(logit_new, rows if entropy else 0), _f32(logit_new, rows),
+            _f32(logit_new, rows if logit_pre is not None else 0))
+
+
+@torch.library.custom_op('b200rl::ppo_lm_bwd', mutates_args=())
+def ppo_lm_bwd(logit_new: Tensor, action: Tensor, weight: Optional[Tensor], lse: Tensor, ent: Tensor, dpol: Tensor,
+               dkl: Tensor, g_out: Tensor) -> Tensor:
+    """-> d / d logit_new for the upstream gradients g_out[0:3] of policy, entropy and kl loss"""
+    x = ops.logits_c(logit_new)
+    keep, upstream = _upstream(g_out, 3)
+    return ops.ppo_lm_bwd_(ops.logit_dtype(x), x, action, weight, lse, ent if ent.numel() else None, dpol,
+                           dkl if dkl.numel() else None, upstream, None, None, torch.empty_like(logit_new))
+
+
+@ppo_lm_bwd.register_fake
+def _(logit_new, *args):
+    return torch.empty_like(logit_new)
+
+
+def _ppo_lm_setup(ctx, inputs, output):
+    ctx.save_for_backward(inputs[0], inputs[3], inputs[5], *output[1:])
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[1:])
+
+
+def _ppo_lm_backward(ctx, g_out, *_):
+    if g_out is None:
+        return (None, ) * 10
+    return (ppo_lm_bwd(*ctx.saved_tensors, g_out), ) + (None, ) * 9
+
+
+ppo_lm_fwd.register_autograd(_ppo_lm_backward, setup_context=_ppo_lm_setup)
+
+
+@torch.library.custom_op('b200rl::a2c_lm_fwd', mutates_args=())
+def a2c_lm_fwd(logit: Tensor, value: Tensor, action: Tensor, adv: Tensor, return_: Tensor,
+               weight: Optional[Tensor]) -> tuple[Tensor, Tensor]:
+    """a2c_error on token rows, value fp32 -> (policy / value / entropy loss, (4, rows): per row logsumexp, entropy, the
+    policy term's unit coefficient, d value_loss / d value)"""
+    x = ops.logits_c(logit)
+    return ops.a2c_lm_fwd_(x, value, action, adv, return_, weight, ops.logit_dtype(x), None, None, None, None)
+
+
+@a2c_lm_fwd.register_fake
+def _(logit, value, action, adv, return_, weight):
+    return _f32(logit, 3), _f32(logit, (4, _rows(logit)))
+
+
+@torch.library.custom_op('b200rl::a2c_lm_bwd', mutates_args=())
+def a2c_lm_bwd(logit: Tensor, value: Tensor, action: Tensor, weight: Optional[Tensor], per_row: Tensor,
+               g_out: Tensor) -> tuple[Tensor, Tensor]:
+    """-> (d / d logit, d / d value) for the upstream gradients g_out[0:3] of policy, value and entropy loss"""
+    x = ops.logits_c(logit)
+    keep, upstream = _upstream(g_out, 3)
+    return ops.a2c_lm_bwd_(ops.logit_dtype(x), x, action, weight, *per_row.unbind(0), upstream, None, None,
+                           torch.empty_like(logit), torch.empty_like(value))
+
+
+@a2c_lm_bwd.register_fake
+def _(logit, value, *args):
+    return torch.empty_like(logit), torch.empty_like(value)
+
+
+def _a2c_lm_setup(ctx, inputs, output):
+    ctx.save_for_backward(inputs[0], inputs[1], inputs[2], inputs[5], output[1])
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(output[1])
+
+
+def _a2c_lm_backward(ctx, g_out, _g_per_row):
+    if g_out is None:
+        return (None, ) * 6
+    grad_logit, grad_value = a2c_lm_bwd(*ctx.saved_tensors, g_out)
+    return (grad_logit, grad_value) + (None, ) * 4
+
+
+a2c_lm_fwd.register_autograd(_a2c_lm_backward, setup_context=_a2c_lm_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # what rl_utils calls while compiling: the autograd.Function signatures of ops, on the ops above
 # ---------------------------------------------------------------------------------------------------------------------
 def _want_grad(*xs):
@@ -488,4 +736,38 @@ def vtrace(target_output, value, behaviour_output, action, reward, weight, gamma
     """-> (policy_loss, value_loss, entropy_loss)"""
     out = vtrace_loss(target_output, value, behaviour_output, action, reward, weight, gamma, lambda_, rho_clip, c_clip,
                      rho_pg_clip, _want_grad(target_output, value))[0]
+    return out[0], out[1], out[2]
+
+
+def ppo_value(value_new, value_old, return_, weight, clip_ratio, use_value_clip):
+    return ppo_value_fwd(value_new, value_old, return_, weight, float(clip_ratio), bool(use_value_clip),
+                         _want_grad(value_new))[0]
+
+
+def token_logp(logits, index):
+    """-> log p(index) per row, as TokenLogProbFunction"""
+    return token_logp_op(logits, index)[0]
+
+
+def lm_policy(logit_new, logit_old, logit_ref, action, side, weight, mode, clip_ratio, beta):
+    """-> (loss, approx_kl, clipfrac), as GRPOFunction / RLOOFunction"""
+    out = lm_policy_fwd(logit_new, logit_old, logit_ref, action, side, weight, mode, clip_ratio, beta)[0]
+    return out[0], out[1], out[2]
+
+
+def token_head(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
+    """-> (loss, approx_kl, clipfrac), as ops.token_head_"""
+    out = token_head_fwd(lp_new, lp_old, lp_ref, adv, reward, weight, float(clip_ratio), float(beta))[0]
+    return out[0], out[1], out[2]
+
+
+def ppo_lm(logit_new, logit_old, logit_pre, action, adv, weight, clip_ratio, dual_clip, kl_type, entropy):
+    """-> (policy_loss, entropy_loss, kl_div, the five floats), as PPOLMFunction"""
+    out = ppo_lm_fwd(logit_new, logit_old, logit_pre, action, adv, weight, clip_ratio, dual_clip, kl_type, entropy)[0]
+    return out[0], out[1], out[2], out
+
+
+def a2c_lm(logit, value, action, adv, return_, weight):
+    """-> (policy_loss, value_loss, entropy_loss), as A2CLMFunction"""
+    out = a2c_lm_fwd(logit, value, action, adv, return_, weight)[0]
     return out[0], out[1], out[2]
