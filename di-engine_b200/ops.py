@@ -326,17 +326,33 @@ def gae_returns_norm_(value, next_value, reward, done, traj_flag, gamma, lambda_
     return adv, vout, rout, stats, astats
 
 
+def value_map_fwd_(x, mode):
+    """The forward launch of symlog / inv_symlog (ValueMapFunction and the ``b200rl::value_map`` custom op)."""
+    y = torch.empty_like(x)
+    if x.numel():
+        with on_device(x.device):
+            rc = lib().b200rl_value_map_fwd(mode, ptr(x), x.numel(), ptr(y), stream_ptr())
+        _lib.check(rc, 'b200rl_value_map_fwd')
+    return y
+
+
+def value_map_bwd_(x, g, mode):
+    """The backward launch of symlog / inv_symlog: d / d x for the contiguous fp32 upstream gradient ``g``."""
+    dx = torch.empty_like(x)
+    if x.numel():
+        with on_device(x.device):
+            rc = lib().b200rl_value_map_bwd(mode, ptr(x), ptr(g), x.numel(), ptr(dx), stream_ptr())
+        _lib.check(rc, 'b200rl_value_map_bwd')
+    return dx
+
+
 class ValueMapFunction(torch.autograd.Function):
     """symlog (mode 0) / inv_symlog (mode 1) of ding/rl_utils/value_rescale.py:37-66 on a contiguous fp32 CUDA tensor; the
     backward is torch's autograd of the reference expression (include/b200rl.h)."""
 
     @staticmethod
     def forward(ctx, x, mode):
-        y = torch.empty_like(x)
-        if x.numel():
-            with on_device(x.device):
-                rc = lib().b200rl_value_map_fwd(mode, ptr(x), x.numel(), ptr(y), stream_ptr())
-            _lib.check(rc, 'b200rl_value_map_fwd')
+        y = value_map_fwd_(x, mode)
         ctx.mode = mode
         ctx.save_for_backward(x)
         return y
@@ -344,13 +360,7 @@ class ValueMapFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         x, = ctx.saved_tensors
-        g = f32c(g, 'grad')
-        dx = torch.empty_like(x)
-        if x.numel():
-            with on_device(x.device):
-                rc = lib().b200rl_value_map_bwd(ctx.mode, ptr(x), ptr(g), x.numel(), ptr(dx), stream_ptr())
-            _lib.check(rc, 'b200rl_value_map_bwd')
-        return dx, None
+        return value_map_bwd_(x, f32c(g, 'grad'), ctx.mode), None
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -785,19 +795,9 @@ class QuantileTDFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, next_n_q, action, next_n_action, reward, done, tau, weight, value_gamma, vg_stride, B, N, n_tau,
                 n_tau_prime, nstep, gamma, q_strides, nq_strides, tau_strides, form, kappa):
-        dev = q.device
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        td = torch.empty(B, dtype=torch.float32, device=dev)
-        dtheta = torch.empty(B, n_tau, dtype=torch.float32, device=dev)
-        grad_unit = torch.empty_like(q) if ctx.needs_input_grad[0] else None
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_quantile_td_fwd(
-                ptr(q), ptr(next_n_q), ptr(action), ptr(next_n_action), ptr(reward), ptr(done), ptr(tau), ptr(weight),
-                ptr(value_gamma), vg_stride, B, N, n_tau, n_tau_prime, nstep, gamma, *q_strides, *nq_strides, *tau_strides,
-                form, kappa, ptr(loss), ptr(td), ptr(dtheta), ptr(grad_unit), ptr(ws), ws.numel() * 4, stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_quantile_td_fwd')
+        loss, td, dtheta, grad_unit = quantile_fwd_(q, next_n_q, action, next_n_action, reward, done, tau, weight,
+                                                    value_gamma, vg_stride, B, N, n_tau, n_tau_prime, nstep, gamma,
+                                                    q_strides, nq_strides, tau_strides, form, kappa, ctx.needs_input_grad[0])
         ctx.save_for_backward(dtheta, action, weight)
         ctx.cfg = (B, N, n_tau, q_strides)
         ctx.q_shape = q.shape
@@ -814,11 +814,36 @@ class QuantileTDFunction(torch.autograd.Function):
         keep, (pg, ptd) = _grads(g_loss, g_td)
         grad_q, skip = _unit_grad(ctx, (g_td, ),
                                   lambda: torch.empty(ctx.q_shape, dtype=torch.float32, device=dtheta.device))
-        with on_device(dtheta.device):
-            rc = lib().b200rl_quantile_td_bwd(ptr(dtheta), ptr(weight), ptr(action), pg, ptd, B, N, n_tau,
-                                              *q_strides, skip, ptr(grad_q), stream_ptr())
-        _lib.check(rc, 'b200rl_quantile_td_bwd')
-        return (grad_q, ) + (None, ) * 20
+        return (quantile_bwd_(dtheta, weight, action, pg, ptd, B, N, n_tau, q_strides, skip, grad_q), ) + (None, ) * 20
+
+
+def quantile_fwd_(q, next_n_q, action, next_n_action, reward, done, tau, weight, value_gamma, vg_stride, B, N, n_tau,
+                  n_tau_prime, nstep, gamma, q_strides, nq_strides, tau_strides, form, kappa, want_grad):
+    """The forward launch of the quantile TD family (QuantileTDFunction and the ``b200rl::quantile_fwd`` custom op).
+    -> (loss, td, dtheta, grad_unit or None)."""
+    dev = q.device
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    td = torch.empty(B, dtype=torch.float32, device=dev)
+    dtheta = torch.empty(B, n_tau, dtype=torch.float32, device=dev)
+    grad_unit = torch.empty_like(q) if want_grad else None
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_quantile_td_fwd(
+            ptr(q), ptr(next_n_q), ptr(action), ptr(next_n_action), ptr(reward), ptr(done), ptr(tau), ptr(weight),
+            ptr(value_gamma), vg_stride, B, N, n_tau, n_tau_prime, nstep, gamma, *q_strides, *nq_strides, *tau_strides,
+            form, kappa, ptr(loss), ptr(td), ptr(dtheta), ptr(grad_unit), ptr(ws), ws.numel() * 4, stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_quantile_td_fwd')
+    return loss, td, dtheta, grad_unit
+
+
+def quantile_bwd_(dtheta, weight, action, pg, ptd, B, N, n_tau, q_strides, skip, grad_q):
+    """The backward launch of the quantile TD family into ``grad_q`` (``pg`` / ``ptd`` / ``skip`` as qntd_bwd_)."""
+    with on_device(dtheta.device):
+        rc = lib().b200rl_quantile_td_bwd(ptr(dtheta), ptr(weight), ptr(action), pg, ptd, B, N, n_tau, *q_strides, skip,
+                                          ptr(grad_q), stream_ptr())
+    _lib.check(rc, 'b200rl_quantile_td_bwd')
+    return grad_q
 
 
 class FQFFractionFunction(torch.autograd.Function):
@@ -1187,46 +1212,61 @@ class PPOContinuousFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight, S,
                 D, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, factor=None):
-        dev = mu.device
         ctx.factor = factor  # happo_error_continuous's per-sample factor (S,) or None; kept alive for the backward launch
-        out = torch.empty(8, dtype=torch.float32, device=dev)
-        want = any(ctx.needs_input_grad[:3])
-        gm = torch.empty_like(mu) if want else None
-        gs = torch.empty_like(sigma) if want else None
-        gv = torch.empty_like(value_new) if want else None
-        g_used = torch.empty(4, dtype=torch.float32, device=dev) if want else None
-        ctx.hint = ppo_hint(dev, hint_kind)
-        ctx.args = (ptr(factor), S, D, clip_ratio, use_value_clip, dual_clip, kl_type)
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_ppo_continuous_fwd_grad(
-                ptr(mu), ptr(sigma), ptr(mu_old), ptr(sigma_old), ptr(mu_pre), ptr(sigma_pre), ptr(action), ptr(value_new),
-                ptr(value_old), ptr(adv), ptr(return_), ptr(weight), *ctx.args, ptr(ctx.hint) if want else None, 0, None,
-                None, None, None, ptr(g_used), None, ptr(out), ptr(gm), ptr(gs), ptr(gv), ptr(ws), ws.numel() * 4,
-                stream_ptr())
-        _lib.check(rc, 'b200rl_ppo_continuous_fwd_grad')
-        ctx.save_for_backward(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_,
-                              weight)
-        ctx.spec = (gm, gs, gv, g_used) if want else None
+        ctx.hint_kind = hint_kind
+        ctx.cfg = (factor, S, D, clip_ratio, use_value_clip, dual_clip, kl_type)
+        saved = (mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight)
+        out, ctx.spec = ppoc_fwd_(saved, ctx.cfg, hint_kind, any(ctx.needs_input_grad[:3]))
+        ctx.save_for_backward(*saved)
         ctx.set_materialize_grads(False)
         ctx.mark_non_differentiable(out)
         return out[0], out[1], out[2], out[3], out
 
     @staticmethod
     def backward(ctx, g_p, g_v, g_e, g_k, _g_out):
-        (mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_,
-         weight) = ctx.saved_tensors
-        keep, (pp, pv, pe, pk) = _grads(g_p, g_v, g_e, g_k)
-        gm, gs, gv, g_used = _forward_grads(ctx) or (torch.empty_like(mu), torch.empty_like(sigma),
-                                                     torch.empty_like(value_new), None)
-        with on_device(mu.device):
-            ws = workspace(mu.device)
-            rc = lib().b200rl_ppo_continuous_fwd_grad(
-                ptr(mu), ptr(sigma), ptr(mu_old), ptr(sigma_old), ptr(mu_pre), ptr(sigma_pre), ptr(action), ptr(value_new),
-                ptr(value_old), ptr(adv), ptr(return_), ptr(weight), *ctx.args, None, 1, pp, pv, pe, pk, ptr(g_used),
-                ptr(ctx.hint), None, ptr(gm), ptr(gs), ptr(gv), ptr(ws), ws.numel() * 4, stream_ptr())
-        _lib.check(rc, 'b200rl_ppo_continuous_fwd_grad(verify)')
-        return (gm, gs, gv) + (None, ) * 17
+        keep, upstream = _grads(g_p, g_v, g_e, g_k)
+        return ppoc_bwd_(ctx.saved_tensors, ctx.cfg, upstream, _forward_grads(ctx), ctx.hint_kind) + (None, ) * 17
+
+
+def ppoc_fwd_(saved, cfg, hint_kind, want_grad):
+    """The forward launch of ppo_error_continuous (PPOContinuousFunction and the ``b200rl::ppoc_loss`` custom op):
+    ``saved`` = (mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight),
+    ``cfg`` = (factor, S, D, clip_ratio, use_value_clip, dual_clip, kl_type).  -> (the 8-float result vector, the
+    forward-written (grad_mu, grad_sigma, grad_value, g_used) or None without ``want_grad``)."""
+    mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight = saved
+    dev = mu.device
+    out = torch.empty(8, dtype=torch.float32, device=dev)
+    gm = torch.empty_like(mu) if want_grad else None
+    gs = torch.empty_like(sigma) if want_grad else None
+    gv = torch.empty_like(value_new) if want_grad else None
+    g_used = torch.empty(4, dtype=torch.float32, device=dev) if want_grad else None
+    hint = ppo_hint(dev, hint_kind)
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_ppo_continuous_fwd_grad(
+            ptr(mu), ptr(sigma), ptr(mu_old), ptr(sigma_old), ptr(mu_pre), ptr(sigma_pre), ptr(action), ptr(value_new),
+            ptr(value_old), ptr(adv), ptr(return_), ptr(weight), ptr(cfg[0]), *cfg[1:], ptr(hint) if want_grad else None,
+            0, None, None, None, None, ptr(g_used), None, ptr(out), ptr(gm), ptr(gs), ptr(gv), ptr(ws), ws.numel() * 4,
+            stream_ptr())
+    _lib.check(rc, 'b200rl_ppo_continuous_fwd_grad')
+    return out, (gm, gs, gv, g_used) if want_grad else None
+
+
+def ppoc_bwd_(saved, cfg, upstream, spec, hint_kind):
+    """The verify launch of ppo_error_continuous (arguments as ppoc_fwd_; ``upstream`` the four device pointers of the
+    upstream gradients, None = 0).  With ``spec`` (the forward-written gradients) it verifies them on the device and
+    recomputes them in place on a mismatch; without, it computes into fresh buffers.  -> (grad_mu, grad_sigma, grad_value)."""
+    mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight = saved
+    dev = mu.device
+    gm, gs, gv, g_used = spec or (torch.empty_like(mu), torch.empty_like(sigma), torch.empty_like(value_new), None)
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_ppo_continuous_fwd_grad(
+            ptr(mu), ptr(sigma), ptr(mu_old), ptr(sigma_old), ptr(mu_pre), ptr(sigma_pre), ptr(action), ptr(value_new),
+            ptr(value_old), ptr(adv), ptr(return_), ptr(weight), ptr(cfg[0]), *cfg[1:], None, 1, *upstream, ptr(g_used),
+            ptr(ppo_hint(dev, hint_kind)), None, ptr(gm), ptr(gs), ptr(gv), ptr(ws), ws.numel() * 4, stream_ptr())
+    _lib.check(rc, 'b200rl_ppo_continuous_fwd_grad(verify)')
+    return gm, gs, gv
 
 
 class ImpalaMaskFunction(torch.autograd.Function):

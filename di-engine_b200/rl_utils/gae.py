@@ -94,8 +94,11 @@ def gae_returns(data: namedtuple, gamma: float = 0.99, lambda_: float = 0.97, va
     d = ops.f32c(ops.to_device(done.detach(), dev), 'done') if done is not None else None
     tf = ops.f32c(ops.to_device(traj_flag.detach(), dev), 'traj_flag') if traj_flag is not None else None
     vs = 0.0 if value_norm_std is None else float(value_norm_std)
-    adv, unnorm, vout, rout, stats, astats = ops.gae_returns_(v, nv, r, d, tf, gamma, lambda_, 1, vs, True, True,
-                                                              want_adv_stats=True)
+    if torch.compiler.is_compiling():
+        adv, unnorm, vout, rout, stats, astats = torch_ops.gae_returns(v, nv, r, d, tf, gamma, lambda_, vs)
+    else:
+        adv, unnorm, vout, rout, stats, astats = ops.gae_returns_(v, nv, r, d, tf, gamma, lambda_, 1, vs, True, True,
+                                                                  want_adv_stats=True)
     if vs == 0.0:
         vout, rout = v, unnorm
     out = gae_returns_out(adv, vout, rout, unnorm, stats, astats)
@@ -168,8 +171,12 @@ def ppof_gae_returns(data: namedtuple, gamma: float = 0.99, lambda_: float = 0.9
         sigma = ops.f32c(ops.to_device(popart_sigma.detach(), dev), 'popart_sigma').reshape(-1)
         if mu.numel() != 1 or sigma.numel() != 1:
             raise ValueError("ppof_gae_returns: popart_mu / popart_sigma must hold one float each (a single-output PopArt head)")
-    adv, vout, rout, stats, astats = ops.gae_returns_norm_(v, nv, r, d, tf, gamma, lambda_, value_norm, std, mu, sigma,
-                                                           value_norm == 'baseline')
+    if torch.compiler.is_compiling():
+        adv, vout, rout, stats, astats = torch_ops.ppof_gae_returns(v, nv, r, d, tf, gamma, lambda_, value_norm, std, mu,
+                                                                    sigma)
+    else:
+        adv, vout, rout, stats, astats = ops.gae_returns_norm_(v, nv, r, d, tf, gamma, lambda_, value_norm, std, mu, sigma,
+                                                               value_norm == 'baseline')
     out = ppof_gae_returns_out(adv.reshape(value.shape), vout.reshape(value.shape), rout.reshape(value.shape), stats, astats)
     if host_out:
         out = ppof_gae_returns_out(*[None if t is None else t.cpu() for t in out])

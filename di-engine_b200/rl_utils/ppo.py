@@ -58,7 +58,10 @@ def normalize_advantage(adv: torch.Tensor) -> torch.Tensor:
     dev = ops.compute_device(adv)
     host_out = not adv.is_cuda
     a = ops.f32c(ops.to_device(adv.detach(), dev), 'adv')
-    out = ops.normalize_(a, ops.adv_stats_(a))
+    if torch.compiler.is_compiling():
+        out = torch_ops.normalize(a, torch_ops.adv_stats(a))
+    else:
+        out = ops.normalize_(a, ops.adv_stats_(a))
     return out.cpu() if host_out else out
 
 
@@ -154,7 +157,7 @@ def _ppo_error(data, clip_ratio, use_value_clip, dual_clip, kl_type, _hint_kind,
     stats = None
     if adv_norm:
         if adv_stats is None:
-            stats = ops.adv_stats_(ad)
+            stats = torch_ops.adv_stats(ad) if torch.compiler.is_compiling() else ops.adv_stats_(ad)
         else:
             stats = ops.f32c(ops.to_device(adv_stats.detach(), ad.device), 'adv_stats').reshape(-1)
             if stats.numel() != 2:
@@ -233,14 +236,20 @@ def _ppo_error_continuous(data, clip_ratio, use_value_clip, dual_clip, kl_type, 
              stage(return_.detach(), 'return_', S),
              stage(weight.detach(), 'weight', S) if weight is not None else None]
     fac = stage(factor.detach(), 'factor', S).reshape(-1) if factor is not None else None
-    p, v, e, k, out = ops.PPOContinuousFunction.apply(
-        *args, S, D, float(clip_ratio), 1 if use_value_clip else 0, float(dual_clip) if dual_clip is not None else 0.0,
-        _KL_TYPES.get(kl_type, 1), hint_kind, fac)
-    if LAZY_INFO:
-        info = ppo_info(out[4], out[5])
+    args += [S, D, float(clip_ratio), 1 if use_value_clip else 0, float(dual_clip) if dual_clip is not None else 0.0,
+             _KL_TYPES.get(kl_type, 1), hint_kind, fac]
+    if torch.compiler.is_compiling():
+        out = torch_ops.ppo_continuous(*args)
+        p, v, e, k = out[0], out[1], out[2], out[3]
+        # the reference's two .item() calls (ppo.py:366-368): what a traced graph can take
+        info = ppo_info(out[4].detach(), out[5].detach()) if LAZY_INFO else ppo_info(out[4].item(), out[5].item())
     else:
-        approx_kl, clipfrac = out[4:6].tolist()
-        info = ppo_info(approx_kl, clipfrac)
+        p, v, e, k, out = ops.PPOContinuousFunction.apply(*args)
+        if LAZY_INFO:
+            info = ppo_info(out[4], out[5])
+        else:
+            approx_kl, clipfrac = out[4:6].tolist()
+            info = ppo_info(approx_kl, clipfrac)
     if host_out:
         p, v, e, k = p.cpu(), v.cpu(), e.cpu(), k.cpu()
     return ppo_loss(p, v, e, k), info

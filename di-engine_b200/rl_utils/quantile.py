@@ -7,8 +7,8 @@ from typing import Optional
 
 import torch
 
-from .. import ops
-from .td import _value_gamma_arg
+from .. import ops, torch_ops
+from .td import _value_gamma_arg, _value_gamma_op_arg
 
 qrdqn_nstep_td_data = namedtuple(
     'qrdqn_nstep_td_data', ['q', 'next_n_q', 'action', 'next_n_action', 'reward', 'done', 'tau', 'weight']
@@ -56,6 +56,11 @@ def _run(q, next_n_q, action, next_n_action, reward, done, tau, weight, gamma, n
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight').reshape(-1)
         if w.numel() != B:
             raise ValueError("weight must have B=%d elements" % B)
+    if torch.compiler.is_compiling():
+        vg, vg_stride = _value_gamma_op_arg(value_gamma, B, dev)
+        loss, td = torch_ops.quantile_td(qd, nq, act, nact, r, d, t, w, vg, vg_stride, B, N, n_tau, n_tau_p, nstep,
+                                         float(gamma), form, float(kappa))
+        return (loss.cpu(), td.cpu()) if host_out else (loss, td)
     vg, vg_stride = _value_gamma_arg(value_gamma, B, dev)
     loss, td = ops.QuantileTDFunction.apply(
         qd, nq, act, nact, r, d, t, w, vg, vg_stride, B, N, n_tau, n_tau_p, nstep, float(gamma),

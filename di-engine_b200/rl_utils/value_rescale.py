@@ -8,7 +8,7 @@ forward and backward.
 """
 import torch
 
-from .. import ops
+from .. import ops, torch_ops
 
 
 def value_transform(x: torch.Tensor, eps: float = 1e-2) -> torch.Tensor:
@@ -28,7 +28,8 @@ def _value_map(x, mode, name):
         raise TypeError("di_engine_b200: %s takes a float32 tensor (got %s); the CUDA path computes in fp32" %
                         (name, getattr(x, 'dtype', type(x).__name__)))
     dev = ops.compute_device(x)
-    y = ops.ValueMapFunction.apply(ops.to_device(x, dev).contiguous(), mode)
+    xd = ops.to_device(x, dev).contiguous()
+    y = torch_ops.value_map(xd, mode) if torch.compiler.is_compiling() else ops.ValueMapFunction.apply(xd, mode)
     return y if x.is_cuda else y.cpu()
 
 

@@ -2,8 +2,10 @@
 trace the eight operators of the reference's plugin boundary (gae, ppo_error, q_nstep_td_error,
 q_nstep_td_error_with_rescale, dist_nstep_td_error, td_lambda_error, upgo_loss, vtrace_error_discrete_action) and the
 language-model losses on (B, S, V) logits (grpo_policy_error, rloo_policy_error, the log-prob methods, ppo_policy_error /
-ppo_error / a2c_error on token rows, ppo_value_error) without a graph break, and ``mode="reduce-overhead"`` can replay a
-compiled learner step as a CUDA graph.
+ppo_error / a2c_error on token rows, ppo_value_error), the advantage recomputes (gae_returns, ppof_gae_returns,
+normalize_advantage, ppo_error_adv_norm), symlog / inv_symlog, the quantile TD losses (QR-DQN, IQN, FQF) and the
+continuous-action PPO losses without a graph break, and ``mode="reduce-overhead"`` can replay a compiled learner step as
+a CUDA graph.
 
 Each op's implementation is the launch function ``ops`` runs in eager mode; ``rl_utils`` calls the wrappers at the bottom
 of this module only while ``torch.compiler.is_compiling()``.  The schemas hold tensors and scalars only: the workspace, the
@@ -684,6 +686,230 @@ a2c_lm_fwd.register_autograd(_a2c_lm_backward, setup_context=_a2c_lm_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# the advantage statistics of PPOPolicy / PPOFPolicy (csrc/policy.cu): no gradient, as in the reference
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::gae_returns', mutates_args=())
+def gae_returns_op(value: Tensor, next_value: Tensor, reward: Tensor, done: Optional[Tensor], traj_flag: Optional[Tensor],
+                   gamma: float, lambda_: float, vscale: float) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """gae_returns -> (adv, unnormalized return, value_out, return_out, return_stats, adv_stats); value_out / return_out
+    are empty when ``vscale`` is 0 (no value_norm).  The inputs are not modified."""
+    adv, unnorm, vout, rout, stats, astats = ops.gae_returns_(value, next_value, reward, done, traj_flag, gamma, lambda_, 1,
+                                                              vscale, True, True, want_adv_stats=True)
+    return (adv, unnorm, vout if vout is not None else _empty(adv), rout if rout is not None else _empty(adv), stats,
+            astats)
+
+
+@gae_returns_op.register_fake
+def _(value, next_value, reward, done, traj_flag, gamma, lambda_, vscale):
+    scaled = (lambda: torch.empty_like(value)) if vscale != 0.0 else (lambda: _empty(value))
+    return (torch.empty_like(value), torch.empty_like(value), scaled(), scaled(), _f32(value, 3), _f32(value, 2))
+
+
+@torch.library.custom_op('b200rl::gae_returns_norm', mutates_args=())
+def gae_returns_norm(value: Tensor, next_value: Tensor, reward: Tensor, done: Optional[Tensor],
+                     traj_flag: Optional[Tensor], gamma: float, lambda_: float, value_norm: str, std: float,
+                     mu: Optional[Tensor], sigma: Optional[Tensor]) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """ppof_gae_returns -> (adv, value_out, return_out, return_stats (empty unless 'baseline'), adv_stats)"""
+    adv, vout, rout, stats, astats = ops.gae_returns_norm_(value, next_value, reward, done, traj_flag, gamma, lambda_,
+                                                           value_norm, std, mu, sigma, value_norm == 'baseline')
+    return adv, vout, rout, stats if stats is not None else _empty(adv), astats
+
+
+@gae_returns_norm.register_fake
+def _(value, next_value, reward, done, traj_flag, gamma, lambda_, value_norm, std, mu, sigma):
+    return (torch.empty_like(value), torch.empty_like(value), torch.empty_like(value),
+            _f32(value, 3 if value_norm == 'baseline' else 0), _f32(value, 2))
+
+
+@torch.library.custom_op('b200rl::adv_stats', mutates_args=())
+def adv_stats(x: Tensor) -> Tensor:
+    """{mean, std (unbiased) + 1e-8} of ``x``"""
+    return ops.adv_stats_(x)
+
+
+@adv_stats.register_fake
+def _(x):
+    return _f32(x, 2)
+
+
+@torch.library.custom_op('b200rl::normalize', mutates_args=())
+def normalize(x: Tensor, stats: Tensor) -> Tensor:
+    return ops.normalize_(x, stats)
+
+
+@normalize.register_fake
+def _(x, stats):
+    return torch.empty_like(x)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# symlog / inv_symlog
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::value_map', mutates_args=())
+def value_map(x: Tensor, mode: int) -> Tensor:
+    """symlog (``mode`` 0) or inv_symlog (1) of a contiguous fp32 tensor"""
+    return ops.value_map_fwd_(x, mode)
+
+
+@value_map.register_fake
+def _(x, mode):
+    return torch.empty_like(x)
+
+
+@torch.library.custom_op('b200rl::value_map_bwd', mutates_args=())
+def value_map_bwd(x: Tensor, g: Tensor, mode: int) -> Tensor:
+    return ops.value_map_bwd_(x, ops.f32c(g, 'grad'), mode)
+
+
+@value_map_bwd.register_fake
+def _(x, g, mode):
+    return torch.empty_like(x)
+
+
+def _value_map_setup(ctx, inputs, output):
+    ctx.save_for_backward(inputs[0])
+    ctx.mode = inputs[1]
+
+
+def _value_map_backward(ctx, g):
+    x, = ctx.saved_tensors
+    return value_map_bwd(x, g, ctx.mode), None
+
+
+value_map.register_autograd(_value_map_backward, setup_context=_value_map_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# qrdqn / iqn / fqf_nstep_td_error: the op reads the element strides of (sample, quantile[, action]) from its tensors
+# ---------------------------------------------------------------------------------------------------------------------
+QUANTILE_AXES = ((0, 2, 1), (1, 0, 2), (0, 1, 2))  # the (sample, quantile, action) axes of q per form: QR-DQN, IQN, FQF
+
+
+def _quantile_strides(t, form):
+    return tuple(t.stride(a) for a in QUANTILE_AXES[form])
+
+
+@torch.library.custom_op('b200rl::quantile_fwd', mutates_args=())
+def quantile_fwd(q: Tensor, next_n_q: Tensor, action: Tensor, next_n_action: Tensor, reward: Tensor, done: Tensor,
+                 tau: Tensor, weight: Optional[Tensor], value_gamma: Optional[Tensor], value_gamma_scalar: Optional[float],
+                 vg_stride: int, B: int, N: int, n_tau: int, n_tau_prime: int, nstep: int, gamma: float, form: int,
+                 kappa: float, want_grad: bool) -> tuple[Tensor, Tensor, Tensor, Tensor]:
+    """-> (loss, td, dtheta, grad_unit); grad_unit is empty without ``want_grad``.  ``tau`` (B, n_tau) may be any strided
+    view, as in eager mode."""
+    if value_gamma_scalar is not None:
+        value_gamma = ops.const_scalar(value_gamma_scalar, q.device)
+    loss, td, dtheta, grad_unit = ops.quantile_fwd_(
+        q, next_n_q, action, next_n_action, reward, done, tau, weight, value_gamma, vg_stride, B, N, n_tau, n_tau_prime,
+        nstep, gamma, _quantile_strides(q, form), _quantile_strides(next_n_q, form), (tau.stride(0), tau.stride(1)), form,
+        kappa, want_grad)
+    return loss, td, dtheta, grad_unit if grad_unit is not None else _empty(loss)
+
+
+@quantile_fwd.register_fake
+def _(q, next_n_q, action, next_n_action, reward, done, tau, weight, value_gamma, value_gamma_scalar, vg_stride, B, N,
+      n_tau, n_tau_prime, nstep, gamma, form, kappa, want_grad):
+    loss = q.new_empty(())
+    return loss, q.new_empty(B), q.new_empty(B, n_tau), torch.empty_like(q) if want_grad else _empty(loss)
+
+
+@torch.library.custom_op('b200rl::quantile_bwd', mutates_args=())
+def quantile_bwd(dtheta: Tensor, weight: Optional[Tensor], action: Tensor, g_loss: Optional[Tensor],
+                 g_td: Optional[Tensor], grad_unit: Tensor, B: int, N: int, n_tau: int, form: int) -> Tensor:
+    """-> d / d q; verifies a copy of the forward-written unit gradient when only the loss has a gradient"""
+    kl, pg = _one(g_loss)
+    kt, ptd = _one(g_td)
+    skip = 1 if g_td is None else 0
+    grad = grad_unit.clone() if skip else torch.empty_like(grad_unit)
+    return ops.quantile_bwd_(dtheta, weight, action, pg, ptd, B, N, n_tau, _quantile_strides(grad, form), skip, grad)
+
+
+@quantile_bwd.register_fake
+def _(dtheta, weight, action, g_loss, g_td, grad_unit, B, N, n_tau, form):
+    return torch.empty_like(grad_unit)
+
+
+def _quantile_setup(ctx, inputs, output):
+    ctx.save_for_backward(output[2], inputs[7], inputs[2], output[3])
+    ctx.cfg = (inputs[11], inputs[12], inputs[13], inputs[17])
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[2:])
+
+
+def _quantile_backward(ctx, g_loss, g_td, *_):
+    if g_loss is None and g_td is None:
+        return (None, ) * 20
+    dtheta, weight, action, grad_unit = ctx.saved_tensors
+    return (quantile_bwd(dtheta, weight, action, g_loss, g_td, grad_unit, *ctx.cfg), ) + (None, ) * 19
+
+
+quantile_fwd.register_autograd(_quantile_backward, setup_context=_quantile_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# ppo_error_continuous and its policy-only / HAPPO call sites (csrc/heads.cu): the forward launch always writes the
+# gradients for the call site's record when a gradient is wanted, so the backward op always verifies a copy
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::ppoc_loss', mutates_args=())
+def ppoc_loss(mu: Tensor, sigma: Tensor, value_new: Tensor, mu_old: Tensor, sigma_old: Tensor, mu_pre: Optional[Tensor],
+              sigma_pre: Optional[Tensor], action: Tensor, value_old: Tensor, adv: Tensor, return_: Tensor,
+              weight: Optional[Tensor], factor: Optional[Tensor], S: int, D: int, clip_ratio: float, use_value_clip: int,
+              dual_clip: float, kl_type: int, hint_kind: str,
+              want_grad: bool) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """-> (the six floats the launch writes: policy, value, entropy, kl loss, approx_kl, clipfrac; grad_mu, grad_sigma,
+    grad_value, g_used); the last four are empty without ``want_grad``"""
+    saved = (mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight)
+    out, spec = ops.ppoc_fwd_(saved, (factor, S, D, clip_ratio, use_value_clip, dual_clip, kl_type), hint_kind, want_grad)
+    out = out[:6]
+    if not want_grad:
+        return (out, ) + (_empty(out), ) * 4
+    return (out, ) + spec
+
+
+@ppoc_loss.register_fake
+def _(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight, factor, S, D,
+      clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, want_grad):
+    out = mu.new_empty(6)
+    if not want_grad:
+        return (out, ) + (_empty(out), ) * 4
+    return out, torch.empty_like(mu), torch.empty_like(sigma), torch.empty_like(value_new), out.new_empty(4)
+
+
+@torch.library.custom_op('b200rl::ppoc_bwd', mutates_args=())
+def ppoc_bwd(mu: Tensor, sigma: Tensor, value_new: Tensor, mu_old: Tensor, sigma_old: Tensor, mu_pre: Optional[Tensor],
+             sigma_pre: Optional[Tensor], action: Tensor, value_old: Tensor, adv: Tensor, return_: Tensor,
+             weight: Optional[Tensor], factor: Optional[Tensor], g_out: Tensor, grad_mu: Tensor, grad_sigma: Tensor,
+             grad_value: Tensor, g_used: Tensor, S: int, D: int, clip_ratio: float, use_value_clip: int, dual_clip: float,
+             kl_type: int, hint_kind: str) -> tuple[Tensor, Tensor, Tensor]:
+    """-> (grad_mu, grad_sigma, grad_value) for the upstream gradients g_out[0:4] of policy, value, entropy and kl loss"""
+    keep, upstream = _upstream(g_out, 4)
+    saved = (mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight)
+    cfg = (factor, S, D, clip_ratio, use_value_clip, dual_clip, kl_type)
+    return ops.ppoc_bwd_(saved, cfg, upstream, _forward_grads(True, g_used, grad_mu, grad_sigma, grad_value), hint_kind)
+
+
+@ppoc_bwd.register_fake
+def _(mu, sigma, value_new, *args):
+    return torch.empty_like(mu), torch.empty_like(sigma), torch.empty_like(value_new)
+
+
+def _ppoc_setup(ctx, inputs, output):
+    ctx.save_for_backward(*inputs[:13], *output[1:])
+    ctx.cfg = inputs[13:20]
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[1:])
+
+
+def _ppoc_backward(ctx, g_out, *_):
+    if g_out is None:
+        return (None, ) * 21
+    saved = ctx.saved_tensors
+    return ppoc_bwd(*saved[:13], g_out, *saved[13:], *ctx.cfg) + (None, ) * 18
+
+
+ppoc_loss.register_autograd(_ppoc_backward, setup_context=_ppoc_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # what rl_utils calls while compiling: the autograd.Function signatures of ops, on the ops above
 # ---------------------------------------------------------------------------------------------------------------------
 def _want_grad(*xs):
@@ -771,3 +997,36 @@ def a2c_lm(logit, value, action, adv, return_, weight):
     """-> (policy_loss, value_loss, entropy_loss), as A2CLMFunction"""
     out = a2c_lm_fwd(logit, value, action, adv, return_, weight)[0]
     return out[0], out[1], out[2]
+
+
+def gae_returns(value, next_value, reward, done, traj_flag, gamma, lambda_, vscale):
+    """-> (adv, unnormalized return, value_out or None, return_out or None, return_stats, adv_stats), as ops.gae_returns_"""
+    adv, unnorm, vout, rout, stats, astats = gae_returns_op(value, next_value, reward, done, traj_flag, float(gamma),
+                                                            float(lambda_), float(vscale))
+    if vscale == 0.0:
+        vout = rout = None
+    return adv, unnorm, vout, rout, stats, astats
+
+
+def ppof_gae_returns(value, next_value, reward, done, traj_flag, gamma, lambda_, value_norm, std, mu, sigma):
+    """-> (adv, value_out, return_out, return_stats or None, adv_stats), as ops.gae_returns_norm_"""
+    adv, vout, rout, stats, astats = gae_returns_norm(value, next_value, reward, done, traj_flag, float(gamma),
+                                                      float(lambda_), value_norm, float(std), mu, sigma)
+    return adv, vout, rout, stats if value_norm == 'baseline' else None, astats
+
+
+def quantile_td(q, next_n_q, action, next_n_action, reward, done, tau, weight, value_gamma, vg_stride, B, N, n_tau,
+                n_tau_prime, nstep, gamma, form, kappa):
+    """-> (loss, td), as QuantileTDFunction"""
+    vg, vg_scalar = _scalar_or_tensor(value_gamma)
+    loss, td, _, _ = quantile_fwd(q, next_n_q, action, next_n_action, reward, done, tau, weight, vg, vg_scalar, vg_stride,
+                                  B, N, n_tau, n_tau_prime, nstep, gamma, form, kappa, _want_grad(q))
+    return loss, td
+
+
+def ppo_continuous(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight, S,
+                   D, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, factor=None):
+    """-> the six floats policy, value, entropy, kl loss, approx_kl, clipfrac, as PPOContinuousFunction's result vector"""
+    return ppoc_loss(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight,
+                     factor, S, D, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind,
+                     _want_grad(mu, sigma, value_new))[0]

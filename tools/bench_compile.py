@@ -1,4 +1,5 @@
-"""What torch.compile buys a learner's loss step at minibatch sizes, where the Python / ctypes path rather than the kernels
+"""What torch.compile buys a learner's loss step at minibatch sizes (the plugin-boundary operators, SAC's
+``v_1step_td_error``, QR-DQN and continuous-action PPO), where the Python / ctypes path rather than the kernels
 sets the time per call.  Each workload is one forward + backward loss step on CUDA tensors, timed as in
 tools/host_overhead.py: wall-clock microseconds per call over a loop, device synchronised once per loop.  Three modes:
 eager, ``torch.compile`` (default inductor) and ``torch.compile(mode="reduce-overhead")`` (the compiled step replayed as
@@ -140,12 +141,58 @@ def gae_workload():
     return api.gae, loss
 
 
+def v1td_workload():
+    """SAC's critic loss at its batch of 256 (ding/policy/sac.py: one v_1step_td_error per Q head)"""
+    g = torch.Generator().manual_seed(4)
+    t = to_dev(dict(next_v=torch.randn(256, generator=g), reward=torch.randn(256, generator=g),
+                    done=(torch.rand(256, generator=g) < 0.05).float()))
+    v = torch.randn(256, generator=g).to(DEV).requires_grad_(True)
+
+    def loss(f):
+        def step():
+            v.grad = None
+            f(api.v_1step_td_data(v, t['next_v'], t['reward'], t['done'], None), 0.99)[0].backward()
+        return step
+    return lambda *a: (lambda loss, per: (loss, per.detach()))(*api.v_1step_td_error(*a)), loss
+
+
+def qrdqn_workload():
+    t = to_dev(cases.quantile_case(5, 'qrdqn', 64, 6, 32, 32, 3)[1])
+    q = t['q'].detach().requires_grad_(True)
+
+    def loss(f):
+        def step():
+            q.grad = None
+            f(api.qrdqn_nstep_td_data(q, t['next_n_q'], t['action'], t['next_n_action'], t['reward'], t['done'], t['tau'],
+                                      None), 0.99, 3)[0].backward()
+        return step
+    return lambda *a: (lambda loss, per: (loss, per.detach()))(*api.qrdqn_nstep_td_error(*a)), loss
+
+
+def ppoc_workload():
+    t = to_dev(cases.ppoc_case(6, 320, 6)[1])
+    mu, sigma = (t[k].detach().requires_grad_(True) for k in ('mu_new', 'sigma_new'))
+    vn = t['value_new'].detach().requires_grad_(True)
+
+    def loss(f):
+        def step():
+            mu.grad = sigma.grad = vn.grad = None
+            out, _ = f(api.ppo_data({'mu': mu, 'sigma': sigma}, {'mu': t['mu_old'], 'sigma': t['sigma_old']}, t['action'],
+                                    vn, t['value_old'], t['adv'], t['return_'], None, None), 0.2)
+            (out.policy_loss + 0.5 * out.value_loss - 0.01 * out.entropy_loss).backward()
+        return step
+    return api.ppo_error_continuous, loss
+
+
 WORKLOADS = {
     'ppo_error_64x6': lambda: ppo_workload(64),
     'ppo_error_320x6': lambda: ppo_workload(320),
     'q_nstep_td_error_64x6_nstep3': qntd_workload,
     'vtrace_error_discrete_action_T64_B32': vtrace_workload,
     'gae_1d_n3200': gae_workload,
+    'v_1step_td_error_256': v1td_workload,
+    'qrdqn_nstep_td_error_64x6x32_nstep3': qrdqn_workload,
+    'ppo_error_continuous_320x6': ppoc_workload,
 }
 
 
