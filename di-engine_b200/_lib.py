@@ -34,6 +34,7 @@ PROTOTYPES = {
     "b200rl_ppo_fwd_grad": [P, P, P, P, P, P, P, P, P, LL, LL, LL, D, I, D, I, P, P, P, P, P, P, P, P, c_size_t, P],
     "b200rl_ppo_value_fwd": [P, P, P, P, LL, D, I, P, P, P, c_size_t, P],
     "b200rl_ppo_fused_supported": [P, P, P, P, P, P, P, P, P, P, LL, LL],
+    "b200rl_ppo_tile_geometry": [LL, LL, I, I, I, I, P],
     "b200rl_qntd_fwd": [P, P, P, P, P, P, P, P, LL, P, LL, LL, LL, I, D, I, I, D, I, D, I, LL, D, P, P, P, P, P, P, P,
                         c_size_t, P],
     "b200rl_qntd_bwd": [P, P, P, P, P, LL, LL, LL, I, LL, I, P, P],

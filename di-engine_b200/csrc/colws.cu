@@ -539,21 +539,10 @@ static int launch_ws(const FusedArgs& f_in, float* out, float* ws, size_t ws_byt
     return B200RL_OK;
 }
 
-// SM count of the current device (cached per device)
-static int cw_sm_count(int& n) {
-    static int sms[MAX_DEVICES];
-    int dev = 0;
-    if (int rc = current_device(dev)) return rc;
-    if (sms[dev] == 0)
-        if (int rc = cuda_rc(cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev))) return rc;
-    n = sms[dev];
-    return B200RL_OK;
-}
-
 template <bool GRADS>
 static int dispatch_ws(const FusedArgs& f, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
     int sm_count = 0;
-    if (int rc = cw_sm_count(sm_count)) return rc;
+    if (int rc = sm_count_of(sm_count)) return rc;
     const int tc = cw_pick_tc(f, sm_count);
     return with_nc(f.p.N, [&](auto nc) {
         return tc == 32 ? launch_ws<nc, GRADS, 32>(f, out, ws, ws_bytes, st) : launch_ws<nc, GRADS, 16>(f, out, ws, ws_bytes, st);

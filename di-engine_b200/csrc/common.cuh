@@ -574,7 +574,7 @@ static inline bool pdl_enabled() {
     return v == 1;
 }
 
-// B200RL_FUSED_TRACE=1: the column-tile kernels of colws.cu and vtws.cu store per-CTA %globaltimer stamps in the
+// B200RL_FUSED_TRACE=1: the column-tile kernels of colws.cu and vtws.cu and ppo.cu's tile kernel store per-CTA %globaltimer stamps in the
 // workspace (tools/trace_col.py)
 static inline bool trace_enabled() {
     static int v = -1;
@@ -717,6 +717,17 @@ static inline int smem_opt_in(size_t smem) {
     if (smem <= opted[dev]) return B200RL_OK;
     if (int rc = cuda_rc(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))) return rc;
     opted[dev] = smem;
+    return B200RL_OK;
+}
+
+// SM count of the current device (cached per device)
+static inline int sm_count_of(int& n) {
+    static int sms[MAX_DEVICES];
+    int dev = 0;
+    if (int rc = current_device(dev)) return rc;
+    if (sms[dev] == 0)
+        if (int rc = cuda_rc(cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev))) return rc;
+    n = sms[dev];
     return B200RL_OK;
 }
 

@@ -6,15 +6,33 @@
 // N logits per row.  logit_* are (S*G, N) row-major, action (S*G) int64, value_new/value_old/adv/return_/weight (S).
 //
 // Main path (G == 1, N <= 32, 16-byte aligned tensors): ppo_tile_kernel
-//   * persistent grid (SM count x resident CTAs), each CTA walks tiles of 128 consecutive rows;
-//   * every input of a tile -- the logit rows (128*N contiguous floats per tensor), the int64 actions and the four
+//   * one CTA per SM (at most), each owning one contiguous span of 256-row tiles (spans differ by at most one tile; only
+//     the grid's last tile may be ragged), geometry picked on the host by ps_pick;
+//   * every input of a tile -- the logit rows (256*N contiguous floats per tensor), the int64 actions and the four
 //     per-sample scalars -- arrives in shared memory by TMA 1-D bulk copies (cp.async.bulk, SASS UBLKCP) that complete
-//     on an mbarrier; a 3-stage ring keeps two tiles in flight per CTA while one is consumed, so HBM latency is hidden
-//     without spending issue slots on address arithmetic;
-//   * thread i owns row i of the tile; N is a template parameter (rows live in registers, loops fully unrolled) and the
-//     softmax statistics use ex2/lg2 approximations (relative error ~1e-7, far inside the 1e-5 parity bar);
-//   * gradient tiles leave through shared memory and TMA bulk stores (cp.async.bulk.global.shared::cta);
+//     on an mbarrier; the ring is as deep as shared memory allows (8 stages at N = 6), and the producer keeps at most
+//     PS_AHEAD = 2 stages in flight;
+//   * thread i of the 8 consumer warps owns row i of the tile; N is a template parameter (rows live in registers, loops
+//     fully unrolled) and the softmax statistics use ex2/lg2 approximations (relative error ~1e-7, far inside the 1e-5
+//     parity bar);
+//   * a gradient row replaces the row's logit_new slot in the stage; each warp's 32 rows leave as one TMA bulk store
+//     (cp.async.bulk.global.shared::cta) and the stage is released once the store has read it;
 //   * loss partial sums stay in registers across tiles; one deterministic grid reduction per CTA at the end.
+//   Why this geometry: the previous one (128-row tiles, 6 CTAs of 4 consumer warps per SM, a 3-stage ring each, tiles
+//   dealt round-robin) put about 22 MB in flight before any tile landed and gave a CTA about 5 tiles, so the ring barely
+//   reached steady state.  Measured at config P (S = 524 288, N = 6) on an H100 SXM (700 W, SM clock 1980 MHz):
+//   * bench.py: step 47.07 - 47.11 us -> 40.47 us (three runs each); the ppo_fwd_grad call alone (kernel + finalize,
+//     back to back over rotated sets) 24.2 -> 23.9 us, 2.28 TB/s on 104 B per transition.  The step gains far more than
+//     the call: the old step was 6.3 us longer than its three calls timed alone, the new one is not.  Likely cause (not
+//     measured): with PDL the PPO launch is resident while gae_returns still runs, and six old CTAs per SM held 960
+//     threads and about 61 K of the 64 K registers there; one new CTA holds 288 threads and 21 K registers.
+//   * tools/trace_ppo.py: a CTA's first stage lands 2.8 us (median) after its griddepcontrol.wait, then one stage every
+//     1.04 us and the CTA ends 1.0 us after its last stage; 21 - 23 us from the first wait to the last CTA's end.  The
+//     per-stage pace is 3.4 TB/s of the 104 B, more than HBM delivers; presumably (not measured) the gradient stores drain
+//     into L2 behind the loads, and adv, value and return, written by gae_returns just before, partly come from L2.
+//   Slower, not kept: a ring of at most 4 stages (42.55 - 42.59 us per config P step), 128-row stages with 4 consumer
+//   warps (63.35 - 63.42 us); no change: 3 stages in flight instead of 2 (40.34 - 40.44 us against 40.39 - 40.42).
+//   Not built: starting the loads before griddepcontrol.wait when the kernel follows gae_returns in a captured step.
 //   Three variants of the same pipeline: FWD (losses), BWD (gradients for given upstream gradients) and FWD_GRAD: the
 //   forward pass also writes the gradients for the upstream gradients it is told to expect (they are constants of the
 //   training loop: policy + c_v*value - c_e*entropy), so the batch crosses HBM once; the backward launch then only
@@ -29,83 +47,107 @@
 
 namespace b200rl {
 
+// Geometry of ppo_tile_kernel (its own: fused.cu and pg.cu keep the PPO_* constants of ppo_math.cuh)
+constexpr int PS_CW = 8;                  // consumer warps
+constexpr int PS_R = PS_CW * 32;          // rows per stage, one per consumer thread
+constexpr int PS_THREADS = PS_R + 32;     // + the producer warp
+constexpr int PS_MAX_STAGES = 8;          // ring depth where shared memory allows
+constexpr int PS_AHEAD = 2;               // stages the producer keeps in flight
+constexpr size_t PS_SMEM_LIMIT = 227 * 1024 - 1024;  // dynamic shared memory of one CTA per SM (static partial sums aside)
+// B200RL_FUSED_TRACE=1: %globaltimer stamps, 64 per CTA at workspace word 65536 (tools/trace_ppo.py).  0 start, 1 the
+// previous launches' results visible (griddepcontrol.wait returned), 2 first stage landed, 3 last stage landed, 4 end
+// (partial sums stored), 5 stages of the CTA (low 32 bits) and its SM (high 32 bits); 8 + j stage j landed (j < 56).
+constexpr int PS_TRACE_STAGES = 56;
+
 template <int NC, int WHAT>
-__global__ void __launch_bounds__(PPO_THREADS) ppo_tile_kernel(PpoArgs a, float* out, float* ws) {
-    // rows per tile: one per consumer thread (256-row tiles can help the forward-only variant, not the gradient-writing
-    // ones or the gae -> ppo -> verify sequence)
-    constexpr int PPO_R = PPO_CT;
-    pdl_prologue();
+__global__ void __launch_bounds__(PS_THREADS, 1) ppo_tile_kernel(PpoArgs a, float* ws, int n_stages, int trace) {
     extern __shared__ __align__(128) unsigned char smem[];
+    unsigned long long* tr = trace ? reinterpret_cast<unsigned long long*>(ws + 65536) + blockIdx.x * 64 : nullptr;
+    if (tr && threadIdx.x == 0) tr[0] = gtimer();
+    pdl_prologue();
+    if (tr && threadIdx.x == 0) tr[1] = gtimer();
     constexpr bool GRADS = (WHAT != PPO_FWD);
     constexpr bool LOSSES = (WHAT != PPO_BWD);
     const int N = NC ? NC : a.N;
     const int tid = threadIdx.x;
     const int wid = tid >> 5, lane = tid & 31;
-    const bool is_producer = wid == PPO_CW;  // warp 4: TMA issue only
     const bool has_pre = a.logit_pre != nullptr, has_w = a.weight != nullptr;
-    const PpoTileLayout L = ppo_layout(N, has_pre, has_w, PPO_R);
-    const int warp_out_bytes = 32 * N * 4;  // one warp's gradient rows of a tile (32 consecutive rows)
-    unsigned char* outbuf = smem + PPO_STAGES * L.stage_bytes;
-    uint64_t* full = reinterpret_cast<uint64_t*>(outbuf + (GRADS ? PPO_OUTBUFS * L.logit_bytes : 0));
-    uint64_t* empty = full + PPO_STAGES;
+    const PpoTileLayout L = ppo_layout(N, has_pre, has_w, PS_R);
+    const int NS = n_stages;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + NS * L.stage_bytes);
+    uint64_t* empty = full + PS_MAX_STAGES;
 
     float g[4] = {0.f, 0.f, 0.f, 0.f};
     // BWD: returns when the forward pass wrote exactly these gradients
     if (GRADS && upstream<4>(a.rec, WHAT == PPO_BWD, ppo_owned(a), g)) return;
     const PpoUpstream up{g[0], g[1], g[2], g[3], 1.f / (float)a.S};
 
-    const long long n_full = a.S / PPO_R;
-    const int tail_rows = (int)(a.S - n_full * PPO_R);
+    // CTA b owns the contiguous tiles [t0, t1): spans differ by at most one tile, and only the grid's last tile may be
+    // ragged.  A static map, so the per-CTA partial sums (and with them the losses) do not depend on timing.
+    const long long n_full = a.S / PS_R;
+    const int tail_rows = (int)(a.S - n_full * PS_R);
     const long long n_tiles = n_full + (tail_rows ? 1 : 0);
-    const int my_n = (n_tiles > blockIdx.x) ? (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0;
+    const long long t0 = n_tiles * blockIdx.x / gridDim.x, t1 = n_tiles * (blockIdx.x + 1) / gridDim.x;
+    const int my_n = (int)(t1 - t0);
 
     if (tid == 0) {
-        for (int s = 0; s < PPO_STAGES; ++s) {
-            mbar_init(&full[s], 1);           // producer's expect_tx arrive + TMA byte count
-            mbar_init(&empty[s], PPO_CW);  // one arrive per consumer warp
+        for (int s = 0; s < NS; ++s) {
+            mbar_init(&full[s], 1);        // producer's expect_tx arrive + TMA byte count
+            mbar_init(&empty[s], PS_CW);   // one arrive per consumer warp
         }
         mbar_fence_init();
     }
     __syncthreads();
 
     float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // policy, value, entropy, kl, approx_kl, clipfrac
-    if (is_producer) {
-        // ---- producer warp: keeps the stage ring full; never touches the data ---------------------------------------
+    if (wid == PS_CW) {
+        // ---- producer: one lane issues every stage's bulk copies, at most PS_AHEAD stages in flight --------------------
         if (lane == 0) {
             for (int i = 0; i < my_n; ++i) {
-                const long long t = blockIdx.x + (long long)i * gridDim.x;
+                const long long t = t0 + i;
                 if (t >= n_full) break;  // the ragged last tile is read with plain loads by its consumers
-                const int sg = i % PPO_STAGES;
-                if (i >= PPO_STAGES) mbar_wait(&empty[sg], (uint32_t)(((i / PPO_STAGES) - 1) & 1));
-                const long long row0 = t * PPO_R;
+                const int sg = i % NS;
+                if (i >= NS) mbar_wait(&empty[sg], (uint32_t)(((i / NS) - 1) & 1));
+                if (NS > PS_AHEAD && i >= PS_AHEAD) {  // stage i - PS_AHEAD has landed
+                    const int jb = i - PS_AHEAD;
+                    mbar_wait(&full[jb % NS], (uint32_t)((jb / NS) & 1));
+                }
+                const long long row0 = t * PS_R;
                 unsigned char* st = smem + sg * L.stage_bytes;
                 uint64_t* bar = &full[sg];
                 mbar_expect_tx(bar, (uint32_t)L.tx_bytes);
                 tma_load_1d(st, a.logit_new + row0 * N, L.logit_bytes, bar);
                 tma_load_1d(st + L.off_old, a.logit_old + row0 * N, L.logit_bytes, bar);
                 if (has_pre) tma_load_1d(st + L.off_pre, a.logit_pre + row0 * N, L.logit_bytes, bar);
-                tma_load_1d(st + L.off_act, a.action + row0, PPO_R * 8, bar);
-                tma_load_1d(st + L.off_vn, a.value_new + row0, PPO_R * 4, bar);
-                tma_load_1d(st + L.off_vo, a.value_old + row0, PPO_R * 4, bar);
-                tma_load_1d(st + L.off_adv, a.adv + row0, PPO_R * 4, bar);
-                tma_load_1d(st + L.off_ret, a.ret + row0, PPO_R * 4, bar);
-                if (has_w) tma_load_1d(st + L.off_w, a.weight + row0, PPO_R * 4, bar);
+                tma_load_1d(st + L.off_act, a.action + row0, PS_R * 8, bar);
+                tma_load_1d(st + L.off_vn, a.value_new + row0, PS_R * 4, bar);
+                tma_load_1d(st + L.off_vo, a.value_old + row0, PS_R * 4, bar);
+                tma_load_1d(st + L.off_adv, a.adv + row0, PS_R * 4, bar);
+                tma_load_1d(st + L.off_ret, a.ret + row0, PS_R * 4, bar);
+                if (has_w) tma_load_1d(st + L.off_w, a.weight + row0, PS_R * 4, bar);
             }
         }
     } else {
-    // ---- consumer warps: warp w owns rows [32w, 32w+32) of every tile; no CTA-wide barrier in this loop ------------
-    const int rit = wid * 32 + lane;  // this thread's row in every tile
-    for (int i = 0; i < my_n; ++i) {
-        const long long t = blockIdx.x + (long long)i * gridDim.x;
-        const long long row0 = t * PPO_R;
-        const int sg = i % PPO_STAGES;
-        unsigned char* st = smem + sg * L.stage_bytes;
-        const bool full_tile = t < n_full;
-        if (full_tile) {
-            mbar_wait(&full[sg], (uint32_t)((i / PPO_STAGES) & 1));
-        } else {
-            // ragged last tile: every thread fetches its own row into its own slots of the stage (no sharing)
-            if (rit < tail_rows) {
+        // ---- consumers: warp w owns rows [32w, 32w+32) of every stage; no CTA-wide barrier in this loop ----------------
+        const int rit = wid * 32 + lane;  // this thread's row in every stage
+        const int warp_out_bytes = 32 * N * 4;
+        for (int i = 0; i < my_n; ++i) {
+            const long long t = t0 + i;
+            const long long row0 = t * PS_R;
+            const int sg = i % NS;
+            unsigned char* st = smem + sg * L.stage_bytes;
+            const bool full_tile = t < n_full;
+            if (full_tile) {
+                mbar_wait(&full[sg], (uint32_t)((i / NS) & 1));
+                if (tr && tid == 0) {
+                    const unsigned long long now = gtimer();
+                    if (i == 0) tr[2] = now;
+                    tr[3] = now;
+                    if (i < PS_TRACE_STAGES) tr[8 + i] = now;
+                }
+            } else if (rit < tail_rows) {
+                // ragged last tile: every thread fetches its own row into its own slots of the stage (no sharing); the
+                // bulk stores that read this slot earlier have finished reading it (wait_read + __syncwarp below)
                 float* d0 = reinterpret_cast<float*>(st) + rit * N;
                 float* d1 = reinterpret_cast<float*>(st + L.off_old) + rit * N;
                 float* d2 = reinterpret_cast<float*>(st + L.off_pre) + rit * N;
@@ -121,31 +163,44 @@ __global__ void __launch_bounds__(PPO_THREADS) ppo_tile_kernel(PpoArgs a, float*
                 reinterpret_cast<float*>(st + L.off_ret)[rit] = a.ret[row0 + rit];
                 if (has_w) reinterpret_cast<float*>(st + L.off_w)[rit] = a.weight[row0 + rit];
             }
-        }
-        // this warp's slice of the gradient-tile ring (2 buffers per warp inside the CTA's output area)
-        float* gtile = reinterpret_cast<float*>(outbuf + (wid * 2 + (i & 1)) * warp_out_bytes) - wid * 32 * N;
-        if (full_tile || rit < tail_rows) {
-            const float adv = reinterpret_cast<const float*>(st + L.off_adv)[rit];
-            ppo_row_compute<NC, LOSSES, GRADS>(a, L, st, rit, N, adv, full_tile, gtile, row0, up, acc);
-        }
-        if (full_tile) {
+            // a full stage's gradient rows replace the rows' own logit_new slots (ppo_row_compute_to reads them first)
+            if (full_tile || rit < tail_rows) {
+                const float adv = reinterpret_cast<const float*>(st + L.off_adv)[rit];
+                ppo_row_compute<NC, LOSSES, GRADS>(a, L, st, rit, N, adv, full_tile, reinterpret_cast<float*>(st), row0,
+                                                   up, acc);
+            }
+            if (!full_tile) continue;
             if (GRADS) {
-                // hand this warp's 32 gradient rows to the TMA store engine; keep at most one store reading smem
+                // this warp's 32 gradient rows are one contiguous span: one bulk store.  The stage is released once the
+                // store has read it -- with a ring of two or more, one stage later, so the warp does not wait for it
                 fence_proxy_async_smem();
                 __syncwarp();
                 if (lane == 0) {
-                    tma_store_1d(a.grad_logit + (row0 + wid * 32) * N, gtile + wid * 32 * N, warp_out_bytes);
+                    tma_store_1d(a.grad_logit + (row0 + wid * 32) * N, st + wid * warp_out_bytes, warp_out_bytes);
                     tma_store_commit();
-                    tma_store_wait_read<1>();
+                    if (NS == 1) {
+                        tma_store_wait_read<0>();
+                        mbar_arrive(&empty[sg]);
+                    } else {
+                        tma_store_wait_read<1>();
+                        if (i > 0) mbar_arrive(&empty[(i - 1) % NS]);
+                    }
                 }
+                // only lane 0 waited for the store's read: the other lanes may write this warp's rows of the ring again
+                // (the ragged last tile's plain loads) only after it
+                __syncwarp();
+            } else {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[sg]);  // stage may be refilled once all consumer warps have arrived
             }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[sg]);  // stage may be refilled once all four warps have arrived
         }
+        if (GRADS && lane == 0) tma_store_wait_read<0>();  // shared memory must outlive the bulk stores that read it
     }
-    if (GRADS && lane == 0) tma_store_wait_read<0>();  // shared memory must outlive the bulk stores that read it
+    if (LOSSES) grid_store_partials<6, PS_THREADS>(acc, ws);  // summed by finalize_sums_kernel, launched right behind
+    if (tr && tid == 0) {
+        tr[4] = gtimer();
+        tr[5] = (unsigned long long)smid() << 32 | (unsigned long long)my_n;
     }
-    if (LOSSES) grid_store_partials<6, PPO_THREADS>(acc, ws);  // summed by finalize_sums_kernel, launched right behind
 }
 
 // ===============================================================================================================
@@ -321,26 +376,47 @@ __global__ void __launch_bounds__(NT) ppo_value_kernel(const float* __restrict__
     if (grid_sum<1, NT>(acc, tot, ws, 0) && threadIdx.x == 0) out[0] = (float)(0.5 * tot[0] / (double)S);
 }
 
-// launch geometry of the persistent kernel: SM count x resident CTAs per SM for this instantiation / smem size
+// Geometry for S rows of N logits on `sm_count` SMs (one CTA per SM at most): the grid, the ring depth and the dynamic
+// shared memory.  The ring is as deep as shared memory allows, up to PS_MAX_STAGES and no deeper than a CTA has tiles
+// (small batches, e.g. PPO minibatches of 64 - 320 rows, get one or two CTAs and a short ring).  The verification launch
+// behind a fused forward normally returns at once: it gets one stage, so that it holds little shared memory while the
+// next step's kernel starts beside it, and recomputes on that one stage when the record says so.  At config D (N = 6)
+// that launch holds 18.5 KB of shared memory, 288 threads and 288 x 72 = 20.7 K registers per SM (ptxas, sm_90a); the
+// column kernel of the next step (gae_ppo_ws_kernel<6, true, 32>) needs about 165 KB, 320 threads and 320 x 96 = 30.7 K
+// registers, so both fit on one SM at once.
+struct PsGeo {
+    int grid, stages;
+    size_t smem;
+};
+static PsGeo ps_pick(long long S, int N, bool has_pre, bool has_w, bool verify_only, int sm_count) {
+    PsGeo g{};
+    const size_t stage = (size_t)ppo_layout(N, has_pre, has_w, PS_R).stage_bytes;
+    const size_t bars = 2 * PS_MAX_STAGES * sizeof(uint64_t);
+    const long long n_tiles = (S + PS_R - 1) / PS_R;
+    g.grid = (int)(n_tiles < sm_count ? n_tiles : sm_count);
+    const long long per_cta = g.grid > 0 ? (n_tiles + g.grid - 1) / g.grid : 0;
+    long long stages = verify_only ? 1 : (long long)((PS_SMEM_LIMIT - bars) / stage);
+    if (stages > PS_MAX_STAGES) stages = PS_MAX_STAGES;
+    if (stages > per_cta) stages = per_cta;
+    g.stages = stages < 1 ? 0 : (int)stages;  // 0: not even one stage fits
+    g.smem = (size_t)g.stages * stage + bars;
+    return g;
+}
+
 template <int NC, int WHAT>
 static int launch_tile(const PpoArgs& a, float* out, float* ws, size_t ws_bytes, cudaStream_t st) {
-    constexpr int PPO_R = PPO_CT;
-    const PpoTileLayout L = ppo_layout(a.N, a.logit_pre != nullptr, a.weight != nullptr, PPO_R);
-    const size_t smem = (size_t)PPO_STAGES * L.stage_bytes + (WHAT != PPO_FWD ? (size_t)PPO_OUTBUFS * L.logit_bytes : 0) +
-                        2 * PPO_STAGES * sizeof(uint64_t);
+    int sm_count = 0;
+    if (int rc = sm_count_of(sm_count)) return rc;
+    const PsGeo g = ps_pick(a.S, a.N, a.logit_pre != nullptr, a.weight != nullptr, WHAT == PPO_BWD && a.rec.used, sm_count);
+    if (g.stages < 1) return B200RL_ERR_ARG;
     constexpr auto kern = ppo_tile_kernel<NC, WHAT>;
-    if (smem > 227 * 1024) return B200RL_ERR_ARG;
-    int sm_count, per_sm;
-    if (int rc = resident_ctas<kern>(PPO_THREADS, smem, sm_count, per_sm)) return rc;
-    if (per_sm > 6) per_sm = 6;
-    const long long n_tiles = (a.S + PPO_R - 1) / PPO_R;
-    // the verification launch that follows a fused forward normally exits at once: keep its grid to one CTA per SM
-    long long grid = (long long)sm_count * ((WHAT == PPO_BWD && a.rec.used) ? 1 : per_sm);
-    if (grid > n_tiles) grid = n_tiles;
-    if (WHAT != PPO_BWD && !ws_partials_fit((long long)(grid * 6), ws_bytes)) return B200RL_ERR_WORKSPACE;
-    if (int rc = launch_k(kern, (int)grid, PPO_THREADS, smem, st, a, out, ws)) return rc;
+    if (int rc = smem_opt_in<kern>(g.smem)) return rc;
+    if (WHAT != PPO_BWD && !ws_partials_fit((long long)g.grid * 6, ws_bytes)) return B200RL_ERR_WORKSPACE;
+    const int trace = WHAT != PPO_BWD && trace_enabled();
+    if (trace && (size_t)65536 * 4 + (size_t)g.grid * 64 * 8 > ws_bytes) return B200RL_ERR_WORKSPACE;  // the stamps
+    if (int rc = launch_k(kern, g.grid, PS_THREADS, g.smem, st, a, ws, g.stages, trace)) return rc;
     if (WHAT == PPO_BWD) return B200RL_OK;
-    return launch_finalize(ws, out, ppo_finalize_args(a.S, a.logit_pre != nullptr, (int)grid), st);
+    return launch_finalize(ws, out, ppo_finalize_args(a.S, a.logit_pre != nullptr, g.grid), st);
 }
 
 template <int WHAT>
@@ -455,6 +531,14 @@ extern "C" int b200rl_ppo_bwd(const float* logit_new, const float* logit_old, co
     if (grid > NUM_SMS * 32) grid = NUM_SMS * 32;  // grid-stride kernels
     if (a.N > 64) return launch_k(ppo_bwd_kernel<NT, 2>, (int)grid, NT, 0, st, a);
     return launch_k(ppo_bwd_kernel<NT, 1>, (int)grid, NT, 0, st, a);
+}
+
+extern "C" int b200rl_ppo_tile_geometry(long long S, long long N, int has_pretrained, int has_weight, int verify_only,
+                                        int sm_count, long long* geometry3) {
+    if (S < 1 || N < 1 || N > 32 || sm_count < 1 || !geometry3) return B200RL_ERR_ARG;
+    const PsGeo g = ps_pick(S, (int)N, has_pretrained != 0, has_weight != 0, verify_only != 0, sm_count);
+    geometry3[0] = g.grid; geometry3[1] = g.stages; geometry3[2] = (long long)g.smem;
+    return B200RL_OK;
 }
 
 extern "C" int b200rl_ppo_value_fwd(const float* value_new, const float* value_old, const float* return_,

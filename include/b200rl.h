@@ -156,6 +156,11 @@ B200RL_API int b200rl_ppo_fwd_grad(const float* logit_new, const float* logit_ol
                         double clip_ratio, int use_value_clip, double dual_clip, int kl_type, const float* adv_stats,
                         const float* factor, const float* g_expected, float* g_used, float* out, float* grad_logit_new,
                         float* grad_value_new, float* workspace, size_t workspace_bytes, void* stream);
+/* Launch geometry of the tile kernel behind b200rl_ppo_fwd / _fwd_grad / _bwd for S rows of N <= 32 logits on a device
+ * with sm_count SMs: geometry3 = {CTAs, ring stages, dynamic shared memory bytes}.  verify_only: the check launch of
+ * b200rl_ppo_bwd behind a fused forward.  Host arithmetic only. */
+B200RL_API int b200rl_ppo_tile_geometry(long long S, long long N, int has_pretrained, int has_weight, int verify_only,
+                                        int sm_count, long long* geometry3);
 B200RL_API int b200rl_ppo_fused_supported(const float* logit_new, const float* logit_old, const float* logit_pretrained,
                                const long long* action, const float* value_new, const float* value_old,
                                const float* adv, const float* return_, const float* weight,
