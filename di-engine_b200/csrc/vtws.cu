@@ -751,7 +751,7 @@ extern "C" int b200rl_vtrace_fwd_grad(const float* target_output, const float* b
     a.grad_logit = grad_target_output; a.grad_value = grad_value;
     cudaStream_t st = (cudaStream_t)stream;
     // streaming column tiles wherever they fit (faster: they overlap loads with the scan); resident tiles take the shapes
-    // they cannot (N > 14: no three-stage ring), and every shape they fit under b200rl_vtrace_set_impl(2)
+    // they cannot (N > 15: no three-stage ring), and every shape they fit under b200rl_vtrace_set_impl(2)
     const int rtc = (vtws_ok(a) && g_vt_impl != 2) ? 0 : vtres_tc(a);
     if (rtc == 8)
         return grads ? dispatch_vtres<true, 8>(a, out3, workspace, workspace_bytes, st)

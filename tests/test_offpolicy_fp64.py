@@ -15,6 +15,7 @@ boundary of the fp64 reference (ratio at fp32(1 +- clip) or at the dual-clip flo
 value errors equal) may take the other branch in fp32: their gradients are left out of the elementwise check but must be
 finite.  Each case prints the largest ratio of the two sides of the bound it measured.
 """
+import ctypes
 import functools
 import math
 from collections import OrderedDict
@@ -32,7 +33,7 @@ pytestmark = pytest.mark.gpu
 DEV = 'cuda'
 K = 8.0
 EPS32 = 2.0 ** -24
-S_BIG = 128 * 512 + 37  # 512 full 128-row tiles and a ragged one
+S_BIG = 128 * 512 + 37  # 256 full 256-row tiles and a ragged one: 257 tiles over 132 CTAs, one or two each (no ring wrap)
 MASKS = {'1e8': -1e8, 'inf': -math.inf}
 MIX_B = [0.7, 2.0, 0.05, -1.5]  # an upstream mix the forward pass does not expect
 
@@ -68,6 +69,25 @@ def _zeros_at(g, x, p):
     x = x.clone()
     x[torch.rand(x.shape, generator=g) < p] = 0.0
     return x
+
+
+def ring_wrap_rows(N, pre=False, w=True, sms=None):
+    """rows of a ppo_error batch on which the tile kernel's ring wraps: b200rl_ppo_tile_geometry on the device's SMs gives
+    every CTA more 256-row tiles than its ring has stages, and the last tile is ragged"""
+    if sms is None:
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+    lib = ops.lib()
+
+    def geo(S):
+        g = (ctypes.c_longlong * 3)()
+        assert lib.b200rl_ppo_tile_geometry(S, N, int(pre), int(w), 0, sms, g) == 0
+        return g[0], g[1]
+
+    stages = geo(1 << 24)[1]
+    S = sms * (stages + 1) * 256 + 37
+    grid, st = geo(S)
+    assert grid == sms and st == stages and (S // 256 + 1) // sms > stages, (N, pre, w, sms, grid, st)
+    return S
 
 
 def _samples(g, S, weight=True):
@@ -312,6 +332,7 @@ PPO_CASES = {
     'pre_k1_N6': dict(S=S_BIG, N=6, pretrained=True, kl_type='k1'),
     'pre_k2_N18_dc': dict(S=4099, N=18, pretrained=True, kl_type='k2', dual_clip=3.0),
     'pre_k3_N13': dict(S=4099, N=13, pretrained=True, kl_type='k3'),
+    'ring_wrap_N6_dc': dict(S='wrap', N=6, dual_clip=3.0),  # every CTA runs its 8-stage ring more than once
 }
 
 
@@ -341,6 +362,8 @@ def _run_ppo_odd(t, p):
 def _ppo_batch(name, mask):
     c = dict(PPO_CASES[name])
     S, N, odd = c.pop('S'), c.pop('N'), c.pop('odd', False)
+    if S == 'wrap':
+        S = ring_wrap_rows(N, c.get('pretrained', False), c.get('weight', True))
     op, t, p, meta = gen_ppo(7000 + list(PPO_CASES).index(name), S, N, mask=mask, clip_ratio=0.2, **c)
     frac, bnd, scales = ppo_meta(op, t, p, meta)
     a, b = mixes(op)
