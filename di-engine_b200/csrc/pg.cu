@@ -1,11 +1,14 @@
 // Policy-gradient heads on (T, B, N) logits:
 //   upgo_loss (ding/rl_utils/upgo.py:77-111, tb_cross_entropy :7-43)           -> upgo_head_fwd / upgo_head_bwd
 //   vtrace_error_discrete_action (ding/rl_utils/vtrace.py:72-136, isw.py:55-58) -> vtrace_fwd / vtrace_bwd
+//   coma_error (ding/rl_utils/coma.py:10-58): value half on td.cu's lambda_scan (HEAD 2), policy half below -> coma_fwd / coma_bwd
 //
 // V-trace forward is two launches: a row kernel (log-softmax statistics of the target and behaviour logits, one pass
 // over the two (T,B,N) tensors, rows staged through shared memory) and a column-tile scan kernel (gae.cu scheme) that
 // turns the importance weights into vs / advantages, reduces the three losses in-kernel and leaves the per-element
 // gradient coefficients for the single backward launch.
+#include <type_traits>
+
 #include "../../include/b200rl.h"
 #include "ppo_math.cuh"
 
@@ -468,9 +471,179 @@ __global__ void __launch_bounds__(256) vtc_bwd_kernel(VtcArgs a) {
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// COMA policy half (coma.py:53-57), one (t, b, a) row per warp, rows r = (t*B + b)*A + a of R = T*B*A:
+//   baseline = sum_j softmax(z)_j q_j and adv = q[act] - baseline, both detached; logp = log softmax(z)[act];
+//   H = -sum_j p_j max(logp_j, fp32 min) (Categorical.entropy's clamp: a -inf logit adds 0, not NaN);
+//   policy_loss = -mean(logp * adv * w), entropy_loss = mean(H * w).
+// Gradients for the record's upstream gradients (slots policy, value, entropy):
+//   d/dz_j = g_p*(-adv*w/R)*(1[j==act] - p_j) + g_e*(w/R)*(-p_j*(logp_j + H));
+//   d/dq_j = g_v*dq[r] at j == act for the rows r < R0 = (T-1)*B*A that the value half saw (dq: its unit gradient), else 0.
+// The row lives in K registers per lane (N <= 32K); K = 0 takes any N and re-reads the row from L1.
+// ---------------------------------------------------------------------------------------------------------------
+struct ComaArgs {
+    const float* logit;       // (R, N)
+    const float* q;           // (R, N); forward only
+    const long long* action;  // (R)
+    const float* weight;      // nullable (R)
+    const float* dq;          // (R0)
+    long long R, R0;
+    int N;
+    float* out;         // the three losses; this kernel writes slots 0 and 2, the value half slot 1
+    float* adv;         // (R): written by the forward launch, read by the verify launch
+    float* grad_logit;  // nullable: losses only
+    float* grad_q;
+    UpstreamRecord rec;
+};
+
+template <int NT, int K>
+__global__ void __launch_bounds__(NT) coma_policy_kernel(ComaArgs a, float* ws) {
+    pdl_prologue();
+    float g[3];
+    if (upstream<3>(a.rec, a.rec.verify, 7u, g)) return;
+    const bool fwd = !a.rec.verify;
+    const bool grads = a.grad_logit != nullptr;
+    const int lane = threadIdx.x & 31;
+    const int N = a.N;
+    const float inv_r = 1.f / (float)a.R;
+    float acc[2] = {0.f, 0.f};
+    for (long long r = (long long)blockIdx.x * (NT / 32) + (threadIdx.x >> 5); r < a.R; r += (long long)gridDim.x * (NT / 32)) {
+        const float* z = a.logit + r * N;
+        const float* q = a.q + r * N;
+        constexpr int KR = K > 0 ? K : 1;
+        float zc[KR], qc[KR];
+        if constexpr (K > 0) {
+#pragma unroll
+            for (int k = 0; k < K; ++k) {
+                const int j = lane + 32 * k;
+                zc[k] = j < N ? z[j] : 0.f;
+                qc[k] = (fwd && j < N) ? q[j] : 0.f;
+            }
+        }
+        // f(j, z_j, q_j) over the lane's entries of the row (q_j is 0 in the verify launch)
+        auto each = [&](auto&& f) {
+            if constexpr (K > 0) {
+#pragma unroll
+                for (int k = 0; k < K; ++k)
+                    if (lane + 32 * k < N) f(lane + 32 * k, zc[k], qc[k]);
+            } else {
+                for (int j = lane; j < N; j += 32) f(j, z[j], fwd ? q[j] : 0.f);
+            }
+        };
+        float m = -INFINITY;
+        each([&](int, float zj, float) { m = fmaxf(m, zj); });
+        m = warp_max(m);
+        float s = 0.f;
+        each([&](int, float zj, float) { s += expf(zj - m); });
+        const float ls = logf(warp_sum(s));
+        float h = 0.f, bl = 0.f;
+        each([&](int, float zj, float qj) {
+            const float lp = (zj - m) - ls;  // torch's log-softmax order (see row_max_logsum)
+            const float p = expf(lp);
+            h += p * fmaxf(lp, kF32Min);
+            bl += p * qj;
+        });
+        const float ent = -warp_sum(h);
+        const int act = (int)a.action[r];
+        const float w = a.weight ? a.weight[r] : 1.f;
+        float adv;
+        if (fwd) {
+            adv = q[act] - warp_sum(bl);
+            const float lpa = (z[act] - m) - ls;
+            if (lane == 0) {
+                a.adv[r] = adv;
+                acc[0] += lpa * adv * w;
+                acc[1] += ent * w;
+            }
+        } else {
+            adv = a.adv[r];
+        }
+        if (grads) {
+            const float c_act = g[0] * (-adv * w) * inv_r, c_ent = g[2] * w * inv_r;
+            const float cq = r < a.R0 ? g[1] * a.dq[r] : 0.f;
+            float* gz = a.grad_logit + r * N;
+            float* gq = a.grad_q + r * N;
+            each([&](int j, float zj, float) {
+                const float lpj = fmaxf((zj - m) - ls, kF32Min);
+                const float p = expf(lpj);
+                float gj = -c_act * p - c_ent * p * (lpj + ent);
+                if (j == act) gj += c_act;
+                gz[j] = gj;
+                gq[j] = j == act ? cq : 0.f;
+            });
+        }
+    }
+    if (!fwd) return;  // the losses were written by the forward launch
+    const double ir = 1.0 / (double)a.R;
+    grid_sum_fx<2, NT>(acc, ws, [&](int k, double t) {
+        if (k == 0) a.out[0] = (float)(-t * ir);
+        else a.out[2] = (float)(t * ir);
+    });
+}
+
+// launches coma_policy_kernel<NT, K> with the K that holds an N-wide row (0: any N)
+template <class F>
+static int with_coma_k(long long N, F&& f) {
+    if (N <= 32) return f(std::integral_constant<int, 1>());
+    if (N <= 128) return f(std::integral_constant<int, 4>());
+    if (N <= 256) return f(std::integral_constant<int, 8>());
+    return f(std::integral_constant<int, 0>());
+}
+
+static int launch_coma_policy(const ComaArgs& a, float* ws, cudaStream_t st) {
+    constexpr int NT = 256;
+    long long grid = div_up(a.R, NT / 32);
+    if (grid > NUM_SMS * 3) grid = NUM_SMS * 3;  // <= FX_MAX_GRID: grid_sum_fx's one atomic round trip per CTA
+    return with_coma_k(a.N, [&](auto k) {
+        return launch_k(coma_policy_kernel<NT, decltype(k)::value>, (int)grid, NT, 0, st, a, ws);
+    });
+}
+
+int launch_coma_value(const float* q, const float* target_q, const long long* action, const float* reward,
+                      const float* weight, double gamma, double lambda_, long long T, long long B, long long A, long long N,
+                      float* loss, float* dq, float* dret, float* ws, size_t ws_bytes, cudaStream_t st);  // csrc/td.cu
+
 }  // namespace b200rl
 
 using namespace b200rl;
+
+extern "C" int b200rl_coma_fwd(const float* logit, const float* q_value, const float* target_q_value,
+                               const long long* action, const float* reward, const float* weight, long long T,
+                               long long B, long long A, long long N, double gamma, double lambda_,
+                               const float* g_expected, float* g_used, float* out3, float* adv_saved, float* dq_saved,
+                               float* dret, float* grad_logit, float* grad_q_value, float* workspace,
+                               size_t workspace_bytes, void* stream) {
+    if (T < 2 || B < 1 || A < 1 || N < 1 || !logit || !q_value || !target_q_value || !action || !reward || !adv_saved ||
+        !dq_saved || !workspace || workspace_bytes < WS_MIN_BYTES)
+        return B200RL_ERR_ARG;
+    if (!upstream_args_ok(0, out3, grad_logit != nullptr, grad_logit && grad_q_value, g_expected, g_used))
+        return B200RL_ERR_ARG;
+    const cudaStream_t st = (cudaStream_t)stream;
+    // the value half first: the policy head's gradient rows read its unit gradient dq
+    const int rc = launch_coma_value(q_value, target_q_value, action, reward, weight, gamma, lambda_, T, B, A, N, out3 + 1,
+                                     dq_saved, dret, workspace, workspace_bytes, st);
+    if (rc != B200RL_OK) return rc;
+    ComaArgs a{};
+    a.logit = logit; a.q = q_value; a.action = action; a.weight = weight; a.dq = dq_saved;
+    a.R = T * B * A; a.R0 = (T - 1) * B * A; a.N = (int)N;
+    a.out = out3; a.adv = adv_saved; a.grad_logit = grad_logit; a.grad_q = grad_q_value;
+    a.rec = forward_record(g_expected, g_used);
+    return launch_coma_policy(a, workspace, st);
+}
+
+extern "C" int b200rl_coma_bwd(const float* logit, const long long* action, const float* weight, const float* adv_saved,
+                               const float* dq_saved, long long T, long long B, long long A, long long N,
+                               const float* g_policy, const float* g_value, const float* g_entropy, const float* g_used,
+                               float* g_hint, float* grad_logit, float* grad_q_value, void* stream) {
+    if (T < 2 || B < 1 || A < 1 || N < 1 || !logit || !action || !adv_saved || !dq_saved) return B200RL_ERR_ARG;
+    if (!upstream_args_ok(1, nullptr, true, grad_logit && grad_q_value, nullptr, g_used)) return B200RL_ERR_ARG;
+    ComaArgs a{};
+    a.logit = logit; a.action = action; a.weight = weight; a.dq = dq_saved;
+    a.R = T * B * A; a.R0 = (T - 1) * B * A; a.N = (int)N;
+    a.adv = const_cast<float*>(adv_saved); a.grad_logit = grad_logit; a.grad_q = grad_q_value;
+    a.rec = verify_record(g_policy, g_value, g_entropy, nullptr, g_used, g_hint);
+    return launch_coma_policy(a, nullptr, (cudaStream_t)stream);
+}
 
 extern "C" int b200rl_upgo_head_fwd(const float* logit, const long long* action, const float* mask, const float* rho,
                                     const float* ret, const float* value, long long TB, long long K, long long N,

@@ -759,6 +759,9 @@ __global__ void dntd_bwd_kernel(const float* __restrict__ dist, const long long*
 // MODE 0: gamma/lambda scalars or (T,B) tensors, optional done (generalized_lambda_returns, td.py:1574-1651)
 // MODE 1: UPGO: gamma = 1, lambda_t = [r_{t+1} + V_{t+2} >= V_{t+1}], last = 1 (upgo.py:66-68)
 // HEAD 1: fused TD(lambda) loss head: loss = 0.5*mean(w*(G - V_t)^2) and the saved gradient dV (td.py:1570)
+// HEAD 2: COMA's value loss (coma.py:45-52), on ComaLamArgs: column c = b*A + a of a (T-1, B*A) scan whose bootstrap values
+//         are target_q_value[t, b, a, action[t, b, a]] and whose reward is reward[t, b], both read in place (no gathered or
+//         broadcast copy); loss = mean(w*(G - q_taken)^2) over rows t < T-1, and the saved unit gradient of each column
 // ---------------------------------------------------------------------------------------------------------------
 struct LamArgs {
     const float* value;   // (T+1, B)
@@ -774,9 +777,19 @@ struct LamArgs {
     float* dvalue;  // HEAD: (T+1, B) saved d loss / d value for unit upstream gradient
 };
 
-template <int TC, int NT, int CHUNK, int MODE, int HEAD>
-__global__ void __launch_bounds__(NT) lambda_scan_kernel(LamArgs a, float* ws) {
-    pdl_prologue();
+// HEAD 2's operands.  The scan runs over T = T_coma - 1 rows and B = B_coma * A columns; value is unused.
+struct ComaLamArgs : LamArgs {
+    const long long* action;  // (T+1, B)
+    const float* target_q;    // (T+1, B, N)
+    const float* q;           // (T+1, B, N)
+    long long A;              // agents: reward column of scan column c is c / A
+    int N;
+    float* dq;    // (T, B) d loss / d q_value[t, b, a, action] for a unit upstream gradient
+    float* dret;  // nullable (T, B): d loss / d G, for callers that differentiate the returns
+};
+
+template <int TC, int NT, int CHUNK, int MODE, int HEAD, class Args>
+__device__ __forceinline__ void lambda_scan(const Args& a, float* ws) {
     // Chunks of CHUNK time steps, newest first, double-buffered: while the TC scan lanes run the dependent chain of chunk k
     // out of shared memory, every thread already has the global loads of chunk k+1 in flight (U elements per thread in
     // registers); they are turned into the scan's operands and written to the other buffer once the scan is done.  (Without
@@ -810,8 +823,17 @@ __global__ void __launch_bounds__(NT) lambda_scan_kernel(LamArgs a, float* ws) {
             x.l[u] = a.lambda;
             if (x.ok[u]) {
                 const long long off = t * B + c;
-                x.rw[u] = a.reward[off];
-                x.vn[u] = a.value[off + B];  // V_{t+1}
+                if constexpr (HEAD == 2) {
+                    const long long nx = off + B;  // (t+1, c): the bootstrap value gathered through the action index
+                    x.rw[u] = a.reward[t * (B / a.A) + c / a.A];
+                    x.vn[u] = a.target_q[nx * a.N + a.action[nx]];
+                    x.hv[u] = a.q[off * a.N + a.action[off]];
+                    x.hw[u] = a.weight ? a.weight[off] : 1.f;
+                    continue;
+                } else {
+                    x.rw[u] = a.reward[off];
+                    x.vn[u] = a.value[off + B];  // V_{t+1}
+                }
                 if (MODE == 1) {
                     if (t < T - 1) {
                         x.r2[u] = a.reward[off + B];
@@ -844,7 +866,7 @@ __global__ void __launch_bounds__(NT) lambda_scan_kernel(LamArgs a, float* ws) {
             }
             const float m = a.done ? fsub(1.f, x.dn[u]) : 1.f;
             const float disc = fmul(gg, ll);
-            if (HEAD == 1) {
+            if (HEAD != 0) {
                 s_hv[r][cc] = x.hv[u];
                 s_hw[r][cc] = x.hw[u];
             }
@@ -919,6 +941,14 @@ __global__ void __launch_bounds__(NT) lambda_scan_kernel(LamArgs a, float* ws) {
                 acc[0] += w * d * d;
                 a.dvalue[off] = -w * d / (float)(T * B);  // 0.5 * w * 2 * (V - G) / count
             }
+            if constexpr (HEAD == 2) {
+                const float w = s_hw[r][cc];
+                const float d = gret - s_hv[r][cc];
+                acc[0] += w * d * d;
+                const float g = 2.f * w * d / (float)(T * B);  // w * 2 * (G - q) / count
+                a.dq[off] = -g;
+                if (a.dret) a.dret[off] = g;
+            }
         }
         if (have_next) commit(buf ^ 1, nlo, nx);
         __syncthreads();
@@ -931,6 +961,22 @@ __global__ void __launch_bounds__(NT) lambda_scan_kernel(LamArgs a, float* ws) {
         if (grid_sum<1, NT>(acc, tot, ws, 0) && threadIdx.x == 0)
             a.loss[0] = (float)(0.5 * tot[0] / ((double)T * (double)B));
     }
+    if constexpr (HEAD == 2) {
+        double tot[1];
+        if (grid_sum<1, NT>(acc, tot, ws, 0) && threadIdx.x == 0) a.loss[0] = (float)(tot[0] / ((double)T * (double)B));
+    }
+}
+
+template <int TC, int NT, int CHUNK, int MODE, int HEAD>
+__global__ void __launch_bounds__(NT) lambda_scan_kernel(LamArgs a, float* ws) {
+    pdl_prologue();
+    lambda_scan<TC, NT, CHUNK, MODE, HEAD>(a, ws);
+}
+
+template <int TC, int NT, int CHUNK>
+__global__ void __launch_bounds__(NT) lambda_scan_coma_kernel(ComaLamArgs a, float* ws) {
+    pdl_prologue();
+    lambda_scan<TC, NT, CHUNK, 0, 2>(a, ws);
 }
 
 // Backward of the lambda-return scan (generalized_lambda_returns is differentiable in the reference, td.py:1574-1651; MBSAC
@@ -1256,6 +1302,25 @@ extern "C" int b200rl_td_lambda_fwd(const float* value, const float* reward, con
     if (!ws_partials_fit((long long)(div_up(B, 8)), workspace_bytes)) return B200RL_ERR_WORKSPACE;
     return launch_lambda<0, 1>(a, workspace, (cudaStream_t)stream);
 }
+
+// COMA's value half (HEAD 2): T, B, A, N are coma_error's (T, B, A, N); the scan covers rows t < T-1.  Launched by
+// b200rl_coma_fwd (csrc/pg.cu) ahead of the policy head, which reads dq.
+namespace b200rl {
+int launch_coma_value(const float* q, const float* target_q, const long long* action, const float* reward,
+                      const float* weight, double gamma, double lambda_, long long T, long long B, long long A, long long N,
+                      float* loss, float* dq, float* dret, float* ws, size_t ws_bytes, cudaStream_t st) {
+    ComaLamArgs a{};
+    a.reward = reward; a.weight = weight; a.gamma = (float)gamma; a.lambda = (float)lambda_;
+    a.T = T - 1; a.B = B * A; a.loss = loss;
+    a.action = action; a.target_q = target_q; a.q = q; a.A = A; a.N = (int)N; a.dq = dq; a.dret = dret;
+    if (a.B >= 16 * 2 * NUM_SMS) {
+        if (!ws_partials_fit(div_up(a.B, 16), ws_bytes)) return B200RL_ERR_WORKSPACE;
+        return launch_k(lambda_scan_coma_kernel<16, 256, 64>, div_up(a.B, 16), 256, 0, st, a, ws);
+    }
+    if (!ws_partials_fit(div_up(a.B, 8), ws_bytes)) return B200RL_ERR_WORKSPACE;
+    return launch_k(lambda_scan_coma_kernel<8, 256, 128>, div_up(a.B, 8), 256, 0, st, a, ws);
+}
+}  // namespace b200rl
 
 extern "C" int b200rl_scale(const float* g, const float* in, float* out, long long n, void* stream) {
     if (n < 0 || !g || (n > 0 && (!in || !out))) return B200RL_ERR_ARG;

@@ -20,10 +20,11 @@ def _originals():
     """name -> set of objects that count as 'the reference implementation' of that name."""
     found = {}
     base = sys.modules.get('ding.rl_utils')
-    for name in _ours.HOT_PATH_FUNCTIONS + _ours.LM_HOT_PATH_FUNCTIONS:
+    for name in _ours.HOT_PATH_FUNCTIONS + _ours.LM_HOT_PATH_FUNCTIONS + _ours.COMA_HOT_PATH_FUNCTIONS:
         objs = set()
         cands = [base] + [sys.modules.get('ding.rl_utils.' + m) for m in ('gae', 'ppo', 'td', 'vtrace', 'upgo', 'a2c', 'retrace', 'happo', 'acer', 'ppg',
-                                                                          'grpo', 'rloo', 'log_prob_utils', 'value_rescale')]
+                                                                          'grpo', 'rloo', 'log_prob_utils', 'value_rescale',
+                                                                          'coma')]
         for mod in cands:
             fn = getattr(mod, name, None) if mod is not None else None
             if fn is not None and fn is not getattr(_ours, name):

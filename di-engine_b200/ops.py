@@ -186,6 +186,7 @@ _HINT_INIT = {
     'happo_policy': [1.0, 0.0, -0.01, 0.0],
     'ppoc_policy': [1.0, 0.0, -0.01, 0.0],
     'vtrace': [1.0, 0.5, -0.01],
+    'coma': [0.001, 1.0, -0.01, 0.0],  # COMAPolicy: policy_weight, value_weight, -entropy_weight (policy/coma.py:77-81, 213-214)
 }
 _HINT = {}
 
@@ -1119,6 +1120,75 @@ def upgo_bwd_(logit, action, mask, adv, pg, TB, K, N, skip, grad):
         )
     _lib.check(rc, 'b200rl_upgo_head_bwd')
     return grad
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# COMA (coma.py:10-58): the value half on the lambda-return scan (td.cu, HEAD 2), the policy half on a row head (pg.cu)
+# ----------------------------------------------------------------------------------------------------------------
+def coma_fwd_(logit, q_value, target_q, action, reward, weight, T, B, A, N, gamma, lambda_, want_grad, want_dret):
+    """The forward launch of coma_error (COMAFunction and the ``b200rl::coma_fwd`` custom op).
+    -> (out (3,): policy, value, entropy loss; adv (T*B*A); dq ((T-1)*B*A); dret or None; (grad_logit, grad_q_value,
+    g_used) or None)."""
+    dev = logit.device
+    out = torch.empty(3, dtype=torch.float32, device=dev)
+    adv = torch.empty(T * B * A, dtype=torch.float32, device=dev)
+    dq = torch.empty((T - 1) * B * A, dtype=torch.float32, device=dev)
+    dret = torch.empty_like(dq) if want_dret else None
+    spec = (torch.empty_like(logit), torch.empty_like(q_value),
+            torch.empty(4, dtype=torch.float32, device=dev)) if want_grad else None
+    with on_device(dev):
+        ws = workspace(dev)
+        gl, gq, g_used = spec if want_grad else (None, None, None)
+        rc = lib().b200rl_coma_fwd(ptr(logit), ptr(q_value), ptr(target_q), ptr(action), ptr(reward), ptr(weight), T, B, A, N,
+                                   float(gamma), float(lambda_), ptr(ppo_hint(dev, 'coma')) if want_grad else None,
+                                   ptr(g_used), ptr(out), ptr(adv), ptr(dq), ptr(dret), ptr(gl), ptr(gq), ptr(ws),
+                                   ws.numel() * 4, stream_ptr())
+    _lib.check(rc, 'b200rl_coma_fwd')
+    return out, adv, dq, dret, spec
+
+
+def coma_bwd_(logit, action, weight, adv, dq, T, B, A, N, upstream, spec):
+    """The verify launch of coma_error into ``spec`` = (grad_logit, grad_q_value, g_used) -- the forward-written buffers and
+    their record, or fresh buffers and None (recompute).  ``upstream``: pointers of the policy, value and entropy gradients."""
+    gl, gq, g_used = spec
+    with on_device(logit.device):
+        rc = lib().b200rl_coma_bwd(ptr(logit), ptr(action), ptr(weight), ptr(adv), ptr(dq), T, B, A, N, *upstream,
+                                   ptr(g_used), ptr(ppo_hint(logit.device, 'coma')), ptr(gl), ptr(gq), stream_ptr())
+    _lib.check(rc, 'b200rl_coma_bwd')
+    return gl, gq
+
+
+class COMAFunction(torch.autograd.Function):
+    """coma_error's three differentiable 0-dim losses.  Gradients reach logit (policy and entropy terms) and q_value (the value
+    loss, at the action column of rows t < T-1).  ``ret`` is None, or the differentiable lambda-return (T-1, B*A) that a
+    caller builds when target_q_value / reward require grad: it receives d q_value_loss / d G (the returns themselves are
+    recomputed in the kernel).  One forward launch pair writes the losses and the gradients for the ``'coma'`` record; one
+    verify launch backward."""
+
+    @staticmethod
+    def forward(ctx, logit, q_value, target_q, action, reward, weight, ret, T, B, A, N, gamma, lambda_):
+        want = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        out, adv, dq, dret, spec = coma_fwd_(logit, q_value, target_q, action, reward, weight, T, B, A, N, gamma, lambda_,
+                                             want, ret is not None)
+        ctx.save_for_backward(logit, action, weight, adv, dq, dret)
+        ctx.cfg = (T, B, A, N)
+        ctx.spec = spec
+        ctx.set_materialize_grads(False)
+        return out[0], out[1], out[2]
+
+    @staticmethod
+    def backward(ctx, g_p, g_v, g_e):
+        logit, action, weight, adv, dq, dret = ctx.saved_tensors
+        T, B, A, N = ctx.cfg
+        need = ctx.needs_input_grad
+        keep, upstream = _grads(g_p, g_v, g_e)
+        gl = gq = g_ret = None
+        if need[0] or need[1]:
+            spec = _forward_grads(ctx) or (torch.empty_like(logit), torch.empty_like(logit), None)
+            gl, gq = coma_bwd_(logit, action, weight, adv, dq, T, B, A, N, upstream, spec)
+        if need[6] and g_v is not None:
+            g_ret = scale_(upstream[1], dret).view(T - 1, B * A)
+        return (gl, gq, None, None, None, None, g_ret) + (None, ) * 6
 
 
 class A2CFunction(torch.autograd.Function):

@@ -2,6 +2,7 @@
 namedtuples, computed by the sm_90a kernels behind the C ABI of ``include/b200rl.h``."""
 from .a2c import a2c_data, a2c_error, a2c_error_continuous, a2c_loss
 from .acer import acer_policy_error, acer_trust_region_update, acer_value_error
+from .coma import coma_data, coma_error, coma_loss
 from .fused import gae_ppo_error
 from .happo import (happo_data, happo_error, happo_error_continuous, happo_policy_error_continuous, happo_info, happo_loss, happo_policy_data, happo_policy_error, happo_policy_loss,
                     happo_value_data, happo_value_error)
@@ -57,3 +58,5 @@ LM_HOT_PATH_FUNCTIONS = [
     'grpo_policy_error', 'rloo_policy_error', 'naive_method', 'efficient_method', 'less_efficient_method'
 ]
 LM_HOT_PATH_TYPES = ['grpo_policy_data', 'grpo_info', 'rloo_policy_data', 'rloo_info']
+# COMA (ding/rl_utils/coma.py), listed apart for the same reason; install() rebinds it with the lists above
+COMA_HOT_PATH_FUNCTIONS = ['coma_error']

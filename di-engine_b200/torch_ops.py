@@ -4,7 +4,7 @@ q_nstep_td_error_with_rescale, dist_nstep_td_error, td_lambda_error, upgo_loss, 
 language-model losses on (B, S, V) logits (grpo_policy_error, rloo_policy_error, the log-prob methods, ppo_policy_error /
 ppo_error / a2c_error on token rows, ppo_value_error), the advantage recomputes (gae_returns, ppof_gae_returns,
 normalize_advantage, ppo_error_adv_norm), symlog / inv_symlog, the quantile TD losses (QR-DQN, IQN, FQF) and the
-continuous-action PPO losses without a graph break, and ``mode="reduce-overhead"`` can replay a compiled learner step as
+continuous-action PPO losses and COMA's loss without a graph break, and ``mode="reduce-overhead"`` can replay a compiled learner step as
 a CUDA graph.
 
 Each op's implementation is the launch function ``ops`` runs in eager mode; ``rl_utils`` calls the wrappers at the bottom
@@ -910,6 +910,64 @@ ppoc_loss.register_autograd(_ppoc_backward, setup_context=_ppoc_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# coma_error (csrc/td.cu HEAD 2 + csrc/pg.cu): as ppoc, the forward launch writes the gradients for the 'coma' record
+# whenever a gradient is wanted, so the backward op always verifies a copy.  The differentiable-returns path (target_q_value
+# or reward requiring grad) is not traced: it runs generalized_lambda_returns' autograd function, as in eager mode
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::coma_fwd', mutates_args=())
+def coma_fwd(logit: Tensor, q_value: Tensor, target_q: Tensor, action: Tensor, reward: Tensor, weight: Optional[Tensor],
+             T: int, B: int, A: int, N: int, gamma: float, lambda_: float,
+             want_grad: bool) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """-> (policy / value / entropy loss, adv, dq, grad_logit, grad_q_value, g_used); the last three are empty without
+    ``want_grad``"""
+    out, adv, dq, _, spec = ops.coma_fwd_(logit, q_value, target_q, action, reward, weight, T, B, A, N, gamma, lambda_,
+                                          want_grad, False)
+    if not want_grad:
+        return (out, adv, dq) + (_empty(out), ) * 3
+    return (out, adv, dq) + spec
+
+
+@coma_fwd.register_fake
+def _(logit, q_value, target_q, action, reward, weight, T, B, A, N, gamma, lambda_, want_grad):
+    out = logit.new_empty(3)
+    adv, dq = logit.new_empty(T * B * A), logit.new_empty((T - 1) * B * A)
+    if not want_grad:
+        return (out, adv, dq) + (_empty(out), ) * 3
+    return out, adv, dq, torch.empty_like(logit), torch.empty_like(q_value), out.new_empty(4)
+
+
+@torch.library.custom_op('b200rl::coma_bwd', mutates_args=())
+def coma_bwd(logit: Tensor, action: Tensor, weight: Optional[Tensor], adv: Tensor, dq: Tensor, g_out: Tensor,
+             grad_logit: Tensor, grad_q: Tensor, g_used: Tensor, T: int, B: int, A: int, N: int) -> tuple[Tensor, Tensor]:
+    """-> (grad_logit, grad_q_value) for the upstream gradients g_out[0:3] of policy, value and entropy loss"""
+    keep, upstream = _upstream(g_out, 3)
+    spec = _forward_grads(True, g_used, grad_logit, grad_q)
+    return ops.coma_bwd_(logit, action, weight, adv, dq, T, B, A, N, upstream, spec)
+
+
+@coma_bwd.register_fake
+def _(logit, action, weight, adv, dq, g_out, grad_logit, grad_q, *args):
+    return torch.empty_like(logit), torch.empty_like(grad_q)
+
+
+def _coma_setup(ctx, inputs, output):
+    logit, q_value, target_q, action, reward, weight = inputs[:6]
+    ctx.save_for_backward(logit, action, weight, *output[1:])
+    ctx.cfg = inputs[6:10]
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[1:])
+
+
+def _coma_backward(ctx, g_out, *_):
+    if g_out is None:
+        return (None, ) * 13
+    return coma_bwd(*ctx.saved_tensors[:5], g_out, *ctx.saved_tensors[5:], *ctx.cfg) + (None, ) * 11
+
+
+coma_fwd.register_autograd(_coma_backward, setup_context=_coma_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # what rl_utils calls while compiling: the autograd.Function signatures of ops, on the ops above
 # ---------------------------------------------------------------------------------------------------------------------
 def _want_grad(*xs):
@@ -1030,3 +1088,10 @@ def ppo_continuous(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, a
     return ppoc_loss(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight,
                      factor, S, D, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind,
                      _want_grad(mu, sigma, value_new))[0]
+
+
+def coma(logit, q_value, target_q, action, reward, weight, T, B, A, N, gamma, lambda_):
+    """-> (policy_loss, q_value_loss, entropy_loss), as COMAFunction without the differentiable returns"""
+    out = coma_fwd(logit, q_value, target_q, action, reward, weight, T, B, A, N, float(gamma), float(lambda_),
+                   _want_grad(logit, q_value))[0]
+    return out[0], out[1], out[2]

@@ -295,6 +295,29 @@ B200RL_API int b200rl_td_lambda_fwd(const float* value, const float* reward, con
 /* out[i] = (*g) * in[i] -- backward of heads whose forward saved the unit-upstream gradient */
 B200RL_API int b200rl_scale(const float* g, const float* in, float* out, long long n, void* stream);
 
+/* ---- coma_error: ding/rl_utils/coma.py:10-58 ----------------------------------------------------------------------------
+ * logit, q_value, target_q_value: (T, B, A, N); action: (T, B, A) int64; reward: (T, B); weight (nullable = 1): (T, B, A).
+ * T >= 2 (the reference's lambda-return over T - 1 rows indexes an empty tensor at T = 1).  Two launches:
+ *   the value half, td.cu's lambda-return scan with a COMA head (coma.py:45-52): G = generalized_lambda_returns(
+ *   target_q_value gathered at action, reward broadcast over the A agents) over rows t < T-1, read in place;
+ *   out3[1] = q_value_loss = mean(w*(G - q_taken)^2); dq_saved ((T-1)*B*A) = d q_value_loss / d q_taken; dret (nullable,
+ *   same shape) = d q_value_loss / d G, for a caller that differentiates the returns;
+ *   the policy half, one warp per (t, b, a) row (coma.py:53-57): adv = q_taken - sum_j softmax(logit)_j q_value_j
+ *   (detached) into adv_saved (T*B*A); out3[0] = policy_loss = -mean(logp*adv*w), out3[2] = entropy_loss = mean(H*w).
+ * Forward-written gradients as b200rl_a2c_fwd_grad (slots policy, value, entropy): with grad_logit / grad_q_value (both
+ * or neither, each (T, B, A, N)) the forward launch writes them for the upstream gradients g_expected and records them in
+ * g_used; b200rl_coma_bwd is the verify launch -- it returns at once when g_policy / g_value / g_entropy equal the
+ * record and recomputes otherwise.  No gradient reaches q_value through the baseline or adv. */
+B200RL_API int b200rl_coma_fwd(const float* logit, const float* q_value, const float* target_q_value, const long long* action,
+                    const float* reward, const float* weight, long long T, long long B, long long A, long long N,
+                    double gamma, double lambda_, const float* g_expected, float* g_used, float* out3, float* adv_saved,
+                    float* dq_saved, float* dret, float* grad_logit, float* grad_q_value, float* workspace,
+                    size_t workspace_bytes, void* stream);
+B200RL_API int b200rl_coma_bwd(const float* logit, const long long* action, const float* weight, const float* adv_saved,
+                    const float* dq_saved, long long T, long long B, long long A, long long N, const float* g_policy,
+                    const float* g_value, const float* g_entropy, const float* g_used, float* g_hint, float* grad_logit,
+                    float* grad_q_value, void* stream);
+
 /* ---- upgo_loss head: ding/rl_utils/upgo.py:77-111 (tb_cross_entropy :7-43) --------------------------------------
  * logit: (TB*K, N) with K = 1 for (T,B,N) logits or N2 for (T,B,N2,N); action, mask(nullable): (TB*K);
  * rho, ret (from b200rl_lambda_returns upgo mode), value (= bootstrap_values[:-1]): (TB).
