@@ -12,11 +12,12 @@ dist_nstep_td_error, generalized_lambda_returns) as hand-written CUDA kernels be
 The on-disk directory is ``di-engine_b200`` (not an importable identifier); ``di_engine_b200.py`` at the repository
 root loads it under the importable name.
 """
-from . import _lib, collate, data, ops, parallel, rl_utils, torch_ops
+from . import _lib, collate, data, ops, parallel, rl_utils, torch_ops, torch_utils
 from .collate import preprocess_learn
 from .data import PackedBatch
 from .installer import install, install_hpc_rll, uninstall
 from .rl_utils import *  # noqa: F401,F403
+from .torch_utils import ScatterConnection
 
 __version__ = '0.1.0'
 

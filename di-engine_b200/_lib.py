@@ -55,6 +55,8 @@ PROTOTYPES = {
     "b200rl_upgo_head_bwd": [P, P, P, P, P, LL, LL, LL, I, P, P],
     "b200rl_coma_fwd": [P, P, P, P, P, P, LL, LL, LL, LL, D, D, P, P, P, P, P, P, P, P, P, c_size_t, P],
     "b200rl_coma_bwd": [P, P, P, P, P, LL, LL, LL, LL, P, P, P, P, P, P, P, P],
+    "b200rl_scatter_fwd": [P, LL, LL, LL, P, LL, LL, P, LL, LL, LL, LL, LL, LL, LL, I, P, P],
+    "b200rl_scatter_bwd": [P, LL, LL, LL, P, LL, LL, P, LL, LL, LL, LL, LL, LL, LL, P, P],
     "b200rl_vtrace_fwd": [P, P, P, P, P, P, LL, LL, LL, D, D, D, D, D, P, P, P, P, P, c_size_t, P],
     "b200rl_vtrace_continuous_fwd": [P, P, P, P, P, P, P, P, LL, LL, LL, D, D, D, D, D, P, P, P, P, P, c_size_t, P],
     "b200rl_vtrace_continuous_bwd": [P, P, P, P, P, P, P, P, P, LL, LL, LL, P, P, P, P],

@@ -5,6 +5,8 @@ Two routes, matching the two ways the reference reaches its operators (SURVEY.md
 * ``install()``: policies bind the operators at import time (``from ding.rl_utils import gae`` -- policy/ppo.py:8-10,
   policy/dqn.py:7, policy/c51.py:6, policy/impala.py:8 ...), so the names are rebound in ``ding.rl_utils``, its
   submodules and every already-imported ``ding.*`` / ``dizoo.*`` module that holds a reference to the original.
+  ScatterConnection is a class the models construct, so ``install()`` sets ``forward`` and ``xy_forward`` on the
+  reference class itself, which also covers instances built before the call.
 * ``install_hpc_rll()``: registers an ``hpc_rll`` module tree so that the reference's own plugin switch
   (``ENABLE_DI_HPC=true`` -> ding/hpc_rl/wrapper.py:61-83) constructs these operators as ``Class(*shape).cuda()``.
 """
@@ -12,8 +14,10 @@ import sys
 import types
 
 from . import rl_utils as _ours
+from .torch_utils import scatter_connection as _scatter
 
-_installed = []  # (module, name, original)
+_installed = []  # (module or class, name, original)
+_SCATTER_MODULE = 'ding.torch_utils.network.scatter_connection'
 
 
 def _originals():
@@ -57,7 +61,29 @@ def install(prefixes=('ding', 'dizoo'), skip_modules=(), verbose=False):
                 done.append((mod_name, name))
                 if verbose:
                     print('di_engine_b200: %s.%s -> CUDA kernel' % (mod_name, name))
+    _patch_scatter_connection(prefixes, skip_modules, done, verbose)
     return done
+
+
+def _patch_scatter_connection(prefixes, skip_modules, done, verbose):
+    """``forward`` / ``xy_forward`` of the reference's ScatterConnection class, once its module is imported"""
+    mod = sys.modules.get(_SCATTER_MODULE)
+    if mod is None or _SCATTER_MODULE in skip_modules:
+        return
+    if not any(_SCATTER_MODULE == p or _SCATTER_MODULE.startswith(p + '.') for p in prefixes):
+        return
+    cls = getattr(mod, 'ScatterConnection', None)
+    if cls is None:
+        return
+    for name, fn in (('forward', _scatter.scatter_forward), ('xy_forward', _scatter.scatter_xy_forward)):
+        cur = cls.__dict__.get(name)
+        if cur is None or cur is fn:
+            continue
+        _installed.append((cls, name, cur))
+        setattr(cls, name, fn)
+        done.append((_SCATTER_MODULE + '.ScatterConnection', name))
+        if verbose:
+            print('di_engine_b200: %s.ScatterConnection.%s -> CUDA kernel' % (_SCATTER_MODULE, name))
 
 
 def uninstall():
@@ -146,6 +172,25 @@ class VTrace(_HpcOp):
                                                   rho_pg_clip_ratio)
 
 
+class ScatterConnection(_HpcOp):
+    """Constructed as ``Class(B, M, N, H, W, scatter_type)`` (shape_fn_scatter_connection, scatter_connection.py:7-27) and
+    called as ``op(x, location)``: the wrapper keeps x and location (include_args=[0, 2], include_kwargs)."""
+
+    def __call__(self, x, location):
+        H, W, scatter_type = self.shape[3:6]
+        return _scatter.scatter_location(x, (H, W), location, scatter_type)
+
+
+class LSTM:
+    """ding/torch_utils/network/rnn.py:9-10 imports this name whenever ``ding.enable_hpc_rl`` is set; only
+    ``lstm_type='hpc'`` constructs it (:358-359).  The library has no LSTM: a dense GEMM recurrence is tensor-core work."""
+
+    def __init__(self, *args, **kwargs):
+        raise NotImplementedError("di_engine_b200 has no LSTM kernel, so lstm_type='hpc' is not available; "
+                                  "use lstm_type 'normal', 'pytorch' or 'gru'")
+
+
+_HPC_PACKAGES = ('hpc_rll.rl_utils', 'hpc_rll.torch_utils', 'hpc_rll.torch_utils.network')
 _HPC_LAYOUT = {
     'hpc_rll.rl_utils.gae': {'GAE': GAE},
     'hpc_rll.rl_utils.td': {'DistNStepTD': DistNStepTD, 'QNStepTD': QNStepTD, 'QNStepTDRescale': QNStepTDRescale,
@@ -153,6 +198,8 @@ _HPC_LAYOUT = {
     'hpc_rll.rl_utils.ppo': {'PPO': PPO},
     'hpc_rll.rl_utils.upgo': {'UPGO': UPGO},
     'hpc_rll.rl_utils.vtrace': {'VTrace': VTrace},
+    'hpc_rll.torch_utils.network.rnn': {'LSTM': LSTM},
+    'hpc_rll.torch_utils.network.scatter_connection': {'ScatterConnection': ScatterConnection},
 }
 
 
@@ -164,14 +211,19 @@ def install_hpc_rll(force=False):
     root.__b200_shim__ = True
     root.__path__ = []
     sys.modules['hpc_rll'] = root
-    sub = types.ModuleType('hpc_rll.rl_utils')
-    sub.__path__ = []
-    sys.modules['hpc_rll.rl_utils'] = sub
-    root.rl_utils = sub
+    for name in _HPC_PACKAGES:
+        _hpc_module(name).__path__ = []
     for mod_name, classes in _HPC_LAYOUT.items():
-        m = types.ModuleType(mod_name)
+        m = _hpc_module(mod_name)
         for k, v in classes.items():
             setattr(m, k, v)
-        sys.modules[mod_name] = m
-        setattr(sub, mod_name.rsplit('.', 1)[1], m)
     return root
+
+
+def _hpc_module(name):
+    """a new module ``name`` in sys.modules, bound as an attribute of its (already registered) parent"""
+    m = types.ModuleType(name)
+    sys.modules[name] = m
+    parent, _, leaf = name.rpartition('.')
+    setattr(sys.modules[parent], leaf, m)
+    return m

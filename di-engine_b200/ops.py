@@ -1191,6 +1191,55 @@ class COMAFunction(torch.autograd.Function):
         return (gl, gq, None, None, None, None, g_ret) + (None, ) * 6
 
 
+# ----------------------------------------------------------------------------------------------------------------
+# ScatterConnection (scatter_connection.py:59-121): csrc/scatter.cu.  x and the two index operands are read through their
+# strides, so a permuted x or the location[..., 0] / [..., 1] views reach the kernels without a copy
+# ----------------------------------------------------------------------------------------------------------------
+SCATTER_MODES = {'add': 0, 'cover': 1}  # B200RL_SCATTER_ADD, B200RL_SCATTER_COVER
+
+
+def scatter_fwd_(x, row, col, H, W, mode):
+    """x (B, M, N) fp32, row / col (B, M) int64 (flat index col + row * W) -> the map (B, N, H, W)"""
+    B, M, N = x.shape
+    out = torch.empty(B, N, H, W, dtype=torch.float32, device=x.device)
+    with on_device(x.device):
+        rc = lib().b200rl_scatter_fwd(ptr(x), *x.stride(), ptr(row), *row.stride(), ptr(col), *col.stride(), B, M, N, H, W,
+                                      mode, ptr(out), stream_ptr())
+    _lib.check(rc, 'b200rl_scatter_fwd')
+    return out
+
+
+def scatter_bwd_(g, row, col, M, H, W):
+    """g (B, N, H, W), the gradient of the map -> d x (B, M, N): g gathered at each entity's index (0 where it is out of
+    range).  The kernels take the cell stride of g viewed as (B, N, H*W): reshape keeps g's memory when its H and W merge
+    into one stride (an expanded gradient costs no copy) and copies otherwise.  The strides of size-1 dims do not describe
+    the layout, so they are never read on their own: at W = 1 the cells step by g.stride(2)."""
+    B, N = g.shape[0], g.shape[1]
+    g = g.float().reshape(B, N, H * W)
+    dx = torch.empty(B, M, N, dtype=torch.float32, device=g.device)
+    with on_device(g.device):
+        rc = lib().b200rl_scatter_bwd(ptr(g), *g.stride(), ptr(row), *row.stride(), ptr(col), *col.stride(), B, M, N, H, W,
+                                      ptr(dx), stream_ptr())
+    _lib.check(rc, 'b200rl_scatter_bwd')
+    return dx
+
+
+class ScatterFunction(torch.autograd.Function):
+    """ScatterConnection's map from x; location gets no gradient.  One launch forward, one launch backward."""
+
+    @staticmethod
+    def forward(ctx, x, row, col, H, W, mode):
+        ctx.save_for_backward(row, col)
+        ctx.cfg = (x.shape[1], H, W)
+        return scatter_fwd_(x, row, col, H, W, mode)
+
+    @staticmethod
+    def backward(ctx, g):
+        row, col = ctx.saved_tensors
+        dx = scatter_bwd_(g, row, col, *ctx.cfg) if ctx.needs_input_grad[0] else None
+        return dx, None, None, None, None, None
+
+
 class A2CFunction(torch.autograd.Function):
     """a2c_error (ding/rl_utils/a2c.py:10-44): three differentiable 0-dim losses; gradients reach logit and value.  One launch
     forward (losses + gradients for the expected upstream gradients), one verification launch backward (csrc/heads.cu)."""

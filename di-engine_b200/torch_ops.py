@@ -4,7 +4,7 @@ q_nstep_td_error_with_rescale, dist_nstep_td_error, td_lambda_error, upgo_loss, 
 language-model losses on (B, S, V) logits (grpo_policy_error, rloo_policy_error, the log-prob methods, ppo_policy_error /
 ppo_error / a2c_error on token rows, ppo_value_error), the advantage recomputes (gae_returns, ppof_gae_returns,
 normalize_advantage, ppo_error_adv_norm), symlog / inv_symlog, the quantile TD losses (QR-DQN, IQN, FQF) and the
-continuous-action PPO losses and COMA's loss without a graph break, and ``mode="reduce-overhead"`` can replay a compiled learner step as
+continuous-action PPO losses, COMA's loss and ScatterConnection without a graph break, and ``mode="reduce-overhead"`` can replay a compiled learner step as
 a CUDA graph.
 
 Each op's implementation is the launch function ``ops`` runs in eager mode; ``rl_utils`` calls the wrappers at the bottom
@@ -965,6 +965,43 @@ def _coma_backward(ctx, g_out, *_):
 
 
 coma_fwd.register_autograd(_coma_backward, setup_context=_coma_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# ScatterConnection (csrc/scatter.cu): x and the index operands keep their strides
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::scatter_fwd', mutates_args=())
+def scatter_fwd(x: Tensor, row: Tensor, col: Tensor, H: int, W: int, mode: int) -> Tensor:
+    return ops.scatter_fwd_(x, row, col, H, W, mode)
+
+
+@scatter_fwd.register_fake
+def _(x, row, col, H, W, mode):
+    return x.new_empty(x.shape[0], x.shape[2], H, W)
+
+
+@torch.library.custom_op('b200rl::scatter_bwd', mutates_args=())
+def scatter_bwd(g: Tensor, row: Tensor, col: Tensor, M: int, H: int, W: int) -> Tensor:
+    return ops.scatter_bwd_(g, row, col, M, H, W)
+
+
+@scatter_bwd.register_fake
+def _(g, row, col, M, H, W):
+    return g.new_empty(g.shape[0], M, g.shape[1], dtype=torch.float32)
+
+
+def _scatter_setup(ctx, inputs, output):
+    x, row, col, H, W, _mode = inputs
+    ctx.save_for_backward(row, col)
+    ctx.cfg = (x.shape[1], H, W)
+
+
+def _scatter_backward(ctx, g):
+    row, col = ctx.saved_tensors
+    return scatter_bwd(g, row, col, *ctx.cfg), None, None, None, None, None
+
+
+scatter_fwd.register_autograd(_scatter_backward, setup_context=_scatter_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

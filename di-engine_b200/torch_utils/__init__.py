@@ -1,0 +1,4 @@
+"""Drop-ins for the ``ding.torch_utils`` modules behind the reference's plugin registry (ding/hpc_rl/wrapper.py:62-73)."""
+from .scatter_connection import ScatterConnection
+
+__all__ = ['ScatterConnection']

@@ -318,6 +318,27 @@ B200RL_API int b200rl_coma_bwd(const float* logit, const long long* action, cons
                     const float* g_value, const float* g_entropy, const float* g_used, float* g_hint, float* grad_logit,
                     float* grad_q_value, void* stream);
 
+/* ---- ScatterConnection: ding/torch_utils/network/scatter_connection.py:59-121 ----------------------------------------
+ * Replaces forward (:79-88) and xy_forward (:112-121): the (B, N, M) int64 index built with repeat, the zero-filled
+ * output and scatter_ / scatter_add_ from a permuted x.
+ * x: (B, M, N) fp32, read through its element strides (x_sb, x_sm, x_sn).  The flat index of entity (b, m) is
+ * idx = col[b*col_sb + m*col_sm] + row[b*row_sb + m*row_sm] * W, two int64 operands each with its own element strides:
+ * forward passes location[..., 0] / location[..., 1], xy_forward coord_x / coord_y.  Only 0 <= idx < H*W is valid, so
+ * (y, W) wraps to (y + 1, 0) as in the reference; an entity with any other idx writes nothing and gets a zero gradient.
+ * b200rl_scatter_fwd writes every element of out (B, N, H, W) dense, once: +0.0f plus the entities of each cell added in
+ * ascending m (mode B200RL_SCATTER_ADD, the CPU scatter_add_ order) or the entity of the largest m (B200RL_SCATTER_COVER,
+ * the CPU scatter_'s result).  Deterministic: no value goes through an atomic.
+ * b200rl_scatter_bwd writes grad_x (B, M, N) dense: grad_x[b, m, n] = g[b*g_sb + n*g_sn + idx*g_sc] (the gradient of both
+ * modes with respect to the source, a gather; covered entities receive their cell's gradient too).  One launch each. */
+#define B200RL_SCATTER_ADD 0
+#define B200RL_SCATTER_COVER 1
+B200RL_API int b200rl_scatter_fwd(const float* x, long long x_sb, long long x_sm, long long x_sn, const long long* row,
+                    long long row_sb, long long row_sm, const long long* col, long long col_sb, long long col_sm,
+                    long long B, long long M, long long N, long long H, long long W, int mode, float* out, void* stream);
+B200RL_API int b200rl_scatter_bwd(const float* g, long long g_sb, long long g_sn, long long g_sc, const long long* row,
+                    long long row_sb, long long row_sm, const long long* col, long long col_sb, long long col_sm,
+                    long long B, long long M, long long N, long long H, long long W, float* grad_x, void* stream);
+
 /* ---- upgo_loss head: ding/rl_utils/upgo.py:77-111 (tb_cross_entropy :7-43) --------------------------------------
  * logit: (TB*K, N) with K = 1 for (T,B,N) logits or N2 for (T,B,N2,N); action, mask(nullable): (TB*K);
  * rho, ret (from b200rl_lambda_returns upgo mode), value (= bootstrap_values[:-1]): (TB).
