@@ -57,6 +57,9 @@ PROTOTYPES = {
     "b200rl_coma_bwd": [P, P, P, P, P, LL, LL, LL, LL, P, P, P, P, P, P, P, P],
     "b200rl_scatter_fwd": [P, LL, LL, LL, P, LL, LL, P, LL, LL, LL, LL, LL, LL, LL, I, P, P],
     "b200rl_scatter_bwd": [P, LL, LL, LL, P, LL, LL, P, LL, LL, LL, LL, LL, LL, LL, P, P],
+    "b200rl_lnlstm_step_fwd": [P, LL, LL, P, LL, LL, P, LL, P, LL, P, LL, P, LL, P, LL, P, LL, LL, LL, LL, P, LL, LL, P, LL, LL, P, LL, LL, P, LL, LL, P, LL, P],
+    "b200rl_lnlstm_step_bwd": [P, LL, LL, P, LL, LL, P, LL, LL, P, LL, LL, P, LL, LL, P, LL, P, LL, P, LL, P, LL, P, LL, P, LL, P, LL, LL, P, LL, LL, LL, LL, P, LL, LL, P, LL, LL, P, LL, LL, P, LL, LL, P],
+    "b200rl_lnlstm_param_grads": [P, LL, LL, P, LL, LL, P, LL, LL, P, LL, LL, LL, P, LL, P, LL, P, LL, P],
     "b200rl_vtrace_fwd": [P, P, P, P, P, P, LL, LL, LL, D, D, D, D, D, P, P, P, P, P, c_size_t, P],
     "b200rl_vtrace_continuous_fwd": [P, P, P, P, P, P, P, P, LL, LL, LL, D, D, D, D, D, P, P, P, P, P, c_size_t, P],
     "b200rl_vtrace_continuous_bwd": [P, P, P, P, P, P, P, P, P, LL, LL, LL, P, P, P, P],

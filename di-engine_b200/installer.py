@@ -6,7 +6,8 @@ Two routes, matching the two ways the reference reaches its operators (SURVEY.md
   policy/dqn.py:7, policy/c51.py:6, policy/impala.py:8 ...), so the names are rebound in ``ding.rl_utils``, its
   submodules and every already-imported ``ding.*`` / ``dizoo.*`` module that holds a reference to the original.
   ScatterConnection is a class the models construct, so ``install()`` sets ``forward`` and ``xy_forward`` on the
-  reference class itself, which also covers instances built before the call.
+  reference class itself, which also covers instances built before the call.  The layer-normalised LSTM is one too:
+  ``install()`` sets ``forward`` on ``ding.torch_utils.network.rnn.LSTM``.
 * ``install_hpc_rll()``: registers an ``hpc_rll`` module tree so that the reference's own plugin switch
   (``ENABLE_DI_HPC=true`` -> ding/hpc_rl/wrapper.py:61-83) constructs these operators as ``Class(*shape).cuda()``.
 """
@@ -14,10 +15,12 @@ import sys
 import types
 
 from . import rl_utils as _ours
+from .torch_utils import lstm as _lstm
 from .torch_utils import scatter_connection as _scatter
 
 _installed = []  # (module or class, name, original)
 _SCATTER_MODULE = 'ding.torch_utils.network.scatter_connection'
+_RNN_MODULE = 'ding.torch_utils.network.rnn'
 
 
 def _originals():
@@ -62,6 +65,7 @@ def install(prefixes=('ding', 'dizoo'), skip_modules=(), verbose=False):
                 if verbose:
                     print('di_engine_b200: %s.%s -> CUDA kernel' % (mod_name, name))
     _patch_scatter_connection(prefixes, skip_modules, done, verbose)
+    _patch_lstm(prefixes, skip_modules, done, verbose)
     return done
 
 
@@ -84,6 +88,25 @@ def _patch_scatter_connection(prefixes, skip_modules, done, verbose):
         done.append((_SCATTER_MODULE + '.ScatterConnection', name))
         if verbose:
             print('di_engine_b200: %s.ScatterConnection.%s -> CUDA kernel' % (_SCATTER_MODULE, name))
+
+
+def _patch_lstm(prefixes, skip_modules, done, verbose):
+    """``forward`` of the reference's layer-normalised LSTM class (lstm_type='normal'), once rnn.py is imported.  The
+    patched forward hands every call the kernels do not compute (not CUDA fp32, not affine LayerNorm) to this original."""
+    mod = sys.modules.get(_RNN_MODULE)
+    if mod is None or _RNN_MODULE in skip_modules:
+        return
+    if not any(_RNN_MODULE == p or _RNN_MODULE.startswith(p + '.') for p in prefixes):
+        return
+    cls = getattr(mod, 'LSTM', None)
+    cur = cls.__dict__.get('forward') if cls is not None else None
+    if cur is None or hasattr(cur, '__b200_original__'):
+        return
+    _installed.append((cls, 'forward', cur))
+    cls.forward = _lstm.patched_forward(cur)
+    done.append((_RNN_MODULE + '.LSTM', 'forward'))
+    if verbose:
+        print('di_engine_b200: %s.LSTM.forward -> CUDA kernels' % _RNN_MODULE)
 
 
 def uninstall():
@@ -183,11 +206,12 @@ class ScatterConnection(_HpcOp):
 
 class LSTM:
     """ding/torch_utils/network/rnn.py:9-10 imports this name whenever ``ding.enable_hpc_rl`` is set; only
-    ``lstm_type='hpc'`` constructs it (:358-359).  The library has no LSTM: a dense GEMM recurrence is tensor-core work."""
+    ``lstm_type='hpc'`` constructs it (:358-359), with extra sequence and batch sizes this shim does not take.  The
+    library's LSTM is ``lstm_type='normal'`` itself, whose ``forward`` ``install()`` patches."""
 
     def __init__(self, *args, **kwargs):
-        raise NotImplementedError("di_engine_b200 has no LSTM kernel, so lstm_type='hpc' is not available; "
-                                  "use lstm_type 'normal', 'pytorch' or 'gru'")
+        raise NotImplementedError("di_engine_b200 has no hpc LSTM, so lstm_type='hpc' is not available; "
+                                  "use lstm_type 'normal', 'pytorch' or 'gru' (install() runs 'normal' on the library)")
 
 
 _HPC_PACKAGES = ('hpc_rll.rl_utils', 'hpc_rll.torch_utils', 'hpc_rll.torch_utils.network')

@@ -1240,6 +1240,146 @@ class ScatterFunction(torch.autograd.Function):
         return dx, None, None, None, None, None
 
 
+# ----------------------------------------------------------------------------------------------------------------
+# The layer-normalised LSTM (rnn.py:131-239, lstm_type='normal', norm_type='LN'): csrc/lstm.cu runs everything between
+# the GEMMs, one launch per step in each direction; the GEMMs are torch.mm on the current stream (cuBLAS)
+# ----------------------------------------------------------------------------------------------------------------
+def _vec(t):
+    return (ptr(t), t.stride(0))
+
+
+def _mat(t):
+    return (ptr(t), t.stride(0), t.stride(1))
+
+
+_NO_MAT = (None, 0, 0)
+
+
+def _rows_mm(a, b, T):
+    """a @ b for the backward GEMMs whose rows are all T*B rows of a layer (dX, dWx, dWh).  At T = 1 they are the
+    reference's own per-step shapes and run in fp32.  Above, they run in float64 and round once: on an H100 an fp32 cuBLAS
+    GEMM of (1600, 512) x (512, 2048) measured about 5x the max error of a (64, 512) x (512, 2048) one, and in fp32 dX and
+    dWx exceeded the reference's error after 25 and 80 steps."""
+    if T == 1:
+        return torch.mm(a, b)
+    return torch.mm(a.double(), b.double()).float()
+
+
+_F32 = 4  # bytes per element: the per-step operands are addressed as base pointer + offset, without a tensor view each
+
+
+def lnlstm_fwd_(x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, save):
+    """One layer over x (T, B, I) from the state h0, c0 (B, H) -> (y (T, B, H), h_T, c_T, GX, GH, C, stats).
+    GX = x Wx (T, B, 4H) is one GEMM, in float64 rounded once at every T: in fp32, even at T = 1 where its shape is the
+    reference's, 80 chained one-step calls (a recurrent learner's unroll) ended 3.6x further from float64 than the reference,
+    with x Wx rounded once they stay within it.  GH[t] = h_{t-1} Wh is one fp32 GEMM per step.  C (T, B, H) holds
+    c_1..c_T.  With ``save`` GH keeps every step and stats (T, B, 4) the LayerNorm statistics the backward reads; without
+    it GH is one step's scratch and stats is None."""
+    T, B, I = x.shape
+    if T == 0:
+        raise ValueError("di_engine_b200: the LSTM needs at least one time step (got an input of shape %s)" %
+                         (tuple(x.shape), ))
+    H = wh.shape[0]
+    G = 4 * H
+    GX = torch.mm(x.reshape(T * B, I).double(), wx.double()).float().view(T, B, G)
+    y = GX.new_empty(T, B, H)
+    hT = GX.new_empty(B, H)
+    cT = GX.new_empty(B, H)
+    C = GX.new_empty(T, B, H) if save or T > 1 else cT.view(1, B, H)  # c_1 of a one-step call without backward is c_T
+    GH = GX.new_empty(T if save else 1, B, G)
+    stats = GX.new_empty(T, B, 4) if save else None
+    params = _vec(gamma_x) + _vec(beta_x) + _vec(gamma_h) + _vec(beta_h) + _vec(bias)
+    p_gx, p_gh, p_y, p_c, p_st, p_ct = ptr(GX), ptr(GH), ptr(y), ptr(C), ptr(stats), ptr(cT)
+    fn = lib().b200rl_lnlstm_step_fwd
+    with on_device(x.device):
+        st = stream_ptr()
+        for t in range(T):
+            last = t == T - 1
+            s = t if save else 0
+            torch.mm(h0 if t == 0 else y[t - 1], wh, out=GH[s])
+            cp = _mat(c0) if t == 0 else (p_c + (t - 1) * B * H * _F32, H, 1)
+            rc = fn(p_gx + t * B * G * _F32, G, 1, p_gh + s * B * G * _F32, G, 1, *params, *cp, B, H,
+                    p_y + t * B * H * _F32, H, 1, p_c + t * B * H * _F32, H, 1, *(_mat(hT) if last else _NO_MAT),
+                    *(_mat(cT) if last and C.data_ptr() != p_ct else _NO_MAT), p_st + t * B * 4 * _F32 if save else None,
+                    4, st)
+            _lib.check(rc, 'b200rl_lnlstm_step_fwd')
+    return y, hT, cT, GX, GH, C, stats
+
+
+def lnlstm_bwd_(g_y, g_hT, g_cT, x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, y, GX, GH, C, stats, needs):
+    """The gradients of ``lnlstm_fwd_``'s (y, h_T, c_T) -> one per input (x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h,
+    beta_h), None where ``needs`` is false.  Any upstream gradient may be None (zero).  One step launch per step, then
+    dX = DGX Wx^T, dWx = X^T DGX, dWh = H_prev^T DGH over all T*B rows (``_rows_mm``) and one launch for the LayerNorm
+    parameters."""
+    T, B, I = x.shape
+    H = wh.shape[0]
+    G = 4 * H
+    D = GX.new_empty(3, T, B, G)  # DGX, DGH, DG (the pre-activation's gradient)
+    W = GX.new_empty(2, B, H)  # dc, and the recurrent term d_gh[t+1] Wh^T
+    DGX, DGH = D[0], D[1]
+    params = _vec(gamma_x) + _vec(beta_x) + _vec(gamma_h) + _vec(beta_h) + _vec(bias)
+    p_d, p_w, p_gx, p_gh, p_c, p_st = ptr(D), ptr(W), ptr(GX), ptr(GH), ptr(C), ptr(stats)
+    if g_y is not None:
+        p_gy, gy_st = ptr(g_y), g_y.stride()
+    L = lib()
+    grads = [None] * 10
+    with on_device(x.device):
+        st = stream_ptr()
+        for t in reversed(range(T)):
+            if t == T - 1:
+                rec = _mat(g_hT) if g_hT is not None else _NO_MAT
+                dc_in = _mat(g_cT) if g_cT is not None else _NO_MAT
+            else:
+                torch.mm(DGH[t + 1], wh.t(), out=W[1])
+                rec, dc_in = (p_w + B * H * _F32, H, 1), (p_w, H, 1)
+            dy = (p_gy + t * gy_st[0] * _F32, gy_st[1], gy_st[2]) if g_y is not None else _NO_MAT
+            cp = _mat(c0) if t == 0 else (p_c + (t - 1) * B * H * _F32, H, 1)
+            step = t * B * G * _F32
+            rc = L.b200rl_lnlstm_step_bwd(*dy, *rec, *dc_in, p_gx + step, G, 1, p_gh + step, G, 1,
+                                          p_st + t * B * 4 * _F32, 4, *params, *cp, p_c + t * B * H * _F32, H, 1, B, H,
+                                          p_d + step, G, 1, p_d + T * B * G * _F32 + step, G, 1,
+                                          p_d + 2 * T * B * G * _F32 + step, G, 1, p_w, H, 1, st)
+            _lib.check(rc, 'b200rl_lnlstm_step_bwd')
+        dgx = DGX.view(T * B, G)
+        if needs[0]:
+            grads[0] = _rows_mm(dgx, wx.t(), T).view(T, B, I)
+        if needs[1]:
+            grads[1] = torch.mm(DGH[0], wh.t())
+        if needs[2]:
+            grads[2] = W[0]
+        if needs[3]:
+            grads[3] = _rows_mm(x.reshape(T * B, I).t(), dgx, T)
+        if needs[4]:
+            h_prev = h0 if T == 1 else torch.cat([h0.unsqueeze(0), y[:-1]]).view(T * B, H)
+            grads[4] = _rows_mm(h_prev.t(), DGH.view(T * B, G), T)
+        if any(needs[5:]):
+            d_gamma_x, d_gamma_h, d_beta = (GX.new_empty(G) for _ in range(3))
+            rc = L.b200rl_lnlstm_param_grads(p_d + 2 * T * B * G * _F32, G, 1, p_gx, G, 1, p_gh, G, 1, p_st, 4, T * B, H,
+                                             *_vec(d_gamma_x), *_vec(d_gamma_h), *_vec(d_beta), st)
+            _lib.check(rc, 'b200rl_lnlstm_param_grads')
+            # bias, beta_x and beta_h all receive d_beta; each gets its own tensor, as autograd may keep one as a .grad
+            grads[5:] = [d_beta, d_gamma_x, d_beta.clone(), d_gamma_h, d_beta.clone()]
+    return [g if n else None for g, n in zip(grads, needs)]
+
+
+class LNLSTMFunction(torch.autograd.Function):
+    """One layer of the layer-normalised LSTM over a whole input sequence: (x (T, B, I), h0, c0 (B, H), wx, wh, bias[l],
+    gamma_x, beta_x, gamma_h, beta_h, save) -> (y (T, B, H), h_T, c_T).  ``save`` (grad enabled and an input requires
+    grad) keeps the backward's tensors; without it the forward keeps nothing beyond its own buffers."""
+
+    @staticmethod
+    def forward(ctx, x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, save):
+        y, hT, cT, GX, GH, C, stats = lnlstm_fwd_(x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, save)
+        if save:
+            ctx.save_for_backward(x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, y, GX, GH, C, stats)
+        ctx.set_materialize_grads(False)
+        return y, hT, cT
+
+    @staticmethod
+    def backward(ctx, g_y, g_hT, g_cT):
+        return tuple(lnlstm_bwd_(g_y, g_hT, g_cT, *ctx.saved_tensors, ctx.needs_input_grad[:10])) + (None, )
+
+
 class A2CFunction(torch.autograd.Function):
     """a2c_error (ding/rl_utils/a2c.py:10-44): three differentiable 0-dim losses; gradients reach logit and value.  One launch
     forward (losses + gradients for the expected upstream gradients), one verification launch backward (csrc/heads.cu)."""

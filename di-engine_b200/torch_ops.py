@@ -1005,6 +1005,61 @@ scatter_fwd.register_autograd(_scatter_backward, setup_context=_scatter_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# The layer-normalised LSTM (csrc/lstm.cu, GEMMs on cuBLAS): one op per layer per call in each direction
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::lnlstm_fwd', mutates_args=())
+def lnlstm_fwd(x: Tensor, h0: Tensor, c0: Tensor, wx: Tensor, wh: Tensor, bias: Tensor, gamma_x: Tensor, beta_x: Tensor,
+               gamma_h: Tensor, beta_h: Tensor,
+               save: bool) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """-> (y, h_T, c_T, GX, GH, C, stats), as ``ops.lnlstm_fwd_``"""
+    out = ops.lnlstm_fwd_(x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, save)
+    # a custom op returns tensors only, none aliasing another: stats is empty and C a copy of c_T where the eager path
+    # keeps no statistics and shares c_T's memory
+    C = out[5] if out[5].data_ptr() != out[2].data_ptr() else out[2].clone().view(out[5].shape)
+    return out[:5] + (C, out[6] if out[6] is not None else x.new_empty(0))
+
+
+@lnlstm_fwd.register_fake
+def _(x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, save):
+    T, B, _ = x.shape
+    H = wh.shape[0]
+    stats = x.new_empty(T, B, 4) if save else x.new_empty(0)
+    return (x.new_empty(T, B, H), x.new_empty(B, H), x.new_empty(B, H), x.new_empty(T, B, 4 * H),
+            x.new_empty(T if save else 1, B, 4 * H), x.new_empty(T, B, H), stats)
+
+
+@torch.library.custom_op('b200rl::lnlstm_bwd', mutates_args=())
+def lnlstm_bwd(g_y: Optional[Tensor], g_hT: Optional[Tensor], g_cT: Optional[Tensor], x: Tensor, h0: Tensor, c0: Tensor,
+               wx: Tensor, wh: Tensor, bias: Tensor, gamma_x: Tensor, beta_x: Tensor, gamma_h: Tensor, beta_h: Tensor,
+               y: Tensor, GX: Tensor, GH: Tensor, C: Tensor, stats: Tensor, needs: list[bool]) -> list[Tensor]:
+    """-> the ten input gradients of ``lnlstm_fwd``; an input whose ``needs`` is false gets an empty tensor"""
+    grads = ops.lnlstm_bwd_(g_y, g_hT, g_cT, x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, y, GX, GH, C,
+                            stats, needs)
+    return [x.new_empty(0) if g is None else g for g in grads]
+
+
+@lnlstm_bwd.register_fake
+def _(g_y, g_hT, g_cT, x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, y, GX, GH, C, stats, needs):
+    ins = (x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h)
+    return [t.new_empty(t.shape) if n else x.new_empty(0) for t, n in zip(ins, needs)]  # contiguous, as the real op's
+
+
+def _lnlstm_setup(ctx, inputs, output):
+    ctx.save_for_backward(*inputs[:10], *output[:1], *output[3:])
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[3:])
+
+
+def _lnlstm_backward(ctx, g_y, g_hT, g_cT, *_):
+    needs = list(ctx.needs_input_grad[:10])
+    grads = lnlstm_bwd(g_y, g_hT, g_cT, *ctx.saved_tensors, needs)
+    return tuple(g if n else None for g, n in zip(grads, needs)) + (None, )
+
+
+lnlstm_fwd.register_autograd(_lnlstm_backward, setup_context=_lnlstm_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # what rl_utils calls while compiling: the autograd.Function signatures of ops, on the ops above
 # ---------------------------------------------------------------------------------------------------------------------
 def _want_grad(*xs):

@@ -339,6 +339,46 @@ B200RL_API int b200rl_scatter_bwd(const float* g, long long g_sb, long long g_sn
                     long long row_sb, long long row_sm, const long long* col, long long col_sb, long long col_sm,
                     long long B, long long M, long long N, long long H, long long W, float* grad_x, void* stream);
 
+/* ---- layer-normalised LSTM step: ding/torch_utils/network/rnn.py:131-239 (lstm_type='normal', norm_type='LN') ----------
+ * Replaces the body of the step loop, rnn.py:219-231: the two LayerNorms (biased variance, eps 1e-5, as nn.LayerNorm),
+ * their sum plus bias, the gate split i, f, o, u (:223-228) through sigmoid / tanh, c_t = f c_{t-1} + i u and
+ * h_t = o tanh(c_t), computed in double with accurate exp / tanh and rounded to fp32 once on the store (no fast-math).  The
+ * GEMMs are the CALLER's: gx = x_t Wx and gh = h_{t-1} Wh before the
+ * forward step, dh_{t-1} = d_gh[t] Wh^T between backward steps, and dX, dWx, dWh after the loop.
+ * Every operand is a pointer plus element strides: a (B, 4H) or (B, H) row operand (sb, sk), a (4H) parameter (s), a
+ * per-row statistics record of 4 consecutive floats (mean_x, rstd_x, mean_h, rstd_h) at row stride st_sb.
+ * b200rl_lnlstm_step_fwd: gx, gh (B, 4H) before normalisation; gamma_x, beta_x, gamma_h, beta_h, bias (4H); c_prev (B, H).
+ *   Writes h and c (B, H); h_next and c_next (nullable) get the same values (the last step's next state); stats
+ *   (nullable) only when a backward will follow.  One launch.
+ * b200rl_lnlstm_step_bwd: dh_t = dy + dh_rec (each nullable = 0; dh_rec is the recurrent term d_gh[t+1] Wh^T, or the
+ *   next state's gradient at the last step), dc_in (nullable = 0) the cell gradient from step t+1; gx, gh and stats as
+ *   saved by the forward; c_prev and c the cell states before and after the step.  Recomputes the gates and writes
+ *   d_gx and d_gh (B, 4H, through both LayerNorm backwards), d_gate (B, 4H, the gradient of the pre-activation, for
+ *   b200rl_lnlstm_param_grads) and dc_prev (B, H), which may be dc_in itself.  One launch.
+ * b200rl_lnlstm_param_grads: over R = T*B rows of d_gate, gx, gh and stats (row strides): d_gamma_x = sum d_gate x^,
+ *   d_gamma_h = sum d_gate h^ and d_beta = sum d_gate (the gradient of beta_x, beta_h and bias alike), each (4H).  Fixed
+ *   summation order, no atomics: bit-identical from run to run.  One launch. */
+B200RL_API int b200rl_lnlstm_step_fwd(const float* gx, long long gx_sb, long long gx_sk, const float* gh, long long gh_sb,
+                    long long gh_sk, const float* gamma_x, long long gamma_x_s, const float* beta_x, long long beta_x_s,
+                    const float* gamma_h, long long gamma_h_s, const float* beta_h, long long beta_h_s, const float* bias,
+                    long long bias_s, const float* c_prev, long long cp_sb, long long cp_sk, long long B, long long H, float* h,
+                    long long h_sb, long long h_sk, float* c, long long c_sb, long long c_sk, float* h_next, long long hn_sb,
+                    long long hn_sk, float* c_next, long long cn_sb, long long cn_sk, float* stats, long long st_sb,
+                    void* stream);
+B200RL_API int b200rl_lnlstm_step_bwd(const float* dy, long long dy_sb, long long dy_sk, const float* dh_rec,
+                    long long dhr_sb, long long dhr_sk, const float* dc_in, long long dci_sb, long long dci_sk, const float* gx,
+                    long long gx_sb, long long gx_sk, const float* gh, long long gh_sb, long long gh_sk, const float* stats,
+                    long long st_sb, const float* gamma_x, long long gamma_x_s, const float* beta_x, long long beta_x_s,
+                    const float* gamma_h, long long gamma_h_s, const float* beta_h, long long beta_h_s, const float* bias,
+                    long long bias_s, const float* c_prev, long long cp_sb, long long cp_sk, const float* c, long long c_sb,
+                    long long c_sk, long long B, long long H, float* d_gx, long long dgx_sb, long long dgx_sk, float* d_gh,
+                    long long dgh_sb, long long dgh_sk, float* d_gate, long long dg_sb, long long dg_sk, float* dc_prev,
+                    long long dcp_sb, long long dcp_sk, void* stream);
+B200RL_API int b200rl_lnlstm_param_grads(const float* d_gate, long long dg_sr, long long dg_sk, const float* gx,
+                    long long gx_sr, long long gx_sk, const float* gh, long long gh_sr, long long gh_sk, const float* stats,
+                    long long st_sr, long long R, long long H, float* d_gamma_x, long long dgx_s, float* d_gamma_h,
+                    long long dgh_s, float* d_beta, long long db_s, void* stream);
+
 /* ---- upgo_loss head: ding/rl_utils/upgo.py:77-111 (tb_cross_entropy :7-43) --------------------------------------
  * logit: (TB*K, N) with K = 1 for (T,B,N) logits or N2 for (T,B,N2,N); action, mask(nullable): (TB*K);
  * rho, ret (from b200rl_lambda_returns upgo mode), value (= bootstrap_values[:-1]): (TB).
