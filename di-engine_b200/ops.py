@@ -620,24 +620,10 @@ class DQfDTDFunction(torch.autograd.Function):
                 vg_stride, is_expert, S, N, nstep, gamma, cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1,
                 lam_s, margin, seq_len, priority_mix, want_targets, want_priority):
         dev = q.device
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        td = torch.empty(S, dtype=torch.float32, device=dev)
-        stats = torch.empty(3, dtype=torch.float32, device=dev)
-        saved = torch.empty(S, 4, dtype=torch.float32, device=dev)
-        tn = torch.empty(S, dtype=torch.float32, device=dev) if want_targets else None
-        t1 = torch.empty(S, dtype=torch.float32, device=dev) if want_targets else None
-        prio = torch.empty(S // seq_len, dtype=torch.float32, device=dev) if want_priority else None
-        grad_unit = torch.empty(S, N, dtype=torch.float32, device=dev) if ctx.needs_input_grad[0] else None
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_dqfd_fwd(
-                ptr(q), ptr(next_n_q), ptr(next_q1), ptr(action), ptr(next_n_action), ptr(next_action1), ptr(reward),
-                ptr(done), ptr(done1), ptr(weight), ptr(value_gamma), vg_stride, ptr(is_expert), S, N, nstep, gamma,
-                cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1, lam_s, margin, seq_len, priority_mix,
-                ptr(loss), ptr(td), ptr(stats), ptr(saved), ptr(tn), ptr(t1), ptr(grad_unit), ptr(prio), ptr(ws),
-                ws.numel() * 4, stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_dqfd_fwd')
+        loss, td, stats, saved, tn, t1, prio, grad_unit = dqfd_fwd_(
+            q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done, done1, weight, value_gamma,
+            vg_stride, is_expert, S, N, nstep, gamma, cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1,
+            lam_s, margin, seq_len, priority_mix, want_targets, want_priority, ctx.needs_input_grad[0])
         ctx.save_for_backward(saved, action, weight)
         ctx.cfg = (S, N, lam_n, lam_1, lam_s, seq_len)
         ctx.q_shape = q.shape
@@ -659,11 +645,45 @@ class DQfDTDFunction(torch.autograd.Function):
         keep, (pg, ptd, psn, ps1, psje) = _grads(g_loss, g_td, g_sn, g_s1, g_sje)
         grad_q, skip = _unit_grad(ctx, (g_td, g_sn, g_s1, g_sje),
                                   lambda: torch.empty(S, N, dtype=torch.float32, device=saved.device))
-        with on_device(saved.device):
-            rc = lib().b200rl_dqfd_bwd(ptr(saved), ptr(weight), ptr(action), pg, ptd, psn, ps1, psje, S, N, lam_n, lam_1,
-                                       lam_s, seq_len, skip, ptr(grad_q), stream_ptr())
-        _lib.check(rc, 'b200rl_dqfd_bwd')
+        dqfd_bwd_(saved, weight, action, pg, ptd, (psn, ps1, psje), S, N, lam_n, lam_1, lam_s, seq_len, skip, grad_q)
         return (grad_q.view(ctx.q_shape), ) + (None, ) * (n_in - 1)
+
+
+def dqfd_fwd_(q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done, done1, weight, value_gamma,
+              vg_stride, is_expert, S, N, nstep, gamma, cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1, lam_s,
+              margin, seq_len, priority_mix, want_targets, want_priority, want_grad):
+    """The forward launch of the DQfD family (DQfDTDFunction and the ``b200rl::dqfd_fwd`` custom op).
+    -> (loss, td, stats (3,), saved (S, 4), tn or None, t1 or None, prio or None, grad_unit or None)."""
+    dev = q.device
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    td = torch.empty(S, dtype=torch.float32, device=dev)
+    stats = torch.empty(3, dtype=torch.float32, device=dev)
+    saved = torch.empty(S, 4, dtype=torch.float32, device=dev)
+    tn = torch.empty(S, dtype=torch.float32, device=dev) if want_targets else None
+    t1 = torch.empty(S, dtype=torch.float32, device=dev) if want_targets else None
+    prio = torch.empty(S // seq_len, dtype=torch.float32, device=dev) if want_priority else None
+    grad_unit = torch.empty(S, N, dtype=torch.float32, device=dev) if want_grad else None
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_dqfd_fwd(
+            ptr(q), ptr(next_n_q), ptr(next_q1), ptr(action), ptr(next_n_action), ptr(next_action1), ptr(reward),
+            ptr(done), ptr(done1), ptr(weight), ptr(value_gamma), vg_stride, ptr(is_expert), S, N, nstep, gamma,
+            cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1, lam_s, margin, seq_len, priority_mix,
+            ptr(loss), ptr(td), ptr(stats), ptr(saved), ptr(tn), ptr(t1), ptr(grad_unit), ptr(prio), ptr(ws),
+            ws.numel() * 4, stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_dqfd_fwd')
+    return loss, td, stats, saved, tn, t1, prio, grad_unit
+
+
+def dqfd_bwd_(saved, weight, action, pg, ptd, pstats, S, N, lam_n, lam_1, lam_s, seq_len, skip, grad_q):
+    """The backward launch of the DQfD family into ``grad_q``: ``pg`` / ``ptd`` / ``pstats`` (three) the device pointers
+    of the upstream gradients of loss, td and the statistics (None = 0); ``skip`` as qntd_bwd_."""
+    with on_device(saved.device):
+        rc = lib().b200rl_dqfd_bwd(ptr(saved), ptr(weight), ptr(action), pg, ptd, *pstats, S, N, lam_n, lam_1, lam_s,
+                                   seq_len, skip, ptr(grad_q), stream_ptr())
+    _lib.check(rc, 'b200rl_dqfd_bwd')
+    return grad_q
 
 
 class SoftTDFunction(torch.autograd.Function):
@@ -681,23 +701,9 @@ class SoftTDFunction(torch.autograd.Function):
                 tau, alpha, cum_reward, criterion, crit_param):
         dev = q.device
         R = S * G
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        td = torch.empty(R, dtype=torch.float32, device=dev)
-        dcrit = torch.empty(R, dtype=torch.float32, device=dev)
-        target = torch.empty(R, dtype=torch.float32, device=dev)
-        gap = torch.empty((), dtype=torch.float32, device=dev) if mode == 0 else None
-        clip = torch.empty(R, dtype=torch.float32, device=dev) if mode == 0 else None
-        rec = torch.empty(R, dtype=torch.float32, device=dev) if mode == 1 else None
-        grad_unit = torch.empty(R, N, dtype=torch.float32, device=dev) if ctx.needs_input_grad[0] else None
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_soft_td_fwd(
-                mode, ptr(q), ptr(target_q), ptr(next_q), ptr(action), ptr(reward), ptr(done), ptr(weight),
-                ptr(value_gamma), vg_stride, S, G, N, nstep, gamma, tau, alpha, cum_reward, criterion, crit_param,
-                ptr(loss), ptr(td), ptr(dcrit), ptr(target), ptr(grad_unit), ptr(gap), ptr(clip), ptr(rec), ptr(ws),
-                ws.numel() * 4, stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_soft_td_fwd')
+        loss, td, dcrit, target, gap, clip, rec, grad_unit = soft_td_fwd_(
+            q, target_q, next_q, action, reward, done, weight, value_gamma, vg_stride, mode, S, G, N, nstep, gamma, tau,
+            alpha, cum_reward, criterion, crit_param, ctx.needs_input_grad[0])
         ctx.save_for_backward(dcrit, action, weight)
         ctx.cfg = (R, 1, N, 0, 0)  # QNStepTDFunction's (S, G, N, group_mean, seq_len): R rows of one
         ctx.q_shape = q.shape
@@ -711,6 +717,32 @@ class SoftTDFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, g_td, _g_target, _g_gap, _g_clip, _g_rec):
         return QNStepTDFunction.backward(ctx, g_loss, g_td, None, None)[:1] + (None, ) * 19
+
+
+def soft_td_fwd_(q, target_q, next_q, action, reward, done, weight, value_gamma, vg_stride, mode, S, G, N, nstep, gamma,
+                 tau, alpha, cum_reward, criterion, crit_param, want_grad):
+    """The forward launch of the soft TD losses (SoftTDFunction and the ``b200rl::soft_td_fwd`` custom op).
+    -> (loss, td, dcrit, target, gap, clip, rec, grad_unit); the mode's missing statistics and grad_unit are None."""
+    dev = q.device
+    R = S * G
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    td = torch.empty(R, dtype=torch.float32, device=dev)
+    dcrit = torch.empty(R, dtype=torch.float32, device=dev)
+    target = torch.empty(R, dtype=torch.float32, device=dev)
+    gap = torch.empty((), dtype=torch.float32, device=dev) if mode == 0 else None
+    clip = torch.empty(R, dtype=torch.float32, device=dev) if mode == 0 else None
+    rec = torch.empty(R, dtype=torch.float32, device=dev) if mode == 1 else None
+    grad_unit = torch.empty(R, N, dtype=torch.float32, device=dev) if want_grad else None
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_soft_td_fwd(
+            mode, ptr(q), ptr(target_q), ptr(next_q), ptr(action), ptr(reward), ptr(done), ptr(weight),
+            ptr(value_gamma), vg_stride, S, G, N, nstep, gamma, tau, alpha, cum_reward, criterion, crit_param,
+            ptr(loss), ptr(td), ptr(dcrit), ptr(target), ptr(grad_unit), ptr(gap), ptr(clip), ptr(rec), ptr(ws),
+            ws.numel() * 4, stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_soft_td_fwd')
+    return loss, td, dcrit, target, gap, clip, rec, grad_unit
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -855,18 +887,8 @@ class FQFFractionFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, q_tau_i, q_value, quantiles, action, B, N, qt_strides, qv_strides, qn_strides):
-        dev = quantiles.device
-        loss = torch.empty((), dtype=torch.float32, device=dev)
-        g = torch.empty(B, N - 1, dtype=torch.float32, device=dev)
-        grad_unit = torch.empty(B, N + 1, dtype=torch.float32, device=dev) if ctx.needs_input_grad[2] else None
-        with on_device(dev):
-            ws = workspace(dev)
-            rc = lib().b200rl_fqf_fraction_fwd(
-                ptr(q_tau_i), ptr(q_value), ptr(quantiles), ptr(action), B, N, q_tau_i.shape[2], q_value.shape[2],
-                *qt_strides, *qv_strides, *qn_strides, ptr(loss), ptr(g), ptr(grad_unit), ptr(ws), ws.numel() * 4,
-                stream_ptr()
-            )
-        _lib.check(rc, 'b200rl_fqf_fraction_fwd')
+        loss, g, grad_unit = fqf_fraction_fwd_(q_tau_i, q_value, quantiles, action, B, N, qt_strides, qv_strides,
+                                               qn_strides, ctx.needs_input_grad[2])
         ctx.save_for_backward(g)
         ctx.cfg = (B, N)
         ctx.spec = grad_unit
@@ -881,10 +903,33 @@ class FQFFractionFunction(torch.autograd.Function):
         B, N = ctx.cfg
         keep, (pg, ) = _grads(g_loss)
         grad, skip = _unit_grad(ctx, (), lambda: torch.empty(B, N + 1, dtype=torch.float32, device=g.device))
-        with on_device(g.device):
-            rc = lib().b200rl_fqf_fraction_bwd(ptr(g), pg, B, N, skip, ptr(grad), stream_ptr())
-        _lib.check(rc, 'b200rl_fqf_fraction_bwd')
-        return (None, None, grad) + (None, ) * 6
+        return (None, None, fqf_fraction_bwd_(g, pg, B, N, skip, grad)) + (None, ) * 6
+
+
+def fqf_fraction_fwd_(q_tau_i, q_value, quantiles, action, B, N, qt_strides, qv_strides, qn_strides, want_grad):
+    """The forward launch of FQF's fraction loss (FQFFractionFunction and the ``b200rl::fqf_fraction_fwd`` custom op).
+    -> (loss, g (B, N-1), grad_unit (B, N+1) or None)."""
+    dev = quantiles.device
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    g = torch.empty(B, N - 1, dtype=torch.float32, device=dev)
+    grad_unit = torch.empty(B, N + 1, dtype=torch.float32, device=dev) if want_grad else None
+    with on_device(dev):
+        ws = workspace(dev)
+        rc = lib().b200rl_fqf_fraction_fwd(
+            ptr(q_tau_i), ptr(q_value), ptr(quantiles), ptr(action), B, N, q_tau_i.shape[2], q_value.shape[2],
+            *qt_strides, *qv_strides, *qn_strides, ptr(loss), ptr(g), ptr(grad_unit), ptr(ws), ws.numel() * 4,
+            stream_ptr()
+        )
+    _lib.check(rc, 'b200rl_fqf_fraction_fwd')
+    return loss, g, grad_unit
+
+
+def fqf_fraction_bwd_(g, pg, B, N, skip, grad):
+    """The backward launch of FQF's fraction loss into ``grad`` (B, N+1) (``pg`` / ``skip`` as qntd_bwd_)."""
+    with on_device(g.device):
+        rc = lib().b200rl_fqf_fraction_bwd(ptr(g), pg, B, N, skip, ptr(grad), stream_ptr())
+    _lib.check(rc, 'b200rl_fqf_fraction_bwd')
+    return grad
 
 
 # ----------------------------------------------------------------------------------------------------------------

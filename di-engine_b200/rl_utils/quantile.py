@@ -162,5 +162,9 @@ def fqf_calculate_fraction_loss(q_tau_i, q_value, quantiles, actions):
     qv = _f32(ops.to_device(q_value.detach(), dev), 'q_value')
     qn = _f32(ops.to_device(quantiles, dev), 'quantiles')
     act = ops.i64c(ops.to_device(actions, dev), min(qt.shape[2], qv.shape[2]), 'actions')
-    loss = ops.FQFFractionFunction.apply(qt, qv, qn, act, batch_size, num_quantiles, qt.stride(), qv.stride(), qn.stride())
+    if torch.compiler.is_compiling():
+        loss = torch_ops.fqf_fraction(qt, qv, qn, act, batch_size, num_quantiles)
+    else:
+        loss = ops.FQFFractionFunction.apply(qt, qv, qn, act, batch_size, num_quantiles, qt.stride(), qv.stride(),
+                                             qn.stride())
     return loss.cpu() if host_out else loss

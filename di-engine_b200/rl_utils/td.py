@@ -464,11 +464,16 @@ def q_nstep_td_error_sequence(
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.numel() != S:
             w = w.expand(T, B).contiguous()
-    vg, vg_stride = _value_gamma_arg(value_gamma, S, dev)
-    loss, per, _, prio = ops.QNStepTDFunction.apply(
-        qd, nq, act, nact, r, d, w, vg, vg_stride, gamma_ps, S, 1, N, int(nstep), float(gamma_f), 0,
-        1 if rescale else 0, 1e-2, code[0], code[1], 0, T, float(priority_mix), True
-    )
+    if torch.compiler.is_compiling():
+        vg, vg_stride = _value_gamma_op_arg(value_gamma, S, dev)
+        loss, per, prio = torch_ops.qntd_seq(qd, nq, act, nact, r, d, w, vg, vg_stride, gamma_ps, S, N, int(nstep),
+                                             float(gamma_f), 1 if rescale else 0, code[0], code[1], T, float(priority_mix))
+    else:
+        vg, vg_stride = _value_gamma_arg(value_gamma, S, dev)
+        loss, per, _, prio = ops.QNStepTDFunction.apply(
+            qd, nq, act, nact, r, d, w, vg, vg_stride, gamma_ps, S, 1, N, int(nstep), float(gamma_f), 0,
+            1 if rescale else 0, 1e-2, code[0], code[1], 0, T, float(priority_mix), True
+        )
     per = per.reshape(T, B)
     if host_out:
         loss, prio, per = loss.cpu(), prio.cpu(), per.cpu()
@@ -500,11 +505,13 @@ def _dqfd_operands(data, S, dev, rows):
     d = ops.f32c(ops.to_device(done.detach(), dev), 'done')
     d1 = ops.f32c(ops.to_device(done_one_step.detach(), dev), 'done_one_step')
     if not isinstance(is_expert, torch.Tensor):
-        ie = ops.const_scalar(is_expert, dev).expand(S).contiguous()
+        # traced: a float, which the custom op reads from the cached device constant when it runs
+        ie = float(is_expert) if torch.compiler.is_compiling() else ops.const_scalar(is_expert, dev).expand(S).contiguous()
     else:
         ie = ops.f32c(ops.to_device(is_expert.detach(), dev), 'is_expert')
-    if ie.numel() == 1:
+    if isinstance(ie, torch.Tensor) and ie.numel() == 1:
         ie = ie.reshape(1).expand(S).contiguous()
+    ie_shape = tuple(ie.shape) if isinstance(ie, torch.Tensor) else (S, )
     w = None
     if weight is not None:
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
@@ -513,12 +520,12 @@ def _dqfd_operands(data, S, dev, rows):
     shape = tuple(qd.shape[:-1])
     if (shape != tuple(rows) or nq.shape != qd.shape or nq1.shape != qd.shape or tuple(act.shape) != shape or
             tuple(nact.shape) != shape or tuple(nact1.shape) != shape or d.numel() != S or d1.numel() != S or
-            ie.numel() != S or (w is not None and w.numel() != S)):
+            (isinstance(ie, torch.Tensor) and ie.numel() != S) or (w is not None and w.numel() != S)):
         raise ValueError("dqfd: q %s / next_n_q %s / new_n_q_one_step %s / actions %s %s %s / done %s %s / is_expert %s / "
                          "weight %s do not match %s" %
                          (tuple(q.shape), tuple(next_n_q.shape), tuple(next_q1.shape), tuple(action.shape),
                           tuple(next_n_action.shape), tuple(next_action1.shape), tuple(done.shape),
-                          tuple(done_one_step.shape), tuple(ie.shape), None if weight is None else tuple(weight.shape),
+                          tuple(done_one_step.shape), ie_shape, None if weight is None else tuple(weight.shape),
                           tuple(rows)))
     return qd, nq, nq1, act, nact, nact1, r, d, d1, w, ie
 
@@ -547,15 +554,17 @@ def _dqfd(data, gamma, lambda_n_step_td, lambda_supervised_loss, lambda_one_step
     host_out = not q.is_cuda
     dev = ops.compute_device(q, next_n_q, next_q1)
     qd, nq, nq1, act, nact, nact1, r, d, d1, w, ie = _dqfd_operands(data, B, dev, (B, ))
-    vg, vg_stride = _value_gamma_arg(value_gamma, B, dev)
+    compiling = torch.compiler.is_compiling()
+    vg, vg_stride = (_value_gamma_op_arg if compiling else _value_gamma_arg)(value_gamma, B, dev)
     custom_trans = rescale and (trans_fn is not value_transform or inv_trans_fn is not value_inv_transform)
     code = _criterion_code(criterion)
     lam_n, lam_1, lam_s = float(lambda_n_step_td), float(lambda_one_step_td), float(lambda_supervised_loss)
 
     def kernel(nq_, nq1_, resc, crit, param, want_targets):
-        return ops.DQfDTDFunction.apply(qd, nq_, nq1_, act, nact, nact1, r, d, d1, w, vg, vg_stride, ie, B, N, int(nstep),
-                                        gamma, 1 if cum_reward else 0, resc, 1e-2, crit, param, lam_n, lam_1, lam_s,
-                                        float(margin_function), 0, 0.0, want_targets, False)
+        return (torch_ops.dqfd if compiling else ops.DQfDTDFunction.apply)(
+            qd, nq_, nq1_, act, nact, nact1, r, d, d1, w, vg, vg_stride, ie, B, N, int(nstep), gamma,
+            1 if cum_reward else 0, resc, 1e-2, crit, param, lam_n, lam_1, lam_s, float(margin_function), 0, 0.0,
+            want_targets, False)
 
     if code is not None and not custom_trans:
         loss, per, s_n, s_1, s_je, _, _, _ = kernel(nq, nq1, 1 if rescale else 0, code[0], code[1], False)
@@ -689,8 +698,9 @@ def dqfd_nstep_td_error_sequence(
     qd, nq, nq1, act, nact, nact1, r, d, d1, w, ie = _dqfd_operands(
         dqfd_nstep_td_data(q, next_n_q, action, next_n_action, reward, done, done_one_step, weight, next_q1, next_action1,
                            is_expert), S, dev, (T, B))
-    vg, vg_stride = _value_gamma_arg(value_gamma, S, dev)
-    loss, per, s_n, s_1, s_je, _, _, prio = ops.DQfDTDFunction.apply(
+    compiling = torch.compiler.is_compiling()
+    vg, vg_stride = (_value_gamma_op_arg if compiling else _value_gamma_arg)(value_gamma, S, dev)
+    loss, per, s_n, s_1, s_je, _, _, prio = (torch_ops.dqfd if compiling else ops.DQfDTDFunction.apply)(
         qd, nq, nq1, act, nact, nact1, r, d, d1, w, vg, vg_stride, ie, S, N, int(nstep), gamma, 0, 1 if rescale else 0,
         1e-2, code[0], code[1], float(lambda_n_step_td), float(lambda_one_step_td), float(lambda_supervised_loss),
         float(margin_function), T, float(priority_mix), False, True
@@ -729,13 +739,14 @@ def _soft_td(mode, q, target_q, next_q, act, reward, done, weight, S, G, gamma, 
     staged there and detached.  -> (loss, td (S*G,), action_gap, clipfrac (S*G,), record_target_v (S*G,)), the last three
     empty where the mode has none."""
     R, N = q.shape
-    vg, vg_stride = _value_gamma_arg(value_gamma, S, q.device)
+    compiling = torch.compiler.is_compiling()
+    vg, vg_stride = (_value_gamma_op_arg if compiling else _value_gamma_arg)(value_gamma, S, q.device)
     code = _criterion_code(criterion)
 
     def kernel(q_, crit, param):
-        return ops.SoftTDFunction.apply(q_, target_q, next_q, act, reward, done, weight, vg, vg_stride, mode, S, G, N,
-                                        int(nstep), float(gamma), float(tau), float(alpha), 1 if cum_reward else 0, crit,
-                                        param)
+        return (torch_ops.soft_td if compiling else ops.SoftTDFunction.apply)(
+            q_, target_q, next_q, act, reward, done, weight, vg, vg_stride, mode, S, G, N, int(nstep), float(gamma),
+            float(tau), float(alpha), 1 if cum_reward else 0, crit, param)
 
     if code is not None:
         loss, per, _, gap, clip, rec = kernel(q, code[0], code[1])

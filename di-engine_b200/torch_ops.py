@@ -4,8 +4,10 @@ q_nstep_td_error_with_rescale, dist_nstep_td_error, td_lambda_error, upgo_loss, 
 language-model losses on (B, S, V) logits (grpo_policy_error, rloo_policy_error, the log-prob methods, ppo_policy_error /
 ppo_error / a2c_error on token rows, ppo_value_error), the advantage recomputes (gae_returns, ppof_gae_returns,
 normalize_advantage, ppo_error_adv_norm), symlog / inv_symlog, the quantile TD losses (QR-DQN, IQN, FQF) and the
-continuous-action PPO losses, COMA's loss and ScatterConnection without a graph break, and ``mode="reduce-overhead"`` can replay a compiled learner step as
-a CUDA graph.
+continuous-action PPO losses, COMA's loss, ScatterConnection, the value-based losses of DQfD / R2D3 (dqfd_nstep_td_error,
+its _with_rescale and _sequence forms), M-DQN, SQL and discrete SAC (m_q_1step_td_error, q_nstep_sql_td_error,
+q_v_1step_td_error), the R2D2 / NGU loop q_nstep_td_error_sequence and FQF's fraction loss without a graph break, and
+``mode="reduce-overhead"`` can replay a compiled learner step as a CUDA graph.
 
 Each op's implementation is the launch function ``ops`` runs in eager mode; ``rl_utils`` calls the wrappers at the bottom
 of this module only while ``torch.compiler.is_compiling()``.  The schemas hold tensors and scalars only: the workspace, the
@@ -192,6 +194,191 @@ def _qntd_backward(ctx, g_loss, g_td, *_):
 
 
 qntd_fwd.register_autograd(_qntd_backward, setup_context=_qntd_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# q_nstep_td_error_sequence (the R2D2 / NGU loop): the q-n-step launches with seq_len = T and the priority output
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::qntd_seq_fwd', mutates_args=())
+def qntd_seq_fwd(q: Tensor, next_n_q: Tensor, action: Tensor, next_n_action: Tensor, reward: Tensor, done: Tensor,
+                 weight: Optional[Tensor], value_gamma: Optional[Tensor], value_gamma_scalar: Optional[float],
+                 vg_stride: int, gamma_ps: Optional[Tensor], S: int, N: int, nstep: int, gamma: float, rescale: int,
+                 criterion: int, crit_param: float, seq_len: int, priority_mix: float,
+                 want_grad: bool) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """-> (loss, td, dcrit, prio (S / seq_len), grad_unit); one row per sample (G = 1), no cum_reward, eps 1e-2, as
+    q_nstep_td_error_sequence calls the launch"""
+    if value_gamma_scalar is not None:
+        value_gamma = ops.const_scalar(value_gamma_scalar, q.device)
+    loss, td, dcrit, _, prio, grad_unit = ops.qntd_fwd_(
+        q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, vg_stride, gamma_ps, S, 1, N, nstep, gamma,
+        0, rescale, 1e-2, criterion, crit_param, 0, seq_len, priority_mix, True, want_grad)
+    return loss, td, dcrit, prio, grad_unit if grad_unit is not None else _empty(loss)
+
+
+@qntd_seq_fwd.register_fake
+def _(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, value_gamma_scalar, vg_stride, gamma_ps, S, N,
+      nstep, gamma, rescale, criterion, crit_param, seq_len, priority_mix, want_grad):
+    loss = q.new_empty(())
+    return (loss, q.new_empty(S), q.new_empty(S), q.new_empty(S // seq_len),
+            q.new_empty(S, N) if want_grad else _empty(loss))
+
+
+@torch.library.custom_op('b200rl::qntd_seq_bwd', mutates_args=())
+def qntd_seq_bwd(dcrit: Tensor, weight: Optional[Tensor], action: Tensor, g_loss: Optional[Tensor],
+                 g_td: Optional[Tensor], grad_unit: Tensor, S: int, N: int, seq_len: int) -> Tensor:
+    """-> d / d q (S, N), as qntd_bwd with the loss averaged over the seq_len steps"""
+    kl, pg = _one(g_loss)
+    kt, ptd = _one(g_td)
+    skip = 1 if (g_td is None and grad_unit.numel()) else 0
+    grad = grad_unit.clone() if skip else dcrit.new_empty(S, N)
+    return ops.qntd_bwd_(dcrit, weight, action, pg, ptd, S, 1, N, 0, seq_len, skip, grad)
+
+
+@qntd_seq_bwd.register_fake
+def _(dcrit, weight, action, g_loss, g_td, grad_unit, S, N, seq_len):
+    return dcrit.new_empty(S, N)
+
+
+def _qntd_seq_setup(ctx, inputs, output):
+    ctx.save_for_backward(output[2], inputs[6], inputs[2], output[4])
+    ctx.cfg = (inputs[11], inputs[12], inputs[18])
+    ctx.q_shape = inputs[0].shape
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[2:])
+
+
+def _qntd_seq_backward(ctx, g_loss, g_td, *_):
+    if g_loss is None and g_td is None:
+        return (None, ) * 21
+    dcrit, weight, action, grad_unit = ctx.saved_tensors
+    grad = qntd_seq_bwd(dcrit, weight, action, g_loss, g_td, grad_unit, *ctx.cfg)
+    return (grad.view(ctx.q_shape), ) + (None, ) * 20
+
+
+qntd_seq_fwd.register_autograd(_qntd_seq_backward, setup_context=_qntd_seq_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# dqfd_nstep_td_error[_with_rescale] and the R2D3 loop (csrc/td.cu dqfd_fwd / dqfd_bwd): the three statistics leave the op
+# as one (3,) tensor, unbound by the caller (a custom op's outputs may not alias each other)
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::dqfd_fwd', mutates_args=())
+def dqfd_fwd(q: Tensor, next_n_q: Tensor, next_q1: Tensor, action: Tensor, next_n_action: Tensor, next_action1: Tensor,
+             reward: Tensor, done: Tensor, done1: Tensor, weight: Optional[Tensor], value_gamma: Optional[Tensor],
+             value_gamma_scalar: Optional[float], vg_stride: int, is_expert: Optional[Tensor],
+             is_expert_scalar: Optional[float], S: int, N: int, nstep: int, gamma: float, cum_reward: int, rescale: int,
+             eps: float, criterion: int, crit_param: float, lam_n: float, lam_1: float, lam_s: float, margin: float,
+             seq_len: int, priority_mix: float, want_targets: bool, want_priority: bool,
+             want_grad: bool) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """-> (loss, td, stats (3,), saved (S, 4), tn, t1, prio, grad_unit); tn / t1 / prio / grad_unit are empty where not
+    wanted.  A python-scalar value_gamma or is_expert comes as a float and is read from a cached device constant (is_expert
+    expanded to S rows, as in eager mode)."""
+    dev = q.device
+    if value_gamma_scalar is not None:
+        value_gamma = ops.const_scalar(value_gamma_scalar, dev)
+    if is_expert_scalar is not None:
+        is_expert = ops.const_scalar(is_expert_scalar, dev).expand(S).contiguous()
+    out = ops.dqfd_fwd_(q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done, done1, weight,
+                        value_gamma, vg_stride, is_expert, S, N, nstep, gamma, cum_reward, rescale, eps, criterion,
+                        crit_param, lam_n, lam_1, lam_s, margin, seq_len, priority_mix, want_targets, want_priority,
+                        want_grad)
+    return tuple(x if x is not None else _empty(out[0]) for x in out)
+
+
+@dqfd_fwd.register_fake
+def _(q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done, done1, weight, value_gamma,
+      value_gamma_scalar, vg_stride, is_expert, is_expert_scalar, S, N, nstep, gamma, cum_reward, rescale, eps, criterion,
+      crit_param, lam_n, lam_1, lam_s, margin, seq_len, priority_mix, want_targets, want_priority, want_grad):
+    loss = q.new_empty(())
+    return (loss, q.new_empty(S), q.new_empty(3), q.new_empty(S, 4), q.new_empty(S if want_targets else 0),
+            q.new_empty(S if want_targets else 0), q.new_empty(S // seq_len if want_priority else 0),
+            q.new_empty(S, N) if want_grad else _empty(loss))
+
+
+@torch.library.custom_op('b200rl::dqfd_bwd', mutates_args=())
+def dqfd_bwd(saved: Tensor, weight: Optional[Tensor], action: Tensor, g_loss: Optional[Tensor], g_td: Optional[Tensor],
+             g_stats: Optional[Tensor], grad_unit: Tensor, S: int, N: int, lam_n: float, lam_1: float, lam_s: float,
+             seq_len: int) -> Tensor:
+    """-> d / d q (S, N); verifies a copy of the forward-written unit gradient when only the loss has a gradient"""
+    kl, pg = _one(g_loss)
+    kt, ptd = _one(g_td)
+    ks, pstats = _upstream(g_stats, 3)
+    skip = 1 if (g_td is None and g_stats is None and grad_unit.numel()) else 0
+    grad = grad_unit.clone() if skip else saved.new_empty(S, N)
+    return ops.dqfd_bwd_(saved, weight, action, pg, ptd, pstats, S, N, lam_n, lam_1, lam_s, seq_len, skip, grad)
+
+
+@dqfd_bwd.register_fake
+def _(saved, weight, action, g_loss, g_td, g_stats, grad_unit, S, N, lam_n, lam_1, lam_s, seq_len):
+    return saved.new_empty(S, N)
+
+
+def _dqfd_setup(ctx, inputs, output):
+    ctx.save_for_backward(output[3], inputs[9], inputs[3], output[7])
+    ctx.cfg = (inputs[15], inputs[16], inputs[24], inputs[25], inputs[26], inputs[28])
+    ctx.q_shape = inputs[0].shape
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[3:])
+
+
+def _dqfd_backward(ctx, g_loss, g_td, g_stats, *_):
+    if g_loss is None and g_td is None and g_stats is None:
+        return (None, ) * 33
+    saved, weight, action, grad_unit = ctx.saved_tensors
+    grad = dqfd_bwd(saved, weight, action, g_loss, g_td, g_stats, grad_unit, *ctx.cfg)
+    return (grad.view(ctx.q_shape), ) + (None, ) * 32
+
+
+dqfd_fwd.register_autograd(_dqfd_backward, setup_context=_dqfd_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# m_q_1step_td_error / q_nstep_sql_td_error / q_v_1step_td_error (csrc/td.cu soft_td_fwd): every target is detached, so
+# the backward is qntd_bwd over the R rows (G = 1), as SoftTDFunction's; the statistics carry no gradient
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::soft_td_fwd', mutates_args=())
+def soft_td_fwd(q: Tensor, target_q: Optional[Tensor], next_q: Tensor, action: Tensor, reward: Tensor, done: Tensor,
+                weight: Optional[Tensor], value_gamma: Optional[Tensor], value_gamma_scalar: Optional[float],
+                vg_stride: int, mode: int, S: int, G: int, N: int, nstep: int, gamma: float, tau: float, alpha: float,
+                cum_reward: int, criterion: int,
+                crit_param: float, want_grad: bool) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """-> (loss, td, dcrit, target, action_gap, clipfrac, record_target_v, grad_unit); the statistics the mode has none
+    of (M-DQN: action_gap and clipfrac; SQL: record_target_v) and grad_unit without ``want_grad`` are empty"""
+    if value_gamma_scalar is not None:
+        value_gamma = ops.const_scalar(value_gamma_scalar, q.device)
+    out = ops.soft_td_fwd_(q, target_q, next_q, action, reward, done, weight, value_gamma, vg_stride, mode, S, G, N, nstep,
+                           gamma, tau, alpha, cum_reward, criterion, crit_param, want_grad)
+    return tuple(x if x is not None else _empty(out[0]) for x in out)
+
+
+@soft_td_fwd.register_fake
+def _(q, target_q, next_q, action, reward, done, weight, value_gamma, value_gamma_scalar, vg_stride, mode, S, G, N, nstep,
+      gamma, tau, alpha, cum_reward, criterion, crit_param, want_grad):
+    R = S * G
+    loss = q.new_empty(())
+    return (loss, q.new_empty(R), q.new_empty(R), q.new_empty(R), q.new_empty(() if mode == 0 else 0),
+            q.new_empty(R if mode == 0 else 0), q.new_empty(R if mode == 1 else 0),
+            q.new_empty(R, N) if want_grad else _empty(loss))
+
+
+def _soft_td_setup(ctx, inputs, output):
+    ctx.save_for_backward(output[2], inputs[6], inputs[3], output[7])
+    S, G, N = inputs[11:14]
+    ctx.cfg = (S * G, 1, N, 0)  # qntd_bwd's (S, G, N, group_mean): R rows of one
+    ctx.q_shape = inputs[0].shape
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[2:])
+
+
+def _soft_td_backward(ctx, g_loss, g_td, *_):
+    if g_loss is None and g_td is None:
+        return (None, ) * 22
+    dcrit, weight, action, grad_unit = ctx.saved_tensors
+    grad = qntd_bwd(dcrit, weight, action, g_loss, g_td, grad_unit, *ctx.cfg)
+    return (grad.view(ctx.q_shape), ) + (None, ) * 21
+
+
+soft_td_fwd.register_autograd(_soft_td_backward, setup_context=_soft_td_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -846,6 +1033,57 @@ quantile_fwd.register_autograd(_quantile_backward, setup_context=_quantile_setup
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# fqf_calculate_fraction_loss: the op reads the element strides of q_tau_i, q_value and quantiles from its tensors; the
+# gradient goes to quantiles only
+# ---------------------------------------------------------------------------------------------------------------------
+@torch.library.custom_op('b200rl::fqf_fraction_fwd', mutates_args=())
+def fqf_fraction_fwd(q_tau_i: Tensor, q_value: Tensor, quantiles: Tensor, action: Tensor, B: int, N: int,
+                     want_grad: bool) -> tuple[Tensor, Tensor, Tensor]:
+    """-> (loss, g (B, N-1), grad_unit (B, N+1)); grad_unit is empty without ``want_grad``.  q_tau_i (B, N-1, A'),
+    q_value (B, N, A) and quantiles (B, N+1) may be any strided views, as in eager mode."""
+    loss, g, grad_unit = ops.fqf_fraction_fwd_(q_tau_i, q_value, quantiles, action, B, N, q_tau_i.stride(),
+                                               q_value.stride(), quantiles.stride(), want_grad)
+    return loss, g, grad_unit if grad_unit is not None else _empty(loss)
+
+
+@fqf_fraction_fwd.register_fake
+def _(q_tau_i, q_value, quantiles, action, B, N, want_grad):
+    loss = quantiles.new_empty(())
+    return loss, quantiles.new_empty(B, N - 1), quantiles.new_empty(B, N + 1) if want_grad else _empty(loss)
+
+
+@torch.library.custom_op('b200rl::fqf_fraction_bwd', mutates_args=())
+def fqf_fraction_bwd(g: Tensor, g_loss: Tensor, grad_unit: Tensor, B: int, N: int) -> Tensor:
+    """-> d / d quantiles (B, N+1); verifies a copy of the forward-written unit gradient when there is one"""
+    kl, pg = _one(g_loss)
+    skip = 1 if grad_unit.numel() else 0
+    grad = grad_unit.clone() if skip else g.new_empty(B, N + 1)
+    return ops.fqf_fraction_bwd_(g, pg, B, N, skip, grad)
+
+
+@fqf_fraction_bwd.register_fake
+def _(g, g_loss, grad_unit, B, N):
+    return g.new_empty(B, N + 1)
+
+
+def _fqf_fraction_setup(ctx, inputs, output):
+    ctx.save_for_backward(output[1], output[2])
+    ctx.cfg = inputs[4:6]
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[1:])
+
+
+def _fqf_fraction_backward(ctx, g_loss, *_):
+    if g_loss is None:
+        return (None, ) * 7
+    g, grad_unit = ctx.saved_tensors
+    return (None, None, fqf_fraction_bwd(g, g_loss, grad_unit, *ctx.cfg)) + (None, ) * 4
+
+
+fqf_fraction_fwd.register_autograd(_fqf_fraction_backward, setup_context=_fqf_fraction_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # ppo_error_continuous and its policy-only / HAPPO call sites (csrc/heads.cu): the forward launch always writes the
 # gradients for the call site's record when a gradient is wanted, so the backward op always verifies a copy
 # ---------------------------------------------------------------------------------------------------------------------
@@ -1187,3 +1425,42 @@ def coma(logit, q_value, target_q, action, reward, weight, T, B, A, N, gamma, la
     out = coma_fwd(logit, q_value, target_q, action, reward, weight, T, B, A, N, float(gamma), float(lambda_),
                    _want_grad(logit, q_value))[0]
     return out[0], out[1], out[2]
+
+
+def qntd_seq(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, vg_stride, gamma_ps, S, N, nstep, gamma,
+             rescale, criterion, crit_param, seq_len, priority_mix):
+    """-> (loss, td, priority), as QNStepTDFunction's sequence form"""
+    vg, vg_scalar = _scalar_or_tensor(value_gamma)
+    loss, td, _, prio, _ = qntd_seq_fwd(q, next_n_q, action, next_n_action, reward, done, weight, vg, vg_scalar, vg_stride,
+                                        gamma_ps, S, N, nstep, gamma, rescale, criterion, crit_param, seq_len,
+                                        priority_mix, _want_grad(q))
+    return loss, td, prio
+
+
+def dqfd(q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done, done1, weight, value_gamma, vg_stride,
+         is_expert, S, N, nstep, gamma, cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1, lam_s, margin,
+         seq_len, priority_mix, want_targets, want_priority):
+    """-> (loss, td, s_n, s_1, s_je, tn, t1, prio), as DQfDTDFunction; value_gamma and is_expert may be python floats"""
+    vg, vg_scalar = _scalar_or_tensor(value_gamma)
+    ie, ie_scalar = _scalar_or_tensor(is_expert)
+    loss, td, stats, _, tn, t1, prio, _ = dqfd_fwd(
+        q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done, done1, weight, vg, vg_scalar, vg_stride,
+        ie, ie_scalar, S, N, nstep, gamma, cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1, lam_s, margin,
+        seq_len, priority_mix, want_targets, want_priority, _want_grad(q))
+    s_n, s_1, s_je = stats.unbind(0)
+    return loss, td, s_n, s_1, s_je, tn, t1, prio
+
+
+def soft_td(q, target_q, next_q, action, reward, done, weight, value_gamma, vg_stride, mode, S, G, N, nstep, gamma, tau,
+            alpha, cum_reward, criterion, crit_param):
+    """-> (loss, td, target, action_gap, clipfrac, record_target_v), as SoftTDFunction"""
+    vg, vg_scalar = _scalar_or_tensor(value_gamma)
+    loss, td, _, target, gap, clip, rec, _ = soft_td_fwd(q, target_q, next_q, action, reward, done, weight, vg, vg_scalar,
+                                                         vg_stride, mode, S, G, N, nstep, gamma, tau, alpha, cum_reward,
+                                                         criterion, crit_param, _want_grad(q))
+    return loss, td, target, gap, clip, rec
+
+
+def fqf_fraction(q_tau_i, q_value, quantiles, action, B, N):
+    """-> the fraction loss, as FQFFractionFunction"""
+    return fqf_fraction_fwd(q_tau_i, q_value, quantiles, action, B, N, _want_grad(quantiles))[0]
