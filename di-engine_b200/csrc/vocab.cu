@@ -58,6 +58,23 @@
 // at once when all three upstream gradients are the forward's, rewrites only d / d value (O(1) per row) when just g_val
 // differs, and otherwise recomputes both.  Traffic: (1 + 1) * V * sizeof(T) per row, plus O(1) per row -- logit_new read
 // once, its gradient written once, with the same L2 re-read of logit_new past VOCAB_SMEM_CAP.
+//
+// GRPO / RLOO from the lm_head's hidden states (rl_utils/lm_linear.py; b200rl_lm_linear_fwd / _bwd): the caller computes
+// the logits one chunk of token rows at a time into a (rows_per_chunk, V) buffer Z with a GEMM, and MODE = VM_GRPO_LIN /
+// VM_RLOO_LIN streams Z alone (NR = 1, as VM_A2C): the old and reference terms come from per-token fp32 log-probabilities
+// logp_old / logp_ref, read with action, weight and the sequence's normaliser at the global row row0 + r.  The
+// normalisers couple rows across chunk boundaries (a chunk may split a sequence), so lm_seq_kernel forms them once,
+// before the first chunk: sum_s w[b, s] and the row's advantage (GRPO: adv[b]; RLOO: the leave-one-out advantage).
+// Each chunk's CTAs store their loss partials into the chunk's own slice of the workspace and the last chunk's launch
+// adds all of them in one finalize_sums (fixed chunk plan -> the same bits on every run).
+// In place: these modes write d loss / d Z over Z itself, which the caller then feeds to the dH / dW GEMMs.  That is safe
+// because (1) one CTA owns a row, (2) each element's gradient is stored by the thread that has just read that element in
+// the softmax pass (from the shared-memory copy, or from Z for the part past VOCAB_SMEM_CAP), and (3) nothing reads the
+// row after that pass.  The logits and the gradient therefore alias: neither pointer is __restrict__ (VocabArgs holds
+// plain pointers), and Z is read with coherent loads (__ldca), never the read-only path (__ldg), which requires the data
+// to stay unwritten for the kernel's lifetime.  The log-prob mode (VM_LOGP) and the in-place backward with a per-row
+// coefficient (VM_BWD, whose load / store pair is already per element and coherent) run on chunk pointers unchanged.
+// Traffic floor per row: 2 * V * sizeof(T) -- Z read once, d Z written once.
 #include <cuda_bf16.h>
 #include <math.h>
 
@@ -74,6 +91,8 @@ constexpr int VM_GRPO = 0, VM_RLOO = 1, VM_LOGP = 2, VM_BWD = 3;
 constexpr int VM_PPO = 4, VM_PPO_BWD = 8, PPO_ENT = 1, PPO_KL = 2;  // VM_PPO + flags: 4..7; VM_PPO_BWD + PPO_ENT: 8, 9
 // A2C: forward 12; backward VM_PPO_BWD + PPO_ENT + PPO_VAL = 11 (the PPO backward with the value slot)
 constexpr int PPO_VAL = 2, VM_A2C = 12;
+// GRPO / RLOO on one chunk of a GEMM's output buffer, in place (see the header)
+constexpr int VM_GRPO_LIN = 13, VM_RLOO_LIN = 14;
 constexpr float kL2E = 1.4426950408889634f;
 
 // 16-byte vectors of T, widened to fp32
@@ -274,15 +293,21 @@ struct VocabArgs {
     const float* ret;          // forward: return_ (rows)
     float* dval;               // forward: d value_loss / d value per row; backward: read
     float* grad_value;         // d / d value (rows), fp32
+    // VM_GRPO_LIN / VM_RLOO_LIN: the per-row operands start at the chunk's first row; the sequence index is (row0 + r) / S
+    const float* lp_old;       // (rows)
+    const float* lp_ref;       // GRPO: (rows)
+    const float* seq;          // (2, nb): sum_s w[b, s], then the advantage of sequence b (lm_seq_kernel)
+    long long row0, nb;
 };
 
-template <int NR, bool CACHE, class T, bool ENT = false>
+// INPL: stream 0 is the buffer the kernel overwrites with its gradient -- coherent loads, not the read-only path
+template <int NR, bool CACHE, class T, bool ENT = false, bool INPL = false>
 __device__ __forceinline__ void stream_vecs(const uint4* const (&p)[NR], int i, float (&m)[NR], float (&s)[NR],
                                             uint4* cache, int capv, float* t = nullptr) {
     constexpr int W = VecT<T>::W;
     uint4 u[NR];
 #pragma unroll
-    for (int r = 0; r < NR; ++r) u[r] = r == 0 ? __ldg(p[0] + i) : __ldcs(p[r] + i);
+    for (int r = 0; r < NR; ++r) u[r] = r == 0 ? (INPL ? __ldca(p[0] + i) : __ldg(p[0] + i)) : __ldcs(p[r] + i);
     if (CACHE && i < capv) cache[i] = u[0];
 #pragma unroll
     for (int r = 0; r < NR; ++r) {
@@ -302,8 +327,9 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
     constexpr bool A2C = MODE == VM_A2C, VAL = A2C || (PBWD && (MODE & PPO_VAL));  // VAL: the A2C value slot
     constexpr bool ENT = ((PPO || PBWD) && (MODE & PPO_ENT)) || A2C, KL = PPO && (MODE & PPO_KL);
     constexpr bool BWD = MODE == VM_BWD || PBWD;
+    constexpr bool LIN = MODE == VM_GRPO_LIN || MODE == VM_RLOO_LIN;  // one in-place stream (NR = 1)
     constexpr int NR = MODE == VM_GRPO ? 3 : (MODE == VM_RLOO ? 2 : (PPO ? (KL ? 3 : 2) : 1));
-    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO || A2C;
+    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO || A2C || LIN;
     constexpr int NP = PPO ? 5 : 3;
     extern __shared__ uint4 s_row[];
     __shared__ float s_m[NR][VOCAB_NT / 32], s_s[NR][VOCAB_NT / 32], s_w[VOCAB_NT / 32];
@@ -374,16 +400,16 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
             int i = tid;
             for (; i + VOCAB_NT < nvec; i += 2 * VOCAB_NT) {
                 if (cache) {
-                    stream_vecs<NR, true, T, ENT>(vp, i, m, s, s_row, a.capv, &t);
-                    stream_vecs<NR, true, T, ENT>(vp, i + VOCAB_NT, m, s, s_row, a.capv, &t);
+                    stream_vecs<NR, true, T, ENT, LIN>(vp, i, m, s, s_row, a.capv, &t);
+                    stream_vecs<NR, true, T, ENT, LIN>(vp, i + VOCAB_NT, m, s, s_row, a.capv, &t);
                 } else {
-                    stream_vecs<NR, false, T, ENT>(vp, i, m, s, s_row, 0, &t);
-                    stream_vecs<NR, false, T, ENT>(vp, i + VOCAB_NT, m, s, s_row, 0, &t);
+                    stream_vecs<NR, false, T, ENT, LIN>(vp, i, m, s, s_row, 0, &t);
+                    stream_vecs<NR, false, T, ENT, LIN>(vp, i + VOCAB_NT, m, s, s_row, 0, &t);
                 }
             }
             if (i < nvec) {
-                if (cache) stream_vecs<NR, true, T, ENT>(vp, i, m, s, s_row, a.capv, &t);
-                else stream_vecs<NR, false, T, ENT>(vp, i, m, s, s_row, 0, &t);
+                if (cache) stream_vecs<NR, true, T, ENT, LIN>(vp, i, m, s, s_row, a.capv, &t);
+                else stream_vecs<NR, false, T, ENT, LIN>(vp, i, m, s, s_row, 0, &t);
             }
             // the unaligned head and tail, < 16 bytes each
             for (long long j = tid; j < h + (V - tail0); j += VOCAB_NT) {
@@ -485,6 +511,18 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
                     part[2] += H * w;
                     s_ce = ce;
                     s_h = H;
+                } else if constexpr (LIN) {  // the token head with the old / ref terms read per token
+                    const long long b = (a.row0 + row) / a.S;
+                    const float W_ = a.seq[b], adv = a.seq[a.nb + b];
+                    const float w = a.weight ? a.weight[row] : 1.f;
+                    const float lpo = a.lp_old[row];
+                    const TokenHead th = token_head<MODE == VM_GRPO_LIN>(
+                        lp[0], lpo, MODE == VM_GRPO_LIN ? a.lp_ref[row] : 0.f, adv, a.lo, a.hi, a.beta, a.inv_b / W_ * w);
+                    c = th.dlp;
+                    if (a.lp) a.lp[row] = lp[0];
+                    part[0] += th.loss * w / W_;
+                    part[1] += lpo - lp[0];
+                    part[2] += th.clipped;
                 } else if (LOSS) {
                     const long long b = row / a.S;
                     if (new_seq) {
@@ -518,7 +556,8 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
         T* gr = reinterpret_cast<T*>(a.grad) + off;
         uint4* gv = reinterpret_cast<uint4*>(gr + h);
         for (int i = tid; i < nvec; i += VOCAB_NT) {
-            const uint4 u = (LOSS && i < a.capv) ? s_row[i] : (BWD ? __ldcs(vp[0] + i) : __ldg(vp[0] + i));
+            const uint4 u = (LOSS && i < a.capv) ? s_row[i]
+                                                 : (BWD ? __ldcs(vp[0] + i) : (LIN ? __ldca(vp[0] + i) : __ldg(vp[0] + i)));
             float x[W];
             V_::unpack(u, x);
             const long long e0 = h + (long long)i * W;
@@ -593,6 +632,55 @@ __global__ void __launch_bounds__(VOCAB_HEAD_NT) token_head_kernel(const float* 
     grid_store_partials<3, VOCAB_HEAD_NT>(part, a.ws);
 }
 
+// The sequence normalisers of VM_GRPO_LIN / VM_RLOO_LIN, once per call: one CTA per sequence b at a time writes
+// seq[b] = sum_s w[b, s] (S without weights; token_head_kernel's order) and seq[nb + b] = the advantage of sequence b.
+__global__ void __launch_bounds__(VOCAB_HEAD_NT) lm_seq_kernel(VocabArgs a) {
+    pdl_prologue();
+    __shared__ float s_w[VOCAB_HEAD_NT / 32];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    float* seq = const_cast<float*>(a.seq);
+    for (long long b = blockIdx.x; b < a.nb; b += gridDim.x) {
+        float W_ = (float)a.S;
+        if (a.weight) {
+            float ws = 0.f;
+            for (long long j = tid; j < a.S; j += VOCAB_HEAD_NT) ws += a.weight[b * a.S + j];
+            ws = warp_sum(ws);
+            if (lane == 0) s_w[wid] = ws;
+            __syncthreads();
+            W_ = 0.f;
+            for (int w = 0; w < VOCAB_HEAD_NT / 32; ++w) W_ += s_w[w];
+            __syncthreads();
+        }
+        if (tid == 0) {
+            seq[b] = W_;
+            seq[a.nb + b] = a.reward ? rloo_adv(a.reward, a.K, a.Bp, b) : a.adv[b];
+        }
+    }
+}
+
+// x *= *g in place, in T, skipped on the device when *g == 1: the backward of the hidden-state losses scales the dH / dW
+// their forward wrote for a unit upstream gradient (b200rl_scale is fp32-only and out of place, which would hold a second
+// copy of a 2 GB dW)
+template <class T>
+__global__ void __launch_bounds__(256) scale_inplace_kernel(const float* __restrict__ g, T* x, long long n) {
+    pdl_prologue();
+    using V_ = VecT<T>;
+    constexpr int W = V_::W;
+    const float s = *g;
+    if (s == 1.f) return;
+    const long long nv = n / W, step = (long long)gridDim.x * blockDim.x;
+    const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    uint4* xv = reinterpret_cast<uint4*>(x);
+    for (long long i = t0; i < nv; i += step) {
+        float v[W];
+        V_::unpack(xv[i], v);
+#pragma unroll
+        for (int k = 0; k < W; ++k) v[k] = s * v[k];
+        xv[i] = V_::pack(v);
+    }
+    for (long long i = nv * W + t0; i < n; i += step) x[i] = V_::from_f(s * V_::to_f(x[i]));
+}
+
 }  // namespace b200rl
 
 using namespace b200rl;
@@ -638,6 +726,32 @@ int launch_dtype(int dtype, VocabArgs& a, float* out3, size_t ws_bytes, long lon
 
 bool sizes_ok(long long B, long long S, long long V) {
     return B > 0 && S > 0 && V > 0 && V < (1ll << 31) && B * S < (1ll << 40);
+}
+
+// One chunk of VM_GRPO_LIN / VM_RLOO_LIN.  Every chunk of a call launches the same grid (the plan's chunk_rows, not this
+// chunk's rows, caps it), so chunk c's CTAs own partial rows [c * grid, (c + 1) * grid); CTAs past the last chunk's rows
+// store zeros.  The last chunk adds all n_chunks * grid rows.
+template <class T, int MODE>
+int launch_lin(VocabArgs& a, long long chunk_rows, long long B, float* out3, size_t ws_bytes, cudaStream_t st) {
+    constexpr auto kern = vocab_rows_kernel<T, MODE>;
+    const long long nvec_max = (a.V * (long long)sizeof(T) + 15) / 16;
+    a.capv = a.grad ? (int)min(nvec_max, (long long)(VOCAB_SMEM_CAP / 16)) : 0;
+    const size_t smem = (size_t)a.capv * 16;
+    int sms = 0, per_sm = 0;
+    if (int rc = resident_ctas<kern>(VOCAB_NT, smem, sms, per_sm)) return rc;
+    const long long grid = min((long long)sms * per_sm, chunk_rows);
+    const long long N = B * a.S, n_chunks = (N + chunk_rows - 1) / chunk_rows, chunk = a.row0 / chunk_rows;
+    if (!ws_partials_fit(n_chunks * grid * 3, ws_bytes)) return B200RL_ERR_WORKSPACE;
+    float* ws = a.ws;
+    a.ws = ws + chunk * grid * 3;
+    if (int rc = launch_k(kern, (int)grid, VOCAB_NT, smem, st, a)) return rc;
+    if (a.row0 + a.rows < N) return B200RL_OK;
+    FinalizeArgs fa{};
+    fa.scale[0] = 1.0 / (double)B;
+    fa.scale[1] = fa.scale[2] = 1.0 / (double)N;
+    fa.k = 3;
+    fa.n_blocks = (int)(n_chunks * grid);
+    return launch_finalize(ws, out3, fa, st);
 }
 
 }  // namespace
@@ -826,4 +940,80 @@ extern "C" int b200rl_token_head_fwd(const float* logp_new, const float* logp_ol
     fa.k = 3;
     fa.n_blocks = (int)grid;
     return launch_finalize(workspace, out3, fa, st);
+}
+
+// GRPO / RLOO / per-token log p from the lm_head's hidden states, one chunk of token rows per call
+// (ding/rl_utils/grpo.py:43-60 and rloo.py:41-62 with log_prob_fn = efficient_method, log_prob_utils.py:29-48, on
+// logits = hidden @ lm_weight^T that the caller computes chunk by chunk; the logit_old / logit_ref streams of
+// b200rl_grpo_fwd_grad become the per-token logp_old / logp_ref)
+extern "C" int b200rl_lm_linear_fwd(int mode, int dtype, void* logits, long long row0, long long rows,
+                                    long long chunk_rows, long long V, long long B, long long S, const long long* action,
+                                    const float* logp_old, const float* logp_ref, const float* adv, const float* reward,
+                                    long long K, const float* weight, float* seq, double clip_ratio, double beta,
+                                    float* logp, float* lse, float* out3, int want_grad, float* workspace,
+                                    size_t workspace_bytes, void* stream) {
+    const long long N = B * S;
+    if (!sizes_ok(B, S, V) || rows < 1 || chunk_rows < rows || row0 < 0 || row0 % chunk_rows || row0 + rows > N ||
+        !aligned_logits(logits) || !action || !lse)
+        return B200RL_ERR_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    VocabArgs a{};
+    a.x[0] = logits; a.action = action + row0; a.lse = lse + row0;
+    a.rows = rows; a.S = S; a.V = V;
+    if (mode == B200RL_LM_LOGP) {
+        if (!logp) return B200RL_ERR_ARG;
+        a.lp = logp + row0;
+        return launch_dtype<VM_LOGP>(dtype, a, nullptr, 0, rows, st);
+    }
+    const bool grpo = mode == B200RL_LM_GRPO;
+    if ((!grpo && mode != B200RL_LM_RLOO) || !logp_old || !seq || !out3 || !workspace ||
+        (grpo ? (!logp_ref || !adv) : (!reward || K < 1 || K > (1 << 20) || B % K)) ||
+        (dtype != B200RL_DTYPE_F32 && dtype != B200RL_DTYPE_BF16))
+        return B200RL_ERR_ARG;
+    a.adv = adv; a.reward = reward; a.K = (int)K; a.Bp = grpo ? 0 : B / K;
+    a.weight = weight; a.seq = seq; a.nb = B; a.row0 = row0; a.ws = workspace;
+    if (row0 == 0) {  // the sequence normalisers, ahead of the first chunk
+        int sms = 0, per_sm = 0;
+        if (int rc = resident_ctas<lm_seq_kernel>(VOCAB_HEAD_NT, 0, sms, per_sm)) return rc;
+        if (int rc = launch_k(lm_seq_kernel, (int)min((long long)sms * per_sm, B), VOCAB_HEAD_NT, 0, st, a)) return rc;
+    }
+    a.weight = weight ? weight + row0 : nullptr;
+    a.lp_old = logp_old + row0; a.lp_ref = grpo ? logp_ref + row0 : nullptr; a.lp = logp ? logp + row0 : nullptr;
+    a.grad = want_grad ? logits : nullptr;
+    a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio); a.beta = grpo ? (float)beta : 0.f;
+    a.inv_b = (float)(1.0 / (double)B);
+    if (dtype == B200RL_DTYPE_F32)
+        return grpo ? launch_lin<float, VM_GRPO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st)
+                    : launch_lin<float, VM_RLOO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st);
+    return grpo ? launch_lin<__nv_bfloat16, VM_GRPO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st)
+                : launch_lin<__nv_bfloat16, VM_RLOO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st);
+}
+
+// The backward of token_logp_linear on one chunk, in place (log_prob_utils.py:29-48's autograd, as b200rl_token_logp_bwd)
+extern "C" int b200rl_lm_linear_bwd(int dtype, void* logits, long long row0, long long rows, long long V,
+                                    const long long* index, const float* lse, const float* dlogp, void* stream) {
+    if (!sizes_ok(rows, 1, V) || row0 < 0 || !aligned_logits(logits) || !index || !lse || !dlogp) return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logits; a.grad = logits;
+    a.action = index + row0; a.lse = const_cast<float*>(lse + row0); a.coef_in = dlogp + row0;
+    a.rows = rows; a.S = 1; a.V = V;
+    return launch_dtype<VM_BWD>(dtype, a, nullptr, 0, rows, (cudaStream_t)stream);
+}
+
+extern "C" int b200rl_lm_linear_scale(int dtype, const float* g, void* x, long long n, void* stream) {
+    if (n < 0 || !g || (n > 0 && (!x || !aligned16(x)))) return B200RL_ERR_ARG;
+    if (n == 0) return B200RL_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    int sms = 0, per_sm = 0;
+    if (dtype == B200RL_DTYPE_F32) {
+        if (int rc = resident_ctas<scale_inplace_kernel<float>>(256, 0, sms, per_sm)) return rc;
+        const long long grid = min((long long)sms * per_sm, (n / 4 + 255) / 256 + 1);
+        return launch_k(scale_inplace_kernel<float>, (int)grid, 256, 0, st, g, (float*)x, n);
+    }
+    if (dtype == B200RL_DTYPE_BF16) {
+        if (int rc = resident_ctas<scale_inplace_kernel<__nv_bfloat16>>(256, 0, sms, per_sm)) return rc;
+        const long long grid = min((long long)sms * per_sm, (n / 8 + 255) / 256 + 1);
+        return launch_k(scale_inplace_kernel<__nv_bfloat16>, (int)grid, 256, 0, st, g, (__nv_bfloat16*)x, n);
+    }
+    return B200RL_ERR_ARG;
 }

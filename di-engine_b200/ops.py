@@ -2072,3 +2072,204 @@ def token_head_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
     if lp_new.requires_grad and torch.is_grad_enabled():
         loss = _ScaleSaved.apply(lp_new, loss, dlp)
     return loss, out[1], out[2]
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# GRPO / RLOO / per-token log p from the lm_head's hidden states (rl_utils/lm_linear.py): the logits exist one chunk of
+# token rows at a time (cuBLAS through torch.mm, with the caller's matmul precision settings, as F.linear), and the row
+# work runs in place on the chunk (csrc/vocab.cu, b200rl_lm_linear_fwd / _bwd)
+# ----------------------------------------------------------------------------------------------------------------
+# Bytes of the one (rows_per_chunk, V) logit buffer of a call.  Chosen by measurement (tools/bench_lm_linear.py --budgets,
+# one H100 80GB HBM3 at 700 W, 16 x 1024 tokens, D = 3584, V = 152 064 bf16): GRPO forward + backward took 147 / 114 /
+# 98 / 90 ms at 128 / 256 / 512 / 1024 MiB, because the dW GEMM's inner dimension is the chunk's rows and short chunks
+# leave it far from peak (390 -> 700 TFLOP/s over the three GEMMs).  Up to 1 GiB the call's peak memory did not move
+# (3.39 GB: the fp32 dW accumulator and the rounded dW, which coexist after the last chunk, outweigh the chunk).
+# Module-level so that a test can shrink it to force many chunks.
+LM_CHUNK_BYTES = 1 << 30
+_LM_MODE = {'grpo': 0, 'rloo': 1, 'logp': 2}  # B200RL_LM_GRPO, B200RL_LM_RLOO, B200RL_LM_LOGP
+_VOCAB_CTAS_PER_SM = 4  # vocab_rows_kernel: 512 threads, at most 2048 resident per SM
+_WS_PARTIAL_WORDS = 256000 - 16  # WS_PARTIAL_LIMIT_WORDS - WS_CTRL_WORDS (csrc/common.cuh)
+
+
+def sm_count(device):
+    return torch.cuda.get_device_properties(device).multi_processor_count
+
+
+def lm_chunk_plan(N, V, itemsize, sms, loss):
+    """(rows per chunk, chunks) for N token rows of V logits of ``itemsize`` bytes: the largest multiple of 128 rows whose
+    logits fit in LM_CHUNK_BYTES (at least 128), or all N rows when there are fewer.  A loss call stores 3 partial sums
+    per CTA per chunk (at most sms * 4 CTAs, and no more than the chunk's rows); raises before any launch when they would
+    not fit in the workspace."""
+    rows = min(N, max(128, LM_CHUNK_BYTES // (V * itemsize) // 128 * 128))
+    n = -(-N // rows)
+    if loss and n * min(rows, sms * _VOCAB_CTAS_PER_SM) * 3 > _WS_PARTIAL_WORDS:
+        raise ValueError("di_engine_b200: %d token rows in %d chunks of %d need more loss partials than the workspace "
+                         "holds; raise ops.LM_CHUNK_BYTES" % (N, n, rows))
+    return rows, n
+
+
+def _acc_dw(acc, z, h):
+    """acc (V, D) fp32 += z^T h: fp32 accumulation of the chunks' dW whatever the GEMM operands' dtype"""
+    if z.dtype == torch.float32:
+        acc.addmm_(z.t(), h)
+    else:
+        torch.addmm(acc, z.t(), h, out_dtype=torch.float32, out=acc)
+
+
+def _dw_out(acc, dtype):
+    """the fp32 dW accumulator rounded once to the weight's dtype"""
+    return acc if acc is None or acc.dtype == dtype else acc.to(dtype)
+
+
+def lm_linear_loss_(hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt, clip_ratio, beta, want_dh,
+                    want_dw):
+    """GRPO (``kind`` 'grpo', side = adv (B)) or RLOO ('rloo', side = reward (K, B / K)) on hidden (N = B*S, D) and
+    lm_weight (V, D), both contiguous and of one dtype; action, lp_old, lp_ref (N), weight (N) or None.  Per chunk: the
+    logit GEMM, the row launch (which overwrites the chunk with d loss / d logits for a unit upstream gradient when a
+    gradient is wanted), then dH[chunk] = dZ W and dW += dZ^T H[chunk].  -> (out3 = loss / approx_kl / clipfrac, dH or
+    None, dW or None)."""
+    N, D = hidden.shape
+    V = lm_weight.shape[0]
+    dev = hidden.device
+    rows, n = lm_chunk_plan(N, V, hidden.element_size(), sm_count(dev), True)
+    want = want_dh or want_dw
+    grpo = kind == 'grpo'
+    z = torch.empty(rows, V, dtype=hidden.dtype, device=dev)
+    dh = torch.empty_like(hidden) if want_dh else None
+    acc = torch.zeros(V, D, dtype=torch.float32, device=dev) if want_dw else None
+    out = torch.empty(3, dtype=torch.float32, device=dev)
+    lse = torch.empty(N, dtype=torch.float32, device=dev)
+    seq = torch.empty(2 * B, dtype=torch.float32, device=dev)
+    wt = lm_weight.t()
+    with on_device(dev):
+        ws = workspace(dev)
+        L, st = lib(), stream_ptr()
+        for c in range(n):
+            r0 = c * rows
+            zc, hc = z[:min(rows, N - r0)], hidden[r0:r0 + rows]
+            torch.mm(hc, wt, out=zc)
+            rc = L.b200rl_lm_linear_fwd(_LM_MODE[kind], dt, ptr(zc), r0, zc.shape[0], rows, V, B, S, ptr(action),
+                                        ptr(lp_old), ptr(lp_ref), ptr(side) if grpo else None,
+                                        None if grpo else ptr(side), 0 if grpo else side.shape[0], ptr(weight), ptr(seq),
+                                        clip_ratio, beta, None, ptr(lse), ptr(out), 1 if want else 0, ptr(ws),
+                                        ws.numel() * 4, st)
+            _lib.check(rc, 'b200rl_lm_linear_fwd')
+            if want_dh:
+                torch.mm(zc, lm_weight, out=dh[r0:r0 + rows])
+            if want_dw:
+                _acc_dw(acc, zc, hc)
+    del z, zc
+    return out, dh, _dw_out(acc, hidden.dtype)
+
+
+def lm_scale_(dt, pg, x):
+    """x *= *pg in place, skipped on the device when *pg == 1 (the forward wrote x for a unit upstream gradient)"""
+    with on_device(x.device):
+        rc = lib().b200rl_lm_linear_scale(dt, pg, ptr(x), x.numel(), stream_ptr())
+    _lib.check(rc, 'b200rl_lm_linear_scale')
+    return x
+
+
+class LMLinearLossFunction(torch.autograd.Function):
+    """grpo_policy_error_linear / rloo_policy_error_linear: outputs loss (differentiable w.r.t. hidden and lm_weight),
+    approx_kl and clipfrac.  The forward also writes dH and dW for a unit upstream gradient, each only if its input
+    requires grad; ``backward`` hands them to autograd, scaled in place by the upstream gradient on the device (a no-op
+    when it is 1).  A repeated backward recomputes them."""
+
+    @staticmethod
+    def forward(ctx, hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt, clip_ratio, beta):
+        want = ctx.needs_input_grad[:2]
+        out, dh, dw = lm_linear_loss_(hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt,
+                                      clip_ratio, beta, *want)
+        ctx.save_for_backward(hidden, lm_weight, action, lp_old, lp_ref, side, weight)
+        ctx.cfg = (kind, B, S, dt, clip_ratio, beta)
+        ctx.spec = (dh, dw)
+        ctx.set_materialize_grads(False)
+        loss, approx_kl, clipfrac = out[0], out[1], out[2]
+        ctx.mark_non_differentiable(approx_kl, clipfrac)
+        return loss, approx_kl, clipfrac
+
+    @staticmethod
+    def backward(ctx, g_loss, _g_kl, _g_cf):
+        if g_loss is None:
+            return (None, ) * 13
+        spec = _forward_grads(ctx)
+        if spec is None:  # a repeated backward: the first one handed out (and scaled) the forward's buffers
+            hidden, lm_weight, *rest = ctx.saved_tensors
+            _, dh, dw = lm_linear_loss_(hidden, lm_weight, *rest, *ctx.cfg, *ctx.needs_input_grad[:2])
+        else:
+            dh, dw = spec
+        keep, (pg, ) = _grads(g_loss)
+        for x in (dh, dw):
+            if x is not None:
+                lm_scale_(ctx.cfg[3], pg, x)
+        return (dh, dw) + (None, ) * 11
+
+
+def lm_logp_fwd_(hidden, lm_weight, index, dt):
+    """per-token log p(index) and logsumexp (N) fp32 of logits = hidden (N, D) @ lm_weight (V, D)^T, chunk by chunk"""
+    N = hidden.shape[0]
+    V = lm_weight.shape[0]
+    dev = hidden.device
+    rows, n = lm_chunk_plan(N, V, hidden.element_size(), sm_count(dev), False)
+    z = torch.empty(rows, V, dtype=hidden.dtype, device=dev)
+    lp = torch.empty(N, dtype=torch.float32, device=dev)
+    lse = torch.empty(N, dtype=torch.float32, device=dev)
+    wt = lm_weight.t()
+    with on_device(dev):
+        L, st = lib(), stream_ptr()
+        for c in range(n):
+            r0 = c * rows
+            zc = z[:min(rows, N - r0)]
+            torch.mm(hidden[r0:r0 + rows], wt, out=zc)
+            rc = L.b200rl_lm_linear_fwd(_LM_MODE['logp'], dt, ptr(zc), r0, zc.shape[0], rows, V, N, 1, ptr(index), None,
+                                        None, None, None, 0, None, None, 0.0, 0.0, ptr(lp), ptr(lse), None, 0, None, 0,
+                                        st)
+            _lib.check(rc, 'b200rl_lm_linear_fwd')
+    return lp, lse
+
+
+def lm_logp_bwd_(hidden, lm_weight, index, lse, g, dt, want_dh, want_dw):
+    """The backward of ``lm_logp_fwd_`` for the upstream gradient g (N) fp32: per chunk the logit GEMM again, the in-place
+    launch dZ = g * (onehot(index) - softmax(Z)), then the gradient GEMMs.  -> (dH or None, dW or None)"""
+    N, D = hidden.shape
+    V = lm_weight.shape[0]
+    dev = hidden.device
+    rows, n = lm_chunk_plan(N, V, hidden.element_size(), sm_count(dev), False)
+    z = torch.empty(rows, V, dtype=hidden.dtype, device=dev)
+    dh = torch.empty_like(hidden) if want_dh else None
+    acc = torch.zeros(V, D, dtype=torch.float32, device=dev) if want_dw else None
+    wt = lm_weight.t()
+    with on_device(dev):
+        L, st = lib(), stream_ptr()
+        for c in range(n):
+            r0 = c * rows
+            zc, hc = z[:min(rows, N - r0)], hidden[r0:r0 + rows]
+            torch.mm(hc, wt, out=zc)
+            rc = L.b200rl_lm_linear_bwd(dt, ptr(zc), r0, zc.shape[0], V, ptr(index), ptr(lse), ptr(g), st)
+            _lib.check(rc, 'b200rl_lm_linear_bwd')
+            if want_dh:
+                torch.mm(zc, lm_weight, out=dh[r0:r0 + rows])
+            if want_dw:
+                _acc_dw(acc, zc, hc)
+    del z, zc
+    return dh, _dw_out(acc, hidden.dtype)
+
+
+class TokenLogpLinearFunction(torch.autograd.Function):
+    """token_logp_linear: log p(index) (N) fp32 of logits = hidden @ lm_weight^T, differentiable w.r.t. hidden and
+    lm_weight.  Saves hidden, lm_weight, index and the per-row logsumexp only; the backward recomputes each chunk's
+    logits."""
+
+    @staticmethod
+    def forward(ctx, hidden, lm_weight, index, dt):
+        lp, lse = lm_logp_fwd_(hidden, lm_weight, index, dt)
+        ctx.save_for_backward(hidden, lm_weight, index, lse)
+        ctx.dt = dt
+        return lp
+
+    @staticmethod
+    def backward(ctx, g):
+        hidden, lm_weight, index, lse = ctx.saved_tensors
+        dh, dw = lm_logp_bwd_(hidden, lm_weight, index, lse, g.float().contiguous(), ctx.dt, *ctx.needs_input_grad[:2])
+        return dh, dw, None, None

@@ -700,6 +700,36 @@ B200RL_API int b200rl_a2c_lm_bwd(int dtype, const void* logit, const long long* 
                       const float* dvalue, const float* g_policy, const float* g_value, const float* g_entropy,
                       const float* g_used, float* g_hint, void* grad_logit, float* grad_value, void* stream);
 
+/* ---- GRPO / RLOO / per-token log p from the lm_head's hidden states, one chunk of token rows per call (csrc/vocab.cu) --
+ * The caller computes logits = hidden @ lm_weight^T (nn.Linear(D, V, bias=False)) one chunk of rows at a time into a
+ * (chunk_rows, V) buffer `logits` (dtype, 16-byte aligned), so that the (B*S, V) logits never exist.  Rows are the B*S
+ * tokens, row = b*S + s; the chunk holds rows [row0, row0 + rows), row0 a multiple of chunk_rows (the plan's rows per
+ * chunk; every chunk but the last has rows = chunk_rows).  Every per-token operand is the whole (B*S) array, read at the
+ * global row; logp_old / logp_ref are fp32 log-probabilities of the old / reference policy (what
+ * log_prob_fn(logit_old, action) gave the reference's loss).
+ * b200rl_lm_linear_fwd: mode B200RL_LM_GRPO (ding/rl_utils/grpo.py:43-60; adv (B), beta) or B200RL_LM_RLOO (rloo.py:41-62;
+ *   reward (K, B / K)): the token head of b200rl_grpo_fwd_grad on the chunk's rows; lse (and logp, nullable) per row.
+ *   With want_grad it overwrites `logits` in place with d loss / d logits for a unit upstream gradient.  The call with
+ *   row0 = 0 first forms seq (2*B floats, the caller's, passed to every call): sum_s w[b, s] and the advantage of b.
+ *   Every chunk stores its loss partials into its own slice of the workspace, and the call that covers the last row
+ *   adds all of them into out3 = {loss, approx_kl, clipfrac} (B200RL_ERR_WORKSPACE if the chunks' partials do not fit).
+ *   Mode B200RL_LM_LOGP (log_prob_utils.py:29-48): logp (B*S) = z[a] - logsumexp(z) and lse for the chunk's rows.
+ * b200rl_lm_linear_bwd: logits[r] = dlogp[row0 + r] * (onehot(index) - softmax(logits[r])) in place, from the saved lse:
+ *   the backward of mode B200RL_LM_LOGP on one recomputed chunk.
+ * b200rl_lm_linear_scale: x (n values of dtype, 16-byte aligned) *= *g in place; returns at once on the device when
+ *   *g == 1 -- the backward of the GRPO / RLOO forward's gradients. */
+#define B200RL_LM_GRPO 0
+#define B200RL_LM_RLOO 1
+#define B200RL_LM_LOGP 2
+B200RL_API int b200rl_lm_linear_fwd(int mode, int dtype, void* logits, long long row0, long long rows, long long chunk_rows,
+                         long long V, long long B, long long S, const long long* action, const float* logp_old,
+                         const float* logp_ref, const float* adv, const float* reward, long long K, const float* weight,
+                         float* seq, double clip_ratio, double beta, float* logp, float* lse, float* out3, int want_grad,
+                         float* workspace, size_t workspace_bytes, void* stream);
+B200RL_API int b200rl_lm_linear_bwd(int dtype, void* logits, long long row0, long long rows, long long V,
+                         const long long* index, const float* lse, const float* dlogp, void* stream);
+B200RL_API int b200rl_lm_linear_scale(int dtype, const float* g, void* x, long long n, void* stream);
+
 /* ---- data-parallel exchange step: one-shot all-reduce (mean) of n <= 8 floats over NVLink peer memory -----------
  * Replaces the small-message NCCL all-reduce of the packed loss scalars (mean of rank means,
  * ding/utils/pytorch_ddp_dist_helper.py:38-47).  mailbox_ptrs_dev: device array of `world` pointers, entry r = the
