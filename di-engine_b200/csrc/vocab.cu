@@ -75,6 +75,22 @@
 // to stay unwritten for the kernel's lifetime.  The log-prob mode (VM_LOGP) and the in-place backward with a per-row
 // coefficient (VM_BWD, whose load / store pair is already per element and coherent) run on chunk pointers unchanged.
 // Traffic floor per row: 2 * V * sizeof(T) -- Z read once, d Z written once.
+//
+// PPO / A2C from the lm_head's hidden states (ppo_policy_error_linear / a2c_error_linear; b200rl_lm_linear_pg_fwd): MODE =
+// VM_PPO_LIN + PPO_ENT / PPO_KL and VM_A2C_LIN run on the same chunk Z in place, one stream (NR = 1), reading fp32
+// logp_old / logp_pretrained, action, adv, weight and (A2C) value / return_ at the global row row0 + r.  Their row
+// epilogues are VM_PPO's (surrogate / kl_term of ppo_math.cuh, H = log s - t / s from the online entropy accumulator) and
+// VM_A2C's, and the gradient is the header's d / d Z = c_act * (onehot(a) - p) - c_ent * p * (log p + H) -- but with
+// the upstream gradients (g_pol, g_ent, g_kl) = (1, w_ent, w_kl) (A2C: (g_pol, g_val, g_ent) = (1, w_val, w_ent)) taken
+// from the launch arguments, so the one differentiable output is loss = policy + w_ent * entropy + w_kl * kl
+// (+ w_val * value).  There is no record to verify: the caller scales d Z's products dH / dW by the actual upstream
+// gradient of that loss, which a per-component mix could not be once the chunk is gone.  A2C also writes
+// d loss / d value = w_val * (-2 * w * dv / M) in fp32 at the global row.  No sequence normaliser: both take plain means
+// over all M = B*S rows, so lm_seq_kernel is not launched.  Each chunk stores its partials (PPO: policy, entropy, kl,
+// approx_kl, clipfrac; A2C: policy, value, entropy) into its own workspace slice, and the last chunk's launch adds them
+// in one finalize_sums.  In place as GRPO / RLOO above: one CTA owns a row; H and lse are known before the gradient pass
+// because the streaming pass forms them; each element's gradient is stored by the thread that has just read that element
+// in the softmax pass; nothing reads the row after that pass; Z is read with __ldca, never __ldg.  Traffic floor per row: 2 * V * sizeof(T) -- Z read once, d Z written once.
 #include <cuda_bf16.h>
 #include <math.h>
 
@@ -93,6 +109,8 @@ constexpr int VM_PPO = 4, VM_PPO_BWD = 8, PPO_ENT = 1, PPO_KL = 2;  // VM_PPO + 
 constexpr int PPO_VAL = 2, VM_A2C = 12;
 // GRPO / RLOO on one chunk of a GEMM's output buffer, in place (see the header)
 constexpr int VM_GRPO_LIN = 13, VM_RLOO_LIN = 14;
+// PPO / A2C on one chunk, in place: VM_PPO_LIN + PPO_ENT / PPO_KL = 16..19, VM_A2C_LIN = 20 (see the header)
+constexpr int VM_PPO_LIN = 16, VM_A2C_LIN = 20;
 constexpr float kL2E = 1.4426950408889634f;
 
 // 16-byte vectors of T, widened to fp32
@@ -298,7 +316,54 @@ struct VocabArgs {
     const float* lp_ref;       // GRPO: (rows)
     const float* seq;          // (2, nb): sum_s w[b, s], then the advantage of sequence b (lm_seq_kernel)
     long long row0, nb;
+    // VM_PPO_LIN / VM_A2C_LIN: the loss mix, i.e. the fixed upstream gradients of the entropy, kl and value terms (lp_ref
+    // is then logp_pretrained; adv, value, ret and grad_value start at the chunk's first row)
+    float w_ent, w_kl, w_val;
 };
+
+// The per-token PPO head of VM_PPO / VM_PPO_LIN (ppo.py:186-230, in its operation order): adds the five loss partials
+// (policy, entropy, kl, approx_kl, clipfrac) to part and returns the unit coefficients d policy_loss / d lp_new and
+// d kl_term / d lp_new (before the 1 / M of the mean)
+struct PPOHead {
+    float cp, dk;
+};
+
+template <bool KL>
+__device__ __forceinline__ PPOHead ppo_head(const VocabArgs& a, float lp_new, float lp_old, float lp_pre, float adv,
+                                            float w, float H, float* part) {
+    PPOHead h;
+    const float ratio = expf(lp_new - lp_old);
+    float dsel, klv = 0.f;
+    h.dk = 0.f;
+    float sel = surrogate(ratio, adv, a.lo, a.hi, a.dual_clip, dsel);
+    if (ratio * adv != ratio * adv) sel = __int_as_float(0x7fc00000);  // torch.min / max propagate NaN
+    h.cp = -w * a.inv_m * dsel * ratio;  // d policy_loss / d lp_new
+    if (KL) klv = kl_term(lp_new - lp_pre, a.kl_type, h.dk);
+    part[0] -= sel * w;
+    part[1] += H * w;
+    part[2] += klv;
+    part[3] += lp_old - lp_new;
+    part[4] += (ratio > a.hi || ratio < a.lo) ? 1.f : 0.f;
+    return h;
+}
+
+// The per-token A2C head of VM_A2C / VM_A2C_LIN (a2c.py:39-44, in its operation order): adds the three loss partials
+// (policy, value, entropy) to part and returns d policy_loss / d lp and d value_loss / d value
+struct A2CHead {
+    float cp, dvu;
+};
+
+__device__ __forceinline__ A2CHead a2c_head(const VocabArgs& a, float lp, float adv, float ret, float value, float w,
+                                            float H, float* part) {
+    A2CHead h;
+    const float dv = ret - value;
+    h.cp = -adv * w * a.inv_m;
+    h.dvu = -2.f * w * dv * a.inv_m;
+    part[0] -= lp * adv * w;
+    part[1] += dv * dv * w;
+    part[2] += H * w;
+    return h;
+}
 
 // INPL: stream 0 is the buffer the kernel overwrites with its gradient -- coherent loads, not the read-only path
 template <int NR, bool CACHE, class T, bool ENT = false, bool INPL = false>
@@ -325,12 +390,15 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
     constexpr int W = V_::W;
     constexpr bool PPO = MODE >= VM_PPO && MODE < VM_PPO_BWD, PBWD = MODE >= VM_PPO_BWD && MODE < VM_A2C;
     constexpr bool A2C = MODE == VM_A2C, VAL = A2C || (PBWD && (MODE & PPO_VAL));  // VAL: the A2C value slot
-    constexpr bool ENT = ((PPO || PBWD) && (MODE & PPO_ENT)) || A2C, KL = PPO && (MODE & PPO_KL);
+    constexpr bool PLIN = MODE >= VM_PPO_LIN && MODE < VM_A2C_LIN, ALIN = MODE == VM_A2C_LIN;
+    constexpr bool ENT = ((PPO || PBWD || PLIN) && (MODE & PPO_ENT)) || A2C || ALIN;
+    constexpr bool KL = (PPO || PLIN) && (MODE & PPO_KL);
     constexpr bool BWD = MODE == VM_BWD || PBWD;
-    constexpr bool LIN = MODE == VM_GRPO_LIN || MODE == VM_RLOO_LIN;  // one in-place stream (NR = 1)
+    constexpr bool LIN = MODE == VM_GRPO_LIN || MODE == VM_RLOO_LIN;
+    constexpr bool INPL = LIN || PLIN || ALIN;  // one in-place stream (NR = 1)
     constexpr int NR = MODE == VM_GRPO ? 3 : (MODE == VM_RLOO ? 2 : (PPO ? (KL ? 3 : 2) : 1));
-    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO || A2C || LIN;
-    constexpr int NP = PPO ? 5 : 3;
+    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO || A2C || INPL;
+    constexpr int NP = (PPO || PLIN) ? 5 : 3;
     extern __shared__ uint4 s_row[];
     __shared__ float s_m[NR][VOCAB_NT / 32], s_s[NR][VOCAB_NT / 32], s_w[VOCAB_NT / 32];
     __shared__ float s_c, s_lse;
@@ -400,16 +468,16 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
             int i = tid;
             for (; i + VOCAB_NT < nvec; i += 2 * VOCAB_NT) {
                 if (cache) {
-                    stream_vecs<NR, true, T, ENT, LIN>(vp, i, m, s, s_row, a.capv, &t);
-                    stream_vecs<NR, true, T, ENT, LIN>(vp, i + VOCAB_NT, m, s, s_row, a.capv, &t);
+                    stream_vecs<NR, true, T, ENT, INPL>(vp, i, m, s, s_row, a.capv, &t);
+                    stream_vecs<NR, true, T, ENT, INPL>(vp, i + VOCAB_NT, m, s, s_row, a.capv, &t);
                 } else {
-                    stream_vecs<NR, false, T, ENT, LIN>(vp, i, m, s, s_row, 0, &t);
-                    stream_vecs<NR, false, T, ENT, LIN>(vp, i + VOCAB_NT, m, s, s_row, 0, &t);
+                    stream_vecs<NR, false, T, ENT, INPL>(vp, i, m, s, s_row, 0, &t);
+                    stream_vecs<NR, false, T, ENT, INPL>(vp, i + VOCAB_NT, m, s, s_row, 0, &t);
                 }
             }
             if (i < nvec) {
-                if (cache) stream_vecs<NR, true, T, ENT, LIN>(vp, i, m, s, s_row, a.capv, &t);
-                else stream_vecs<NR, false, T, ENT, LIN>(vp, i, m, s, s_row, 0, &t);
+                if (cache) stream_vecs<NR, true, T, ENT, INPL>(vp, i, m, s, s_row, a.capv, &t);
+                else stream_vecs<NR, false, T, ENT, INPL>(vp, i, m, s, s_row, 0, &t);
             }
             // the unaligned head and tail, < 16 bytes each
             for (long long j = tid; j < h + (V - tail0); j += VOCAB_NT) {
@@ -464,51 +532,48 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
                     if (r == 0) lse = l;
                     lp[r] = ok ? V_::to_f(rp[r][act]) - l : __int_as_float(0x7fc00000);
                 }
-                a.lse[row] = lse;
+                if (!PLIN && !ALIN) a.lse[row] = lse;  // the PPO / A2C chunks keep nothing per row
                 if (MODE == VM_LOGP) a.lp[row] = lp[0];
                 if constexpr (PPO) {
                     const float w = a.weight ? a.weight[row] : 1.f;
-                    const float ratio = expf(lp[0] - lp[1]);
-                    float dsel, dk = 0.f, klv = 0.f;
-                    const float adv = a.adv[row];
-                    float sel = surrogate(ratio, adv, a.lo, a.hi, a.dual_clip, dsel);
-                    if (ratio * adv != ratio * adv) sel = __int_as_float(0x7fc00000);  // torch.min / max propagate NaN
-                    const float cp = -w * a.inv_m * dsel * ratio;  // d policy_loss / d lp_new
-                    a.coef[row] = cp;
-                    if (KL) {
-                        klv = kl_term(lp[0] - lp[NR - 1], a.kl_type, dk);
-                        a.coef_kl[row] = dk * a.inv_m;  // d kl_div / d lp_new
-                    }
+                    const PPOHead ph = ppo_head<KL>(a, lp[0], lp[1], lp[NR - 1], a.adv[row], w, H, part);
+                    a.coef[row] = ph.cp;
+                    if (KL) a.coef_kl[row] = ph.dk * a.inv_m;  // d kl_div / d lp_new
                     if (ENT) a.ent[row] = H;
                     if (want_grad) {
-                        c = upstream_value(a.rec, owned, 0) * cp +
-                            (KL ? upstream_value(a.rec, owned, 3) * dk * a.inv_m : 0.f);
+                        c = upstream_value(a.rec, owned, 0) * ph.cp +
+                            (KL ? upstream_value(a.rec, owned, 3) * ph.dk * a.inv_m : 0.f);
                         ce = upstream_value(a.rec, owned, 2) * w * a.inv_m;
                     }
-                    part[0] -= sel * w;
-                    part[1] += H * w;
-                    part[2] += klv;
-                    part[3] += lp[1] - lp[0];
-                    part[4] += (ratio > a.hi || ratio < a.lo) ? 1.f : 0.f;
                     s_ce = ce;
                     s_h = H;
-                } else if constexpr (A2C) {  // a2c.py:39-44, in its operation order
+                } else if constexpr (PLIN) {  // VM_PPO's head, old / pretrained terms read per token, mix (1, w_ent, w_kl)
                     const float w = a.weight ? a.weight[row] : 1.f;
-                    const float adv = a.adv[row];
-                    const float dv = a.ret[row] - a.value[row];
-                    const float cp = -adv * w * a.inv_m;            // d policy_loss / d lp
-                    const float dvu = -2.f * w * dv * a.inv_m;      // d value_loss / d value
-                    a.coef[row] = cp;
-                    a.dval[row] = dvu;
+                    const PPOHead ph = ppo_head<KL>(a, lp[0], a.lp_old[row], KL ? a.lp_ref[row] : 0.f, a.adv[row], w, H,
+                                                    part);
+                    c = ph.cp + (KL ? a.w_kl * ph.dk * a.inv_m : 0.f);
+                    ce = a.w_ent * w * a.inv_m;
+                    s_ce = ce;
+                    s_h = H;
+                } else if constexpr (A2C) {
+                    const float w = a.weight ? a.weight[row] : 1.f;
+                    const A2CHead ah = a2c_head(a, lp[0], a.adv[row], a.ret[row], a.value[row], w, H, part);
+                    a.coef[row] = ah.cp;
+                    a.dval[row] = ah.dvu;
                     a.ent[row] = H;
                     if (want_grad) {
-                        c = upstream_value(a.rec, owned, 0) * cp;
+                        c = upstream_value(a.rec, owned, 0) * ah.cp;
                         ce = upstream_value(a.rec, owned, 2) * w * a.inv_m;
-                        a.grad_value[row] = upstream_value(a.rec, owned, 1) * dvu;
+                        a.grad_value[row] = upstream_value(a.rec, owned, 1) * ah.dvu;
                     }
-                    part[0] -= lp[0] * adv * w;
-                    part[1] += dv * dv * w;
-                    part[2] += H * w;
+                    s_ce = ce;
+                    s_h = H;
+                } else if constexpr (ALIN) {  // VM_A2C's head, mix (1, w_val, w_ent)
+                    const float w = a.weight ? a.weight[row] : 1.f;
+                    const A2CHead ah = a2c_head(a, lp[0], a.adv[row], a.ret[row], a.value[row], w, H, part);
+                    c = ah.cp;
+                    ce = a.w_ent * w * a.inv_m;
+                    if (a.grad_value) a.grad_value[row] = a.w_val * ah.dvu;
                     s_ce = ce;
                     s_h = H;
                 } else if constexpr (LIN) {  // the token head with the old / ref terms read per token
@@ -557,7 +622,7 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
         uint4* gv = reinterpret_cast<uint4*>(gr + h);
         for (int i = tid; i < nvec; i += VOCAB_NT) {
             const uint4 u = (LOSS && i < a.capv) ? s_row[i]
-                                                 : (BWD ? __ldcs(vp[0] + i) : (LIN ? __ldca(vp[0] + i) : __ldg(vp[0] + i)));
+                                                 : (BWD ? __ldcs(vp[0] + i) : (INPL ? __ldca(vp[0] + i) : __ldg(vp[0] + i)));
             float x[W];
             V_::unpack(u, x);
             const long long e0 = h + (long long)i * W;
@@ -587,7 +652,7 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
     if (LOSS) {
         float v[NP] = {0.f, 0.f, 0.f};
         if (tid == 0) v[0] = part[0], v[1] = part[1], v[2] = part[2];
-        if constexpr (PPO) {
+        if constexpr (PPO || PLIN) {
             if (tid == 0) v[3] = part[3], v[4] = part[4];
         }
         grid_store_partials<NP, VOCAB_NT>(v, a.ws);
@@ -728,12 +793,15 @@ bool sizes_ok(long long B, long long S, long long V) {
     return B > 0 && S > 0 && V > 0 && V < (1ll << 31) && B * S < (1ll << 40);
 }
 
-// One chunk of VM_GRPO_LIN / VM_RLOO_LIN.  Every chunk of a call launches the same grid (the plan's chunk_rows, not this
-// chunk's rows, caps it), so chunk c's CTAs own partial rows [c * grid, (c + 1) * grid); CTAs past the last chunk's rows
-// store zeros.  The last chunk adds all n_chunks * grid rows.
+// One chunk of VM_GRPO_LIN / VM_RLOO_LIN / VM_PPO_LIN / VM_A2C_LIN.  Every chunk of a call launches the same grid (the
+// plan's chunk_rows, not this chunk's rows, caps it), so chunk c's CTAs own partial rows [c * grid, (c + 1) * grid);
+// CTAs past the last chunk's rows store zeros.  The last chunk adds all n_chunks * grid rows: GRPO / RLOO's loss over B
+// sequences and approx_kl / clipfrac over N tokens, PPO / A2C's NP sums all over N tokens.
 template <class T, int MODE>
-int launch_lin(VocabArgs& a, long long chunk_rows, long long B, float* out3, size_t ws_bytes, cudaStream_t st) {
+int launch_lin(VocabArgs& a, long long chunk_rows, long long B, float* out, size_t ws_bytes, cudaStream_t st) {
     constexpr auto kern = vocab_rows_kernel<T, MODE>;
+    constexpr bool PG = MODE >= VM_PPO_LIN;
+    constexpr int NP = (MODE >= VM_PPO_LIN && MODE < VM_A2C_LIN) ? 5 : 3;
     const long long nvec_max = (a.V * (long long)sizeof(T) + 15) / 16;
     a.capv = a.grad ? (int)min(nvec_max, (long long)(VOCAB_SMEM_CAP / 16)) : 0;
     const size_t smem = (size_t)a.capv * 16;
@@ -741,17 +809,28 @@ int launch_lin(VocabArgs& a, long long chunk_rows, long long B, float* out3, siz
     if (int rc = resident_ctas<kern>(VOCAB_NT, smem, sms, per_sm)) return rc;
     const long long grid = min((long long)sms * per_sm, chunk_rows);
     const long long N = B * a.S, n_chunks = (N + chunk_rows - 1) / chunk_rows, chunk = a.row0 / chunk_rows;
-    if (!ws_partials_fit(n_chunks * grid * 3, ws_bytes)) return B200RL_ERR_WORKSPACE;
+    if (!ws_partials_fit(n_chunks * grid * NP, ws_bytes)) return B200RL_ERR_WORKSPACE;
     float* ws = a.ws;
-    a.ws = ws + chunk * grid * 3;
+    a.ws = ws + chunk * grid * NP;
     if (int rc = launch_k(kern, (int)grid, VOCAB_NT, smem, st, a)) return rc;
     if (a.row0 + a.rows < N) return B200RL_OK;
     FinalizeArgs fa{};
-    fa.scale[0] = 1.0 / (double)B;
-    fa.scale[1] = fa.scale[2] = 1.0 / (double)N;
-    fa.k = 3;
+    if (PG) {
+        for (int k = 0; k < NP; ++k) fa.scale[k] = 1.0 / (double)N;
+    } else {
+        fa.scale[0] = 1.0 / (double)B;
+        fa.scale[1] = fa.scale[2] = 1.0 / (double)N;
+    }
+    fa.k = NP;
     fa.n_blocks = (int)(n_chunks * grid);
-    return launch_finalize(ws, out3, fa, st);
+    return launch_finalize(ws, out, fa, st);
+}
+
+template <int MODE>
+int launch_lin_dtype(int dtype, VocabArgs& a, long long chunk_rows, long long B, float* out, size_t ws_bytes,
+                     cudaStream_t st) {
+    if (dtype == B200RL_DTYPE_F32) return launch_lin<float, MODE>(a, chunk_rows, B, out, ws_bytes, st);
+    return launch_lin<__nv_bfloat16, MODE>(a, chunk_rows, B, out, ws_bytes, st);
 }
 
 }  // namespace
@@ -987,6 +1066,48 @@ extern "C" int b200rl_lm_linear_fwd(int mode, int dtype, void* logits, long long
                     : launch_lin<float, VM_RLOO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st);
     return grpo ? launch_lin<__nv_bfloat16, VM_GRPO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st)
                 : launch_lin<__nv_bfloat16, VM_RLOO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st);
+}
+
+// PPO / A2C from the lm_head's hidden states, one chunk of token rows per call (ding/rl_utils/ppo.py:143-230 with
+// calculate_kl_div :30-54, and a2c.py:10-44, on logits = hidden @ lm_weight^T that the caller computes chunk by chunk; the
+// logit_old / logit_pretrained streams of b200rl_ppo_lm_fwd_grad become the per-token logp_old / logp_pre)
+extern "C" int b200rl_lm_linear_pg_fwd(int mode, int dtype, void* logits, long long row0, long long rows,
+                                       long long chunk_rows, long long V, long long N, const long long* action,
+                                       const float* logp_old, const float* logp_pre, const float* adv,
+                                       const float* value, const float* return_, const float* weight, double clip_ratio,
+                                       double dual_clip, int kl_type, int entropy, double w_ent, double w_kl,
+                                       double w_val, float* dvalue, float* out, int want_grad, float* workspace,
+                                       size_t workspace_bytes, void* stream) {
+    const bool ppo = mode == B200RL_LM_PPO, kl = logp_pre != nullptr;
+    if (!sizes_ok(N, 1, V) || rows < 1 || chunk_rows < rows || row0 < 0 || row0 % chunk_rows || row0 + rows > N ||
+        !aligned_logits(logits) || !action || !adv || !out || !workspace ||
+        (dtype != B200RL_DTYPE_F32 && dtype != B200RL_DTYPE_BF16) || (!ppo && mode != B200RL_LM_A2C))
+        return B200RL_ERR_ARG;
+    if (ppo ? (!logp_old || (kl && (kl_type < 1 || kl_type > 3)) || (!kl && w_kl != 0.0) || (!entropy && w_ent != 0.0) ||
+               dvalue || w_val != 0.0)
+            : (!value || !return_ || logp_old || kl || w_kl != 0.0))
+        return B200RL_ERR_ARG;
+    VocabArgs a{};
+    a.x[0] = logits; a.grad = want_grad ? logits : nullptr;
+    a.action = action + row0; a.adv = adv + row0; a.weight = weight ? weight + row0 : nullptr;
+    a.lp_old = ppo ? logp_old + row0 : nullptr; a.lp_ref = kl ? logp_pre + row0 : nullptr;
+    a.value = ppo ? nullptr : value + row0; a.ret = ppo ? nullptr : return_ + row0;
+    a.grad_value = dvalue ? dvalue + row0 : nullptr;
+    a.ws = workspace; a.row0 = row0;
+    a.rows = rows; a.S = 1; a.V = V;
+    a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio); a.dual_clip = (float)dual_clip;
+    a.kl_type = kl_type; a.inv_m = (float)(1.0 / (double)N);
+    a.w_ent = (float)w_ent; a.w_kl = (float)w_kl; a.w_val = (float)w_val;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!ppo) return launch_lin_dtype<VM_A2C_LIN>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
+    switch (VM_PPO_LIN + (entropy ? PPO_ENT : 0) + (kl ? PPO_KL : 0)) {
+        case VM_PPO_LIN: return launch_lin_dtype<VM_PPO_LIN>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
+        case VM_PPO_LIN + PPO_ENT:
+            return launch_lin_dtype<VM_PPO_LIN + PPO_ENT>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
+        case VM_PPO_LIN + PPO_KL:
+            return launch_lin_dtype<VM_PPO_LIN + PPO_KL>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
+        default: return launch_lin_dtype<VM_PPO_LIN + PPO_ENT + PPO_KL>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
+    }
 }
 
 // The backward of token_logp_linear on one chunk, in place (log_prob_utils.py:29-48's autograd, as b200rl_token_logp_bwd)

@@ -2086,7 +2086,7 @@ def token_head_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
 # (3.39 GB: the fp32 dW accumulator and the rounded dW, which coexist after the last chunk, outweigh the chunk).
 # Module-level so that a test can shrink it to force many chunks.
 LM_CHUNK_BYTES = 1 << 30
-_LM_MODE = {'grpo': 0, 'rloo': 1, 'logp': 2}  # B200RL_LM_GRPO, B200RL_LM_RLOO, B200RL_LM_LOGP
+_LM_MODE = {'grpo': 0, 'rloo': 1, 'logp': 2, 'ppo': 3, 'a2c': 4}  # B200RL_LM_GRPO .. B200RL_LM_A2C
 _VOCAB_CTAS_PER_SM = 4  # vocab_rows_kernel: 512 threads, at most 2048 resident per SM
 _WS_PARTIAL_WORDS = 256000 - 16  # WS_PARTIAL_LIMIT_WORDS - WS_CTRL_WORDS (csrc/common.cuh)
 
@@ -2095,14 +2095,14 @@ def sm_count(device):
     return torch.cuda.get_device_properties(device).multi_processor_count
 
 
-def lm_chunk_plan(N, V, itemsize, sms, loss):
+def lm_chunk_plan(N, V, itemsize, sms, loss, sums=3):
     """(rows per chunk, chunks) for N token rows of V logits of ``itemsize`` bytes: the largest multiple of 128 rows whose
-    logits fit in LM_CHUNK_BYTES (at least 128), or all N rows when there are fewer.  A loss call stores 3 partial sums
-    per CTA per chunk (at most sms * 4 CTAs, and no more than the chunk's rows); raises before any launch when they would
-    not fit in the workspace."""
+    logits fit in LM_CHUNK_BYTES (at least 128), or all N rows when there are fewer.  A loss call stores ``sums`` partial
+    sums (GRPO / RLOO / A2C 3, PPO 5) per CTA per chunk (at most sms * 4 CTAs, and no more than the chunk's rows); raises
+    before any launch when they would not fit in the workspace."""
     rows = min(N, max(128, LM_CHUNK_BYTES // (V * itemsize) // 128 * 128))
     n = -(-N // rows)
-    if loss and n * min(rows, sms * _VOCAB_CTAS_PER_SM) * 3 > _WS_PARTIAL_WORDS:
+    if loss and n * min(rows, sms * _VOCAB_CTAS_PER_SM) * sums > _WS_PARTIAL_WORDS:
         raise ValueError("di_engine_b200: %d token rows in %d chunks of %d need more loss partials than the workspace "
                          "holds; raise ops.LM_CHUNK_BYTES" % (N, n, rows))
     return rows, n
@@ -2121,45 +2121,92 @@ def _dw_out(acc, dtype):
     return acc if acc is None or acc.dtype == dtype else acc.to(dtype)
 
 
+def lm_chunks_(hidden, lm_weight, rows, n, launch, want_dh, want_dw):
+    """The chunk loop of every hidden-state loss: hidden (N, D) and lm_weight (V, D), both contiguous and of one dtype,
+    in ``n`` chunks of ``rows`` token rows through one (rows, V) buffer z.  Per chunk: the logit GEMM z = H[chunk] W^T,
+    ``launch(z, r0)`` (the row launch, which overwrites z in place with d loss / d logits when a gradient is wanted), then
+    dH[chunk] = z W only if ``want_dh`` and dW += z^T H[chunk] (fp32) only if ``want_dw``.  -> (dH or None, dW rounded
+    once to the weight's dtype, or None)."""
+    N, D = hidden.shape
+    V = lm_weight.shape[0]
+    dev = hidden.device
+    z = torch.empty(rows, V, dtype=hidden.dtype, device=dev)
+    dh = torch.empty_like(hidden) if want_dh else None
+    acc = torch.zeros(V, D, dtype=torch.float32, device=dev) if want_dw else None
+    wt = lm_weight.t()
+    for c in range(n):
+        r0 = c * rows
+        zc, hc = z[:min(rows, N - r0)], hidden[r0:r0 + rows]
+        torch.mm(hc, wt, out=zc)
+        launch(zc, r0)
+        if want_dh:
+            torch.mm(zc, lm_weight, out=dh[r0:r0 + rows])
+        if want_dw:
+            _acc_dw(acc, zc, hc)
+    del z, zc
+    return dh, _dw_out(acc, hidden.dtype)
+
+
 def lm_linear_loss_(hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt, clip_ratio, beta, want_dh,
                     want_dw):
     """GRPO (``kind`` 'grpo', side = adv (B)) or RLOO ('rloo', side = reward (K, B / K)) on hidden (N = B*S, D) and
-    lm_weight (V, D), both contiguous and of one dtype; action, lp_old, lp_ref (N), weight (N) or None.  Per chunk: the
-    logit GEMM, the row launch (which overwrites the chunk with d loss / d logits for a unit upstream gradient when a
-    gradient is wanted), then dH[chunk] = dZ W and dW += dZ^T H[chunk].  -> (out3 = loss / approx_kl / clipfrac, dH or
-    None, dW or None)."""
-    N, D = hidden.shape
+    lm_weight (V, D), both contiguous and of one dtype; action, lp_old, lp_ref (N), weight (N) or None.  ``lm_chunks_``
+    with the GRPO / RLOO row launch.  -> (out3 = loss / approx_kl / clipfrac, dH or None, dW or None)."""
+    N = hidden.shape[0]
     V = lm_weight.shape[0]
     dev = hidden.device
     rows, n = lm_chunk_plan(N, V, hidden.element_size(), sm_count(dev), True)
     want = want_dh or want_dw
     grpo = kind == 'grpo'
-    z = torch.empty(rows, V, dtype=hidden.dtype, device=dev)
-    dh = torch.empty_like(hidden) if want_dh else None
-    acc = torch.zeros(V, D, dtype=torch.float32, device=dev) if want_dw else None
     out = torch.empty(3, dtype=torch.float32, device=dev)
     lse = torch.empty(N, dtype=torch.float32, device=dev)
     seq = torch.empty(2 * B, dtype=torch.float32, device=dev)
-    wt = lm_weight.t()
     with on_device(dev):
         ws = workspace(dev)
         L, st = lib(), stream_ptr()
-        for c in range(n):
-            r0 = c * rows
-            zc, hc = z[:min(rows, N - r0)], hidden[r0:r0 + rows]
-            torch.mm(hc, wt, out=zc)
+
+        def launch(zc, r0):
             rc = L.b200rl_lm_linear_fwd(_LM_MODE[kind], dt, ptr(zc), r0, zc.shape[0], rows, V, B, S, ptr(action),
                                         ptr(lp_old), ptr(lp_ref), ptr(side) if grpo else None,
                                         None if grpo else ptr(side), 0 if grpo else side.shape[0], ptr(weight), ptr(seq),
                                         clip_ratio, beta, None, ptr(lse), ptr(out), 1 if want else 0, ptr(ws),
                                         ws.numel() * 4, st)
             _lib.check(rc, 'b200rl_lm_linear_fwd')
-            if want_dh:
-                torch.mm(zc, lm_weight, out=dh[r0:r0 + rows])
-            if want_dw:
-                _acc_dw(acc, zc, hc)
-    del z, zc
-    return out, dh, _dw_out(acc, hidden.dtype)
+
+        dh, dw = lm_chunks_(hidden, lm_weight, rows, n, launch, want_dh, want_dw)
+    return out, dh, dw
+
+
+def lm_linear_pg_(hidden, lm_weight, action, adv, weight, lp_old, lp_pre, value, ret, kind, dt, cfg, want_dh, want_dw,
+                  want_dv):
+    """PPO (``kind`` 'ppo': lp_old (N), lp_pre (N) or None) or A2C ('a2c': value, ret (N)) on hidden (N = B*S, D) and
+    lm_weight (V, D), both contiguous and of one dtype; action, adv (N), weight (N) or None.  cfg = (clip_ratio,
+    dual_clip (0 = off), kl_type, entropy, w_ent, w_kl, w_val): the loss is policy + w_val * value + w_ent * entropy +
+    w_kl * kl.  ``lm_chunks_`` with the PPO / A2C row launch, whose forward-written gradients are for a unit upstream
+    gradient of that loss.  -> (out: PPO's five sums policy / entropy / kl / approx_kl / clipfrac, A2C's three policy /
+    value / entropy; dH or None; dW or None; d value (N) fp32 or None)."""
+    N = hidden.shape[0]
+    V = lm_weight.shape[0]
+    dev = hidden.device
+    ppo = kind == 'ppo'
+    rows, n = lm_chunk_plan(N, V, hidden.element_size(), sm_count(dev), True, 5 if ppo else 3)
+    want = want_dh or want_dw
+    clip_ratio, dual_clip, kl_type, entropy, w_ent, w_kl, w_val = cfg
+    out = torch.empty(5 if ppo else 3, dtype=torch.float32, device=dev)
+    dv = torch.empty(N, dtype=torch.float32, device=dev) if want_dv else None
+    with on_device(dev):
+        ws = workspace(dev)
+        L, st = lib(), stream_ptr()
+
+        def launch(zc, r0):
+            rc = L.b200rl_lm_linear_pg_fwd(_LM_MODE[kind], dt, ptr(zc), r0, zc.shape[0], rows, V, N, ptr(action),
+                                           ptr(lp_old), ptr(lp_pre), ptr(adv), ptr(value), ptr(ret), ptr(weight),
+                                           clip_ratio, dual_clip, kl_type, 1 if entropy else 0, w_ent, w_kl, w_val,
+                                           ptr(dv), ptr(out), 1 if want else 0, ptr(ws), ws.numel() * 4, st)
+            _lib.check(rc, 'b200rl_lm_linear_pg_fwd')
+
+        dh, dw = lm_chunks_(hidden, lm_weight, rows, n, launch, want_dh, want_dw)
+    return out, dh, dw, dv
 
 
 def lm_scale_(dt, pg, x):
@@ -2168,6 +2215,19 @@ def lm_scale_(dt, pg, x):
         rc = lib().b200rl_lm_linear_scale(dt, pg, ptr(x), x.numel(), stream_ptr())
     _lib.check(rc, 'b200rl_lm_linear_scale')
     return x
+
+
+def _lm_backward(ctx, g_loss, recompute):
+    """The backward of the hidden-state losses: the gradients their forward wrote for a unit upstream gradient of the one
+    loss (``ctx.spec``; dH, dW and, for A2C, d value), scaled in place by ``g_loss`` on the device (a no-op when it is 1).
+    A repeated backward gets them from ``recompute()`` instead, since the first one handed the forward's buffers out."""
+    spec = _forward_grads(ctx)
+    grads = recompute() if spec is None else spec
+    keep, (pg, ) = _grads(g_loss)
+    for x in grads:
+        if x is not None:
+            lm_scale_(_LOGIT_DTYPES[x.dtype], pg, x)
+    return grads
 
 
 class LMLinearLossFunction(torch.autograd.Function):
@@ -2193,17 +2253,55 @@ class LMLinearLossFunction(torch.autograd.Function):
     def backward(ctx, g_loss, _g_kl, _g_cf):
         if g_loss is None:
             return (None, ) * 13
-        spec = _forward_grads(ctx)
-        if spec is None:  # a repeated backward: the first one handed out (and scaled) the forward's buffers
+
+        def recompute():
             hidden, lm_weight, *rest = ctx.saved_tensors
-            _, dh, dw = lm_linear_loss_(hidden, lm_weight, *rest, *ctx.cfg, *ctx.needs_input_grad[:2])
-        else:
-            dh, dw = spec
-        keep, (pg, ) = _grads(g_loss)
-        for x in (dh, dw):
-            if x is not None:
-                lm_scale_(ctx.cfg[3], pg, x)
-        return (dh, dw) + (None, ) * 11
+            return lm_linear_loss_(hidden, lm_weight, *rest, *ctx.cfg, *ctx.needs_input_grad[:2])[1:]
+
+        return tuple(_lm_backward(ctx, g_loss, recompute)) + (None, ) * 11
+
+
+def lm_pg_loss_(out, kind, cfg):
+    """the one loss of ``lm_linear_pg_``'s sums: PPO policy + w_ent * entropy + w_kl * kl, A2C policy + w_val * value +
+    w_ent * entropy (fp32, left to right; a zero weight adds nothing)"""
+    _, _, _, _, w_ent, w_kl, w_val = cfg
+    loss = out[0].clone()
+    for k, wk in enumerate((w_ent, w_kl) if kind == 'ppo' else (w_val, w_ent), 1):
+        if wk != 0.0:
+            loss = loss + wk * out[k]
+    return loss
+
+
+class LMLinearPGFunction(torch.autograd.Function):
+    """ppo_policy_error_linear / a2c_error_linear: outputs the one loss (policy + w_val * value + w_ent * entropy + w_kl *
+    kl; differentiable w.r.t. hidden, lm_weight and, for A2C, value) and the raw result vector (non differentiable: PPO's
+    policy / entropy / kl / approx_kl / clipfrac, A2C's policy / value / entropy).  The forward also writes dH, dW and
+    d value for a unit upstream gradient of the loss, each only if its input requires grad; ``backward`` is
+    ``LMLinearLossFunction``'s: scaled in place, recomputed on a repeated backward."""
+
+    @staticmethod
+    def forward(ctx, hidden, lm_weight, value, action, adv, weight, lp_old, lp_pre, ret, kind, dt, cfg):
+        want = ctx.needs_input_grad[:3]
+        out, dh, dw, dv = lm_linear_pg_(hidden, lm_weight, action, adv, weight, lp_old, lp_pre, value, ret, kind, dt,
+                                        cfg, *want)
+        ctx.save_for_backward(hidden, lm_weight, value, action, adv, weight, lp_old, lp_pre, ret)
+        ctx.cfg = (kind, dt, cfg)
+        ctx.spec = (dh, dw, dv)
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(out)
+        return lm_pg_loss_(out, kind, cfg), out
+
+    @staticmethod
+    def backward(ctx, g_loss, _g_out):
+        if g_loss is None:
+            return (None, ) * 12
+
+        def recompute():
+            hidden, lm_weight, value, action, adv, weight, lp_old, lp_pre, ret = ctx.saved_tensors
+            return lm_linear_pg_(hidden, lm_weight, action, adv, weight, lp_old, lp_pre, value, ret, *ctx.cfg,
+                                 *ctx.needs_input_grad[:3])[1:]
+
+        return tuple(_lm_backward(ctx, g_loss, recompute)) + (None, ) * 9
 
 
 def lm_logp_fwd_(hidden, lm_weight, index, dt):
@@ -2212,48 +2310,36 @@ def lm_logp_fwd_(hidden, lm_weight, index, dt):
     V = lm_weight.shape[0]
     dev = hidden.device
     rows, n = lm_chunk_plan(N, V, hidden.element_size(), sm_count(dev), False)
-    z = torch.empty(rows, V, dtype=hidden.dtype, device=dev)
     lp = torch.empty(N, dtype=torch.float32, device=dev)
     lse = torch.empty(N, dtype=torch.float32, device=dev)
-    wt = lm_weight.t()
     with on_device(dev):
         L, st = lib(), stream_ptr()
-        for c in range(n):
-            r0 = c * rows
-            zc = z[:min(rows, N - r0)]
-            torch.mm(hidden[r0:r0 + rows], wt, out=zc)
+
+        def launch(zc, r0):
             rc = L.b200rl_lm_linear_fwd(_LM_MODE['logp'], dt, ptr(zc), r0, zc.shape[0], rows, V, N, 1, ptr(index), None,
                                         None, None, None, 0, None, None, 0.0, 0.0, ptr(lp), ptr(lse), None, 0, None, 0,
                                         st)
             _lib.check(rc, 'b200rl_lm_linear_fwd')
+
+        lm_chunks_(hidden, lm_weight, rows, n, launch, False, False)
     return lp, lse
 
 
 def lm_logp_bwd_(hidden, lm_weight, index, lse, g, dt, want_dh, want_dw):
     """The backward of ``lm_logp_fwd_`` for the upstream gradient g (N) fp32: per chunk the logit GEMM again, the in-place
     launch dZ = g * (onehot(index) - softmax(Z)), then the gradient GEMMs.  -> (dH or None, dW or None)"""
-    N, D = hidden.shape
+    N = hidden.shape[0]
     V = lm_weight.shape[0]
     dev = hidden.device
     rows, n = lm_chunk_plan(N, V, hidden.element_size(), sm_count(dev), False)
-    z = torch.empty(rows, V, dtype=hidden.dtype, device=dev)
-    dh = torch.empty_like(hidden) if want_dh else None
-    acc = torch.zeros(V, D, dtype=torch.float32, device=dev) if want_dw else None
-    wt = lm_weight.t()
     with on_device(dev):
         L, st = lib(), stream_ptr()
-        for c in range(n):
-            r0 = c * rows
-            zc, hc = z[:min(rows, N - r0)], hidden[r0:r0 + rows]
-            torch.mm(hc, wt, out=zc)
+
+        def launch(zc, r0):
             rc = L.b200rl_lm_linear_bwd(dt, ptr(zc), r0, zc.shape[0], V, ptr(index), ptr(lse), ptr(g), st)
             _lib.check(rc, 'b200rl_lm_linear_bwd')
-            if want_dh:
-                torch.mm(zc, lm_weight, out=dh[r0:r0 + rows])
-            if want_dw:
-                _acc_dw(acc, zc, hc)
-    del z, zc
-    return dh, _dw_out(acc, hidden.dtype)
+
+        return lm_chunks_(hidden, lm_weight, rows, n, launch, want_dh, want_dw)
 
 
 class TokenLogpLinearFunction(torch.autograd.Function):

@@ -9,8 +9,9 @@ from .happo import (happo_data, happo_error, happo_error_continuous, happo_polic
 from .grpo import grpo_info, grpo_policy_data, grpo_policy_error
 from .log_prob_utils import efficient_method, less_efficient_method, naive_method
 # composites from the lm_head's hidden states (not reference names: outside the hot-path lists below)
-from .lm_linear import (grpo_linear_data, grpo_policy_error_linear, rloo_linear_data, rloo_policy_error_linear,
-                        token_logp_linear)
+from .lm_linear import (a2c_error_linear, a2c_linear_data, a2c_linear_loss, grpo_linear_data, grpo_policy_error_linear,
+                        ppo_linear_loss, ppo_policy_error_linear, ppo_policy_linear_data, rloo_linear_data,
+                        rloo_policy_error_linear, token_logp_linear)
 from .gae import gae, gae_data, gae_returns, gae_returns_out, ppof_gae_returns, ppof_gae_returns_out, shape_fn_gae
 from .ppo import (normalize_advantage, ppo_data, ppo_data_continuous, ppo_error, ppo_error_adv_norm, ppo_error_continuous, ppo_info, ppo_loss,
                   ppo_policy_data, ppo_policy_data_continuous, ppo_policy_error, ppo_policy_error_continuous, ppo_policy_loss,

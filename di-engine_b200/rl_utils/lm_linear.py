@@ -15,10 +15,27 @@ These are composites, not names of ding.rl_utils:
   ``F.linear(hidden, lm_weight)`` with ``logp_old = efficient_method(logit_old, action)`` and likewise for ``logp_ref``.
 - ``rloo_policy_error_linear(rloo_linear_data(...), clip_ratio)`` likewise for ``rloo_policy_error``.
 
-``weight`` is the reference's per-token mask.  ``logp_old``, ``logp_ref``, ``adv``, ``reward`` and ``weight`` of any float
-dtype are read as fp32.  Under ``torch.compile`` these functions run eagerly behind a graph break."""
+- ``ppo_policy_error_linear(ppo_policy_linear_data(...), clip_ratio, dual_clip, entropy_bonus, kl_type, entropy_weight,
+  kl_weight)`` equals ``ppo_policy_error`` on ``F.linear(hidden, lm_weight)`` with ``logp_old = efficient_method(logit_old,
+  action)`` and likewise for ``logp_pretrained``.
+- ``a2c_error_linear(a2c_linear_data(...), value_weight, entropy_weight)`` likewise for ``a2c_error``; the gradient also
+  reaches ``value``.
+
+``weight`` is the reference's per-token mask.  ``logp_old``, ``logp_ref``, ``logp_pretrained``, ``adv``, ``reward``,
+``return_``, ``value`` and ``weight`` of any float dtype are read as fp32.  Under ``torch.compile`` these functions run
+eagerly behind a graph break.
+
+PPO and A2C return their loss mix as one differentiable ``loss`` -- ``policy_loss - entropy_weight * entropy_loss +
+kl_weight * kl_div``, or ``policy_loss + value_weight * value_loss - entropy_weight * entropy_loss`` -- and the components
+as detached 0-dim tensors for logging, rather than three separately differentiable outputs.  The forward writes dH / dW
+(and A2C's d value) for a unit upstream gradient of ``loss``, and the backward scales them in place on the device; a
+repeated backward recomputes them.  Any other mix of the components would need the logits again, which are gone after
+each chunk's dW GEMM: dW = sum over chunks of dZ^T H cannot be re-weighted afterwards without one (V, D) fp32
+accumulator per component (2.2 GB each at Qwen2-7B's lm_head), or a host read of the upstream gradients (a sync in the
+backward).  So the weights of the mix are arguments.  A learner that wants ``ppo_error`` adds ``ppo_value_error`` on its
+value head's (B, S) output to this ``loss``."""
 from collections import namedtuple
-from typing import Tuple
+from typing import Optional, Tuple
 
 import torch
 
@@ -26,11 +43,17 @@ from .. import ops
 from . import _lm_policy
 from . import ppo as _ppo
 from .grpo import grpo_info
+from .ppo import ppo_info
 from .rloo import rloo_info
 
 grpo_linear_data = namedtuple('grpo_linear_data',
                               ['hidden', 'lm_weight', 'logp_old', 'logp_ref', 'action', 'adv', 'weight'])
 rloo_linear_data = namedtuple('rloo_linear_data', ['hidden', 'lm_weight', 'logp_old', 'action', 'reward', 'weight'])
+ppo_policy_linear_data = namedtuple('ppo_policy_linear_data',
+                                    ['hidden', 'lm_weight', 'logp_old', 'action', 'adv', 'weight', 'logp_pretrained'])
+ppo_linear_loss = namedtuple('ppo_linear_loss', ['loss', 'policy_loss', 'entropy_loss', 'kl_div'])
+a2c_linear_data = namedtuple('a2c_linear_data', ['hidden', 'lm_weight', 'action', 'value', 'adv', 'return_', 'weight'])
+a2c_linear_loss = namedtuple('a2c_linear_loss', ['loss', 'policy_loss', 'value_loss', 'entropy_loss'])
 
 
 def _check_linear(hidden, lm_weight):
@@ -128,6 +151,83 @@ def rloo_policy_error_linear(data: namedtuple, clip_ratio: float = 0.2) -> Tuple
                 ('reward', data.reward), clip_ratio, 0.0, rloo_info)
 
 
+def _run_pg(kind, hidden, lm_weight, action, weight, rows, value, cfg):
+    """the shared body of the PPO and A2C losses: rows = the per-token (B, S) operands by name (adv, and logp_old /
+    logp_pretrained or return_), value (B, S) (A2C, differentiable) or None.  -> (the one loss, the raw sums)"""
+    dt = _check_linear(hidden, lm_weight)
+    B, S, _ = hidden.shape
+    V = lm_weight.shape[0]
+    for name, t in [('action', action), ('weight', weight)] + list(rows.items()) + [('value', value)]:
+        if t is not None and tuple(t.shape) != (B, S):  # check_tokens' message
+            raise RuntimeError("%s must be (B, S) = %s, got %s" % (name, (B, S), tuple(t.shape)))
+    dev = ops.compute_device(hidden, lm_weight)
+    host_out = not hidden.is_cuda
+    # the per-token operands are read as fp32 whatever their dtype; value keeps its graph (autograd casts its gradient)
+    f = {k: None if t is None else ops.to_device(t.detach(), dev).float().contiguous().reshape(-1) for k, t in rows.items()}
+    w = None if weight is None else ops.to_device(weight.detach(), dev).float().contiguous().reshape(-1)
+    v = None if value is None else ops.to_device(value, dev).float().contiguous().reshape(-1)
+    a = ops.i64c(ops.to_device(action, dev), V).reshape(-1)
+    h, wt = _stage(hidden, lm_weight, dev)
+    args = (a, f['adv'], w, f.get('logp_old'), f.get('logp_pretrained'), f.get('return_'), kind, dt, cfg)
+    if torch.is_grad_enabled() and (h.requires_grad or wt.requires_grad or (v is not None and v.requires_grad)):
+        loss, out = ops.LMLinearPGFunction.apply(h, wt, v, *args)
+    else:
+        out = ops.lm_linear_pg_(h.detach(), wt.detach(), a, f['adv'], w, f.get('logp_old'), f.get('logp_pretrained'),
+                                None if v is None else v.detach(), f.get('return_'), kind, dt, cfg, False, False,
+                                False)[0]
+        loss = ops.lm_pg_loss_(out, kind, cfg)
+    if host_out:
+        loss, out = loss.cpu(), out.cpu()
+    return loss, out
+
+
+@torch.compiler.disable
+def ppo_policy_error_linear(data: namedtuple, clip_ratio: float = 0.2, dual_clip: Optional[float] = None,
+                            entropy_bonus: bool = True, kl_type: str = 'k1', entropy_weight: float = 0.0,
+                            kl_weight: float = 0.0) -> Tuple[namedtuple, namedtuple]:
+    """``ppo_policy_error`` (rl_utils/ppo.py) on logits = hidden @ lm_weight^T, computed chunk by chunk.  data =
+    ppo_policy_linear_data(hidden (B, S, D), lm_weight (V, D), logp_old (B, S), action (B, S), adv (B, S), weight (B, S)
+    or None, logp_pretrained (B, S) or None).  Returns (ppo_linear_loss(loss, policy_loss, entropy_loss, kl_div),
+    ppo_info(approx_kl, clipfrac)): ``loss = policy_loss - entropy_weight * entropy_loss + kl_weight * kl_div`` is the one
+    differentiable output (to hidden and lm_weight); the components are detached, entropy_loss 0 without
+    ``entropy_bonus`` and kl_div 0 without ``logp_pretrained``."""
+    assert dual_clip is None or dual_clip > 1.0, "dual_clip value must be greater than 1.0, but get value: {}".format(
+        dual_clip
+    )
+    hidden, lm_weight, logp_old, action, adv, weight, logp_pre = data
+    if logp_pre is not None and kl_type not in _ppo._KL_TYPES:
+        raise ValueError(f"Unknown kl_type: {kl_type}")
+    if entropy_weight != 0.0 and not entropy_bonus:
+        raise ValueError("ppo_policy_error_linear: entropy_weight %r needs entropy_bonus=True" % (entropy_weight, ))
+    if kl_weight != 0.0 and logp_pre is None:
+        raise ValueError("ppo_policy_error_linear: kl_weight %r needs logp_pretrained" % (kl_weight, ))
+    cfg = (float(clip_ratio), float(dual_clip) if dual_clip is not None else 0.0, _ppo._KL_TYPES.get(kl_type, 1),
+           bool(entropy_bonus), -float(entropy_weight), float(kl_weight), 0.0)
+    loss, out = _run_pg('ppo', hidden, lm_weight, action, weight,
+                        {'adv': adv, 'logp_old': logp_old, 'logp_pretrained': logp_pre}, None, cfg)
+    if _ppo.LAZY_INFO:
+        info = ppo_info(out[3], out[4])
+    else:
+        approx_kl, clipfrac = out[3:5].tolist()  # one host sync
+        info = ppo_info(approx_kl, clipfrac)
+    return ppo_linear_loss(loss, out[0], out[1], out[2]), info
+
+
+@torch.compiler.disable
+def a2c_error_linear(data: namedtuple, value_weight: float = 0.5, entropy_weight: float = 0.01) -> namedtuple:
+    """``a2c_error`` (rl_utils/a2c.py) on logits = hidden @ lm_weight^T, computed chunk by chunk.  data =
+    a2c_linear_data(hidden (B, S, D), lm_weight (V, D), action (B, S), value (B, S), adv (B, S), return_ (B, S), weight
+    (B, S) or None).  Returns a2c_linear_loss(loss, policy_loss, value_loss, entropy_loss): ``loss = policy_loss +
+    value_weight * value_loss - entropy_weight * entropy_loss`` is the one differentiable output (to hidden, lm_weight
+    and value); the components are detached."""
+    hidden, lm_weight, action, value, adv, return_, weight = data
+    cfg = (0.0, 0.0, 1, True, -float(entropy_weight), 0.0, float(value_weight))
+    loss, out = _run_pg('a2c', hidden, lm_weight, action, weight, {'adv': adv, 'return_': return_}, value, cfg)
+    return a2c_linear_loss(loss, out[0], out[1], out[2])
+
+
 __all__ = [
-    'grpo_linear_data', 'rloo_linear_data', 'token_logp_linear', 'grpo_policy_error_linear', 'rloo_policy_error_linear'
+    'grpo_linear_data', 'rloo_linear_data', 'token_logp_linear', 'grpo_policy_error_linear', 'rloo_policy_error_linear',
+    'ppo_policy_linear_data', 'ppo_linear_loss', 'ppo_policy_error_linear', 'a2c_linear_data', 'a2c_linear_loss',
+    'a2c_error_linear'
 ]

@@ -717,10 +717,23 @@ B200RL_API int b200rl_a2c_lm_bwd(int dtype, const void* logit, const long long* 
  * b200rl_lm_linear_bwd: logits[r] = dlogp[row0 + r] * (onehot(index) - softmax(logits[r])) in place, from the saved lse:
  *   the backward of mode B200RL_LM_LOGP on one recomputed chunk.
  * b200rl_lm_linear_scale: x (n values of dtype, 16-byte aligned) *= *g in place; returns at once on the device when
- *   *g == 1 -- the backward of the GRPO / RLOO forward's gradients. */
+ *   *g == 1 -- the backward of the GRPO / RLOO / PPO / A2C forward's gradients.
+ * b200rl_lm_linear_pg_fwd: mode B200RL_LM_PPO (ding/rl_utils/ppo.py:143-230, calculate_kl_div :30-54) or B200RL_LM_A2C
+ *   (a2c.py:10-44) on the chunk's rows of N = B*S tokens; M = N, every sum a plain mean over the N rows.  Per-token
+ *   operands (N) fp32: action, adv, weight (nullable = ones); PPO: logp_old, logp_pre (nullable = no KL term); A2C: value,
+ *   return_.  PPO: out (5) = {policy_loss, entropy_loss (0 without `entropy`), kl_div (0 without logp_pre), approx_kl,
+ *   clipfrac}, each as b200rl_ppo_lm_fwd_grad forms it (clip_ratio, dual_clip <= 0 = off, kl_type 1..3).  A2C: out (3) =
+ *   {policy_loss, value_loss, entropy_loss} as b200rl_a2c_lm_fwd_grad.  With want_grad it overwrites `logits` in place
+ *   with d loss / d logits for a unit upstream gradient of the one loss = policy_loss + w_val * value_loss +
+ *   w_ent * entropy_loss + w_kl * kl_div (w_ent != 0 requires `entropy`, w_kl != 0 requires logp_pre, w_val is A2C's):
+ *   c_act * (onehot(a) - p) - c_ent * p * (log p + H) with (g_pol, g_ent, g_kl / g_val) = (1, w_ent, w_kl / w_val) in the
+ *   formula of b200rl_ppo_lm_fwd_grad / b200rl_a2c_lm_fwd_grad.  A2C: dvalue (N, nullable = not wanted) = w_val *
+ *   d value_loss / d value at the chunk's rows.  Partials and the last chunk's finalize as b200rl_lm_linear_fwd. */
 #define B200RL_LM_GRPO 0
 #define B200RL_LM_RLOO 1
 #define B200RL_LM_LOGP 2
+#define B200RL_LM_PPO 3
+#define B200RL_LM_A2C 4
 B200RL_API int b200rl_lm_linear_fwd(int mode, int dtype, void* logits, long long row0, long long rows, long long chunk_rows,
                          long long V, long long B, long long S, const long long* action, const float* logp_old,
                          const float* logp_ref, const float* adv, const float* reward, long long K, const float* weight,
@@ -729,6 +742,12 @@ B200RL_API int b200rl_lm_linear_fwd(int mode, int dtype, void* logits, long long
 B200RL_API int b200rl_lm_linear_bwd(int dtype, void* logits, long long row0, long long rows, long long V,
                          const long long* index, const float* lse, const float* dlogp, void* stream);
 B200RL_API int b200rl_lm_linear_scale(int dtype, const float* g, void* x, long long n, void* stream);
+B200RL_API int b200rl_lm_linear_pg_fwd(int mode, int dtype, void* logits, long long row0, long long rows,
+                            long long chunk_rows, long long V, long long N, const long long* action,
+                            const float* logp_old, const float* logp_pre, const float* adv, const float* value,
+                            const float* return_, const float* weight, double clip_ratio, double dual_clip,
+                            int kl_type, int entropy, double w_ent, double w_kl, double w_val, float* dvalue, float* out,
+                            int want_grad, float* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- data-parallel exchange step: one-shot all-reduce (mean) of n <= 8 floats over NVLink peer memory -----------
  * Replaces the small-message NCCL all-reduce of the packed loss scalars (mean of rank means,
