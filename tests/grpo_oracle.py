@@ -82,17 +82,22 @@ def head64(lp_new, lp_old, lp_ref, adv, weight, clip=CLIP, beta=BETA):
     return loss, (lp_old - lp_new).mean().detach(), ((ratio > hi) | (ratio < lo)).to(tok.dtype).mean()
 
 
-def run64(d, clip=CLIP, beta=BETA, dtype=torch.float64):
+def run64(d, clip=CLIP, beta=BETA, dtype=torch.float64, lp_old=None, lp_ref=None):
     """float64 results of the case dict `d` (any device): loss, approx_kl, clipfrac, lp_new (B, S) and dlp (B, S) =
     d loss / d lp_new; d loss / d logit_new[row] = dlp[row] * (onehot - softmax) (``grad_rows64``).  ``dtype`` float32
-    restates the reference's own fp32 arithmetic on the same inputs (bf16 logits widened to fp32); 'scale' stays float64"""
+    restates the reference's own fp32 arithmetic on the same inputs (bf16 logits widened to fp32); 'scale' stays float64.
+    ``lp_old`` / ``lp_ref`` (B, S): per-token log-probabilities given instead of ``logit_old`` / ``logit_ref`` (the
+    hidden-state losses' inputs), upcast to ``dtype``"""
     B = d['logit_new'].shape[0]
     lp = {k: torch.stack([logp64(d[k][b], d['action'][b], dtype) for b in range(B)])
           for k in ('logit_new', 'logit_old', 'logit_ref') if k in d}
+    for k, t in (('logit_old', lp_old), ('logit_ref', lp_ref)):
+        if t is not None:
+            lp[k] = t.to(lp['logit_new'].device, dtype).reshape(lp['logit_new'].shape)
     lp_new = lp['logit_new'].clone().requires_grad_(True)
     adv = d['adv'] if 'adv' in d else rloo_adv64(d['reward'], dtype)
     loss, kl, cf = head64(lp_new, lp['logit_old'], lp.get('logit_ref'), adv.to(lp_new.device), d['weight'], clip,
-                          beta if 'logit_ref' in d else 0.0)
+                          beta if 'logit_ref' in lp else 0.0)
     loss.backward()
     # the size of the terms that make up dlp: gt * (|adv| * ratio [+ beta * (exp(lp_ref - lp_new) + 1)]) with
     # gt = w / (B * sum_s w).  One ulp of an fp32 logsumexp moves dlp by about that much times 2^-23 * |logsumexp|, even
@@ -102,7 +107,7 @@ def run64(d, clip=CLIP, beta=BETA, dtype=torch.float64):
     a = adv.double().to(lp_new.device).reshape(-1, 1).abs()
     lpd = {k: v.double() for k, v in lp.items()}
     scale = gt * a * torch.exp(lpd['logit_new'] - lpd['logit_old'])
-    if 'logit_ref' in d:
+    if 'logit_ref' in lp:
         scale = scale + gt * beta * (torch.exp(lpd['logit_ref'] - lpd['logit_new']) + 1)
     return {'loss': loss.item(), 'approx_kl': kl.item(), 'clipfrac': cf.item(), 'lp_new': lp['logit_new'],
             'dlp': lp_new.grad, 'scale': scale.detach()}

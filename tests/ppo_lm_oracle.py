@@ -82,17 +82,23 @@ def _normalized(x):
     return x - x.logsumexp(-1, keepdim=True)
 
 
-def run64(d, clip=CLIP, dual_clip=None, kl_type='k1', entropy_bonus=True, mix=MIX, dtype=torch.float64):
+def run64(d, clip=CLIP, dual_clip=None, kl_type='k1', entropy_bonus=True, mix=MIX, dtype=torch.float64, lp_old=None,
+          lp_pre=None):
     """float64 results of the case dict `d` (any device): policy, entropy, kl, approx_kl, clipfrac and grad = d (mix[0] *
     policy + mix[1] * entropy + mix[2] * kl) / d logit_new, and per row lse, lp_new and H (entropy_bonus).  The clamp /
     clipfrac bounds are fp32(1 -+ clip), as torch forms them for fp32 ratios; Categorical.entropy's clamp of log p at
     finfo.min makes a -inf logit contribute 0.  ``dtype`` float32 restates the reference's own fp32 arithmetic on the same
-    inputs (bf16 logits widened to fp32), the clamp at finfo(float32).min included."""
+    inputs (bf16 logits widened to fp32), the clamp at finfo(float32).min included.  ``lp_old`` / ``lp_pre`` (B, S):
+    per-token log-probabilities given instead of ``logit_old`` / ``logit_pretrained`` (the hidden-state losses' inputs),
+    upcast to ``dtype``."""
     x = d['logit_new'].detach().to(dtype, copy=True).requires_grad_(True)
     a = d['action'].unsqueeze(-1)
     lsm = _normalized(x)
     lp_new = lsm.gather(-1, a).squeeze(-1)
-    lp_old = _normalized(d['logit_old'].to(dtype)).gather(-1, a).squeeze(-1)
+    if lp_old is None:
+        lp_old = _normalized(d['logit_old'].to(dtype)).gather(-1, a).squeeze(-1)
+    else:
+        lp_old = lp_old.to(x.device, dtype).reshape(lp_new.shape)
     adv = d['adv'].to(dtype).reshape(lp_new.shape)
     w = torch.ones_like(adv) if d['weight'] is None else d['weight'].to(dtype).expand_as(adv)
     ratio = torch.exp(lp_new - lp_old)
@@ -110,8 +116,11 @@ def run64(d, clip=CLIP, dual_clip=None, kl_type='k1', entropy_bonus=True, mix=MI
         ent = (H * w).mean()
         total = total + mix[1] * ent
     kl = torch.zeros((), dtype=dtype)
-    if d['logit_pretrained'] is not None:
+    if lp_pre is not None:
+        lr = lp_new - lp_pre.to(x.device, dtype).reshape(lp_new.shape)
+    elif d.get('logit_pretrained') is not None:
         lr = lp_new - _normalized(d['logit_pretrained'].to(dtype)).gather(-1, a).squeeze(-1)
+    if lp_pre is not None or d.get('logit_pretrained') is not None:
         kl = {'k1': lr, 'k2': lr ** 2 / 2, 'k3': torch.exp(-lr) - 1 + lr}[kl_type].mean()
         total = total + mix[2] * kl
     total.backward()

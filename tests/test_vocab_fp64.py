@@ -3,7 +3,10 @@ wrong.
 
 Kernels: ``vocab_rows_kernel<T, MODE>`` for fp32 and bf16 logits -- grpo_policy_error, rloo_policy_error (forward with
 and without the cached row, VM_BWD), the three log-prob methods (VM_LOGP, VM_BWD) and language-model ppo_policy_error
-(VM_PPO + entropy / KL flags, VM_PPO_BWD) -- and ``token_head_kernel`` (a custom log_prob_fn).
+(VM_PPO + entropy / KL flags, VM_PPO_BWD), language-model a2c_error (VM_A2C, backward VM_PPO_BWD + PPO_ENT + PPO_VAL,
+on the regimes without an old policy, returns at 1e3 with a 1e-2 spread, value == return and adv = 0, each mix from the
+record with the forward's gradient buffers poisoned: a mix that differs only in the value slot keeps d logit and
+rewrites d value) -- and ``token_head_kernel`` (a custom log_prob_fn).
 
 The seeded parity cases of test_grpo_rloo.py / test_ppo_lm.py draw ``logit_old = new + 0.1 randn`` and logit scales of
 1..4: almost no ratio leaves the clip band.  Here every token row draws one regime, in equal shares: ``plain`` (those
@@ -65,11 +68,13 @@ POISON = 7.0
 # ----------------------------------------------------------------------------------------------------------------
 # the row plan of csrc/vocab.cu, and the generator
 # ----------------------------------------------------------------------------------------------------------------
-def row_layout(rows, V, esize):
+def row_layout(rows, V, esize, chunk=None):
     """per row: the unaligned head length h, the tail start tail0 and the end of the cached part (as vocab_rows_kernel
-    splits a row whose byte offset row * V * esize is not a multiple of 16)"""
+    splits a row whose byte offset row * V * esize is not a multiple of 16).  ``chunk``: the rows of one chunk buffer of the
+    hidden-state losses, whose kernel sees row r at r mod chunk"""
     W = 16 // esize
-    mis = (torch.arange(rows, dtype=torch.int64) * V * esize % 16) // esize
+    r = torch.arange(rows, dtype=torch.int64)
+    mis = ((r if chunk is None else r % chunk) * V * esize % 16) // esize
     h = torch.where(mis > 0, torch.clamp(W - mis, max=V), torch.zeros_like(mis))
     tail0 = h + (V - h) // W * W
     capv = min((V * esize + 15) // 16, CACHE_BYTES // 16)
@@ -83,9 +88,9 @@ def _pick(u, lo, hi):
                        torch.full_like(lo, -1))
 
 
-def _placements(g, rows, V, esize):
+def _placements(g, rows, V, esize, chunk=None):
     """(position class, taken-token position or -1, row-max position class, row-max position or -1)"""
-    h, tail0, cend = row_layout(rows, V, esize)
+    h, tail0, cend = row_layout(rows, V, esize, chunk)
     u = torch.rand(rows, generator=g)
     zero = torch.zeros(rows, dtype=torch.int64)
     cand = torch.stack([torch.full((rows, ), -1), zero, zero + V - 1, _pick(u, zero, h), _pick(u, tail0, zero + V),
@@ -99,8 +104,10 @@ def _placements(g, rows, V, esize):
     return cls, pos, torch.where(mpos < 0, torch.zeros_like(mcls), mcls), mpos
 
 
-def gen_rows(seed, rows, V, dtype, names=REGIMES, with_ref=True):
-    """rows token rows of V logits: new, old, ref (None without), action and meta (regime per row, placements, masks)"""
+def gen_rows(seed, rows, V, dtype, names=REGIMES, with_ref=True, mask_values=(-math.inf, -1e4), chunk=None):
+    """rows token rows of V logits: new, old, ref (None without), action and meta (regime per row, placements, masks).
+    ``mask_values``: the masked regime's (hard, soft) logit -- a finite hard one where the logits come out of a GEMM, in
+    which -inf * 0 is NaN; ``chunk``: place tokens by their row in a chunk buffer of that many rows (row_layout)"""
     g = torch.Generator().manual_seed(seed)
     esize = 4 if dtype == F32 else 2
     reg = _regimes(g, rows, names)
@@ -111,7 +118,7 @@ def gen_rows(seed, rows, V, dtype, names=REGIMES, with_ref=True):
     n_old = 0.1 * torch.randn(rows, V, generator=g)
     n_ref = 0.2 * torch.randn(rows, V, generator=g)
     action = torch.randint(0, V, (rows, ), generator=g)
-    cls, pos, mcls, mpos = _placements(g, rows, V, esize)
+    cls, pos, mcls, mpos = _placements(g, rows, V, esize, chunk)
     action = torch.where(pos >= 0, pos, action)
     r = torch.arange(rows)
     has_m = mpos >= 0
@@ -153,12 +160,13 @@ def gen_rows(seed, rows, V, dtype, names=REGIMES, with_ref=True):
     mask |= only.unsqueeze(1)
     mask &= mr.unsqueeze(1)
     mask[r, action] = False
-    mval = torch.where(only | (torch.rand(rows, generator=g) < 0.5), -math.inf, -1e4).unsqueeze(1).expand(rows, V)
+    mval = torch.where(only | (torch.rand(rows, generator=g) < 0.5), mask_values[0],
+                       mask_values[1]).unsqueeze(1).expand(rows, V)
     for x in (new, old) + ((ref, ) if ref is not None else ()):
         x[mask] = mval[mask]
     out = [x.to(dtype) for x in (new, old)] + [None if ref is None else ref.to(dtype)]
     meta = dict(regime=reg.numpy(), names=tuple(names), place=cls.numpy(), pos=pos.numpy(), mplace=mcls.numpy(),
-                mpos=mpos.numpy(), peaked_take=(pk & take).numpy(), only=only.numpy(), mask=mask, esize=esize)
+                mpos=mpos.numpy(), peaked_take=(pk & take).numpy(), only=only.numpy(), mask=mask, esize=esize, chunk=chunk)
     return out[0], out[1], out[2], action, meta
 
 
@@ -180,6 +188,18 @@ def _rewards(g, K, Bp):
     r = torch.randn(K, Bp, generator=g)
     r = torch.where(kind == 1, 1e3 + 1e-2 * r, r)
     return torch.where(kind == 2, (1e3 + 1e-2 * torch.randn(1, Bp, generator=g)).expand(K, Bp), r)
+
+
+def a2c_side(g, B, S):
+    """(adv, return_, value) (B, S): adv with 10 % exact zeros; returns N(0, 1) or 1e3 + 1e-2 N(0, 1) (cancellation in
+    return - value), value == return exactly in a fifth of the tokens"""
+    adv = torch.randn(B, S, generator=g)
+    adv[torch.rand(B, S, generator=g) < 0.1] = 0.0
+    u = torch.rand(B, S, generator=g)
+    ret = torch.where(u < 0.4, 1e3 + 1e-2 * torch.randn(B, S, generator=g), torch.randn(B, S, generator=g))
+    value = ret + torch.where(ret > 500, 1e-2, 1.0) * torch.randn(B, S, generator=g)
+    value = torch.where(torch.rand(B, S, generator=g) < 0.2, ret, value)
+    return adv, ret, value
 
 
 def gen_lm(seed, kind, B, S, V, dtype, wkind, K=0, names=None):
@@ -549,7 +569,7 @@ def test_ppo_lm_fp64(name):
     from di_engine_b200 import ops
     d, meta, p, parts = _ppo_case(name)
     bf16 = d['logit_new'].dtype == BF16
-    hint = ops.ppo_hint(torch.device(DEV), 'policy')
+    hint = ops.ppo_hint(torch.device(DEV, torch.cuda.current_device()), 'policy')  # the record the calls read
     saved_hint = hint.clone()
     worst = 0.0
     WORST.clear()
@@ -707,6 +727,159 @@ def test_token_head_fp64(S, kind):
     WORST.clear()
     worst = compare_regimes('head %s S=%d' % (kind, S), got, *refs, meta, scales, bnd)
     print('[fp64] head %s S=%d worst %.2f  per regime %s' % (kind, S, worst, _per_regime()))
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# A2C on token rows (VM_A2C, backward VM_PPO_BWD + PPO_ENT + PPO_VAL) and its upstream-gradient record
+# ----------------------------------------------------------------------------------------------------------------
+A2C_NAMES = ('plain', 'shift', 'peaked', 'flat', 'masked', 'large')  # the regimes without an old policy
+A2C_CASES = {
+    # name: (dtype, B, S, V, weight kind)
+    'a2c_f32_v1_r16384': (F32, 16, 1024, 1, 'frac'),
+    'a2c_f32_v3_r529': (F32, 23, 23, 3, None),
+    'a2c_f32_v1027_s1500': (F32, 3, 1500, 1027, 'mask'),
+    'a2c_f32_v1027_r4099_s1': (F32, 4099, 1, 1027, 'frac'),
+    'a2c_f32_v4100_r529': (F32, 23, 23, 4100, None),
+    'a2c_f32_v56320_r131': (F32, 131, 1, 56320, 'frac'),
+    'a2c_f32_v56324_r133': (F32, 1, 133, 56324, None),
+    'a2c_f32_v56333_r132_s3': (F32, 44, 3, 56333, 'mask'),
+    'a2c_f32_v152063_r3': (F32, 1, 3, 152063, 'frac'),
+    'a2c_bf16_v1_r1': (BF16, 1, 1, 1, None),
+    'a2c_bf16_v7_r4099': (BF16, 4099, 1, 7, 'mask'),
+    'a2c_bf16_v1003_r529': (BF16, 23, 23, 1003, 'frac'),
+    'a2c_bf16_v8200_r133': (BF16, 7, 19, 8200, 'mask'),
+    'a2c_bf16_v112640_r131': (BF16, 131, 1, 112640, 'frac'),
+    'a2c_bf16_v112648_r133': (BF16, 1, 133, 112648, None),
+    'a2c_bf16_v112647_r132_s3': (BF16, 44, 3, 112647, 'frac'),
+    'a2c_bf16_v152064_r3': (BF16, 3, 1, 152064, 'frac'),
+}
+A2C_RECORD = (1.0, 0.5, -0.01)  # ops._HINT_INIT['a2c']: the upstream gradients the forward writes for
+# the record; nextafter(1, 2) in the policy slot; the record but for the value slot; (0.37, -2, 0); all zeros
+A2C_MIXES = (A2C_RECORD, (NEXT1, 0.5, -0.01), (1.0, 0.37, -0.01), (0.37, -2.0, 0.0), (0.0, 0.0, 0.0))
+
+
+@functools.lru_cache(maxsize=1)
+def _a2c_case(name):
+    from oracle import rl_oracle
+    dtype, B, S, V, wk = A2C_CASES[name]
+    seed = 10100 + list(A2C_CASES).index(name)
+    new, _, _, action, meta = gen_rows(seed, B * S, V, dtype, A2C_NAMES, False)
+    g = torch.Generator().manual_seed(seed + 1)
+    adv, ret, value = a2c_side(g, B, S)
+    d = _to({'logit': new.reshape(B, S, V), 'action': action.reshape(B, S), 'weight': _weights(g, B, S, wk),
+             'adv': adv, 'return_': ret, 'value': value}, DEV)
+    parts = {}
+    for dt in (torch.float64, torch.float32):
+        res = []
+        for unit in ((1.0, 0.0, 0.0), (0.0, 1.0, 0.0), (0.0, 0.0, 1.0)):
+            x = d['logit'].to(dt, copy=True).requires_grad_(True)
+            v = d['value'].to(dt, copy=True).requires_grad_(True)
+            w = None if d['weight'] is None else d['weight'].to(dt)
+            p, vl, e = rl_oracle.a2c_error(x, d['action'], v, d['adv'].to(dt), d['return_'].to(dt), w)
+            (unit[0] * p + unit[1] * vl + unit[2] * e).backward()
+            res.append(dict(policy=p.item(), value=vl.item(), entropy=e.item(), grad=x.grad.reshape(B * S, V),
+                            grad_value=v.grad.reshape(-1)))
+        parts[dt] = res
+    x = d['logit'].double()
+    lsm = torch.log_softmax(x, -1)
+    H = -(torch.exp(lsm) * lsm.clamp(min=torch.finfo(torch.float64).min)).sum(-1).reshape(-1).cpu().numpy()
+    w = np.ones(B * S) if d['weight'] is None else d['weight'].double().reshape(-1).cpu().numpy()
+    lp = _lp64(x, d['action'])
+    a_ = d['adv'].double().reshape(-1).cpu().numpy()
+    dv = (d['return_'] - d['value']).double().reshape(-1).cpu().numpy()
+    scales = {'out_policy': float(np.mean(np.abs(lp * a_ * w))), 'out_value': float(np.mean(dv ** 2 * w)),
+              'out_entropy': float(np.mean(np.abs(H * w)))}
+    return d, meta, parts, scales, (w * np.abs(a_), w * (1.0 + H), w * np.abs(dv))
+
+
+def _a2c_refs(parts, mix, div, mult=1.0):
+    out = []
+    for dt in (torch.float32, torch.float64):
+        r = parts[dt]
+        res = OrderedDict([('out_policy', r[0]['policy']), ('out_value', r[0]['value']),
+                           ('out_entropy', r[0]['entropy'])])
+        dev = r[0]['grad'].device
+        gr = sum(torch.tensor(m * mult, dtype=dt, device=dev) * ri['grad'] for m, ri in zip(mix, r))
+        gv = sum(torch.tensor(m * mult, dtype=dt, device=dev) * ri['grad_value'] for m, ri in zip(mix, r))
+        res['grad_logit'] = _np(gr) / div[:, None]
+        res['grad_value'] = _np(gv)
+        out.append(res)
+    return out
+
+
+def _a2c_run(d, mix, div, bf16, want64, poison=False, twice=False, grad=True):
+    import di_engine_b200 as b2
+    R = b2.rl_utils
+    x = d['logit'].clone().requires_grad_(grad)
+    v = d['value'].clone().requires_grad_(grad)
+    loss = R.a2c_error(R.a2c_data(x, d['action'], v, d['adv'], d['return_'], d['weight']))
+    res = OrderedDict([('out_policy', loss.policy_loss.item()), ('out_value', loss.value_loss.item()),
+                       ('out_entropy', loss.entropy_loss.item())])
+    if not grad:
+        return res, None, None
+    if poison:
+        spec = loss.policy_loss.grad_fn.spec
+        spec[0].fill_(POISON)
+        spec[1].fill_(POISON)
+    total = mix[0] * loss.policy_loss + mix[1] * loss.value_loss + mix[2] * loss.entropy_loss
+    total.backward(retain_graph=twice)
+    if twice:
+        total.backward()
+    res['grad_logit'] = grad_entry(x.grad, div, bf16, want64)
+    res['grad_value'] = _np(v.grad).reshape(-1)
+    return res, x.grad, v.grad
+
+
+def _bits(a, b):
+    return np.float32(a).view(np.uint32) == np.float32(b).view(np.uint32)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('name', list(A2C_CASES))
+def test_a2c_lm_fp64(name, monkeypatch):
+    """the forward alone, then each mix with the forward's gradient buffers poisoned (the record's policy and entropy
+    slots kept: d logit is the forward's, untouched; the value slot too: both), again unpoisoned, and a repeated
+    backward (the recompute path); every run starts from the record"""
+    import di_engine_b200 as b2
+    from di_engine_b200 import ops
+    monkeypatch.setattr(b2.rl_utils.ppo, 'LM_MIN_VOCAB', 1)  # fp32 V < 1024 takes the vocabulary kernel too
+    d, meta, parts, scales, (rp, re, rv) = _a2c_case(name)
+    bf16 = d['logit'].dtype == BF16
+    M = rp.size
+    record = ops.ppo_hint(torch.device(DEV, torch.cuda.current_device()), 'a2c')  # the record the calls read
+    saved = record.clone()
+    worst = 0.0
+    WORST.clear()
+    try:
+        ones = np.ones(M)
+        r32, r64 = _a2c_refs(parts, A2C_RECORD, ones)
+        for dd in (r32, r64):
+            dd.pop('grad_logit'), dd.pop('grad_value')
+        worst = compare_regimes(name + ' nograd', _a2c_run(d, A2C_RECORD, ones, bf16, None, grad=False)[0], r32, r64,
+                                meta, scales)
+        for mix in A2C_MIXES:
+            keep_logit = _bits(mix[0], A2C_RECORD[0]) and _bits(mix[2], A2C_RECORD[2])
+            keep_value = keep_logit and _bits(mix[1], A2C_RECORD[1])
+            for path, poison, twice in (('poisoned', True, False), ('', False, False), ('twice', False, True)):
+                mult = 2.0 if twice else 1.0
+                div = row_divisor((abs(mix[0]) * rp + abs(mix[2]) * re) * mult / M)
+                r32, r64 = _a2c_refs(parts, mix, div, mult)
+                record.copy_(torch.tensor(list(A2C_RECORD) + [0.0]))
+                got, gx, gv = _a2c_run(d, mix, div, bf16, r64['grad_logit'] * div[:, None], poison, twice)
+                if poison and keep_logit:  # the backward returned without touching d logit: the forward's buffer
+                    assert bool((gx == POISON).all()), (name, mix)
+                    for dd in (got, r32, r64):
+                        dd.pop('grad_logit')
+                if poison and keep_value:
+                    assert bool((gv == POISON).all()), (name, mix)
+                    for dd in (got, r32, r64):
+                        dd.pop('grad_value')
+                elif poison:
+                    assert not bool((gv == POISON).any()), (name, mix, 'd value not rewritten')
+                worst = max(worst, compare_regimes('%s mix %s %s' % (name, mix, path), got, r32, r64, meta, scales))
+    finally:
+        record.copy_(saved)
+    print('[fp64] %s worst %.2f  per regime %s' % (name, worst, _per_regime()))
 
 
 # ----------------------------------------------------------------------------------------------------------------
