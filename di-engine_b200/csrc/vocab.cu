@@ -2,21 +2,29 @@
 //   grpo_policy_error                 ding/rl_utils/grpo.py             clipped ratio loss + beta * k3 KL to the reference policy
 //   rloo_policy_error                 ding/rl_utils/rloo.py             clipped ratio loss, leave-one-out advantage from reward (K, B')
 //   naive / efficient / less_efficient_method   ding/rl_utils/log_prob_utils.py   per-token log p(a) and its backward
+//   ppo_policy_error / ppo_error's policy part  ding/rl_utils/ppo.py:143-230      on token rows (B, S, V)
+//   a2c_error                                   ding/rl_utils/a2c.py:10-44        on token rows, with a per-token value head
+// and the same losses from the lm_head's hidden states (rl_utils/lm_linear.py), one chunk of logits at a time.
 //
-// vocab_rows_kernel<T, MODE>: persistent CTAs of VOCAB_NT threads, each owning one token row of V logits at a time
-// (row += gridDim.x).  Per row, in ONE streaming pass over every logit tensor of the call (16-byte vector loads, all
-// streams' loads of an iteration in flight together), an online max / sum of exp in fp32 per tensor gives
+// THE CORE, vocab_rows_kernel<T, Head>: persistent CTAs of VOCAB_NT threads, each owning one token row of V logits at a
+// time (row += gridDim.x).  Per row, in ONE streaming pass over the head's Head::NR logit streams (16-byte vector loads,
+// all streams' loads of an iteration in flight together), an online max / sum of exp in fp32 per stream gives
 // logsumexp = max + log(sum exp(z - max)) with torch's rule for an infinite max (treated as 0); the gathered z[a] gives
-// lp = z[a] - logsumexp.  The row epilogue (thread 0) runs the token head (token_head below, in the reference's operation
-// order) and forms c = d loss / d lp_new for a unit upstream gradient; the CTA then writes
-// d loss / d logit_new[row] = c * (onehot(a) - softmax(logit_new[row])) in T.  MODE = LOGP writes lp and logsumexp only;
-// MODE = BWD applies a per-row coefficient g * coef[row] to (onehot - softmax) -- the backward of the log-prob methods, and
-// of the GRPO / RLOO launch when the upstream gradient is not the unit one the forward launch assumed.
+// lp = z[a] - logsumexp.  With Head::ENT the pass also keeps, next to logit_new's max / sum,
+// t = sum e^(z - r) * max(z - r, -FLT_MAX) (r the running max, rescaled with it like s), so H = log s - t / s reuses the
+// exponentials already taken.  After the warp / CTA merge, thread 0 runs the head's row function on lp[] and H: it writes
+// the head's per-row outputs, adds to the CTA's loss partials and returns (c, ce); the CTA then writes
+//   d loss / d logit_new[row] = c * (onehot(a) - p) - ce * p * (max(log p, -FLT_MAX) + H),   p = softmax(logit_new[row])
+// in T (ce = 0 without entropy).  A head that does not stream (the two backward heads) takes c, ce and H from the rows a
+// forward launch saved and goes straight to that gradient pass.  Loss sums: per-CTA partials (grid_store_partials) added
+// in a fixed order by finalize_sums_kernel -- deterministic, no atomics, no host sync.  One launch plan (launch_rows)
+// serves whole tensors and chunks alike; a whole tensor is the one-chunk case.
 //
-// Traffic floor per token row: every logit read once plus the gradient written once, (3 + 1) * V * sizeof(T) for GRPO and
-// (2 + 1) * V * sizeof(T) for RLOO; per-row side data (action, weight, lse, coefficient) is O(1) per row.
+// Traffic floor per token row: every logit stream read once plus the gradient written once, (NR + 1) * V * sizeof(T):
+// (3 + 1) for GRPO and for PPO with logit_pretrained, (2 + 1) for RLOO and for PPO without, (1 + 1) for A2C and for every
+// head on a chunk.  Per-row side data (action, weight, lse, coefficients, per-token operands) is O(1) per row.
 //
-// The softmax of the gradient needs logit_new a second time.  The forward launch keeps the row in dynamic shared memory
+// The softmax of the gradient needs logit_new a second time.  The streaming pass keeps the row in dynamic shared memory
 // as it streams it, up to VOCAB_SMEM_CAP bytes (all of V = 32k in fp32 or V = 64k in bf16).  A longer row (bf16
 // V = 152 064 is 304 KB) keeps its first VOCAB_SMEM_CAP bytes there and reads the rest back from L2 right after the
 // same CTA streamed it: such a row runs one CTA per SM, so the bytes to re-read across the GPU are at most 132 * 84 KB
@@ -28,69 +36,47 @@
 // across the GPU) part of the second read of logit_new goes to HBM and the call moves up to 5 * V * sizeof(T) bytes per
 // row (GRPO) instead of the floor.
 //
+// In place on a chunk (Head::INPL): from hidden states the caller computes the logits one chunk of token rows at a time
+// into a (rows_per_chunk, V) buffer Z with a GEMM, and the chunk heads write d loss / d Z over Z itself, which the caller
+// then feeds to the dH / dW GEMMs.  That is safe because (1) one CTA owns a row, (2) H and lse are known before the
+// gradient pass because the streaming pass forms them, (3) each element's gradient is stored by the thread that has
+// just read that element in the softmax pass (from the shared-memory copy, or from Z for the part past VOCAB_SMEM_CAP),
+// and (4) nothing reads the row after that pass.  The logits and the gradient therefore alias: neither pointer is
+// __restrict__ (VocabArgs holds plain pointers), and Z is read with coherent loads (__ldca), never the read-only path
+// (__ldg), which requires the data to stay unwritten for the kernel's lifetime.  LogpRow and CoefBwdRow (whose
+// load / store pair is already per element and coherent) run on chunk pointers unchanged.  Each chunk launches the same
+// grid and its CTAs store their partials into the chunk's own slice of the workspace; the last chunk's launch adds all
+// of them in one finalize_sums (a fixed chunk plan gives the same bits on every run).
+//
+// Forward-written gradients (the upstream-gradient record of common.cuh).  On logits, the PPO and A2C forward launches
+// write d / d logit_new (and A2C's d / d value) for the upstream gradients the call site expects, read from the device
+// and recorded as used, and save per row what a recompute needs: lse, H and the unit coefficients.  Their backward
+// launch (PgBwdRow) verifies the record on the device: it returns at once when every owned upstream gradient is the one
+// the forward used, and otherwise re-reads logit_new once and writes the gradient once from the saved rows.  GRPO / RLOO
+// save the unit coefficient d loss / d lp_new, and CoefBwdRow applies the actual upstream scalar, returning at once
+// when it is 1.  The chunk heads keep no record: the gradient of the one differentiable output, the loss mix, is fixed
+// at launch, and the caller scales d Z's products dH / dW by its actual upstream gradient, which a per-component mix
+// could not be once the chunk is gone.
+//
+// THE HEADS (each below, with its operands):
+//   GrpoRow<KL, LIN>     GRPO (KL) / RLOO via token_head, in the reference's operation order.  On logits it streams
+//                        logit_new, logit_old (and logit_ref) and sums a sequence's weights inside the row reduction, once
+//                        per visit of a CTA to the sequence; on a chunk it reads per-token fp32 logp_old / logp_ref, and
+//                        the sequence normalisers that couple rows across chunk boundaries (a chunk may split a
+//                        sequence) come from lm_seq_kernel, launched once before the first chunk.
+//   LogpRow              per-token log p(a) and lse (the log-prob methods, token_logp_linear).
+//   CoefBwdRow           d / d logit_new from g * coef[row] (their backward; GRPO / RLOO's for a non-unit upstream).
+//   PpoRow<ENT, KL, LIN> surrogate / kl_term of ppo_math.cuh via ppo_head, so a call carries only the streams and terms
+//                        it has (the common RLHF call: no entropy, 2 or 3 streams).  Loss sums: policy, entropy, kl,
+//                        approx_kl, clipfrac, all over M rows.  Upstream gradients: (g_pol, g_ent, g_kl) from the record
+//                        on logits, the loss mix (1, w_ent, w_kl) on a chunk.
+//   A2cRow<LIN>          a2c_head: lp, H, dv = return_ - value, partials -lp * adv * w, dv^2 * w, H * w, means over M;
+//                        d / d value = g_val * (-2 * w * dv / M) in fp32, so the value head needs no second launch.
+//   PgBwdRow<ENT, VAL>   the backward of PpoRow / A2cRow on logits; with A2C's value slot (VAL) it always rewrites
+//                        d / d value (O(1) per row), and d / d logit_new only when g_pol or g_ent differs.
+//
 // The loss head on a custom log_prob_fn's (B, S) output is a second, small kernel (token_head_kernel below): it reads no
 // logits, so it shares the head arithmetic (token_head) but none of the row machinery.
-//
-// Loss sums (loss, approx_kl, clipfrac): per-CTA partials (grid_store_partials) added in a fixed order by
-// finalize_sums_kernel -- deterministic, no atomics, no host sync.
-//
-// PPO on token rows (ppo_policy_error / the policy part of ppo_error, ding/rl_utils/ppo.py:143-230, at (B, S, V)): MODE =
-// VM_PPO + PPO_ENT (entropy bonus) + PPO_KL (logit_pretrained given), so the common RLHF call (no entropy, 2 or 3 streams)
-// carries neither the entropy accumulator nor the third stream.  Next to logit_new's online max / sum of exp the pass keeps
-// t = sum e^(z - r) * max(z - r, -FLT_MAX) (r the running max, rescaled with it like s), so H = log s - t / s reuses the
-// exponentials already taken.  The row epilogue runs surrogate / kl_term (ppo_math.cuh) and, for the upstream gradients
-// the call site expects (g_pol, g_ent, g_kl: its device-resident record), writes
-// d / d logit_new = c_act * (onehot(a) - p) - c_ent * p * (log p + H), c_act = g_pol * (-w / M) * dsel * r + g_kl * dk / M,
-// c_ent = g_ent * w / M (M rows).  Saved per row: lse, H (entropy only) and the unit coefficients (-w / M) * dsel * r and
-// dk / M, from which VM_PPO_BWD recomputes the gradient for the actual upstream gradients (one read of logit_new, one
-// write) -- unless they are the ones the forward used, in which case it returns at once on the device.  Loss sums:
-// policy, entropy, kl, approx_kl, clipfrac, all over M.  Traffic: (3 + 1) * V * sizeof(T) per row with logit_pretrained,
-// (2 + 1) without -- the same streams and the same L2 re-read of logit_new as GRPO / RLOO.
-//
-// A2C on token rows (a2c_error, ding/rl_utils/a2c.py:10-44, at (B, S, V) with a per-token value head): MODE = VM_A2C
-// streams logit_new alone (NR = 1) with the entropy accumulator always on, and keeps the row in shared memory for the
-// gradient's softmax as the other loss modes do.  The row epilogue follows the reference's order: lp = z[a] - lse,
-// H, dv = return_ - value, partials -lp * adv * w, dv^2 * w, H * w (w = 1 without weight), all three means over M rows.
-// For the expected upstream gradients (g_pol, g_val, g_ent: the call site's record) it writes
-// d / d logit_new = c * (onehot(a) - p) - c_ent * p * (log p + H), c = g_pol * (-adv * w / M), c_ent = g_ent * w / M,
-// and d / d value = g_val * (-2 * w * dv / M) in fp32.  Saved per row: lse, H, the unit coefficients -adv * w / M and
-// -2 * w * dv / M.  The backward is VM_PPO_BWD + PPO_ENT + PPO_VAL, the PPO backward pass with the value slot: it returns
-// at once when all three upstream gradients are the forward's, rewrites only d / d value (O(1) per row) when just g_val
-// differs, and otherwise recomputes both.  Traffic: (1 + 1) * V * sizeof(T) per row, plus O(1) per row -- logit_new read
-// once, its gradient written once, with the same L2 re-read of logit_new past VOCAB_SMEM_CAP.
-//
-// GRPO / RLOO from the lm_head's hidden states (rl_utils/lm_linear.py; b200rl_lm_linear_fwd / _bwd): the caller computes
-// the logits one chunk of token rows at a time into a (rows_per_chunk, V) buffer Z with a GEMM, and MODE = VM_GRPO_LIN /
-// VM_RLOO_LIN streams Z alone (NR = 1, as VM_A2C): the old and reference terms come from per-token fp32 log-probabilities
-// logp_old / logp_ref, read with action, weight and the sequence's normaliser at the global row row0 + r.  The
-// normalisers couple rows across chunk boundaries (a chunk may split a sequence), so lm_seq_kernel forms them once,
-// before the first chunk: sum_s w[b, s] and the row's advantage (GRPO: adv[b]; RLOO: the leave-one-out advantage).
-// Each chunk's CTAs store their loss partials into the chunk's own slice of the workspace and the last chunk's launch
-// adds all of them in one finalize_sums (fixed chunk plan -> the same bits on every run).
-// In place: these modes write d loss / d Z over Z itself, which the caller then feeds to the dH / dW GEMMs.  That is safe
-// because (1) one CTA owns a row, (2) each element's gradient is stored by the thread that has just read that element in
-// the softmax pass (from the shared-memory copy, or from Z for the part past VOCAB_SMEM_CAP), and (3) nothing reads the
-// row after that pass.  The logits and the gradient therefore alias: neither pointer is __restrict__ (VocabArgs holds
-// plain pointers), and Z is read with coherent loads (__ldca), never the read-only path (__ldg), which requires the data
-// to stay unwritten for the kernel's lifetime.  The log-prob mode (VM_LOGP) and the in-place backward with a per-row
-// coefficient (VM_BWD, whose load / store pair is already per element and coherent) run on chunk pointers unchanged.
-// Traffic floor per row: 2 * V * sizeof(T) -- Z read once, d Z written once.
-//
-// PPO / A2C from the lm_head's hidden states (ppo_policy_error_linear / a2c_error_linear; b200rl_lm_linear_pg_fwd): MODE =
-// VM_PPO_LIN + PPO_ENT / PPO_KL and VM_A2C_LIN run on the same chunk Z in place, one stream (NR = 1), reading fp32
-// logp_old / logp_pretrained, action, adv, weight and (A2C) value / return_ at the global row row0 + r.  Their row
-// epilogues are VM_PPO's (surrogate / kl_term of ppo_math.cuh, H = log s - t / s from the online entropy accumulator) and
-// VM_A2C's, and the gradient is the header's d / d Z = c_act * (onehot(a) - p) - c_ent * p * (log p + H) -- but with
-// the upstream gradients (g_pol, g_ent, g_kl) = (1, w_ent, w_kl) (A2C: (g_pol, g_val, g_ent) = (1, w_val, w_ent)) taken
-// from the launch arguments, so the one differentiable output is loss = policy + w_ent * entropy + w_kl * kl
-// (+ w_val * value).  There is no record to verify: the caller scales d Z's products dH / dW by the actual upstream
-// gradient of that loss, which a per-component mix could not be once the chunk is gone.  A2C also writes
-// d loss / d value = w_val * (-2 * w * dv / M) in fp32 at the global row.  No sequence normaliser: both take plain means
-// over all M = B*S rows, so lm_seq_kernel is not launched.  Each chunk stores its partials (PPO: policy, entropy, kl,
-// approx_kl, clipfrac; A2C: policy, value, entropy) into its own workspace slice, and the last chunk's launch adds them
-// in one finalize_sums.  In place as GRPO / RLOO above: one CTA owns a row; H and lse are known before the gradient pass
-// because the streaming pass forms them; each element's gradient is stored by the thread that has just read that element
-// in the softmax pass; nothing reads the row after that pass; Z is read with __ldca, never __ldg.  Traffic floor per row: 2 * V * sizeof(T) -- Z read once, d Z written once.
 #include <cuda_bf16.h>
 #include <math.h>
 
@@ -103,14 +89,6 @@ namespace b200rl {
 constexpr int VOCAB_NT = 512;
 constexpr int VOCAB_HEAD_NT = 256;
 constexpr int VOCAB_SMEM_CAP = 220 * 1024;  // dynamic shared memory for the cached part of logit_new (227 KB opt-in max)
-constexpr int VM_GRPO = 0, VM_RLOO = 1, VM_LOGP = 2, VM_BWD = 3;
-constexpr int VM_PPO = 4, VM_PPO_BWD = 8, PPO_ENT = 1, PPO_KL = 2;  // VM_PPO + flags: 4..7; VM_PPO_BWD + PPO_ENT: 8, 9
-// A2C: forward 12; backward VM_PPO_BWD + PPO_ENT + PPO_VAL = 11 (the PPO backward with the value slot)
-constexpr int PPO_VAL = 2, VM_A2C = 12;
-// GRPO / RLOO on one chunk of a GEMM's output buffer, in place (see the header)
-constexpr int VM_GRPO_LIN = 13, VM_RLOO_LIN = 14;
-// PPO / A2C on one chunk, in place: VM_PPO_LIN + PPO_ENT / PPO_KL = 16..19, VM_A2C_LIN = 20 (see the header)
-constexpr int VM_PPO_LIN = 16, VM_A2C_LIN = 20;
 constexpr float kL2E = 1.4426950408889634f;
 
 // 16-byte vectors of T, widened to fp32
@@ -285,43 +263,43 @@ __device__ __forceinline__ float rloo_adv(const float* __restrict__ reward, int 
 }
 
 struct VocabArgs {
-    const void* x[3];          // logit_new, logit_old, logit_ref (streams in that order; BWD / LOGP: x[0] only)
+    const void* x[3];          // the head's logit streams: logit_new, logit_old, logit_ref / logit_pretrained
     const long long* action;   // (rows)
     const float* adv;          // GRPO: (B)
     const float* reward;       // RLOO: (K, B / K)
     const float* weight;       // (B, S) nullable = ones
-    const float* coef_in;      // BWD: per-row coefficient
-    const float* g;            // BWD: upstream scalar (nullable = 1)
-    float* lp;                 // LOGP: (rows)
-    float* lse;                // forward: logsumexp of logit_new per row; BWD: read
+    const float* coef_in;      // backward: per-row coefficient
+    const float* g;            // CoefBwdRow: upstream scalar (nullable = 1)
+    float* lp;                 // LogpRow, GrpoRow on a chunk (nullable): log p(a) (rows)
+    float* lse;                // forward: logsumexp of logit_new per row; backward: read
     float* coef;               // GRPO / RLOO: d loss / d lp_new per row for a unit upstream gradient
     void* grad;                // d / d logit_new (nullable in the forward = no gradient)
     float* ws;
     long long rows, S, V, Bp;
     int K, skip_if_unit, capv;  // capv: 16-byte vectors of logit_new kept in shared memory
     float lo, hi, beta, inv_b;
-    // PPO (VM_PPO*, VM_PPO_BWD*); adv is then per row and coef / coef_in the policy term's unit coefficient
-    float* ent;                // forward: entropy of logit_new per row (PPO_ENT); VM_PPO_BWD: read (null = no entropy)
-    float* coef_kl;            // forward: d kl_div / d lp_new per row (PPO_KL); VM_PPO_BWD: read (null = no KL)
-    UpstreamRecord rec;        // PPO forward and VM_PPO_BWD (slots policy, entropy, kl)
+    // PpoRow, PgBwdRow; adv is then per row and coef / coef_in the policy term's unit coefficient
+    float* ent;                // forward: entropy of logit_new per row (ENT); backward: read (null = no entropy)
+    float* coef_kl;            // forward: d kl_div / d lp_new per row (KL); backward: read (null = no KL)
+    UpstreamRecord rec;        // PpoRow / A2cRow on logits and PgBwdRow (slots policy, value, entropy, kl)
     float dual_clip, inv_m;    // dual_clip <= 0: off; inv_m = 1 / rows
     int kl_type;
-    // A2C (VM_A2C, VM_PPO_BWD + PPO_ENT + PPO_VAL); adv is per row, rec also owns the value slot
+    // A2cRow, PgBwdRow with the value slot; adv is per row
     const float* value;        // forward: (rows)
     const float* ret;          // forward: return_ (rows)
     float* dval;               // forward: d value_loss / d value per row; backward: read
     float* grad_value;         // d / d value (rows), fp32
-    // VM_GRPO_LIN / VM_RLOO_LIN: the per-row operands start at the chunk's first row; the sequence index is (row0 + r) / S
+    // GrpoRow on a chunk: the per-row operands start at the chunk's first row; the sequence index is (row0 + r) / S
     const float* lp_old;       // (rows)
     const float* lp_ref;       // GRPO: (rows)
     const float* seq;          // (2, nb): sum_s w[b, s], then the advantage of sequence b (lm_seq_kernel)
-    long long row0, nb;
-    // VM_PPO_LIN / VM_A2C_LIN: the loss mix, i.e. the fixed upstream gradients of the entropy, kl and value terms (lp_ref
+    long long row0, nb;        // nb: the number of sequences B (GrpoRow)
+    // PpoRow / A2cRow on a chunk: the loss mix, i.e. the fixed upstream gradients of the entropy, kl and value terms (lp_ref
     // is then logp_pretrained; adv, value, ret and grad_value start at the chunk's first row)
     float w_ent, w_kl, w_val;
 };
 
-// The per-token PPO head of VM_PPO / VM_PPO_LIN (ppo.py:186-230, in its operation order): adds the five loss partials
+// The per-token PPO head of PpoRow (ppo.py:186-230, in its operation order): adds the five loss partials
 // (policy, entropy, kl, approx_kl, clipfrac) to part and returns the unit coefficients d policy_loss / d lp_new and
 // d kl_term / d lp_new (before the 1 / M of the mean)
 struct PPOHead {
@@ -347,7 +325,7 @@ __device__ __forceinline__ PPOHead ppo_head(const VocabArgs& a, float lp_new, fl
     return h;
 }
 
-// The per-token A2C head of VM_A2C / VM_A2C_LIN (a2c.py:39-44, in its operation order): adds the three loss partials
+// The per-token A2C head of A2cRow (a2c.py:39-44, in its operation order): adds the three loss partials
 // (policy, value, entropy) to part and returns d policy_loss / d lp and d value_loss / d value
 struct A2CHead {
     float cp, dvu;
@@ -383,54 +361,189 @@ __device__ __forceinline__ void stream_vecs(const uint4* const (&p)[NR], int i, 
     }
 }
 
-template <class T, int MODE>
+// d loss / d logit_new[row] = c * (onehot(a) - p) - ce * p * (max(log p, -FLT_MAX) + H): the coefficients a head returns
+struct RowCoef {
+    float c, ce;
+};
+
+// What the core knows of a launch before its row loop and hands to every head call: whether it writes a gradient, the
+// upstream-record slots the head owns (common.cuh; 0 without a record) and CoefBwdRow's upstream scalar
+struct RowLaunch {
+    bool want_grad;
+    unsigned owned;
+    float g;
+};
+
+// What a head does not say: one stream, no loss sums, no entropy accumulator, the read-only path, streams the row, no
+// sequence weight in the row reduction, every loss sum over the N rows of the call, no record, no prologue
+struct HeadBase {
+    static constexpr int NR = 1, NP = 0;
+    static constexpr bool ENT = false, INPL = false, STREAM = true, SEQW = false, LOSS_OVER_B = false;
+    static __device__ __forceinline__ unsigned owned(const VocabArgs&) { return 0u; }
+    static __device__ __forceinline__ bool prologue(const VocabArgs&, RowLaunch&) { return false; }
+};
+
+// A forward head with a record on logits (not LIN): it owns the slots OWNED, and its prologue writes the values it applies
+template <bool LIN, unsigned OWNED>
+struct RecordHead : HeadBase {
+    static __device__ __forceinline__ unsigned owned(const VocabArgs&) { return OWNED; }
+    static __device__ __forceinline__ bool prologue(const VocabArgs& a, RowLaunch& L) {
+        float g[4];
+        if (!LIN && L.want_grad) upstream<4>(a.rec, false, L.owned, g);
+        return false;
+    }
+};
+
+// GRPO (KL) / RLOO; w_seq: the sequence's weight sum from the row reduction (logits).  Sums: loss, approx_kl, clipfrac
+template <bool KL, bool LIN>
+struct GrpoRow : HeadBase {
+    static constexpr int NR = LIN ? 1 : (KL ? 3 : 2), NP = 3;
+    static constexpr bool INPL = LIN, SEQW = !LIN, LOSS_OVER_B = true;
+    static __device__ __forceinline__ RowCoef row(const VocabArgs& a, const RowLaunch&, long long row, const float* lp,
+                                                  float lse, float, float w_seq, float* part) {
+        a.lse[row] = lse;
+        const long long b = LIN ? (a.row0 + row) / a.S : row / a.S;
+        const float W_ = LIN ? a.seq[b] : w_seq;
+        const float w = a.weight ? a.weight[row] : 1.f;
+        const float adv = LIN ? a.seq[a.nb + b] : (KL ? a.adv[b] : rloo_adv(a.reward, a.K, a.Bp, b));
+        const float lpo = LIN ? a.lp_old[row] : lp[1];
+        const TokenHead th = token_head<KL>(lp[0], lpo, KL ? (LIN ? a.lp_ref[row] : lp[NR - 1]) : 0.f, adv, a.lo, a.hi,
+                                            a.beta, a.inv_b / W_ * w);
+        if (LIN && a.lp) a.lp[row] = lp[0];
+        if (!LIN) a.coef[row] = th.dlp;
+        part[0] += th.loss * w / W_;
+        part[1] += lpo - lp[0];
+        part[2] += th.clipped;
+        return {th.dlp, 0.f};
+    }
+};
+
+// log p(a) and logsumexp per row, no gradient
+struct LogpRow : HeadBase {
+    static __device__ __forceinline__ RowCoef row(const VocabArgs& a, const RowLaunch&, long long row, const float* lp,
+                                                  float lse, float, float, float*) {
+        a.lse[row] = lse;
+        a.lp[row] = lp[0];
+        return {0.f, 0.f};
+    }
+};
+
+// c = g * coef[row] on the saved lse; with skip_if_unit it returns at once when g == 1 (the forward wrote this gradient)
+struct CoefBwdRow : HeadBase {
+    static constexpr bool STREAM = false;
+    static __device__ __forceinline__ bool prologue(const VocabArgs& a, RowLaunch& L) {
+        if (a.g) L.g = *a.g;
+        return a.skip_if_unit && L.g == 1.f;
+    }
+    static __device__ __forceinline__ RowCoef coef(const VocabArgs& a, const RowLaunch& L, long long row, float&) {
+        return {L.g * a.coef_in[row], 0.f};
+    }
+};
+
+// PPO (ENT: entropy bonus, KL: pretrained log p given); upstream gradients: the record, or on a chunk (1, w_ent, w_kl)
+template <bool ENT_, bool KL, bool LIN>
+struct PpoRow : RecordHead<LIN, 1u | (ENT_ ? 4u : 0u) | (KL ? 8u : 0u)> {  // slots policy, entropy, kl
+    static constexpr int NR = LIN ? 1 : (KL ? 3 : 2), NP = 5;
+    static constexpr bool ENT = ENT_, INPL = LIN;
+    static __device__ __forceinline__ RowCoef row(const VocabArgs& a, const RowLaunch& L, long long row, const float* lp,
+                                                  float lse, float H, float, float* part) {
+        if (!LIN) a.lse[row] = lse;
+        const float w = a.weight ? a.weight[row] : 1.f;
+        const PPOHead ph = ppo_head<KL>(a, lp[0], LIN ? a.lp_old[row] : lp[1],
+                                        LIN ? (KL ? a.lp_ref[row] : 0.f) : lp[NR - 1], a.adv[row], w, H, part);
+        if (!LIN) {
+            a.coef[row] = ph.cp;
+            if (KL) a.coef_kl[row] = ph.dk * a.inv_m;  // d kl_div / d lp_new
+            if (ENT) a.ent[row] = H;
+        }
+        RowCoef r{0.f, 0.f};
+        // The record is read here, once per row, rather than held across the row loop; each value is read where it is
+        // used, as loading all first lets nvcc contract the other product of c into the FMA (a different last bit)
+        if (LIN || L.want_grad) {
+            r.c = (LIN ? 1.f : upstream_value(a.rec, L.owned, 0)) * ph.cp +
+                  (KL ? (LIN ? a.w_kl : upstream_value(a.rec, L.owned, 3)) * ph.dk * a.inv_m : 0.f);
+            r.ce = (LIN ? a.w_ent : upstream_value(a.rec, L.owned, 2)) * w * a.inv_m;
+        }
+        return r;
+    }
+};
+
+// A2C; upstream gradients: the record, or on a chunk (1, w_val, w_ent), where d / d value is written only when wanted
+template <bool LIN>
+struct A2cRow : RecordHead<LIN, 7u> {  // slots policy, value, entropy
+    static constexpr int NP = 3;
+    static constexpr bool ENT = true, INPL = LIN;
+    static __device__ __forceinline__ RowCoef row(const VocabArgs& a, const RowLaunch& L, long long row, const float* lp,
+                                                  float lse, float H, float, float* part) {
+        if (!LIN) a.lse[row] = lse;
+        const float w = a.weight ? a.weight[row] : 1.f;
+        const A2CHead ah = a2c_head(a, lp[0], a.adv[row], a.ret[row], a.value[row], w, H, part);
+        if (!LIN) {
+            a.coef[row] = ah.cp;
+            a.dval[row] = ah.dvu;
+            a.ent[row] = H;
+        }
+        RowCoef r{0.f, 0.f};
+        if (LIN || L.want_grad) {
+            const float gp = LIN ? 1.f : upstream_value(a.rec, L.owned, 0);
+            const float gv = LIN ? a.w_val : upstream_value(a.rec, L.owned, 1);
+            const float ge = LIN ? a.w_ent : upstream_value(a.rec, L.owned, 2);
+            r.c = gp * ah.cp;
+            r.ce = ge * w * a.inv_m;
+            if (!LIN || a.grad_value) a.grad_value[row] = gv * ah.dvu;
+        }
+        return r;
+    }
+};
+
+// The verify launch of PpoRow / A2cRow on logits (ENT: entropy saved, VAL: A2C's value slot, kl when coef_kl is given)
+template <bool ENT_, bool VAL>
+struct PgBwdRow : HeadBase {
+    static constexpr bool ENT = ENT_, STREAM = false;
+    static __device__ __forceinline__ unsigned owned(const VocabArgs& a) {
+        return 1u | (VAL ? 2u : 0u) | (ENT ? 4u : 0u) | (a.coef_kl ? 8u : 0u);
+    }
+    static __device__ __forceinline__ bool prologue(const VocabArgs& a, RowLaunch& L) {
+        float g[4];
+        if (upstream<4>(a.rec, true, L.owned, g)) return true;
+        if (VAL) {
+            for (long long r = (long long)blockIdx.x * VOCAB_NT + threadIdx.x; r < a.rows;
+                 r += (long long)gridDim.x * VOCAB_NT)
+                a.grad_value[r] = g[1] * a.dval[r];
+            const float* u = a.rec.used;
+            if (u && __float_as_uint(g[0]) == __float_as_uint(u[0]) && __float_as_uint(g[2]) == __float_as_uint(u[2]))
+                return true;
+        }
+        return false;
+    }
+    static __device__ __forceinline__ RowCoef coef(const VocabArgs& a, const RowLaunch& L, long long row, float& H) {
+        const float gp = upstream_value(a.rec, L.owned, 0), gk = upstream_value(a.rec, L.owned, 3);
+        RowCoef r{gp * a.coef_in[row] + (a.coef_kl ? gk * a.coef_kl[row] : 0.f), 0.f};
+        if (ENT) {
+            r.ce = upstream_value(a.rec, L.owned, 2) * (a.weight ? a.weight[row] : 1.f) * a.inv_m;
+            H = a.ent[row];
+        }
+        return r;
+    }
+};
+
+template <class T, class Head>
 __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
     pdl_prologue();
     using V_ = VecT<T>;
-    constexpr int W = V_::W;
-    constexpr bool PPO = MODE >= VM_PPO && MODE < VM_PPO_BWD, PBWD = MODE >= VM_PPO_BWD && MODE < VM_A2C;
-    constexpr bool A2C = MODE == VM_A2C, VAL = A2C || (PBWD && (MODE & PPO_VAL));  // VAL: the A2C value slot
-    constexpr bool PLIN = MODE >= VM_PPO_LIN && MODE < VM_A2C_LIN, ALIN = MODE == VM_A2C_LIN;
-    constexpr bool ENT = ((PPO || PBWD || PLIN) && (MODE & PPO_ENT)) || A2C || ALIN;
-    constexpr bool KL = (PPO || PLIN) && (MODE & PPO_KL);
-    constexpr bool BWD = MODE == VM_BWD || PBWD;
-    constexpr bool LIN = MODE == VM_GRPO_LIN || MODE == VM_RLOO_LIN;
-    constexpr bool INPL = LIN || PLIN || ALIN;  // one in-place stream (NR = 1)
-    constexpr int NR = MODE == VM_GRPO ? 3 : (MODE == VM_RLOO ? 2 : (PPO ? (KL ? 3 : 2) : 1));
-    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO || A2C || INPL;
-    constexpr int NP = (PPO || PLIN) ? 5 : 3;
+    constexpr int W = V_::W, NR = Head::NR, NP = Head::NP;
+    constexpr bool ENT = Head::ENT, INPL = Head::INPL, STREAM = Head::STREAM, LOSS = NP > 0;
     extern __shared__ uint4 s_row[];
     __shared__ float s_m[NR][VOCAB_NT / 32], s_s[NR][VOCAB_NT / 32], s_w[VOCAB_NT / 32];
     __shared__ float s_c, s_lse;
     __shared__ long long s_a;
-    __shared__ float s_t[ENT ? VOCAB_NT / 32 : 1], s_ce, s_h;  // PPO entropy: t partials, c_ent, H
+    __shared__ float s_t[ENT ? VOCAB_NT / 32 : 1], s_ce, s_h;  // entropy: t partials, c_ent, H
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const long long V = a.V;
-    const bool want_grad = a.grad != nullptr;
-    float gscale = 1.f;
-    if (MODE == VM_BWD) {
-        if (a.g) gscale = *a.g;
-        if (a.skip_if_unit && gscale == 1.f) return;  // the forward launch already wrote exactly this gradient
-    }
-    // PPO upstream-gradient slots: policy, entropy with the bonus, kl with logit_pretrained.  The record is written (forward)
-    // or verified (VM_PPO_BWD) here; the values are read again where they are used, once per row, rather than held in
-    // registers across the row loop.
-    const unsigned owned = 1u | (VAL ? 2u : 0u) | (ENT ? 4u : 0u) | ((KL || (PBWD && a.coef_kl)) ? 8u : 0u);
-    if (PBWD || ((PPO || A2C) && want_grad)) {
-        float g[4];
-        if (upstream<4>(a.rec, PBWD, owned, g)) return;  // VM_PPO_BWD: the forward wrote exactly this gradient
-        if (PBWD && VAL) {
-            // A2C: d / d value = g_val * dval, O(1) per row and always rewritten; d / d logit_new only when the policy
-            // or entropy upstream gradient differs from the forward's (the gradient the forward wrote stays exact)
-            for (long long r = (long long)blockIdx.x * VOCAB_NT + tid; r < a.rows; r += (long long)gridDim.x * VOCAB_NT)
-                a.grad_value[r] = g[1] * a.dval[r];
-            const float* u = a.rec.used;
-            if (u && __float_as_uint(g[0]) == __float_as_uint(u[0]) && __float_as_uint(g[2]) == __float_as_uint(u[2]))
-                return;
-        }
-    }
-    float part[NP] = {0.f, 0.f, 0.f};  // thread 0: the loss partial sums of this CTA's rows (loss, approx_kl, clipfrac; PPO: 5)
-    float w_tot = (float)a.S;  // thread 0: sum_s w[b, s] of the current row's sequence (S without weights)
+    RowLaunch L{a.grad != nullptr, Head::owned(a), 1.f};
+    if (Head::prologue(a, L)) return;
+    float part[LOSS ? NP : 1] = {};  // thread 0: the loss partial sums of this CTA's rows
+    float w_tot = (float)a.S;  // thread 0: sum_s w[b, s] of the current row's sequence (SEQW; S without weights)
     for (long long row = blockIdx.x; row < a.rows; row += gridDim.x) {
         const size_t off = (size_t)row * (size_t)V;
         // elements before the row's first 16-byte boundary (the base pointers are 16-byte aligned)
@@ -445,26 +558,19 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
             rp[r] = reinterpret_cast<const T*>(a.x[r]) + off;
             vp[r] = reinterpret_cast<const uint4*>(rp[r] + h);
         }
-        float c = 0.f, lse = 0.f, ce = 0.f, H = 0.f;  // ce, H: PPO entropy term
+        float c = 0.f, lse = 0.f, ce = 0.f, H = 0.f;  // ce, H: entropy term
         long long act = 0;
-        if (MODE == VM_BWD) {
-            c = gscale * a.coef_in[row];
-            lse = a.lse[row];
-            act = a.action[row];
-        } else if (PBWD) {
-            const float gp = upstream_value(a.rec, owned, 0), gk = upstream_value(a.rec, owned, 3);
-            c = gp * a.coef_in[row] + (a.coef_kl ? gk * a.coef_kl[row] : 0.f);
-            if (ENT) {
-                ce = upstream_value(a.rec, owned, 2) * (a.weight ? a.weight[row] : 1.f) * a.inv_m;
-                H = a.ent[row];
-            }
+        if constexpr (!STREAM) {
+            const RowCoef rc = Head::coef(a, L, row, H);
+            c = rc.c;
+            ce = rc.ce;
             lse = a.lse[row];
             act = a.action[row];
         } else {
-            float m[NR], s[NR], t = 0.f;  // t: PPO entropy accumulator of logit_new
+            float m[NR], s[NR], t = 0.f;  // t: entropy accumulator of logit_new
 #pragma unroll
             for (int r = 0; r < NR; ++r) m[r] = -INFINITY, s[r] = 0.f;
-            const bool cache = LOSS && want_grad;
+            const bool cache = LOSS && L.want_grad;
             int i = tid;
             for (; i + VOCAB_NT < nvec; i += 2 * VOCAB_NT) {
                 if (cache) {
@@ -491,9 +597,8 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
             }
             float wsum = 0.f;
             // a CTA's rows step by gridDim.x (< S at language-model sizes): it sums a sequence's weights once per visit to
-            // that sequence, not once per token
-            const bool new_seq = (MODE == VM_GRPO || MODE == VM_RLOO) && a.weight &&
-                                 (row < gridDim.x || row / a.S != (row - gridDim.x) / a.S);
+            // that sequence, not once per token, here in the row reduction so that it shares the reduction's barrier
+            const bool new_seq = Head::SEQW && a.weight && (row < gridDim.x || row / a.S != (row - gridDim.x) / a.S);
             if (new_seq) {
                 const float* wr = a.weight + (row / a.S) * a.S;
                 for (long long j = tid; j < a.S; j += VOCAB_NT) wsum += wr[j];
@@ -532,97 +637,29 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
                     if (r == 0) lse = l;
                     lp[r] = ok ? V_::to_f(rp[r][act]) - l : __int_as_float(0x7fc00000);
                 }
-                if (!PLIN && !ALIN) a.lse[row] = lse;  // the PPO / A2C chunks keep nothing per row
-                if (MODE == VM_LOGP) a.lp[row] = lp[0];
-                if constexpr (PPO) {
-                    const float w = a.weight ? a.weight[row] : 1.f;
-                    const PPOHead ph = ppo_head<KL>(a, lp[0], lp[1], lp[NR - 1], a.adv[row], w, H, part);
-                    a.coef[row] = ph.cp;
-                    if (KL) a.coef_kl[row] = ph.dk * a.inv_m;  // d kl_div / d lp_new
-                    if (ENT) a.ent[row] = H;
-                    if (want_grad) {
-                        c = upstream_value(a.rec, owned, 0) * ph.cp +
-                            (KL ? upstream_value(a.rec, owned, 3) * ph.dk * a.inv_m : 0.f);
-                        ce = upstream_value(a.rec, owned, 2) * w * a.inv_m;
-                    }
-                    s_ce = ce;
-                    s_h = H;
-                } else if constexpr (PLIN) {  // VM_PPO's head, old / pretrained terms read per token, mix (1, w_ent, w_kl)
-                    const float w = a.weight ? a.weight[row] : 1.f;
-                    const PPOHead ph = ppo_head<KL>(a, lp[0], a.lp_old[row], KL ? a.lp_ref[row] : 0.f, a.adv[row], w, H,
-                                                    part);
-                    c = ph.cp + (KL ? a.w_kl * ph.dk * a.inv_m : 0.f);
-                    ce = a.w_ent * w * a.inv_m;
-                    s_ce = ce;
-                    s_h = H;
-                } else if constexpr (A2C) {
-                    const float w = a.weight ? a.weight[row] : 1.f;
-                    const A2CHead ah = a2c_head(a, lp[0], a.adv[row], a.ret[row], a.value[row], w, H, part);
-                    a.coef[row] = ah.cp;
-                    a.dval[row] = ah.dvu;
-                    a.ent[row] = H;
-                    if (want_grad) {
-                        c = upstream_value(a.rec, owned, 0) * ah.cp;
-                        ce = upstream_value(a.rec, owned, 2) * w * a.inv_m;
-                        a.grad_value[row] = upstream_value(a.rec, owned, 1) * ah.dvu;
-                    }
-                    s_ce = ce;
-                    s_h = H;
-                } else if constexpr (ALIN) {  // VM_A2C's head, mix (1, w_val, w_ent)
-                    const float w = a.weight ? a.weight[row] : 1.f;
-                    const A2CHead ah = a2c_head(a, lp[0], a.adv[row], a.ret[row], a.value[row], w, H, part);
-                    c = ah.cp;
-                    ce = a.w_ent * w * a.inv_m;
-                    if (a.grad_value) a.grad_value[row] = a.w_val * ah.dvu;
-                    s_ce = ce;
-                    s_h = H;
-                } else if constexpr (LIN) {  // the token head with the old / ref terms read per token
-                    const long long b = (a.row0 + row) / a.S;
-                    const float W_ = a.seq[b], adv = a.seq[a.nb + b];
-                    const float w = a.weight ? a.weight[row] : 1.f;
-                    const float lpo = a.lp_old[row];
-                    const TokenHead th = token_head<MODE == VM_GRPO_LIN>(
-                        lp[0], lpo, MODE == VM_GRPO_LIN ? a.lp_ref[row] : 0.f, adv, a.lo, a.hi, a.beta, a.inv_b / W_ * w);
-                    c = th.dlp;
-                    if (a.lp) a.lp[row] = lp[0];
-                    part[0] += th.loss * w / W_;
-                    part[1] += lpo - lp[0];
-                    part[2] += th.clipped;
-                } else if (LOSS) {
-                    const long long b = row / a.S;
-                    if (new_seq) {
-                        w_tot = 0.f;
-                        for (int w = 0; w < VOCAB_NT / 32; ++w) w_tot += s_w[w];
-                    }
-                    const float W_ = w_tot;
-                    const float w = a.weight ? a.weight[row] : 1.f;
-                    const float adv = MODE == VM_GRPO ? a.adv[b] : rloo_adv(a.reward, a.K, a.Bp, b);
-                    const float gt = a.inv_b / W_ * w;
-                    const TokenHead th = token_head<MODE == VM_GRPO>(lp[0], lp[1], NR > 2 ? lp[NR - 1] : 0.f, adv, a.lo,
-                                                                     a.hi, a.beta, gt);
-                    c = th.dlp;
-                    a.coef[row] = c;
-                    part[0] += th.loss * w / W_;
-                    part[1] += lp[1] - lp[0];
-                    part[2] += th.clipped;
+                if (new_seq) {
+                    w_tot = 0.f;
+                    for (int w = 0; w < VOCAB_NT / 32; ++w) w_tot += s_w[w];
                 }
-                s_c = c;
+                const RowCoef rc = Head::row(a, L, row, lp, lse, H, w_tot, part);
+                s_c = rc.c;
                 s_lse = lse;
                 s_a = act;
+                if (ENT) s_ce = rc.ce, s_h = H;
             }
             __syncthreads();
-            if (!LOSS || !want_grad) continue;
+            if (!LOSS || !L.want_grad) continue;
             c = s_c;
             lse = s_lse;
             act = s_a;
             if (ENT) ce = s_ce, H = s_h;
         }
-        // d / d logit_new[row] = c * (onehot(a) - softmax) [PPO entropy: - ce * p * (max(log p, -FLT_MAX) + H)]
+        // d / d logit_new[row] = c * (onehot(a) - softmax) [entropy: - ce * p * (max(log p, -FLT_MAX) + H)]
         T* gr = reinterpret_cast<T*>(a.grad) + off;
         uint4* gv = reinterpret_cast<uint4*>(gr + h);
         for (int i = tid; i < nvec; i += VOCAB_NT) {
-            const uint4 u = (LOSS && i < a.capv) ? s_row[i]
-                                                 : (BWD ? __ldcs(vp[0] + i) : (INPL ? __ldca(vp[0] + i) : __ldg(vp[0] + i)));
+            const uint4 u = (STREAM && i < a.capv) ? s_row[i]
+                                                   : (!STREAM ? __ldcs(vp[0] + i) : (INPL ? __ldca(vp[0] + i) : __ldg(vp[0] + i)));
             float x[W];
             V_::unpack(u, x);
             const long long e0 = h + (long long)i * W;
@@ -649,14 +686,30 @@ __global__ void __launch_bounds__(VOCAB_NT) vocab_rows_kernel(VocabArgs a) {
         }
         if (LOSS) __syncthreads();  // s_row and s_c are rewritten by the next row
     }
-    if (LOSS) {
-        float v[NP] = {0.f, 0.f, 0.f};
-        if (tid == 0) v[0] = part[0], v[1] = part[1], v[2] = part[2];
-        if constexpr (PPO || PLIN) {
-            if (tid == 0) v[3] = part[3], v[4] = part[4];
-        }
+    if constexpr (LOSS) {
+        float v[NP] = {};
+        if (tid == 0)
+#pragma unroll
+            for (int k = 0; k < NP; ++k) v[k] = part[k];
         grid_store_partials<NP, VOCAB_NT>(v, a.ws);
     }
+}
+
+// sum_s w[b, s] of the sequence whose S weights start at weight + o (S without weights), in every thread of a
+// VOCAB_HEAD_NT-thread CTA
+__device__ __forceinline__ float seq_weight_sum(const float* weight, long long o, long long S) {
+    __shared__ float s_w[VOCAB_HEAD_NT / 32];
+    if (!weight) return (float)S;
+    const int tid = threadIdx.x;
+    float ws = 0.f;
+    for (long long j = tid; j < S; j += VOCAB_HEAD_NT) ws += weight[o + j];
+    ws = warp_sum(ws);
+    if ((tid & 31) == 0) s_w[tid >> 5] = ws;
+    __syncthreads();
+    float W_ = 0.f;
+    for (int w = 0; w < VOCAB_HEAD_NT / 32; ++w) W_ += s_w[w];
+    __syncthreads();
+    return W_;
 }
 
 // The token head alone, on per-token log-probabilities a caller computed itself (a custom log_prob_fn): one CTA per
@@ -666,23 +719,12 @@ __global__ void __launch_bounds__(VOCAB_HEAD_NT) token_head_kernel(const float* 
                                                                    const float* __restrict__ lp_old,
                                                                    const float* __restrict__ lp_ref, VocabArgs a) {
     pdl_prologue();
-    __shared__ float s_w[VOCAB_HEAD_NT / 32];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int tid = threadIdx.x;
     const long long B = a.rows / a.S;
     float part[3] = {0.f, 0.f, 0.f};
     for (long long b = blockIdx.x; b < B; b += gridDim.x) {
         const long long o = b * a.S;
-        float W_ = (float)a.S;
-        if (a.weight) {
-            float ws = 0.f;
-            for (long long j = tid; j < a.S; j += VOCAB_HEAD_NT) ws += a.weight[o + j];
-            ws = warp_sum(ws);
-            if (lane == 0) s_w[wid] = ws;
-            __syncthreads();
-            W_ = 0.f;
-            for (int w = 0; w < VOCAB_HEAD_NT / 32; ++w) W_ += s_w[w];
-            __syncthreads();
-        }
+        const float W_ = seq_weight_sum(a.weight, o, a.S);
         const float adv = KL ? a.adv[b] : rloo_adv(a.reward, a.K, a.Bp, b);
         for (long long j = tid; j < a.S; j += VOCAB_HEAD_NT) {
             const float w = a.weight ? a.weight[o + j] : 1.f;
@@ -697,26 +739,14 @@ __global__ void __launch_bounds__(VOCAB_HEAD_NT) token_head_kernel(const float* 
     grid_store_partials<3, VOCAB_HEAD_NT>(part, a.ws);
 }
 
-// The sequence normalisers of VM_GRPO_LIN / VM_RLOO_LIN, once per call: one CTA per sequence b at a time writes
-// seq[b] = sum_s w[b, s] (S without weights; token_head_kernel's order) and seq[nb + b] = the advantage of sequence b.
+// The sequence normalisers of GrpoRow on a chunk, once per call: one CTA per sequence b at a time writes
+// seq[b] = sum_s w[b, s] (token_head_kernel's sum) and seq[nb + b] = the advantage of sequence b.
 __global__ void __launch_bounds__(VOCAB_HEAD_NT) lm_seq_kernel(VocabArgs a) {
     pdl_prologue();
-    __shared__ float s_w[VOCAB_HEAD_NT / 32];
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     float* seq = const_cast<float*>(a.seq);
     for (long long b = blockIdx.x; b < a.nb; b += gridDim.x) {
-        float W_ = (float)a.S;
-        if (a.weight) {
-            float ws = 0.f;
-            for (long long j = tid; j < a.S; j += VOCAB_HEAD_NT) ws += a.weight[b * a.S + j];
-            ws = warp_sum(ws);
-            if (lane == 0) s_w[wid] = ws;
-            __syncthreads();
-            W_ = 0.f;
-            for (int w = 0; w < VOCAB_HEAD_NT / 32; ++w) W_ += s_w[w];
-            __syncthreads();
-        }
-        if (tid == 0) {
+        const float W_ = seq_weight_sum(a.weight, b * a.S, a.S);
+        if (threadIdx.x == 0) {
             seq[b] = W_;
             seq[a.nb + b] = a.reward ? rloo_adv(a.reward, a.K, a.Bp, b) : a.adv[b];
         }
@@ -754,83 +784,51 @@ namespace {
 
 bool aligned_logits(const void* p) { return p && aligned16(p); }
 
-template <class T, int MODE>
-int launch_rows(VocabArgs& a, float* out3, size_t ws_bytes, long long B, cudaStream_t st) {
-    constexpr auto kern = vocab_rows_kernel<T, MODE>;
-    constexpr bool PPO = MODE >= VM_PPO && MODE < VM_PPO_BWD;
-    constexpr bool LOSS = MODE == VM_GRPO || MODE == VM_RLOO || PPO || MODE == VM_A2C;
-    constexpr int NP = PPO ? 5 : 3;
-    const long long nvec_max = (a.V * (long long)sizeof(T) + 15) / 16;
-    a.capv = (LOSS && a.grad) ? (int)min(nvec_max, (long long)(VOCAB_SMEM_CAP / 16)) : 0;
-    const size_t smem = (size_t)a.capv * 16;
-    int sms = 0, per_sm = 0;
-    if (int rc = resident_ctas<kern>(VOCAB_NT, smem, sms, per_sm)) return rc;
-    long long grid = (long long)sms * per_sm;
-    if (grid > a.rows) grid = a.rows;
-    if (LOSS && !ws_partials_fit(grid * NP, ws_bytes)) return B200RL_ERR_WORKSPACE;
-    if (int rc = launch_k(kern, (int)grid, VOCAB_NT, smem, st, a)) return rc;
-    if (!LOSS) return B200RL_OK;
-    FinalizeArgs fa{};
-    if (PPO || MODE == VM_A2C) {  // PPO: policy, entropy, kl, approx_kl, clipfrac; A2C: policy, value, entropy; row means
-        for (int k = 0; k < NP; ++k) fa.scale[k] = 1.0 / (double)a.rows;
-    } else {
-        fa.scale[0] = 1.0 / (double)B;
-        fa.scale[1] = fa.scale[2] = 1.0 / (double)a.rows;
-    }
-    fa.k = NP;
-    fa.n_blocks = (int)grid;
-    return launch_finalize(a.ws, out3, fa, st);
-}
-
-template <int MODE>
-int launch_dtype(int dtype, VocabArgs& a, float* out3, size_t ws_bytes, long long B, cudaStream_t st) {
-    if (dtype == B200RL_DTYPE_F32) return launch_rows<float, MODE>(a, out3, ws_bytes, B, st);
-    if (dtype == B200RL_DTYPE_BF16) return launch_rows<__nv_bfloat16, MODE>(a, out3, ws_bytes, B, st);
-    return B200RL_ERR_ARG;
-}
-
 bool sizes_ok(long long B, long long S, long long V) {
     return B > 0 && S > 0 && V > 0 && V < (1ll << 31) && B * S < (1ll << 40);
 }
 
-// One chunk of VM_GRPO_LIN / VM_RLOO_LIN / VM_PPO_LIN / VM_A2C_LIN.  Every chunk of a call launches the same grid (the
-// plan's chunk_rows, not this chunk's rows, caps it), so chunk c's CTAs own partial rows [c * grid, (c + 1) * grid);
-// CTAs past the last chunk's rows store zeros.  The last chunk adds all n_chunks * grid rows: GRPO / RLOO's loss over B
-// sequences and approx_kl / clipfrac over N tokens, PPO / A2C's NP sums all over N tokens.
-template <class T, int MODE>
-int launch_lin(VocabArgs& a, long long chunk_rows, long long B, float* out, size_t ws_bytes, cudaStream_t st) {
-    constexpr auto kern = vocab_rows_kernel<T, MODE>;
-    constexpr bool PG = MODE >= VM_PPO_LIN;
-    constexpr int NP = (MODE >= VM_PPO_LIN && MODE < VM_A2C_LIN) ? 5 : 3;
+// The launch plan of vocab_rows_kernel: rows [a.row0, a.row0 + a.rows) of a call over N rows cut into chunks of
+// chunk_rows (a whole tensor is the one chunk row0 = 0, rows = chunk_rows = N).  Every chunk of a call launches the same
+// grid (the plan's chunk_rows, not this chunk's rows, caps it), so chunk c's CTAs own partial rows [c * grid,
+// (c + 1) * grid); CTAs past the last chunk's rows store zeros.  The chunk that ends the call adds all n_chunks * grid
+// rows of partials: GRPO / RLOO's loss term over a.nb = B sequences, everything else over N rows.
+template <class Head, class T>
+int launch_rows(T, VocabArgs& a, long long chunk_rows, long long N, float* out, size_t ws_bytes, cudaStream_t st) {
+    constexpr auto kern = vocab_rows_kernel<T, Head>;
+    constexpr int NP = Head::NP;
     const long long nvec_max = (a.V * (long long)sizeof(T) + 15) / 16;
-    a.capv = a.grad ? (int)min(nvec_max, (long long)(VOCAB_SMEM_CAP / 16)) : 0;
+    a.capv = (NP > 0 && a.grad) ? (int)min(nvec_max, (long long)(VOCAB_SMEM_CAP / 16)) : 0;
     const size_t smem = (size_t)a.capv * 16;
     int sms = 0, per_sm = 0;
     if (int rc = resident_ctas<kern>(VOCAB_NT, smem, sms, per_sm)) return rc;
     const long long grid = min((long long)sms * per_sm, chunk_rows);
-    const long long N = B * a.S, n_chunks = (N + chunk_rows - 1) / chunk_rows, chunk = a.row0 / chunk_rows;
+    if (NP == 0) return launch_k(kern, (int)grid, VOCAB_NT, smem, st, a);
+    const long long n_chunks = (N + chunk_rows - 1) / chunk_rows, chunk = a.row0 / chunk_rows;
     if (!ws_partials_fit(n_chunks * grid * NP, ws_bytes)) return B200RL_ERR_WORKSPACE;
     float* ws = a.ws;
     a.ws = ws + chunk * grid * NP;
     if (int rc = launch_k(kern, (int)grid, VOCAB_NT, smem, st, a)) return rc;
     if (a.row0 + a.rows < N) return B200RL_OK;
     FinalizeArgs fa{};
-    if (PG) {
-        for (int k = 0; k < NP; ++k) fa.scale[k] = 1.0 / (double)N;
-    } else {
-        fa.scale[0] = 1.0 / (double)B;
-        fa.scale[1] = fa.scale[2] = 1.0 / (double)N;
-    }
+    for (int k = 0; k < NP; ++k) fa.scale[k] = 1.0 / (double)N;
+    if (Head::LOSS_OVER_B) fa.scale[0] = 1.0 / (double)a.nb;
     fa.k = NP;
     fa.n_blocks = (int)(n_chunks * grid);
     return launch_finalize(ws, out, fa, st);
 }
 
-template <int MODE>
-int launch_lin_dtype(int dtype, VocabArgs& a, long long chunk_rows, long long B, float* out, size_t ws_bytes,
-                     cudaStream_t st) {
-    if (dtype == B200RL_DTYPE_F32) return launch_lin<float, MODE>(a, chunk_rows, B, out, ws_bytes, st);
-    return launch_lin<__nv_bfloat16, MODE>(a, chunk_rows, B, out, ws_bytes, st);
+// The instantiation table of this file's kernels: f(T(), std::bool_constant<ENT>(), std::bool_constant<KL>()) for the
+// runtime dtype (fp32 or bf16) and entropy / kl flags; a kernel that takes neither flag ignores them
+template <class F>
+int with_vocab(int dtype, bool ent, bool kl, F&& f) {
+    const auto flags = [&](auto t) {
+        if (ent) return kl ? f(t, std::true_type(), std::true_type()) : f(t, std::true_type(), std::false_type());
+        return kl ? f(t, std::false_type(), std::true_type()) : f(t, std::false_type(), std::false_type());
+    };
+    if (dtype == B200RL_DTYPE_F32) return flags(float());
+    if (dtype == B200RL_DTYPE_BF16) return flags(__nv_bfloat16());
+    return B200RL_ERR_ARG;
 }
 
 }  // namespace
@@ -850,8 +848,10 @@ extern "C" int b200rl_grpo_fwd_grad(int dtype, const void* logit_new, const void
     a.lse = lse_new; a.coef = dlogp_unit; a.grad = grad_logit_new; a.ws = workspace;
     a.rows = B * S; a.S = S; a.V = V;
     a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio); a.beta = (float)beta;
-    a.inv_b = (float)(1.0 / (double)B);
-    return launch_dtype<VM_GRPO>(dtype, a, out3, workspace_bytes, B, (cudaStream_t)stream);
+    a.inv_b = (float)(1.0 / (double)B); a.nb = B;
+    return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+        return launch_rows<GrpoRow<true, false>>(t, a, a.rows, a.rows, out3, workspace_bytes, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200rl_rloo_fwd_grad(int dtype, const void* logit_new, const void* logit_old, const long long* action,
@@ -868,8 +868,10 @@ extern "C" int b200rl_rloo_fwd_grad(int dtype, const void* logit_new, const void
     a.lse = lse_new; a.coef = dlogp_unit; a.grad = grad_logit_new; a.ws = workspace;
     a.rows = B * S; a.S = S; a.V = V;
     a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio);
-    a.inv_b = (float)(1.0 / (double)B);
-    return launch_dtype<VM_RLOO>(dtype, a, out3, workspace_bytes, B, (cudaStream_t)stream);
+    a.inv_b = (float)(1.0 / (double)B); a.nb = B;
+    return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+        return launch_rows<GrpoRow<false, false>>(t, a, a.rows, a.rows, out3, workspace_bytes, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200rl_ppo_lm_fwd_grad(int dtype, const void* logit_new, const void* logit_old,
@@ -895,14 +897,9 @@ extern "C" int b200rl_ppo_lm_fwd_grad(int dtype, const void* logit_new, const vo
     a.rows = rows; a.S = 1; a.V = V;
     a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio); a.dual_clip = (float)dual_clip;
     a.kl_type = kl_type; a.inv_m = (float)(1.0 / (double)rows);
-    cudaStream_t st = (cudaStream_t)stream;
-    const int mode = VM_PPO + (entropy ? PPO_ENT : 0) + (kl ? PPO_KL : 0);
-    switch (mode) {
-        case VM_PPO: return launch_dtype<VM_PPO>(dtype, a, out5, workspace_bytes, rows, st);
-        case VM_PPO + PPO_ENT: return launch_dtype<VM_PPO + PPO_ENT>(dtype, a, out5, workspace_bytes, rows, st);
-        case VM_PPO + PPO_KL: return launch_dtype<VM_PPO + PPO_KL>(dtype, a, out5, workspace_bytes, rows, st);
-        default: return launch_dtype<VM_PPO + PPO_ENT + PPO_KL>(dtype, a, out5, workspace_bytes, rows, st);
-    }
+    return with_vocab(dtype, entropy != 0, kl, [&](auto t, auto ent, auto k) {
+        return launch_rows<PpoRow<ent, k, false>>(t, a, rows, rows, out5, workspace_bytes, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200rl_ppo_lm_bwd(int dtype, const void* logit_new, const long long* action, const float* weight,
@@ -921,9 +918,9 @@ extern "C" int b200rl_ppo_lm_bwd(int dtype, const void* logit_new, const long lo
     a.grad = grad_logit_new;
     a.rows = rows; a.S = 1; a.V = V;
     a.inv_m = (float)(1.0 / (double)rows);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (entropy_row) return launch_dtype<VM_PPO_BWD + PPO_ENT>(dtype, a, nullptr, 0, rows, st);
-    return launch_dtype<VM_PPO_BWD>(dtype, a, nullptr, 0, rows, st);
+    return with_vocab(dtype, entropy_row != nullptr, false, [&](auto t, auto ent, auto) {
+        return launch_rows<PgBwdRow<ent, false>>(t, a, rows, rows, nullptr, 0, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200rl_a2c_lm_fwd_grad(int dtype, const void* logit, const long long* action, const float* value,
@@ -944,7 +941,9 @@ extern "C" int b200rl_a2c_lm_fwd_grad(int dtype, const void* logit, const long l
     a.rec = forward_record(g_expected, g_used);
     a.rows = rows; a.S = 1; a.V = V;
     a.inv_m = (float)(1.0 / (double)rows);
-    return launch_dtype<VM_A2C>(dtype, a, out3, workspace_bytes, rows, (cudaStream_t)stream);
+    return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+        return launch_rows<A2cRow<false>>(t, a, rows, rows, out3, workspace_bytes, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200rl_a2c_lm_bwd(int dtype, const void* logit, const long long* action, const float* weight,
@@ -964,7 +963,9 @@ extern "C" int b200rl_a2c_lm_bwd(int dtype, const void* logit, const long long* 
     a.grad = grad_logit; a.grad_value = grad_value;
     a.rows = rows; a.S = 1; a.V = V;
     a.inv_m = (float)(1.0 / (double)rows);
-    return launch_dtype<VM_PPO_BWD + PPO_ENT + PPO_VAL>(dtype, a, nullptr, 0, rows, (cudaStream_t)stream);
+    return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+        return launch_rows<PgBwdRow<true, true>>(t, a, rows, rows, nullptr, 0, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200rl_token_logp_fwd(int dtype, const void* logits, const long long* index, long long rows, long long V,
@@ -973,7 +974,9 @@ extern "C" int b200rl_token_logp_fwd(int dtype, const void* logits, const long l
     VocabArgs a{};
     a.x[0] = logits; a.action = index; a.lp = logp; a.lse = lse;
     a.rows = rows; a.S = 1; a.V = V;
-    return launch_dtype<VM_LOGP>(dtype, a, nullptr, 0, rows, (cudaStream_t)stream);
+    return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+        return launch_rows<LogpRow>(t, a, rows, rows, nullptr, 0, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200rl_token_logp_bwd(int dtype, const void* logits, const long long* index, const float* lse,
@@ -986,7 +989,9 @@ extern "C" int b200rl_token_logp_bwd(int dtype, const void* logits, const long l
     a.x[0] = logits; a.action = index; a.lse = const_cast<float*>(lse); a.coef_in = dlogp; a.g = g_scale;
     a.skip_if_unit = skip_if_unit; a.grad = grad_logits;
     a.rows = rows; a.S = 1; a.V = V;
-    return launch_dtype<VM_BWD>(dtype, a, nullptr, 0, rows, (cudaStream_t)stream);
+    return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+        return launch_rows<CoefBwdRow>(t, a, rows, rows, nullptr, 0, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200rl_token_head_fwd(const float* logp_new, const float* logp_old, const float* logp_ref,
@@ -1042,7 +1047,8 @@ extern "C" int b200rl_lm_linear_fwd(int mode, int dtype, void* logits, long long
     if (mode == B200RL_LM_LOGP) {
         if (!logp) return B200RL_ERR_ARG;
         a.lp = logp + row0;
-        return launch_dtype<VM_LOGP>(dtype, a, nullptr, 0, rows, st);
+        return with_vocab(dtype, false, false,
+                          [&](auto t, auto, auto) { return launch_rows<LogpRow>(t, a, rows, rows, nullptr, 0, st); });
     }
     const bool grpo = mode == B200RL_LM_GRPO;
     if ((!grpo && mode != B200RL_LM_RLOO) || !logp_old || !seq || !out3 || !workspace ||
@@ -1061,11 +1067,9 @@ extern "C" int b200rl_lm_linear_fwd(int mode, int dtype, void* logits, long long
     a.grad = want_grad ? logits : nullptr;
     a.lo = (float)(1.0 - clip_ratio); a.hi = (float)(1.0 + clip_ratio); a.beta = grpo ? (float)beta : 0.f;
     a.inv_b = (float)(1.0 / (double)B);
-    if (dtype == B200RL_DTYPE_F32)
-        return grpo ? launch_lin<float, VM_GRPO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st)
-                    : launch_lin<float, VM_RLOO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st);
-    return grpo ? launch_lin<__nv_bfloat16, VM_GRPO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st)
-                : launch_lin<__nv_bfloat16, VM_RLOO_LIN>(a, chunk_rows, B, out3, workspace_bytes, st);
+    return with_vocab(dtype, false, grpo, [&](auto t, auto, auto k) {
+        return launch_rows<GrpoRow<k, true>>(t, a, chunk_rows, N, out3, workspace_bytes, st);
+    });
 }
 
 // PPO / A2C from the lm_head's hidden states, one chunk of token rows per call (ding/rl_utils/ppo.py:143-230 with
@@ -1099,15 +1103,13 @@ extern "C" int b200rl_lm_linear_pg_fwd(int mode, int dtype, void* logits, long l
     a.kl_type = kl_type; a.inv_m = (float)(1.0 / (double)N);
     a.w_ent = (float)w_ent; a.w_kl = (float)w_kl; a.w_val = (float)w_val;
     cudaStream_t st = (cudaStream_t)stream;
-    if (!ppo) return launch_lin_dtype<VM_A2C_LIN>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
-    switch (VM_PPO_LIN + (entropy ? PPO_ENT : 0) + (kl ? PPO_KL : 0)) {
-        case VM_PPO_LIN: return launch_lin_dtype<VM_PPO_LIN>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
-        case VM_PPO_LIN + PPO_ENT:
-            return launch_lin_dtype<VM_PPO_LIN + PPO_ENT>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
-        case VM_PPO_LIN + PPO_KL:
-            return launch_lin_dtype<VM_PPO_LIN + PPO_KL>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
-        default: return launch_lin_dtype<VM_PPO_LIN + PPO_ENT + PPO_KL>(dtype, a, chunk_rows, N, out, workspace_bytes, st);
-    }
+    if (!ppo)
+        return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+            return launch_rows<A2cRow<true>>(t, a, chunk_rows, N, out, workspace_bytes, st);
+        });
+    return with_vocab(dtype, entropy != 0, kl, [&](auto t, auto ent, auto k) {
+        return launch_rows<PpoRow<ent, k, true>>(t, a, chunk_rows, N, out, workspace_bytes, st);
+    });
 }
 
 // The backward of token_logp_linear on one chunk, in place (log_prob_utils.py:29-48's autograd, as b200rl_token_logp_bwd)
@@ -1118,23 +1120,20 @@ extern "C" int b200rl_lm_linear_bwd(int dtype, void* logits, long long row0, lon
     a.x[0] = logits; a.grad = logits;
     a.action = index + row0; a.lse = const_cast<float*>(lse + row0); a.coef_in = dlogp + row0;
     a.rows = rows; a.S = 1; a.V = V;
-    return launch_dtype<VM_BWD>(dtype, a, nullptr, 0, rows, (cudaStream_t)stream);
+    return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+        return launch_rows<CoefBwdRow>(t, a, rows, rows, nullptr, 0, (cudaStream_t)stream);
+    });
 }
 
 extern "C" int b200rl_lm_linear_scale(int dtype, const float* g, void* x, long long n, void* stream) {
     if (n < 0 || !g || (n > 0 && (!x || !aligned16(x)))) return B200RL_ERR_ARG;
     if (n == 0) return B200RL_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    int sms = 0, per_sm = 0;
-    if (dtype == B200RL_DTYPE_F32) {
-        if (int rc = resident_ctas<scale_inplace_kernel<float>>(256, 0, sms, per_sm)) return rc;
-        const long long grid = min((long long)sms * per_sm, (n / 4 + 255) / 256 + 1);
-        return launch_k(scale_inplace_kernel<float>, (int)grid, 256, 0, st, g, (float*)x, n);
-    }
-    if (dtype == B200RL_DTYPE_BF16) {
-        if (int rc = resident_ctas<scale_inplace_kernel<__nv_bfloat16>>(256, 0, sms, per_sm)) return rc;
-        const long long grid = min((long long)sms * per_sm, (n / 8 + 255) / 256 + 1);
-        return launch_k(scale_inplace_kernel<__nv_bfloat16>, (int)grid, 256, 0, st, g, (__nv_bfloat16*)x, n);
-    }
-    return B200RL_ERR_ARG;
+    return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+        using T = decltype(t);
+        int sms = 0, per_sm = 0;
+        if (int rc = resident_ctas<scale_inplace_kernel<T>>(256, 0, sms, per_sm)) return rc;
+        const long long grid = min((long long)sms * per_sm, (n / VecT<T>::W + 255) / 256 + 1);
+        return launch_k(scale_inplace_kernel<T>, (int)grid, 256, 0, st, g, (T*)x, n);
+    });
 }

@@ -1,12 +1,12 @@
 """The vocabulary-scale kernels of csrc/vocab.cu against a float64 reference, on token rows where an online softmax goes
 wrong.
 
-Kernels: ``vocab_rows_kernel<T, MODE>`` for fp32 and bf16 logits -- grpo_policy_error, rloo_policy_error (forward with
-and without the cached row, VM_BWD), the three log-prob methods (VM_LOGP, VM_BWD) and language-model ppo_policy_error
-(VM_PPO + entropy / KL flags, VM_PPO_BWD), language-model a2c_error (VM_A2C, backward VM_PPO_BWD + PPO_ENT + PPO_VAL,
-on the regimes without an old policy, returns at 1e3 with a 1e-2 spread, value == return and adv = 0, each mix from the
-record with the forward's gradient buffers poisoned: a mix that differs only in the value slot keeps d logit and
-rewrites d value) -- and ``token_head_kernel`` (a custom log_prob_fn).
+Kernels: ``vocab_rows_kernel<T, Head>`` for fp32 and bf16 logits -- grpo_policy_error, rloo_policy_error (GrpoRow with
+and without the cached row, CoefBwdRow), the three log-prob methods (LogpRow, CoefBwdRow) and language-model
+ppo_policy_error (PpoRow with its entropy / KL flags, PgBwdRow), language-model a2c_error (A2cRow, backward PgBwdRow with
+the value slot, on the regimes without an old policy, returns at 1e3 with a 1e-2 spread, value == return and adv = 0,
+each mix from the record with the forward's gradient buffers poisoned: a mix that differs only in the value slot keeps
+d logit and rewrites d value) -- and ``token_head_kernel`` (a custom log_prob_fn).
 
 The seeded parity cases of test_grpo_rloo.py / test_ppo_lm.py draw ``logit_old = new + 0.1 randn`` and logit scales of
 1..4: almost no ratio leaves the clip band.  Here every token row draws one regime, in equal shares: ``plain`` (those
@@ -596,7 +596,7 @@ def test_ppo_lm_fp64(name):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# the log-prob methods (VM_LOGP, VM_BWD with a per-row upstream)
+# the log-prob methods (LogpRow, CoefBwdRow with a per-row upstream)
 # ----------------------------------------------------------------------------------------------------------------
 LP_CASES = OrderedDict(
     [('f32_v%d_r%d' % (V, r), (F32, r, V)) for V, r in ((1, 16384), (3, 4099), (1027, 529), (2048, 133), (4100, 132),
@@ -730,7 +730,7 @@ def test_token_head_fp64(S, kind):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# A2C on token rows (VM_A2C, backward VM_PPO_BWD + PPO_ENT + PPO_VAL) and its upstream-gradient record
+# A2C on token rows (A2cRow, backward PgBwdRow with the value slot) and its upstream-gradient record
 # ----------------------------------------------------------------------------------------------------------------
 A2C_NAMES = ('plain', 'shift', 'peaked', 'flat', 'masked', 'large')  # the regimes without an old policy
 A2C_CASES = {
