@@ -87,6 +87,7 @@ PROTOTYPES = {
     "b200rl_lm_linear_fwd": [I, I, P, LL, LL, LL, LL, LL, LL, P, P, P, P, P, LL, P, P, D, D, P, P, P, I, P, c_size_t, P],
     "b200rl_lm_linear_bwd": [I, P, LL, LL, LL, P, P, P, P],
     "b200rl_lm_linear_scale": [I, P, P, LL, P],
+    "b200rl_lm_linear_scale_out": [I, P, P, P, LL, P],
     "b200rl_lm_linear_pg_fwd": [I, I, P, LL, LL, LL, LL, LL, P, P, P, P, P, P, P, D, D, I, I, D, D, D, P, P, I, P,
                                 c_size_t, P],
     "b200rl_gae_ppo_set_impl": [I],

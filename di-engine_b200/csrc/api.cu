@@ -79,7 +79,7 @@ void chain_report(cudaStream_t st, const ChainPoint& at, bool starts, const Byte
 }
 }  // namespace b200rl
 
-extern "C" int b200rl_version(void) { return 114; }
+extern "C" int b200rl_version(void) { return 115; }
 extern "C" int b200rl_built_for_sm(void) { return 90; }
 extern "C" size_t b200rl_workspace_bytes(void) { return (size_t)WS_MIN_BYTES; }
 

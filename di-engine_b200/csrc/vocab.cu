@@ -776,6 +776,34 @@ __global__ void __launch_bounds__(256) scale_inplace_kernel(const float* __restr
     for (long long i = nv * W + t0; i < n; i += step) x[i] = V_::from_f(s * V_::to_f(x[i]));
 }
 
+// out = *g * in, in T, always written: the out-of-place form of scale_inplace_kernel for a backward that may not hand
+// back the buffer its forward wrote (a torch.library op).  Same bits: s * v rounded to T, and in's bits when *g == 1.
+template <class T>
+__global__ void __launch_bounds__(256) scale_out_kernel(const float* __restrict__ g, const T* __restrict__ in,
+                                                        T* __restrict__ out, long long n) {
+    pdl_prologue();
+    using V_ = VecT<T>;
+    constexpr int W = V_::W;
+    const float s = *g;
+    const long long nv = n / W, step = (long long)gridDim.x * blockDim.x;
+    const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint4* iv = reinterpret_cast<const uint4*>(in);
+    uint4* ov = reinterpret_cast<uint4*>(out);
+    if (s == 1.f) {
+        for (long long i = t0; i < nv; i += step) ov[i] = iv[i];
+        for (long long i = nv * W + t0; i < n; i += step) out[i] = in[i];
+        return;
+    }
+    for (long long i = t0; i < nv; i += step) {
+        float v[W];
+        V_::unpack(iv[i], v);
+#pragma unroll
+        for (int k = 0; k < W; ++k) v[k] = s * v[k];
+        ov[i] = V_::pack(v);
+    }
+    for (long long i = nv * W + t0; i < n; i += step) out[i] = V_::from_f(s * V_::to_f(in[i]));
+}
+
 }  // namespace b200rl
 
 using namespace b200rl;
@@ -1135,5 +1163,19 @@ extern "C" int b200rl_lm_linear_scale(int dtype, const float* g, void* x, long l
         if (int rc = resident_ctas<scale_inplace_kernel<T>>(256, 0, sms, per_sm)) return rc;
         const long long grid = min((long long)sms * per_sm, (n / VecT<T>::W + 255) / 256 + 1);
         return launch_k(scale_inplace_kernel<T>, (int)grid, 256, 0, st, g, (T*)x, n);
+    });
+}
+
+extern "C" int b200rl_lm_linear_scale_out(int dtype, const float* g, const void* in, void* out, long long n,
+                                          void* stream) {
+    if (n < 0 || !g || (n > 0 && (!in || !out || !aligned16(in) || !aligned16(out)))) return B200RL_ERR_ARG;
+    if (n == 0) return B200RL_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    return with_vocab(dtype, false, false, [&](auto t, auto, auto) {
+        using T = decltype(t);
+        int sms = 0, per_sm = 0;
+        if (int rc = resident_ctas<scale_out_kernel<T>>(256, 0, sms, per_sm)) return rc;
+        const long long grid = min((long long)sms * per_sm, (n / VecT<T>::W + 255) / 256 + 1);
+        return launch_k(scale_out_kernel<T>, (int)grid, 256, 0, st, g, (const T*)in, (T*)out, n);
     });
 }

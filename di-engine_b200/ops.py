@@ -2217,6 +2217,18 @@ def lm_scale_(dt, pg, x):
     return x
 
 
+def lm_scale_out_(dt, pg, x):
+    """*pg * x into a fresh tensor, the bits of ``lm_scale_`` (x's own when *pg == 1): the backward op of the hidden-state
+    losses under torch.compile, which may not hand back the buffer its forward op wrote.  The kernel reads x.numel()
+    values from x's address, so a strided view is made contiguous first."""
+    x = x.contiguous()
+    out = torch.empty_like(x)
+    with on_device(x.device):
+        rc = lib().b200rl_lm_linear_scale_out(dt, pg, ptr(x), ptr(out), x.numel(), stream_ptr())
+    _lib.check(rc, 'b200rl_lm_linear_scale_out')
+    return out
+
+
 def _lm_backward(ctx, g_loss, recompute):
     """The backward of the hidden-state losses: the gradients their forward wrote for a unit upstream gradient of the one
     loss (``ctx.spec``; dH, dW and, for A2C, d value), scaled in place by ``g_loss`` on the device (a no-op when it is 1).

@@ -22,14 +22,23 @@ These are composites, not names of ding.rl_utils:
   reaches ``value``.
 
 ``weight`` is the reference's per-token mask.  ``logp_old``, ``logp_ref``, ``logp_pretrained``, ``adv``, ``reward``,
-``return_``, ``value`` and ``weight`` of any float dtype are read as fp32.  Under ``torch.compile`` these functions run
-eagerly behind a graph break.
+``return_``, ``value`` and ``weight`` of any float dtype are read as fp32.
+
+Under ``torch.compile`` each call traces as one ``b200rl`` custom op (torch_ops.py) whose body is the same chunk loop, so a
+learner step that ends in one of these losses compiles with ``fullgraph=True``.  The gradient rule is eager's: the forward
+op writes dH / dW / d value for a unit upstream gradient, and the backward op scales them by the actual one -- out of place,
+since a backward op may not return its forward's buffer (same bits as the in-place scale).  So during the backward the
+saved and the scaled dW coexist: 2 x 1.09 GB at Qwen2-7B's lm_head in bf16, below the forward's own peak (the fp32
+accumulator plus the rounded dW); in fp32, where eager's dW is the accumulator itself, the backward holds one (V, D)
+fp32 copy more than eager's, which at D = 4096, V = 32 768 still stayed below the forward's peak (README).  A
+repeated backward rescales the saved unit gradients instead of recomputing them.  ``token_logp_linear``'s backward op
+recomputes each chunk's logits, as in eager mode.
 
 PPO and A2C return their loss mix as one differentiable ``loss`` -- ``policy_loss - entropy_weight * entropy_loss +
 kl_weight * kl_div``, or ``policy_loss + value_weight * value_loss - entropy_weight * entropy_loss`` -- and the components
 as detached 0-dim tensors for logging, rather than three separately differentiable outputs.  The forward writes dH / dW
-(and A2C's d value) for a unit upstream gradient of ``loss``, and the backward scales them in place on the device; a
-repeated backward recomputes them.  Any other mix of the components would need the logits again, which are gone after
+(and A2C's d value) for a unit upstream gradient of ``loss``, and the backward scales them in place on the device; in
+eager mode a repeated backward recomputes them.  Any other mix of the components would need the logits again, which are gone after
 each chunk's dW GEMM: dW = sum over chunks of dZ^T H cannot be re-weighted afterwards without one (V, D) fp32
 accumulator per component (2.2 GB each at Qwen2-7B's lm_head), or a host read of the upstream gradients (a sync in the
 backward).  So the weights of the mix are arguments.  A learner that wants ``ppo_error`` adds ``ppo_value_error`` on its
@@ -39,7 +48,7 @@ from typing import Optional, Tuple
 
 import torch
 
-from .. import ops
+from .. import ops, torch_ops
 from . import _lm_policy
 from . import ppo as _ppo
 from .grpo import grpo_info
@@ -79,7 +88,6 @@ def _wants_grad(h, w):
     return torch.is_grad_enabled() and (h.requires_grad or w.requires_grad)
 
 
-@torch.compiler.disable
 def token_logp_linear(hidden: torch.Tensor, lm_weight: torch.Tensor, index: torch.Tensor) -> torch.Tensor:
     """log softmax(hidden @ lm_weight^T)[index]: hidden (B, S, D), lm_weight (V, D), index (B, S) -> fp32 (B, S),
     differentiable w.r.t. hidden and lm_weight."""
@@ -92,7 +100,9 @@ def token_logp_linear(hidden: torch.Tensor, lm_weight: torch.Tensor, index: torc
     host_out = not hidden.is_cuda
     h, w = _stage(hidden, lm_weight, dev)
     a = ops.i64c(ops.to_device(index, dev), V, 'index').reshape(-1)
-    if _wants_grad(h, w):
+    if torch.compiler.is_compiling():
+        lp = torch_ops.lm_logp(h, w, a, dt)[0]
+    elif _wants_grad(h, w):
         lp = ops.TokenLogpLinearFunction.apply(h, w, a, dt)
     else:
         lp = ops.lm_logp_fwd_(h.detach(), w.detach(), a, dt)[0]
@@ -120,6 +130,15 @@ def _run(kind, hidden, lm_weight, lps, action, weight, side, clip_ratio, beta, i
     a = ops.i64c(ops.to_device(action, dev), V).reshape(-1)
     h, wt = _stage(hidden, lm_weight, dev)
     cfg = (kind, B, S, dt, float(clip_ratio), float(beta))
+    if torch.compiler.is_compiling():
+        grad = torch.is_grad_enabled()
+        out = torch_ops.lm_linear_loss(h, wt, a, lp[0], lp_ref, side_t, w, *cfg, grad and h.requires_grad,
+                                       grad and wt.requires_grad)[0]
+        loss, kl, cf = out[0], out[1].detach(), out[2].detach()
+        if host_out:
+            loss = loss.cpu()
+        # the monitors as the logit-form losses return them under compile
+        return loss, info_type(kl, cf) if _ppo.LAZY_INFO else info_type(kl.item(), cf.item())
     if _wants_grad(h, wt):
         loss, kl, cf = ops.LMLinearLossFunction.apply(h, wt, a, lp[0], lp_ref, side_t, w, *cfg)
     else:
@@ -133,7 +152,6 @@ def _run(kind, hidden, lm_weight, lps, action, weight, side, clip_ratio, beta, i
     return loss, info_type(kl, cf)
 
 
-@torch.compiler.disable
 def grpo_policy_error_linear(data: namedtuple, clip_ratio: float = 0.2, beta: float = 0.1) -> Tuple[torch.Tensor, namedtuple]:
     """``grpo_policy_error`` (rl_utils/grpo.py) on logits = hidden @ lm_weight^T, computed chunk by chunk.  data =
     grpo_linear_data(hidden (B, S, D), lm_weight (V, D), logp_old (B, S), logp_ref (B, S), action (B, S), adv (B),
@@ -142,7 +160,6 @@ def grpo_policy_error_linear(data: namedtuple, clip_ratio: float = 0.2, beta: fl
                 ('adv', data.adv), clip_ratio, beta, grpo_info)
 
 
-@torch.compiler.disable
 def rloo_policy_error_linear(data: namedtuple, clip_ratio: float = 0.2) -> Tuple[torch.Tensor, namedtuple]:
     """``rloo_policy_error`` (rl_utils/rloo.py) on logits = hidden @ lm_weight^T, computed chunk by chunk.  data =
     rloo_linear_data(hidden (B, S, D), lm_weight (V, D), logp_old (B, S), action (B, S), reward (K, B / K), weight
@@ -169,7 +186,11 @@ def _run_pg(kind, hidden, lm_weight, action, weight, rows, value, cfg):
     a = ops.i64c(ops.to_device(action, dev), V).reshape(-1)
     h, wt = _stage(hidden, lm_weight, dev)
     args = (a, f['adv'], w, f.get('logp_old'), f.get('logp_pretrained'), f.get('return_'), kind, dt, cfg)
-    if torch.is_grad_enabled() and (h.requires_grad or wt.requires_grad or (v is not None and v.requires_grad)):
+    grad = torch.is_grad_enabled()
+    if torch.compiler.is_compiling():
+        loss, out = torch_ops.lm_linear_pg(h, wt, v, *args[:-1], *cfg, grad and h.requires_grad,
+                                           grad and wt.requires_grad, grad and v is not None and v.requires_grad)[:2]
+    elif grad and (h.requires_grad or wt.requires_grad or (v is not None and v.requires_grad)):
         loss, out = ops.LMLinearPGFunction.apply(h, wt, v, *args)
     else:
         out = ops.lm_linear_pg_(h.detach(), wt.detach(), a, f['adv'], w, f.get('logp_old'), f.get('logp_pretrained'),
@@ -181,7 +202,6 @@ def _run_pg(kind, hidden, lm_weight, action, weight, rows, value, cfg):
     return loss, out
 
 
-@torch.compiler.disable
 def ppo_policy_error_linear(data: namedtuple, clip_ratio: float = 0.2, dual_clip: Optional[float] = None,
                             entropy_bonus: bool = True, kl_type: str = 'k1', entropy_weight: float = 0.0,
                             kl_weight: float = 0.0) -> Tuple[namedtuple, namedtuple]:
@@ -207,13 +227,14 @@ def ppo_policy_error_linear(data: namedtuple, clip_ratio: float = 0.2, dual_clip
                         {'adv': adv, 'logp_old': logp_old, 'logp_pretrained': logp_pre}, None, cfg)
     if _ppo.LAZY_INFO:
         info = ppo_info(out[3], out[4])
+    elif torch.compiler.is_compiling():  # the logit-form losses' host read under compile
+        info = ppo_info(out[3].item(), out[4].item())
     else:
         approx_kl, clipfrac = out[3:5].tolist()  # one host sync
         info = ppo_info(approx_kl, clipfrac)
     return ppo_linear_loss(loss, out[0], out[1], out[2]), info
 
 
-@torch.compiler.disable
 def a2c_error_linear(data: namedtuple, value_weight: float = 0.5, entropy_weight: float = 0.01) -> namedtuple:
     """``a2c_error`` (rl_utils/a2c.py) on logits = hidden @ lm_weight^T, computed chunk by chunk.  data =
     a2c_linear_data(hidden (B, S, D), lm_weight (V, D), action (B, S), value (B, S), adv (B, S), return_ (B, S), weight

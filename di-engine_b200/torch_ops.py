@@ -6,8 +6,9 @@ ppo_error / a2c_error on token rows, ppo_value_error), the advantage recomputes 
 normalize_advantage, ppo_error_adv_norm), symlog / inv_symlog, the quantile TD losses (QR-DQN, IQN, FQF) and the
 continuous-action PPO losses, COMA's loss, ScatterConnection, the value-based losses of DQfD / R2D3 (dqfd_nstep_td_error,
 its _with_rescale and _sequence forms), M-DQN, SQL and discrete SAC (m_q_1step_td_error, q_nstep_sql_td_error,
-q_v_1step_td_error), the R2D2 / NGU loop q_nstep_td_error_sequence and FQF's fraction loss without a graph break, and
-``mode="reduce-overhead"`` can replay a compiled learner step as a CUDA graph.
+q_v_1step_td_error), the R2D2 / NGU loop q_nstep_td_error_sequence, FQF's fraction loss and the language-model losses
+from the lm_head's hidden states (grpo / rloo / ppo_policy_error_linear, a2c_error_linear, token_logp_linear) without a
+graph break, and ``mode="reduce-overhead"`` can replay a compiled learner step as a CUDA graph.
 
 Each op's implementation is the launch function ``ops`` runs in eager mode; ``rl_utils`` calls the wrappers at the bottom
 of this module only while ``torch.compiler.is_compiling()``.  The schemas hold tensors and scalars only: the workspace, the
@@ -17,7 +18,9 @@ The forward-written gradients work as in eager mode, with one difference that fu
 not return its input, so after a forward launch that wrote the gradients the backward op copies them once and runs the
 verify launch on the copy (recomputing on the device when the upstream gradients differ from the record, no host sync).
 At vocabulary scale that copy would cost as much as the loss: the language-model ops write no gradient in the forward op
-and recompute it in the backward op from the saved per-row values, at the price of one more read of logit_new.
+and recompute it in the backward op from the saved per-row values, at the price of one more read of logit_new.  The
+hidden-state losses keep eager's rule instead, since recomputing there would repeat the logit GEMMs: their forward op
+writes dH / dW for a unit upstream gradient and the backward op scales them into fresh buffers.
 """
 from typing import Optional
 
@@ -870,6 +873,148 @@ def _a2c_lm_backward(ctx, g_out, _g_per_row):
 
 
 a2c_lm_fwd.register_autograd(_a2c_lm_backward, setup_context=_a2c_lm_setup)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# The language-model losses from the lm_head's hidden states (rl_utils/lm_linear.py): the op's body is eager's whole chunk
+# loop (ops.lm_chunks_: logit GEMM, in-place row launch, dH / dW GEMMs), so the compiler sees one opaque op per call.  Here
+# the GEMMs are the cost, so the gradient is not recomputed: as in eager mode the forward op writes dH / dW (and A2C's
+# d value) for a unit upstream gradient, each only when ``want_*`` says so, and the backward op scales them out of place
+# (b200rl_lm_linear_scale_out, the bits of eager's in-place scale; A2C's fp32 d value through ``scale``).  A repeated
+# backward rescales the same saved unit gradients.  Not wanted, a gradient output is an empty tensor.
+# ---------------------------------------------------------------------------------------------------------------------
+def _or_empty(x, like):
+    return x if x is not None else _empty(like)
+
+
+@torch.library.custom_op('b200rl::lm_linear_loss', mutates_args=())
+def lm_linear_loss(hidden: Tensor, lm_weight: Tensor, action: Tensor, lp_old: Tensor, lp_ref: Optional[Tensor],
+                   side: Tensor, weight: Optional[Tensor], kind: str, B: int, S: int, dt: int, clip_ratio: float,
+                   beta: float, want_dh: bool, want_dw: bool) -> tuple[Tensor, Tensor, Tensor]:
+    """grpo / rloo_policy_error_linear on hidden (N, D), lm_weight (V, D) -> (loss / approx_kl / clipfrac, dH, dW)"""
+    out, dh, dw = ops.lm_linear_loss_(hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt, clip_ratio,
+                                      beta, want_dh, want_dw)
+    return out, _or_empty(dh, hidden), _or_empty(dw, lm_weight)
+
+
+@lm_linear_loss.register_fake
+def _(hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt, clip_ratio, beta, want_dh, want_dw):
+    return (_f32(hidden, 3), torch.empty_like(hidden) if want_dh else _empty(hidden),
+            torch.empty_like(lm_weight) if want_dw else _empty(lm_weight))
+
+
+@torch.library.custom_op('b200rl::lm_linear_pg', mutates_args=())
+def lm_linear_pg(hidden: Tensor, lm_weight: Tensor, value: Optional[Tensor], action: Tensor, adv: Tensor,
+                 weight: Optional[Tensor], lp_old: Optional[Tensor], lp_pre: Optional[Tensor], ret: Optional[Tensor],
+                 kind: str, dt: int, clip_ratio: float, dual_clip: float, kl_type: int, entropy: bool, w_ent: float,
+                 w_kl: float, w_val: float, want_dh: bool, want_dw: bool,
+                 want_dv: bool) -> tuple[Tensor, Tensor, Tensor, Tensor, Tensor]:
+    """ppo_policy_error_linear / a2c_error_linear -> (the one loss, the raw sums (PPO 5, A2C 3), dH, dW, d value (N)
+    fp32); the loss is eager's ``ops.lm_pg_loss_`` of the sums"""
+    cfg = (clip_ratio, dual_clip, kl_type, entropy, w_ent, w_kl, w_val)
+    out, dh, dw, dv = ops.lm_linear_pg_(hidden, lm_weight, action, adv, weight, lp_old, lp_pre, value, ret, kind, dt, cfg,
+                                        want_dh, want_dw, want_dv)
+    return ops.lm_pg_loss_(out, kind, cfg), out, _or_empty(dh, hidden), _or_empty(dw, lm_weight), _or_empty(dv, out)
+
+
+@lm_linear_pg.register_fake
+def _(hidden, lm_weight, value, action, adv, weight, lp_old, lp_pre, ret, kind, dt, clip_ratio, dual_clip, kl_type,
+      entropy, w_ent, w_kl, w_val, want_dh, want_dw, want_dv):
+    return (_f32(hidden, ()), _f32(hidden, 5 if kind == 'ppo' else 3),
+            torch.empty_like(hidden) if want_dh else _empty(hidden),
+            torch.empty_like(lm_weight) if want_dw else _empty(lm_weight), _f32(hidden, hidden.shape[0] if want_dv else 0))
+
+
+@torch.library.custom_op('b200rl::lm_linear_scale_out', mutates_args=())
+def lm_linear_scale_out(g: Tensor, x: Tensor) -> Tensor:
+    """``g * x`` into a fresh contiguous tensor of x's shape and dtype (fp32 or bf16, any layout) for a one-element
+    upstream gradient ``g``"""
+    kg, pg = _one(g)
+    return ops.lm_scale_out_(ops.logit_dtype(x), pg, x)
+
+
+@lm_linear_scale_out.register_fake
+def _(g, x):
+    return x.new_empty(x.shape)
+
+
+def _lm_linear_loss_setup(ctx, inputs, output):
+    ctx.save_for_backward(output[1], output[2])
+    ctx.want = inputs[13:15]
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(output[1], output[2])
+
+
+def _lm_linear_loss_backward(ctx, g_out, _g_dh, _g_dw):
+    if g_out is None:
+        return (None, ) * 15
+    dh, dw = ctx.saved_tensors
+    g = g_out[:1]  # the loss's; approx_kl and clipfrac leave the wrapper detached
+    return (lm_linear_scale_out(g, dh) if ctx.want[0] else None,
+            lm_linear_scale_out(g, dw) if ctx.want[1] else None) + (None, ) * 13
+
+
+lm_linear_loss.register_autograd(_lm_linear_loss_backward, setup_context=_lm_linear_loss_setup)
+
+
+def _lm_linear_pg_setup(ctx, inputs, output):
+    ctx.save_for_backward(*output[2:])
+    ctx.want = inputs[18:21]
+    ctx.set_materialize_grads(False)
+    ctx.mark_non_differentiable(*output[1:])
+
+
+def _lm_linear_pg_backward(ctx, g_loss, *_):
+    if g_loss is None:
+        return (None, ) * 21
+    dh, dw, dv = ctx.saved_tensors
+    want_dh, want_dw, want_dv = ctx.want
+    return (lm_linear_scale_out(g_loss, dh) if want_dh else None, lm_linear_scale_out(g_loss, dw) if want_dw else None,
+            scale(g_loss, dv) if want_dv else None) + (None, ) * 18
+
+
+lm_linear_pg.register_autograd(_lm_linear_pg_backward, setup_context=_lm_linear_pg_setup)
+
+
+@torch.library.custom_op('b200rl::lm_logp', mutates_args=())
+def lm_logp(hidden: Tensor, lm_weight: Tensor, index: Tensor, dt: int) -> tuple[Tensor, Tensor]:
+    """token_logp_linear -> (log p(index), logsumexp), fp32 per token row"""
+    return ops.lm_logp_fwd_(hidden, lm_weight, index, dt)
+
+
+@lm_logp.register_fake
+def _(hidden, lm_weight, index, dt):
+    return _f32(hidden, hidden.shape[0]), _f32(hidden, hidden.shape[0])
+
+
+@torch.library.custom_op('b200rl::lm_logp_bwd', mutates_args=())
+def lm_logp_bwd(hidden: Tensor, lm_weight: Tensor, index: Tensor, lse: Tensor, g: Tensor, dt: int, want_dh: bool,
+                want_dw: bool) -> tuple[Tensor, Tensor]:
+    """-> (dH, dW) for the upstream gradient g (N) of log p: per chunk the logit GEMM again, as in eager mode"""
+    dh, dw = ops.lm_logp_bwd_(hidden, lm_weight, index, lse, g.float().contiguous(), dt, want_dh, want_dw)
+    return _or_empty(dh, hidden), _or_empty(dw, lm_weight)
+
+
+@lm_logp_bwd.register_fake
+def _(hidden, lm_weight, index, lse, g, dt, want_dh, want_dw):
+    return (torch.empty_like(hidden) if want_dh else _empty(hidden),
+            torch.empty_like(lm_weight) if want_dw else _empty(lm_weight))
+
+
+def _lm_logp_setup(ctx, inputs, output):
+    ctx.save_for_backward(inputs[0], inputs[1], inputs[2], output[1])
+    ctx.dt = inputs[3]
+    ctx.mark_non_differentiable(output[1])
+
+
+def _lm_logp_backward(ctx, g, _g_lse):
+    hidden, lm_weight, index, lse = ctx.saved_tensors
+    want_dh, want_dw = ctx.needs_input_grad[:2]
+    dh, dw = lm_logp_bwd(hidden, lm_weight, index, lse, g, ctx.dt, want_dh, want_dw)
+    return dh if want_dh else None, dw if want_dw else None, None, None
+
+
+lm_logp.register_autograd(_lm_logp_backward, setup_context=_lm_logp_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

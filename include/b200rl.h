@@ -718,6 +718,9 @@ B200RL_API int b200rl_a2c_lm_bwd(int dtype, const void* logit, const long long* 
  *   the backward of mode B200RL_LM_LOGP on one recomputed chunk.
  * b200rl_lm_linear_scale: x (n values of dtype, 16-byte aligned) *= *g in place; returns at once on the device when
  *   *g == 1 -- the backward of the GRPO / RLOO / PPO / A2C forward's gradients.
+ * b200rl_lm_linear_scale_out: out = *g * in (n values of dtype, both 16-byte aligned), always written; the same bits as
+ *   b200rl_lm_linear_scale (in's own bits when *g == 1) -- the backward op under torch.compile, which may not return the
+ *   forward's buffer.
  * b200rl_lm_linear_pg_fwd: mode B200RL_LM_PPO (ding/rl_utils/ppo.py:143-230, calculate_kl_div :30-54) or B200RL_LM_A2C
  *   (a2c.py:10-44) on the chunk's rows of N = B*S tokens; M = N, every sum a plain mean over the N rows.  Per-token
  *   operands (N) fp32: action, adv, weight (nullable = ones); PPO: logp_old, logp_pre (nullable = no KL term); A2C: value,
@@ -742,6 +745,8 @@ B200RL_API int b200rl_lm_linear_fwd(int mode, int dtype, void* logits, long long
 B200RL_API int b200rl_lm_linear_bwd(int dtype, void* logits, long long row0, long long rows, long long V,
                          const long long* index, const float* lse, const float* dlogp, void* stream);
 B200RL_API int b200rl_lm_linear_scale(int dtype, const float* g, void* x, long long n, void* stream);
+B200RL_API int b200rl_lm_linear_scale_out(int dtype, const float* g, const void* in, void* out, long long n,
+                                          void* stream);
 B200RL_API int b200rl_lm_linear_pg_fwd(int mode, int dtype, void* logits, long long row0, long long rows,
                             long long chunk_rows, long long V, long long N, const long long* action,
                             const float* logp_old, const float* logp_pre, const float* adv, const float* value,
