@@ -25,7 +25,7 @@ def check_tokens(B, S, action, weight, side):
         raise RuntimeError("%s must hold B = %d values, got shape %s" % (side[0], B, tuple(side[1].shape)))
 
 
-def run(fn_fused, logits, action, weight, side, log_prob_fn, clip_ratio, beta, info_type):
+def run(logits, action, weight, side, log_prob_fn, clip_ratio, beta, info_type):
     """logits: (new, old[, ref]); side: ('adv', adv) or ('reward', reward (K, B / K)).  Returns (loss, info_type)."""
     logit_new = logits[0]
     dev = ops.compute_device(*logits)
@@ -48,31 +48,24 @@ def run(fn_fused, logits, action, weight, side, log_prob_fn, clip_ratio, beta, i
     side_t = ops.to_device(side[1].detach(), dev).float().contiguous()
     if side[0] == 'reward':
         side_t = side_t.reshape(side_t.shape[0], -1)
-    compiling = torch.compiler.is_compiling()
     if fused:
         dt = ops.logit_dtype(*logits)
-        # a traced tensor has no address: the custom op makes the kernel's 16-byte-aligned copy itself
-        xs = [ops.to_device(x, dev).contiguous() if compiling else ops.logits_c(ops.to_device(x, dev)) for x in logits]
+        xs = [torch_ops.stage_logits(ops.to_device(x, dev)) for x in logits]
         xs[1:] = [x.detach() for x in xs[1:]]
         a = ops.i64c(ops.to_device(action, dev), V)
-        if compiling:
-            grpo = side[0] == 'adv'
-            loss, kl, cf = torch_ops.lm_policy(xs[0], xs[1], xs[2] if grpo else None, a,
-                                               side_t.reshape(-1) if grpo else side_t, w, 'grpo' if grpo else 'rloo',
-                                               float(clip_ratio), float(beta))
-        else:
-            loss, kl, cf = fn_fused(xs, a, side_t, w, dt)
+        grpo = side[0] == 'adv'
+        loss, kl, cf = torch_ops.lm_policy(xs[0], xs[1], xs[2] if grpo else None, a, side_t.reshape(-1) if grpo else side_t,
+                                           w, 'grpo' if grpo else 'rloo', dt, clip_ratio, beta)
     else:
         lp_new = ops.to_device(lp_new, dev).float().contiguous()
         lp_rest = [ops.f32c(ops.to_device(x.detach(), dev).float()) for x in lp_rest]
         lp_ref = lp_rest[1] if len(lp_rest) > 1 else None
         adv = side_t if side[0] == 'adv' else None
         reward = side_t if side[0] == 'reward' else None
-        head = torch_ops.token_head if compiling else ops.token_head_
-        loss, kl, cf = head(lp_new, lp_rest[0], lp_ref, adv, reward, w, clip_ratio, beta)
+        loss, kl, cf = torch_ops.token_head(lp_new, lp_rest[0], lp_ref, adv, reward, w, clip_ratio, beta)
     if host_out:
         loss = loss.cpu()
-    if compiling:  # the reference's two .item() calls: what a traced graph can take (as ppo_error's)
+    if torch.compiler.is_compiling():  # the host read a traced graph can take: the reference's two .item() calls
         kl, cf = kl.detach(), cf.detach()
         return loss, info_type(kl, cf) if _ppo.LAZY_INFO else info_type(kl.item(), cf.item())
     if _ppo.LAZY_INFO:

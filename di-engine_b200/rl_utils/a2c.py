@@ -58,15 +58,13 @@ def _a2c_lm(logit, action, value, adv, return_, weight):
                         value.dtype)
     dev = ops.compute_device(logit, value)
     host_out = not logit.is_cuda
-    compiling = torch.compiler.is_compiling()
-    # a traced tensor has no address: the custom op makes the kernel's 16-byte-aligned copy itself
-    z = ops.to_device(logit, dev).contiguous() if compiling else ops.logits_c(ops.to_device(logit, dev))
+    z = torch_ops.stage_logits(ops.to_device(logit, dev))
     # a bf16 value is read as fp32; autograd's cast hands its gradient back in bf16
     v = ops.to_device(value, dev).float().contiguous()
     a = ops.i64c(ops.to_device(action, dev), V)
     ad, rt = (ops.to_device(t_.detach(), dev).float().contiguous() for t_ in (adv, return_))
     w = ops.to_device(weight.detach(), dev).float().contiguous() if weight is not None else None
-    p, vl, e = torch_ops.a2c_lm(z, v, a, ad, rt, w) if compiling else ops.A2CLMFunction.apply(z, v, a, ad, rt, w, dt)
+    p, vl, e = torch_ops.a2c_lm(z, v, a, ad, rt, w, dt)
     if host_out:
         p, vl, e = p.cpu(), vl.cpu(), e.cpu()
     return a2c_loss(p, vl, e)

@@ -58,10 +58,8 @@ def coma_error(data: namedtuple, gamma: float, lambda_: float) -> namedtuple:
         r = rw.unsqueeze(-1).expand(T, B, A).reshape(T, B * A)[:-1].contiguous()
         ret = ops.LambdaReturnsFunction.apply(tq_taken, r, None, None, None, float(gamma), float(lambda_), False)
         p, v, e = ops.COMAFunction.apply(z, qv, tq.detach(), act, rw.detach(), w, ret, T, B, A, N, gamma, lambda_)
-    elif torch.compiler.is_compiling():
-        p, v, e = torch_ops.coma(z, qv, tq.detach(), act, rw.detach(), w, T, B, A, N, gamma, lambda_)
     else:
-        p, v, e = ops.COMAFunction.apply(z, qv, tq.detach(), act, rw.detach(), w, None, T, B, A, N, gamma, lambda_)
+        p, v, e = torch_ops.coma(z, qv, tq.detach(), act, rw.detach(), w, T, B, A, N, gamma, lambda_)
     if host_out:
         p, v, e = p.cpu(), v.cpu(), e.cpu()
     return coma_loss(p, v, e)

@@ -49,12 +49,9 @@ def gae(data: namedtuple, gamma: float = 0.99, lambda_: float = 0.97) -> torch.F
         d = d.expand_as(r).contiguous()
     if tf is not None and tf.shape != r.shape:
         tf = tf.expand_as(r).contiguous()
-    if torch.compiler.is_compiling():
-        adv = torch_ops.gae_op(v, nv, r, d, tf, float(gamma), float(lambda_), agents)
-        staged = nv is not nv_src
-    else:
-        adv = ops.gae_(v, nv, r, d, tf, gamma, lambda_, agents)
-        staged = nv.data_ptr() != nv_src.data_ptr()
+    adv = torch_ops.gae(v, nv, r, d, tf, gamma, lambda_, agents)
+    # a traced tensor has no address: under compile a staged copy is told by identity
+    staged = (nv is not nv_src) if torch.compiler.is_compiling() else nv.data_ptr() != nv_src.data_ptr()
     if d is not None and staged:
         # the kernel masked a staged / re-laid-out copy: propagate the reference's in-place side effect
         with torch.no_grad():
@@ -94,11 +91,7 @@ def gae_returns(data: namedtuple, gamma: float = 0.99, lambda_: float = 0.97, va
     d = ops.f32c(ops.to_device(done.detach(), dev), 'done') if done is not None else None
     tf = ops.f32c(ops.to_device(traj_flag.detach(), dev), 'traj_flag') if traj_flag is not None else None
     vs = 0.0 if value_norm_std is None else float(value_norm_std)
-    if torch.compiler.is_compiling():
-        adv, unnorm, vout, rout, stats, astats = torch_ops.gae_returns(v, nv, r, d, tf, gamma, lambda_, vs)
-    else:
-        adv, unnorm, vout, rout, stats, astats = ops.gae_returns_(v, nv, r, d, tf, gamma, lambda_, 1, vs, True, True,
-                                                                  want_adv_stats=True)
+    adv, unnorm, vout, rout, stats, astats = torch_ops.gae_returns(v, nv, r, d, tf, gamma, lambda_, vs)
     if vs == 0.0:
         vout, rout = v, unnorm
     out = gae_returns_out(adv, vout, rout, unnorm, stats, astats)
@@ -171,12 +164,8 @@ def ppof_gae_returns(data: namedtuple, gamma: float = 0.99, lambda_: float = 0.9
         sigma = ops.f32c(ops.to_device(popart_sigma.detach(), dev), 'popart_sigma').reshape(-1)
         if mu.numel() != 1 or sigma.numel() != 1:
             raise ValueError("ppof_gae_returns: popart_mu / popart_sigma must hold one float each (a single-output PopArt head)")
-    if torch.compiler.is_compiling():
-        adv, vout, rout, stats, astats = torch_ops.ppof_gae_returns(v, nv, r, d, tf, gamma, lambda_, value_norm, std, mu,
-                                                                    sigma)
-    else:
-        adv, vout, rout, stats, astats = ops.gae_returns_norm_(v, nv, r, d, tf, gamma, lambda_, value_norm, std, mu, sigma,
-                                                               value_norm == 'baseline')
+    adv, vout, rout, stats, astats = torch_ops.ppof_gae_returns(v, nv, r, d, tf, gamma, lambda_, value_norm, std, mu,
+                                                                sigma)
     out = ppof_gae_returns_out(adv.reshape(value.shape), vout.reshape(value.shape), rout.reshape(value.shape), stats, astats)
     if host_out:
         out = ppof_gae_returns_out(*[None if t is None else t.cpu() for t in out])

@@ -7,7 +7,6 @@ carry 0-dim device tensors instead of python floats."""
 from collections import namedtuple
 from typing import Tuple
 
-from .. import ops
 from . import _lm_policy
 from .log_prob_utils import LogProbFunction, efficient_method
 
@@ -25,8 +24,5 @@ def grpo_policy_error(
     (B, S, V) fp32 or bf16, action (B, S), adv (B), weight (B, S) or None.  Returns (loss, grpo_info(approx_kl,
     clipfrac)); loss = mean_b(sum_s(w * l) / sum_s(w)) with the per-token loss
     l = -min(r * adv, clamp(r, 1 - clip, 1 + clip) * adv) + beta * (exp(lp_ref - lp) - (lp_ref - lp) - 1)."""
-    def fused(xs, action, adv, weight, dt):
-        return ops.GRPOFunction.apply(xs[0], xs[1], xs[2], action, adv.reshape(-1), weight, dt, clip_ratio, beta)
-
-    return _lm_policy.run(fused, (data.logit_new, data.logit_old, data.logit_ref), data.action, data.weight,
+    return _lm_policy.run((data.logit_new, data.logit_old, data.logit_ref), data.action, data.weight,
                           ('adv', data.adv), log_prob_fn, clip_ratio, beta, grpo_info)

@@ -84,10 +84,6 @@ def _stage(hidden, lm_weight, dev):
     return h.reshape(-1, h.shape[-1]).contiguous(), ops.to_device(lm_weight, dev).contiguous()
 
 
-def _wants_grad(h, w):
-    return torch.is_grad_enabled() and (h.requires_grad or w.requires_grad)
-
-
 def token_logp_linear(hidden: torch.Tensor, lm_weight: torch.Tensor, index: torch.Tensor) -> torch.Tensor:
     """log softmax(hidden @ lm_weight^T)[index]: hidden (B, S, D), lm_weight (V, D), index (B, S) -> fp32 (B, S),
     differentiable w.r.t. hidden and lm_weight."""
@@ -100,13 +96,7 @@ def token_logp_linear(hidden: torch.Tensor, lm_weight: torch.Tensor, index: torc
     host_out = not hidden.is_cuda
     h, w = _stage(hidden, lm_weight, dev)
     a = ops.i64c(ops.to_device(index, dev), V, 'index').reshape(-1)
-    if torch.compiler.is_compiling():
-        lp = torch_ops.lm_logp(h, w, a, dt)[0]
-    elif _wants_grad(h, w):
-        lp = ops.TokenLogpLinearFunction.apply(h, w, a, dt)
-    else:
-        lp = ops.lm_logp_fwd_(h.detach(), w.detach(), a, dt)[0]
-    lp = lp.view(B, S)
+    lp = torch_ops.lm_logp(h, w, a, dt).view(B, S)
     return lp.cpu() if host_out else lp
 
 
@@ -130,22 +120,11 @@ def _run(kind, hidden, lm_weight, lps, action, weight, side, clip_ratio, beta, i
     a = ops.i64c(ops.to_device(action, dev), V).reshape(-1)
     h, wt = _stage(hidden, lm_weight, dev)
     cfg = (kind, B, S, dt, float(clip_ratio), float(beta))
-    if torch.compiler.is_compiling():
-        grad = torch.is_grad_enabled()
-        out = torch_ops.lm_linear_loss(h, wt, a, lp[0], lp_ref, side_t, w, *cfg, grad and h.requires_grad,
-                                       grad and wt.requires_grad)[0]
-        loss, kl, cf = out[0], out[1].detach(), out[2].detach()
-        if host_out:
-            loss = loss.cpu()
-        # the monitors as the logit-form losses return them under compile
-        return loss, info_type(kl, cf) if _ppo.LAZY_INFO else info_type(kl.item(), cf.item())
-    if _wants_grad(h, wt):
-        loss, kl, cf = ops.LMLinearLossFunction.apply(h, wt, a, lp[0], lp_ref, side_t, w, *cfg)
-    else:
-        out = ops.lm_linear_loss_(h.detach(), wt.detach(), a, lp[0], lp_ref, side_t, w, *cfg, False, False)[0]
-        loss, kl, cf = out[0], out[1], out[2]
+    loss, kl, cf = torch_ops.lm_linear_loss(h, wt, a, lp[0], lp_ref, side_t, w, *cfg)
     if host_out:
         loss = loss.cpu()
+    if torch.compiler.is_compiling():  # the host read a traced graph can take, as the logit-form losses make it
+        return loss, info_type(kl, cf) if _ppo.LAZY_INFO else info_type(kl.item(), cf.item())
     if _ppo.LAZY_INFO:
         return loss, info_type(kl, cf)
     kl, cf = torch.stack([kl, cf]).tolist()  # one host sync
@@ -185,18 +164,8 @@ def _run_pg(kind, hidden, lm_weight, action, weight, rows, value, cfg):
     v = None if value is None else ops.to_device(value, dev).float().contiguous().reshape(-1)
     a = ops.i64c(ops.to_device(action, dev), V).reshape(-1)
     h, wt = _stage(hidden, lm_weight, dev)
-    args = (a, f['adv'], w, f.get('logp_old'), f.get('logp_pretrained'), f.get('return_'), kind, dt, cfg)
-    grad = torch.is_grad_enabled()
-    if torch.compiler.is_compiling():
-        loss, out = torch_ops.lm_linear_pg(h, wt, v, *args[:-1], *cfg, grad and h.requires_grad,
-                                           grad and wt.requires_grad, grad and v is not None and v.requires_grad)[:2]
-    elif grad and (h.requires_grad or wt.requires_grad or (v is not None and v.requires_grad)):
-        loss, out = ops.LMLinearPGFunction.apply(h, wt, v, *args)
-    else:
-        out = ops.lm_linear_pg_(h.detach(), wt.detach(), a, f['adv'], w, f.get('logp_old'), f.get('logp_pretrained'),
-                                None if v is None else v.detach(), f.get('return_'), kind, dt, cfg, False, False,
-                                False)[0]
-        loss = ops.lm_pg_loss_(out, kind, cfg)
+    loss, out = torch_ops.lm_linear_pg(h, wt, v, a, f['adv'], w, f.get('logp_old'), f.get('logp_pretrained'),
+                                       f.get('return_'), kind, dt, cfg)
     if host_out:
         loss, out = loss.cpu(), out.cpu()
     return loss, out
@@ -227,7 +196,7 @@ def ppo_policy_error_linear(data: namedtuple, clip_ratio: float = 0.2, dual_clip
                         {'adv': adv, 'logp_old': logp_old, 'logp_pretrained': logp_pre}, None, cfg)
     if _ppo.LAZY_INFO:
         info = ppo_info(out[3], out[4])
-    elif torch.compiler.is_compiling():  # the logit-form losses' host read under compile
+    elif torch.compiler.is_compiling():  # the host read a traced graph can take, as the logit-form losses make it
         info = ppo_info(out[3].item(), out[4].item())
     else:
         approx_kl, clipfrac = out[3:5].tolist()  # one host sync

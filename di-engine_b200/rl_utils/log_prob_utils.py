@@ -5,7 +5,6 @@ Python loop over B.  Logits may be fp32 or bf16; the result is fp32 either way (
 logits, rounded at each step)."""
 from typing import Callable
 
-import torch
 from torch import Tensor
 
 from .. import ops, torch_ops
@@ -31,10 +30,7 @@ def _token_logp(logits: Tensor, index: Tensor) -> Tensor:
     V = logits.shape[-1]
     x = ops.to_device(logits, dev)
     a = ops.i64c(ops.to_device(index, dev), V, 'index').view(-1)
-    if torch.compiler.is_compiling():  # the custom op makes the kernel's 16-byte-aligned copy itself
-        lp = torch_ops.token_logp(x.contiguous().view(-1, V), a)
-    else:
-        lp = ops.TokenLogProbFunction.apply(ops.logits_c(x).view(-1, V), a, dt)
+    lp = torch_ops.token_logp(torch_ops.stage_logits(x).view(-1, V), a, dt)
     lp = lp.view(index.shape)
     return lp.cpu() if host_out else lp
 

@@ -58,10 +58,7 @@ def normalize_advantage(adv: torch.Tensor) -> torch.Tensor:
     dev = ops.compute_device(adv)
     host_out = not adv.is_cuda
     a = ops.f32c(ops.to_device(adv.detach(), dev), 'adv')
-    if torch.compiler.is_compiling():
-        out = torch_ops.normalize(a, torch_ops.adv_stats(a))
-    else:
-        out = ops.normalize_(a, ops.adv_stats_(a))
+    out = torch_ops.normalize(a, torch_ops.adv_stats(a))
     return out.cpu() if host_out else out
 
 
@@ -157,7 +154,7 @@ def _ppo_error(data, clip_ratio, use_value_clip, dual_clip, kl_type, _hint_kind,
     stats = None
     if adv_norm:
         if adv_stats is None:
-            stats = torch_ops.adv_stats(ad) if torch.compiler.is_compiling() else ops.adv_stats_(ad)
+            stats = torch_ops.adv_stats(ad)
         else:
             stats = ops.f32c(ops.to_device(adv_stats.detach(), ad.device), 'adv_stats').reshape(-1)
             if stats.numel() != 2:
@@ -169,18 +166,14 @@ def _ppo_error(data, clip_ratio, use_value_clip, dual_clip, kl_type, _hint_kind,
             raise ValueError("happo_error: factor %s does not match adv %s" % (tuple(factor.shape), tuple(adv.shape)))
     args = (ln, vn, lo, act, vo, ad, rt, w, lp, S, G, N, float(clip_ratio), 1 if use_value_clip else 0,
             float(dual_clip) if dual_clip is not None else 0.0, _KL_TYPES.get(kl_type, 1), _hint_kind, stats, fac)
-    if torch.compiler.is_compiling():
-        out = torch_ops.ppo(*args)
-        p, v, e, k = out[0], out[1], out[2], out[3]
-        # the reference's two .item() calls (ppo.py:218-220): what a traced graph can take
+    p, v, e, k, out = torch_ops.ppo(*args)
+    if torch.compiler.is_compiling():  # the host read a traced graph can take: the reference's two .item() (ppo.py:218-220)
         info = ppo_info(out[4].detach(), out[5].detach()) if LAZY_INFO else ppo_info(out[4].item(), out[5].item())
+    elif LAZY_INFO:
+        info = ppo_info(out[4], out[5])
     else:
-        p, v, e, k, out = ops.PPOFunction.apply(*args)
-        if LAZY_INFO:
-            info = ppo_info(out[4], out[5])
-        else:
-            approx_kl, clipfrac = out[4:6].tolist()  # one D2H read for both monitors (reference: two .item() syncs)
-            info = ppo_info(approx_kl, clipfrac)
+        approx_kl, clipfrac = out[4:6].tolist()  # one D2H read for both monitors (reference: two .item() syncs)
+        info = ppo_info(approx_kl, clipfrac)
     if host_out:
         p, v, e, k = p.cpu(), v.cpu(), e.cpu(), k.cpu()
     return ppo_loss(p, v, e, k), info
@@ -238,18 +231,14 @@ def _ppo_error_continuous(data, clip_ratio, use_value_clip, dual_clip, kl_type, 
     fac = stage(factor.detach(), 'factor', S).reshape(-1) if factor is not None else None
     args += [S, D, float(clip_ratio), 1 if use_value_clip else 0, float(dual_clip) if dual_clip is not None else 0.0,
              _KL_TYPES.get(kl_type, 1), hint_kind, fac]
-    if torch.compiler.is_compiling():
-        out = torch_ops.ppo_continuous(*args)
-        p, v, e, k = out[0], out[1], out[2], out[3]
-        # the reference's two .item() calls (ppo.py:366-368): what a traced graph can take
+    p, v, e, k, out = torch_ops.ppo_continuous(*args)
+    if torch.compiler.is_compiling():  # the host read a traced graph can take: the reference's two .item() (ppo.py:366-368)
         info = ppo_info(out[4].detach(), out[5].detach()) if LAZY_INFO else ppo_info(out[4].item(), out[5].item())
+    elif LAZY_INFO:
+        info = ppo_info(out[4], out[5])
     else:
-        p, v, e, k, out = ops.PPOContinuousFunction.apply(*args)
-        if LAZY_INFO:
-            info = ppo_info(out[4], out[5])
-        else:
-            approx_kl, clipfrac = out[4:6].tolist()
-            info = ppo_info(approx_kl, clipfrac)
+        approx_kl, clipfrac = out[4:6].tolist()
+        info = ppo_info(approx_kl, clipfrac)
     if host_out:
         p, v, e, k = p.cpu(), v.cpu(), e.cpu(), k.cpu()
     return ppo_loss(p, v, e, k), info
@@ -310,10 +299,8 @@ def _ppo_lm(data, clip_ratio, dual_clip, entropy_bonus, kl_type, hint_kind):
                              (name, tuple(t_.shape), tuple(logit_new.shape)))
     dev = ops.compute_device(*logits)
     host_out = not logit_new.is_cuda
-    compiling = torch.compiler.is_compiling()
-    # logit_old / logit_pretrained get no gradient; weight and adv are read as fp32 whatever their dtype.  A traced tensor
-    # has no address: the custom op makes the kernel's 16-byte-aligned copy itself
-    xs = [ops.to_device(x, dev).contiguous() if compiling else ops.logits_c(ops.to_device(x, dev)) for x in logits]
+    # logit_old / logit_pretrained get no gradient; weight and adv are read as fp32 whatever their dtype
+    xs = [torch_ops.stage_logits(ops.to_device(x, dev)) for x in logits]
     xs[1:] = [x.detach() for x in xs[1:]]
     ad = ops.to_device(adv.detach(), dev).float().contiguous()
     w = None
@@ -324,17 +311,14 @@ def _ppo_lm(data, clip_ratio, dual_clip, entropy_bonus, kl_type, hint_kind):
     args = (xs[0], xs[1], xs[2] if len(xs) > 2 else None, act, ad, w)
     cfg = (float(clip_ratio), float(dual_clip) if dual_clip is not None else 0.0, _KL_TYPES.get(kl_type, 1),
            bool(entropy_bonus))
-    if compiling:
-        p, e, k, out = torch_ops.ppo_lm(*args, *cfg)
-        # the reference's two .item() calls (ppo.py:218-220): what a traced graph can take
+    p, e, k, out = torch_ops.ppo_lm(*args, dt, *cfg, hint_kind)
+    if torch.compiler.is_compiling():  # the host read a traced graph can take: the reference's two .item() (ppo.py:218-220)
         info = ppo_info(out[3].detach(), out[4].detach()) if LAZY_INFO else ppo_info(out[3].item(), out[4].item())
+    elif LAZY_INFO:
+        info = ppo_info(out[3], out[4])
     else:
-        p, e, k, out = ops.PPOLMFunction.apply(*args, dt, *cfg, hint_kind)
-        if LAZY_INFO:
-            info = ppo_info(out[3], out[4])
-        else:
-            approx_kl, clipfrac = out[3:5].tolist()
-            info = ppo_info(approx_kl, clipfrac)
+        approx_kl, clipfrac = out[3:5].tolist()
+        info = ppo_info(approx_kl, clipfrac)
     if host_out:
         p, e, k = p.cpu(), e.cpu(), k.cpu()
     entropy = e if entropy_bonus else torch.tensor(0.0)  # ppo.py:203
@@ -388,6 +372,5 @@ def ppo_value_error(
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.numel() != vn.numel():
             w = w.expand_as(vn).contiguous()
-    value = torch_ops.ppo_value if torch.compiler.is_compiling() else ops.ppo_value_
-    loss = value(vn, vo, rt, w, clip_ratio, use_value_clip)
+    loss = torch_ops.ppo_value(vn, vo, rt, w, clip_ratio, use_value_clip)
     return loss.cpu() if host_out else loss

@@ -8,7 +8,7 @@ from typing import Optional
 import torch
 
 from .. import ops, torch_ops
-from .td import _value_gamma_arg, _value_gamma_op_arg
+from .td import _value_gamma_arg
 
 qrdqn_nstep_td_data = namedtuple(
     'qrdqn_nstep_td_data', ['q', 'next_n_q', 'action', 'next_n_action', 'reward', 'done', 'tau', 'weight']
@@ -56,16 +56,9 @@ def _run(q, next_n_q, action, next_n_action, reward, done, tau, weight, gamma, n
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight').reshape(-1)
         if w.numel() != B:
             raise ValueError("weight must have B=%d elements" % B)
-    if torch.compiler.is_compiling():
-        vg, vg_stride = _value_gamma_op_arg(value_gamma, B, dev)
-        loss, td = torch_ops.quantile_td(qd, nq, act, nact, r, d, t, w, vg, vg_stride, B, N, n_tau, n_tau_p, nstep,
-                                         float(gamma), form, float(kappa))
-        return (loss.cpu(), td.cpu()) if host_out else (loss, td)
     vg, vg_stride = _value_gamma_arg(value_gamma, B, dev)
-    loss, td = ops.QuantileTDFunction.apply(
-        qd, nq, act, nact, r, d, t, w, vg, vg_stride, B, N, n_tau, n_tau_p, nstep, float(gamma),
-        tuple(qd.stride(a) for a in axes), tuple(nq.stride(a) for a in axes), (t.stride(0), t.stride(1)), form, float(kappa)
-    )
+    loss, td = torch_ops.quantile_td(qd, nq, act, nact, r, d, t, w, vg, vg_stride, B, N, n_tau, n_tau_p, nstep,
+                                     float(gamma), form, float(kappa))
     return (loss.cpu(), td.cpu()) if host_out else (loss, td)
 
 
@@ -162,9 +155,5 @@ def fqf_calculate_fraction_loss(q_tau_i, q_value, quantiles, actions):
     qv = _f32(ops.to_device(q_value.detach(), dev), 'q_value')
     qn = _f32(ops.to_device(quantiles, dev), 'quantiles')
     act = ops.i64c(ops.to_device(actions, dev), min(qt.shape[2], qv.shape[2]), 'actions')
-    if torch.compiler.is_compiling():
-        loss = torch_ops.fqf_fraction(qt, qv, qn, act, batch_size, num_quantiles)
-    else:
-        loss = ops.FQFFractionFunction.apply(qt, qv, qn, act, batch_size, num_quantiles, qt.stride(), qv.stride(),
-                                             qn.stride())
+    loss = torch_ops.fqf_fraction(qt, qv, qn, act, batch_size, num_quantiles)
     return loss.cpu() if host_out else loss

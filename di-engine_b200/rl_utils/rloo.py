@@ -6,7 +6,6 @@ callables and ``ppo.LAZY_INFO`` as for ``grpo_policy_error``."""
 from collections import namedtuple
 from typing import Tuple
 
-from .. import ops
 from . import _lm_policy
 from .log_prob_utils import LogProbFunction, efficient_method
 
@@ -22,8 +21,5 @@ def rloo_policy_error(
     """REINFORCE Leave-One-Out (https://arxiv.org/abs/2402.14740).  logit_new / logit_old (B, S, V) fp32 or bf16, action
     (B, S), reward (K, B / K), weight (B, S) or None.  Returns (loss, rloo_info(approx_kl, clipfrac)) with the loss of
     ``grpo_policy_error`` without its KL term."""
-    def fused(xs, action, reward, weight, dt):
-        return ops.RLOOFunction.apply(xs[0], xs[1], action, reward, weight, dt, clip_ratio)
-
-    return _lm_policy.run(fused, (data.logit_new, data.logit_old), data.action, data.weight, ('reward', data.reward),
+    return _lm_policy.run((data.logit_new, data.logit_old), data.action, data.weight, ('reward', data.reward),
                           log_prob_fn, clip_ratio, 0.0, rloo_info)

@@ -85,25 +85,18 @@ def _criterion_code(criterion):
 
 
 def _value_gamma_arg(value_gamma, B, dev):
-    """-> (tensor or None, stride): None | python scalar | 0-dim / 1-element tensor (stride 0) | (B,) tensor (stride 1)."""
+    """-> (value_gamma, stride): None | python scalar (kept a float, stride 0) | 0-dim / 1-element tensor (stride 0) |
+    (B,) tensor (stride 1)."""
     if value_gamma is None:
         return None, 0
     if not isinstance(value_gamma, torch.Tensor):
-        return ops.const_scalar(value_gamma, dev), 0
+        return float(value_gamma), 0
     vg = ops.f32c(ops.to_device(value_gamma.detach(), dev), 'value_gamma')
     if vg.numel() == 1:
         return vg.reshape(1), 0
     if vg.numel() != B:
         raise ValueError("value_gamma must have 1 or B=%d elements, got %s" % (B, tuple(value_gamma.shape)))
     return vg.reshape(B), 1
-
-
-def _value_gamma_op_arg(value_gamma, B, dev):
-    """``_value_gamma_arg`` for the custom ops (rl_utils' traced path): a python scalar stays a float, which the op reads
-    from the cached device constant when it runs, so that tracing allocates nothing"""
-    if value_gamma is not None and not isinstance(value_gamma, torch.Tensor):
-        return float(value_gamma), 0
-    return _value_gamma_arg(value_gamma, B, dev)
 
 
 def _gamma_arg(gamma, B, dev, cum_reward):
@@ -145,18 +138,14 @@ def _qntd_rows(q, next_n_q, action, next_n_action, reward, done, weight, value_g
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.numel() != S:
             w = w.expand(S).contiguous()
-    vg, vg_stride = (_value_gamma_op_arg if torch.compiler.is_compiling() else _value_gamma_arg)(value_gamma, S, dev)
+    vg, vg_stride = _value_gamma_arg(value_gamma, S, dev)
     custom_trans = rescale and (trans_fn is not value_transform or inv_trans_fn is not value_inv_transform)
     code = _criterion_code(criterion)
     gm = 1 if group_mean else 0
 
     def kernel(q_, nq_, act_, nact_, n_, resc, crit, param):
-        if torch.compiler.is_compiling():
-            return torch_ops.qntd(q_, nq_, act_, nact_, r, d, w, vg, vg_stride, gamma_ps, S, G, n_, int(nstep),
-                                  float(gamma_f), 1 if cum_reward else 0, resc, 1e-2, crit, param, gm) + (None, )
-        return ops.QNStepTDFunction.apply(q_, nq_, act_, nact_, r, d, w, vg, vg_stride, gamma_ps, S, G, n_, int(nstep),
-                                          float(gamma_f), 1 if cum_reward else 0, resc, 1e-2, crit, param, gm, 0, 0.0,
-                                          False)
+        return torch_ops.qntd(q_, nq_, act_, nact_, r, d, w, vg, vg_stride, gamma_ps, S, G, n_, int(nstep), float(gamma_f),
+                              1 if cum_reward else 0, resc, 1e-2, crit, param, gm)
 
     if custom_trans or code is None:
         # user-supplied transforms / criterion are torch callables: the kernel produces the detached n-step target (of the
@@ -464,16 +453,9 @@ def q_nstep_td_error_sequence(
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.numel() != S:
             w = w.expand(T, B).contiguous()
-    if torch.compiler.is_compiling():
-        vg, vg_stride = _value_gamma_op_arg(value_gamma, S, dev)
-        loss, per, prio = torch_ops.qntd_seq(qd, nq, act, nact, r, d, w, vg, vg_stride, gamma_ps, S, N, int(nstep),
-                                             float(gamma_f), 1 if rescale else 0, code[0], code[1], T, float(priority_mix))
-    else:
-        vg, vg_stride = _value_gamma_arg(value_gamma, S, dev)
-        loss, per, _, prio = ops.QNStepTDFunction.apply(
-            qd, nq, act, nact, r, d, w, vg, vg_stride, gamma_ps, S, 1, N, int(nstep), float(gamma_f), 0,
-            1 if rescale else 0, 1e-2, code[0], code[1], 0, T, float(priority_mix), True
-        )
+    vg, vg_stride = _value_gamma_arg(value_gamma, S, dev)
+    loss, per, prio = torch_ops.qntd_seq(qd, nq, act, nact, r, d, w, vg, vg_stride, gamma_ps, S, N, int(nstep),
+                                         float(gamma_f), 1 if rescale else 0, code[0], code[1], T, float(priority_mix))
     per = per.reshape(T, B)
     if host_out:
         loss, prio, per = loss.cpu(), prio.cpu(), per.cpu()
@@ -505,8 +487,7 @@ def _dqfd_operands(data, S, dev, rows):
     d = ops.f32c(ops.to_device(done.detach(), dev), 'done')
     d1 = ops.f32c(ops.to_device(done_one_step.detach(), dev), 'done_one_step')
     if not isinstance(is_expert, torch.Tensor):
-        # traced: a float, which the custom op reads from the cached device constant when it runs
-        ie = float(is_expert) if torch.compiler.is_compiling() else ops.const_scalar(is_expert, dev).expand(S).contiguous()
+        ie = float(is_expert)  # torch_ops.dqfd expands it to the S rows
     else:
         ie = ops.f32c(ops.to_device(is_expert.detach(), dev), 'is_expert')
     if isinstance(ie, torch.Tensor) and ie.numel() == 1:
@@ -554,14 +535,13 @@ def _dqfd(data, gamma, lambda_n_step_td, lambda_supervised_loss, lambda_one_step
     host_out = not q.is_cuda
     dev = ops.compute_device(q, next_n_q, next_q1)
     qd, nq, nq1, act, nact, nact1, r, d, d1, w, ie = _dqfd_operands(data, B, dev, (B, ))
-    compiling = torch.compiler.is_compiling()
-    vg, vg_stride = (_value_gamma_op_arg if compiling else _value_gamma_arg)(value_gamma, B, dev)
+    vg, vg_stride = _value_gamma_arg(value_gamma, B, dev)
     custom_trans = rescale and (trans_fn is not value_transform or inv_trans_fn is not value_inv_transform)
     code = _criterion_code(criterion)
     lam_n, lam_1, lam_s = float(lambda_n_step_td), float(lambda_one_step_td), float(lambda_supervised_loss)
 
     def kernel(nq_, nq1_, resc, crit, param, want_targets):
-        return (torch_ops.dqfd if compiling else ops.DQfDTDFunction.apply)(
+        return torch_ops.dqfd(
             qd, nq_, nq1_, act, nact, nact1, r, d, d1, w, vg, vg_stride, ie, B, N, int(nstep), gamma,
             1 if cum_reward else 0, resc, 1e-2, crit, param, lam_n, lam_1, lam_s, float(margin_function), 0, 0.0,
             want_targets, False)
@@ -698,9 +678,8 @@ def dqfd_nstep_td_error_sequence(
     qd, nq, nq1, act, nact, nact1, r, d, d1, w, ie = _dqfd_operands(
         dqfd_nstep_td_data(q, next_n_q, action, next_n_action, reward, done, done_one_step, weight, next_q1, next_action1,
                            is_expert), S, dev, (T, B))
-    compiling = torch.compiler.is_compiling()
-    vg, vg_stride = (_value_gamma_op_arg if compiling else _value_gamma_arg)(value_gamma, S, dev)
-    loss, per, s_n, s_1, s_je, _, _, prio = (torch_ops.dqfd if compiling else ops.DQfDTDFunction.apply)(
+    vg, vg_stride = _value_gamma_arg(value_gamma, S, dev)
+    loss, per, s_n, s_1, s_je, _, _, prio = torch_ops.dqfd(
         qd, nq, nq1, act, nact, nact1, r, d, d1, w, vg, vg_stride, ie, S, N, int(nstep), gamma, 0, 1 if rescale else 0,
         1e-2, code[0], code[1], float(lambda_n_step_td), float(lambda_one_step_td), float(lambda_supervised_loss),
         float(margin_function), T, float(priority_mix), False, True
@@ -739,12 +718,11 @@ def _soft_td(mode, q, target_q, next_q, act, reward, done, weight, S, G, gamma, 
     staged there and detached.  -> (loss, td (S*G,), action_gap, clipfrac (S*G,), record_target_v (S*G,)), the last three
     empty where the mode has none."""
     R, N = q.shape
-    compiling = torch.compiler.is_compiling()
-    vg, vg_stride = (_value_gamma_op_arg if compiling else _value_gamma_arg)(value_gamma, S, q.device)
+    vg, vg_stride = _value_gamma_arg(value_gamma, S, q.device)
     code = _criterion_code(criterion)
 
     def kernel(q_, crit, param):
-        return (torch_ops.soft_td if compiling else ops.SoftTDFunction.apply)(
+        return torch_ops.soft_td(
             q_, target_q, next_q, act, reward, done, weight, vg, vg_stride, mode, S, G, N, int(nstep), float(gamma),
             float(tau), float(alpha), 1 if cum_reward else 0, crit, param)
 
@@ -1041,7 +1019,7 @@ def _dntd(data, gamma, v_min, v_max, n_atom, nstep, value_gamma, check_positive)
     if weight is None:
         w, w_stride = None, 0
     elif not isinstance(weight, torch.Tensor):
-        w, w_stride = (float(weight) if torch.compiler.is_compiling() else ops.const_scalar(weight, dev)), 0
+        w, w_stride = float(weight), 0
     else:
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.numel() == 1:
@@ -1050,19 +1028,9 @@ def _dntd(data, gamma, v_min, v_max, n_atom, nstep, value_gamma, check_positive)
             w, w_stride = w.reshape(R), 1
         else:
             raise ValueError("weight must have 1 or %d elements, got %s" % (R, tuple(weight.shape)))
-    if torch.compiler.is_compiling():
-        vg, vg_stride = _value_gamma_op_arg(value_gamma, B, dev)
-        loss, per = torch_ops.dist_nstep_td(dd, nd, a, na, r, d, w, w_stride, vg, vg_stride, B, A, N, int(n_atom),
-                                            int(nstep), float(gamma), float(v_min), float(v_max), check_positive)
-        return (loss.cpu(), per.cpu()) if host_out else (loss, per)
     vg, vg_stride = _value_gamma_arg(value_gamma, B, dev)
-    bad = torch.zeros(1, dtype=torch.int32, device=dev) if check_positive else None
-    loss, per = ops.DistNStepTDFunction.apply(
-        dd, nd, a, na, r, d, w, w_stride, vg, vg_stride, _support(v_min, v_max, n_atom, dev), B, A, N, int(n_atom),
-        int(nstep), float(gamma), float(v_min), float(v_max), bad
-    )
-    if check_positive:
-        assert bad.item() == 0, ("dist act", "non-positive probability in dist[batch_range, act]")  # td.py:513
+    loss, per = torch_ops.dist_nstep_td(dd, nd, a, na, r, d, w, w_stride, vg, vg_stride, B, A, N, int(n_atom), int(nstep),
+                                        float(gamma), float(v_min), float(v_max), check_positive)
     if host_out:
         loss, per = loss.cpu(), per.cpu()
     return loss, per
@@ -1172,8 +1140,5 @@ def td_lambda_error(data: namedtuple, gamma: float = 0.9, lambda_: float = 0.8) 
         w = ops.f32c(ops.to_device(weight.detach(), dev), 'weight')
         if w.shape != r.shape:
             w = w.expand_as(r).contiguous()
-    if torch.compiler.is_compiling():
-        loss = torch_ops.td_lambda(v, r, w, float(gamma), float(lambda_))
-    else:
-        loss = ops.td_lambda_(v, r, w, gamma, lambda_)
+    loss = torch_ops.td_lambda(v, r, w, gamma, lambda_)
     return loss.cpu() if host_out else loss

@@ -86,9 +86,5 @@ def upgo_loss(
     rho = ops.f32c(ops.to_device(rhos.detach(), dev), 'rhos')
     r = ops.f32c(ops.to_device(rewards.detach(), dev), 'rewards')
     v = ops.f32c(ops.to_device(bootstrap_values.detach(), dev), 'bootstrap_values')
-    if torch.compiler.is_compiling():
-        loss = torch_ops.upgo(logit, act, m, rho, r, v, T * B, K, N)
-    else:
-        ret = ops.lambda_returns_(v, r, None, 1.0, None, 1.0, None, True)
-        loss = ops.UPGOFunction.apply(logit, act, m, rho, ret, v, T * B, K, N)
+    loss = torch_ops.upgo(logit, act, m, rho, r, v, T * B, K, N)
     return loss.cpu() if host_out else loss

@@ -29,7 +29,7 @@ def _value_map(x, mode, name):
                         (name, getattr(x, 'dtype', type(x).__name__)))
     dev = ops.compute_device(x)
     xd = ops.to_device(x, dev).contiguous()
-    y = torch_ops.value_map(xd, mode) if torch.compiler.is_compiling() else ops.ValueMapFunction.apply(xd, mode)
+    y = torch_ops.value_map(xd, mode)
     return y if x.is_cuda else y.cpu()
 
 

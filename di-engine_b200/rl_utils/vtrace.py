@@ -52,7 +52,7 @@ def vtrace_error_discrete_action(
             w = w.expand_as(r).contiguous()
     args = (tgt, v, beh, act, r, w, float(gamma), float(lambda_), float(rho_clip_ratio), float(c_clip_ratio),
             float(rho_pg_clip_ratio))
-    p, vl, e = torch_ops.vtrace(*args) if torch.compiler.is_compiling() else ops.VTraceFunction.apply(*args)
+    p, vl, e = torch_ops.vtrace(*args)
     if host_out:
         p, vl, e = p.cpu(), vl.cpu(), e.cpu()
     return vtrace_loss(p, vl, e)

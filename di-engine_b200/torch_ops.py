@@ -10,9 +10,13 @@ q_v_1step_td_error), the R2D2 / NGU loop q_nstep_td_error_sequence, FQF's fracti
 from the lm_head's hidden states (grpo / rloo / ppo_policy_error_linear, a2c_error_linear, token_logp_linear) without a
 graph break, and ``mode="reduce-overhead"`` can replay a compiled learner step as a CUDA graph.
 
-Each op's implementation is the launch function ``ops`` runs in eager mode; ``rl_utils`` calls the wrappers at the bottom
-of this module only while ``torch.compiler.is_compiling()``.  The schemas hold tensors and scalars only: the workspace, the
-upstream-gradient records and cached constants are looked up inside the implementations, when the op runs.
+Each op's implementation is the launch function ``ops`` runs in eager mode.  ``rl_utils`` and ``torch_utils`` call the
+entry points at the bottom of this module, one per operator: each runs its custom op while
+``torch.compiler.is_compiling()`` and eager mode's ``autograd.Function`` (or no-grad shortcut) otherwise, and converts
+the arguments the two modes take differently.  The schemas hold tensors and scalars only: the workspace, the
+upstream-gradient records and cached constants are looked up inside the implementations, when the op runs.  Each
+``setup_context`` reads the op's arguments by name (``_bind``) and each backward names the gradients it returns
+(``_input_grads``), so neither depends on the position of an argument in the schema.
 
 The forward-written gradients work as in eager mode, with one difference that functional ops impose: a backward op may
 not return its input, so after a forward launch that wrote the gradients the backward op copies them once and runs the
@@ -22,6 +26,8 @@ and recompute it in the backward op from the saved per-row values, at the price 
 hidden-state losses keep eager's rule instead, since recomputing there would repeat the logit GEMMs: their forward op
 writes dH / dW for a unit upstream gradient and the backward op scales them into fresh buffers.
 """
+import functools
+from types import SimpleNamespace
 from typing import Optional
 
 import torch
@@ -34,6 +40,32 @@ def _empty(like):
     return like.new_empty(0)
 
 
+@functools.cache
+def _names(op):
+    """the op's argument names, in schema order"""
+    return tuple(a.name for a in op._opoverload._schema.arguments)
+
+
+def _bind(op, inputs):
+    """a setup_context's ``inputs`` as named fields"""
+    return SimpleNamespace(**dict(zip(_names(op), inputs)))
+
+
+def _input_grads(op, **grads):
+    """a backward's return tuple: the named input gradients, None for every other argument"""
+    assert grads.keys() <= set(_names(op)), (op, grads.keys())
+    return tuple(grads.get(n) for n in _names(op))
+
+
+def _unit_grad(grad_unit, other_grads, fresh):
+    """ops._unit_grad's rule for the backward ops that take ``skip_if_unit``: (a copy of the forward-written gradient
+    for a unit upstream gradient, 1) when the forward wrote one (a non-empty ``grad_unit``) and no gradient arrived
+    through an output other than the loss; else (fresh(), 0), and the launch recomputes"""
+    if grad_unit.numel() and all(g is None for g in other_grads):
+        return grad_unit.clone(), 1
+    return fresh(), 0
+
+
 def _forward_grads(written, g_used, *grads):
     """copies of the forward-written gradients and their record, or None when the forward wrote none"""
     return tuple(g.clone() for g in grads) + (g_used, ) if written else None
@@ -41,11 +73,8 @@ def _forward_grads(written, g_used, *grads):
 
 def _upstream(g, n):
     """the device pointers of the first ``n`` floats of an upstream-gradient vector (None: no gradient, 0)"""
-    if g is None:
-        return None, (None, ) * n
-    g = g.float().contiguous()
-    base = g.data_ptr()
-    return g, tuple(base + 4 * i for i in range(n))
+    g = None if g is None else g.float().contiguous()
+    return g, tuple(None if g is None else g.data_ptr() + 4 * i for i in range(n))
 
 
 def _one(g):
@@ -119,17 +148,19 @@ def _(logit_new, value_new, *args):
 
 
 def _ppo_setup(ctx, inputs, output):
-    ctx.save_for_backward(*inputs[:11], *output[1:])
-    ctx.cfg = inputs[11:19]
+    a = _bind(ppo_loss, inputs)
+    ctx.save_for_backward(a.logit_new, a.value_new, a.logit_old, a.action, a.value_old, a.adv, a.return_, a.weight,
+                          a.logit_pre, a.adv_stats, a.factor, *output[1:])
+    ctx.cfg = (a.S, a.G, a.N, a.clip_ratio, a.use_value_clip, a.dual_clip, a.kl_type, a.hint_kind)
     ctx.mark_non_differentiable(*output[1:])
 
 
 def _ppo_backward(ctx, g_out, *_):
-    saved = ctx.saved_tensors
     if g_out is None:
-        return (None, ) * 20
+        return _input_grads(ppo_loss)
+    saved = ctx.saved_tensors
     grad_logit, grad_value = ppo_bwd(*saved[:11], g_out, *saved[11:], *ctx.cfg)
-    return (grad_logit, grad_value) + (None, ) * 18
+    return _input_grads(ppo_loss, logit_new=grad_logit, value_new=grad_value)
 
 
 ppo_loss.register_autograd(_ppo_backward, setup_context=_ppo_setup)
@@ -169,8 +200,7 @@ def qntd_bwd(dcrit: Tensor, weight: Optional[Tensor], action: Tensor, g_loss: Op
     """-> d / d q (S * G, N); verifies a copy of the forward-written unit gradient when only the loss has a gradient"""
     kl, pg = _one(g_loss)
     kt, ptd = _one(g_td)
-    skip = 1 if (g_td is None and grad_unit.numel()) else 0
-    grad = grad_unit.clone() if skip else dcrit.new_empty(S * G, N)
+    grad, skip = _unit_grad(grad_unit, (g_td, ), lambda: dcrit.new_empty(S * G, N))
     return ops.qntd_bwd_(dcrit, weight, action, pg, ptd, S, G, N, group_mean, 0, skip, grad)
 
 
@@ -180,20 +210,20 @@ def _(dcrit, weight, action, g_loss, g_td, grad_unit, S, G, N, group_mean):
 
 
 def _qntd_setup(ctx, inputs, output):
-    q, action, weight = inputs[0], inputs[2], inputs[6]
-    ctx.save_for_backward(output[2], weight, action, output[4])
-    ctx.cfg = (inputs[11], inputs[12], inputs[13], inputs[21])
-    ctx.q_shape = q.shape
+    a = _bind(qntd_fwd, inputs)
+    ctx.save_for_backward(output[2], a.weight, a.action, output[4])
+    ctx.cfg = (a.S, a.G, a.N, a.group_mean)
+    ctx.q_shape = a.q.shape
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[2:])
 
 
 def _qntd_backward(ctx, g_loss, g_td, *_):
     if g_loss is None and g_td is None:
-        return (None, ) * 23
+        return _input_grads(qntd_fwd)
     dcrit, weight, action, grad_unit = ctx.saved_tensors
     grad = qntd_bwd(dcrit, weight, action, g_loss, g_td, grad_unit, *ctx.cfg)
-    return (grad.view(ctx.q_shape), ) + (None, ) * 22
+    return _input_grads(qntd_fwd, q=grad.view(ctx.q_shape))
 
 
 qntd_fwd.register_autograd(_qntd_backward, setup_context=_qntd_setup)
@@ -232,8 +262,7 @@ def qntd_seq_bwd(dcrit: Tensor, weight: Optional[Tensor], action: Tensor, g_loss
     """-> d / d q (S, N), as qntd_bwd with the loss averaged over the seq_len steps"""
     kl, pg = _one(g_loss)
     kt, ptd = _one(g_td)
-    skip = 1 if (g_td is None and grad_unit.numel()) else 0
-    grad = grad_unit.clone() if skip else dcrit.new_empty(S, N)
+    grad, skip = _unit_grad(grad_unit, (g_td, ), lambda: dcrit.new_empty(S, N))
     return ops.qntd_bwd_(dcrit, weight, action, pg, ptd, S, 1, N, 0, seq_len, skip, grad)
 
 
@@ -243,19 +272,20 @@ def _(dcrit, weight, action, g_loss, g_td, grad_unit, S, N, seq_len):
 
 
 def _qntd_seq_setup(ctx, inputs, output):
-    ctx.save_for_backward(output[2], inputs[6], inputs[2], output[4])
-    ctx.cfg = (inputs[11], inputs[12], inputs[18])
-    ctx.q_shape = inputs[0].shape
+    a = _bind(qntd_seq_fwd, inputs)
+    ctx.save_for_backward(output[2], a.weight, a.action, output[4])
+    ctx.cfg = (a.S, a.N, a.seq_len)
+    ctx.q_shape = a.q.shape
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[2:])
 
 
 def _qntd_seq_backward(ctx, g_loss, g_td, *_):
     if g_loss is None and g_td is None:
-        return (None, ) * 21
+        return _input_grads(qntd_seq_fwd)
     dcrit, weight, action, grad_unit = ctx.saved_tensors
     grad = qntd_seq_bwd(dcrit, weight, action, g_loss, g_td, grad_unit, *ctx.cfg)
-    return (grad.view(ctx.q_shape), ) + (None, ) * 20
+    return _input_grads(qntd_seq_fwd, q=grad.view(ctx.q_shape))
 
 
 qntd_seq_fwd.register_autograd(_qntd_seq_backward, setup_context=_qntd_seq_setup)
@@ -306,8 +336,7 @@ def dqfd_bwd(saved: Tensor, weight: Optional[Tensor], action: Tensor, g_loss: Op
     kl, pg = _one(g_loss)
     kt, ptd = _one(g_td)
     ks, pstats = _upstream(g_stats, 3)
-    skip = 1 if (g_td is None and g_stats is None and grad_unit.numel()) else 0
-    grad = grad_unit.clone() if skip else saved.new_empty(S, N)
+    grad, skip = _unit_grad(grad_unit, (g_td, g_stats), lambda: saved.new_empty(S, N))
     return ops.dqfd_bwd_(saved, weight, action, pg, ptd, pstats, S, N, lam_n, lam_1, lam_s, seq_len, skip, grad)
 
 
@@ -317,19 +346,20 @@ def _(saved, weight, action, g_loss, g_td, g_stats, grad_unit, S, N, lam_n, lam_
 
 
 def _dqfd_setup(ctx, inputs, output):
-    ctx.save_for_backward(output[3], inputs[9], inputs[3], output[7])
-    ctx.cfg = (inputs[15], inputs[16], inputs[24], inputs[25], inputs[26], inputs[28])
-    ctx.q_shape = inputs[0].shape
+    a = _bind(dqfd_fwd, inputs)
+    ctx.save_for_backward(output[3], a.weight, a.action, output[7])
+    ctx.cfg = (a.S, a.N, a.lam_n, a.lam_1, a.lam_s, a.seq_len)
+    ctx.q_shape = a.q.shape
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[3:])
 
 
 def _dqfd_backward(ctx, g_loss, g_td, g_stats, *_):
     if g_loss is None and g_td is None and g_stats is None:
-        return (None, ) * 33
+        return _input_grads(dqfd_fwd)
     saved, weight, action, grad_unit = ctx.saved_tensors
     grad = dqfd_bwd(saved, weight, action, g_loss, g_td, g_stats, grad_unit, *ctx.cfg)
-    return (grad.view(ctx.q_shape), ) + (None, ) * 32
+    return _input_grads(dqfd_fwd, q=grad.view(ctx.q_shape))
 
 
 dqfd_fwd.register_autograd(_dqfd_backward, setup_context=_dqfd_setup)
@@ -365,20 +395,20 @@ def _(q, target_q, next_q, action, reward, done, weight, value_gamma, value_gamm
 
 
 def _soft_td_setup(ctx, inputs, output):
-    ctx.save_for_backward(output[2], inputs[6], inputs[3], output[7])
-    S, G, N = inputs[11:14]
-    ctx.cfg = (S * G, 1, N, 0)  # qntd_bwd's (S, G, N, group_mean): R rows of one
-    ctx.q_shape = inputs[0].shape
+    a = _bind(soft_td_fwd, inputs)
+    ctx.save_for_backward(output[2], a.weight, a.action, output[7])
+    ctx.cfg = (a.S * a.G, 1, a.N, 0)  # qntd_bwd's (S, G, N, group_mean): R rows of one
+    ctx.q_shape = a.q.shape
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[2:])
 
 
 def _soft_td_backward(ctx, g_loss, g_td, *_):
     if g_loss is None and g_td is None:
-        return (None, ) * 22
+        return _input_grads(soft_td_fwd)
     dcrit, weight, action, grad_unit = ctx.saved_tensors
     grad = qntd_bwd(dcrit, weight, action, g_loss, g_td, grad_unit, *ctx.cfg)
-    return (grad.view(ctx.q_shape), ) + (None, ) * 21
+    return _input_grads(soft_td_fwd, q=grad.view(ctx.q_shape))
 
 
 soft_td_fwd.register_autograd(_soft_td_backward, setup_context=_soft_td_setup)
@@ -432,8 +462,7 @@ def dntd_bwd(dist: Tensor, act: Tensor, proj: Tensor, weight: Optional[Tensor], 
         weight = ops.const_scalar(weight_scalar, dist.device)
     kl, pg = _one(g_loss)
     kt, ptd = _one(g_td)
-    skip = 1 if (g_td is None and grad_unit.numel()) else 0
-    grad = grad_unit.clone() if skip else torch.empty_like(dist)
+    grad, skip = _unit_grad(grad_unit, (g_td, ), lambda: torch.empty_like(dist))
     return ops.dntd_bwd_(dist, act, proj, weight, w_stride, pg, ptd, R, N, n_atom, skip, grad)
 
 
@@ -443,20 +472,20 @@ def _(dist, *args):
 
 
 def _dntd_setup(ctx, inputs, output):
-    ctx.save_for_backward(inputs[0], inputs[2], output[2], inputs[6], output[3])
-    B, A, N, n_atom = inputs[12:16]
-    ctx.cfg = (inputs[7], inputs[8], B * A, N, n_atom)
+    a = _bind(dntd_fwd, inputs)
+    ctx.save_for_backward(a.dist, a.act, output[2], a.weight, output[3])
+    ctx.cfg = (a.weight_scalar, a.w_stride, a.B * a.A, a.N, a.n_atom)
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[2:])
 
 
 def _dntd_backward(ctx, g_loss, g_td, *_):
     if g_loss is None and g_td is None:
-        return (None, ) * 22
+        return _input_grads(dntd_fwd)
     dist, act, proj, weight, grad_unit = ctx.saved_tensors
     weight_scalar, w_stride, R, N, n_atom = ctx.cfg
     grad = dntd_bwd(dist, act, proj, weight, weight_scalar, w_stride, g_loss, g_td, grad_unit, R, N, n_atom)
-    return (grad, ) + (None, ) * 21
+    return _input_grads(dntd_fwd, dist=grad)
 
 
 dntd_fwd.register_autograd(_dntd_backward, setup_context=_dntd_setup)
@@ -495,7 +524,7 @@ def _td_lambda_setup(ctx, inputs, output):
 
 def _td_lambda_backward(ctx, g_loss, _g_dvalue):
     dvalue, = ctx.saved_tensors
-    return scale(g_loss, dvalue), None, None, None, None
+    return _input_grads(td_lambda_fwd, value=scale(g_loss, dvalue))
 
 
 td_lambda_fwd.register_autograd(_td_lambda_backward, setup_context=_td_lambda_setup)
@@ -531,8 +560,7 @@ def _(logit, action, mask, rho, ret, value, TB, K, N, want_grad):
 @torch.library.custom_op('b200rl::upgo_bwd', mutates_args=())
 def upgo_bwd(logit: Tensor, action: Tensor, mask: Optional[Tensor], adv: Tensor, g_loss: Tensor, grad_unit: Tensor,
              TB: int, K: int, N: int) -> Tensor:
-    skip = 1 if grad_unit.numel() else 0
-    grad = grad_unit.clone() if skip else torch.empty_like(logit)
+    grad, skip = _unit_grad(grad_unit, (), lambda: torch.empty_like(logit))  # adv, the other output, is not differentiable
     kg, pg = _one(g_loss)
     return ops.upgo_bwd_(logit, action, mask, adv, pg, TB, K, N, skip, grad)
 
@@ -543,14 +571,15 @@ def _(logit, *args):
 
 
 def _upgo_setup(ctx, inputs, output):
-    ctx.save_for_backward(inputs[0], inputs[1], inputs[2], output[1], output[2])
-    ctx.cfg = inputs[6:9]
+    a = _bind(upgo_fwd, inputs)
+    ctx.save_for_backward(a.logit, a.action, a.mask, output[1], output[2])
+    ctx.cfg = (a.TB, a.K, a.N)
     ctx.mark_non_differentiable(*output[1:])
 
 
 def _upgo_backward(ctx, g_loss, *_):
     logit, action, mask, adv, grad_unit = ctx.saved_tensors
-    return (upgo_bwd(logit, action, mask, adv, g_loss, grad_unit, *ctx.cfg), ) + (None, ) * 9
+    return _input_grads(upgo_fwd, logit=upgo_bwd(logit, action, mask, adv, g_loss, grad_unit, *ctx.cfg))
 
 
 upgo_fwd.register_autograd(_upgo_backward, setup_context=_upgo_setup)
@@ -616,16 +645,17 @@ def _(target_output, behaviour_output, action, value, *args):
 
 
 def _vtrace_setup(ctx, inputs, output):
-    ctx.save_for_backward(inputs[0], inputs[2], inputs[3], inputs[1], inputs[4], inputs[5], *output[1:])
-    ctx.scal = inputs[6:11]
+    a = _bind(vtrace_loss, inputs)
+    ctx.save_for_backward(a.target_output, a.behaviour_output, a.action, a.value, a.reward, a.weight, *output[1:])
+    ctx.scal = (a.gamma, a.lambda_, a.rho_clip, a.c_clip, a.rho_pg_clip)
     ctx.mark_non_differentiable(*output[1:])
 
 
 def _vtrace_backward(ctx, g_out, *_):
     if g_out is None:
-        return (None, ) * 12
+        return _input_grads(vtrace_loss)
     grad_logit, grad_value = vtrace_bwd(*ctx.saved_tensors[:6], g_out, *ctx.saved_tensors[6:], *ctx.scal)
-    return (grad_logit, grad_value) + (None, ) * 10
+    return _input_grads(vtrace_loss, target_output=grad_logit, value=grad_value)
 
 
 vtrace_loss.register_autograd(_vtrace_backward, setup_context=_vtrace_setup)
@@ -655,7 +685,7 @@ def _ppo_value_setup(ctx, inputs, output):
 
 def _ppo_value_backward(ctx, g_loss, _g_dvalue):
     dvalue, = ctx.saved_tensors
-    return (scale(g_loss, dvalue), ) + (None, ) * 6
+    return _input_grads(ppo_value_fwd, value_new=scale(g_loss, dvalue))
 
 
 ppo_value_fwd.register_autograd(_ppo_value_backward, setup_context=_ppo_value_setup)
@@ -707,13 +737,14 @@ def _(logits, *args):
 
 
 def _token_logp_setup(ctx, inputs, output):
-    ctx.save_for_backward(inputs[0], inputs[1], output[1])
+    a = _bind(token_logp_op, inputs)
+    ctx.save_for_backward(a.logits, a.index, output[1])
     ctx.mark_non_differentiable(output[1])
 
 
 def _token_logp_backward(ctx, g_lp, _g_lse):
     logits, index, lse = ctx.saved_tensors
-    return vocab_bwd(logits, index, lse, g_lp.float().contiguous(), None), None
+    return _input_grads(token_logp_op, logits=vocab_bwd(logits, index, lse, g_lp.float().contiguous(), None))
 
 
 token_logp_op.register_autograd(_token_logp_backward, setup_context=_token_logp_setup)
@@ -739,16 +770,17 @@ def _(logit_new, logit_old, logit_ref, action, side, weight, mode, clip_ratio, b
 
 
 def _lm_policy_setup(ctx, inputs, output):
-    ctx.save_for_backward(inputs[0], inputs[3], output[1], output[2])
+    a = _bind(lm_policy_fwd, inputs)
+    ctx.save_for_backward(a.logit_new, a.action, output[1], output[2])
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(output[1], output[2])
 
 
 def _lm_policy_backward(ctx, g_out, _g_lse, _g_dlp):
     if g_out is None:
-        return (None, ) * 9
+        return _input_grads(lm_policy_fwd)
     logit_new, action, lse, dlp = ctx.saved_tensors
-    return (vocab_bwd(logit_new, action, lse, dlp, g_out), ) + (None, ) * 8
+    return _input_grads(lm_policy_fwd, logit_new=vocab_bwd(logit_new, action, lse, dlp, g_out))
 
 
 lm_policy_fwd.register_autograd(_lm_policy_backward, setup_context=_lm_policy_setup)
@@ -775,7 +807,7 @@ def _token_head_setup(ctx, inputs, output):
 
 def _token_head_backward(ctx, g_out, _g_dlp):
     dlp, = ctx.saved_tensors
-    return (scale(g_out[:1], dlp), ) + (None, ) * 7
+    return _input_grads(token_head_fwd, lp_new=scale(g_out[:1], dlp))
 
 
 token_head_fwd.register_autograd(_token_head_backward, setup_context=_token_head_setup)
@@ -816,15 +848,16 @@ def _(logit_new, *args):
 
 
 def _ppo_lm_setup(ctx, inputs, output):
-    ctx.save_for_backward(inputs[0], inputs[3], inputs[5], *output[1:])
+    a = _bind(ppo_lm_fwd, inputs)
+    ctx.save_for_backward(a.logit_new, a.action, a.weight, *output[1:])
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[1:])
 
 
 def _ppo_lm_backward(ctx, g_out, *_):
     if g_out is None:
-        return (None, ) * 10
-    return (ppo_lm_bwd(*ctx.saved_tensors, g_out), ) + (None, ) * 9
+        return _input_grads(ppo_lm_fwd)
+    return _input_grads(ppo_lm_fwd, logit_new=ppo_lm_bwd(*ctx.saved_tensors, g_out))
 
 
 ppo_lm_fwd.register_autograd(_ppo_lm_backward, setup_context=_ppo_lm_setup)
@@ -860,16 +893,17 @@ def _(logit, value, *args):
 
 
 def _a2c_lm_setup(ctx, inputs, output):
-    ctx.save_for_backward(inputs[0], inputs[1], inputs[2], inputs[5], output[1])
+    a = _bind(a2c_lm_fwd, inputs)
+    ctx.save_for_backward(a.logit, a.value, a.action, a.weight, output[1])
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(output[1])
 
 
 def _a2c_lm_backward(ctx, g_out, _g_per_row):
     if g_out is None:
-        return (None, ) * 6
+        return _input_grads(a2c_lm_fwd)
     grad_logit, grad_value = a2c_lm_bwd(*ctx.saved_tensors, g_out)
-    return (grad_logit, grad_value) + (None, ) * 4
+    return _input_grads(a2c_lm_fwd, logit=grad_logit, value=grad_value)
 
 
 a2c_lm_fwd.register_autograd(_a2c_lm_backward, setup_context=_a2c_lm_setup)
@@ -888,7 +922,7 @@ def _or_empty(x, like):
 
 
 @torch.library.custom_op('b200rl::lm_linear_loss', mutates_args=())
-def lm_linear_loss(hidden: Tensor, lm_weight: Tensor, action: Tensor, lp_old: Tensor, lp_ref: Optional[Tensor],
+def lm_linear_loss_op(hidden: Tensor, lm_weight: Tensor, action: Tensor, lp_old: Tensor, lp_ref: Optional[Tensor],
                    side: Tensor, weight: Optional[Tensor], kind: str, B: int, S: int, dt: int, clip_ratio: float,
                    beta: float, want_dh: bool, want_dw: bool) -> tuple[Tensor, Tensor, Tensor]:
     """grpo / rloo_policy_error_linear on hidden (N, D), lm_weight (V, D) -> (loss / approx_kl / clipfrac, dH, dW)"""
@@ -897,14 +931,14 @@ def lm_linear_loss(hidden: Tensor, lm_weight: Tensor, action: Tensor, lp_old: Te
     return out, _or_empty(dh, hidden), _or_empty(dw, lm_weight)
 
 
-@lm_linear_loss.register_fake
+@lm_linear_loss_op.register_fake
 def _(hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt, clip_ratio, beta, want_dh, want_dw):
     return (_f32(hidden, 3), torch.empty_like(hidden) if want_dh else _empty(hidden),
             torch.empty_like(lm_weight) if want_dw else _empty(lm_weight))
 
 
 @torch.library.custom_op('b200rl::lm_linear_pg', mutates_args=())
-def lm_linear_pg(hidden: Tensor, lm_weight: Tensor, value: Optional[Tensor], action: Tensor, adv: Tensor,
+def lm_linear_pg_op(hidden: Tensor, lm_weight: Tensor, value: Optional[Tensor], action: Tensor, adv: Tensor,
                  weight: Optional[Tensor], lp_old: Optional[Tensor], lp_pre: Optional[Tensor], ret: Optional[Tensor],
                  kind: str, dt: int, clip_ratio: float, dual_clip: float, kl_type: int, entropy: bool, w_ent: float,
                  w_kl: float, w_val: float, want_dh: bool, want_dw: bool,
@@ -917,7 +951,7 @@ def lm_linear_pg(hidden: Tensor, lm_weight: Tensor, value: Optional[Tensor], act
     return ops.lm_pg_loss_(out, kind, cfg), out, _or_empty(dh, hidden), _or_empty(dw, lm_weight), _or_empty(dv, out)
 
 
-@lm_linear_pg.register_fake
+@lm_linear_pg_op.register_fake
 def _(hidden, lm_weight, value, action, adv, weight, lp_old, lp_pre, ret, kind, dt, clip_ratio, dual_clip, kl_type,
       entropy, w_ent, w_kl, w_val, want_dh, want_dw, want_dv):
     return (_f32(hidden, ()), _f32(hidden, 5 if kind == 'ppo' else 3),
@@ -939,50 +973,54 @@ def _(g, x):
 
 
 def _lm_linear_loss_setup(ctx, inputs, output):
+    a = _bind(lm_linear_loss_op, inputs)
     ctx.save_for_backward(output[1], output[2])
-    ctx.want = inputs[13:15]
+    ctx.want = (a.want_dh, a.want_dw)
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(output[1], output[2])
 
 
 def _lm_linear_loss_backward(ctx, g_out, _g_dh, _g_dw):
     if g_out is None:
-        return (None, ) * 15
+        return _input_grads(lm_linear_loss_op)
     dh, dw = ctx.saved_tensors
+    want_dh, want_dw = ctx.want
     g = g_out[:1]  # the loss's; approx_kl and clipfrac leave the wrapper detached
-    return (lm_linear_scale_out(g, dh) if ctx.want[0] else None,
-            lm_linear_scale_out(g, dw) if ctx.want[1] else None) + (None, ) * 13
+    return _input_grads(lm_linear_loss_op, hidden=lm_linear_scale_out(g, dh) if want_dh else None,
+                        lm_weight=lm_linear_scale_out(g, dw) if want_dw else None)
 
 
-lm_linear_loss.register_autograd(_lm_linear_loss_backward, setup_context=_lm_linear_loss_setup)
+lm_linear_loss_op.register_autograd(_lm_linear_loss_backward, setup_context=_lm_linear_loss_setup)
 
 
 def _lm_linear_pg_setup(ctx, inputs, output):
+    a = _bind(lm_linear_pg_op, inputs)
     ctx.save_for_backward(*output[2:])
-    ctx.want = inputs[18:21]
+    ctx.want = (a.want_dh, a.want_dw, a.want_dv)
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[1:])
 
 
 def _lm_linear_pg_backward(ctx, g_loss, *_):
     if g_loss is None:
-        return (None, ) * 21
+        return _input_grads(lm_linear_pg_op)
     dh, dw, dv = ctx.saved_tensors
     want_dh, want_dw, want_dv = ctx.want
-    return (lm_linear_scale_out(g_loss, dh) if want_dh else None, lm_linear_scale_out(g_loss, dw) if want_dw else None,
-            scale(g_loss, dv) if want_dv else None) + (None, ) * 18
+    return _input_grads(lm_linear_pg_op, hidden=lm_linear_scale_out(g_loss, dh) if want_dh else None,
+                        lm_weight=lm_linear_scale_out(g_loss, dw) if want_dw else None,
+                        value=scale(g_loss, dv) if want_dv else None)
 
 
-lm_linear_pg.register_autograd(_lm_linear_pg_backward, setup_context=_lm_linear_pg_setup)
+lm_linear_pg_op.register_autograd(_lm_linear_pg_backward, setup_context=_lm_linear_pg_setup)
 
 
 @torch.library.custom_op('b200rl::lm_logp', mutates_args=())
-def lm_logp(hidden: Tensor, lm_weight: Tensor, index: Tensor, dt: int) -> tuple[Tensor, Tensor]:
+def lm_logp_op(hidden: Tensor, lm_weight: Tensor, index: Tensor, dt: int) -> tuple[Tensor, Tensor]:
     """token_logp_linear -> (log p(index), logsumexp), fp32 per token row"""
     return ops.lm_logp_fwd_(hidden, lm_weight, index, dt)
 
 
-@lm_logp.register_fake
+@lm_logp_op.register_fake
 def _(hidden, lm_weight, index, dt):
     return _f32(hidden, hidden.shape[0]), _f32(hidden, hidden.shape[0])
 
@@ -1002,8 +1040,9 @@ def _(hidden, lm_weight, index, lse, g, dt, want_dh, want_dw):
 
 
 def _lm_logp_setup(ctx, inputs, output):
-    ctx.save_for_backward(inputs[0], inputs[1], inputs[2], output[1])
-    ctx.dt = inputs[3]
+    a = _bind(lm_logp_op, inputs)
+    ctx.save_for_backward(a.hidden, a.lm_weight, a.index, output[1])
+    ctx.dt = a.dt
     ctx.mark_non_differentiable(output[1])
 
 
@@ -1011,10 +1050,10 @@ def _lm_logp_backward(ctx, g, _g_lse):
     hidden, lm_weight, index, lse = ctx.saved_tensors
     want_dh, want_dw = ctx.needs_input_grad[:2]
     dh, dw = lm_logp_bwd(hidden, lm_weight, index, lse, g, ctx.dt, want_dh, want_dw)
-    return dh if want_dh else None, dw if want_dw else None, None, None
+    return _input_grads(lm_logp_op, hidden=dh if want_dh else None, lm_weight=dw if want_dw else None)
 
 
-lm_logp.register_autograd(_lm_logp_backward, setup_context=_lm_logp_setup)
+lm_logp_op.register_autograd(_lm_logp_backward, setup_context=_lm_logp_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -1054,22 +1093,22 @@ def _(value, next_value, reward, done, traj_flag, gamma, lambda_, value_norm, st
 
 
 @torch.library.custom_op('b200rl::adv_stats', mutates_args=())
-def adv_stats(x: Tensor) -> Tensor:
+def adv_stats_op(x: Tensor) -> Tensor:
     """{mean, std (unbiased) + 1e-8} of ``x``"""
     return ops.adv_stats_(x)
 
 
-@adv_stats.register_fake
+@adv_stats_op.register_fake
 def _(x):
     return _f32(x, 2)
 
 
 @torch.library.custom_op('b200rl::normalize', mutates_args=())
-def normalize(x: Tensor, stats: Tensor) -> Tensor:
+def normalize_op(x: Tensor, stats: Tensor) -> Tensor:
     return ops.normalize_(x, stats)
 
 
-@normalize.register_fake
+@normalize_op.register_fake
 def _(x, stats):
     return torch.empty_like(x)
 
@@ -1078,12 +1117,12 @@ def _(x, stats):
 # symlog / inv_symlog
 # ---------------------------------------------------------------------------------------------------------------------
 @torch.library.custom_op('b200rl::value_map', mutates_args=())
-def value_map(x: Tensor, mode: int) -> Tensor:
+def value_map_op(x: Tensor, mode: int) -> Tensor:
     """symlog (``mode`` 0) or inv_symlog (1) of a contiguous fp32 tensor"""
     return ops.value_map_fwd_(x, mode)
 
 
-@value_map.register_fake
+@value_map_op.register_fake
 def _(x, mode):
     return torch.empty_like(x)
 
@@ -1099,16 +1138,17 @@ def _(x, g, mode):
 
 
 def _value_map_setup(ctx, inputs, output):
-    ctx.save_for_backward(inputs[0])
-    ctx.mode = inputs[1]
+    a = _bind(value_map_op, inputs)
+    ctx.save_for_backward(a.x)
+    ctx.mode = a.mode
 
 
 def _value_map_backward(ctx, g):
     x, = ctx.saved_tensors
-    return value_map_bwd(x, g, ctx.mode), None
+    return _input_grads(value_map_op, x=value_map_bwd(x, g, ctx.mode))
 
 
-value_map.register_autograd(_value_map_backward, setup_context=_value_map_setup)
+value_map_op.register_autograd(_value_map_backward, setup_context=_value_map_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -1150,8 +1190,9 @@ def quantile_bwd(dtheta: Tensor, weight: Optional[Tensor], action: Tensor, g_los
     """-> d / d q; verifies a copy of the forward-written unit gradient when only the loss has a gradient"""
     kl, pg = _one(g_loss)
     kt, ptd = _one(g_td)
-    skip = 1 if g_td is None else 0
-    grad = grad_unit.clone() if skip else torch.empty_like(grad_unit)
+    # the forward writes grad_unit whenever q wants a gradient, so it is never empty here; a fresh buffer takes its
+    # strides, which the launch reads
+    grad, skip = _unit_grad(grad_unit, (g_td, ), lambda: torch.empty_like(grad_unit))
     return ops.quantile_bwd_(dtheta, weight, action, pg, ptd, B, N, n_tau, _quantile_strides(grad, form), skip, grad)
 
 
@@ -1161,17 +1202,18 @@ def _(dtheta, weight, action, g_loss, g_td, grad_unit, B, N, n_tau, form):
 
 
 def _quantile_setup(ctx, inputs, output):
-    ctx.save_for_backward(output[2], inputs[7], inputs[2], output[3])
-    ctx.cfg = (inputs[11], inputs[12], inputs[13], inputs[17])
+    a = _bind(quantile_fwd, inputs)
+    ctx.save_for_backward(output[2], a.weight, a.action, output[3])
+    ctx.cfg = (a.B, a.N, a.n_tau, a.form)
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[2:])
 
 
 def _quantile_backward(ctx, g_loss, g_td, *_):
     if g_loss is None and g_td is None:
-        return (None, ) * 20
+        return _input_grads(quantile_fwd)
     dtheta, weight, action, grad_unit = ctx.saved_tensors
-    return (quantile_bwd(dtheta, weight, action, g_loss, g_td, grad_unit, *ctx.cfg), ) + (None, ) * 19
+    return _input_grads(quantile_fwd, q=quantile_bwd(dtheta, weight, action, g_loss, g_td, grad_unit, *ctx.cfg))
 
 
 quantile_fwd.register_autograd(_quantile_backward, setup_context=_quantile_setup)
@@ -1201,8 +1243,7 @@ def _(q_tau_i, q_value, quantiles, action, B, N, want_grad):
 def fqf_fraction_bwd(g: Tensor, g_loss: Tensor, grad_unit: Tensor, B: int, N: int) -> Tensor:
     """-> d / d quantiles (B, N+1); verifies a copy of the forward-written unit gradient when there is one"""
     kl, pg = _one(g_loss)
-    skip = 1 if grad_unit.numel() else 0
-    grad = grad_unit.clone() if skip else g.new_empty(B, N + 1)
+    grad, skip = _unit_grad(grad_unit, (), lambda: g.new_empty(B, N + 1))  # g, the other output, is not differentiable
     return ops.fqf_fraction_bwd_(g, pg, B, N, skip, grad)
 
 
@@ -1212,17 +1253,18 @@ def _(g, g_loss, grad_unit, B, N):
 
 
 def _fqf_fraction_setup(ctx, inputs, output):
+    a = _bind(fqf_fraction_fwd, inputs)
     ctx.save_for_backward(output[1], output[2])
-    ctx.cfg = inputs[4:6]
+    ctx.cfg = (a.B, a.N)
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[1:])
 
 
 def _fqf_fraction_backward(ctx, g_loss, *_):
     if g_loss is None:
-        return (None, ) * 7
+        return _input_grads(fqf_fraction_fwd)
     g, grad_unit = ctx.saved_tensors
-    return (None, None, fqf_fraction_bwd(g, g_loss, grad_unit, *ctx.cfg)) + (None, ) * 4
+    return _input_grads(fqf_fraction_fwd, quantiles=fqf_fraction_bwd(g, g_loss, grad_unit, *ctx.cfg))
 
 
 fqf_fraction_fwd.register_autograd(_fqf_fraction_backward, setup_context=_fqf_fraction_setup)
@@ -1276,17 +1318,20 @@ def _(mu, sigma, value_new, *args):
 
 
 def _ppoc_setup(ctx, inputs, output):
-    ctx.save_for_backward(*inputs[:13], *output[1:])
-    ctx.cfg = inputs[13:20]
+    a = _bind(ppoc_loss, inputs)
+    ctx.save_for_backward(a.mu, a.sigma, a.value_new, a.mu_old, a.sigma_old, a.mu_pre, a.sigma_pre, a.action, a.value_old,
+                          a.adv, a.return_, a.weight, a.factor, *output[1:])
+    ctx.cfg = (a.S, a.D, a.clip_ratio, a.use_value_clip, a.dual_clip, a.kl_type, a.hint_kind)
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[1:])
 
 
 def _ppoc_backward(ctx, g_out, *_):
     if g_out is None:
-        return (None, ) * 21
+        return _input_grads(ppoc_loss)
     saved = ctx.saved_tensors
-    return ppoc_bwd(*saved[:13], g_out, *saved[13:], *ctx.cfg) + (None, ) * 18
+    grad_mu, grad_sigma, grad_value = ppoc_bwd(*saved[:13], g_out, *saved[13:], *ctx.cfg)
+    return _input_grads(ppoc_loss, mu=grad_mu, sigma=grad_sigma, value_new=grad_value)
 
 
 ppoc_loss.register_autograd(_ppoc_backward, setup_context=_ppoc_setup)
@@ -1334,17 +1379,18 @@ def _(logit, action, weight, adv, dq, g_out, grad_logit, grad_q, *args):
 
 
 def _coma_setup(ctx, inputs, output):
-    logit, q_value, target_q, action, reward, weight = inputs[:6]
-    ctx.save_for_backward(logit, action, weight, *output[1:])
-    ctx.cfg = inputs[6:10]
+    a = _bind(coma_fwd, inputs)
+    ctx.save_for_backward(a.logit, a.action, a.weight, *output[1:])
+    ctx.cfg = (a.T, a.B, a.A, a.N)
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[1:])
 
 
 def _coma_backward(ctx, g_out, *_):
     if g_out is None:
-        return (None, ) * 13
-    return coma_bwd(*ctx.saved_tensors[:5], g_out, *ctx.saved_tensors[5:], *ctx.cfg) + (None, ) * 11
+        return _input_grads(coma_fwd)
+    grad_logit, grad_q = coma_bwd(*ctx.saved_tensors[:5], g_out, *ctx.saved_tensors[5:], *ctx.cfg)
+    return _input_grads(coma_fwd, logit=grad_logit, q_value=grad_q)
 
 
 coma_fwd.register_autograd(_coma_backward, setup_context=_coma_setup)
@@ -1374,14 +1420,14 @@ def _(g, row, col, M, H, W):
 
 
 def _scatter_setup(ctx, inputs, output):
-    x, row, col, H, W, _mode = inputs
-    ctx.save_for_backward(row, col)
-    ctx.cfg = (x.shape[1], H, W)
+    a = _bind(scatter_fwd, inputs)
+    ctx.save_for_backward(a.row, a.col)
+    ctx.cfg = (a.x.shape[1], a.H, a.W)
 
 
 def _scatter_backward(ctx, g):
     row, col = ctx.saved_tensors
-    return scatter_bwd(g, row, col, *ctx.cfg), None, None, None, None, None
+    return _input_grads(scatter_fwd, x=scatter_bwd(g, row, col, *ctx.cfg))
 
 
 scatter_fwd.register_autograd(_scatter_backward, setup_context=_scatter_setup)
@@ -1428,53 +1474,114 @@ def _(g_y, g_hT, g_cT, x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h
 
 
 def _lnlstm_setup(ctx, inputs, output):
-    ctx.save_for_backward(*inputs[:10], *output[:1], *output[3:])
+    a = _bind(lnlstm_fwd, inputs)
+    ctx.save_for_backward(a.x, a.h0, a.c0, a.wx, a.wh, a.bias, a.gamma_x, a.beta_x, a.gamma_h, a.beta_h, *output[:1],
+                          *output[3:])
     ctx.set_materialize_grads(False)
     ctx.mark_non_differentiable(*output[3:])
 
 
 def _lnlstm_backward(ctx, g_y, g_hT, g_cT, *_):
-    needs = list(ctx.needs_input_grad[:10])
+    needs = list(ctx.needs_input_grad[:10])  # x ... beta_h: every argument but ``save``
     grads = lnlstm_bwd(g_y, g_hT, g_cT, *ctx.saved_tensors, needs)
-    return tuple(g if n else None for g, n in zip(grads, needs)) + (None, )
+    return _input_grads(lnlstm_fwd, **{n: g for n, g, need in zip(_names(lnlstm_fwd), grads, needs) if need})
 
 
 lnlstm_fwd.register_autograd(_lnlstm_backward, setup_context=_lnlstm_setup)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# what rl_utils calls while compiling: the autograd.Function signatures of ops, on the ops above
+# The one entry point of each operator for rl_utils / torch_utils: the custom op above while torch.compile traces, and
+# otherwise exactly eager mode's call -- the autograd.Function of ops, or its no-grad shortcut.  A python-scalar weight /
+# value_gamma / is_expert comes in as a python number: eager mode reads it from a cached device constant, the custom ops
+# take it as a float (they look the constant up when they run, so tracing allocates nothing).
 # ---------------------------------------------------------------------------------------------------------------------
 def _want_grad(*xs):
     return torch.is_grad_enabled() and any(x.requires_grad for x in xs)
 
 
+def _is_scalar(x):
+    return x is not None and not isinstance(x, Tensor)
+
+
 def _scalar_or_tensor(x):
     """(tensor, None) or (None, python float): the custom ops take a python-scalar weight / value_gamma as a float"""
-    return (None, float(x)) if (x is not None and not isinstance(x, Tensor)) else (x, None)
+    return (None, float(x)) if _is_scalar(x) else (x, None)
+
+
+def _const(x, dev):
+    """eager mode's form of a python-scalar weight / value_gamma: the cached device constant"""
+    return ops.const_scalar(x, dev) if _is_scalar(x) else x
+
+
+def stage_logits(x):
+    """language-model logits for the vocabulary-scale kernels: eager mode makes the 16-byte-aligned copy of an odd-offset
+    view (ops.logits_c); a traced tensor has no address, so under compile the custom op makes that copy itself"""
+    return x.contiguous() if torch.compiler.is_compiling() else ops.logits_c(x)
+
+
+def gae(value, next_value, reward, done, traj_flag, gamma, lambda_, agents):
+    """-> adv; next_value is masked in place by (1 - done)"""
+    if not torch.compiler.is_compiling():
+        return ops.gae_(value, next_value, reward, done, traj_flag, gamma, lambda_, agents)
+    return gae_op(value, next_value, reward, done, traj_flag, float(gamma), float(lambda_), agents)
 
 
 def ppo(logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre, S, G, N, clip_ratio,
         use_value_clip, dual_clip, kl_type, hint_kind, adv_stats=None, factor=None):
-    """-> the six floats policy, value, entropy, kl loss, approx_kl, clipfrac"""
-    return ppo_loss(logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre, adv_stats, factor,
+    """-> (policy, value, entropy, kl loss, a vector whose [4:6] are approx_kl, clipfrac), as PPOFunction"""
+    if not torch.compiler.is_compiling():
+        return ops.PPOFunction.apply(logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre,
+                                     S, G, N, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, adv_stats, factor)
+    out = ppo_loss(logit_new, value_new, logit_old, action, value_old, adv, return_, weight, logit_pre, adv_stats, factor,
                    S, G, N, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind,
                    _want_grad(logit_new, value_new))[0]
+    return out[0], out[1], out[2], out[3], out
 
 
 def qntd(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, vg_stride, gamma_ps, S, G, N, nstep, gamma,
          cum_reward, rescale, eps, criterion, crit_param, group_mean):
-    """-> (loss, td, target), as QNStepTDFunction's first three outputs"""
+    """-> (loss, td, target, priority; None under compile), as QNStepTDFunction without the sequence form"""
+    if not torch.compiler.is_compiling():
+        return ops.QNStepTDFunction.apply(q, next_n_q, action, next_n_action, reward, done, weight,
+                                          _const(value_gamma, q.device), vg_stride, gamma_ps, S, G, N, nstep, gamma,
+                                          cum_reward, rescale, eps, criterion, crit_param, group_mean, 0, 0.0, False)
     vg, vg_scalar = _scalar_or_tensor(value_gamma)
     loss, td, _, target, _ = qntd_fwd(q, next_n_q, action, next_n_action, reward, done, weight, vg, vg_scalar, vg_stride,
                                       gamma_ps, S, G, N, nstep, gamma, cum_reward, rescale, eps, criterion, crit_param,
                                       group_mean, _want_grad(q))
-    return loss, td, target
+    return loss, td, target, None
+
+
+def qntd_seq(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, vg_stride, gamma_ps, S, N, nstep, gamma,
+             rescale, criterion, crit_param, seq_len, priority_mix):
+    """-> (loss, td, priority), as QNStepTDFunction's sequence form"""
+    if not torch.compiler.is_compiling():
+        loss, td, _, prio = ops.QNStepTDFunction.apply(
+            q, next_n_q, action, next_n_action, reward, done, weight, _const(value_gamma, q.device), vg_stride, gamma_ps,
+            S, 1, N, nstep, gamma, 0, rescale, 1e-2, criterion, crit_param, 0, seq_len, priority_mix, True)
+        return loss, td, prio
+    vg, vg_scalar = _scalar_or_tensor(value_gamma)
+    loss, td, _, prio, _ = qntd_seq_fwd(q, next_n_q, action, next_n_action, reward, done, weight, vg, vg_scalar, vg_stride,
+                                        gamma_ps, S, N, nstep, gamma, rescale, criterion, crit_param, seq_len,
+                                        priority_mix, _want_grad(q))
+    return loss, td, prio
 
 
 def dist_nstep_td(dist, next_n_dist, act, next_n_act, reward, done, weight, w_stride, value_gamma, vg_stride, B, A, N,
                   n_atom, nstep, gamma, v_min, v_max, check_positive):
-    """-> (loss, td)"""
+    """-> (loss, td), as DistNStepTDFunction; with ``check_positive`` the reference's assertion that dist[b, act] > 0"""
+    from .rl_utils.td import _support
+    if not torch.compiler.is_compiling():
+        dev = dist.device
+        w, vg = _const(weight, dev), _const(value_gamma, dev)
+        bad = torch.zeros(1, dtype=torch.int32, device=dev) if check_positive else None
+        loss, td = ops.DistNStepTDFunction.apply(dist, next_n_dist, act, next_n_act, reward, done, w, w_stride, vg,
+                                                 vg_stride, _support(v_min, v_max, n_atom, dev), B, A, N, n_atom, nstep,
+                                                 gamma, v_min, v_max, bad)
+        if check_positive:
+            assert bad.item() == 0, ("dist act", "non-positive probability in dist[batch_range, act]")  # td.py:513
+        return loss, td
     w, w_scalar = _scalar_or_tensor(weight)
     vg, vg_scalar = _scalar_or_tensor(value_gamma)
     loss, td, _, _ = dntd_fwd(dist, next_n_dist, act, next_n_act, reward, done, w, w_scalar, w_stride, vg, vg_scalar,
@@ -1483,57 +1590,124 @@ def dist_nstep_td(dist, next_n_dist, act, next_n_act, reward, done, weight, w_st
 
 
 def td_lambda(value, reward, weight, gamma, lambda_):
-    return td_lambda_fwd(value, reward, weight, gamma, lambda_)[0]
+    if not torch.compiler.is_compiling():
+        return ops.td_lambda_(value, reward, weight, gamma, lambda_)
+    return td_lambda_fwd(value, reward, weight, float(gamma), float(lambda_))[0]
 
 
 def upgo(logit, action, mask, rho, reward, value, TB, K, N):
+    if not torch.compiler.is_compiling():
+        ret = ops.lambda_returns_(value, reward, None, 1.0, None, 1.0, None, True)
+        return ops.UPGOFunction.apply(logit, action, mask, rho, ret, value, TB, K, N)
     ret = lambda_returns(value, reward, None, 1.0, None, 1.0, None, True)
     return upgo_fwd(logit, action, mask, rho, ret, value, TB, K, N, _want_grad(logit))[0]
 
 
 def vtrace(target_output, value, behaviour_output, action, reward, weight, gamma, lambda_, rho_clip, c_clip, rho_pg_clip):
-    """-> (policy_loss, value_loss, entropy_loss)"""
+    """-> (policy_loss, value_loss, entropy_loss), as VTraceFunction"""
+    if not torch.compiler.is_compiling():
+        return ops.VTraceFunction.apply(target_output, value, behaviour_output, action, reward, weight, gamma, lambda_,
+                                        rho_clip, c_clip, rho_pg_clip)
     out = vtrace_loss(target_output, value, behaviour_output, action, reward, weight, gamma, lambda_, rho_clip, c_clip,
-                     rho_pg_clip, _want_grad(target_output, value))[0]
+                      rho_pg_clip, _want_grad(target_output, value))[0]
     return out[0], out[1], out[2]
 
 
 def ppo_value(value_new, value_old, return_, weight, clip_ratio, use_value_clip):
+    if not torch.compiler.is_compiling():
+        return ops.ppo_value_(value_new, value_old, return_, weight, clip_ratio, use_value_clip)
     return ppo_value_fwd(value_new, value_old, return_, weight, float(clip_ratio), bool(use_value_clip),
                          _want_grad(value_new))[0]
 
 
-def token_logp(logits, index):
-    """-> log p(index) per row, as TokenLogProbFunction"""
+def token_logp(logits, index, dt):
+    """-> log p(index) per row of logits (rows, V) staged by ``stage_logits``, as TokenLogProbFunction"""
+    if not torch.compiler.is_compiling():
+        return ops.TokenLogProbFunction.apply(logits, index, dt)
     return token_logp_op(logits, index)[0]
 
 
-def lm_policy(logit_new, logit_old, logit_ref, action, side, weight, mode, clip_ratio, beta):
-    """-> (loss, approx_kl, clipfrac), as GRPOFunction / RLOOFunction"""
-    out = lm_policy_fwd(logit_new, logit_old, logit_ref, action, side, weight, mode, clip_ratio, beta)[0]
+def lm_policy(logit_new, logit_old, logit_ref, action, side, weight, mode, dt, clip_ratio, beta):
+    """-> (loss, approx_kl, clipfrac), as GRPOFunction (``mode`` 'grpo': side = adv (B)) or RLOOFunction ('rloo': side =
+    reward (K, B / K), no logit_ref); logits staged by ``stage_logits``"""
+    if not torch.compiler.is_compiling():
+        if mode == 'grpo':
+            return ops.GRPOFunction.apply(logit_new, logit_old, logit_ref, action, side, weight, dt, clip_ratio, beta)
+        return ops.RLOOFunction.apply(logit_new, logit_old, action, side, weight, dt, clip_ratio)
+    out = lm_policy_fwd(logit_new, logit_old, logit_ref, action, side, weight, mode, float(clip_ratio), float(beta))[0]
     return out[0], out[1], out[2]
 
 
 def token_head(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta):
     """-> (loss, approx_kl, clipfrac), as ops.token_head_"""
+    if not torch.compiler.is_compiling():
+        return ops.token_head_(lp_new, lp_old, lp_ref, adv, reward, weight, clip_ratio, beta)
     out = token_head_fwd(lp_new, lp_old, lp_ref, adv, reward, weight, float(clip_ratio), float(beta))[0]
     return out[0], out[1], out[2]
 
 
-def ppo_lm(logit_new, logit_old, logit_pre, action, adv, weight, clip_ratio, dual_clip, kl_type, entropy):
-    """-> (policy_loss, entropy_loss, kl_div, the five floats), as PPOLMFunction"""
+def ppo_lm(logit_new, logit_old, logit_pre, action, adv, weight, dt, clip_ratio, dual_clip, kl_type, entropy, hint_kind):
+    """-> (policy_loss, entropy_loss, kl_div, the five floats), as PPOLMFunction; logits staged by ``stage_logits``"""
+    if not torch.compiler.is_compiling():
+        return ops.PPOLMFunction.apply(logit_new, logit_old, logit_pre, action, adv, weight, dt, clip_ratio, dual_clip,
+                                       kl_type, entropy, hint_kind)
     out = ppo_lm_fwd(logit_new, logit_old, logit_pre, action, adv, weight, clip_ratio, dual_clip, kl_type, entropy)[0]
     return out[0], out[1], out[2], out
 
 
-def a2c_lm(logit, value, action, adv, return_, weight):
-    """-> (policy_loss, value_loss, entropy_loss), as A2CLMFunction"""
+def a2c_lm(logit, value, action, adv, return_, weight, dt):
+    """-> (policy_loss, value_loss, entropy_loss), as A2CLMFunction; logit staged by ``stage_logits``"""
+    if not torch.compiler.is_compiling():
+        return ops.A2CLMFunction.apply(logit, value, action, adv, return_, weight, dt)
     out = a2c_lm_fwd(logit, value, action, adv, return_, weight)[0]
     return out[0], out[1], out[2]
 
 
+def lm_logp(hidden, lm_weight, index, dt):
+    """-> log p(index) per token row, as TokenLogpLinearFunction"""
+    if torch.compiler.is_compiling():
+        return lm_logp_op(hidden, lm_weight, index, dt)[0]
+    if _want_grad(hidden, lm_weight):
+        return ops.TokenLogpLinearFunction.apply(hidden, lm_weight, index, dt)
+    return ops.lm_logp_fwd_(hidden.detach(), lm_weight.detach(), index, dt)[0]
+
+
+def lm_linear_loss(hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt, clip_ratio, beta):
+    """-> (loss, approx_kl, clipfrac), as LMLinearLossFunction"""
+    if torch.compiler.is_compiling():
+        grad = torch.is_grad_enabled()
+        out = lm_linear_loss_op(hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt, clip_ratio, beta,
+                                grad and hidden.requires_grad, grad and lm_weight.requires_grad)[0]
+        return out[0], out[1].detach(), out[2].detach()
+    if _want_grad(hidden, lm_weight):
+        return ops.LMLinearLossFunction.apply(hidden, lm_weight, action, lp_old, lp_ref, side, weight, kind, B, S, dt,
+                                              clip_ratio, beta)
+    out = ops.lm_linear_loss_(hidden.detach(), lm_weight.detach(), action, lp_old, lp_ref, side, weight, kind, B, S, dt,
+                              clip_ratio, beta, False, False)[0]
+    return out[0], out[1], out[2]
+
+
+def lm_linear_pg(hidden, lm_weight, value, action, adv, weight, lp_old, lp_pre, ret, kind, dt, cfg):
+    """-> (the one loss, the raw sums), as LMLinearPGFunction"""
+    grad = torch.is_grad_enabled()
+    want = (grad and hidden.requires_grad, grad and lm_weight.requires_grad,
+            grad and value is not None and value.requires_grad)
+    if torch.compiler.is_compiling():
+        return lm_linear_pg_op(hidden, lm_weight, value, action, adv, weight, lp_old, lp_pre, ret, kind, dt, *cfg,
+                               *want)[:2]
+    if any(want):
+        return ops.LMLinearPGFunction.apply(hidden, lm_weight, value, action, adv, weight, lp_old, lp_pre, ret, kind, dt,
+                                            cfg)
+    out = ops.lm_linear_pg_(hidden.detach(), lm_weight.detach(), action, adv, weight, lp_old, lp_pre,
+                            None if value is None else value.detach(), ret, kind, dt, cfg, False, False, False)[0]
+    return ops.lm_pg_loss_(out, kind, cfg), out
+
+
 def gae_returns(value, next_value, reward, done, traj_flag, gamma, lambda_, vscale):
     """-> (adv, unnormalized return, value_out or None, return_out or None, return_stats, adv_stats), as ops.gae_returns_"""
+    if not torch.compiler.is_compiling():
+        return ops.gae_returns_(value, next_value, reward, done, traj_flag, gamma, lambda_, 1, vscale, True, True,
+                                want_adv_stats=True)
     adv, unnorm, vout, rout, stats, astats = gae_returns_op(value, next_value, reward, done, traj_flag, float(gamma),
                                                             float(lambda_), float(vscale))
     if vscale == 0.0:
@@ -1543,14 +1717,36 @@ def gae_returns(value, next_value, reward, done, traj_flag, gamma, lambda_, vsca
 
 def ppof_gae_returns(value, next_value, reward, done, traj_flag, gamma, lambda_, value_norm, std, mu, sigma):
     """-> (adv, value_out, return_out, return_stats or None, adv_stats), as ops.gae_returns_norm_"""
+    if not torch.compiler.is_compiling():
+        return ops.gae_returns_norm_(value, next_value, reward, done, traj_flag, gamma, lambda_, value_norm, std, mu, sigma,
+                                     value_norm == 'baseline')
     adv, vout, rout, stats, astats = gae_returns_norm(value, next_value, reward, done, traj_flag, float(gamma),
                                                       float(lambda_), value_norm, float(std), mu, sigma)
     return adv, vout, rout, stats if value_norm == 'baseline' else None, astats
 
 
+def adv_stats(x):
+    """{mean, std (unbiased) + 1e-8} of ``x``"""
+    return adv_stats_op(x) if torch.compiler.is_compiling() else ops.adv_stats_(x)
+
+
+def normalize(x, stats):
+    return normalize_op(x, stats) if torch.compiler.is_compiling() else ops.normalize_(x, stats)
+
+
+def value_map(x, mode):
+    """symlog (``mode`` 0) or inv_symlog (1) of a contiguous fp32 tensor, differentiable"""
+    return value_map_op(x, mode) if torch.compiler.is_compiling() else ops.ValueMapFunction.apply(x, mode)
+
+
 def quantile_td(q, next_n_q, action, next_n_action, reward, done, tau, weight, value_gamma, vg_stride, B, N, n_tau,
                 n_tau_prime, nstep, gamma, form, kappa):
-    """-> (loss, td), as QuantileTDFunction"""
+    """-> (loss, td), as QuantileTDFunction; the layout of q / next_n_q is QUANTILE_AXES[form]"""
+    if not torch.compiler.is_compiling():
+        return ops.QuantileTDFunction.apply(q, next_n_q, action, next_n_action, reward, done, tau, weight,
+                                            _const(value_gamma, q.device), vg_stride, B, N, n_tau, n_tau_prime, nstep,
+                                            gamma, _quantile_strides(q, form), _quantile_strides(next_n_q, form),
+                                            (tau.stride(0), tau.stride(1)), form, kappa)
     vg, vg_scalar = _scalar_or_tensor(value_gamma)
     loss, td, _, _ = quantile_fwd(q, next_n_q, action, next_n_action, reward, done, tau, weight, vg, vg_scalar, vg_stride,
                                   B, N, n_tau, n_tau_prime, nstep, gamma, form, kappa, _want_grad(q))
@@ -1559,33 +1755,38 @@ def quantile_td(q, next_n_q, action, next_n_action, reward, done, tau, weight, v
 
 def ppo_continuous(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight, S,
                    D, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind, factor=None):
-    """-> the six floats policy, value, entropy, kl loss, approx_kl, clipfrac, as PPOContinuousFunction's result vector"""
-    return ppoc_loss(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight,
-                     factor, S, D, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind,
-                     _want_grad(mu, sigma, value_new))[0]
+    """-> (policy, value, entropy, kl loss, a vector whose [4:6] are approx_kl, clipfrac), as PPOContinuousFunction"""
+    if not torch.compiler.is_compiling():
+        return ops.PPOContinuousFunction.apply(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action,
+                                               value_old, adv, return_, weight, S, D, clip_ratio, use_value_clip,
+                                               dual_clip, kl_type, hint_kind, factor)
+    out = ppoc_loss(mu, sigma, value_new, mu_old, sigma_old, mu_pre, sigma_pre, action, value_old, adv, return_, weight,
+                    factor, S, D, clip_ratio, use_value_clip, dual_clip, kl_type, hint_kind,
+                    _want_grad(mu, sigma, value_new))[0]
+    return out[0], out[1], out[2], out[3], out
 
 
 def coma(logit, q_value, target_q, action, reward, weight, T, B, A, N, gamma, lambda_):
     """-> (policy_loss, q_value_loss, entropy_loss), as COMAFunction without the differentiable returns"""
+    if not torch.compiler.is_compiling():
+        return ops.COMAFunction.apply(logit, q_value, target_q, action, reward, weight, None, T, B, A, N, gamma, lambda_)
     out = coma_fwd(logit, q_value, target_q, action, reward, weight, T, B, A, N, float(gamma), float(lambda_),
                    _want_grad(logit, q_value))[0]
     return out[0], out[1], out[2]
 
 
-def qntd_seq(q, next_n_q, action, next_n_action, reward, done, weight, value_gamma, vg_stride, gamma_ps, S, N, nstep, gamma,
-             rescale, criterion, crit_param, seq_len, priority_mix):
-    """-> (loss, td, priority), as QNStepTDFunction's sequence form"""
-    vg, vg_scalar = _scalar_or_tensor(value_gamma)
-    loss, td, _, prio, _ = qntd_seq_fwd(q, next_n_q, action, next_n_action, reward, done, weight, vg, vg_scalar, vg_stride,
-                                        gamma_ps, S, N, nstep, gamma, rescale, criterion, crit_param, seq_len,
-                                        priority_mix, _want_grad(q))
-    return loss, td, prio
-
-
 def dqfd(q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done, done1, weight, value_gamma, vg_stride,
          is_expert, S, N, nstep, gamma, cum_reward, rescale, eps, criterion, crit_param, lam_n, lam_1, lam_s, margin,
          seq_len, priority_mix, want_targets, want_priority):
-    """-> (loss, td, s_n, s_1, s_je, tn, t1, prio), as DQfDTDFunction; value_gamma and is_expert may be python floats"""
+    """-> (loss, td, s_n, s_1, s_je, tn, t1, prio), as DQfDTDFunction; value_gamma and is_expert may be python floats
+    (is_expert then holds for all S rows)"""
+    if not torch.compiler.is_compiling():
+        dev = q.device
+        ie = ops.const_scalar(is_expert, dev).expand(S).contiguous() if _is_scalar(is_expert) else is_expert
+        return ops.DQfDTDFunction.apply(q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done, done1,
+                                        weight, _const(value_gamma, dev), vg_stride, ie, S, N, nstep, gamma, cum_reward,
+                                        rescale, eps, criterion, crit_param, lam_n, lam_1, lam_s, margin, seq_len,
+                                        priority_mix, want_targets, want_priority)
     vg, vg_scalar = _scalar_or_tensor(value_gamma)
     ie, ie_scalar = _scalar_or_tensor(is_expert)
     loss, td, stats, _, tn, t1, prio, _ = dqfd_fwd(
@@ -1599,6 +1800,10 @@ def dqfd(q, next_n_q, next_q1, action, next_n_action, next_action1, reward, done
 def soft_td(q, target_q, next_q, action, reward, done, weight, value_gamma, vg_stride, mode, S, G, N, nstep, gamma, tau,
             alpha, cum_reward, criterion, crit_param):
     """-> (loss, td, target, action_gap, clipfrac, record_target_v), as SoftTDFunction"""
+    if not torch.compiler.is_compiling():
+        return ops.SoftTDFunction.apply(q, target_q, next_q, action, reward, done, weight, _const(value_gamma, q.device),
+                                        vg_stride, mode, S, G, N, nstep, gamma, tau, alpha, cum_reward, criterion,
+                                        crit_param)
     vg, vg_scalar = _scalar_or_tensor(value_gamma)
     loss, td, _, target, gap, clip, rec, _ = soft_td_fwd(q, target_q, next_q, action, reward, done, weight, vg, vg_scalar,
                                                          vg_stride, mode, S, G, N, nstep, gamma, tau, alpha, cum_reward,
@@ -1608,4 +1813,24 @@ def soft_td(q, target_q, next_q, action, reward, done, weight, value_gamma, vg_s
 
 def fqf_fraction(q_tau_i, q_value, quantiles, action, B, N):
     """-> the fraction loss, as FQFFractionFunction"""
+    if not torch.compiler.is_compiling():
+        return ops.FQFFractionFunction.apply(q_tau_i, q_value, quantiles, action, B, N, q_tau_i.stride(), q_value.stride(),
+                                             quantiles.stride())
     return fqf_fraction_fwd(q_tau_i, q_value, quantiles, action, B, N, _want_grad(quantiles))[0]
+
+
+def scatter(x, row, col, H, W, mode):
+    """ScatterConnection's scatter of x (B, M, N) into (B, N, H, W), as ScatterFunction"""
+    if not torch.compiler.is_compiling():
+        return ops.ScatterFunction.apply(x, row, col, H, W, mode)
+    return scatter_fwd(x, row, col, H, W, mode)
+
+
+def lnlstm(x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h, save):
+    """one layer of the layer-normalised LSTM -> (y, h_T, c_T), as LNLSTMFunction; ``save`` when a gradient is wanted"""
+    args = (x, h0, c0, wx, wh, bias, gamma_x, beta_x, gamma_h, beta_h)
+    if torch.compiler.is_compiling():
+        return lnlstm_fwd(*args, save)[:3]
+    if not save:  # nothing to differentiate: no autograd node
+        return ops.lnlstm_fwd_(*args, False)[:3]
+    return ops.LNLSTMFunction.apply(*args, save)

@@ -53,12 +53,7 @@ def layers(m, inputs, H0, C0):
         nx, nh = m.norm[2 * l], m.norm[2 * l + 1]
         args = (x, H0[l], C0[l], m.wx[l], m.wh[l], m.bias[l], nx.weight, nx.bias, nh.weight, nh.bias)
         save = grad and any(t.requires_grad for t in args)
-        if torch.compiler.is_compiling():
-            x, h, c = torch_ops.lnlstm_fwd(*args, save)[:3]
-        elif not save:  # nothing to differentiate: no autograd node
-            x, h, c = ops.lnlstm_fwd_(*args, False)[:3]
-        else:
-            x, h, c = ops.LNLSTMFunction.apply(*args, save)
+        x, h, c = torch_ops.lnlstm(*args, save)
         hs.append(h)
         cs.append(c)
         if m.use_dropout and l != m.num_layers - 1:

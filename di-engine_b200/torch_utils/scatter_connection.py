@@ -36,10 +36,7 @@ def _scatter(x, spatial_size, row, col, scatter_type):
             raise IndexError("di_engine_b200: ScatterConnection index %d is out of range for a %d x %d map" %
                              (lo if lo < 0 else hi, H, W))
     mode = ops.SCATTER_MODES[scatter_type]
-    if torch.compiler.is_compiling():
-        out = torch_ops.scatter_fwd(x, row, col, H, W, mode)
-    else:
-        out = ops.ScatterFunction.apply(x, row, col, H, W, mode)
+    out = torch_ops.scatter(x, row, col, H, W, mode)
     return out.cpu() if host_out else out
 
 
